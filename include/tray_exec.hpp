@@ -27,6 +27,8 @@ inline void check(trb_status s) { if (s != TRB_OK) throw Error(s, trb_last_error
 
 struct FrameInfo { size_t frames = 1; float time = 0.f; size_t start = 0, end = 0; };
 
+struct Adaptive { uint32_t min_spp = 0, max_spp = 0; }; // sampler::Adaptive (sampler/adaptive.rs); rounded up to powers of two
+
 struct Config {
     std::string out_path, scene_file;
     size_t spp = 0;                          // 0: the scene's film.samples
@@ -35,6 +37,8 @@ struct Config {
     size_t current_frame = 0;
     std::pair<size_t, size_t> select_blocks{0, 0}; // (start, count) into the Morton-sorted 8x8 block list; count 0 = all
     uint32_t seed = 1;
+    bool adaptive = false;                   // false: LowDiscrepancy at spp; true: the Adaptive sampler below (spp unused)
+    Adaptive sampler;
 };
 
 class RenderTarget {
@@ -81,10 +85,20 @@ struct Exec { // trait Exec (exec/mod.rs:41-49)
 class B200 : public Exec {
   public:
     trb_stats last_stats{};
+    std::vector<uint32_t> last_pixel_spp; // Adaptive: samples per pixel (width * height, zero outside the selected blocks)
     void render(Scene& scene, RenderTarget& rt, const Config& c) override {
         trb_render_cfg cfg{};
-        cfg.spp = (uint32_t)c.spp; cfg.block_start = (uint32_t)c.select_blocks.first; cfg.block_count = (uint32_t)c.select_blocks.second;
+        cfg.block_start = (uint32_t)c.select_blocks.first; cfg.block_count = (uint32_t)c.select_blocks.second;
         cfg.current_frame = (uint32_t)c.current_frame; cfg.seed = c.seed;
+        if (c.adaptive) {
+            const trb_adaptive ad{c.sampler.min_spp, c.sampler.max_spp};
+            const auto d = rt.dimensions();
+            last_pixel_spp.assign(d.first * d.second, 0u);
+            check(trb_render_adaptive(scene.handle(), &cfg, &ad, rt.data(), last_pixel_spp.data(), &last_stats));
+            return;
+        }
+        last_pixel_spp.clear();
+        cfg.spp = (uint32_t)c.spp;
         check(trb_render(scene.handle(), &cfg, rt.data(), &last_stats)); // includes Scene::update_frame, like MultiThreaded::render
     }
 };

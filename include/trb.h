@@ -398,6 +398,39 @@ trb_status trb_film_to_srgb8(trb_scene* scene, const float* film_rgbw, uint8_t* 
  * master (exec/distrib/master.rs:137-142): an 8-bit RGB PNG (stored deflate blocks; host only, no device needed). */
 trb_status trb_write_png(const char* path, const uint8_t* rgb8, uint32_t width, uint32_t height);
 
+/* -- Adaptive sampler (sampler/adaptive.rs) ------------------------------------------
+ * min_spp samples per pixel, then `step` more per round while the pixel's samples disagree (some sample's
+ * |luminance - average| / average > 0.5), until samples_taken >= max_spp. min_spp and max_spp are rounded up to powers of
+ * two (0 -> 1), step = ((max - min) / 5) rounded up to a power of two; a pixel ends with at most max_per_pixel samples,
+ * which can exceed max_spp (min 4, max 64: step 16, up to 68). Path integrator, wavefront pipeline only. */
+typedef struct trb_adaptive {
+    uint32_t min_spp, max_spp;
+} trb_adaptive;
+
+/* Exec::render with the Adaptive sampler: every selected block, all rounds, one blocking call; the film is ADDED to
+ * film_rgbw like trb_render. cfg->spp, sample_first and sample_count must be 0 (the sampler owns the schedule).
+ * pixel_spp (width*height, or NULL) receives the sample count of each pixel of the selected blocks; other entries are
+ * left as they are. TRB_INVALID_ARG when max < min after rounding; TRB_UNSUPPORTED for the Whitted / NormalsDebug
+ * integrators and TRB_RENDER_MEGAKERNEL. */
+trb_status trb_render_adaptive(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                               uint32_t* pixel_spp, trb_stats* stats);
+
+/* Parity variant of trb_render_adaptive: the clamped sample of every (block, pixel, slot) in the trb_render_samples order
+ * with max_per_pixel slots per pixel: n = blocks*64*max_per_pixel, slots a pixel did not take are zero. Does not update
+ * the frame. */
+trb_status trb_render_samples_adaptive(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, size_t n,
+                                       trb_sample* samples, uint32_t* pixel_spp, trb_stats* stats);
+
+/* The rounded schedule of Adaptive::new (adaptive.rs:34-49); any output may be NULL. Host only. */
+trb_status trb_adaptive_schedule(const trb_adaptive* adaptive, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step,
+                                 uint32_t* max_per_pixel);
+
+/* The per-pixel decision the device runs (csrc/trb_adaptive.h), over a caller-given luminance sequence lum[0..n) in slot
+ * order: the pixel's final sample count and average luminance. TRB_INVALID_ARG when the sequence ends before the pixel
+ * stops sampling. Host only. */
+trb_status trb_host_adaptive_decide(const trb_adaptive* adaptive, const float* lum, size_t n, uint32_t* samples_taken,
+                                    float* avg);
+
 /* -- introspection for parity tests ------------------------------------------------ */
 
 /* The Morton-sorted 8x8 block list (block_queue.rs:28-46) after select_blocks: pairs (bx,by). */

@@ -112,6 +112,10 @@ class Stats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class Adaptive(C.Structure):
+    _fields_ = [("min_spp", u32), ("max_spp", u32)]
+
+
 class Ray(C.Structure):
     _fields_ = [("o", f32 * 3), ("d", f32 * 3), ("min_t", f32), ("max_t", f32)]
 
@@ -144,6 +148,7 @@ TRB_SYMBOLS = [
     "trb_host_build_bvh", "trb_host_keyframe_transform", "trb_host_animated_transform", "trb_host_animated_color", "trb_host_quad_check", "trb_selftest_box", "trb_launch_count", "trb_scene_trace_time", "trb_scene_check_error", "trb_scene_set_option", "trb_write_png",
     "trb_nccl_unique_id", "trb_comm_create", "trb_comm_destroy", "trb_comm_info", "trb_comm_reduce_film", "trb_render_sharded",
     "trb_group_create", "trb_group_load_json", "trb_group_render", "trb_group_scene", "trb_group_destroy",
+    "trb_render_adaptive", "trb_render_samples_adaptive", "trb_adaptive_schedule", "trb_host_adaptive_decide",
 ]
 
 _trb = None
@@ -178,6 +183,10 @@ def load_trb():
     lib.trb_intersect_device.argtypes = [vp, sz, vp, vp, vp, vp]
     lib.trb_camera_rays.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
+    lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
+    lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
+    lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
+    lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]
     lib.trb_block_list.argtypes = [vp, u32, u32, C.POINTER(u32), vp, u32]
     lib.trb_scene_get_bvh.argtypes = [vp, C.c_int, C.POINTER(u32), vp, C.POINTER(u32), vp]

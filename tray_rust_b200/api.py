@@ -25,8 +25,25 @@ def _cfg(spp=0, sample_first=0, sample_count=0, block_start=0, block_count=0, cu
                        shard_index, shard_count, shard_chunk)
 
 
+def adaptive_schedule(min_spp, max_spp):
+    """trb_adaptive_schedule: Adaptive::new's rounded (min, max, step) and the largest per-pixel sample count."""
+    lib = F.load_trb()
+    out = [F.u32() for _ in range(4)]
+    rc = lib.trb_adaptive_schedule(C.byref(F.Adaptive(min_spp, max_spp)), *(C.byref(x) for x in out))
+    if rc != F.TRB_OK:
+        raise TrbError(rc, (lib.trb_last_error() or b"").decode())
+    return tuple(x.value for x in out)
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
+
+    def _n_selected_blocks(self, cfg):
+        nb = self.n_blocks(cfg.block_start, cfg.block_count)
+        if cfg.shard_count > 1:
+            ch = max(1, cfg.shard_chunk)
+            nb = sum(1 for j in range(nb) if (j // ch) % cfg.shard_count == cfg.shard_index)
+        return nb
 
     def _n_samples(self, cfg):
         nb = self.n_blocks(cfg.block_start, cfg.block_count)
@@ -137,6 +154,28 @@ class Scene(_Base):
         st = F.Stats()
         self._check(self._lib.trb_render_samples(self._h, C.byref(cfg), n, F.ptr(out), C.byref(st)))
         return out, st
+
+    def render_adaptive(self, min_spp, max_spp, film=None, **kw):
+        """trb_render_adaptive: the Adaptive sampler over the selected blocks, film accumulated into.
+        Returns (film, pixel_spp (height, width) uint32, zero outside the selection, Stats)."""
+        cfg = _cfg(**kw)
+        if film is None:
+            film = np.zeros((self.height, self.width, 4), np.float32)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_adaptive(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), F.ptr(spp), C.byref(st)))
+        return film, spp, st
+
+    def render_samples_adaptive(self, min_spp, max_spp, **kw):
+        """trb_render_samples_adaptive: (samples (blocks, 64, max_per_pixel) flattened, unused slots zero; pixel_spp; Stats)."""
+        cfg = _cfg(**kw)
+        n = self._n_selected_blocks(cfg) * 64 * adaptive_schedule(min_spp, max_spp)[3]
+        out = np.zeros(n, F.SAMPLE_DTYPE)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_samples_adaptive(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), n, F.ptr(out), F.ptr(spp),
+                                                          C.byref(st)))
+        return out, spp, st
 
     def camera_rays(self, **kw):
         cfg = _cfg(**kw)

@@ -253,7 +253,17 @@ struct trb_scene {
     std::vector<void*> wf_allocs;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> trace_events; // TRB_RENDER_TIME_TRACE
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> event_pool;
+    // Adaptive sampler (trb_render_adaptive), allocated on first use: per-pixel state (trbh::AdPixel), the round's block list
+    // twice (compaction ping-pong) with each block's index in the selection, per-block "still sampling" flags
+    uint4* d_ad_state = nullptr;
+    uint2* d_ad_list[2] = {nullptr, nullptr};
+    uint32_t* d_ad_index[2] = {nullptr, nullptr};
+    uint32_t* d_ad_flags = nullptr;
+    uint32_t* d_ad_count = nullptr;
+    uint32_t* d_ad_spp = nullptr;
     ~trb_scene() {
+        for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
+                        (void*)d_ad_count, (void*)d_ad_spp}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -468,7 +478,10 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     CU(cudaMemsetAsync(wf.counters, 0, 64 * trb::WF_CNT * sizeof(uint32_t), st));
     const unsigned gen_grid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
     const bool anim = s->ds.has_anim != 0; // static scenes run kernels with no animation code in them at all
-    if (anim) trb::k_wf_generate<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+    if (rp.ad_state) { // Adaptive sampler round: only the pixels still sampling queue their paths
+        if (anim) trb::k_wf_generate_ad<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+        else trb::k_wf_generate_ad<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+    } else if (anim) trb::k_wf_generate<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
     else trb::k_wf_generate<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
     g_launches++;
     if (anim && wf.xf_tab && s->tune.anim_table) { // AnimatedTransform::transform(ray.time) once per (path, keyframed instance)
@@ -580,10 +593,13 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
         else trb::k_wf_shade<1, false, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
         g_launches += 2;
     }
-    if (mode == 0) {
+    if (mode == 0 && rp.film) { // (an Adaptive parity dump has no film: its records are written by k_ad_decide)
         const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
         const unsigned film_grid = std::min<unsigned>(rp.n_blocks, (unsigned)s->sm_count * 8);
-        if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
+        if (rp.ad_state) {
+            if (tu.film_v2) trb::k_wf_film_v2<true><<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
+            else trb::k_wf_film<true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, rp, wf);
+        } else if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
         else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, rp, wf);
         g_launches++;
     }
@@ -622,6 +638,104 @@ trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int
             trb_status r = launch_wavefront(s, rp, flags, mode, st);
             if (r != TRB_OK) return r;
         }
+    return TRB_OK;
+}
+
+// ---- Adaptive sampler (DESIGN.md §2 "Adaptive sampler", §5) ----------------------------------------------------------
+trb_status adaptive_check(const trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, trbh::AdSchedule& sch) {
+    if (cfg->spp || cfg->sample_first || cfg->sample_count)
+        return fail(TRB_INVALID_ARG, "the Adaptive sampler owns the sample schedule: spp, sample_first and sample_count must be 0");
+    if (!trbh::ad_schedule(ad->min_spp, ad->max_spp, sch))
+        return fail(TRB_INVALID_ARG, "Adaptive sampler: max_spp < min_spp after rounding up to powers of two (the reference panics), or more than 2^24");
+    if (s->integrator.type != TRB_INTEGRATOR_PATH) return fail(TRB_UNSUPPORTED, "the Adaptive sampler is built for the path integrator only");
+    if (cfg->flags & TRB_RENDER_MEGAKERNEL) return fail(TRB_UNSUPPORTED, "the Adaptive sampler runs on the wavefront pipeline only");
+    return TRB_OK;
+}
+
+trb_status ensure_adaptive(trb_scene* s) {
+    if (s->d_ad_state) return TRB_OK;
+    const size_t npx = (size_t)s->film.width * s->film.height, nblk = npx / 64;
+    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_state), npx * sizeof(uint4)));
+    for (int k = 0; k < 2; ++k) {
+        CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_list[k]), std::max<size_t>(1, nblk) * sizeof(uint2)));
+        CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_index[k]), std::max<size_t>(1, nblk) * sizeof(uint32_t)));
+    }
+    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_flags), std::max<size_t>(1, nblk) * sizeof(uint32_t)));
+    CU(cudaMemset(s->d_ad_flags, 0, std::max<size_t>(1, nblk) * sizeof(uint32_t)));
+    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_count), sizeof(uint32_t)));
+    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_spp), npx * sizeof(uint32_t)));
+    return TRB_OK;
+}
+
+// thread_work with the Adaptive sampler over the selected blocks: round 0 over all of them, round k over the blocks that still
+// have a pixel sampling, each round cut into passes of whole blocks (a pass holds all of a pixel's samples of the round, so
+// k_ad_decide sees them together). rp carries the film or the parity records, stats, seed. Blocks on st; reads back 4 bytes
+// per round. Afterwards d_ad_spp[block * 64 + pixel] holds each selected pixel's sample count.
+trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb::RenderParams rp, const uint2* d_blocks, uint32_t nb, uint32_t flags,
+                                  cudaStream_t st, uint32_t* rounds_run) {
+    trb_status r = ensure_adaptive(s);
+    if (r != TRB_OK) return r;
+    const uint64_t per_block = (uint64_t)64 * std::max(sch.min, sch.step); // paths of one block in the largest round
+    if (per_block >= (1ull << 30)) return fail(TRB_INVALID_ARG, "Adaptive sampler: one block of one round exceeds 2^30 paths");
+    uint64_t want = std::min<uint64_t>((uint64_t)nb * per_block, std::min<uint64_t>(std::max<uint64_t>(s->tune.pass_paths, 64), (1ull << 30) - 64));
+    want = ((std::max(want, per_block) + 63) / 64) * 64;
+    if (want > s->wf_capacity) {
+        while ((r = ensure_wavefront(s, (size_t)want)) == TRB_OOM && want / 2 >= per_block && want > (1u << 16)) want = ((want / 2 + 63) / 64) * 64;
+        if (r != TRB_OK) return r;
+    }
+    const uint64_t cap = want;
+    rp.ad_state = s->d_ad_state;
+    rp.ad_min = sch.min; rp.ad_max = sch.max; rp.ad_step = sch.step; rp.ad_max_per_pixel = sch.max_per_pixel;
+    rp.spp = sch.max; rp.ad_time_len = sch.max;
+    const unsigned init_grid = (unsigned)std::min<size_t>(((size_t)nb * 64 + 255) / 256, (size_t)s->sm_count * 8);
+    trb::k_ad_init<<<std::max(1u, init_grid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, s->d_ad_list[0], s->d_ad_index[0]);
+    g_launches++;
+    int cur = 0;
+    uint32_t n_cur = nb;
+    *rounds_run = 0;
+    for (uint32_t round = 0; round < sch.rounds && n_cur > 0; ++round) {
+        const uint32_t count = trbh::ad_count(sch, round);
+        rp.ad_round = round; rp.sample_first = trbh::ad_slot_base(sch, round); rp.sample_count = count;
+        rp.ld_offset = trbh::ad_offset(sch, round); rp.ad_pos_len = count;
+        const uint32_t bp = (uint32_t)std::max<uint64_t>(1, cap / ((uint64_t)64 * count));
+        for (uint32_t b0 = 0; b0 < n_cur; b0 += bp) {
+            rp.blocks = s->d_ad_list[cur] + b0; rp.n_blocks = std::min(bp, n_cur - b0); rp.ad_block_index = s->d_ad_index[cur] + b0;
+            r = launch_wavefront(s, rp, flags, 0, st);
+            if (r != TRB_OK) return r;
+            const unsigned dgrid = (unsigned)std::min<size_t>(((size_t)rp.n_blocks * 64 + 127) / 128, (size_t)s->sm_count * 16);
+            trb::k_ad_decide<<<dgrid, 128, 0, st>>>(s->ds, rp, s->wf, s->d_ad_flags + b0);
+            g_launches++;
+        }
+        ++*rounds_run;
+        if (round + 1 == sch.rounds) break;
+        trb::k_ad_compact<<<1, 1024, 0, st>>>(s->d_ad_flags, n_cur, s->d_ad_list[cur], s->d_ad_index[cur], s->d_ad_list[cur ^ 1], s->d_ad_index[cur ^ 1], s->d_ad_count);
+        g_launches++;
+        CU(cudaMemcpyAsync(&n_cur, s->d_ad_count, sizeof n_cur, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        cur ^= 1;
+    }
+    const unsigned sgrid = (unsigned)std::min<size_t>(((size_t)nb * 64 + 255) / 256, (size_t)s->sm_count * 8);
+    trb::k_ad_pixel_spp<<<std::max(1u, sgrid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, s->d_ad_spp);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// the selection's host block list (bx, by pairs) of a device list made by ensure_blocks
+const std::vector<uint32_t>* host_blocks(const trb_scene* s, const uint2* d_blocks) {
+    for (const BlockList& b : s->block_lists) if (b.dev == d_blocks) return &b.host;
+    return nullptr;
+}
+// d_ad_spp (selection order) -> pixel_spp[y * width + x] for the selected pixels
+trb_status adaptive_pixel_spp_out(trb_scene* s, const uint2* d_blocks, uint32_t nb, uint32_t* pixel_spp) {
+    if (!pixel_spp || nb == 0) return TRB_OK;
+    const std::vector<uint32_t>* hb = host_blocks(s, d_blocks);
+    if (!hb) return fail(TRB_CUDA, "block list not found");
+    std::vector<uint32_t> v((size_t)nb * 64);
+    CU(cudaMemcpy(v.data(), s->d_ad_spp, v.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    for (uint32_t b = 0; b < nb; ++b)
+        for (uint32_t k = 0; k < 64; ++k)
+            pixel_spp[((*hb)[2 * b + 1] * 8 + k / 8) * (size_t)s->film.width + (*hb)[2 * b] * 8 + k % 8] = v[(size_t)b * 64 + k];
     return TRB_OK;
 }
 
@@ -1170,6 +1284,126 @@ trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n,
     cudaFree(d_out);
     CU(e);
     r = check_error_flag(s);
+    if (r != TRB_OK) return r;
+    if (stats) {
+        trb::DStats h;
+        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
+        std::memset(stats, 0, sizeof *stats);
+        stats_out(h, stats);
+        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
+    }
+    return TRB_OK;
+}
+
+trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {
+    if (!ad) return fail(TRB_INVALID_ARG, "null argument");
+    trbh::AdSchedule sch;
+    if (!trbh::ad_schedule(ad->min_spp, ad->max_spp, sch))
+        return fail(TRB_INVALID_ARG, "Adaptive sampler: max_spp < min_spp after rounding up to powers of two (the reference panics), or more than 2^24");
+    if (min_spp) *min_spp = sch.min;
+    if (max_spp) *max_spp = sch.max;
+    if (step) *step = sch.step;
+    if (max_per_pixel) *max_per_pixel = sch.max_per_pixel;
+    return TRB_OK;
+}
+
+trb_status trb_host_adaptive_decide(const trb_adaptive* ad, const float* lum, size_t n, uint32_t* samples_taken, float* avg) {
+    if (!ad || (n && !lum) || !samples_taken) return fail(TRB_INVALID_ARG, "null argument");
+    trbh::AdSchedule sch;
+    if (!trbh::ad_schedule(ad->min_spp, ad->max_spp, sch)) return fail(TRB_INVALID_ARG, "Adaptive sampler: max_spp < min_spp after rounding up to powers of two");
+    trbh::AdPixel p = trbh::ad_initial();
+    for (uint32_t round = 0; round < sch.rounds; ++round) {
+        const uint32_t first = trbh::ad_slot_base(sch, round), count = trbh::ad_count(sch, round);
+        if ((uint64_t)first + count > n) return fail(TRB_INVALID_ARG, "luminance sequence ends before the pixel stops sampling");
+        for (uint32_t k = 0; k < count; ++k) trbh::ad_add(p, first + k, lum[first + k], round == 0);
+        if (!trbh::ad_finish(p, sch, round)) break;
+    }
+    *samples_taken = p.taken & ~trbh::AD_ACTIVE;
+    if (avg) *avg = p.avg;
+    return TRB_OK;
+}
+
+trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
+    if (!s || !cfg || !ad || !film) return fail(TRB_INVALID_ARG, "null argument");
+    trbh::AdSchedule sch;
+    trb_status r = adaptive_check(s, cfg, ad, sch);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    float update_ms = 0.f;
+    if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) { // Exec::render: scene.update_frame first (multithreaded.rs:57-60)
+        auto t0 = std::chrono::steady_clock::now();
+        const float step = s->film.scene_time / (float)s->film.frames;
+        r = trb_scene_update_frame(s, cfg->current_frame, (float)cfg->current_frame * step, ((float)cfg->current_frame + 1.0f) * step);
+        if (r != TRB_OK) return r;
+        update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
+    uint32_t nb;
+    const uint2* d_blocks = nullptr;
+    r = ensure_blocks(s, cfg, &d_blocks, &nb);
+    if (r != TRB_OK) return r;
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
+    CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
+    CU(cudaEventRecord(s->ev0, 0));
+    uint32_t rounds = 0;
+    if (nb) { // an empty selection renders nothing (block_queue.rs:42-44)
+        trb::RenderParams rp{};
+        rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = s->d_film; rp.stats = s->d_stats; rp.error_flag = s->d_error;
+        r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, &rounds);
+        if (r != TRB_OK) return r;
+    }
+    CU(cudaEventRecord(s->ev1, 0));
+    CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, 0));
+    CU(cudaStreamSynchronize(0));
+    r = check_error_flag(s);
+    if (r != TRB_OK) return r;
+    for (size_t i = 0; i < npx * 4; ++i) film[i] += s->h_film_staging[i]; // additive, like trb_render
+    r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
+    if (r != TRB_OK) return r;
+    if (stats) {
+        trb::DStats h;
+        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
+        std::memset(stats, 0, sizeof *stats);
+        stats_out(h, stats);
+        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
+        stats->update_ms = update_ms;
+    }
+    return TRB_OK;
+}
+
+trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, uint32_t* pixel_spp,
+                                       trb_stats* stats) {
+    if (!s || !cfg || !ad || !samples) return fail(TRB_INVALID_ARG, "null argument");
+    trbh::AdSchedule sch;
+    trb_status r = adaptive_check(s, cfg, ad, sch);
+    if (r != TRB_OK) return r;
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    CU(cudaSetDevice(s->device));
+    uint32_t nb;
+    const uint2* d_blocks = nullptr;
+    r = ensure_blocks(s, cfg, &d_blocks, &nb);
+    if (r != TRB_OK) return r;
+    if (n != (size_t)nb * 64 * sch.max_per_pixel) return fail(TRB_INVALID_ARG, "sample buffer size must be blocks*64*max_per_pixel");
+    if (n == 0) return TRB_OK;
+    trb_sample* d_out = nullptr;
+    CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
+    cudaError_t e = cudaMemsetAsync(d_out, 0, n * sizeof(trb_sample), 0); // unused slots stay zero
+    if (e != cudaSuccess) { cudaFree(d_out); CU(e); }
+    CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
+    CU(cudaEventRecord(s->ev0, 0));
+    trb::RenderParams rp{};
+    rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
+    uint32_t rounds = 0;
+    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, &rounds);
+    if (r != TRB_OK) { cudaDeviceSynchronize(); cudaFree(d_out); return r; }
+    CU(cudaEventRecord(s->ev1, 0));
+    e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
+    cudaFree(d_out);
+    CU(e);
+    r = check_error_flag(s);
+    if (r != TRB_OK) return r;
+    r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
     if (r != TRB_OK) return r;
     if (stats) {
         trb::DStats h;

@@ -167,6 +167,7 @@ __host__ __device__ __forceinline__ uint32_t permute_index(uint32_t i, uint32_t 
 
 // stream addressing (DESIGN.md "RNG")
 constexpr uint32_t PIXEL_STREAM = 0xffffffffU;
+constexpr uint32_t AD_PIXEL_STREAM0 = 0xfffffffeU; // Adaptive sampler, round r: AD_PIXEL_STREAM0 - r (camera-sample slots stay below 2^25)
 enum { PX_POS0 = 0, PX_POS1 = 1, PX_POS_PERM = 2, PX_TIME = 3, PX_TIME_PERM = 4 };
 enum { S_L0 = 0, S_L1 = 1, S_L_PERM = 2, S_B0 = 3, S_B1 = 4, S_B_PERM = 5, S_P0 = 6, S_P1 = 7, S_P_PERM = 8,
        S_LC = 9, S_LC_PERM = 10, S_BC = 11, S_BC_PERM = 12, S_PC = 13, S_PC_PERM = 14, S_RR = 32 };

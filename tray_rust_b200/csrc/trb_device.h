@@ -166,6 +166,14 @@ struct RenderParams {
     void* samples_out;     // trb_sample*, mode 1
     DStats* stats;
     int* error_flag;
+    // Adaptive sampler round (zero for LowDiscrepancy): entry s of the round is sample_02(perm_pos(s) + ld_offset) at slot
+    // sample_first + s (DESIGN.md §2 "Adaptive sampler"). The per-path sample arrays read ld_offset, LowDiscrepancy's is 0.
+    uint32_t ld_offset;
+    uint32_t ad_pos_len, ad_time_len; // permutation lengths of the positions (the round's count) and the times (max_spp)
+    uint32_t ad_round;                // round index: pixel streams (seed, pixel, 0xfffffffe - round, dim)
+    uint4* ad_state;                  // per image pixel trbh::AdPixel; nullptr: LowDiscrepancy
+    const uint32_t* ad_block_index;   // index of each pass block in the caller's selected block list (parity records)
+    uint32_t ad_min, ad_max, ad_step, ad_max_per_pixel;
 };
 
 } // namespace trb

@@ -18,6 +18,7 @@
 #include "trb_device.h"
 #include "trb_detmath.cuh"
 #include "trb_anim.h"
+#include "trb_adaptive.h"
 #include "../../include/trb.h"
 
 namespace trb {
@@ -1348,14 +1349,15 @@ __device__ float shape_pdf(uint32_t shape, float p0, float p1, f3 pt, f3 wi) {
 struct PathRng {
     uint32_t h;   // hash state after (seed, pixel, sample)
     uint32_t len; // max_depth + 1 (path.rs:48)
+    uint32_t off; // LD offset of ld::sample_2d / sample_1d: 0 for LowDiscrepancy (ld.rs:57,62), samples_taken for Adaptive (adaptive.rs:110,115)
     __device__ __forceinline__ uint32_t draw(uint32_t dim) const { return rng_absorb(h, dim); }
     __device__ __forceinline__ void two_d(uint32_t b, uint32_t d0, uint32_t d1, uint32_t dp, float& x, float& y) const {
-        const uint32_t i = permute_index(b, len, draw(dp));
+        const uint32_t i = permute_index(b, len, draw(dp)) + off;
         x = ld_vdc(i, scramble_of(draw(d0)));
         y = ld_sobol(i, scramble_of(draw(d1)));
     }
     __device__ __forceinline__ float one_d(uint32_t b, uint32_t d0, uint32_t dp) const {
-        return ld_vdc(permute_index(b, len, draw(dp)), scramble_of(draw(d0)));
+        return ld_vdc(permute_index(b, len, draw(dp)) + off, scramble_of(draw(d0)));
     }
 };
 
@@ -1497,8 +1499,8 @@ __device__ __forceinline__ void bounce_emission(const DScene& sc, uint32_t hit_i
 }
 template <bool ANIM, int KIND = -1>
 __device__ __forceinline__ void bounce_direct(const DScene& sc, const Mat& m, const Frame& fr, f3 wo, uint32_t bounce, uint32_t hsample, float time, DirectSetup& ds,
-                                              uint32_t& light, const float* xf_row = nullptr) {
-    PathRng rng; rng.h = hsample; rng.len = sc.max_depth + 1;
+                                              uint32_t& light, const float* xf_row = nullptr, uint32_t ld_off = 0) {
+    PathRng rng; rng.h = hsample; rng.len = sc.max_depth + 1; rng.off = ld_off;
     float l0, l1, b0, b1;
     rng.two_d(bounce, S_L0, S_L1, S_L_PERM, l0, l1);
     rng.two_d(bounce, S_B0, S_B1, S_B_PERM, b0, b1);
@@ -1510,8 +1512,8 @@ __device__ __forceinline__ void bounce_direct(const DScene& sc, const Mat& m, co
 }
 struct ScatterOut { f3 throughput, next_d; bool specular, terminate; };
 template <int KIND = -1>
-__device__ __forceinline__ void bounce_scatter(const DScene& sc, const Mat& m, const Frame& fr, f3 wo, uint32_t bounce, uint32_t hsample, f3 throughput_in, ScatterOut& o) {
-    PathRng rng; rng.h = hsample; rng.len = sc.max_depth + 1;
+__device__ __forceinline__ void bounce_scatter(const DScene& sc, const Mat& m, const Frame& fr, f3 wo, uint32_t bounce, uint32_t hsample, f3 throughput_in, ScatterOut& o, uint32_t ld_off = 0) {
+    PathRng rng; rng.h = hsample; rng.len = sc.max_depth + 1; rng.off = ld_off;
     float q0, q1;
     rng.two_d(bounce, S_P0, S_P1, S_P_PERM, q0, q1);
     const float qc = rng.one_d(bounce, S_PC, S_PC_PERM);
@@ -1534,18 +1536,19 @@ __device__ __forceinline__ void bounce_scatter(const DScene& sc, const Mat& m, c
 }
 template <bool ANIM>
 __device__ __forceinline__ void shade_bounce(const DScene& sc, const Surf& s, uint32_t hit_inst, f3 ray_d, f3 first_ng, uint32_t bounce, bool prev_specular,
-                                             uint32_t hsample, f3 throughput_in, float time, f3& illum, BounceOut& o, const float* xf_row = nullptr) {
+                                             uint32_t hsample, f3 throughput_in, float time, f3& illum, BounceOut& o, const float* xf_row = nullptr,
+                                             uint32_t ld_off = 0) {
     bounce_emission<ANIM>(sc, hit_inst, ray_d, first_ng, bounce, prev_specular, throughput_in, time, illum);
     Mat m;
     load_mat_at(sc, __ldg(&sc.instances[hit_inst].material), s.u, s.v, time, m);
     Frame fr;
     make_frame(s, fr);
     const f3 wo = -ray_d;
-    bounce_direct<ANIM>(sc, m, fr, wo, bounce, hsample, time, o.ds, o.light, xf_row);
+    bounce_direct<ANIM>(sc, m, fr, wo, bounce, hsample, time, o.ds, o.light, xf_row, ld_off);
     o.t_before = throughput_in;
     o.org = fr.p;
     ScatterOut so;
-    bounce_scatter(sc, m, fr, wo, bounce, hsample, throughput_in, so);
+    bounce_scatter(sc, m, fr, wo, bounce, hsample, throughput_in, so, ld_off);
     o.throughput = so.throughput; o.next_d = so.next_d; o.specular = so.specular; o.terminate = so.terminate;
 }
 
@@ -1821,6 +1824,28 @@ __device__ __forceinline__ void sample_position(const RenderParams& rp, const Pi
     sx = ld_vdc(ip, ps.scr0) + (float)id.px;
     sy = ld_sobol(ip, ps.scr1) + (float)id.py;
     tm = ld_vdc(permute_index(id.si, rp.spp, ps.ktime), ps.scrt);
+}
+// Adaptive sampler, round r (adaptive.rs:82-117): every round draws fresh scrambles and shuffle keys from the pixel stream
+// (seed, pixel, 0xfffffffe - r, dim), next to LowDiscrepancy's (seed, pixel, 0xffffffff, dim); slots stay below 2^25.
+__device__ __forceinline__ PixelStreams pixel_streams_round(uint32_t seed, uint32_t pixel, uint32_t round) {
+    PixelStreams p;
+    p.hpix = rng_absorb(rng_seed(seed), pixel);
+    const uint32_t hs = rng_absorb(p.hpix, AD_PIXEL_STREAM0 - round);
+    p.scr0 = scramble_of(rng_absorb(hs, PX_POS0));
+    p.scr1 = scramble_of(rng_absorb(hs, PX_POS1));
+    p.kpos = rng_absorb(hs, PX_POS_PERM);
+    p.scrt = scramble_of(rng_absorb(hs, PX_TIME));
+    p.ktime = rng_absorb(hs, PX_TIME_PERM);
+    return p;
+}
+// entry s = si - sample_first of the round: position sample_02(perm_count(s) + offset), time vdc(perm_max(s) + offset)
+// (thread_work sizes time_samples by max_spp and zips its first entries, multithreaded.rs:76,93-94)
+__device__ __forceinline__ void sample_position_ad(const RenderParams& rp, const PixelStreams& ps, const SampleId& id, float& sx, float& sy, float& tm) {
+    const uint32_t s = id.si - rp.sample_first;
+    const uint32_t ip = permute_index(s, rp.ad_pos_len, ps.kpos) + rp.ld_offset;
+    sx = ld_vdc(ip, ps.scr0) + (float)id.px;
+    sy = ld_sobol(ip, ps.scr1) + (float)id.py;
+    tm = ld_vdc(permute_index(s, rp.ad_time_len, ps.ktime) + rp.ld_offset, ps.scrt);
 }
 
 // warp-aggregated append: every lane of the warp must call it
@@ -2266,7 +2291,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ 
                     const SampleId id = sample_id(sc, rp, p);
                     const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
                     BounceOut o;
-                    shade_bounce<ANIM>(sc, s, h.inst, ray.d, first_ng, round, (fl & WF_F_SPECULAR) != 0, hs, mk(th4.x, th4.y, th4.z), time, illum, o, xf_row);
+                    shade_bounce<ANIM>(sc, s, h.inst, ray.d, first_ng, round, (fl & WF_F_SPECULAR) != 0, hs, mk(th4.x, th4.y, th4.z), time, illum, o, xf_row, rp.ld_offset);
                     const uint32_t nf = (o.specular ? WF_F_SPECULAR : 0u) | (o.terminate ? WF_F_TERMINATE : 0u) | (o.ds.has_shadow ? WF_F_SHADOW : 0u) |
                                         (o.ds.has_mis ? WF_F_MIS : 0u);
                     push_cont = !o.terminate; push_shadow = o.ds.has_shadow; push_mis = o.ds.has_mis;
@@ -2554,7 +2579,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_b(const __grid_constant_
             const SampleId id = sample_id(sc, rp, p);
             const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
             DirectSetup ds; uint32_t light;
-            bounce_direct<ANIM, KIND>(sc, m, fr, wo, round, hs, th4.w, ds, light, wf_xf_row<ANIM>(wf, p));
+            bounce_direct<ANIM, KIND>(sc, m, fr, wo, round, hs, th4.w, ds, light, wf_xf_row<ANIM>(wf, p), rp.ld_offset);
             push_shadow = ds.has_shadow; push_mis = ds.has_mis;
             wf.org[p] = make_float4(fr.p.x, fr.p.y, fr.p.z, __uint_as_float((push_shadow ? WF_F_SHADOW : 0u) | (push_mis ? WF_F_MIS : 0u)));
             if (push_shadow) wf.shadow[p] = make_float4(ds.shadow_d.x, ds.shadow_d.y, ds.shadow_d.z, 0.0f);
@@ -2601,7 +2626,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
             const SampleId id = sample_id(sc, rp, p);
             const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
             ScatterOut so;
-            bounce_scatter<KIND>(sc, m, fr, wo, round, hs, mk(th4.x, th4.y, th4.z), so);
+            bounce_scatter<KIND>(sc, m, fr, wo, round, hs, mk(th4.x, th4.y, th4.z), so, rp.ld_offset);
             const uint32_t fb = __float_as_uint(wf.org[p].w); // WF_F_SHADOW | WF_F_MIS from k_wf_shade_b
             push_cont = !so.terminate;
             push_active = push_cont || (fb & (WF_F_SHADOW | WF_F_MIS)) != 0u;
@@ -2623,6 +2648,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
 }
 
 // RenderTarget::write for a whole pass: one CTA per 8x8 block, footprint accumulated in shared memory.
+template <bool ADAPT = false>
 __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
     extern __shared__ float4 tile[];
     __shared__ float s_table[256];
@@ -2636,14 +2662,16 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constan
         const uint2 blk = rp.blocks[item];
         const uint32_t bx = blk.x * 8, by = blk.y * 8;
         SampleId id; id.item = item; id.pix = pix; id.px = bx + (pix & 7); id.py = by + (pix >> 3); id.pixel = id.py * sc.width + id.px;
-        const PixelStreams ps = pixel_streams(rp.seed, id.pixel);
+        const PixelStreams ps = ADAPT ? pixel_streams_round(rp.seed, id.pixel, rp.ad_round) : pixel_streams(rp.seed, id.pixel);
+        const bool on = !ADAPT || (rp.ad_state[id.pixel].x & trbh::AD_ACTIVE) != 0u; // Adaptive: pixels that took this round's samples
         const int x_lo = max((int)bx - sc.fpw_x, 0), x_hi = min((int)bx + 8 + sc.fpw_x, (int)sc.width - 1);
         const int y_lo = max((int)by - sc.fpw_y, 0), y_hi = min((int)by + 8 + sc.fpw_y, (int)sc.height - 1);
         const int tx0 = (int)bx - sc.fpw_x, ty0 = (int)by - sc.fpw_y;
-        for (uint32_t s = lane_s; s < rp.sample_count; s += 2) {
+        for (uint32_t s = lane_s; on && s < rp.sample_count; s += 2) {
             id.si = rp.sample_first + s;
             float sx, sy, tm;
-            sample_position(rp, ps, id, sx, sy, tm);
+            if (ADAPT) sample_position_ad(rp, ps, id, sx, sy, tm);
+            else sample_position(rp, ps, id, sx, sy, tm);
             const float4 c4 = wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s];
             splat_sample(sc, tile, s_table, T, tx0, ty0, x_lo, x_hi, y_lo, y_hi, id.px, id.py, sx, sy, mk(c4.x, c4.y, c4.z));
         }
@@ -2665,6 +2693,7 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constan
 // in lockstep (same (dy, dx) offset at the same time, __syncwarp per offset), so their targets are always 32 different tile
 // pixels and a plain 16-byte read-modify-write is race-free; the four copies are summed at the flush. Same weights and
 // products as RenderTarget::write; only the order of the float additions differs (the film bar is an RMSE tolerance).
+template <bool ADAPT = false>
 __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
     extern __shared__ float4 tiles[]; // 4 x T*T
     __shared__ float s_table[256];
@@ -2680,15 +2709,19 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_cons
         const uint2 blk = rp.blocks[item];
         const uint32_t bx = blk.x * 8, by = blk.y * 8;
         SampleId id; id.item = item; id.pix = pix; id.px = bx + (pix & 7); id.py = by + (pix >> 3); id.pixel = id.py * sc.width + id.px;
-        const PixelStreams ps = pixel_streams(rp.seed, id.pixel);
+        const PixelStreams ps = ADAPT ? pixel_streams_round(rp.seed, id.pixel, rp.ad_round) : pixel_streams(rp.seed, id.pixel);
+        // Adaptive: a pixel that took no samples this round walks the footprint with the others (the __syncwarp lockstep below
+        // is what makes the plain read-modify-write race-free) but writes nothing
+        const bool on = !ADAPT || (rp.ad_state[id.pixel].x & trbh::AD_ACTIVE) != 0u;
         const int x_lo = max((int)bx - sc.fpw_x, 0), x_hi = min((int)bx + 8 + sc.fpw_x, (int)sc.width - 1);
         const int y_lo = max((int)by - sc.fpw_y, 0), y_hi = min((int)by + 8 + sc.fpw_y, (int)sc.height - 1);
         const int tx0 = (int)bx - sc.fpw_x, ty0 = (int)by - sc.fpw_y;
         for (uint32_t s = lane_s; s < rp.sample_count; s += 2) { // uniform trip count inside a warp (one lane_s per warp)
             id.si = rp.sample_first + s;
             float sx, sy, tm;
-            sample_position(rp, ps, id, sx, sy, tm);
-            const float4 c4 = wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s];
+            if (ADAPT) sample_position_ad(rp, ps, id, sx, sy, tm);
+            else sample_position(rp, ps, id, sx, sy, tm);
+            const float4 c4 = on ? wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s] : make_float4(0.f, 0.f, 0.f, 0.f);
             const float img_x = sx - 0.5f, img_y = sy - 0.5f;
             for (int dy = -ry; dy <= ry + 1; ++dy) {
                 const int iy = (int)id.py + dy;
@@ -2699,7 +2732,7 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_cons
                 for (int dx = -rx; dx <= rx + 1; ++dx) {
                     const int ix = (int)id.px + dx;
                     const float fx = fabsf((float)ix - img_x) * sc.filter_inv_w;
-                    if (vy && ix >= x_lo && ix <= x_hi && !(fx > sc.filter_w) && (!sc.film_block_filter || lock_block_takes(sx, ix, x_lo, x_hi, sc.fpw_x))) {
+                    if (on && vy && ix >= x_lo && ix <= x_hi && !(fx > sc.filter_w) && (!sc.film_block_filter || lock_block_takes(sx, ix, x_lo, x_hi, sc.fpw_x))) {
                         const uint32_t fxi = min(f2u(fx * 16.0f), 15u);
                         const float wgt = s_table[fyi * 16 + fxi];
                         float4* t = &mine[(iy - ty0) * T + (ix - tx0)];
@@ -2862,6 +2895,136 @@ __global__ void k_srgb8(size_t n, const float4* __restrict__ film, uint8_t* __re
             }
         }
         rgb8[3 * i] = o[0]; rgb8[3 * i + 1] = o[1]; rgb8[3 * i + 2] = o[2];
+    }
+}
+
+// ==========================================================================================
+// Adaptive sampler (src/sampler/adaptive.rs driven by thread_work, multithreaded.rs:72-114; DESIGN.md §2 and §5). A render is
+// a sequence of rounds over the selected blocks; a round is cut into passes by block sub-ranges only, so one pass holds all of a
+// pixel's samples of the round. Per pass: k_wf_generate_ad, the unchanged trace / shade rounds (the per-path sample arrays get
+// the round's LD offset), the film kernels' ADAPT variant, then k_ad_decide. Between rounds k_ad_compact keeps the blocks that
+// still have a pixel sampling.
+// ==========================================================================================
+// A pass's path p = (block, pixel, entry) as in LowDiscrepancy, slot = sample_first + entry. Only the paths of pixels that are
+// still sampling are queued for the primary trace (warp-aggregated push) and counted as camera samples; the others enter shade
+// round 0 as primary misses, which only writes a black sample that neither the film nor the decision reads.
+template <bool ANIM>
+__global__ void __launch_bounds__(256) k_wf_generate_ad(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
+    const uint32_t n = wf.n_paths;
+    const uint32_t lane = threadIdx.x & 31, stride = gridDim.x * blockDim.x;
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p - lane < n; p += stride) { // whole warps iterate (wf_push)
+        bool on = false;
+        if (p < n) {
+            const SampleId id = sample_id(sc, rp, p);
+            on = (rp.ad_state[id.pixel].x & trbh::AD_ACTIVE) != 0u;
+            float time = 0.0f;
+            if (on) {
+                const PixelStreams ps = pixel_streams_round(rp.seed, id.pixel, rp.ad_round);
+                float sx, sy, tm;
+                sample_position_ad(rp, ps, id, sx, sy, tm);
+                Ray ray;
+                time = camera_ray<ANIM>(sc, sx, sy, tm, ray);
+                wf.org[p] = make_float4(ray.o.x, ray.o.y, ray.o.z, __uint_as_float(0u));
+                wf.cont[p] = make_float4(ray.d.x, ray.d.y, ray.d.z, finf());
+            } else {
+                wf.org[p] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0u));
+                wf.cont[p] = make_float4(0.0f, 0.0f, 0.0f, finf());
+                wf.hit[p] = make_uint4(TRB_MISS, 0u, 0u, 0u);
+            }
+            wf.thr[p] = make_float4(1.0f, 1.0f, 1.0f, time);
+            wf.illum[p] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, on);
+        wf_push(wf.q_cont, &wf.counters[WF_N_CONT], on, p);
+        if (lane == 0 && m && rp.stats) atomicAdd(&rp.stats->camera_samples, (unsigned long long)__popc(m));
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) wf.counters[WF_N_ACTIVE] = n; // shade round 0 walks every path of the pass
+    if (blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid
+        uint32_t* b = wf.bounds + threadIdx.x * 8;
+        b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
+    }
+}
+
+// report_results for every pixel of the pass that sampled this round: fold the round's luminances in slot order into the
+// 16-byte state (trb_adaptive.h), decide, flag the block when the pixel goes on. With samples_out: the parity records
+// (trb_render_samples_adaptive), max_per_pixel slots per pixel in the caller's block order.
+__global__ void __launch_bounds__(128) k_ad_decide(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
+                                                   uint32_t* block_flags) {
+    trbh::AdSchedule sch;
+    sch.min = rp.ad_min; sch.max = rp.ad_max; sch.step = rp.ad_step; sch.max_per_pixel = rp.ad_max_per_pixel; sch.rounds = 0;
+    const uint32_t n = rp.n_blocks * 64;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        SampleId id;
+        id.item = t >> 6; id.pix = t & 63;
+        const uint2 blk = rp.blocks[id.item];
+        id.px = blk.x * 8 + (id.pix & 7); id.py = blk.y * 8 + (id.pix >> 3); id.pixel = id.py * sc.width + id.px;
+        const uint4 st4 = rp.ad_state[id.pixel];
+        if (!(st4.x & trbh::AD_ACTIVE)) continue;
+        trbh::AdPixel st; st.taken = st4.x; st.avg = __uint_as_float(st4.y); st.lmin = __uint_as_float(st4.z); st.lmax = __uint_as_float(st4.w);
+        PixelStreams ps;
+        if (rp.samples_out) ps = pixel_streams_round(rp.seed, id.pixel, rp.ad_round);
+        for (uint32_t s = 0; s < rp.sample_count; ++s) {
+            const float4 c = wf.rad[(size_t)t * rp.sample_count + s];
+            const uint32_t slot = rp.sample_first + s;
+            trbh::ad_add(st, slot, trbh::ad_luminance(c.x, c.y, c.z), rp.ad_round == 0);
+            if (rp.samples_out) {
+                id.si = slot;
+                float sx, sy, tm;
+                sample_position_ad(rp, ps, id, sx, sy, tm);
+                trb_sample* out = reinterpret_cast<trb_sample*>(rp.samples_out) + ((size_t)rp.ad_block_index[id.item] * 64 + id.pix) * rp.ad_max_per_pixel + slot;
+                out->x = sx; out->y = sy; out->r = c.x; out->g = c.y; out->b = c.z;
+            }
+        }
+        const bool more = trbh::ad_finish(st, sch, rp.ad_round);
+        rp.ad_state[id.pixel] = make_uint4(st.taken, __float_as_uint(st.avg), __float_as_uint(st.lmin), __float_as_uint(st.lmax));
+        if (more) block_flags[id.item] = 1u;
+    }
+}
+
+// Start of a render: every pixel of the selected blocks samples round 0; the round list starts as the selection.
+__global__ void k_ad_init(const __grid_constant__ DScene sc, const uint2* blocks, uint32_t n_blocks, uint4* state, uint2* list, uint32_t* list_index) {
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_blocks * 64; t += gridDim.x * blockDim.x) {
+        const uint2 blk = blocks[t >> 6];
+        const uint32_t pixel = (blk.y * 8 + ((t & 63) >> 3)) * sc.width + blk.x * 8 + (t & 7);
+        const trbh::AdPixel p = trbh::ad_initial();
+        state[pixel] = make_uint4(p.taken, __float_as_uint(p.avg), __float_as_uint(p.lmin), __float_as_uint(p.lmax));
+        if ((t & 63) == 0) { list[t >> 6] = blk; list_index[t >> 6] = t >> 6; }
+    }
+}
+
+// Order-preserving compaction of the round's block list to the blocks flagged by k_ad_decide (one CTA; at most ~32 K blocks
+// at 1080p). Clears the flags it read. out_count: the new length (read back by the host: 4 bytes per round).
+__global__ void __launch_bounds__(1024) k_ad_compact(uint32_t* flags, uint32_t n, const uint2* in_list, const uint32_t* in_index,
+                                                     uint2* out_list, uint32_t* out_index, uint32_t* out_count) {
+    __shared__ uint32_t part[1024];
+    __shared__ uint32_t base;
+    if (threadIdx.x == 0) base = 0;
+    for (uint32_t c0 = 0; c0 < n; c0 += 1024) {
+        const uint32_t i = c0 + threadIdx.x;
+        const uint32_t f = i < n && flags[i] ? 1u : 0u;
+        __syncthreads();
+        part[threadIdx.x] = f;
+        __syncthreads();
+        for (uint32_t s = 1; s < 1024; s <<= 1) { // Hillis-Steele inclusive scan
+            const uint32_t v = threadIdx.x >= s ? part[threadIdx.x - s] : 0u;
+            __syncthreads();
+            part[threadIdx.x] += v;
+            __syncthreads();
+        }
+        if (f) { const uint32_t o = base + part[threadIdx.x] - 1u; out_list[o] = in_list[i]; out_index[o] = in_index[i]; }
+        if (i < n) flags[i] = 0u;
+        __syncthreads();
+        if (threadIdx.x == 1023) base += part[1023];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *out_count = base;
+}
+
+// Samples per pixel of the selected blocks (the reference's per-pixel count: samples_taken when report_results let go)
+__global__ void k_ad_pixel_spp(const __grid_constant__ DScene sc, const uint2* blocks, uint32_t n_blocks, const uint4* state, uint32_t* spp) {
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_blocks * 64; t += gridDim.x * blockDim.x) {
+        const uint2 blk = blocks[t >> 6];
+        spp[(size_t)t] = state[(blk.y * 8 + ((t & 63) >> 3)) * sc.width + blk.x * 8 + (t & 7)].x & ~trbh::AD_ACTIVE;
     }
 }
 

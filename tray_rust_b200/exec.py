@@ -29,6 +29,14 @@ class FrameInfo:
     end: int = 0
 
 
+@dataclasses.dataclass(frozen=True)
+class Adaptive:
+    """sampler::Adaptive (sampler/adaptive.rs): min_spp per pixel, then more in rounds while the pixel's samples disagree,
+    up to about max_spp. Both are rounded up to powers of two."""
+    min_spp: int
+    max_spp: int
+
+
 @dataclasses.dataclass
 class Config:
     """exec::Config. ``num_threads`` is accepted for signature compatibility and ignored (the GPU decides).
@@ -41,6 +49,7 @@ class Config:
     current_frame: int = 0
     select_blocks: tuple = (0, 0)  # (start, count) into the Morton-sorted block list; count 0 = all
     seed: int = 1
+    sampler: Adaptive = None  # None: LowDiscrepancy at ``spp``; an Adaptive value: the adaptive sampler (``spp`` unused)
 
 
 class RenderTarget:
@@ -116,16 +125,24 @@ class Exec:
 
 class B200(Exec):
     """Renders the frame ``config.current_frame`` on the scene's GPU and accumulates into ``rt``.
-    Blocking, like MultiThreaded::render. ``last_stats`` holds the ray counters of the call."""
+    Blocking, like MultiThreaded::render. ``last_stats`` holds the ray counters of the call; with an Adaptive sampler
+    ``last_pixel_spp`` holds each pixel's sample count ((height, width), zero outside the selected blocks)."""
 
     def __init__(self, samples_per_pass=0):
         self.samples_per_pass = samples_per_pass  # 0: the whole spp in one launch
         self.last_stats = None
+        self.last_pixel_spp = None
 
     def render(self, scene, rt, config):
         g = scene.gpu
         if rt.dimensions() != (g.width, g.height):
             raise ValueError("render target does not match the scene's film")
+        if config.sampler is not None:
+            _, spp, st = g.render_adaptive(config.sampler.min_spp, config.sampler.max_spp, rt.pixels, block_start=config.select_blocks[0],
+                                           block_count=config.select_blocks[1], current_frame=config.current_frame, seed=config.seed)
+            self.last_stats, self.last_pixel_spp = st, spp
+            return st
+        self.last_pixel_spp = None
         spp = config.spp if config.spp else g.spp
         spp_p2 = 1 << (max(1, spp) - 1).bit_length()
         step = self.samples_per_pass or spp_p2
