@@ -421,6 +421,30 @@ trb_status trb_render_adaptive(trb_scene* scene, const trb_render_cfg* cfg, cons
 trb_status trb_render_samples_adaptive(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, size_t n,
                                        trb_sample* samples, uint32_t* pixel_spp, trb_stats* stats);
 
+/* trb_render_adaptive with the contract of trb_render_device: the film is a DEVICE buffer on the scene's GPU (accumulated
+ * into), every round is enqueued on `cuda_stream` (a cudaStream_t; NULL = default stream) without host synchronisation,
+ * and update_frame is never called. The rounds are driven by the device: the host enqueues every round of the schedule
+ * with the passes the whole selection would need, and passes past a round's live blocks return at once. `d_pixel_spp`
+ * is NULL or a DEVICE buffer of width*height u32 with the layout of trb_render_adaptive's pixel_spp; only the selected
+ * pixels are written. `d_stats` (may be NULL) is a DEVICE trb_stats the kernels accumulate into. The first call on a
+ * scene allocates the sampler's per-pixel state (20 B per pixel), and a call that needs more path state than earlier
+ * calls grows it, as trb_render_device does; both synchronise the device once. Same one-stream-per-scene rule as
+ * trb_render_device; the same argument checks and statuses as trb_render_adaptive. */
+trb_status trb_render_adaptive_device(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* d_film_rgbw,
+                                      uint32_t* d_pixel_spp, trb_stats* d_stats, void* cuda_stream);
+
+/* trb_render_sharded with the Adaptive sampler: this rank's shard (interleaved chunks, or the reference's contiguous
+ * ranges with cfg->shard_count == 0xffffffff) runs the Adaptive rounds into the device film, then ONE reduce to `root`,
+ * whose host film_rgbw the summed film is ADDED to. pixel_spp (width*height, or NULL) receives the counts of this rank's
+ * own pixels only; other entries are left as they are. Blocking. */
+trb_status trb_render_sharded_adaptive(trb_scene* scene, trb_comm* comm, const trb_render_cfg* cfg, const trb_adaptive* adaptive,
+                                       int root, float* film_rgbw, uint32_t* pixel_spp, trb_stats* stats);
+
+/* trb_group_render with the Adaptive sampler: the replicas run their shards' rounds concurrently, then one reduce to
+ * devices[0]; each replica's pixel counts are written into the one pixel_spp (the shards are disjoint). Blocking. */
+trb_status trb_group_render_adaptive(trb_group* group, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                                     uint32_t* pixel_spp, trb_stats* stats);
+
 /* The rounded schedule of Adaptive::new (adaptive.rs:34-49); any output may be NULL. Host only. */
 trb_status trb_adaptive_schedule(const trb_adaptive* adaptive, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step,
                                  uint32_t* max_per_pixel);

@@ -3,7 +3,9 @@ against a high-spp LowDiscrepancy render of the same scene. Measures and reports
 
     python tools/adaptive_bench.py [--n 8] [--ref-spp 256] [--scenes c2,c4] [--out results/adaptive_bench.json]
 
-LD runs at N spp, Adaptive at (N/4, 4N); both one trb_render / trb_render_adaptive call each, after one warm-up call.
+LD runs at N spp, Adaptive at (N/4, 4N); both one trb_render / trb_render_adaptive call each, after one warm-up call. The
+"adaptive_device" row is the same Adaptive render through trb_render_adaptive_device on a torch stream into a device film:
+GPU time between CUDA events on that stream, and the host time the call took to enqueue every round.
 """
 import argparse
 import json
@@ -60,6 +62,29 @@ def timed(fn):
     return r, time.perf_counter() - t0
 
 
+def device_timed(g, mn, mx, seed):
+    """trb_render_adaptive_device on a non-default stream: (GPU ms between events, enqueue ms, camera samples)"""
+    import torch
+    s = torch.cuda.Stream(device=g.device)
+    film = torch.zeros((g.height, g.width, 4), dtype=torch.float32, device="cuda:%d" % g.device)
+    stats = torch.zeros(9, dtype=torch.int64, device=film.device)
+    s.wait_stream(torch.cuda.current_stream(film.device))
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    g.render_adaptive_device(mn, mx, film.data_ptr(), None, stats.data_ptr(), s.cuda_stream, seed=seed, flags=F.RENDER_NO_UPDATE)  # warm-up
+    s.synchronize()
+    film.zero_()
+    stats.zero_()
+    torch.cuda.synchronize(film.device)
+    e0.record(s)
+    t0 = time.perf_counter()
+    g.render_adaptive_device(mn, mx, film.data_ptr(), None, stats.data_ptr(), s.cuda_stream, seed=seed, flags=F.RENDER_NO_UPDATE)
+    enqueue = time.perf_counter() - t0
+    e1.record(s)
+    e1.synchronize()
+    st = F.Stats.from_buffer_copy(stats.cpu().numpy().tobytes())
+    return e0.elapsed_time(e1), enqueue * 1e3, st
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=8)
@@ -80,6 +105,9 @@ def main():
             "adaptive": {"wall_s": t_ad, "camera_samples": st_ad.camera_samples, "mrays_s": st_ad.rays_total() / t_ad / 1e6, "rmse": rmse(ad, ref),
                          "rounds": rounds_of(spp, a.n // 4, 4 * a.n), "mean_spp": float(spp.mean()), "pixels_at_min": float((spp == spp.min()).mean())},
         }
+        gpu_ms, enqueue_ms, st_dev = device_timed(g, a.n // 4, 4 * a.n, 2)
+        row["adaptive_device"] = {"gpu_ms": gpu_ms, "enqueue_ms": enqueue_ms, "camera_samples": st_dev.camera_samples,
+                                  "mrays_s": st_dev.rays_total() / gpu_ms / 1e3}
         res["scenes"][name] = row
         print(name, json.dumps(row), flush=True)
         g.close()

@@ -2,7 +2,9 @@
    torchrun --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tools/multi_gpu_check.py   # one process per GPU
    python tools/multi_gpu_check.py --group 2                                                                       # one process, 2 GPUs
 Checks trb_render_sharded (interleaved and reference-style contiguous sharding, ONE ncclReduce per frame issued by libtrb) and
-trb_group_render against the single-GPU render of the same frame: same ray counts, film equal up to float addition order."""
+trb_group_render against the single-GPU render of the same frame: same ray counts, film equal up to float addition order. The
+Adaptive cases (trb_render_sharded_adaptive, trb_group_render_adaptive) check the same against trb_render_adaptive on one GPU,
+and that every pixel's sample count is equal."""
 import json
 import os
 import sys
@@ -13,6 +15,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tray_rust_b200 import _ffi as F, api, scenebuild as SB  # noqa: E402
 
 W, H, SPP = 640, 360, 4
+AD = (2, 16)  # Adaptive (min_spp, max_spp)
+RAYS = ["camera_samples", "rays_primary", "rays_shadow", "rays_mis", "rays_continuation"]
 
 
 def desc():
@@ -32,7 +36,13 @@ def group_mode(n):
     ok = st.rays_total() == st1.rays_total() and st.camera_samples == st1.camera_samples and np.allclose(film, ref, rtol=2e-4, atol=2e-5) and np.allclose(film2, film, rtol=2e-4, atol=2e-5)
     print(json.dumps({"mode": "trb_group_render", "devices": n, "rays": st.rays_total(), "rays_single": st1.rays_total(),
                       "rmse": float(np.sqrt(np.mean((img(film) - img(ref)) ** 2))), "kernel_ms": st.kernel_ms, "kernel_ms_single": st1.kernel_ms, "ok": bool(ok)}))
-    return ok
+    aref, aspp1, ast1 = g1.render_adaptive(*AD, seed=3)
+    afilm, aspp, ast = grp.render_adaptive(*AD, seed=3)
+    aok = bool((aspp == aspp1).all()) and [getattr(ast, k) for k in RAYS] == [getattr(ast1, k) for k in RAYS] and np.allclose(afilm, aref, rtol=2e-4, atol=2e-5)
+    print(json.dumps({"mode": "trb_group_render_adaptive", "devices": n, "adaptive": AD, "rays": ast.rays_total(), "rays_single": ast1.rays_total(),
+                      "pixels_with_other_count": int((aspp != aspp1).sum()), "rmse": float(np.sqrt(np.mean((img(afilm) - img(aref)) ** 2))),
+                      "kernel_ms": ast.kernel_ms, "kernel_ms_single": ast1.kernel_ms, "ok": bool(aok)}))
+    return ok and aok
 
 
 def rank_mode():
@@ -54,6 +64,19 @@ def rank_mode():
             ref, st1 = g.render(spp=SPP, seed=3)
             good = int(t[0]) == st1.rays_total() and int(t[1]) == st1.camera_samples and np.allclose(film, ref, rtol=2e-4, atol=2e-5)
             print(json.dumps({"mode": "trb_render_sharded " + name, "ranks": world, "rays": int(t[0]), "rays_single": st1.rays_total(),
+                              "rmse": float(np.sqrt(np.mean((img(film) - img(ref)) ** 2))), "ok": bool(good)}))
+            ok = ok and good
+    for name, kw in (("interleaved", {}), ("contiguous (master.rs:91-93)", dict(shard_count=0xffffffff))):
+        film, spp, st = comm.render_sharded_adaptive(g, *AD, None, None, 0, seed=3, **kw)
+        t = torch.tensor([getattr(st, k) for k in RAYS], dtype=torch.int64)
+        dist.all_reduce(t)
+        counts = torch.from_numpy(spp.astype(np.int64))
+        dist.all_reduce(counts)                          # each rank filled in its own pixels only
+        if rank == 0:
+            ref, spp1, st1 = g.render_adaptive(*AD, seed=3)
+            good = t.tolist() == [getattr(st1, k) for k in RAYS] and bool((counts.numpy() == spp1).all()) and np.allclose(film, ref, rtol=2e-4, atol=2e-5)
+            print(json.dumps({"mode": "trb_render_sharded_adaptive " + name, "ranks": world, "adaptive": AD, "rays": int(t[1:].sum()),
+                              "rays_single": st1.rays_total(), "pixels_with_other_count": int((counts.numpy() != spp1).sum()),
                               "rmse": float(np.sqrt(np.mean((img(film) - img(ref)) ** 2))), "ok": bool(good)}))
             ok = ok and good
     dist.barrier()

@@ -149,6 +149,7 @@ TRB_SYMBOLS = [
     "trb_nccl_unique_id", "trb_comm_create", "trb_comm_destroy", "trb_comm_info", "trb_comm_reduce_film", "trb_render_sharded",
     "trb_group_create", "trb_group_load_json", "trb_group_render", "trb_group_scene", "trb_group_destroy",
     "trb_render_adaptive", "trb_render_samples_adaptive", "trb_adaptive_schedule", "trb_host_adaptive_decide",
+    "trb_render_adaptive_device", "trb_render_sharded_adaptive", "trb_group_render_adaptive",
 ]
 
 _trb = None
@@ -185,6 +186,7 @@ def load_trb():
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
+    lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]
     lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
     lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]
@@ -216,6 +218,8 @@ def load_trb():
     lib.trb_group_create.argtypes = [C.POINTER(SceneDesc), C.POINTER(C.c_int), C.c_int, C.POINTER(vp)]
     lib.trb_group_load_json.argtypes = [C.c_char_p, u32, u32, u32, C.POINTER(C.c_int), C.c_int, C.POINTER(vp)]
     lib.trb_group_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
+    lib.trb_render_sharded_adaptive.argtypes = [vp, vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), C.c_int, vp, vp, C.POINTER(Stats)]
+    lib.trb_group_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_group_scene.argtypes = [vp, C.c_int]
     lib.trb_group_scene.restype = vp
     lib.trb_group_destroy.argtypes = [vp]

@@ -166,6 +166,15 @@ class Scene(_Base):
         self._check(self._lib.trb_render_adaptive(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), F.ptr(spp), C.byref(st)))
         return film, spp, st
 
+    def render_adaptive_device(self, min_spp, max_spp, d_film_ptr, d_pixel_spp_ptr=None, d_stats_ptr=None, stream=None, **kw):
+        """trb_render_adaptive_device: the Adaptive sampler into a device film (accumulated into), enqueued on `stream` (a
+        cudaStream_t as an int, e.g. torch.cuda.Stream().cuda_stream; None = default stream) without host synchronisation.
+        d_pixel_spp_ptr: device buffer of height*width uint32 (only the selected pixels are written) or None; d_stats_ptr: a
+        device trb_stats (72 bytes) or None. Never updates the frame."""
+        cfg = _cfg(**kw)
+        self._check(self._lib.trb_render_adaptive_device(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), d_film_ptr, d_pixel_spp_ptr,
+                                                         d_stats_ptr, stream))
+
     def render_samples_adaptive(self, min_spp, max_spp, **kw):
         """trb_render_samples_adaptive: (samples (blocks, 64, max_per_pixel) flattened, unused slots zero; pixel_spp; Stats)."""
         cfg = _cfg(**kw)
@@ -241,6 +250,19 @@ class Comm:
         self._check(self._lib.trb_render_sharded(scene._h, self._h, C.byref(cfg), root, F.ptr(film) if film is not None else None, C.byref(st)))
         return film, st
 
+    def render_sharded_adaptive(self, scene, min_spp, max_spp, film=None, pixel_spp=None, root=0, **kw):
+        """trb_render_sharded_adaptive: this rank's shard with the Adaptive sampler, ONE film reduce, root adds into its host
+        film. Returns (film (None off the root), pixel_spp (height, width) uint32 with this rank's pixels filled in, Stats)."""
+        cfg = _cfg(**kw)
+        if film is None and self.rank == root:
+            film = np.zeros((scene.height, scene.width, 4), np.float32)
+        if pixel_spp is None:
+            pixel_spp = np.zeros((scene.height, scene.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_sharded_adaptive(scene._h, self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), root,
+                                                          F.ptr(film) if film is not None else None, F.ptr(pixel_spp), C.byref(st)))
+        return film, pixel_spp, st
+
     def close(self):
         if self._h is not None:
             self._lib.trb_comm_destroy(self._h)
@@ -277,6 +299,18 @@ class Group:
         if rc != F.TRB_OK:
             raise TrbError(rc, (self._lib.trb_last_error() or b"").decode())
         return film, st
+
+    def render_adaptive(self, min_spp, max_spp, film=None, **kw):
+        """trb_group_render_adaptive: the Adaptive sampler on every replica, one reduce. Returns (film, pixel_spp, Stats)."""
+        cfg = _cfg(**kw)
+        if film is None:
+            film = np.zeros((self.height, self.width, 4), np.float32)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        rc = self._lib.trb_group_render_adaptive(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), F.ptr(spp), C.byref(st))
+        if rc != F.TRB_OK:
+            raise TrbError(rc, (self._lib.trb_last_error() or b"").decode())
+        return film, spp, st
 
     def close(self):
         if self._h is not None:

@@ -453,7 +453,7 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     if (n_paths > s->wf_capacity || n_paths >= (1ull << 30)) return fail(TRB_INVALID_ARG, "pass larger than the wavefront state");
     const Tuning& tu = s->tune;
     trb::WfState wf = s->wf;
-    wf.n_paths = (uint32_t)n_paths;
+    wf.n_paths = (uint32_t)n_paths; // Adaptive passes: the worst case (the stride of the q_mid lists); their kernels read the live count on the device
     wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
     if (s->integrator.type != TRB_INTEGRATOR_PATH) { // Whitted / NormalsDebug: one thread per camera sample, then the same film kernel
         const unsigned grid = (unsigned)std::min<size_t>((n_paths + 127) / 128, (size_t)s->sm_count * 8);
@@ -491,9 +491,13 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
             const uint32_t per_iter = std::max(1u, std::min(32u, 128u / nu));
             const size_t smem = (size_t)per_iter * nu * 32 * sizeof(float);
             const unsigned grid = (unsigned)std::min<size_t>((n_paths + per_iter - 1) / per_iter, (size_t)s->sm_count * 16);
-            trb::k_wf_anim_table2<<<grid, 128, smem, st>>>(s->ds, wf, per_iter);
-        } else
-            trb::k_wf_anim_table<<<(unsigned)std::min<size_t>((items + 127) / 128, (size_t)s->sm_count * 16), 128, 0, st>>>(s->ds, wf);
+            if (rp.ad_state) trb::k_wf_anim_table2<true><<<grid, 128, smem, st>>>(s->ds, wf, per_iter); // Adaptive: the pass's live paths
+            else trb::k_wf_anim_table2<<<grid, 128, smem, st>>>(s->ds, wf, per_iter);
+        } else {
+            const unsigned grid = (unsigned)std::min<size_t>((items + 127) / 128, (size_t)s->sm_count * 16);
+            if (rp.ad_state) trb::k_wf_anim_table<true><<<grid, 128, 0, st>>>(s->ds, wf);
+            else trb::k_wf_anim_table<<<grid, 128, 0, st>>>(s->ds, wf);
+        }
         g_launches++;
     } else wf.xf_tab = nullptr;
     const unsigned shade_grid = (unsigned)s->sm_count * 4;
@@ -662,17 +666,20 @@ trb_status ensure_adaptive(trb_scene* s) {
     }
     CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_flags), std::max<size_t>(1, nblk) * sizeof(uint32_t)));
     CU(cudaMemset(s->d_ad_flags, 0, std::max<size_t>(1, nblk) * sizeof(uint32_t)));
-    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_count), sizeof(uint32_t)));
+    CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_count), 2 * sizeof(uint32_t))); // live length of each block list
     CU(cudaMalloc(reinterpret_cast<void**>(&s->d_ad_spp), npx * sizeof(uint32_t)));
     return TRB_OK;
 }
 
 // thread_work with the Adaptive sampler over the selected blocks: round 0 over all of them, round k over the blocks that still
 // have a pixel sampling, each round cut into passes of whole blocks (a pass holds all of a pixel's samples of the round, so
-// k_ad_decide sees them together). rp carries the film or the parity records, stats, seed. Blocks on st; reads back 4 bytes
-// per round. Afterwards d_ad_spp[block * 64 + pixel] holds each selected pixel's sample count.
+// k_ad_decide sees them together). rp carries the film or the parity records, stats, seed. Enqueued on st with no host
+// synchronisation: the host cannot know how many blocks a round keeps, so it enqueues every round of the schedule with the
+// passes the whole selection would need, and each pass clamps itself to the round's live block count, which k_ad_init /
+// k_ad_compact keep on the device (DESIGN.md §5 "Adaptive rounds"). Afterwards d_spp[y * width + x] holds the sample count
+// of each selected pixel (d_spp: width*height u32, or nullptr).
 trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb::RenderParams rp, const uint2* d_blocks, uint32_t nb, uint32_t flags,
-                                  cudaStream_t st, uint32_t* rounds_run) {
+                                  cudaStream_t st, uint32_t* d_spp) {
     trb_status r = ensure_adaptive(s);
     if (r != TRB_OK) return r;
     const uint64_t per_block = (uint64_t)64 * std::max(sch.min, sch.step); // paths of one block in the largest round
@@ -688,35 +695,33 @@ trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb
     rp.ad_min = sch.min; rp.ad_max = sch.max; rp.ad_step = sch.step; rp.ad_max_per_pixel = sch.max_per_pixel;
     rp.spp = sch.max; rp.ad_time_len = sch.max;
     const unsigned init_grid = (unsigned)std::min<size_t>(((size_t)nb * 64 + 255) / 256, (size_t)s->sm_count * 8);
-    trb::k_ad_init<<<std::max(1u, init_grid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, s->d_ad_list[0], s->d_ad_index[0]);
+    trb::k_ad_init<<<std::max(1u, init_grid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, s->d_ad_list[0], s->d_ad_index[0], s->d_ad_count);
     g_launches++;
-    int cur = 0;
-    uint32_t n_cur = nb;
-    *rounds_run = 0;
-    for (uint32_t round = 0; round < sch.rounds && n_cur > 0; ++round) {
+    for (uint32_t round = 0; round < sch.rounds; ++round) {
+        const int cur = round & 1; // round r reads list r % 2 and (compaction) writes the other one
         const uint32_t count = trbh::ad_count(sch, round);
         rp.ad_round = round; rp.sample_first = trbh::ad_slot_base(sch, round); rp.sample_count = count;
         rp.ld_offset = trbh::ad_offset(sch, round); rp.ad_pos_len = count;
+        rp.ad_live = s->d_ad_count + cur;
         const uint32_t bp = (uint32_t)std::max<uint64_t>(1, cap / ((uint64_t)64 * count));
-        for (uint32_t b0 = 0; b0 < n_cur; b0 += bp) {
-            rp.blocks = s->d_ad_list[cur] + b0; rp.n_blocks = std::min(bp, n_cur - b0); rp.ad_block_index = s->d_ad_index[cur] + b0;
+        for (uint32_t b0 = 0; b0 < nb; b0 += bp) { // worst case: the whole selection is still live; passes past the live count exit at once
+            rp.blocks = s->d_ad_list[cur] + b0; rp.n_blocks = std::min(bp, nb - b0); rp.ad_block_index = s->d_ad_index[cur] + b0; rp.ad_b0 = b0;
             r = launch_wavefront(s, rp, flags, 0, st);
             if (r != TRB_OK) return r;
             const unsigned dgrid = (unsigned)std::min<size_t>(((size_t)rp.n_blocks * 64 + 127) / 128, (size_t)s->sm_count * 16);
             trb::k_ad_decide<<<dgrid, 128, 0, st>>>(s->ds, rp, s->wf, s->d_ad_flags + b0);
             g_launches++;
         }
-        ++*rounds_run;
         if (round + 1 == sch.rounds) break;
-        trb::k_ad_compact<<<1, 1024, 0, st>>>(s->d_ad_flags, n_cur, s->d_ad_list[cur], s->d_ad_index[cur], s->d_ad_list[cur ^ 1], s->d_ad_index[cur ^ 1], s->d_ad_count);
+        trb::k_ad_compact<<<1, 1024, 0, st>>>(s->d_ad_flags, s->d_ad_count + cur, s->d_ad_list[cur], s->d_ad_index[cur], s->d_ad_list[cur ^ 1],
+                                              s->d_ad_index[cur ^ 1], s->d_ad_count + (cur ^ 1));
         g_launches++;
-        CU(cudaMemcpyAsync(&n_cur, s->d_ad_count, sizeof n_cur, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        cur ^= 1;
     }
-    const unsigned sgrid = (unsigned)std::min<size_t>(((size_t)nb * 64 + 255) / 256, (size_t)s->sm_count * 8);
-    trb::k_ad_pixel_spp<<<std::max(1u, sgrid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, s->d_ad_spp);
-    g_launches++;
+    if (d_spp) {
+        const unsigned sgrid = (unsigned)std::min<size_t>(((size_t)nb * 64 + 255) / 256, (size_t)s->sm_count * 8);
+        trb::k_ad_pixel_spp<<<std::max(1u, sgrid), 256, 0, st>>>(s->ds, d_blocks, nb, s->d_ad_state, d_spp);
+        g_launches++;
+    }
     CU(cudaGetLastError());
     return TRB_OK;
 }
@@ -726,16 +731,18 @@ const std::vector<uint32_t>* host_blocks(const trb_scene* s, const uint2* d_bloc
     for (const BlockList& b : s->block_lists) if (b.dev == d_blocks) return &b.host;
     return nullptr;
 }
-// d_ad_spp (selection order) -> pixel_spp[y * width + x] for the selected pixels
+// d_ad_spp (image layout, written by k_ad_pixel_spp) -> pixel_spp[y * width + x] for the selected pixels only
 trb_status adaptive_pixel_spp_out(trb_scene* s, const uint2* d_blocks, uint32_t nb, uint32_t* pixel_spp) {
     if (!pixel_spp || nb == 0) return TRB_OK;
     const std::vector<uint32_t>* hb = host_blocks(s, d_blocks);
     if (!hb) return fail(TRB_CUDA, "block list not found");
-    std::vector<uint32_t> v((size_t)nb * 64);
+    std::vector<uint32_t> v((size_t)s->film.width * s->film.height);
     CU(cudaMemcpy(v.data(), s->d_ad_spp, v.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     for (uint32_t b = 0; b < nb; ++b)
-        for (uint32_t k = 0; k < 64; ++k)
-            pixel_spp[((*hb)[2 * b + 1] * 8 + k / 8) * (size_t)s->film.width + (*hb)[2 * b] * 8 + k % 8] = v[(size_t)b * 64 + k];
+        for (uint32_t k = 0; k < 64; ++k) {
+            const size_t pixel = ((*hb)[2 * b + 1] * 8 + k / 8) * (size_t)s->film.width + (*hb)[2 * b] * 8 + k % 8;
+            pixel_spp[pixel] = v[pixel];
+        }
     return TRB_OK;
 }
 
@@ -1346,11 +1353,12 @@ trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const tr
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     CU(cudaEventRecord(s->ev0, 0));
-    uint32_t rounds = 0;
     if (nb) { // an empty selection renders nothing (block_queue.rs:42-44)
+        r = ensure_adaptive(s);
+        if (r != TRB_OK) return r;
         trb::RenderParams rp{};
         rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = s->d_film; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-        r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, &rounds);
+        r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr);
         if (r != TRB_OK) return r;
     }
     CU(cudaEventRecord(s->ev1, 0));
@@ -1386,6 +1394,8 @@ trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, 
     if (r != TRB_OK) return r;
     if (n != (size_t)nb * 64 * sch.max_per_pixel) return fail(TRB_INVALID_ARG, "sample buffer size must be blocks*64*max_per_pixel");
     if (n == 0) return TRB_OK;
+    r = ensure_adaptive(s);
+    if (r != TRB_OK) return r;
     trb_sample* d_out = nullptr;
     CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
     cudaError_t e = cudaMemsetAsync(d_out, 0, n * sizeof(trb_sample), 0); // unused slots stay zero
@@ -1394,8 +1404,7 @@ trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, 
     CU(cudaEventRecord(s->ev0, 0));
     trb::RenderParams rp{};
     rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-    uint32_t rounds = 0;
-    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, &rounds);
+    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr);
     if (r != TRB_OK) { cudaDeviceSynchronize(); cudaFree(d_out); return r; }
     CU(cudaEventRecord(s->ev1, 0));
     e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
@@ -1413,6 +1422,25 @@ trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, 
         CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
     }
     return TRB_OK;
+}
+
+trb_status trb_render_adaptive_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, uint32_t* d_pixel_spp,
+                                      trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !ad || !d_film) return fail(TRB_INVALID_ARG, "null argument");
+    trbh::AdSchedule sch;
+    trb_status r = adaptive_check(s, cfg, ad, sch);
+    if (r != TRB_OK) return r;
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
+    CU(cudaSetDevice(s->device));
+    uint32_t nb;
+    const uint2* d_blocks = nullptr;
+    r = ensure_blocks(s, cfg, &d_blocks, &nb);
+    if (r != TRB_OK) return r;
+    if (nb == 0) return TRB_OK; // "Warning: This block queue is empty!" (block_queue.rs:42-44)
+    trb::RenderParams rp{};
+    rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = reinterpret_cast<float4*>(d_film); rp.stats = reinterpret_cast<trb::DStats*>(d_stats);
+    rp.error_flag = s->d_error;
+    return render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, static_cast<cudaStream_t>(stream), d_pixel_spp);
 }
 
 trb_status trb_camera_rays(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_ray* rays, float* xy) {
@@ -1759,8 +1787,9 @@ trb_status shard_cfg(const trb_scene* s, const trb_render_cfg* in, int rank, int
     out->shard_index = (uint32_t)rank; out->shard_count = (uint32_t)n_ranks; out->shard_chunk = in->shard_chunk ? in->shard_chunk : 32u;
     return TRB_OK;
 }
-// Exec::render on one replica with the film left on the device: update_frame, clear, all passes of this shard.
-trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, bool empty, cudaStream_t st) {
+// Exec::render on one replica with the film left on the device: update_frame, clear, all passes of this shard (LowDiscrepancy,
+// or the Adaptive sampler's rounds when `ad` is set).
+trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, bool empty, cudaStream_t st) {
     CU(cudaSetDevice(s->device));
     if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) {
         const float step = s->film.scene_time / (float)s->film.frames;
@@ -1771,7 +1800,22 @@ trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, bool e
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), st));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), st));
     if (empty) return TRB_OK;
+    if (ad) { // per-pixel counts to d_ad_spp, for shard_pixel_spp_out
+        trb_status r = ensure_adaptive(s);
+        if (r != TRB_OK) return r;
+        return trb_render_adaptive_device(s, cfg, ad, reinterpret_cast<float*>(s->d_film), s->d_ad_spp, reinterpret_cast<trb_stats*>(s->d_stats), st);
+    }
     return trb_render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), st);
+}
+// the Adaptive sampler's per-pixel counts of this replica's shard -> pixel_spp (host, width*height; other entries untouched)
+trb_status shard_pixel_spp_out(trb_scene* s, const trb_render_cfg* mine, bool empty, uint32_t* pixel_spp) {
+    if (!pixel_spp || empty) return TRB_OK;
+    CU(cudaSetDevice(s->device));
+    uint32_t nb;
+    const uint2* d_blocks = nullptr;
+    trb_status r = ensure_blocks(s, mine, &d_blocks, &nb); // the list the render used (cached per selection)
+    if (r != TRB_OK) return r;
+    return adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
 }
 trb_status film_to_host_add(trb_scene* s, float* film, cudaStream_t st) { // additive, like film::Image::add_pixels (image.rs:21-33)
     const size_t npx = (size_t)s->film.width * s->film.height;
@@ -1852,17 +1896,27 @@ trb_status trb_comm_reduce_film(trb_comm* c, float* d_film, size_t n, int root, 
     return TRB_OK;
 }
 
-trb_status trb_render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, int root, float* film, trb_stats* stats) {
+} // extern "C"
+
+namespace {
+// trb_render_sharded (ad == nullptr) and trb_render_sharded_adaptive
+trb_status render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, const trb_adaptive* ad, int root, float* film, uint32_t* pixel_spp,
+                          trb_stats* stats) {
     if (!s || !c || !cfg || root < 0 || root >= c->n_ranks) return fail(TRB_INVALID_ARG, "null or bad argument");
     if (c->rank == root && !film) return fail(TRB_INVALID_ARG, "the root rank needs a film buffer");
     if (c->device != s->device) return fail(TRB_INVALID_ARG, "scene and communicator live on different devices");
+    if (ad) { // before sharding: a rank whose shard is empty answers like the others
+        trbh::AdSchedule sch;
+        trb_status r = adaptive_check(s, cfg, ad, sch);
+        if (r != TRB_OK) return r;
+    }
     trb_render_cfg mine; bool empty;
     trb_status r = shard_cfg(s, cfg, c->rank, c->n_ranks, &mine, &empty);
     if (r != TRB_OK) return r;
     auto t0 = std::chrono::steady_clock::now();
     CU(cudaSetDevice(s->device));
     CU(cudaEventRecord(s->ev0, 0));
-    r = render_to_device_film(s, &mine, empty, nullptr);
+    r = render_to_device_film(s, &mine, ad, empty, nullptr);
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev1, 0));
     r = trb_comm_reduce_film(c, reinterpret_cast<float*>(s->d_film), (size_t)s->film.width * s->film.height * 4, root, nullptr); // ONE reduce per frame
@@ -1871,6 +1925,7 @@ trb_status trb_render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* c
     else CU(cudaStreamSynchronize(nullptr));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
+    if (ad) { r = shard_pixel_spp_out(s, &mine, empty, pixel_spp); if (r != TRB_OK) return r; }
     if (stats) {
         r = stats_to_host(s, stats, false);
         if (r != TRB_OK) return r;
@@ -1878,6 +1933,19 @@ trb_status trb_render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* c
         stats->update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count() - stats->kernel_ms;
     }
     return TRB_OK;
+}
+} // namespace
+
+extern "C" {
+
+trb_status trb_render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, int root, float* film, trb_stats* stats) {
+    return render_sharded(s, c, cfg, nullptr, root, film, nullptr, stats);
+}
+
+trb_status trb_render_sharded_adaptive(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, const trb_adaptive* ad, int root, float* film,
+                                       uint32_t* pixel_spp, trb_stats* stats) {
+    if (!ad) return fail(TRB_INVALID_ARG, "null argument");
+    return render_sharded(s, c, cfg, ad, root, film, pixel_spp, stats);
 }
 
 trb_status trb_group_create(const trb_scene_desc* desc, const int* devices, int n, trb_group** out) {
@@ -1927,19 +1995,31 @@ void trb_group_destroy(trb_group* g) {
     delete g;
 }
 
-trb_status trb_group_render(trb_group* g, const trb_render_cfg* cfg, float* film, trb_stats* stats) {
+} // extern "C"
+
+namespace {
+// trb_group_render (ad == nullptr) and trb_group_render_adaptive
+trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
     if (!g || !cfg || !film) return fail(TRB_INVALID_ARG, "null argument");
     const int n = (int)g->scenes.size();
-    if (n == 1) return trb_render(g->scenes[0], cfg, film, stats);
+    if (n == 1) return ad ? trb_render_adaptive(g->scenes[0], cfg, ad, film, pixel_spp, stats) : trb_render(g->scenes[0], cfg, film, stats);
+    if (ad) {
+        trbh::AdSchedule sch;
+        trb_status r = adaptive_check(g->scenes[0], cfg, ad, sch);
+        if (r != TRB_OK) return r;
+    }
     auto t0 = std::chrono::steady_clock::now();
     // enqueue every replica's shard (update_frame is host work per replica; the kernels of all devices then run concurrently)
     std::vector<trb_status> rc(n, TRB_OK);
     std::vector<std::string> msg(n);
+    std::vector<trb_render_cfg> mine(n);
+    std::vector<char> empty(n, 0);
     std::vector<std::thread> th;
     for (int i = 0; i < n; ++i) th.emplace_back([&, i]() {
-        trb_render_cfg mine; bool empty;
-        rc[i] = shard_cfg(g->scenes[i], cfg, i, n, &mine, &empty);
-        if (rc[i] == TRB_OK) { cudaSetDevice(g->scenes[i]->device); cudaEventRecord(g->scenes[i]->ev0, 0); rc[i] = render_to_device_film(g->scenes[i], &mine, empty, nullptr); cudaEventRecord(g->scenes[i]->ev1, 0); }
+        bool e = false;
+        rc[i] = shard_cfg(g->scenes[i], cfg, i, n, &mine[i], &e);
+        empty[i] = e;
+        if (rc[i] == TRB_OK) { cudaSetDevice(g->scenes[i]->device); cudaEventRecord(g->scenes[i]->ev0, 0); rc[i] = render_to_device_film(g->scenes[i], &mine[i], ad, e, nullptr); cudaEventRecord(g->scenes[i]->ev1, 0); }
         if (rc[i] != TRB_OK) msg[i] = trb_last_error();
     });
     for (auto& t : th) t.join();
@@ -1961,6 +2041,7 @@ trb_status trb_group_render(trb_group* g, const trb_render_cfg* cfg, float* film
         CU(cudaDeviceSynchronize());
         r = check_error_flag(g->scenes[i]);
         if (r != TRB_OK) return r;
+        if (ad) { r = shard_pixel_spp_out(g->scenes[i], &mine[i], empty[i] != 0, pixel_spp); if (r != TRB_OK) return r; } // the replicas' pixels are disjoint
         if (stats) {
             r = stats_to_host(g->scenes[i], stats, true);
             if (r != TRB_OK) return r;
@@ -1971,6 +2052,18 @@ trb_status trb_group_render(trb_group* g, const trb_render_cfg* cfg, float* film
     }
     if (stats) { stats->kernel_ms = kernel_ms; stats->update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count() - kernel_ms; }
     return TRB_OK;
+}
+} // namespace
+
+extern "C" {
+
+trb_status trb_group_render(trb_group* g, const trb_render_cfg* cfg, float* film, trb_stats* stats) {
+    return group_render(g, cfg, nullptr, film, nullptr, stats);
+}
+
+trb_status trb_group_render_adaptive(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
+    if (!ad) return fail(TRB_INVALID_ARG, "null argument");
+    return group_render(g, cfg, ad, film, pixel_spp, stats);
 }
 
 } // extern "C"

@@ -174,6 +174,10 @@ struct RenderParams {
     uint4* ad_state;                  // per image pixel trbh::AdPixel; nullptr: LowDiscrepancy
     const uint32_t* ad_block_index;   // index of each pass block in the caller's selected block list (parity records)
     uint32_t ad_min, ad_max, ad_step, ad_max_per_pixel;
+    // Adaptive passes are enqueued for the worst case: the pass covers blocks [ad_b0, ad_b0 + n_blocks) of the round's list,
+    // and *ad_live (written on the device by k_ad_init / k_ad_compact) is how many blocks that list really holds
+    const uint32_t* ad_live;
+    uint32_t ad_b0;
 };
 
 } // namespace trb

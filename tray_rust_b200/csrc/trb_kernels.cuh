@@ -1803,6 +1803,7 @@ constexpr uint32_t WF_PATH_MASK = 0x3fffffffu;
 constexpr int WF_SORT_MAX_BITS = 6; // origin grid up to 64^3 cells x 8 octants x 3 ray types = 6.3 M bins
 enum { WF_N_ACTIVE = 0, WF_N_CONT = 1, WF_N_SHADOW = 2, WF_N_MIS = 3, WF_TRACE_HEAD = 4, WF_SHADE_HEAD = 5, WF_N_MID = 6, WF_SHADE_B_HEAD = 7, WF_SHADE_C_HEAD = 8,
        WF_N_ENDING = 9, WF_ENDING_HEAD = 10,
+       WF_N_PATHS = 11, // Adaptive passes: the paths the pass really holds (k_wf_generate_ad), read by k_wf_anim_table<true> / 2<true>
        // split shading with the paths bucketed by material kind (k_wf_shade_a fills, _b and _c drain bucket after bucket)
        WF_MID_K = 12, WF_B_HEAD_K = 20, WF_C_HEAD_K = 28, WF_CNT = 36 };
 constexpr uint32_t WF_MID_BUCKETS = 8;
@@ -1847,6 +1848,11 @@ __device__ __forceinline__ void sample_position_ad(const RenderParams& rp, const
     sy = ld_sobol(ip, ps.scr1) + (float)id.py;
     tm = ld_vdc(permute_index(s, rp.ad_time_len, ps.ktime) + rp.ld_offset, ps.scrt);
 }
+// blocks an Adaptive pass really covers: min(n_blocks, live - b0), 0 when the round's list ends before the pass starts
+__device__ __forceinline__ uint32_t ad_pass_blocks(const RenderParams& rp) {
+    const uint32_t live = *rp.ad_live;
+    return live > rp.ad_b0 ? min(rp.n_blocks, live - rp.ad_b0) : 0u;
+}
 
 // warp-aggregated append: every lane of the warp must call it
 __device__ __forceinline__ void wf_push(uint32_t* q, uint32_t* counter, bool want, uint32_t value) {
@@ -1876,8 +1882,10 @@ __device__ __forceinline__ const float* wf_xf_row(const WfState& wf, uint32_t p)
     return (ANIM && wf.xf_tab) ? wf.xf_tab + (size_t)p * wf.n_anim * 32 : nullptr;
 }
 // AnimatedTransform::transform(ray.time) once per (path, keyframed instance) — see instance_inv(). One thread per table entry.
+// ADAPT: the pass's path count is the one k_wf_generate_ad found on the device (WF_N_PATHS), not the worst case wf.n_paths.
+template <bool ADAPT = false>
 __global__ void __launch_bounds__(128) k_wf_anim_table(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf) {
-    const size_t n = (size_t)wf.n_paths * wf.n_anim;
+    const size_t n = (size_t)(ADAPT ? wf.counters[WF_N_PATHS] : wf.n_paths) * wf.n_anim;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const uint32_t p = (uint32_t)(i / wf.n_anim), k = (uint32_t)(i % wf.n_anim);
         const DInstance& in = sc.instances[__ldg(&sc.anim_instances[k])];
@@ -1897,11 +1905,13 @@ __global__ void __launch_bounds__(128) k_wf_anim_table(const __grid_constant__ D
 // (path, distinct spline) -> shared memory; phase 2: one thread per (path, keyframed instance) composes its stack in the
 // reference's order from those and the precomputed one-control-point levels — the operations of trbh::animated_xf, so the rows
 // are bit-identical to k_wf_anim_table's.
+template <bool ADAPT = false>
 __global__ void __launch_bounds__(128) k_wf_anim_table2(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, uint32_t per_iter) {
     extern __shared__ float s_lvl[]; // [path of this iteration][distinct spline][fwd 16 | inv 16]
     const uint32_t nu = sc.n_uniq_splines;
-    for (uint32_t p0 = blockIdx.x * per_iter; p0 < wf.n_paths; p0 += gridDim.x * per_iter) {
-        const uint32_t np = min(per_iter, wf.n_paths - p0);
+    const uint32_t n_paths = ADAPT ? wf.counters[WF_N_PATHS] : wf.n_paths; // as in k_wf_anim_table
+    for (uint32_t p0 = blockIdx.x * per_iter; p0 < n_paths; p0 += gridDim.x * per_iter) {
+        const uint32_t np = min(per_iter, n_paths - p0);
         for (uint32_t i = threadIdx.x; i < np * nu; i += blockDim.x) {
             const uint32_t lp = i / nu, u = i % nu;
             const trb_spline& sp = sc.splines[__ldg(&sc.uniq_splines[u])];
@@ -2655,7 +2665,9 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constan
     const int T = 9 + 2 * max(sc.fpw_x, sc.fpw_y);
     for (int i = threadIdx.x; i < 256; i += RENDER_THREADS) s_table[i] = sc.filter_table[i];
     const uint32_t pix = threadIdx.x & 63, lane_s = threadIdx.x >> 6;
-    for (uint32_t item = blockIdx.x; item < rp.n_blocks; item += gridDim.x) {
+    uint32_t n_live = 0; // ADAPT: the blocks this pass really covers; the LowDiscrepancy loop reads rp.n_blocks as before
+    if (ADAPT) n_live = ad_pass_blocks(rp);
+    for (uint32_t item = blockIdx.x; item < (ADAPT ? n_live : rp.n_blocks); item += gridDim.x) {
         __syncthreads();
         for (int i = threadIdx.x; i < T * T; i += RENDER_THREADS) tile[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         __syncthreads();
@@ -2702,7 +2714,9 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_cons
     const uint32_t pix = threadIdx.x & 63, lane_s = threadIdx.x >> 6;
     float4* mine = tiles + (threadIdx.x >> 5) * (T * T);
     const int ry = (int)ceilf(sc.filter_h / sc.filter_inv_h) + 1, rx = (int)ceilf(sc.filter_w / sc.filter_inv_w) + 1;
-    for (uint32_t item = blockIdx.x; item < rp.n_blocks; item += gridDim.x) {
+    uint32_t n_live = 0; // ADAPT: the blocks this pass really covers (CTA-uniform: the per-offset __syncwarp lockstep is untouched)
+    if (ADAPT) n_live = ad_pass_blocks(rp);
+    for (uint32_t item = blockIdx.x; item < (ADAPT ? n_live : rp.n_blocks); item += gridDim.x) {
         __syncthreads();
         for (int i = threadIdx.x; i < 4 * T * T; i += RENDER_THREADS) tiles[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         __syncthreads();
@@ -2903,14 +2917,18 @@ __global__ void k_srgb8(size_t n, const float4* __restrict__ film, uint8_t* __re
 // a sequence of rounds over the selected blocks; a round is cut into passes by block sub-ranges only, so one pass holds all of a
 // pixel's samples of the round. Per pass: k_wf_generate_ad, the unchanged trace / shade rounds (the per-path sample arrays get
 // the round's LD offset), the film kernels' ADAPT variant, then k_ad_decide. Between rounds k_ad_compact keeps the blocks that
-// still have a pixel sampling.
+// still have a pixel sampling. The rounds are driven by the device: the host enqueues every round with the passes the whole
+// selection would need, and each pass reads the live length of its round's list (RenderParams::ad_live, ad_pass_blocks) and
+// does nothing past it.
 // ==========================================================================================
 // A pass's path p = (block, pixel, entry) as in LowDiscrepancy, slot = sample_first + entry. Only the paths of pixels that are
 // still sampling are queued for the primary trace (warp-aggregated push) and counted as camera samples; the others enter shade
-// round 0 as primary misses, which only writes a black sample that neither the film nor the decision reads.
+// round 0 as primary misses, which only writes a black sample that neither the film nor the decision reads. The pass's real
+// path count goes to WF_N_ACTIVE (shade round 0) and WF_N_PATHS (the keyframed tables); an empty pass leaves every count 0.
 template <bool ANIM>
 __global__ void __launch_bounds__(256) k_wf_generate_ad(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
-    const uint32_t n = wf.n_paths;
+    const uint32_t n = ad_pass_blocks(rp) * 64 * rp.sample_count;
+    if (n == 0) return;
     const uint32_t lane = threadIdx.x & 31, stride = gridDim.x * blockDim.x;
     for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p - lane < n; p += stride) { // whole warps iterate (wf_push)
         bool on = false;
@@ -2938,7 +2956,7 @@ __global__ void __launch_bounds__(256) k_wf_generate_ad(const __grid_constant__ 
         wf_push(wf.q_cont, &wf.counters[WF_N_CONT], on, p);
         if (lane == 0 && m && rp.stats) atomicAdd(&rp.stats->camera_samples, (unsigned long long)__popc(m));
     }
-    if (blockIdx.x == 0 && threadIdx.x == 0) wf.counters[WF_N_ACTIVE] = n; // shade round 0 walks every path of the pass
+    if (blockIdx.x == 0 && threadIdx.x == 0) { wf.counters[WF_N_ACTIVE] = n; wf.counters[WF_N_PATHS] = n; } // shade round 0 walks every path of the pass
     if (blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid
         uint32_t* b = wf.bounds + threadIdx.x * 8;
         b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
@@ -2952,7 +2970,7 @@ __global__ void __launch_bounds__(128) k_ad_decide(const __grid_constant__ DScen
                                                    uint32_t* block_flags) {
     trbh::AdSchedule sch;
     sch.min = rp.ad_min; sch.max = rp.ad_max; sch.step = rp.ad_step; sch.max_per_pixel = rp.ad_max_per_pixel; sch.rounds = 0;
-    const uint32_t n = rp.n_blocks * 64;
+    const uint32_t n = ad_pass_blocks(rp) * 64;
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
         SampleId id;
         id.item = t >> 6; id.pix = t & 63;
@@ -2982,7 +3000,9 @@ __global__ void __launch_bounds__(128) k_ad_decide(const __grid_constant__ DScen
 }
 
 // Start of a render: every pixel of the selected blocks samples round 0; the round list starts as the selection.
-__global__ void k_ad_init(const __grid_constant__ DScene sc, const uint2* blocks, uint32_t n_blocks, uint4* state, uint2* list, uint32_t* list_index) {
+__global__ void k_ad_init(const __grid_constant__ DScene sc, const uint2* blocks, uint32_t n_blocks, uint4* state, uint2* list, uint32_t* list_index,
+                          uint32_t* list_count) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) *list_count = n_blocks;
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_blocks * 64; t += gridDim.x * blockDim.x) {
         const uint2 blk = blocks[t >> 6];
         const uint32_t pixel = (blk.y * 8 + ((t & 63) >> 3)) * sc.width + blk.x * 8 + (t & 7);
@@ -2993,11 +3013,13 @@ __global__ void k_ad_init(const __grid_constant__ DScene sc, const uint2* blocks
 }
 
 // Order-preserving compaction of the round's block list to the blocks flagged by k_ad_decide (one CTA; at most ~32 K blocks
-// at 1080p). Clears the flags it read. out_count: the new length (read back by the host: 4 bytes per round).
-__global__ void __launch_bounds__(1024) k_ad_compact(uint32_t* flags, uint32_t n, const uint2* in_list, const uint32_t* in_index,
+// at 1080p). Clears the flags it read. in_count / out_count: the lists' lengths, which stay on the device (one word per list,
+// so a round reads its input length while it writes its output length).
+__global__ void __launch_bounds__(1024) k_ad_compact(uint32_t* flags, const uint32_t* in_count, const uint2* in_list, const uint32_t* in_index,
                                                      uint2* out_list, uint32_t* out_index, uint32_t* out_count) {
     __shared__ uint32_t part[1024];
     __shared__ uint32_t base;
+    const uint32_t n = *in_count;
     if (threadIdx.x == 0) base = 0;
     for (uint32_t c0 = 0; c0 < n; c0 += 1024) {
         const uint32_t i = c0 + threadIdx.x;
@@ -3020,11 +3042,13 @@ __global__ void __launch_bounds__(1024) k_ad_compact(uint32_t* flags, uint32_t n
     if (threadIdx.x == 0) *out_count = base;
 }
 
-// Samples per pixel of the selected blocks (the reference's per-pixel count: samples_taken when report_results let go)
+// Samples per pixel of the selected blocks (the reference's per-pixel count: samples_taken when report_results let go), written
+// at spp[y * width + x]; other pixels are not touched
 __global__ void k_ad_pixel_spp(const __grid_constant__ DScene sc, const uint2* blocks, uint32_t n_blocks, const uint4* state, uint32_t* spp) {
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n_blocks * 64; t += gridDim.x * blockDim.x) {
         const uint2 blk = blocks[t >> 6];
-        spp[(size_t)t] = state[(blk.y * 8 + ((t & 63) >> 3)) * sc.width + blk.x * 8 + (t & 7)].x & ~trbh::AD_ACTIVE;
+        const uint32_t pixel = (blk.y * 8 + ((t & 63) >> 3)) * sc.width + blk.x * 8 + (t & 7);
+        spp[pixel] = state[pixel].x & ~trbh::AD_ACTIVE;
     }
 }
 
