@@ -260,6 +260,32 @@ typedef struct trb_hit {
     uint32_t pad;
 } trb_hit;
 
+/* linalg::Ray with its time (src/linalg/ray.rs:9-22) for the ray queries: the segment [min_t, max_t] of o + t*d,
+ * traced at `time`. 48 bytes (three 16-byte loads); pad is ignored. */
+typedef struct trb_query_ray {
+    float o[3];
+    float d[3];
+    float min_t, max_t;
+    float time;
+    uint32_t pad[3];
+} trb_query_ray;
+
+/* geometry::Intersection (src/geometry/intersection.rs) of one ray query: ray.max_t after the query (the input max_t on a
+ * miss), the instance and, for meshes, the triangle hit, the instance's material, and the hit's DifferentialGeometry
+ * (differential_geometry.rs) in world space, transformed as Receiver / Emitter::intersect do (receiver.rs:36-41: p as a
+ * point, n and ng as normals, dp_du and dp_dv as vectors). On a miss inst == TRB_MISS and every field after it is 0.
+ * 96 bytes. */
+typedef struct trb_intersection {
+    float t;
+    uint32_t inst;
+    uint32_t prim;      /* triangle index for meshes, else 0 */
+    uint32_t material;  /* trb_instance.material of the hit instance */
+    float p[3], n[3], ng[3];
+    float u, v, time;   /* time: the ray's */
+    float dp_du[3], dp_dv[3];
+    uint32_t pad[2];
+} trb_intersection;
+
 /* Per camera sample record for parity tests: film position and the clamped radiance
  * pushed as ImageSample (multithreaded.rs:98-102). */
 typedef struct trb_sample {
@@ -378,6 +404,35 @@ trb_status trb_intersect(trb_scene* scene, size_t n, const trb_ray* rays, trb_hi
 /* Device-buffer variant of trb_intersect, enqueued on cuda_stream. */
 trb_status trb_intersect_device(trb_scene* scene, size_t n, const trb_ray* d_rays, trb_hit* d_hits,
                                 trb_stats* d_stats, void* cuda_stream);
+
+/* -- ray queries on the render's trace kernel ------------------------------------------
+ * ≙ Scene::intersect (scene.rs:148-150) for a batch of rays, each traced at its own `time` with the reference's inclusive
+ * [min_t, max_t] tests, returning the whole geometry::Intersection. The rays run through the wavefront trace kernel the
+ * renders use, in passes of at most "pass.paths" rays (trb_scene_set_option). The TLAS is the one trb_scene_update_frame built
+ * for the current shutter interval: a time outside that interval is traced against those boxes, exactly as the reference
+ * would trace it. flags: TRB_RENDER_STATS also counts node / triangle / instance tests; stats->rays_primary counts the
+ * queries. TRB_INVALID_ARG for null arguments, other flag bits, or before the first update_frame ("Update frame must be
+ * called before rendering"); n == 0 is TRB_OK. A traversal-stack overflow returns TRB_CUDA. Host buffers; blocking. */
+trb_status trb_intersect_records(trb_scene* scene, size_t n, const trb_query_ray* rays, trb_intersection* out, uint32_t flags,
+                                 trb_stats* stats);
+
+/* Device-buffer variant of trb_intersect_records, enqueued on cuda_stream (a cudaStream_t; NULL = default stream) without host
+ * synchronisation. d_rays and d_out must be 16-byte aligned; d_stats (may be NULL) is a DEVICE trb_stats the kernels accumulate
+ * into. A call that needs more path state than earlier calls grows it and synchronises the device once, as trb_render_device
+ * does; the same one-stream-per-scene rule applies, and a traversal-stack overflow is reported by trb_scene_check_error. */
+trb_status trb_intersect_records_device(trb_scene* scene, size_t n, const trb_query_ray* d_rays, trb_intersection* d_out, uint32_t flags,
+                                        trb_stats* d_stats, void* cuda_stream);
+
+/* ≙ OcclusionTester::occluded (light/mod.rs:30-37) for a batch: occluded[i] = 1 iff Scene::intersect finds a hit on ray i's
+ * segment at its time, else 0. Callers build the segment as OcclusionTester::test_points / test_ray do (light/mod.rs:21-28).
+ * By default a ray stops at its first accepted hit (same booleans, fewer tests); TRB_RENDER_REFERENCE_SHADOW walks to the
+ * closest hit like the reference, so the test counters of TRB_RENDER_STATS equal its. stats->rays_shadow counts the queries.
+ * Statuses, passes and TLAS as trb_intersect_records. Host buffers; blocking. */
+trb_status trb_occluded(trb_scene* scene, size_t n, const trb_query_ray* rays, uint8_t* occluded, uint32_t flags, trb_stats* stats);
+
+/* Device-buffer variant of trb_occluded, with trb_intersect_records_device's contract (d_rays 16-byte aligned). */
+trb_status trb_occluded_device(trb_scene* scene, size_t n, const trb_query_ray* d_rays, uint8_t* d_occluded, uint32_t flags,
+                               trb_stats* d_stats, void* cuda_stream);
 
 /* ≙ LowDiscrepancy::get_samples + get_samples_1d + Camera::generate_ray
  * (ld.rs:33-64, camera.rs:150-157) for the selected blocks/samples: writes one ray and

@@ -1,0 +1,96 @@
+"""Ray-query throughput on one GPU: trb_intersect (k_intersect, one thread per ray), trb_intersect_records and trb_occluded (the
+render's wavefront trace kernel) on the C4 workload (1 M triangles), device buffers, GPU time between CUDA events on one stream.
+Measures and reports; gates nothing.
+
+    python tools/query_bench.py [--rays 4194304] [--reps 5] [--tris 1000000] [--out results/query_bench.json]
+
+The rays are incoherent: seeded origins uniform in the Cornell box and directions uniform on the sphere, as a render's bounce rays
+are. trb_intersect has no per-ray time and returns (t, inst, prim); trb_intersect_records also builds the whole world-space
+Intersection (96 bytes per ray); trb_occluded is timed in both shadow modes. The median of --reps timed calls after one warm-up.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, REPO)
+from tray_rust_b200 import _ffi as F, api, scenebuild as SB  # noqa: E402
+
+
+def device_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return q.stdout.strip().splitlines()[0]
+    except Exception as e:  # noqa: BLE001
+        return "unknown (%s)" % e
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rays", type=int, default=1 << 22)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--tris", type=int, default=1_000_000)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    import torch as T
+    dev = T.device("cuda:0")
+    g = api.Scene(SB.scene_c4(a.tris, 64, 64, 1).finish())
+    g.update_frame(0, 0.0, 0.0)
+    rng = np.random.default_rng(0x0C4)
+    q = np.zeros(a.rays, F.QUERY_RAY_DTYPE)
+    q["o"] = rng.uniform((-14, 1, -10), (14, 23, 18), size=(a.rays, 3))
+    d = rng.normal(size=(a.rays, 3))
+    q["d"] = d / np.linalg.norm(d, axis=1, keepdims=True)
+    q["max_t"] = np.inf
+    r = np.zeros(a.rays, F.RAY_DTYPE)
+    for k in ("o", "d", "min_t", "max_t"):
+        r[k] = q[k]
+    d_q = T.from_numpy(q.view(np.uint8).copy()).to(dev)
+    d_r = T.from_numpy(r.view(np.uint8).copy()).to(dev)
+    d_hits = T.empty(a.rays * 16, dtype=T.uint8, device=dev)
+    d_rec = T.empty(a.rays * F.INTERSECTION_DTYPE.itemsize, dtype=T.uint8, device=dev)
+    d_occ = T.empty(a.rays, dtype=T.uint8, device=dev)
+    s = T.cuda.Stream()
+    s.wait_stream(T.cuda.current_stream())
+    n = a.rays
+    cases = {
+        "trb_intersect (k_intersect)": lambda: g.intersect_device(n, d_r.data_ptr(), d_hits.data_ptr(), None, s.cuda_stream),
+        "trb_intersect_records": lambda: g.intersect_records_device(n, d_q.data_ptr(), d_rec.data_ptr(), None, s.cuda_stream),
+        "trb_occluded (any hit)": lambda: g.occluded_device(n, d_q.data_ptr(), d_occ.data_ptr(), None, s.cuda_stream),
+        "trb_occluded (reference closest hit)": lambda: g.occluded_device(n, d_q.data_ptr(), d_occ.data_ptr(), None, s.cuda_stream, reference=True),
+    }
+    res = {"device": device_info(), "rays": n, "triangles": a.tris, "reps": a.reps, "mrays_per_s": {}, "ms": {}}
+    for name, call in cases.items():
+        call()  # warm-up (and the first query call grows the path state)
+        s.synchronize()
+        ms = []
+        for _ in range(a.reps):
+            e0, e1 = T.cuda.Event(enable_timing=True), T.cuda.Event(enable_timing=True)
+            e0.record(s)
+            call()
+            e1.record(s)
+            s.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        med = float(np.median(ms))
+        res["ms"][name] = med
+        res["mrays_per_s"][name] = n / med / 1e3
+    g.check_error()
+    hits = np.frombuffer(d_hits.cpu().numpy().tobytes(), F.HIT_DTYPE)
+    rec = np.frombuffer(d_rec.cpu().numpy().tobytes(), F.INTERSECTION_DTYPE)
+    res["hit_fraction"] = float((hits["inst"] != F.MISS).mean())
+    res["records_match_trb_intersect"] = bool(rec["t"].tobytes() == hits["t"].tobytes() and (rec["inst"] == hits["inst"]).all())
+    print("device: %s   %d incoherent rays on C4 (%d triangles), median of %d" % (res["device"], n, a.tris, a.reps))
+    for name in cases:
+        print("  %-40s %8.3f ms  %8.1f Mrays/s" % (name, res["ms"][name], res["mrays_per_s"][name]))
+    print("  hit fraction %.3f, records equal trb_intersect's (t, inst): %s" % (res["hit_fraction"], res["records_match_trb_intersect"]))
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        json.dump(res, open(a.out, "w"), indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -124,6 +124,15 @@ class Hit(C.Structure):
     _fields_ = [("t", f32), ("inst", u32), ("prim", u32), ("pad", u32)]
 
 
+class QueryRay(C.Structure):
+    _fields_ = [("o", f32 * 3), ("d", f32 * 3), ("min_t", f32), ("max_t", f32), ("time", f32), ("pad", u32 * 3)]
+
+
+class Intersection(C.Structure):
+    _fields_ = [("t", f32), ("inst", u32), ("prim", u32), ("material", u32), ("p", f32 * 3), ("n", f32 * 3), ("ng", f32 * 3),
+                ("u", f32), ("v", f32), ("time", f32), ("dp_du", f32 * 3), ("dp_dv", f32 * 3), ("pad", u32 * 2)]
+
+
 class Sample(C.Structure):
     _fields_ = [("x", f32), ("y", f32), ("r", f32), ("g", f32), ("b", f32)]
 
@@ -139,6 +148,10 @@ RAY_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("min_t", "<f4"), ("max_
 HIT_DTYPE = np.dtype([("t", "<f4"), ("inst", "<u4"), ("prim", "<u4"), ("pad", "<u4")])
 SAMPLE_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("r", "<f4"), ("g", "<f4"), ("b", "<f4")])
 NODE_DTYPE = np.dtype([("bmin", "<f4", 3), ("bmax", "<f4", 3), ("a", "<u4"), ("b", "<u4")])
+QUERY_RAY_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("min_t", "<f4"), ("max_t", "<f4"), ("time", "<f4"), ("pad", "<u4", 3)])
+INTERSECTION_DTYPE = np.dtype([("t", "<f4"), ("inst", "<u4"), ("prim", "<u4"), ("material", "<u4"), ("p", "<f4", 3), ("n", "<f4", 3),
+                               ("ng", "<f4", 3), ("u", "<f4"), ("v", "<f4"), ("time", "<f4"), ("dp_du", "<f4", 3), ("dp_dv", "<f4", 3),
+                               ("pad", "<u4", 2)])
 
 TRB_SYMBOLS = [
     "trb_scene_create", "trb_scene_load_json", "trb_scene_destroy", "trb_scene_info", "trb_scene_update_frame",
@@ -150,6 +163,7 @@ TRB_SYMBOLS = [
     "trb_group_create", "trb_group_load_json", "trb_group_render", "trb_group_scene", "trb_group_destroy",
     "trb_render_adaptive", "trb_render_samples_adaptive", "trb_adaptive_schedule", "trb_host_adaptive_decide",
     "trb_render_adaptive_device", "trb_render_sharded_adaptive", "trb_group_render_adaptive",
+    "trb_intersect_records", "trb_intersect_records_device", "trb_occluded", "trb_occluded_device",
 ]
 
 _trb = None
@@ -182,6 +196,10 @@ def load_trb():
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]
     lib.trb_intersect_device.argtypes = [vp, sz, vp, vp, vp, vp]
+    lib.trb_intersect_records.argtypes = [vp, sz, vp, vp, u32, C.POINTER(Stats)]
+    lib.trb_intersect_records_device.argtypes = [vp, sz, vp, vp, u32, vp, vp]
+    lib.trb_occluded.argtypes = [vp, sz, vp, vp, u32, C.POINTER(Stats)]
+    lib.trb_occluded_device.argtypes = [vp, sz, vp, vp, u32, vp, vp]
     lib.trb_camera_rays.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]

@@ -203,6 +203,35 @@ class Scene(_Base):
     def intersect_device(self, n, d_rays, d_hits, d_stats=None, stream=None):
         self._check(self._lib.trb_intersect_device(self._h, n, d_rays, d_hits, d_stats, stream))
 
+    def intersect_records(self, rays, stats=False):
+        """trb_intersect_records: Scene::intersect of each QUERY_RAY_DTYPE ray at its own time. Returns (INTERSECTION_DTYPE records,
+        Stats); stats=True also counts node / triangle / instance tests."""
+        rays = np.ascontiguousarray(rays, dtype=F.QUERY_RAY_DTYPE)
+        out = np.zeros(len(rays), F.INTERSECTION_DTYPE)
+        st = F.Stats()
+        self._check(self._lib.trb_intersect_records(self._h, len(rays), F.ptr(rays), F.ptr(out), F.RENDER_STATS if stats else 0, C.byref(st)))
+        return out, st
+
+    def intersect_records_device(self, n, d_rays, d_out, d_stats=None, stream=None, stats=False):
+        """trb_intersect_records_device: device buffers of n query rays (48 B each) and n records (96 B each), both 16-byte
+        aligned, enqueued on `stream` (a cudaStream_t as an int; None = default stream) without host synchronisation."""
+        self._check(self._lib.trb_intersect_records_device(self._h, n, d_rays, d_out, F.RENDER_STATS if stats else 0, d_stats, stream))
+
+    def occluded(self, rays, reference=False, stats=False):
+        """trb_occluded: OcclusionTester::occluded of each QUERY_RAY_DTYPE segment at its own time. Returns (bool array, Stats).
+        reference=True walks to the closest hit like the reference (its test counters); the default stops at the first hit."""
+        rays = np.ascontiguousarray(rays, dtype=F.QUERY_RAY_DTYPE)
+        out = np.zeros(len(rays), np.uint8)
+        st = F.Stats()
+        flags = (F.RENDER_STATS if stats else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0)
+        self._check(self._lib.trb_occluded(self._h, len(rays), F.ptr(rays), F.ptr(out), flags, C.byref(st)))
+        return out.astype(bool), st
+
+    def occluded_device(self, n, d_rays, d_occluded, d_stats=None, stream=None, reference=False, stats=False):
+        """trb_occluded_device: n query rays (16-byte aligned) -> n uint8 flags, enqueued on `stream` without host synchronisation."""
+        flags = (F.RENDER_STATS if stats else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0)
+        self._check(self._lib.trb_occluded_device(self._h, n, d_rays, d_occluded, flags, d_stats, stream))
+
     def to_srgb8(self, film):
         film = np.ascontiguousarray(film, dtype=np.float32)
         out = np.zeros((self.height, self.width, 3), np.uint8)

@@ -446,6 +446,27 @@ trb_status ensure_wavefront(trb_scene* s, size_t n_paths) {
     return TRB_OK;
 }
 
+// AnimatedTransform::transform(ray.time) once per (path, keyframed instance) of a pass of n_paths paths whose times are in
+// wf.thr[].w. Leaves wf.xf_tab == nullptr when there is no table (static scene, or option anim.table 0): the trace kernel then
+// evaluates the transforms per instance test. adapt: an Adaptive pass, whose live path count the device holds.
+void launch_anim_table(trb_scene* s, trb::WfState& wf, size_t n_paths, bool adapt, cudaStream_t st) {
+    if (!(s->ds.has_anim && wf.xf_tab && s->tune.anim_table)) { wf.xf_tab = nullptr; return; }
+    const size_t items = n_paths * wf.n_anim;
+    const uint32_t nu = s->ds.n_uniq_splines;
+    if (s->tune.anim_table >= 2 && nu > 0 && nu <= 256) { // each distinct keyframed spline once per path, in shared memory; then the stacks
+        const uint32_t per_iter = std::max(1u, std::min(32u, 128u / nu));
+        const size_t smem = (size_t)per_iter * nu * 32 * sizeof(float);
+        const unsigned grid = (unsigned)std::min<size_t>((n_paths + per_iter - 1) / per_iter, (size_t)s->sm_count * 16);
+        if (adapt) trb::k_wf_anim_table2<true><<<grid, 128, smem, st>>>(s->ds, wf, per_iter); // Adaptive: the pass's live paths
+        else trb::k_wf_anim_table2<<<grid, 128, smem, st>>>(s->ds, wf, per_iter);
+    } else {
+        const unsigned grid = (unsigned)std::min<size_t>((items + 127) / 128, (size_t)s->sm_count * 16);
+        if (adapt) trb::k_wf_anim_table<true><<<grid, 128, 0, st>>>(s->ds, wf);
+        else trb::k_wf_anim_table<<<grid, 128, 0, st>>>(s->ds, wf);
+    }
+    g_launches++;
+}
+
 // One wavefront pass over rp's blocks x samples: generate, then (trace, shade) per bounce round, then the film
 // (DESIGN.md "Execution shape"). n_paths = blocks * 64 * sample_count must fit the allocated path state.
 trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st) {
@@ -484,22 +505,7 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     } else if (anim) trb::k_wf_generate<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
     else trb::k_wf_generate<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
     g_launches++;
-    if (anim && wf.xf_tab && s->tune.anim_table) { // AnimatedTransform::transform(ray.time) once per (path, keyframed instance)
-        const size_t items = n_paths * wf.n_anim;
-        const uint32_t nu = s->ds.n_uniq_splines;
-        if (s->tune.anim_table >= 2 && nu > 0 && nu <= 256) { // each distinct keyframed spline once per path, in shared memory; then the stacks
-            const uint32_t per_iter = std::max(1u, std::min(32u, 128u / nu));
-            const size_t smem = (size_t)per_iter * nu * 32 * sizeof(float);
-            const unsigned grid = (unsigned)std::min<size_t>((n_paths + per_iter - 1) / per_iter, (size_t)s->sm_count * 16);
-            if (rp.ad_state) trb::k_wf_anim_table2<true><<<grid, 128, smem, st>>>(s->ds, wf, per_iter); // Adaptive: the pass's live paths
-            else trb::k_wf_anim_table2<<<grid, 128, smem, st>>>(s->ds, wf, per_iter);
-        } else {
-            const unsigned grid = (unsigned)std::min<size_t>((items + 127) / 128, (size_t)s->sm_count * 16);
-            if (rp.ad_state) trb::k_wf_anim_table<true><<<grid, 128, 0, st>>>(s->ds, wf);
-            else trb::k_wf_anim_table<<<grid, 128, 0, st>>>(s->ds, wf);
-        }
-        g_launches++;
-    } else wf.xf_tab = nullptr;
+    launch_anim_table(s, wf, n_paths, rp.ad_state != nullptr, st);
     const unsigned shade_grid = (unsigned)s->sm_count * 4;
     const int refill = tu.refill;
     // persistent CTAs: two rounds of what is resident per SM (9 for the default variant, 7 keyframed, 4 with counters) unless set
@@ -767,6 +773,102 @@ trb_status check_error_flag(trb_scene* s) {
     int e = 0;
     CU(cudaMemcpy(&e, s->d_error, sizeof e, cudaMemcpyDeviceToHost));
     if (e) { CU(cudaMemset(s->d_error, 0, sizeof(int))); return fail(TRB_CUDA, "BVH traversal stack overflow (depth > 64; the reference would panic)"); }
+    return TRB_OK;
+}
+
+// ---- ray queries (trb_intersect_records / trb_occluded; DESIGN.md §5 "Ray queries") ---------------------------------------
+// Argument checks shared by the four entry points. `allowed`: the flag bits the query accepts; device buffers are read and
+// written with 16-byte accesses (`out16`: the output buffer too).
+trb_status query_check(const trb_scene* s, size_t n, const void* rays, const void* out, uint32_t flags, uint32_t allowed, bool device, bool out16) {
+    if (!s || (n && (!rays || !out))) return fail(TRB_INVALID_ARG, "null argument");
+    if (flags & ~allowed) return fail(TRB_INVALID_ARG, "unsupported flag bits for a ray query");
+    if (device && n && ((reinterpret_cast<uintptr_t>(rays) | (out16 ? reinterpret_cast<uintptr_t>(out) : 0u)) & 15u))
+        return fail(TRB_INVALID_ARG, "device query buffers must be 16-byte aligned");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
+    return TRB_OK;
+}
+
+// Enqueue the queries on st in passes of at most pass.paths rays (the path state grows as for renders, halving on OOM). Each pass:
+// k_query_load -> keyframed transform table -> k_wf_trace (default variant, PIPE bit 64) -> k_query_records (d_out) or
+// k_query_occluded (d_occ). The rays of a pass are round 0 of a wavefront: continuation rays for records, shadow rays for occlusion.
+trb_status query_passes(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb_intersection* d_out, uint8_t* d_occ, uint32_t flags,
+                        trb::DStats* d_stats, cudaStream_t st) {
+    uint64_t want = std::min<uint64_t>(n, std::min<uint64_t>(std::max<uint64_t>(s->tune.pass_paths, 64), (1ull << 30) - 64));
+    want = ((want + 63) / 64) * 64;
+    if (want > s->wf_capacity) {
+        trb_status r;
+        while ((r = ensure_wavefront(s, (size_t)want)) == TRB_OOM && want > (1u << 16)) want = ((want / 2 + 63) / 64) * 64;
+        if (r != TRB_OK) return r;
+    }
+    const Tuning& tu = s->tune;
+    const bool stats = (flags & TRB_RENDER_STATS) != 0, anim = s->ds.has_anim != 0, occl = d_occ != nullptr;
+    trb::RenderParams rp{};
+    rp.stats = d_stats; rp.error_flag = s->d_error;
+    const unsigned resident = stats ? 4u : (anim ? 8u : 9u); // as for renders: two rounds of what is resident per SM
+    const unsigned tgrid = (unsigned)s->sm_count * (tu.trace_grid ? tu.trace_grid : 2u * resident);
+    const uint32_t tflags = (flags & TRB_RENDER_REFERENCE_SHADOW) | (tu.exact_box ? trb::WF_TRACE_FORCE_EXACT_BOX : 0u);
+    const uint32_t sched = std::max(1u, tu.sched);
+    const uint32_t* no_sort = nullptr;
+    for (size_t b = 0; b < n; b += want) {
+        const size_t m = std::min<size_t>(want, n - b);
+        trb::WfState wf = s->wf;
+        wf.n_paths = (uint32_t)m;
+        const unsigned lgrid = (unsigned)std::min<size_t>((m + 255) / 256, (size_t)s->sm_count * 8);
+        if (occl) trb::k_query_load<true><<<lgrid, 256, 0, st>>>(wf, d_rays + b);
+        else trb::k_query_load<false><<<lgrid, 256, 0, st>>>(wf, d_rays + b);
+        g_launches++;
+        launch_anim_table(s, wf, m, false, st);
+        // the default trace variant (trace.pipe 36: box_hit_finite + RayHome) with each ray's own [min_t, max_t]
+        if (anim) {
+            if (stats) trb::k_wf_trace<true, 4, 16, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
+            else trb::k_wf_trace<false, 8, 12, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
+        } else if (stats) trb::k_wf_trace<true, 4, 16, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
+        else trb::k_wf_trace<false, 9, 12, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
+        g_launches++;
+        if (occl) trb::k_query_occluded<<<lgrid, 256, 0, st>>>(wf, d_occ + b);
+        else {
+            const unsigned rgrid = (unsigned)std::min<size_t>((m + 127) / 128, (size_t)s->sm_count * 16);
+            if (anim) trb::k_query_records<true><<<rgrid, 128, 0, st>>>(s->ds, wf, d_out + b);
+            else trb::k_query_records<false><<<rgrid, 128, 0, st>>>(s->ds, wf, d_out + b);
+        }
+        g_launches++;
+    }
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// The blocking host-buffer form of a query: stage the rays, run the passes on the default stream, copy the results back.
+trb_status query_host(trb_scene* s, size_t n, const trb_query_ray* rays, trb_intersection* out, uint8_t* occluded, uint32_t flags, trb_stats* stats) {
+    if (n == 0) { if (stats) std::memset(stats, 0, sizeof *stats); return TRB_OK; }
+    CU(cudaSetDevice(s->device));
+    const size_t out_bytes = out ? n * sizeof(trb_intersection) : n;
+    void* d_rays = nullptr; void* d_res = nullptr;
+    CU(cudaMalloc(&d_rays, n * sizeof(trb_query_ray)));
+    cudaError_t e = cudaMalloc(&d_res, out_bytes);
+    if (e != cudaSuccess) { cudaFree(d_rays); CU(e); }
+    e = cudaMemcpy(d_rays, rays, n * sizeof(trb_query_ray), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0);
+    trb_status r = TRB_OK;
+    if (e == cudaSuccess) {
+        cudaEventRecord(s->ev0, 0);
+        r = query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), out ? static_cast<trb_intersection*>(d_res) : nullptr,
+                         out ? nullptr : static_cast<uint8_t*>(d_res), flags, s->d_stats, 0);
+        cudaEventRecord(s->ev1, 0);
+    }
+    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out ? static_cast<void*>(out) : static_cast<void*>(occluded), d_res, out_bytes, cudaMemcpyDeviceToHost);
+    if (r != TRB_OK) cudaDeviceSynchronize(); // passes already enqueued still read the buffers
+    cudaFree(d_rays); cudaFree(d_res);
+    if (r != TRB_OK) return r;
+    CU(e);
+    r = check_error_flag(s);
+    if (r != TRB_OK) return r;
+    if (stats) {
+        trb::DStats h;
+        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
+        std::memset(stats, 0, sizeof *stats);
+        stats_out(h, stats);
+        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
+    }
     return TRB_OK;
 }
 
@@ -1516,6 +1618,32 @@ trb_status trb_intersect(trb_scene* s, size_t n, const trb_ray* rays, trb_hit* h
         CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
     }
     return TRB_OK;
+}
+
+trb_status trb_intersect_records(trb_scene* s, size_t n, const trb_query_ray* rays, trb_intersection* out, uint32_t flags, trb_stats* stats) {
+    const trb_status r = query_check(s, n, rays, out, flags, TRB_RENDER_STATS, false, false);
+    return r != TRB_OK ? r : query_host(s, n, rays, out, nullptr, flags, stats);
+}
+
+trb_status trb_intersect_records_device(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb_intersection* d_out, uint32_t flags,
+                                        trb_stats* d_stats, void* stream) {
+    const trb_status r = query_check(s, n, d_rays, d_out, flags, TRB_RENDER_STATS, true, true);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return query_passes(s, n, d_rays, d_out, nullptr, flags, reinterpret_cast<trb::DStats*>(d_stats), static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_occluded(trb_scene* s, size_t n, const trb_query_ray* rays, uint8_t* occluded, uint32_t flags, trb_stats* stats) {
+    const trb_status r = query_check(s, n, rays, occluded, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW, false, false);
+    return r != TRB_OK ? r : query_host(s, n, rays, nullptr, occluded, flags, stats);
+}
+
+trb_status trb_occluded_device(trb_scene* s, size_t n, const trb_query_ray* d_rays, uint8_t* d_occluded, uint32_t flags, trb_stats* d_stats,
+                               void* stream) {
+    const trb_status r = query_check(s, n, d_rays, d_occluded, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW, true, false);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return query_passes(s, n, d_rays, nullptr, d_occluded, flags, reinterpret_cast<trb::DStats*>(d_stats), static_cast<cudaStream_t>(stream));
 }
 
 trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {

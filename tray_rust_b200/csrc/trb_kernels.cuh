@@ -745,8 +745,11 @@ __device__ __noinline__ bool scene_trace(const DScene& sc, Ray& ray, HitRec& hit
 // ------------------------------------------------------------------------------------------
 struct Surf { f3 p, n, ng, dp_du; float u, v; }; // u, v: only filled when the scene has image textures (DScene::n_textures)
 
-template <bool ANIM>
-__device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, const HitRec& hit, Surf& s, float time, const float* xf_row = nullptr) {
+// RECORD (ray-query records, k_query_records): the whole DifferentialGeometry — u, v for every shape whatever the scene's
+// textures, and dp_dv, transformed to world space into *dp_dv_world. The shading kernels instantiate RECORD = false only.
+template <bool ANIM, bool RECORD = false>
+__device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, const HitRec& hit, Surf& s, float time, const float* xf_row = nullptr,
+                                           f3* dp_dv_world = nullptr) {
     const DInstance& in = sc.instances[hit.inst];
     float m[16], w[16];
     instance_inv_mat<ANIM>(sc, in, time, m, w, xf_row);
@@ -754,6 +757,7 @@ __device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, con
     const f3 p = o + d * hit.t; // ray.at(t) of the local ray
     const uint32_t shape = __ldg(&in.shape);
     f3 n, ng, dp_du;
+    f3 dp_dv_rec; // RECORD only
     if (shape == TRB_SHAPE_MESH) {
         const DMesh& me = sc.meshes[__ldg(&in.mesh)];
         const uint32_t ia = __ldg(&me.indices[3 * hit.prim]), ib = __ldg(&me.indices[3 * hit.prim + 1]), ic = __ldg(&me.indices[3 * hit.prim + 2]);
@@ -776,19 +780,26 @@ __device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, con
         if (det == 0.0f) {
             f3 dp_dv;
             coord_system(unit(cross3(pc - pa, pb - pa)), dp_du, dp_dv); // cross(e[1], e[0])
+            if (RECORD) dp_dv_rec = dp_dv;
         } else {
             const float idet = 1.0f / det;
             const f3 dp0 = pa - pc, dp1 = pb - pc;
             dp_du = (dv1 * dp0 - dv0 * dp1) * idet;
+            if (RECORD) dp_dv_rec = (-du1 * dp0 + du0 * dp1) * idet;    // mesh.rs:194
         }
     } else if (shape == TRB_SHAPE_SPHERE) {
         n = unit(p); ng = n;                                            // sphere.rs:58, with_normal
         dp_du = mk(-TRB_PI * 2.0f * p.y, TRB_PI * 2.0f * p.x, 0.0f);    // sphere.rs:75
-        if (sc.n_textures) { // sphere.rs:59-73
+        if (RECORD || sc.n_textures) { // sphere.rs:59-73
             const float radius = __ldg(&in.p0);
             const float theta = dacos(clampf(p.z / radius, -1.0f, 1.0f));
             const float uu = datan2(p.x, p.y) / (2.0f * TRB_PI);
             s.u = uu < 0.0f ? uu + 1.0f : uu; s.v = theta / TRB_PI;
+            if (RECORD) { // sphere.rs:64-66,77-78
+                const float inv_z = 1.0f / sqrtf(p.x * p.x + p.y * p.y);
+                const float cos_phi = p.x * inv_z, sin_phi = p.y * inv_z;
+                dp_dv_rec = mk(p.z * cos_phi, p.z * sin_phi, -radius * dsin(theta)) * TRB_PI;
+            }
         }
     } else if (shape == TRB_SHAPE_DISK) {
         const float radius = __ldg(&in.p0), inner = __ldg(&in.p1);
@@ -797,7 +808,8 @@ __device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, con
         const f3 dp_dv = ((inner - radius) / hr) * mk(p.x, p.y, 0.0f);  // disk.rs:72
         n = unit(cross3(dp_du, dp_dv));                                  // DifferentialGeometry::new
         ng = unit(mk(0.0f, 0.0f, 1.0f));
-        if (sc.n_textures) { // disk.rs:60-70
+        if (RECORD) dp_dv_rec = dp_dv;
+        if (RECORD || sc.n_textures) { // disk.rs:60-70
             float phi = datan2(p.y, p.x);
             if (phi < 0.0f) phi += TRB_PI * 2.0f;
             s.u = phi / (2.0f * TRB_PI); s.v = 1.0f - (hr - inner) / (radius - inner);
@@ -808,12 +820,14 @@ __device__ __forceinline__ void surface_at(const DScene& sc, const Ray& ray, con
         const f3 dp_dv = mk(0.0f, hh * 2.0f, 0.0f);
         n = unit(cross3(dp_du, dp_dv));
         ng = unit(mk(0.0f, 0.0f, 1.0f));
+        if (RECORD) dp_dv_rec = dp_dv;
         s.u = (p.x + hw) / (2.0f * hw); s.v = (p.y + hh) / (2.0f * hh);  // rectangle.rs:54-55
     }
     s.p = xf_point(w, p);
     s.n = xf_normal_t(m, n);
     s.ng = xf_normal_t(m, ng);
     s.dp_du = xf_vector(w, dp_du);
+    if (RECORD) *dp_dv_world = xf_vector(w, dp_dv_rec);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2075,6 +2089,7 @@ template <bool STATS, int MINB, int SMEM_STACK, bool ANIM, bool PHASED, bool QUA
 __global__ void __launch_bounds__(128, MINB) k_wf_trace(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
                                                          uint32_t round, uint32_t flags, int WF_REFILL_IDLE, uint32_t sched, const uint32_t* __restrict__ q_sorted) {
     constexpr bool HOME = PHASED && (PIPE & 32) != 0; // RayHome: world ray and hit record live in the path state, not in registers
+    constexpr bool QUERY = (PIPE & 64) != 0;          // ray queries (k_query_load): each ray's [min_t, max_t] is org.w and the direction entry's .w
     uint32_t* cnt_r = wf.counters + round * WF_CNT;
     const uint32_t n_cont = cnt_r[WF_N_CONT], n_shadow = cnt_r[WF_N_SHADOW], n_mis = cnt_r[WF_N_MIS];
     const uint32_t total = n_cont + n_shadow + n_mis;
@@ -2134,8 +2149,8 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(const __grid_constant__ 
                     const float4 o4 = __ldcs(&wf.org[p]);
                     const float4 d4 = __ldcs(type == 0 ? &wf.cont[p] : (type == 1 ? &wf.shadow[p] : &wf.mis[p])); // streamed: keep L2 for the BVH
                     Ray ray; ray.o = mk(o4.x, o4.y, o4.z); ray.d = mk(d4.x, d4.y, d4.z);
-                    ray.tmin = (type == 0 && round == 0) ? 0.0f : 0.001f;
-                    ray.tmax = type == 1 ? 0.999f : finf();
+                    ray.tmin = QUERY ? o4.w : ((type == 0 && round == 0) ? 0.0f : 0.001f);
+                    ray.tmax = QUERY ? d4.w : (type == 1 ? 0.999f : finf());
                     trace_init(sc, t, ray, type == 1 && shadow_any, ANIM ? __ldg(&wf.thr[p].w) : 0.0f, QUADS && PHASED, (flags & WF_TRACE_FORCE_EXACT_BOX) != 0);
                     t.xf_row = wf_xf_row<ANIM>(wf, p);
                     if (PHASED) { stack.put(0, (unsigned long long)ST_DONE); t.sp = 1; } // bottom sentinel: popping it ends the ray
@@ -2808,6 +2823,60 @@ __global__ void __launch_bounds__(128) k_intersect(const __grid_constant__ DScen
         *reinterpret_cast<uint4*>(hits + i) = o;
     }
     if (stats) flush_stats(stats, rc, cnt, 0, STATS);
+}
+
+// ------------------------------------------------------------------------------------------
+// Ray queries (trb_intersect_records / trb_occluded) on the render's trace kernel: one pass = k_query_load writes the pass's
+// rays into the path state as round 0 of a wavefront (continuation rays for records, shadow rays for occlusion), keyframed
+// scenes fill the transform table from each ray's time (k_wf_anim_table[2], unchanged), k_wf_trace runs with PIPE bit 64 (each
+// ray's own [min_t, max_t]), then k_query_records / k_query_occluded read the results out of the path state.
+// ------------------------------------------------------------------------------------------
+template <bool OCCLUSION>
+__global__ void __launch_bounds__(256) k_query_load(const __grid_constant__ WfState wf, const trb_query_ray* __restrict__ rays) {
+    const uint32_t n = wf.n_paths;
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const float4* r = reinterpret_cast<const float4*>(rays + p); // (o, d.x) (d.yz, min_t, max_t) (time, pad)
+        const float4 a = __ldg(r), b = __ldg(r + 1), c = __ldg(r + 2);
+        wf.org[p] = make_float4(a.x, a.y, a.z, b.z);
+        (OCCLUSION ? wf.shadow : wf.cont)[p] = make_float4(a.w, b.x, b.y, b.w);
+        wf.thr[p] = make_float4(0.0f, 0.0f, 0.0f, c.x); // .w: ray.time, as k_wf_generate leaves it for the transform table and the trace
+        (OCCLUSION ? wf.q_shadow : wf.q_cont)[p] = p;
+    }
+    if (blockIdx.x == 0 && threadIdx.x < WF_CNT) wf.counters[threadIdx.x] = threadIdx.x == (OCCLUSION ? WF_N_SHADOW : WF_N_CONT) ? n : 0u;
+}
+// geometry::Intersection of each ray (scene.rs:148-150): the DifferentialGeometry of Receiver / Emitter::intersect in world space
+// (receiver.rs:36-41, emitter.rs:128-134), built by surface_at's shape code from the trace kernel's (t, inst, prim, b1, b2)
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_query_records(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, trb_intersection* __restrict__ out) {
+    const uint32_t n = wf.n_paths;
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const float4 o4 = wf.org[p], d4 = wf.cont[p];
+        const uint4 h4 = wf.hit[p];
+        float4 q[6] = {make_float4(d4.w, __uint_as_float(TRB_MISS), 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f),
+                       make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f), make_float4(0.0f, 0.0f, 0.0f, 0.0f)};
+        if (h4.x != TRB_MISS) {
+            Ray ray; ray.o = mk(o4.x, o4.y, o4.z); ray.d = mk(d4.x, d4.y, d4.z); ray.tmin = o4.w; ray.tmax = d4.w;
+            HitRec hit; hit.t = d4.w; hit.inst = h4.x; hit.prim = h4.y; hit.b1 = __uint_as_float(h4.z); hit.b2 = __uint_as_float(h4.w);
+            const float time = wf.thr[p].w;
+            Surf s;
+            f3 dp_dv;
+            surface_at<ANIM, true>(sc, ray, hit, s, time, wf_xf_row<ANIM>(wf, p), &dp_dv);
+            const uint32_t material = __ldg(&sc.instances[hit.inst].material);
+            // t inst prim material | p n.x | n.yz ng.xy | ng.z u v time | dp_du dp_dv.x | dp_dv.yz pad
+            q[0] = make_float4(d4.w, __uint_as_float(hit.inst), __uint_as_float(hit.prim), __uint_as_float(material));
+            q[1] = make_float4(s.p.x, s.p.y, s.p.z, s.n.x);
+            q[2] = make_float4(s.n.y, s.n.z, s.ng.x, s.ng.y);
+            q[3] = make_float4(s.ng.z, s.u, s.v, time);
+            q[4] = make_float4(s.dp_du.x, s.dp_du.y, s.dp_du.z, dp_dv.x);
+            q[5] = make_float4(dp_dv.y, dp_dv.z, 0.0f, 0.0f);
+        }
+        float4* dst = reinterpret_cast<float4*>(out + p);
+#pragma unroll
+        for (int k = 0; k < 6; ++k) dst[k] = q[k];
+    }
+}
+__global__ void __launch_bounds__(256) k_query_occluded(const __grid_constant__ WfState wf, uint8_t* __restrict__ out) {
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < wf.n_paths; p += gridDim.x * blockDim.x) out[p] = __float_as_uint(wf.shadow[p].w) != 0u ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------
