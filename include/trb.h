@@ -286,6 +286,22 @@ typedef struct trb_intersection {
     uint32_t pad[2];
 } trb_intersection;
 
+/* A caller's ray for trb_illumination: linalg::Ray (src/linalg/ray.rs) with its time, plus the key of its sample streams.
+ * d is used as given (the reference does not normalise a caller's ray); [min_t, max_t] bounds the primary intersection only,
+ * child rays start at 0.001 as Ray::child does (path.rs:109-110); time is ray.time of the whole path (keyframed transforms,
+ * AnimatedColor emission). Sample j of the ray draws from the camera-sample stream (seed, key, sample + j): key plays the role
+ * of the render's pixel index, sample of its sample index. 48 bytes (three 16-byte loads); pad is ignored. */
+typedef struct trb_illum_ray {
+    float o[3];
+    float d[3];
+    float min_t, max_t;
+    float time;
+    uint32_t key;
+    uint32_t sample;
+    uint32_t pad;
+} trb_illum_ray;
+enum { TRB_QUERY_CLAMP = 32u }; /* trb_illumination: clamp each sample to [0, 1] before averaging, as thread_work does (multithreaded.rs:99) */
+
 /* Per camera sample record for parity tests: film position and the clamped radiance
  * pushed as ImageSample (multithreaded.rs:98-102). */
 typedef struct trb_sample {
@@ -433,6 +449,25 @@ trb_status trb_occluded(trb_scene* scene, size_t n, const trb_query_ray* rays, u
 /* Device-buffer variant of trb_occluded, with trb_intersect_records_device's contract (d_rays 16-byte aligned). */
 trb_status trb_occluded_device(trb_scene* scene, size_t n, const trb_query_ray* d_rays, uint8_t* d_occluded, uint32_t flags,
                                trb_stats* d_stats, void* cuda_stream);
+
+/* ≙ the per-sample body of thread_work (multithreaded.rs:95-103) along caller rays: sample j (0 <= j < spp) of ray i runs
+ * Scene::intersect and, on a hit, the scene integrator's Integrator::illumination (Path, Whitted or NormalsDebug); a miss is
+ * black. Its per-path sample arrays, Russian roulette and Whitted node streams come from the camera-sample stream
+ * (seed, rays[i].key, rays[i].sample + j mod 2^32) with LD offset 0, so a trb_camera_rays ray submitted with key = its pixel,
+ * sample = its sample index, spp = 1 and TRB_QUERY_CLAMP returns trb_render_samples' r, g, b bits.
+ * rgb[3i + c] = (sum of the spp samples' radiance, added in sample order) / spp in float32; each sample is clamped to [0, 1]
+ * first only with TRB_QUERY_CLAMP. flags: TRB_RENDER_STATS, TRB_RENDER_REFERENCE_SHADOW, TRB_QUERY_CLAMP; anything else is
+ * TRB_INVALID_ARG. stats: camera_samples = rays_primary = n * spp, shadow / MIS / continuation rays as a render counts them.
+ * The paths run on the render's wavefront kernels in passes of at most "pass.paths" samples holding whole rays. TRB_INVALID_ARG
+ * for null arguments, spp == 0 or > 65536, or before the first update_frame; n == 0 is TRB_OK. TLAS as trb_intersect_records.
+ * Host buffers; blocking. */
+trb_status trb_illumination(trb_scene* scene, size_t n, const trb_illum_ray* rays, uint32_t spp, uint32_t seed, float* rgb, uint32_t flags,
+                            trb_stats* stats);
+
+/* Device-buffer variant of trb_illumination, with trb_intersect_records_device's contract: d_rays 16-byte aligned, d_rgb 4-byte
+ * aligned, d_stats NULL or a DEVICE trb_stats, enqueued on cuda_stream without host synchronisation. */
+trb_status trb_illumination_device(trb_scene* scene, size_t n, const trb_illum_ray* d_rays, uint32_t spp, uint32_t seed, float* d_rgb,
+                                   uint32_t flags, trb_stats* d_stats, void* cuda_stream);
 
 /* ≙ LowDiscrepancy::get_samples + get_samples_1d + Camera::generate_ray
  * (ld.rs:33-64, camera.rs:150-157) for the selected blocks/samples: writes one ray and

@@ -2,7 +2,7 @@
 TEST INFRASTRUCTURE, like oracle/pyoracle.py.
 
 ``QueryOracleScene`` is an ``OracleScene`` backed by that library (the detmath oracle with the ray queries added), so it has
-every oracle method plus ``intersect_records`` and ``occluded`` with the signatures of ``tray_rust_b200.api.Scene``.
+every oracle method plus ``intersect_records``, ``occluded`` and ``illumination`` with the signatures of ``tray_rust_b200.api.Scene``.
 """
 import ctypes as C
 
@@ -18,12 +18,14 @@ def load():
         vp, sz = C.c_void_p, C.c_size_t
         lib.orc_intersect_records.argtypes = [vp, sz, vp, vp, C.POINTER(F.Stats)]
         lib.orc_occluded.argtypes = [vp, sz, vp, vp, C.POINTER(F.Stats)]
+        lib.orc_illumination.argtypes = [vp, sz, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, C.POINTER(F.Stats)]
         lib._queries_ready = True
     return lib
 
 
 class QueryOracleScene(O.OracleScene):
-    """The oracle with Scene::intersect returning the whole Intersection and OcclusionTester::occluded, per-ray times."""
+    """The oracle with Scene::intersect returning the whole Intersection, OcclusionTester::occluded and Integrator::illumination
+    along caller rays, per-ray times."""
 
     def __init__(self, desc, baseline=False):
         load()
@@ -44,3 +46,12 @@ class QueryOracleScene(O.OracleScene):
         st = F.Stats()
         self._check(self._lib.orc_occluded(self._h, len(rays), F.ptr(rays), F.ptr(out), C.byref(st)))
         return out.astype(bool), st
+
+    def illumination(self, rays, spp=1, seed=1, clamp=False, stats=None, reference=True):
+        """Returns the (n, 3) float32 means; a Stats passed as `stats` receives the counters. The oracle always counts its tests and
+        walks shadow rays to the closest hit."""
+        rays = np.ascontiguousarray(rays, dtype=F.ILLUM_RAY_DTYPE)
+        out = np.zeros((len(rays), 3), np.float32)
+        st = stats if stats is not None else F.Stats()
+        self._check(self._lib.orc_illumination(self._h, len(rays), F.ptr(rays), spp, seed, F.ptr(out), 1 if clamp else 0, C.byref(st)))
+        return out

@@ -1,12 +1,17 @@
 """Ray-query throughput on one GPU: trb_intersect (k_intersect, one thread per ray), trb_intersect_records and trb_occluded (the
 render's wavefront trace kernel) on the C4 workload (1 M triangles), device buffers, GPU time between CUDA events on one stream.
-Measures and reports; gates nothing.
+Then trb_illumination against trb_render_device on the same camera samples. Measures and reports; gates nothing.
 
-    python tools/query_bench.py [--rays 4194304] [--reps 5] [--tris 1000000] [--out results/query_bench.json]
+    python tools/query_bench.py [--rays 4194304] [--reps 5] [--tris 1000000] [--width 1920 --height 1080] [--out results/query_bench.json]
 
 The rays are incoherent: seeded origins uniform in the Cornell box and directions uniform on the sphere, as a render's bounce rays
 are. trb_intersect has no per-ray time and returns (t, inst, prim); trb_intersect_records also builds the whole world-space
 Intersection (96 bytes per ray); trb_occluded is timed in both shadow modes. The median of --reps timed calls after one warm-up.
+
+trb_illumination takes the --width x --height camera rays of C4 at 1 spp (trb_camera_rays, key = pixel, sample = 0, clamped), the
+camera samples trb_render_device renders at 1 spp with the same seed, so the two compute the same radiance and differ in what
+they start from (caller rays vs. the camera) and end with (per-ray means vs. the film). Both report camera samples/s and Mrays/s
+over every traced ray (primary, shadow, MIS, continuation).
 """
 import argparse
 import json
@@ -34,6 +39,8 @@ def main():
     ap.add_argument("--rays", type=int, default=1 << 22)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--tris", type=int, default=1_000_000)
+    ap.add_argument("--width", type=int, default=1920)
+    ap.add_argument("--height", type=int, default=1080)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch as T
@@ -87,9 +94,61 @@ def main():
     for name in cases:
         print("  %-40s %8.3f ms  %8.1f Mrays/s" % (name, res["ms"][name], res["mrays_per_s"][name]))
     print("  hit fraction %.3f, records equal trb_intersect's (t, inst): %s" % (res["hit_fraction"], res["records_match_trb_intersect"]))
+    illumination_vs_render(a, res)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         json.dump(res, open(a.out, "w"), indent=1)
+
+
+def illumination_vs_render(a, res):
+    import torch as T
+    dev = T.device("cuda:0")
+    g = api.Scene(SB.scene_c4(a.tris, a.width, a.height, 1).finish())
+    g.update_frame(0, 0.0, 0.0)
+    rays, _ = g.camera_rays(seed=1)
+    blocks = g.block_list().astype(np.int64)
+    i = np.arange(len(rays))
+    item, pix = i // 64, i % 64
+    q = np.zeros(len(rays), F.ILLUM_RAY_DTYPE)
+    for k in ("o", "d", "min_t", "max_t"):
+        q[k] = rays[k]
+    q["key"] = (blocks[item, 1] * 8 + pix // 8) * g.width + blocks[item, 0] * 8 + pix % 8
+    n = len(q)
+    d_q = T.from_numpy(q.view(np.uint8).copy()).to(dev)
+    d_rgb = T.empty(n * 3, dtype=T.float32, device=dev)
+    d_film = T.zeros(a.width * a.height * 4, dtype=T.float32, device=dev)
+    d_st = T.zeros(9, dtype=T.int64, device=dev)
+    s = T.cuda.Stream()
+    s.wait_stream(T.cuda.current_stream())
+    cases = {
+        "trb_illumination (camera rays, 1 spp)": lambda st: g.illumination_device(n, d_q.data_ptr(), d_rgb.data_ptr(), spp=1, seed=1, clamp=True,
+                                                                               d_stats=st, stream=s.cuda_stream),
+        "trb_render_device (1 spp)": lambda st: g.render_device(d_film.data_ptr(), st, s.cuda_stream, seed=1, spp=1),
+    }
+    res["illumination"] = {"camera_samples": n, "width": a.width, "height": a.height, "ms": {}, "samples_per_s": {}, "mrays_per_s": {}}
+    for name, call in cases.items():
+        d_st.zero_()
+        call(d_st.data_ptr())  # warm-up, and one call's ray counts
+        s.synchronize()
+        st = F.Stats.from_buffer_copy(d_st.cpu().numpy().tobytes())
+        ms = []
+        for _ in range(a.reps):
+            e0, e1 = T.cuda.Event(enable_timing=True), T.cuda.Event(enable_timing=True)
+            e0.record(s)
+            call(None)
+            e1.record(s)
+            s.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        med = float(np.median(ms))
+        r = res["illumination"]
+        r["ms"][name] = med
+        r["samples_per_s"][name] = st.camera_samples / med * 1e3
+        r["mrays_per_s"][name] = st.rays_total() / med / 1e3
+    g.check_error()
+    print("  %d camera samples of C4 at %dx%d, 1 spp:" % (n, a.width, a.height))
+    for name in cases:
+        r = res["illumination"]
+        print("  %-40s %8.3f ms  %8.2f M samples/s  %8.1f Mrays/s" % (name, r["ms"][name], r["samples_per_s"][name] / 1e6, r["mrays_per_s"][name]))
 
 
 if __name__ == "__main__":

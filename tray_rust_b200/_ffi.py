@@ -21,6 +21,7 @@ MAT_MATTE, MAT_PLASTIC, MAT_METAL, MAT_SPECULAR_METAL, MAT_GLASS, MAT_ROUGH_GLAS
 FILTER_MITCHELL_NETRAVALI, FILTER_GAUSSIAN = 0, 1
 INTEGRATOR_PATH, INTEGRATOR_WHITTED, INTEGRATOR_NORMALS_DEBUG = 0, 1, 2
 RENDER_STATS, RENDER_NO_UPDATE, RENDER_REFERENCE_SHADOW, RENDER_MEGAKERNEL, RENDER_TIME_TRACE = 1, 2, 4, 8, 16
+QUERY_CLAMP = 32  # trb_illumination: clamp each sample to [0, 1] before averaging
 MISS = 0xFFFFFFFF
 BVH_LEAF = 0x80000000
 MERL_TABLE_FLOATS = 90 * 90 * 180 * 3
@@ -133,6 +134,10 @@ class Intersection(C.Structure):
                 ("u", f32), ("v", f32), ("time", f32), ("dp_du", f32 * 3), ("dp_dv", f32 * 3), ("pad", u32 * 2)]
 
 
+class IllumRay(C.Structure):
+    _fields_ = [("o", f32 * 3), ("d", f32 * 3), ("min_t", f32), ("max_t", f32), ("time", f32), ("key", u32), ("sample", u32), ("pad", u32)]
+
+
 class Sample(C.Structure):
     _fields_ = [("x", f32), ("y", f32), ("r", f32), ("g", f32), ("b", f32)]
 
@@ -152,6 +157,8 @@ QUERY_RAY_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("min_t", "<f4"), 
 INTERSECTION_DTYPE = np.dtype([("t", "<f4"), ("inst", "<u4"), ("prim", "<u4"), ("material", "<u4"), ("p", "<f4", 3), ("n", "<f4", 3),
                                ("ng", "<f4", 3), ("u", "<f4"), ("v", "<f4"), ("time", "<f4"), ("dp_du", "<f4", 3), ("dp_dv", "<f4", 3),
                                ("pad", "<u4", 2)])
+ILLUM_RAY_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("min_t", "<f4"), ("max_t", "<f4"), ("time", "<f4"), ("key", "<u4"),
+                            ("sample", "<u4"), ("pad", "<u4")])
 
 TRB_SYMBOLS = [
     "trb_scene_create", "trb_scene_load_json", "trb_scene_destroy", "trb_scene_info", "trb_scene_update_frame",
@@ -164,6 +171,7 @@ TRB_SYMBOLS = [
     "trb_render_adaptive", "trb_render_samples_adaptive", "trb_adaptive_schedule", "trb_host_adaptive_decide",
     "trb_render_adaptive_device", "trb_render_sharded_adaptive", "trb_group_render_adaptive",
     "trb_intersect_records", "trb_intersect_records_device", "trb_occluded", "trb_occluded_device",
+    "trb_illumination", "trb_illumination_device",
 ]
 
 _trb = None
@@ -200,6 +208,8 @@ def load_trb():
     lib.trb_intersect_records_device.argtypes = [vp, sz, vp, vp, u32, vp, vp]
     lib.trb_occluded.argtypes = [vp, sz, vp, vp, u32, C.POINTER(Stats)]
     lib.trb_occluded_device.argtypes = [vp, sz, vp, vp, u32, vp, vp]
+    lib.trb_illumination.argtypes = [vp, sz, vp, u32, u32, vp, u32, C.POINTER(Stats)]
+    lib.trb_illumination_device.argtypes = [vp, sz, vp, u32, u32, vp, u32, vp, vp]
     lib.trb_camera_rays.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]

@@ -232,6 +232,24 @@ class Scene(_Base):
         flags = (F.RENDER_STATS if stats else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0)
         self._check(self._lib.trb_occluded_device(self._h, n, d_rays, d_occluded, flags, d_stats, stream))
 
+    def illumination(self, rays, spp=1, seed=1, clamp=False, stats=None, reference=False):
+        """trb_illumination: Integrator::illumination along each ILLUM_RAY_DTYPE ray, spp samples from the camera-sample streams
+        (seed, key, sample + j). Returns the (n, 3) float32 means. clamp=True clamps each sample to [0, 1] first, as a render does.
+        stats: None, or a Stats that receives the counters, node / triangle / instance tests included. reference=True traces shadow
+        rays to the closest hit like the reference (same radiance, the reference's test counters)."""
+        rays = np.ascontiguousarray(rays, dtype=F.ILLUM_RAY_DTYPE)
+        out = np.zeros((len(rays), 3), np.float32)
+        flags = (F.RENDER_STATS if stats is not None else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0) | (F.QUERY_CLAMP if clamp else 0)
+        self._check(self._lib.trb_illumination(self._h, len(rays), F.ptr(rays), spp, seed, F.ptr(out), flags,
+                                               C.byref(stats) if stats is not None else None))
+        return out
+
+    def illumination_device(self, n, d_rays, d_rgb, spp=1, seed=1, clamp=False, d_stats=None, stream=None, stats=False, reference=False):
+        """trb_illumination_device: n illumination rays (48 B each, 16-byte aligned) -> n * 3 float32 means in d_rgb, enqueued on
+        `stream` (a cudaStream_t as an int; None = default stream) without host synchronisation."""
+        flags = (F.RENDER_STATS if stats else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0) | (F.QUERY_CLAMP if clamp else 0)
+        self._check(self._lib.trb_illumination_device(self._h, n, d_rays, spp, seed, d_rgb, flags, d_stats, stream))
+
     def to_srgb8(self, film):
         film = np.ascontiguousarray(film, dtype=np.float32)
         out = np.zeros((self.height, self.width, 3), np.uint8)

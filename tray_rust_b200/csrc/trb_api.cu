@@ -467,46 +467,71 @@ void launch_anim_table(trb_scene* s, trb::WfState& wf, size_t n_paths, bool adap
     g_launches++;
 }
 
-// One wavefront pass over rp's blocks x samples: generate, then (trace, shade) per bounce round, then the film
-// (DESIGN.md "Execution shape"). n_paths = blocks * 64 * sample_count must fit the allocated path state.
-trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st) {
-    const size_t n_paths = (size_t)rp.n_blocks * 64 * rp.sample_count;
-    if (n_paths > s->wf_capacity || n_paths >= (1ull << 30)) return fail(TRB_INVALID_ARG, "pass larger than the wavefront state");
+// The default trace variant (trace.pipe 36: box_hit_finite + RayHome) with PIPE bit 64: each ray's own [min_t, max_t] from the
+// path state (k_query_load, k_illum_load). The ray queries' only trace, and round 0 of the illumination queries.
+void launch_query_trace(trb_scene* s, const trb::RenderParams& rp, const trb::WfState& wf, uint32_t tflags, bool stats, const uint32_t* q_sorted,
+                        cudaStream_t st) {
     const Tuning& tu = s->tune;
-    trb::WfState wf = s->wf;
-    wf.n_paths = (uint32_t)n_paths; // Adaptive passes: the worst case (the stride of the q_mid lists); their kernels read the live count on the device
-    wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
-    if (s->integrator.type != TRB_INTEGRATOR_PATH) { // Whitted / NormalsDebug: one thread per camera sample, then the same film kernel
-        const unsigned grid = (unsigned)std::min<size_t>((n_paths + 127) / 128, (size_t)s->sm_count * 8);
-        const bool anim = s->ds.has_anim != 0;
-        if (anim) { if (mode == 0) trb::k_simple_integrator<0, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags);
-                    else trb::k_simple_integrator<1, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags); }
-        else if (mode == 0) trb::k_simple_integrator<0, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags);
-        else trb::k_simple_integrator<1, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags);
-        g_launches++;
-        if (mode == 0) {
-            const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
-            const unsigned film_grid = std::min<unsigned>(rp.n_blocks, (unsigned)s->sm_count * 8);
-            if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
-            else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, rp, wf);
-            g_launches++;
-        }
-        CU(cudaGetLastError());
-        return TRB_OK;
-    }
-    const bool stats = (flags & TRB_RENDER_STATS) != 0;
-    const uint32_t rounds = s->integrator.max_depth + 2; // bounces 0..max_depth, plus the round that only resolves
-    CU(cudaMemsetAsync(wf.counters, 0, 64 * trb::WF_CNT * sizeof(uint32_t), st));
-    const unsigned gen_grid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
-    const bool anim = s->ds.has_anim != 0; // static scenes run kernels with no animation code in them at all
-    if (rp.ad_state) { // Adaptive sampler round: only the pixels still sampling queue their paths
-        if (anim) trb::k_wf_generate_ad<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
-        else trb::k_wf_generate_ad<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
-    } else if (anim) trb::k_wf_generate<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
-    else trb::k_wf_generate<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
-    g_launches++;
-    launch_anim_table(s, wf, n_paths, rp.ad_state != nullptr, st);
+    const bool anim = s->ds.has_anim != 0;
+    const unsigned resident = stats ? 4u : (anim ? 8u : 9u); // as for renders: two rounds of what is resident per SM
+    const unsigned tgrid = (unsigned)s->sm_count * (tu.trace_grid ? tu.trace_grid : 2u * resident);
+    const uint32_t sched = std::max(1u, tu.sched);
+    if (anim) {
+        if (stats) trb::k_wf_trace<true, 4, 16, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+        else trb::k_wf_trace<false, 8, 12, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+    } else if (stats) trb::k_wf_trace<true, 4, 16, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+    else trb::k_wf_trace<false, 9, 12, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+}
+
+// The shade kernels of one bounce round, chosen per scene (split or fused, material buckets). MODE 0: film, 1: parity records,
+// 2: illumination queries. Counts the round's trace launch with its own.
+template <int MODE>
+void launch_shade(trb_scene* s, const trb::RenderParams& rp, const trb::WfState& wf, uint32_t round, cudaStream_t st) {
+    const Tuning& tu = s->tune;
+    const bool anim = s->ds.has_anim != 0;
     const unsigned shade_grid = (unsigned)s->sm_count * 4;
+    constexpr int MB = MODE == 2 ? 2 : 0; // k_wf_shade_b: the renders' two modes shade alike
+    // per scene (shade_split < 0): split when the scene mixes material kinds, and also when it is all matte — the matte instantiations of
+    // _b / _c carry less code and fewer live values than the fused kernel; other one-kind scenes stay fused
+    const bool split_auto = s->mixed_materials || (tu.shade_sort && tu.shade_kind && s->material_kinds == (1u << TRB_MAT_MATTE));
+    if (tu.shade_split > 0 || (tu.shade_split < 0 && split_auto)) { // three kernels with fewer live values each (DESIGN.md "Split shading"); same device functions, same results
+        // with the material buckets, _b and _c run once per kind that has an instantiation of its own (matte: the commonest), and once
+        // for the other kinds the scene uses
+        const uint32_t all = 0xffu, own = (tu.shade_sort && tu.shade_kind) ? (s->material_kinds & (1u << TRB_MAT_MATTE)) : 0u;
+        const uint32_t rest = tu.shade_sort ? (s->material_kinds & ~own) : all;
+        if (anim) {
+            trb::k_wf_shade_a<MODE, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+            if (own) trb::k_wf_shade_b<true, 4, TRB_MAT_MATTE, MB><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_b<true, 3, -1, MB><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+            if (own) trb::k_wf_shade_c<MODE, true, 6, TRB_MAT_MATTE><<<(unsigned)s->sm_count * 6, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_c<MODE, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+        } else {
+            const unsigned ga = (unsigned)s->sm_count * 6, gb = (unsigned)s->sm_count * 5, gc = (unsigned)s->sm_count * 6;
+            trb::k_wf_shade_a<MODE, false, 6><<<ga, 128, 0, st>>>(s->ds, rp, wf, round);
+            if (own) trb::k_wf_shade_b<false, 5, TRB_MAT_MATTE, MB><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_b<false, 5, -1, MB><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+            if (own) trb::k_wf_shade_c<MODE, false, 6, TRB_MAT_MATTE><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_c<MODE, false, 6><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+        }
+        g_launches += 4;
+        return;
+    }
+    if (anim) { // keyframed variant: 168 registers at 3 CTAs per SM, or capped to 128 (some spills) at 4
+        if constexpr (MODE == 1) trb::k_wf_shade<1, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+        else if constexpr (MODE == 2) trb::k_wf_shade<2, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+        else if (tu.shade_anim_occ >= 4) trb::k_wf_shade<0, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+        else trb::k_wf_shade<0, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+    } else trb::k_wf_shade<MODE, false, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
+    g_launches += 2;
+}
+
+// The bounce rounds of a wavefront pass whose round-0 paths are in place (k_wf_generate or k_illum_load, then the transform
+// table): per round the optional ray sort, the trace, the shade kernels (DESIGN.md "Execution shape"). mode as launch_shade; the
+// illumination queries' round 0 traces each ray's own [min_t, max_t] (launch_query_trace).
+trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb::WfState& wf, uint32_t flags, int mode, cudaStream_t st) {
+    const Tuning& tu = s->tune;
+    const bool stats = (flags & TRB_RENDER_STATS) != 0, anim = s->ds.has_anim != 0;
+    const uint32_t rounds = s->integrator.max_depth + 2; // bounces 0..max_depth, plus the round that only resolves
     const int refill = tu.refill;
     // persistent CTAs: two rounds of what is resident per SM (9 for the default variant, 7 keyframed, 4 with counters) unless set
     const unsigned resident = (flags & TRB_RENDER_STATS) ? 4u : (tu.pipe == 0 || tu.pipe == 1 || tu.pipe == 33 ? 7u : (tu.pipe == 34 || tu.pipe == 35 || s->ds.has_anim ? 8u : 9u));
@@ -536,7 +561,8 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
         // CTAs per SM it is compiled for: 36 (default) = 9 CTAs / 12 stack entries in shared memory. The STATS and keyframed
         // variants run the same code at their own occupancy, so the parity tests' counters cover it.
         const bool v2 = tu.pipe != 0;
-        if (anim) {
+        if (mode == 2 && round == 0) launch_query_trace(s, rp, wf, tflags, stats, q_sorted, st);
+        else if (anim) {
             if (stats) { if (v2) TRB_TRACE_LAUNCH(true, 4, 16, true, true, false, 33); else TRB_TRACE_LAUNCH(true, 4, 16, true, true, false, 0); }
             else if (!v2) TRB_TRACE_LAUNCH(false, 7, 16, true, true, false, 0);
             else if (tu.pipe == 33) TRB_TRACE_LAUNCH(false, 7, 16, true, true, false, 33);
@@ -558,51 +584,53 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
         }
 #undef TRB_TRACE_LAUNCH
         if (ev.first) { CU(cudaEventRecord(ev.second, st)); s->trace_events.push_back(ev); }
-        // per scene (shade_split < 0): split when the scene mixes material kinds, and also when it is all matte — the matte instantiations of
-        // _b / _c carry less code and fewer live values than the fused kernel; other one-kind scenes stay fused
-        const bool split_auto = s->mixed_materials || (tu.shade_sort && tu.shade_kind && s->material_kinds == (1u << TRB_MAT_MATTE));
-        if (tu.shade_split > 0 || (tu.shade_split < 0 && split_auto)) { // three kernels with fewer live values each (DESIGN.md "Split shading"); same device functions, same results
-            // with the material buckets, _b and _c run once per kind that has an instantiation of its own (matte: the commonest), and once
-            // for the other kinds the scene uses
-            const uint32_t all = 0xffu, own = (tu.shade_sort && tu.shade_kind) ? (s->material_kinds & (1u << TRB_MAT_MATTE)) : 0u;
-            const uint32_t rest = tu.shade_sort ? (s->material_kinds & ~own) : all;
-            if (anim) {
-                if (mode == 0) trb::k_wf_shade_a<0, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-                else trb::k_wf_shade_a<1, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-                if (own) trb::k_wf_shade_b<true, 4, TRB_MAT_MATTE><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                if (rest) trb::k_wf_shade_b<true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                if (mode == 0) {
-                    if (own) trb::k_wf_shade_c<0, true, 6, TRB_MAT_MATTE><<<(unsigned)s->sm_count * 6, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                    if (rest) trb::k_wf_shade_c<0, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                } else {
-                    if (own) trb::k_wf_shade_c<1, true, 6, TRB_MAT_MATTE><<<(unsigned)s->sm_count * 6, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                    if (rest) trb::k_wf_shade_c<1, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                }
-            } else {
-                const unsigned ga = (unsigned)s->sm_count * 6, gb = (unsigned)s->sm_count * 5, gc = (unsigned)s->sm_count * 6;
-                if (mode == 0) trb::k_wf_shade_a<0, false, 6><<<ga, 128, 0, st>>>(s->ds, rp, wf, round);
-                else trb::k_wf_shade_a<1, false, 6><<<ga, 128, 0, st>>>(s->ds, rp, wf, round);
-                if (own) trb::k_wf_shade_b<false, 5, TRB_MAT_MATTE><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                if (rest) trb::k_wf_shade_b<false, 5><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                if (mode == 0) {
-                    if (own) trb::k_wf_shade_c<0, false, 6, TRB_MAT_MATTE><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                    if (rest) trb::k_wf_shade_c<0, false, 6><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                } else {
-                    if (own) trb::k_wf_shade_c<1, false, 6, TRB_MAT_MATTE><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, own);
-                    if (rest) trb::k_wf_shade_c<1, false, 6><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, rest);
-                }
-            }
-            g_launches += 4;
-            continue;
-        }
-        if (anim) { // keyframed variant: 168 registers at 3 CTAs per SM, or capped to 128 (some spills) at 4
-            if (mode != 0) trb::k_wf_shade<1, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-            else if (tu.shade_anim_occ >= 4) trb::k_wf_shade<0, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-            else trb::k_wf_shade<0, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-        } else if (mode == 0) trb::k_wf_shade<0, false, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-        else trb::k_wf_shade<1, false, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-        g_launches += 2;
+        if (mode == 0) launch_shade<0>(s, rp, wf, round, st);
+        else if (mode == 1) launch_shade<1>(s, rp, wf, round, st);
+        else launch_shade<2>(s, rp, wf, round, st);
     }
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// One wavefront pass over rp's blocks x samples: generate, then (trace, shade) per bounce round, then the film
+// (DESIGN.md "Execution shape"). n_paths = blocks * 64 * sample_count must fit the allocated path state.
+trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st) {
+    const size_t n_paths = (size_t)rp.n_blocks * 64 * rp.sample_count;
+    if (n_paths > s->wf_capacity || n_paths >= (1ull << 30)) return fail(TRB_INVALID_ARG, "pass larger than the wavefront state");
+    const Tuning& tu = s->tune;
+    trb::WfState wf = s->wf;
+    wf.n_paths = (uint32_t)n_paths; // Adaptive passes: the worst case (the stride of the q_mid lists); their kernels read the live count on the device
+    wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
+    if (s->integrator.type != TRB_INTEGRATOR_PATH) { // Whitted / NormalsDebug: one thread per camera sample, then the same film kernel
+        const unsigned grid = (unsigned)std::min<size_t>((n_paths + 127) / 128, (size_t)s->sm_count * 8);
+        const bool anim = s->ds.has_anim != 0;
+        if (anim) { if (mode == 0) trb::k_simple_integrator<0, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
+                    else trb::k_simple_integrator<1, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr); }
+        else if (mode == 0) trb::k_simple_integrator<0, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
+        else trb::k_simple_integrator<1, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
+        g_launches++;
+        if (mode == 0) {
+            const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
+            const unsigned film_grid = std::min<unsigned>(rp.n_blocks, (unsigned)s->sm_count * 8);
+            if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
+            else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, rp, wf);
+            g_launches++;
+        }
+        CU(cudaGetLastError());
+        return TRB_OK;
+    }
+    CU(cudaMemsetAsync(wf.counters, 0, 64 * trb::WF_CNT * sizeof(uint32_t), st));
+    const unsigned gen_grid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
+    const bool anim = s->ds.has_anim != 0; // static scenes run kernels with no animation code in them at all
+    if (rp.ad_state) { // Adaptive sampler round: only the pixels still sampling queue their paths
+        if (anim) trb::k_wf_generate_ad<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+        else trb::k_wf_generate_ad<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+    } else if (anim) trb::k_wf_generate<true><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+    else trb::k_wf_generate<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
+    g_launches++;
+    launch_anim_table(s, wf, n_paths, rp.ad_state != nullptr, st);
+    const trb_status r = wavefront_rounds(s, rp, wf, flags, mode, st);
+    if (r != TRB_OK) return r;
     if (mode == 0 && rp.film) { // (an Adaptive parity dump has no film: its records are written by k_ad_decide)
         const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
         const unsigned film_grid = std::min<unsigned>(rp.n_blocks, (unsigned)s->sm_count * 8);
@@ -804,11 +832,7 @@ trb_status query_passes(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb
     const bool stats = (flags & TRB_RENDER_STATS) != 0, anim = s->ds.has_anim != 0, occl = d_occ != nullptr;
     trb::RenderParams rp{};
     rp.stats = d_stats; rp.error_flag = s->d_error;
-    const unsigned resident = stats ? 4u : (anim ? 8u : 9u); // as for renders: two rounds of what is resident per SM
-    const unsigned tgrid = (unsigned)s->sm_count * (tu.trace_grid ? tu.trace_grid : 2u * resident);
     const uint32_t tflags = (flags & TRB_RENDER_REFERENCE_SHADOW) | (tu.exact_box ? trb::WF_TRACE_FORCE_EXACT_BOX : 0u);
-    const uint32_t sched = std::max(1u, tu.sched);
-    const uint32_t* no_sort = nullptr;
     for (size_t b = 0; b < n; b += want) {
         const size_t m = std::min<size_t>(want, n - b);
         trb::WfState wf = s->wf;
@@ -818,12 +842,7 @@ trb_status query_passes(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb
         else trb::k_query_load<false><<<lgrid, 256, 0, st>>>(wf, d_rays + b);
         g_launches++;
         launch_anim_table(s, wf, m, false, st);
-        // the default trace variant (trace.pipe 36: box_hit_finite + RayHome) with each ray's own [min_t, max_t]
-        if (anim) {
-            if (stats) trb::k_wf_trace<true, 4, 16, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
-            else trb::k_wf_trace<false, 8, 12, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
-        } else if (stats) trb::k_wf_trace<true, 4, 16, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
-        else trb::k_wf_trace<false, 9, 12, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, no_sort);
+        launch_query_trace(s, rp, wf, tflags, stats, nullptr, st);
         g_launches++;
         if (occl) trb::k_query_occluded<<<lgrid, 256, 0, st>>>(wf, d_occ + b);
         else {
@@ -837,25 +856,74 @@ trb_status query_passes(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb
     return TRB_OK;
 }
 
-// The blocking host-buffer form of a query: stage the rays, run the passes on the default stream, copy the results back.
-trb_status query_host(trb_scene* s, size_t n, const trb_query_ray* rays, trb_intersection* out, uint8_t* occluded, uint32_t flags, trb_stats* stats) {
+// Enqueue the illumination queries on st (DESIGN.md §5 "Illumination queries"). A pass holds whole rays, floor(pass paths / spp) of
+// them, so that k_illum_reduce finds all of a ray's samples in the pass; the path state grows as for renders, halving on OOM.
+// Path integrator: k_illum_load -> keyframed transform table -> the render's bounce rounds (wavefront_rounds, mode 2). Whitted
+// and NormalsDebug: k_simple_integrator<2> reads the caller's rays itself. Then k_illum_reduce writes each ray's mean.
+trb_status illum_passes(trb_scene* s, size_t n, const trb_illum_ray* d_rays, uint32_t spp, uint32_t seed, float* d_rgb, uint32_t flags,
+                        trb::DStats* d_stats, cudaStream_t st) {
+    uint64_t want = std::min<uint64_t>((uint64_t)n * spp, std::min<uint64_t>(std::max<uint64_t>(s->tune.pass_paths, 64), (1ull << 30) - 64));
+    want = ((std::max<uint64_t>(want, spp) + 63) / 64) * 64;
+    if (want > s->wf_capacity) {
+        trb_status r;
+        while ((r = ensure_wavefront(s, (size_t)want)) == TRB_OOM && want / 2 >= spp && want > (1u << 16)) want = ((want / 2 + 63) / 64) * 64;
+        if (r != TRB_OK) return r;
+    }
+    const size_t per = (size_t)(want / spp); // rays per pass
+    const bool anim = s->ds.has_anim != 0;
+    trb::RenderParams rp{}; // LD offset 0; no blocks: the MODE 2 kernels never call sample_id
+    rp.stats = d_stats; rp.error_flag = s->d_error; rp.seed = seed; rp.spp = spp;
+    for (size_t b = 0; b < n; b += per) {
+        const size_t m = std::min(per, n - b);
+        trb::WfState wf = s->wf;
+        wf.n_paths = (uint32_t)(m * spp);
+        wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
+        if (s->integrator.type != TRB_INTEGRATOR_PATH) {
+            const unsigned grid = (unsigned)std::min<size_t>((wf.n_paths + 127) / 128, (size_t)s->sm_count * 8);
+            if (anim) trb::k_simple_integrator<2, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);
+            else trb::k_simple_integrator<2, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);
+            g_launches++;
+        } else {
+            CU(cudaMemsetAsync(wf.counters, 0, 64 * trb::WF_CNT * sizeof(uint32_t), st));
+            const unsigned lgrid = (unsigned)std::min<size_t>((wf.n_paths + 255) / 256, (size_t)s->sm_count * 8);
+            trb::k_illum_load<<<lgrid, 256, 0, st>>>(wf, d_rays + b, spp, seed, d_stats);
+            g_launches++;
+            launch_anim_table(s, wf, wf.n_paths, false, st);
+            const trb_status r = wavefront_rounds(s, rp, wf, flags, 2, st);
+            if (r != TRB_OK) return r;
+        }
+        const unsigned rgrid = (unsigned)std::min<size_t>((m + 127) / 128, (size_t)s->sm_count * 16);
+        trb::k_illum_reduce<<<rgrid, 128, 0, st>>>(wf.rad, (uint32_t)m, spp, (flags & TRB_QUERY_CLAMP) ? 1u : 0u, d_rgb + 3 * b);
+        g_launches++;
+    }
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+trb_status illum_check(const trb_scene* s, size_t n, const void* rays, uint32_t spp, const void* rgb, uint32_t flags, bool device) {
+    if (spp == 0 || spp > 65536) return fail(TRB_INVALID_ARG, "spp must be in [1, 65536]");
+    if (device && n && (reinterpret_cast<uintptr_t>(rgb) & 3u)) return fail(TRB_INVALID_ARG, "the device rgb buffer must be 4-byte aligned");
+    return query_check(s, n, rays, rgb, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW | TRB_QUERY_CLAMP, device, false);
+}
+
+// The blocking host-buffer form of a query: stage the rays, run enqueue(d_rays, d_out) on the default stream, copy the results back.
+template <class Enqueue>
+trb_status query_host(trb_scene* s, size_t n, const void* rays, size_t ray_bytes, void* out, size_t out_bytes, trb_stats* stats, Enqueue enqueue) {
     if (n == 0) { if (stats) std::memset(stats, 0, sizeof *stats); return TRB_OK; }
     CU(cudaSetDevice(s->device));
-    const size_t out_bytes = out ? n * sizeof(trb_intersection) : n;
     void* d_rays = nullptr; void* d_res = nullptr;
-    CU(cudaMalloc(&d_rays, n * sizeof(trb_query_ray)));
+    CU(cudaMalloc(&d_rays, ray_bytes));
     cudaError_t e = cudaMalloc(&d_res, out_bytes);
     if (e != cudaSuccess) { cudaFree(d_rays); CU(e); }
-    e = cudaMemcpy(d_rays, rays, n * sizeof(trb_query_ray), cudaMemcpyHostToDevice);
+    e = cudaMemcpy(d_rays, rays, ray_bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0);
     trb_status r = TRB_OK;
     if (e == cudaSuccess) {
         cudaEventRecord(s->ev0, 0);
-        r = query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), out ? static_cast<trb_intersection*>(d_res) : nullptr,
-                         out ? nullptr : static_cast<uint8_t*>(d_res), flags, s->d_stats, 0);
+        r = enqueue(d_rays, d_res);
         cudaEventRecord(s->ev1, 0);
     }
-    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out ? static_cast<void*>(out) : static_cast<void*>(occluded), d_res, out_bytes, cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out, d_res, out_bytes, cudaMemcpyDeviceToHost);
     if (r != TRB_OK) cudaDeviceSynchronize(); // passes already enqueued still read the buffers
     cudaFree(d_rays); cudaFree(d_res);
     if (r != TRB_OK) return r;
@@ -946,7 +1014,10 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     std::unique_ptr<trb_scene> s(new trb_scene);
     s->device = device;
     tuning_from_env(s->tune);
-    if (d->integrator.type == TRB_INTEGRATOR_WHITTED) { // the reference's recursion is kept as device recursion: one frame per ray depth
+    // k_simple_integrator (Whitted and NormalsDebug) is recursive, so its stack is the context's limit, not a size ptxas computed: the
+    // reference's recursion is kept as device recursion (one frame per ray depth), and even NormalsDebug's one scene_trace call
+    // (kernel frame + scene_trace's, about 1.8 KB on sm_90a) needs more than CUDA's default 1 KB
+    if (d->integrator.type == TRB_INTEGRATOR_WHITTED || d->integrator.type == TRB_INTEGRATOR_NORMALS_DEBUG) {
         size_t have = 0;
         CU(cudaDeviceGetLimit(&have, cudaLimitStackSize));
         const size_t need = 4096 + (size_t)2048 * (d->integrator.max_depth + 2);
@@ -1622,7 +1693,9 @@ trb_status trb_intersect(trb_scene* s, size_t n, const trb_ray* rays, trb_hit* h
 
 trb_status trb_intersect_records(trb_scene* s, size_t n, const trb_query_ray* rays, trb_intersection* out, uint32_t flags, trb_stats* stats) {
     const trb_status r = query_check(s, n, rays, out, flags, TRB_RENDER_STATS, false, false);
-    return r != TRB_OK ? r : query_host(s, n, rays, out, nullptr, flags, stats);
+    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_query_ray), out, n * sizeof(trb_intersection), stats, [&](const void* d_rays, void* d_out) {
+        return query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), static_cast<trb_intersection*>(d_out), nullptr, flags, s->d_stats, 0);
+    });
 }
 
 trb_status trb_intersect_records_device(trb_scene* s, size_t n, const trb_query_ray* d_rays, trb_intersection* d_out, uint32_t flags,
@@ -1635,7 +1708,9 @@ trb_status trb_intersect_records_device(trb_scene* s, size_t n, const trb_query_
 
 trb_status trb_occluded(trb_scene* s, size_t n, const trb_query_ray* rays, uint8_t* occluded, uint32_t flags, trb_stats* stats) {
     const trb_status r = query_check(s, n, rays, occluded, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW, false, false);
-    return r != TRB_OK ? r : query_host(s, n, rays, nullptr, occluded, flags, stats);
+    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_query_ray), occluded, n, stats, [&](const void* d_rays, void* d_out) {
+        return query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), nullptr, static_cast<uint8_t*>(d_out), flags, s->d_stats, 0);
+    });
 }
 
 trb_status trb_occluded_device(trb_scene* s, size_t n, const trb_query_ray* d_rays, uint8_t* d_occluded, uint32_t flags, trb_stats* d_stats,
@@ -1644,6 +1719,21 @@ trb_status trb_occluded_device(trb_scene* s, size_t n, const trb_query_ray* d_ra
     if (r != TRB_OK || n == 0) return r;
     CU(cudaSetDevice(s->device));
     return query_passes(s, n, d_rays, nullptr, d_occluded, flags, reinterpret_cast<trb::DStats*>(d_stats), static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_illumination(trb_scene* s, size_t n, const trb_illum_ray* rays, uint32_t spp, uint32_t seed, float* rgb, uint32_t flags, trb_stats* stats) {
+    const trb_status r = illum_check(s, n, rays, spp, rgb, flags, false);
+    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_illum_ray), rgb, n * 3 * sizeof(float), stats, [&](const void* d_rays, void* d_rgb) {
+        return illum_passes(s, n, static_cast<const trb_illum_ray*>(d_rays), spp, seed, static_cast<float*>(d_rgb), flags, s->d_stats, 0);
+    });
+}
+
+trb_status trb_illumination_device(trb_scene* s, size_t n, const trb_illum_ray* d_rays, uint32_t spp, uint32_t seed, float* d_rgb, uint32_t flags,
+                                   trb_stats* d_stats, void* stream) {
+    const trb_status r = illum_check(s, n, d_rays, spp, d_rgb, flags, true);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return illum_passes(s, n, d_rays, spp, seed, d_rgb, flags, reinterpret_cast<trb::DStats*>(d_stats), static_cast<cudaStream_t>(stream));
 }
 
 trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {

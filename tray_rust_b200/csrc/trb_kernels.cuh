@@ -2216,8 +2216,10 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(const __grid_constant__ 
     }
 }
 
-// per-sample clamp (multithreaded.rs:99, Q12) and hand-over to the film (MODE 0) or the parity records (MODE 1)
+// per-sample clamp (multithreaded.rs:99, Q12) and hand-over to the film (MODE 0) or the parity records (MODE 1); MODE 2 (illumination
+// queries) keeps the integrator's unclamped radiance: k_illum_reduce clamps on request
 __device__ __forceinline__ void finish_sample(const DScene& sc, const RenderParams& rp, const WfState& wf, uint32_t p, f3 illum, int mode) {
+    if (mode == 2) { wf.rad[p] = make_float4(illum.x, illum.y, illum.z, 1.0f); return; }
     const f3 c = mk(clampf(illum.x, 0.0f, 1.0f), clampf(illum.y, 0.0f, 1.0f), clampf(illum.z, 0.0f, 1.0f)); // multithreaded.rs:99 (Q12)
     if (mode == 0) wf.rad[p] = make_float4(c.x, c.y, c.z, 1.0f);
     else {
@@ -2229,7 +2231,20 @@ __device__ __forceinline__ void finish_sample(const DScene& sc, const RenderPara
         out->x = sx; out->y = sy; out->r = c.x; out->g = c.y; out->b = c.z;
     }
 }
-// Shade round r (== bounce r of every live path). MODE 0: finished samples go to wf.rad; MODE 1: to trb_sample records.
+// Illumination queries (MODE 2 of the shade kernels): k_illum_load leaves each path's stream hash (seed, key, sample) in
+// wf.illum[p].w, which the shade kernels carry along instead of deriving it from sample_id, and min_t in wf.org[p].w, which
+// round 0 must not read as the path's WF_F_* flags.
+template <int MODE>
+__device__ __forceinline__ uint32_t wf_flags(float4 o4, uint32_t round) { return (MODE == 2 && round == 0) ? 0u : __float_as_uint(o4.w); }
+template <int MODE>
+__device__ __forceinline__ uint32_t wf_stream(const DScene& sc, const RenderParams& rp, const WfState& wf, uint32_t p) {
+    if (MODE == 2) return __float_as_uint(wf.illum[p].w);
+    const SampleId id = sample_id(sc, rp, p);
+    return rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
+}
+
+// Shade round r (== bounce r of every live path). MODE 0: finished samples go to wf.rad; MODE 1: to trb_sample records;
+// MODE 2: illumination queries, unclamped to wf.rad.
 template <int MODE, bool ANIM, int MINB>
 __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
                                                    uint32_t round) {
@@ -2282,7 +2297,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ 
         if (valid) {
             p = round == 0 ? i : act[i];
             const float4 o4 = wf.org[p];
-            const uint32_t fl = __float_as_uint(o4.w);
+            const uint32_t fl = wf_flags<MODE>(o4, round);
             const f3 org = mk(o4.x, o4.y, o4.z);
             float4 il4 = wf.illum[p];
             f3 illum = mk(il4.x, il4.y, il4.z);
@@ -2313,8 +2328,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ 
                     f3 first_ng;
                     if (round == 0) { first_ng = s.ng; wf.ng[p] = make_float4(s.ng.x, s.ng.y, s.ng.z, 0.0f); }
                     else { const float4 n4 = wf.ng[p]; first_ng = mk(n4.x, n4.y, n4.z); }
-                    const SampleId id = sample_id(sc, rp, p);
-                    const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
+                    const uint32_t hs = MODE == 2 ? __float_as_uint(il4.w) : wf_stream<MODE>(sc, rp, wf, p);
                     BounceOut o;
                     shade_bounce<ANIM>(sc, s, h.inst, ray.d, first_ng, round, (fl & WF_F_SPECULAR) != 0, hs, mk(th4.x, th4.y, th4.z), time, illum, o, xf_row, rp.ld_offset);
                     const uint32_t nf = (o.specular ? WF_F_SPECULAR : 0u) | (o.terminate ? WF_F_TERMINATE : 0u) | (o.ds.has_shadow ? WF_F_SHADOW : 0u) |
@@ -2332,11 +2346,12 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ 
                         wf.b[p] = make_float4(o.ds.b.x, o.ds.b.y, o.ds.b.z, __uint_as_float(o.light));
                         wf.tprev[p] = make_float4(o.t_before.x, o.t_before.y, o.t_before.z, 0.0f);
                         wf.thr[p] = make_float4(o.throughput.x, o.throughput.y, o.throughput.z, time);
-                        wf.illum[p] = make_float4(illum.x, illum.y, illum.z, 0.0f);
+                        wf.illum[p] = make_float4(illum.x, illum.y, illum.z, MODE == 2 ? il4.w : 0.0f);
                     } else done = true; // nothing pending: direct light of this bounce is zero, the path ends here
                 }
             }
-            if (done) { // per-sample clamp (multithreaded.rs:99, Q12) and hand-over to the film
+            if (done && MODE == 2) finish_sample(sc, rp, wf, p, illum, MODE);
+            else if (done) { // per-sample clamp (multithreaded.rs:99, Q12) and hand-over to the film
                 const f3 c = mk(clampf(illum.x, 0.0f, 1.0f), clampf(illum.y, 0.0f, 1.0f), clampf(illum.z, 0.0f, 1.0f));
                 if (MODE == 0) wf.rad[p] = make_float4(c.x, c.y, c.z, 1.0f);
                 else {
@@ -2457,20 +2472,31 @@ __device__ f3 whitted_illum(const DScene& sc, const Ray& ray, uint32_t depth, co
 }
 
 // One camera sample per thread for the Whitted / NormalsDebug integrators; radiance to wf.rad (MODE 0, then the film kernel) or to trb_sample records (MODE 1).
+// MODE 2 (illumination queries): path p is sample p % rp.spp of the caller's ray rays[p / rp.spp], whose key and sample index key the
+// streams; the unclamped radiance goes to rad[p] (then k_illum_reduce).
 template <int MODE, bool ANIM>
 __global__ void __launch_bounds__(128) k_simple_integrator(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, float4* rad, uint32_t n_paths,
-                                                           uint32_t integrator, uint32_t flags) {
+                                                           uint32_t integrator, uint32_t flags, const trb_illum_ray* __restrict__ rays) {
     RayCounts rc = {0, 0, 0, 0};
     Cnt cnt = {0, 0, 0};
     uint32_t mine = 0;
     for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n_paths; p += gridDim.x * blockDim.x) {
-        const SampleId id = sample_id(sc, rp, p);
-        const PixelStreams ps = pixel_streams(rp.seed, id.pixel);
-        const uint32_t hpix = ps.hpix;
-        float sx, sy, tm;
-        sample_position(rp, ps, id, sx, sy, tm);
         Ray ray;
-        const float time = camera_ray<ANIM>(sc, sx, sy, tm, ray);
+        float time, sx = 0.0f, sy = 0.0f;
+        uint32_t hpix, si;
+        if (MODE == 2) {
+            const trb_illum_ray& q = rays[p / rp.spp];
+            ray.o = mk(q.o[0], q.o[1], q.o[2]); ray.d = mk(q.d[0], q.d[1], q.d[2]); ray.tmin = q.min_t; ray.tmax = q.max_t;
+            time = q.time;
+            hpix = rng_absorb(rng_seed(rp.seed), q.key); si = q.sample + p % rp.spp;
+        } else {
+            const SampleId id = sample_id(sc, rp, p);
+            const PixelStreams ps = pixel_streams(rp.seed, id.pixel);
+            hpix = ps.hpix; si = id.si;
+            float tm;
+            sample_position(rp, ps, id, sx, sy, tm);
+            time = camera_ray<ANIM>(sc, sx, sy, tm, ray);
+        }
         mine++; rc.primary++;
         HitRec hit;
         f3 c = splat(0.0f);
@@ -2481,8 +2507,9 @@ __global__ void __launch_bounds__(128) k_simple_integrator(const __grid_constant
                 Frame fr;
                 make_frame(s, fr);
                 c = (fr.n + splat(1.0f)) / 2.0f;
-            } else c = whitted_illum<ANIM>(sc, ray, 0, hit, 1, rng_absorb(hpix, id.si), time, (flags & 4u) != 0, rc, cnt, rp.error_flag);
+            } else c = whitted_illum<ANIM>(sc, ray, 0, hit, 1, rng_absorb(hpix, si), time, (flags & 4u) != 0, rc, cnt, rp.error_flag);
         }
+        if (MODE == 2) { rad[p] = make_float4(c.x, c.y, c.z, 1.0f); continue; }
         c = mk(clampf(c.x, 0.0f, 1.0f), clampf(c.y, 0.0f, 1.0f), clampf(c.z, 0.0f, 1.0f)); // multithreaded.rs:99 (Q12)
         if (MODE == 0) rad[p] = make_float4(c.x, c.y, c.z, 1.0f);
         else { trb_sample* out = reinterpret_cast<trb_sample*>(rp.samples_out) + p; out->x = sx; out->y = sy; out->r = c.x; out->g = c.y; out->b = c.z; }
@@ -2523,7 +2550,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
         if (i < n) {
             p = round == 0 ? i : act[i];
             const float4 o4 = wf.org[p];
-            const uint32_t fl = __float_as_uint(o4.w);
+            const uint32_t fl = wf_flags<MODE>(o4, round);
             const f3 org = mk(o4.x, o4.y, o4.z);
             const float4 il4 = wf.illum[p];
             f3 illum = mk(il4.x, il4.y, il4.z);
@@ -2561,7 +2588,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
                     wf.f_n[p] = make_float4(fr.n.x, fr.n.y, fr.n.z, s.u); // .w: the hit's (u, v) for image textures
                     wf.f_t[p] = make_float4(fr.tan.x, fr.tan.y, fr.tan.z, s.v);
                     wf.f_b[p] = make_float4(fr.bitan.x, fr.bitan.y, fr.bitan.z, 0.0f);
-                    wf.illum[p] = make_float4(illum.x, illum.y, illum.z, 0.0f);
+                    wf.illum[p] = make_float4(illum.x, illum.y, illum.z, MODE == 2 ? il4.w : 0.0f);
                     push_mid = true;
                     if (wf.mid_keyed) mid_key = __ldg(&sc.materials[__ldg(&sc.instances[h.inst].material)].type) & (WF_MID_BUCKETS - 1u);
                 }
@@ -2573,8 +2600,9 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
 }
 
 // KIND >= 0: the instantiation compiled for that material kind alone; it drains that kind's bucket. KIND = -1: any kind; drains the
-// buckets of `bucket_mask` (the kinds the scene uses that have no instantiation of their own).
-template <bool ANIM, int MINB, int KIND = -1>
+// buckets of `bucket_mask` (the kinds the scene uses that have no instantiation of their own). MODE 2: illumination queries (the
+// stream hash the path carries); the renders' modes 0 and 1 shade alike and share MODE 0.
+template <bool ANIM, int MINB, int KIND = -1, int MODE = 0>
 __global__ void __launch_bounds__(128, MINB) k_wf_shade_b(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
                                                      uint32_t round, uint32_t bucket_mask) {
     uint32_t* cnt_r = wf.counters + round * WF_CNT;
@@ -2601,8 +2629,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_b(const __grid_constant_
             const f3 wo = -mk(c4.x, c4.y, c4.z);
             Mat m;
             load_mat_at(sc, __ldg(&sc.instances[inst].material), tu, tv, th4.w, m);
-            const SampleId id = sample_id(sc, rp, p);
-            const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
+            const uint32_t hs = wf_stream<MODE>(sc, rp, wf, p);
             DirectSetup ds; uint32_t light;
             bounce_direct<ANIM, KIND>(sc, m, fr, wo, round, hs, th4.w, ds, light, wf_xf_row<ANIM>(wf, p), rp.ld_offset);
             push_shadow = ds.has_shadow; push_mis = ds.has_mis;
@@ -2648,8 +2675,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
             const f3 wo = -mk(c4.x, c4.y, c4.z);
             Mat m;
             load_mat_at(sc, __ldg(&sc.instances[inst].material), tu, tv, th4.w, m);
-            const SampleId id = sample_id(sc, rp, p);
-            const uint32_t hs = rng_absorb(rng_absorb(rng_seed(rp.seed), id.pixel), id.si);
+            const uint32_t hs = wf_stream<MODE>(sc, rp, wf, p);
             ScatterOut so;
             bounce_scatter<KIND>(sc, m, fr, wo, round, hs, mk(th4.x, th4.y, th4.z), so, rp.ld_offset);
             const uint32_t fb = __float_as_uint(wf.org[p].w); // WF_F_SHADOW | WF_F_MIS from k_wf_shade_b
@@ -2877,6 +2903,51 @@ __global__ void __launch_bounds__(128) k_query_records(const __grid_constant__ D
 }
 __global__ void __launch_bounds__(256) k_query_occluded(const __grid_constant__ WfState wf, uint8_t* __restrict__ out) {
     for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < wf.n_paths; p += gridDim.x * blockDim.x) out[p] = __float_as_uint(wf.shadow[p].w) != 0u ? 1 : 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// Illumination queries (trb_illumination): Integrator::illumination along caller rays on the render's wavefront. Path p of a pass
+// is sample j = p % spp of ray i = p / spp. k_illum_load writes it as a round-0 path the way k_wf_generate writes a camera sample:
+// the ray with its [min_t, max_t] as PIPE bit 64 of k_wf_trace reads them (min_t in org.w: the MODE 2 shade kernels do not take
+// it for flags), throughput (1, 1, 1, time), and in illum.w the hash of the camera-sample stream (seed, key, sample + j) that
+// the render derives from (seed, pixel, si). The bounce rounds then run the render's trace and MODE 2 shade kernels, which
+// leave each sample's unclamped radiance in wf.rad; k_illum_reduce averages each ray's spp samples.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_illum_load(const __grid_constant__ WfState wf, const trb_illum_ray* __restrict__ rays, uint32_t spp, uint32_t seed,
+                                                    DStats* stats) {
+    const uint32_t n = wf.n_paths, hseed = rng_seed(seed);
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const float4* r = reinterpret_cast<const float4*>(rays + p / spp); // (o, d.x) (d.yz, min_t, max_t) (time, key, sample, pad)
+        const float4 a = __ldg(r), b = __ldg(r + 1), c = __ldg(r + 2);
+        const uint32_t hs = rng_absorb(rng_absorb(hseed, __float_as_uint(c.y)), __float_as_uint(c.z) + p % spp);
+        wf.org[p] = make_float4(a.x, a.y, a.z, b.z);
+        wf.cont[p] = make_float4(a.w, b.x, b.y, b.w);
+        wf.thr[p] = make_float4(1.0f, 1.0f, 1.0f, c.x);
+        wf.illum[p] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(hs));
+        wf.q_cont[p] = p;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) { // as k_wf_generate: the host zeroed every round's counters
+        wf.counters[WF_N_ACTIVE] = n; wf.counters[WF_N_CONT] = n;
+        if (stats) atomicAdd(&stats->camera_samples, (unsigned long long)n);
+    }
+    if (blockIdx.x == 0 && threadIdx.x < 64) {
+        uint32_t* b = wf.bounds + threadIdx.x * 8;
+        b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
+    }
+}
+// rgb[3i + c] = (sum over j in order of sample j's radiance, each clamped to [0, 1] first if asked) / spp
+__global__ void __launch_bounds__(128) k_illum_reduce(const float4* __restrict__ rad, uint32_t n_rays, uint32_t spp, uint32_t clamp, float* __restrict__ rgb) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_rays; i += gridDim.x * blockDim.x) {
+        const float4* r = rad + (size_t)i * spp;
+        f3 sum = splat(0.0f);
+        for (uint32_t j = 0; j < spp; ++j) {
+            const float4 v = r[j];
+            const f3 c = clamp ? mk(clampf(v.x, 0.0f, 1.0f), clampf(v.y, 0.0f, 1.0f), clampf(v.z, 0.0f, 1.0f)) : mk(v.x, v.y, v.z);
+            sum = j == 0 ? c : sum + c; // starts at sample 0, not at 0.0f: one sample returns its own bits, -0.0 included
+        }
+        const float k = (float)spp;
+        rgb[3 * (size_t)i] = sum.x / k; rgb[3 * (size_t)i + 1] = sum.y / k; rgb[3 * (size_t)i + 2] = sum.z / k;
+    }
 }
 
 // ------------------------------------------------------------------------------------------
