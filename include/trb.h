@@ -469,6 +469,125 @@ trb_status trb_illumination(trb_scene* scene, size_t n, const trb_illum_ray* ray
 trb_status trb_illumination_device(trb_scene* scene, size_t n, const trb_illum_ray* d_rays, uint32_t spp, uint32_t seed, float* d_rgb,
                                    uint32_t flags, trb_stats* d_stats, void* cuda_stream);
 
+/* -- shading queries: the render's BSDF and light functions on caller inputs ---------------------------------------------
+ * Material::bsdf with BSDF::eval / pdf / sample, Light::sample_incident / pdf and Emitter::radiance (bsdf.rs:66-125, light/mod.rs:43-53,
+ * emitter.rs:140-204) for batches of queries, on the device code the renders run, so they return the render's bits. They trace
+ * nothing: a caller composes them with trb_intersect_records and trb_occluded into an integrator of its own.
+ *
+ * A BSDF query i builds Material::bsdf at record rec[i] (a trb_intersection as trb_intersect_records returns it, or filled in by the
+ * caller): material rec.material, textures sampled at (rec.u, rec.v, rec.time), shading frame from rec.n and rec.dp_du (bsdf.rs:38-44);
+ * no other field is read. `bxdf` is the EnumSet<BxDFType> of the call (bxdf/mod.rs:37-41), TRB_BXDF_ALL for every lobe.
+ * A light query names its light by instance index (trb_scene_lights lists them in light order); its transform and emission are
+ * evaluated at the query's time.
+ *
+ * Out-of-range inputs are not errors: the query writes an all-zero output and reads nothing out of bounds. That is a record with
+ * inst == TRB_MISS or material >= the scene's material count, a light or inst >= the instance count, and a light that is not an
+ * emitter.
+ * Statuses: TRB_INVALID_ARG for null arguments with n > 0 and for unaligned device buffers; n == 0 is TRB_OK. The light queries read the
+ * instance matrices of trb_scene_update_frame and return TRB_INVALID_ARG before the first one; the BSDF queries and trb_emitted work
+ * right after scene creation. The host forms take host buffers and block. The _device forms take device buffers on the scene's GPU
+ * (queries, records and 16-byte outputs 16-byte aligned, float outputs 4-byte aligned) and enqueue one kernel on cuda_stream (a
+ * cudaStream_t; NULL = default stream) without host synchronisation, under trb_render_device's one-stream-per-scene rule. */
+enum { /* bxdf::BxDFType (bxdf/mod.rs:37-41) */
+    TRB_BXDF_REFLECTION = 1u,
+    TRB_BXDF_TRANSMISSION = 2u,
+    TRB_BXDF_DIFFUSE = 4u,
+    TRB_BXDF_GLOSSY = 8u,
+    TRB_BXDF_SPECULAR = 16u,
+    TRB_BXDF_ALL = 31u
+};
+
+/* BSDF::eval / pdf arguments: w_o, the lobe set, w_i (world space, used as given). 32 bytes; pad is ignored. */
+typedef struct trb_bsdf_eval_query {
+    float wo[3];
+    uint32_t bxdf;
+    float wi[3];
+    uint32_t pad;
+} trb_bsdf_eval_query;
+
+/* BSDF::sample arguments: w_o, the lobe set and Sample { two_d: u, one_d: u_comp } (u_comp chooses the lobe). 32 bytes. */
+typedef struct trb_bsdf_sample_query {
+    float wo[3];
+    uint32_t bxdf;
+    float u[2];
+    float u_comp;
+    uint32_t pad;
+} trb_bsdf_sample_query;
+
+/* BSDF::sample's (f, w_i, pdf, sampled type) (bsdf.rs:85-111); sampled = the chosen lobe's type bits, 0 when nothing was sampled.
+ * 32 bytes. */
+typedef struct trb_bsdf_sample_result {
+    float f[3];
+    float pdf;
+    float wi[3];
+    uint32_t sampled;
+} trb_bsdf_sample_result;
+
+/* Light::sample_incident arguments: the receiving point, the time, the 2-D sample and the light's instance index. 32 bytes. */
+typedef struct trb_light_query {
+    float p[3];
+    float time;
+    float u[2];
+    uint32_t light;
+    uint32_t pad;
+} trb_light_query;
+
+/* Light::sample_incident's (Li, w_i, pdf, OcclusionTester) (emitter.rs:164-190) and delta_light() (1 for point lights). shadow is the
+ * OcclusionTester as a ray: test_points(p, p_light, time) = Ray::segment(p, p_light - p, 0.001, 0.999, time) (light/mod.rs:21-23), ready
+ * for trb_occluded. 80 bytes. */
+typedef struct trb_light_sample_result {
+    float li[3];
+    float pdf;
+    float wi[3];
+    uint32_t delta;
+    trb_query_ray shadow;
+} trb_light_sample_result;
+
+/* Light::pdf arguments: p, time, w_i, the light's instance index. 32 bytes. */
+typedef struct trb_light_pdf_query {
+    float p[3];
+    float time;
+    float wi[3];
+    uint32_t light;
+} trb_light_pdf_query;
+
+/* Emitter::radiance arguments: the outgoing direction w, time, the surface normal n, the instance index. 32 bytes. */
+typedef struct trb_emit_query {
+    float w[3];
+    float time;
+    float n[3];
+    uint32_t inst;
+} trb_emit_query;
+
+/* out4[4i .. 4i+3] = BSDF::eval(wo, wi, bxdf) r, g, b, then BSDF::pdf(wo, wi, bxdf), of Material::bsdf at rec[i]. */
+trb_status trb_bsdf_eval(trb_scene* scene, size_t n, const trb_intersection* rec, const trb_bsdf_eval_query* q, float* out4);
+trb_status trb_bsdf_eval_device(trb_scene* scene, size_t n, const trb_intersection* d_rec, const trb_bsdf_eval_query* d_q, float* d_out4,
+                                void* cuda_stream);
+
+/* out[i] = BSDF::sample(wo, bxdf, (u, u_comp)) of Material::bsdf at rec[i]. */
+trb_status trb_bsdf_sample(trb_scene* scene, size_t n, const trb_intersection* rec, const trb_bsdf_sample_query* q, trb_bsdf_sample_result* out);
+trb_status trb_bsdf_sample_device(trb_scene* scene, size_t n, const trb_intersection* d_rec, const trb_bsdf_sample_query* d_q,
+                                  trb_bsdf_sample_result* d_out, void* cuda_stream);
+
+/* out[i] = Light::sample_incident(p, u, time) of instance q[i].light. */
+trb_status trb_light_sample(trb_scene* scene, size_t n, const trb_light_query* q, trb_light_sample_result* out);
+trb_status trb_light_sample_device(trb_scene* scene, size_t n, const trb_light_query* d_q, trb_light_sample_result* d_out, void* cuda_stream);
+
+/* pdf[i] = Light::pdf(p, wi, time) of instance q[i].light (emitter.rs:193-203): 0 for point lights and for directions that miss the
+ * light's shape. */
+trb_status trb_light_pdf(trb_scene* scene, size_t n, const trb_light_pdf_query* q, float* pdf);
+trb_status trb_light_pdf_device(trb_scene* scene, size_t n, const trb_light_pdf_query* d_q, float* d_pdf, void* cuda_stream);
+
+/* rgb[3i .. 3i+2] = Emitter::radiance(w, _, n, time) of instance q[i].inst (its emission when dot(w, n) > 0, else black); black when the
+ * instance is a receiver. This is the emitted term of Path::illumination (path.rs:71-74) and of the MIS ray (integrator/mod.rs:156-162);
+ * the caller chooses the normal. */
+trb_status trb_emitted(trb_scene* scene, size_t n, const trb_emit_query* q, float* rgb);
+trb_status trb_emitted_device(trb_scene* scene, size_t n, const trb_emit_query* d_q, float* d_rgb, void* cuda_stream);
+
+/* The light list of sample_one_light (integrator/mod.rs:106-111): the instance indices of the emitters in object order (Q20),
+ * n_lights of them (trb_scene_info). Host buffer; no device work. */
+trb_status trb_scene_lights(const trb_scene* scene, uint32_t* inst);
+
 /* ≙ LowDiscrepancy::get_samples + get_samples_1d + Camera::generate_ray
  * (ld.rs:33-64, camera.rs:150-157) for the selected blocks/samples: writes one ray and
  * one film position per camera sample, in block-list order, pixel row-major within the

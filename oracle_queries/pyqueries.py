@@ -2,7 +2,8 @@
 TEST INFRASTRUCTURE, like oracle/pyoracle.py.
 
 ``QueryOracleScene`` is an ``OracleScene`` backed by that library (the detmath oracle with the ray queries added), so it has
-every oracle method plus ``intersect_records``, ``occluded`` and ``illumination`` with the signatures of ``tray_rust_b200.api.Scene``.
+every oracle method plus ``intersect_records``, ``occluded``, ``illumination`` and the shading queries ``bsdf_eval``, ``bsdf_sample``,
+``light_sample``, ``light_pdf``, ``emitted`` and ``lights`` with the signatures of ``tray_rust_b200.api.Scene``.
 """
 import ctypes as C
 
@@ -19,6 +20,11 @@ def load():
         lib.orc_intersect_records.argtypes = [vp, sz, vp, vp, C.POINTER(F.Stats)]
         lib.orc_occluded.argtypes = [vp, sz, vp, vp, C.POINTER(F.Stats)]
         lib.orc_illumination.argtypes = [vp, sz, vp, C.c_uint32, C.c_uint32, vp, C.c_uint32, C.POINTER(F.Stats)]
+        for name in ("orc_bsdf_eval", "orc_bsdf_sample"):
+            getattr(lib, name).argtypes = [vp, sz, vp, vp, vp]
+        for name in ("orc_light_sample", "orc_light_pdf", "orc_emitted"):
+            getattr(lib, name).argtypes = [vp, sz, vp, vp]
+        lib.orc_scene_lights.argtypes = [vp, vp]
         lib._queries_ready = True
     return lib
 
@@ -54,4 +60,43 @@ class QueryOracleScene(O.OracleScene):
         out = np.zeros((len(rays), 3), np.float32)
         st = stats if stats is not None else F.Stats()
         self._check(self._lib.orc_illumination(self._h, len(rays), F.ptr(rays), spp, seed, F.ptr(out), 1 if clamp else 0, C.byref(st)))
+        return out
+
+    def bsdf_eval(self, records, queries):
+        rec = np.ascontiguousarray(records, dtype=F.INTERSECTION_DTYPE)
+        q = np.ascontiguousarray(queries, dtype=F.BSDF_EVAL_QUERY_DTYPE)
+        out = np.zeros((len(q), 4), np.float32)
+        self._check(self._lib.orc_bsdf_eval(self._h, len(q), F.ptr(rec), F.ptr(q), F.ptr(out)))
+        return out
+
+    def bsdf_sample(self, records, queries):
+        rec = np.ascontiguousarray(records, dtype=F.INTERSECTION_DTYPE)
+        q = np.ascontiguousarray(queries, dtype=F.BSDF_SAMPLE_QUERY_DTYPE)
+        out = np.zeros(len(q), F.BSDF_SAMPLE_DTYPE)
+        self._check(self._lib.orc_bsdf_sample(self._h, len(q), F.ptr(rec), F.ptr(q), F.ptr(out)))
+        return out
+
+    def light_sample(self, queries):
+        q = np.ascontiguousarray(queries, dtype=F.LIGHT_QUERY_DTYPE)
+        out = np.zeros(len(q), F.LIGHT_SAMPLE_DTYPE)
+        self._check(self._lib.orc_light_sample(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def light_pdf(self, queries):
+        q = np.ascontiguousarray(queries, dtype=F.LIGHT_PDF_QUERY_DTYPE)
+        out = np.zeros(len(q), np.float32)
+        self._check(self._lib.orc_light_pdf(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def emitted(self, queries):
+        q = np.ascontiguousarray(queries, dtype=F.EMIT_QUERY_DTYPE)
+        out = np.zeros((len(q), 3), np.float32)
+        self._check(self._lib.orc_emitted(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def lights(self):
+        """the light list of sample_one_light (instance indices, object order)"""
+        n = sum(1 for i in range(self._desc.n_instances) if self._desc.instances[i].kind != F.INST_RECEIVER)
+        out = np.zeros(n, np.uint32)
+        self._check(self._lib.orc_scene_lights(self._h, F.ptr(out)))
         return out

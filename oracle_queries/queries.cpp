@@ -9,6 +9,12 @@
  *   orc_illumination       thread_work's per-sample body (multithreaded.rs:95-103) along caller rays: Scene::intersect, then the
  *                          scene integrator's Integrator::illumination with the camera-sample stream (seed, key, sample + j)
  * Each ray is Ray::segment(o, d, min_t, max_t, time) and is traced against the TLAS of the current frame.
+ * and the shading half of that interface, which traces nothing:
+ *   orc_bsdf_eval / orc_bsdf_sample   Material::bsdf at a DifferentialGeometry built from a record's fields, then BSDF::eval and pdf,
+ *                                     or BSDF::sample (bsdf.rs:66-125)
+ *   orc_light_sample / orc_light_pdf  SceneShade::sample_incident and light_pdf (emitter.rs:164-204)
+ *   orc_emitted                       SceneShade::radiance (emitter.rs:140-142)
+ *   orc_scene_lights                  the light list of sample_one_light
  */
 #include "../oracle/oracle.cpp"
 
@@ -105,6 +111,88 @@ int orc_illumination(orc_scene* s, size_t n, const trb_illum_ray* rays, uint32_t
         stats->rays_primary = total.rays[0]; stats->rays_shadow = total.rays[1]; stats->rays_mis = total.rays[2]; stats->rays_continuation = total.rays[3];
         stats->node_tests = total.node_tests; stats->tri_tests = total.tri_tests; stats->inst_tests = total.inst_tests;
     }
+    return TRB_OK;
+}
+
+/* ---- shading queries: Material::bsdf with BSDF::eval / pdf / sample at a record, Light::sample_incident / pdf, Emitter::radiance.
+ * Out-of-range indices (a missed record, material, light or instance past the scene's, a light that is not an emitter) give zeros. */
+static bool record_bsdf(const orc_scene* s, const trb_intersection& r, BSDF& bsdf) {
+    if (r.inst == TRB_MISS || r.material >= s->shade.materials.size()) return false;
+    DG dg;
+    dg.p = V3(r.p[0], r.p[1], r.p[2]); dg.n = V3(r.n[0], r.n[1], r.n[2]); dg.ng = V3(r.ng[0], r.ng[1], r.ng[2]);
+    dg.u = r.u; dg.v = r.v; dg.time = r.time;
+    dg.dp_du = V3(r.dp_du[0], r.dp_du[1], r.dp_du[2]); dg.dp_dv = V3(r.dp_dv[0], r.dp_dv[1], r.dp_dv[2]);
+    s->shade.materials[r.material].bsdf(dg, bsdf);
+    return true;
+}
+static bool is_light(const orc_scene* s, uint32_t li) { return li < s->geom.instances.size() && s->geom.instances[li].is_emitter(); }
+
+int orc_bsdf_eval(orc_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_eval_query* q, float* out4) {
+#pragma omp parallel for schedule(dynamic, 1024)
+    for (long i = 0; i < (long)n; ++i) {
+        float* o = out4 + 4 * i;
+        o[0] = o[1] = o[2] = o[3] = 0.0f;
+        BSDF bsdf;
+        if (!record_bsdf(s, rec[i], bsdf)) continue;
+        const V3 wo(q[i].wo[0], q[i].wo[1], q[i].wo[2]), wi(q[i].wi[0], q[i].wi[1], q[i].wi[2]);
+        const Col f = bsdf.eval(wo, wi, q[i].bxdf);
+        o[0] = f.r; o[1] = f.g; o[2] = f.b; o[3] = bsdf.pdf(wo, wi, q[i].bxdf);
+    }
+    return TRB_OK;
+}
+
+int orc_bsdf_sample(orc_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_sample_query* q, trb_bsdf_sample_result* out) {
+#pragma omp parallel for schedule(dynamic, 1024)
+    for (long i = 0; i < (long)n; ++i) {
+        trb_bsdf_sample_result& o = out[i];
+        memset(&o, 0, sizeof o);
+        BSDF bsdf;
+        if (!record_bsdf(s, rec[i], bsdf)) continue;
+        Col f; V3 wi; float pdf; uint32_t sampled;
+        bsdf.sample(V3(q[i].wo[0], q[i].wo[1], q[i].wo[2]), q[i].bxdf, q[i].u[0], q[i].u[1], q[i].u_comp, f, wi, pdf, sampled);
+        o.f[0] = f.r; o.f[1] = f.g; o.f[2] = f.b; o.pdf = pdf; put3(o.wi, wi); o.sampled = sampled;
+    }
+    return TRB_OK;
+}
+
+int orc_light_sample(orc_scene* s, size_t n, const trb_light_query* q, trb_light_sample_result* out) {
+    if (s->active_camera < 0) { g_err = "update_frame must be called before rendering"; return TRB_INVALID_ARG; }
+#pragma omp parallel for schedule(dynamic, 1024)
+    for (long i = 0; i < (long)n; ++i) {
+        trb_light_sample_result& o = out[i];
+        memset(&o, 0, sizeof o);
+        if (!is_light(s, q[i].light)) continue;
+        Col li; V3 wi; float pdf; Ray occl;
+        s->shade.sample_incident(q[i].light, V3(q[i].p[0], q[i].p[1], q[i].p[2]), q[i].u[0], q[i].u[1], q[i].time, li, wi, pdf, occl);
+        o.li[0] = li.r; o.li[1] = li.g; o.li[2] = li.b; o.pdf = pdf; put3(o.wi, wi);
+        o.delta = s->geom.instances[q[i].light].kind == TRB_INST_EMITTER_POINT ? 1u : 0u;
+        put3(o.shadow.o, occl.o); put3(o.shadow.d, occl.d);
+        o.shadow.min_t = occl.min_t; o.shadow.max_t = occl.max_t; o.shadow.time = occl.time;
+    }
+    return TRB_OK;
+}
+
+int orc_light_pdf(orc_scene* s, size_t n, const trb_light_pdf_query* q, float* pdf) {
+    if (s->active_camera < 0) { g_err = "update_frame must be called before rendering"; return TRB_INVALID_ARG; }
+#pragma omp parallel for schedule(dynamic, 1024)
+    for (long i = 0; i < (long)n; ++i)
+        pdf[i] = is_light(s, q[i].light) ? s->shade.light_pdf(q[i].light, V3(q[i].p[0], q[i].p[1], q[i].p[2]), V3(q[i].wi[0], q[i].wi[1], q[i].wi[2]), q[i].time) : 0.0f;
+    return TRB_OK;
+}
+
+int orc_emitted(orc_scene* s, size_t n, const trb_emit_query* q, float* rgb) {
+#pragma omp parallel for schedule(dynamic, 1024)
+    for (long i = 0; i < (long)n; ++i) {
+        Col c(0.0f);
+        if (is_light(s, q[i].inst)) c = s->shade.radiance(s->geom.instances[q[i].inst], V3(q[i].w[0], q[i].w[1], q[i].w[2]), V3(q[i].n[0], q[i].n[1], q[i].n[2]), q[i].time);
+        rgb[3 * i] = c.r; rgb[3 * i + 1] = c.g; rgb[3 * i + 2] = c.b;
+    }
+    return TRB_OK;
+}
+
+/* the light list of sample_one_light: instance indices of the emitters in object order */
+int orc_scene_lights(const orc_scene* s, uint32_t* inst) {
+    for (size_t k = 0; k < s->shade.lights.size(); ++k) inst[k] = s->shade.lights[k];
     return TRB_OK;
 }
 

@@ -12,6 +12,10 @@ trb_illumination takes the --width x --height camera rays of C4 at 1 spp (trb_ca
 camera samples trb_render_device renders at 1 spp with the same seed, so the two compute the same radiance and differ in what
 they start from (caller rays vs. the camera) and end with (per-ray means vs. the film). Both report camera samples/s and Mrays/s
 over every traced ray (primary, shadow, MIS, continuation).
+
+Last, the five shading queries (trb_bsdf_eval, trb_bsdf_sample, trb_light_sample, trb_light_pdf, trb_emitted; device forms) on the
+records of those camera rays and on --rays synthetic records on the material zoo: Mqueries/s and the GB/s of the query, record and
+output bytes, with their share of the H100 SXM's 3.35 TB/s HBM3 peak.
 """
 import argparse
 import json
@@ -95,6 +99,7 @@ def main():
         print("  %-40s %8.3f ms  %8.1f Mrays/s" % (name, res["ms"][name], res["mrays_per_s"][name]))
     print("  hit fraction %.3f, records equal trb_intersect's (t, inst): %s" % (res["hit_fraction"], res["records_match_trb_intersect"]))
     illumination_vs_render(a, res)
+    shading_queries(a, res)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         json.dump(res, open(a.out, "w"), indent=1)
@@ -149,6 +154,115 @@ def illumination_vs_render(a, res):
     for name in cases:
         r = res["illumination"]
         print("  %-40s %8.3f ms  %8.2f M samples/s  %8.1f Mrays/s" % (name, r["ms"][name], r["samples_per_s"][name] / 1e6, r["mrays_per_s"][name]))
+
+
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet, HBM3
+# bytes each query moves: its query, its record (BSDF queries) and its output
+SHADING_BYTES = {"trb_bsdf_eval": 32 + 96 + 16, "trb_bsdf_sample": 32 + 96 + 32, "trb_light_sample": 32 + 80, "trb_light_pdf": 32 + 4,
+                 "trb_emitted": 32 + 12}
+
+
+def _unit(v):
+    return (v / np.linalg.norm(v, axis=1, keepdims=True)).astype(np.float32)
+
+
+def shading_inputs(g, rec, d, rng):
+    """the five queries' inputs at records rec seen along directions d: wo = -d, random wi, u and lights"""
+    n = len(rec)
+    lights = g.lights()
+    eq = np.zeros(n, F.BSDF_EVAL_QUERY_DTYPE)
+    eq["wo"], eq["wi"], eq["bxdf"] = -d, _unit(rng.normal(size=(n, 3))), F.BXDF_ALL
+    sq = np.zeros(n, F.BSDF_SAMPLE_QUERY_DTYPE)
+    sq["wo"], sq["bxdf"], sq["u"], sq["u_comp"] = -d, F.BXDF_ALL, rng.random((n, 2)), rng.random(n)
+    lq = np.zeros(n, F.LIGHT_QUERY_DTYPE)
+    lq["p"], lq["u"], lq["light"], lq["time"] = rec["p"], rng.random((n, 2)), lights[rng.integers(0, len(lights), n)], rec["time"]
+    pq = np.zeros(n, F.LIGHT_PDF_QUERY_DTYPE)
+    pq["p"], pq["wi"], pq["light"], pq["time"] = rec["p"], eq["wi"], lq["light"], rec["time"]
+    mq = np.zeros(n, F.EMIT_QUERY_DTYPE)
+    mq["w"], mq["n"], mq["inst"], mq["time"] = -d, rec["ng"], rec["inst"], rec["time"]
+    return {"trb_bsdf_eval": eq, "trb_bsdf_sample": sq, "trb_light_sample": lq, "trb_light_pdf": pq, "trb_emitted": mq}
+
+
+def time_shading(g, rec, inputs, reps, T):
+    """median device time (CUDA events, one stream) of each _device query over the inputs, after one warm-up call"""
+    dev = T.device("cuda:0")
+    n = len(rec)
+    up = lambda a: T.from_numpy(np.ascontiguousarray(a).view(np.uint8).copy()).to(dev)  # noqa: E731
+    d_rec = up(rec)
+    d_in = {k: up(v) for k, v in inputs.items()}
+    d_out = {k: T.empty(n * size, dtype=T.uint8, device=dev) for k, size in (("trb_bsdf_eval", 16), ("trb_bsdf_sample", 32), ("trb_light_sample", 80),
+                                                                             ("trb_light_pdf", 4), ("trb_emitted", 12))}
+    s = T.cuda.Stream()
+    s.wait_stream(T.cuda.current_stream())
+    st = s.cuda_stream
+    calls = {
+        "trb_bsdf_eval": lambda: g.bsdf_eval_device(n, d_rec.data_ptr(), d_in["trb_bsdf_eval"].data_ptr(), d_out["trb_bsdf_eval"].data_ptr(), st),
+        "trb_bsdf_sample": lambda: g.bsdf_sample_device(n, d_rec.data_ptr(), d_in["trb_bsdf_sample"].data_ptr(), d_out["trb_bsdf_sample"].data_ptr(), st),
+        "trb_light_sample": lambda: g.light_sample_device(n, d_in["trb_light_sample"].data_ptr(), d_out["trb_light_sample"].data_ptr(), st),
+        "trb_light_pdf": lambda: g.light_pdf_device(n, d_in["trb_light_pdf"].data_ptr(), d_out["trb_light_pdf"].data_ptr(), st),
+        "trb_emitted": lambda: g.emitted_device(n, d_in["trb_emitted"].data_ptr(), d_out["trb_emitted"].data_ptr(), st),
+    }
+    out = {}
+    for name, call in calls.items():
+        call()
+        s.synchronize()
+        ms = []
+        for _ in range(reps):
+            e0, e1 = T.cuda.Event(enable_timing=True), T.cuda.Event(enable_timing=True)
+            e0.record(s)
+            call()
+            e1.record(s)
+            s.synchronize()
+            ms.append(e0.elapsed_time(e1))
+        med = float(np.median(ms))
+        gbs = n * SHADING_BYTES[name] / med / 1e6
+        out[name] = {"ms": med, "mqueries_per_s": n / med / 1e3, "gb_per_s": gbs, "hbm_fraction": gbs / HBM_PEAK_GBS}
+    return out
+
+
+def shading_queries(a, res):
+    """The shading queries on two workloads: the records of C4's --width x --height camera rays (1 spp; every surface matte, 1 M
+    triangles), and --rays synthetic records on the material zoo (every material kind and a MERL table, random frames)."""
+    import torch as T
+    dev = T.device("cuda:0")
+    rng = np.random.default_rng(0x5AD)
+    res["shading"] = {}
+    # C4 camera rays -> records on the device
+    g = api.Scene(SB.scene_c4(a.tris, a.width, a.height, 1).finish())
+    g.update_frame(0, 0.0, 0.0)
+    rays, _ = g.camera_rays(seed=1)
+    q = np.zeros(len(rays), F.QUERY_RAY_DTYPE)
+    for k in ("o", "d", "min_t", "max_t"):
+        q[k] = rays[k]
+    n = len(q)
+    d_q = T.from_numpy(q.view(np.uint8).copy()).to(dev)
+    d_rec = T.empty(n * F.INTERSECTION_DTYPE.itemsize, dtype=T.uint8, device=dev)
+    g.intersect_records_device(n, d_q.data_ptr(), d_rec.data_ptr())
+    rec = np.frombuffer(d_rec.cpu().numpy().tobytes(), F.INTERSECTION_DTYPE).copy()
+    res["shading"]["c4_camera"] = {"queries": n, "hit_fraction": float((rec["inst"] != F.MISS).mean()),
+                                   "results": time_shading(g, rec, shading_inputs(g, rec, q["d"], rng), a.reps, T)}
+    del g
+    # synthetic records on the material zoo
+    desc = SB.scene_materials_zoo(64, 64, 1, SB.synthetic_merl_table()).finish()
+    z = api.Scene(desc)
+    z.update_frame(0, 0.0, 0.0)
+    m = a.rays
+    rec = np.zeros(m, F.INTERSECTION_DTYPE)
+    rec["material"] = rng.integers(0, desc.n_materials, m)
+    rec["p"] = rng.uniform((-14, 1, -10), (14, 23, 18), size=(m, 3))
+    rec["n"] = _unit(rng.normal(size=(m, 3)))
+    rec["ng"] = rec["n"]
+    rec["dp_du"] = _unit(rng.normal(size=(m, 3)))
+    rec["inst"] = rng.integers(0, desc.n_instances, m)
+    d = _unit(rng.normal(size=(m, 3)))
+    d = np.where(((d * rec["n"]).sum(1) > 0)[:, None], -d, d)  # seen from the front
+    res["shading"]["zoo_synthetic"] = {"queries": m, "materials": int(desc.n_materials),
+                                       "results": time_shading(z, rec, shading_inputs(z, rec, d, rng), a.reps, T)}
+    for wl, r in res["shading"].items():
+        print("  shading queries, %s (%d queries), median of %d:" % (wl, r["queries"], a.reps))
+        for name, x in r["results"].items():
+            print("  %-40s %8.3f ms  %8.1f Mqueries/s  %7.1f GB/s (%.1f%% of %.0f GB/s HBM)" % (name, x["ms"], x["mqueries_per_s"], x["gb_per_s"],
+                                                                                           100 * x["hbm_fraction"], HBM_PEAK_GBS))
 
 
 if __name__ == "__main__":

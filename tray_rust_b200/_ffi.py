@@ -22,6 +22,8 @@ FILTER_MITCHELL_NETRAVALI, FILTER_GAUSSIAN = 0, 1
 INTEGRATOR_PATH, INTEGRATOR_WHITTED, INTEGRATOR_NORMALS_DEBUG = 0, 1, 2
 RENDER_STATS, RENDER_NO_UPDATE, RENDER_REFERENCE_SHADOW, RENDER_MEGAKERNEL, RENDER_TIME_TRACE = 1, 2, 4, 8, 16
 QUERY_CLAMP = 32  # trb_illumination: clamp each sample to [0, 1] before averaging
+BXDF_REFLECTION, BXDF_TRANSMISSION, BXDF_DIFFUSE, BXDF_GLOSSY, BXDF_SPECULAR = 1, 2, 4, 8, 16  # bxdf::BxDFType
+BXDF_ALL = 31
 MISS = 0xFFFFFFFF
 BVH_LEAF = 0x80000000
 MERL_TABLE_FLOATS = 90 * 90 * 180 * 3
@@ -138,6 +140,34 @@ class IllumRay(C.Structure):
     _fields_ = [("o", f32 * 3), ("d", f32 * 3), ("min_t", f32), ("max_t", f32), ("time", f32), ("key", u32), ("sample", u32), ("pad", u32)]
 
 
+class BsdfEvalQuery(C.Structure):
+    _fields_ = [("wo", f32 * 3), ("bxdf", u32), ("wi", f32 * 3), ("pad", u32)]
+
+
+class BsdfSampleQuery(C.Structure):
+    _fields_ = [("wo", f32 * 3), ("bxdf", u32), ("u", f32 * 2), ("u_comp", f32), ("pad", u32)]
+
+
+class BsdfSampleResult(C.Structure):
+    _fields_ = [("f", f32 * 3), ("pdf", f32), ("wi", f32 * 3), ("sampled", u32)]
+
+
+class LightQuery(C.Structure):
+    _fields_ = [("p", f32 * 3), ("time", f32), ("u", f32 * 2), ("light", u32), ("pad", u32)]
+
+
+class LightSampleResult(C.Structure):
+    _fields_ = [("li", f32 * 3), ("pdf", f32), ("wi", f32 * 3), ("delta", u32), ("shadow", QueryRay)]
+
+
+class LightPdfQuery(C.Structure):
+    _fields_ = [("p", f32 * 3), ("time", f32), ("wi", f32 * 3), ("light", u32)]
+
+
+class EmitQuery(C.Structure):
+    _fields_ = [("w", f32 * 3), ("time", f32), ("n", f32 * 3), ("inst", u32)]
+
+
 class Sample(C.Structure):
     _fields_ = [("x", f32), ("y", f32), ("r", f32), ("g", f32), ("b", f32)]
 
@@ -159,6 +189,13 @@ INTERSECTION_DTYPE = np.dtype([("t", "<f4"), ("inst", "<u4"), ("prim", "<u4"), (
                                ("pad", "<u4", 2)])
 ILLUM_RAY_DTYPE = np.dtype([("o", "<f4", 3), ("d", "<f4", 3), ("min_t", "<f4"), ("max_t", "<f4"), ("time", "<f4"), ("key", "<u4"),
                             ("sample", "<u4"), ("pad", "<u4")])
+BSDF_EVAL_QUERY_DTYPE = np.dtype([("wo", "<f4", 3), ("bxdf", "<u4"), ("wi", "<f4", 3), ("pad", "<u4")])
+BSDF_SAMPLE_QUERY_DTYPE = np.dtype([("wo", "<f4", 3), ("bxdf", "<u4"), ("u", "<f4", 2), ("u_comp", "<f4"), ("pad", "<u4")])
+BSDF_SAMPLE_DTYPE = np.dtype([("f", "<f4", 3), ("pdf", "<f4"), ("wi", "<f4", 3), ("sampled", "<u4")])
+LIGHT_QUERY_DTYPE = np.dtype([("p", "<f4", 3), ("time", "<f4"), ("u", "<f4", 2), ("light", "<u4"), ("pad", "<u4")])
+LIGHT_SAMPLE_DTYPE = np.dtype([("li", "<f4", 3), ("pdf", "<f4"), ("wi", "<f4", 3), ("delta", "<u4"), ("shadow", QUERY_RAY_DTYPE)])
+LIGHT_PDF_QUERY_DTYPE = np.dtype([("p", "<f4", 3), ("time", "<f4"), ("wi", "<f4", 3), ("light", "<u4")])
+EMIT_QUERY_DTYPE = np.dtype([("w", "<f4", 3), ("time", "<f4"), ("n", "<f4", 3), ("inst", "<u4")])
 
 TRB_SYMBOLS = [
     "trb_scene_create", "trb_scene_load_json", "trb_scene_destroy", "trb_scene_info", "trb_scene_update_frame",
@@ -172,6 +209,8 @@ TRB_SYMBOLS = [
     "trb_render_adaptive_device", "trb_render_sharded_adaptive", "trb_group_render_adaptive",
     "trb_intersect_records", "trb_intersect_records_device", "trb_occluded", "trb_occluded_device",
     "trb_illumination", "trb_illumination_device",
+    "trb_bsdf_eval", "trb_bsdf_eval_device", "trb_bsdf_sample", "trb_bsdf_sample_device", "trb_light_sample", "trb_light_sample_device",
+    "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
 ]
 
 _trb = None
@@ -210,6 +249,17 @@ def load_trb():
     lib.trb_occluded_device.argtypes = [vp, sz, vp, vp, u32, vp, vp]
     lib.trb_illumination.argtypes = [vp, sz, vp, u32, u32, vp, u32, C.POINTER(Stats)]
     lib.trb_illumination_device.argtypes = [vp, sz, vp, u32, u32, vp, u32, vp, vp]
+    lib.trb_bsdf_eval.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_bsdf_eval_device.argtypes = [vp, sz, vp, vp, vp, vp]
+    lib.trb_bsdf_sample.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_bsdf_sample_device.argtypes = [vp, sz, vp, vp, vp, vp]
+    lib.trb_light_sample.argtypes = [vp, sz, vp, vp]
+    lib.trb_light_sample_device.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_light_pdf.argtypes = [vp, sz, vp, vp]
+    lib.trb_light_pdf_device.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_emitted.argtypes = [vp, sz, vp, vp]
+    lib.trb_emitted_device.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_scene_lights.argtypes = [vp, vp]
     lib.trb_camera_rays.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]

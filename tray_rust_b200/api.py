@@ -250,6 +250,76 @@ class Scene(_Base):
         flags = (F.RENDER_STATS if stats else 0) | (F.RENDER_REFERENCE_SHADOW if reference else 0) | (F.QUERY_CLAMP if clamp else 0)
         self._check(self._lib.trb_illumination_device(self._h, n, d_rays, spp, seed, d_rgb, flags, d_stats, stream))
 
+    # ---- shading queries: the render's BSDF and light functions on caller inputs (trace nothing) ----
+    def bsdf_eval(self, records, queries):
+        """trb_bsdf_eval: Material::bsdf at each INTERSECTION_DTYPE record, then BSDF::eval and BSDF::pdf of the BSDF_EVAL_QUERY_DTYPE
+        query. Returns (n, 4) float32: r, g, b, pdf. A missed record or a material out of range gives zeros."""
+        rec = np.ascontiguousarray(records, dtype=F.INTERSECTION_DTYPE)
+        q = np.ascontiguousarray(queries, dtype=F.BSDF_EVAL_QUERY_DTYPE)
+        assert len(rec) == len(q)
+        out = np.zeros((len(q), 4), np.float32)
+        self._check(self._lib.trb_bsdf_eval(self._h, len(q), F.ptr(rec), F.ptr(q), F.ptr(out)))
+        return out
+
+    def bsdf_eval_device(self, n, d_rec, d_q, d_out, stream=None):
+        """trb_bsdf_eval_device: n records (96 B), n queries (32 B) -> n * 4 float32, device buffers 16-byte aligned, enqueued on
+        `stream` (a cudaStream_t as an int; None = default stream) without host synchronisation."""
+        self._check(self._lib.trb_bsdf_eval_device(self._h, n, d_rec, d_q, d_out, stream))
+
+    def bsdf_sample(self, records, queries):
+        """trb_bsdf_sample: Material::bsdf at each record, then BSDF::sample of the BSDF_SAMPLE_QUERY_DTYPE query. Returns
+        BSDF_SAMPLE_DTYPE (f, pdf, wi, sampled type bits)."""
+        rec = np.ascontiguousarray(records, dtype=F.INTERSECTION_DTYPE)
+        q = np.ascontiguousarray(queries, dtype=F.BSDF_SAMPLE_QUERY_DTYPE)
+        assert len(rec) == len(q)
+        out = np.zeros(len(q), F.BSDF_SAMPLE_DTYPE)
+        self._check(self._lib.trb_bsdf_sample(self._h, len(q), F.ptr(rec), F.ptr(q), F.ptr(out)))
+        return out
+
+    def bsdf_sample_device(self, n, d_rec, d_q, d_out, stream=None):
+        """trb_bsdf_sample_device: n records, n queries -> n BSDF_SAMPLE_DTYPE results (32 B), device buffers 16-byte aligned."""
+        self._check(self._lib.trb_bsdf_sample_device(self._h, n, d_rec, d_q, d_out, stream))
+
+    def light_sample(self, queries):
+        """trb_light_sample: Light::sample_incident of each LIGHT_QUERY_DTYPE query. Returns LIGHT_SAMPLE_DTYPE (li, pdf, wi, delta and
+        the shadow ray as a QUERY_RAY_DTYPE, ready for occluded())."""
+        q = np.ascontiguousarray(queries, dtype=F.LIGHT_QUERY_DTYPE)
+        out = np.zeros(len(q), F.LIGHT_SAMPLE_DTYPE)
+        self._check(self._lib.trb_light_sample(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def light_sample_device(self, n, d_q, d_out, stream=None):
+        """trb_light_sample_device: n queries (32 B) -> n LIGHT_SAMPLE_DTYPE results (80 B), device buffers 16-byte aligned."""
+        self._check(self._lib.trb_light_sample_device(self._h, n, d_q, d_out, stream))
+
+    def light_pdf(self, queries):
+        """trb_light_pdf: Light::pdf of each LIGHT_PDF_QUERY_DTYPE query. Returns (n,) float32."""
+        q = np.ascontiguousarray(queries, dtype=F.LIGHT_PDF_QUERY_DTYPE)
+        out = np.zeros(len(q), np.float32)
+        self._check(self._lib.trb_light_pdf(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def light_pdf_device(self, n, d_q, d_pdf, stream=None):
+        """trb_light_pdf_device: n queries (32 B, 16-byte aligned) -> n float32 (4-byte aligned)."""
+        self._check(self._lib.trb_light_pdf_device(self._h, n, d_q, d_pdf, stream))
+
+    def emitted(self, queries):
+        """trb_emitted: Emitter::radiance of each EMIT_QUERY_DTYPE query (black for receivers). Returns (n, 3) float32."""
+        q = np.ascontiguousarray(queries, dtype=F.EMIT_QUERY_DTYPE)
+        out = np.zeros((len(q), 3), np.float32)
+        self._check(self._lib.trb_emitted(self._h, len(q), F.ptr(q), F.ptr(out)))
+        return out
+
+    def emitted_device(self, n, d_q, d_rgb, stream=None):
+        """trb_emitted_device: n queries (32 B, 16-byte aligned) -> n * 3 float32 (4-byte aligned)."""
+        self._check(self._lib.trb_emitted_device(self._h, n, d_q, d_rgb, stream))
+
+    def lights(self):
+        """trb_scene_lights: the instance indices of the light list, in sample_one_light's order."""
+        out = np.zeros(self.n_lights, np.uint32)
+        self._check(self._lib.trb_scene_lights(self._h, F.ptr(out)))
+        return out
+
     def to_srgb8(self, film):
         film = np.ascontiguousarray(film, dtype=np.float32)
         out = np.zeros((self.height, self.width, 3), np.uint8)

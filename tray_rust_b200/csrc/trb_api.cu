@@ -214,6 +214,7 @@ struct trb_scene {
     bool frame_set = false; uint32_t last_frame = 0; float last_start = 0, last_end = 0; // the arguments of the last update_frame (re-run when an option changes what it builds)
     uint32_t material_kinds = 0;         // bit k: some hittable instance's material is of kind k (TRB_MAT_*)
     bool mixed_materials = false;        // the hittable instances use >= 2 material kinds or a MERL table: the split shade kernels with material buckets win (Tuning::shade_split = -1)
+    bool anim_emission = false;          // some emitter's colour is keyframed (ds.has_anim is only known after update_frame; trb_emitted runs before it)
     uint32_t* d_anim_instances = nullptr;
     // per-frame host state
     int active_camera = -1;
@@ -940,6 +941,103 @@ trb_status query_host(trb_scene* s, size_t n, const void* rays, size_t ray_bytes
     return TRB_OK;
 }
 
+// The static part of the device instance records (everything but the matrices, which update_frame writes); keyframed / animated flags
+// are scene properties. anim_list: the keyframed instances. Returns whether any instance's transform or emission depends on time.
+bool static_instance_records(const trb_scene* s, std::vector<trb::DInstance>& di, std::vector<uint32_t>& anim_list) {
+    const size_t n = s->instances.size();
+    bool any_anim = false;
+    di.assign(n, trb::DInstance{});
+    anim_list.clear();
+    for (size_t i = 0; i < n; ++i) {
+        const trb_instance& in = s->instances[i];
+        trb::DInstance& o = di[i];
+        std::memset(&o, 0, sizeof o);
+        o.kind = in.kind; o.shape = in.shape; o.p0 = in.p0; o.p1 = in.p1; o.mesh = in.mesh; o.material = in.material;
+        o.xf_first = in.spline_first; o.xf_count = in.n_splines;
+        if (!trbh::xf_is_static(s->splines.data(), in.spline_first, in.n_splines)) {
+            o.flags |= trb::DI_ANIM_XF; o.spline_first = in.spline_first; o.n_splines = in.n_splines; any_anim = true;
+            o.anim_slot = (uint32_t)anim_list.size(); anim_list.push_back((uint32_t)i);
+        }
+        if (in.kind != TRB_INST_RECEIVER) {
+            for (int k = 0; k < 3; ++k) o.emission[k] = s->color_keys[in.emission_first].rgba[k];
+            if (in.n_emission > 1) { o.flags |= trb::DI_ANIM_EMISSION; o.emission_first = in.emission_first; o.n_emission = in.n_emission; any_anim = true; }
+        }
+    }
+    return any_anim;
+}
+
+// ---- shading queries (trb_bsdf_eval / trb_bsdf_sample / trb_light_sample / trb_light_pdf / trb_emitted; DESIGN.md §5) ------------------
+// Argument checks: `a` and `b` are the input buffers (the light and emission queries have one and pass it twice), read with 16-byte
+// loads on the device; `out_align` is the device output's required alignment. `frame`: the query reads the instance matrices.
+trb_status shade_check(const trb_scene* s, size_t n, const void* a, const void* b, const void* out, uintptr_t out_align, bool device, bool frame) {
+    if (!s || (n && (!a || !b || !out))) return fail(TRB_INVALID_ARG, "null argument");
+    if (device && n && (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15u) || (reinterpret_cast<uintptr_t>(out) & (out_align - 1))))
+        return fail(TRB_INVALID_ARG, out_align == 16 ? "device query buffers must be 16-byte aligned"
+                                                     : "device query buffers must be 16-byte aligned, the float output 4-byte aligned");
+    if (frame && !s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
+    return TRB_OK;
+}
+
+// One thread per query, grid-stride: at most 16 CTAs of 128 threads per SM
+inline unsigned shade_grid(const trb_scene* s, size_t n) { return (unsigned)std::min<size_t>((n + 127) / 128, (size_t)s->sm_count * 16); }
+
+// The blocking host-buffer form of a shading query: stage the inputs (b may be null) in one device allocation, run enqueue(d_a, d_b,
+// d_out) on the default stream, copy the results back.
+template <class Enqueue>
+trb_status shade_host(trb_scene* s, size_t n, const void* a, size_t a_bytes, const void* b, size_t b_bytes, void* out, size_t out_bytes,
+                      Enqueue enqueue) {
+    if (n == 0) return TRB_OK;
+    CU(cudaSetDevice(s->device));
+    const size_t b_off = (a_bytes + 255) / 256 * 256, o_off = b_off + (b_bytes + 255) / 256 * 256;
+    char* d = nullptr;
+    CU(cudaMalloc(&d, o_off + out_bytes));
+    cudaError_t e = cudaMemcpy(d, a, a_bytes, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && b) e = cudaMemcpy(d + b_off, b, b_bytes, cudaMemcpyHostToDevice);
+    trb_status r = TRB_OK;
+    if (e == cudaSuccess) r = enqueue(d, d + b_off, d + o_off);
+    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out, d + o_off, out_bytes, cudaMemcpyDeviceToHost);
+    if (r != TRB_OK) cudaDeviceSynchronize();
+    cudaFree(d);
+    if (r != TRB_OK) return r;
+    CU(e);
+    return TRB_OK;
+}
+
+trb_status launch_bsdf_eval(trb_scene* s, size_t n, const trb_intersection* d_rec, const trb_bsdf_eval_query* d_q, float* d_out, cudaStream_t st) {
+    trb::k_bsdf_eval<<<shade_grid(s, n), 128, 0, st>>>(s->ds, (uint32_t)s->materials.size(), n, d_rec, d_q, reinterpret_cast<float4*>(d_out));
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+trb_status launch_bsdf_sample(trb_scene* s, size_t n, const trb_intersection* d_rec, const trb_bsdf_sample_query* d_q, trb_bsdf_sample_result* d_out,
+                              cudaStream_t st) {
+    trb::k_bsdf_sample<<<shade_grid(s, n), 128, 0, st>>>(s->ds, (uint32_t)s->materials.size(), n, d_rec, d_q, d_out);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+trb_status launch_light_sample(trb_scene* s, size_t n, const trb_light_query* d_q, trb_light_sample_result* d_out, cudaStream_t st) {
+    if (s->ds.has_anim) trb::k_light_sample<true><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_out);
+    else trb::k_light_sample<false><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_out);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+trb_status launch_light_pdf(trb_scene* s, size_t n, const trb_light_pdf_query* d_q, float* d_pdf, cudaStream_t st) {
+    if (s->ds.has_anim) trb::k_light_pdf<true><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_pdf);
+    else trb::k_light_pdf<false><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_pdf);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+trb_status launch_emitted(trb_scene* s, size_t n, const trb_emit_query* d_q, float* d_rgb, cudaStream_t st) {
+    if (s->ds.has_anim || s->anim_emission) trb::k_emitted<true><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_rgb);
+    else trb::k_emitted<false><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_rgb);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -1213,6 +1311,13 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
         ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
         ds.splines = d_sp; ds.keyframes = d_kf; ds.knots = d_kn; ds.color_keys = d_ck; ds.level_xf = d_lv; ds.has_anim = 0;
     }
+    { // the instance records without matrices, so that trb_emitted runs before the first update_frame
+        std::vector<trb::DInstance> di;
+        std::vector<uint32_t> anim_list;
+        static_instance_records(s.get(), di, anim_list);
+        CU(cudaMemcpy(s->d_instances, di.data(), di.size() * sizeof(trb::DInstance), cudaMemcpyHostToDevice));
+        for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_RECEIVER && in.n_emission > 1) s->anim_emission = true;
+    }
     // Scene::load_file builds the BVH<Instance> for [0, scene_time] (scene.rs:141); the first render rebuilds it
     *out = s.release();
     return TRB_OK;
@@ -1276,24 +1381,9 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
 
     // instance transforms + bounds, then BVH<Instance>::rebuild(shutter_open, shutter_close) (scene.rs:175, bvh.rs:61-78)
     const size_t n = s->instances.size();
-    // static part of the device instance records (everything but the matrices); keyframed / animated flags are scene properties
-    std::vector<trb::DInstance> di(n);
+    std::vector<trb::DInstance> di;
     std::vector<uint32_t> anim_list;
-    for (size_t i = 0; i < n; ++i) {
-        const trb_instance& in = s->instances[i];
-        trb::DInstance& o = di[i];
-        std::memset(&o, 0, sizeof o);
-        o.kind = in.kind; o.shape = in.shape; o.p0 = in.p0; o.p1 = in.p1; o.mesh = in.mesh; o.material = in.material;
-        o.xf_first = in.spline_first; o.xf_count = in.n_splines;
-        if (!trbh::xf_is_static(s->splines.data(), in.spline_first, in.n_splines)) {
-            o.flags |= trb::DI_ANIM_XF; o.spline_first = in.spline_first; o.n_splines = in.n_splines; any_anim = true;
-            o.anim_slot = (uint32_t)anim_list.size(); anim_list.push_back((uint32_t)i);
-        }
-        if (in.kind != TRB_INST_RECEIVER) {
-            for (int k = 0; k < 3; ++k) o.emission[k] = s->color_keys[in.emission_first].rgba[k];
-            if (in.n_emission > 1) { o.flags |= trb::DI_ANIM_EMISSION; o.emission_first = in.emission_first; o.n_emission = in.n_emission; any_anim = true; }
-        }
-    }
+    if (static_instance_records(s, di, anim_list)) any_anim = true;
     s->ds.has_anim = any_anim ? 1u : 0u;
     if (n + 1 > s->tlas_capacity) { // a tree over n instances has < n interior records and < 2n nodes
         CU(s->arena.alloc(n + 1, &s->d_tlas_quads));
@@ -1734,6 +1824,84 @@ trb_status trb_illumination_device(trb_scene* s, size_t n, const trb_illum_ray* 
     if (r != TRB_OK || n == 0) return r;
     CU(cudaSetDevice(s->device));
     return illum_passes(s, n, d_rays, spp, seed, d_rgb, flags, reinterpret_cast<trb::DStats*>(d_stats), static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_bsdf_eval(trb_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_eval_query* q, float* out4) {
+    const trb_status r = shade_check(s, n, rec, q, out4, 16, false, false);
+    return r != TRB_OK ? r : shade_host(s, n, rec, n * sizeof *rec, q, n * sizeof *q, out4, n * 4 * sizeof(float), [&](void* a, void* b, void* o) {
+        return launch_bsdf_eval(s, n, static_cast<const trb_intersection*>(a), static_cast<const trb_bsdf_eval_query*>(b), static_cast<float*>(o), 0);
+    });
+}
+
+trb_status trb_bsdf_eval_device(trb_scene* s, size_t n, const trb_intersection* d_rec, const trb_bsdf_eval_query* d_q, float* d_out4, void* stream) {
+    const trb_status r = shade_check(s, n, d_rec, d_q, d_out4, 16, true, false);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return launch_bsdf_eval(s, n, d_rec, d_q, d_out4, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_bsdf_sample(trb_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_sample_query* q, trb_bsdf_sample_result* out) {
+    const trb_status r = shade_check(s, n, rec, q, out, 16, false, false);
+    return r != TRB_OK ? r : shade_host(s, n, rec, n * sizeof *rec, q, n * sizeof *q, out, n * sizeof *out, [&](void* a, void* b, void* o) {
+        return launch_bsdf_sample(s, n, static_cast<const trb_intersection*>(a), static_cast<const trb_bsdf_sample_query*>(b), static_cast<trb_bsdf_sample_result*>(o), 0);
+    });
+}
+
+trb_status trb_bsdf_sample_device(trb_scene* s, size_t n, const trb_intersection* d_rec, const trb_bsdf_sample_query* d_q, trb_bsdf_sample_result* d_out,
+                                  void* stream) {
+    const trb_status r = shade_check(s, n, d_rec, d_q, d_out, 16, true, false);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return launch_bsdf_sample(s, n, d_rec, d_q, d_out, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_light_sample(trb_scene* s, size_t n, const trb_light_query* q, trb_light_sample_result* out) {
+    const trb_status r = shade_check(s, n, q, q, out, 16, false, true);
+    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, out, n * sizeof *out, [&](void* a, void*, void* o) {
+        return launch_light_sample(s, n, static_cast<const trb_light_query*>(a), static_cast<trb_light_sample_result*>(o), 0);
+    });
+}
+
+trb_status trb_light_sample_device(trb_scene* s, size_t n, const trb_light_query* d_q, trb_light_sample_result* d_out, void* stream) {
+    const trb_status r = shade_check(s, n, d_q, d_q, d_out, 16, true, true);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return launch_light_sample(s, n, d_q, d_out, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_light_pdf(trb_scene* s, size_t n, const trb_light_pdf_query* q, float* pdf) {
+    const trb_status r = shade_check(s, n, q, q, pdf, 4, false, true);
+    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, pdf, n * sizeof(float), [&](void* a, void*, void* o) {
+        return launch_light_pdf(s, n, static_cast<const trb_light_pdf_query*>(a), static_cast<float*>(o), 0);
+    });
+}
+
+trb_status trb_light_pdf_device(trb_scene* s, size_t n, const trb_light_pdf_query* d_q, float* d_pdf, void* stream) {
+    const trb_status r = shade_check(s, n, d_q, d_q, d_pdf, 4, true, true);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return launch_light_pdf(s, n, d_q, d_pdf, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_emitted(trb_scene* s, size_t n, const trb_emit_query* q, float* rgb) {
+    const trb_status r = shade_check(s, n, q, q, rgb, 4, false, false);
+    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, rgb, n * 3 * sizeof(float), [&](void* a, void*, void* o) {
+        return launch_emitted(s, n, static_cast<const trb_emit_query*>(a), static_cast<float*>(o), 0);
+    });
+}
+
+trb_status trb_emitted_device(trb_scene* s, size_t n, const trb_emit_query* d_q, float* d_rgb, void* stream) {
+    const trb_status r = shade_check(s, n, d_q, d_q, d_rgb, 4, true, false);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return launch_emitted(s, n, d_q, d_rgb, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_scene_lights(const trb_scene* s, uint32_t* inst) {
+    if (!s || (s->ds.n_lights && !inst)) return fail(TRB_INVALID_ARG, "null argument");
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < (uint32_t)s->instances.size(); ++i) if (s->instances[i].kind != TRB_INST_RECEIVER) inst[k++] = i; // as trb_scene_create builds ds.lights
+    return TRB_OK;
 }
 
 trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {

@@ -2951,6 +2951,124 @@ __global__ void __launch_bounds__(128) k_illum_reduce(const float4* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------
+// Shading queries (trb_bsdf_eval / trb_bsdf_sample / trb_light_sample / trb_light_pdf / trb_emitted): the render's shading functions
+// on caller inputs, one query per thread, grid-stride, 16-byte loads of every query and record. Nothing is traced. An index out of
+// range (a missed record, a material, light or instance past the scene's, a light that is not an emitter) writes zeros and reads
+// nothing else.
+// ------------------------------------------------------------------------------------------
+// Material::bsdf(&Intersection) (material/*.rs, bsdf.rs:38-44) at record r: the material's parameters sampled at (u, v, time), the
+// frame from n and dp_du. The record is already in world space, so no transform is involved.
+__device__ __forceinline__ bool record_bsdf(const DScene& sc, uint32_t n_materials, const trb_intersection* rec, Mat& m, Frame& fr) {
+    const float4* r = reinterpret_cast<const float4*>(rec); // t inst prim material | p n.x | n.yz ng.xy | ng.z u v time | dp_du dp_dv.x
+    const float4 a = __ldg(r);
+    if (__float_as_uint(a.y) == TRB_MISS || __float_as_uint(a.w) >= n_materials) return false;
+    const float4 b = __ldg(r + 1), c = __ldg(r + 2), d = __ldg(r + 3), e = __ldg(r + 4);
+    Surf s;
+    s.p = mk(b.x, b.y, b.z); s.n = mk(b.w, c.x, c.y); s.ng = mk(c.z, c.w, d.x); s.u = d.y; s.v = d.z; s.dp_du = mk(e.x, e.y, e.z);
+    load_mat_at(sc, __float_as_uint(a.w), d.y, d.z, d.w, m);
+    make_frame(s, fr);
+    return true;
+}
+// out[i] = (BSDF::eval(wo, wi, bxdf), BSDF::pdf(wo, wi, bxdf)) (bsdf.rs:66-78, 114-125)
+__global__ void __launch_bounds__(128) k_bsdf_eval(const __grid_constant__ DScene sc, uint32_t n_materials, size_t n, const trb_intersection* __restrict__ rec,
+                                                   const trb_bsdf_eval_query* __restrict__ q, float4* __restrict__ out) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        float4 o = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        Mat m; Frame fr;
+        if (record_bsdf(sc, n_materials, rec + i, m, fr)) {
+            const float4* qq = reinterpret_cast<const float4*>(q + i); // (wo, bxdf) (wi, pad)
+            const float4 a = __ldg(qq), b = __ldg(qq + 1);
+            const f3 wo = mk(a.x, a.y, a.z), wi = mk(b.x, b.y, b.z);
+            const uint32_t flags = __float_as_uint(a.w);
+            const f3 f = bsdf_eval(sc, m, fr, wo, wi, flags);
+            o = make_float4(f.x, f.y, f.z, bsdf_pdf(m, fr, wo, wi, flags));
+        }
+        out[i] = o;
+    }
+}
+// out[i] = BSDF::sample(wo, bxdf, Sample { two_d: u, one_d: u_comp }) (bsdf.rs:85-112): (f, pdf) (wi, sampled type bits)
+__global__ void __launch_bounds__(128) k_bsdf_sample(const __grid_constant__ DScene sc, uint32_t n_materials, size_t n, const trb_intersection* __restrict__ rec,
+                                                     const trb_bsdf_sample_query* __restrict__ q, trb_bsdf_sample_result* __restrict__ out) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        float4 o0 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), o1 = o0;
+        Mat m; Frame fr;
+        if (record_bsdf(sc, n_materials, rec + i, m, fr)) {
+            const float4* qq = reinterpret_cast<const float4*>(q + i); // (wo, bxdf) (u, u_comp, pad)
+            const float4 a = __ldg(qq), b = __ldg(qq + 1);
+            f3 f, wi; float pdf; uint32_t sampled;
+            bsdf_sample(sc, m, fr, mk(a.x, a.y, a.z), __float_as_uint(a.w), b.x, b.y, b.z, f, wi, pdf, sampled);
+            o0 = make_float4(f.x, f.y, f.z, pdf);
+            o1 = make_float4(wi.x, wi.y, wi.z, __uint_as_float(sampled));
+        }
+        float4* dst = reinterpret_cast<float4*>(out + i);
+        dst[0] = o0; dst[1] = o1;
+    }
+}
+// Is `li` an emitter of the scene? (anything else gives a zero result)
+__device__ __forceinline__ bool is_light(const DScene& sc, uint32_t li) { return li < sc.n_instances && __ldg(&sc.instances[li].kind) != TRB_INST_RECEIVER; }
+// out[i] = Light::sample_incident(p, u, time) of light q.light (emitter.rs:164-190): (Li, pdf) (wi, delta_light) and the
+// OcclusionTester as a ray, test_points(p, p_light, time) = Ray::segment(p, p_light - p, 0.001, 0.999, time) (light/mod.rs:21-23)
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_light_sample(const __grid_constant__ DScene sc, size_t n, const trb_light_query* __restrict__ q, trb_light_sample_result* __restrict__ out) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const float4* qq = reinterpret_cast<const float4*>(q + i); // (p, time) (u, light, pad)
+        const float4 a = __ldg(qq), b = __ldg(qq + 1);
+        const uint32_t li = __float_as_uint(b.z);
+        const float4 z = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        float4 o[5] = {z, z, z, z, z};
+        if (is_light(sc, li)) {
+            const f3 p = mk(a.x, a.y, a.z);
+            f3 lrad, wi, seg; float pdf;
+            light_sample_incident<ANIM>(sc, li, p, b.x, b.y, a.w, lrad, wi, pdf, seg);
+            const uint32_t delta = __ldg(&sc.instances[li].kind) == TRB_INST_EMITTER_POINT ? 1u : 0u;
+            // li pdf | wi delta | shadow: (o, d.x) (d.yz, min_t, max_t) (time, pad)
+            o[0] = make_float4(lrad.x, lrad.y, lrad.z, pdf);
+            o[1] = make_float4(wi.x, wi.y, wi.z, __uint_as_float(delta));
+            o[2] = make_float4(p.x, p.y, p.z, seg.x);
+            o[3] = make_float4(seg.y, seg.z, 0.001f, 0.999f);
+            o[4] = make_float4(a.w, 0.0f, 0.0f, 0.0f);
+        }
+        float4* dst = reinterpret_cast<float4*>(out + i);
+#pragma unroll
+        for (int k = 0; k < 5; ++k) dst[k] = o[k];
+    }
+}
+// Light::pdf of Emitter (emitter.rs:193-203): 0 for a point light, else the shape's pdf of the object-space point and normalised
+// direction — the operations of direct_setup's MIS weight, with the light's transform at `time`
+template <bool ANIM>
+__device__ __noinline__ float light_pdf(const DScene& sc, uint32_t li, f3 p, f3 wi, float time) {
+    const DInstance& light = sc.instances[li];
+    if (__ldg(&light.kind) == TRB_INST_EMITTER_POINT) return 0.0f;
+    float linv[16];
+    instance_inv<ANIM>(sc, light, time, linv);
+    const f3 pl = xf_point(linv, p);
+    const f3 wl = unit(xf_vector(linv, wi));
+    return shape_pdf(__ldg(&light.shape), __ldg(&light.p0), __ldg(&light.p1), pl, wl);
+}
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_light_pdf(const __grid_constant__ DScene sc, size_t n, const trb_light_pdf_query* __restrict__ q, float* __restrict__ pdf) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const float4* qq = reinterpret_cast<const float4*>(q + i); // (p, time) (wi, light)
+        const float4 a = __ldg(qq), b = __ldg(qq + 1);
+        const uint32_t li = __float_as_uint(b.w);
+        pdf[i] = is_light(sc, li) ? light_pdf<ANIM>(sc, li, mk(a.x, a.y, a.z), mk(b.x, b.y, b.z), a.w) : 0.0f;
+    }
+}
+// rgb[3i..3i+2] = Emitter::radiance(w, _, n, time) (emitter.rs:140-142) of instance q.inst: its emission at `time` when
+// dot(w, n) > 0, else black; black for a receiver
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_emitted(const __grid_constant__ DScene sc, size_t n, const trb_emit_query* __restrict__ q, float* __restrict__ rgb) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const float4* qq = reinterpret_cast<const float4*>(q + i); // (w, time) (n, inst)
+        const float4 a = __ldg(qq), b = __ldg(qq + 1);
+        const uint32_t inst = __float_as_uint(b.w);
+        f3 le = splat(0.0f);
+        if (is_light(sc, inst) && dot3(mk(a.x, a.y, a.z), mk(b.x, b.y, b.z)) > 0.0f) emission_at<ANIM>(sc, sc.instances[inst], a.w, le.x, le.y, le.z);
+        rgb[3 * i] = le.x; rgb[3 * i + 1] = le.y; rgb[3 * i + 2] = le.z;
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // Scene::update_frame on the device (SURVEY 8f N1; scene.rs:152-176, bvh.rs:61-78): per instance the world transform at the
 // shutter-open time and its bounds over the shutter interval (animation_bounds, animated_transform.rs:57-70: 128 time
 // samples when every stacked level is keyframed, one box otherwise — Q22), then BVH<Instance>::rebuild with the reference's
