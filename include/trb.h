@@ -599,6 +599,37 @@ trb_status trb_camera_rays(trb_scene* scene, const trb_render_cfg* cfg, size_t n
 trb_status trb_render_samples(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_sample* samples,
                               trb_stats* stats);
 
+/* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
+ * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
+ * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */
+trb_status trb_camera_rays_device(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_ray* d_rays, float* d_xy,
+                                  void* cuda_stream);
+
+/* -- film writes: RenderTarget::write (render_target.rs:77-165) for caller samples ---------------------------------------------
+ * samples[i] is an ImageSample: film position (x, y) and colour (r, g, b); trb_render_samples' output goes straight in.
+ * regions[i] is the Region `write` receives for the sample: the 8x8 block with row-major index by * (width / 8) + bx. A region
+ * index >= the block count skips the sample. Regions are not derived from floor(x): a low-discrepancy position vdc + px can round
+ * up to exactly px + 1, into the next pixel and sometimes the next block, and the render writes that sample with the block it came
+ * from, so only an explicit region reproduces the render.
+ * Order: the result equals, bit for bit, the film left by this sequence of reference calls: start from the caller's film, call
+ * RenderTarget::write once per region that has at least one sample, regions in the order of the scene's Morton block list
+ * (block_queue.rs:28-46, trb_block_list), each region's samples in input order. That is the order a one-thread
+ * MultiThreaded::render writes in, so trb_render_samples of a whole frame written with this call gives the film of a one-thread
+ * reference render. Consequences: a pixel inside the write range [start - fpw, start + 8 + fpw] (clipped to the image) of a
+ * non-empty region gets += S_r even when S_r is zero, which turns -0.0 into +0.0; pixels outside every write range keep their
+ * bits; two calls compose as two sequences of writes; splitting one block's samples across calls changes the last bits.
+ * Film: RGBW, row-major, width*height*4 floats (get_renderf32 layout), added into in place like trb_render. The filter is fixed
+ * when the scene is created, so no update_frame is needed. No float atomics: the result does not depend on scheduling.
+ * Statuses: TRB_INVALID_ARG for null arguments with n > 0, unaligned device buffers (4 bytes) and n >= 2^32 (checked before
+ * anything is read); n == 0 is TRB_OK. The sort needs about 16 bytes of scratch per sample on the device (kept by the scene and
+ * grown on demand); TRB_OOM when it does not fit: the write is never split into passes, because a split would change the result.
+ * The host form takes host buffers and blocks. The _device form takes device buffers on the scene's GPU and enqueues on
+ * cuda_stream under trb_render_device's one-stream-per-scene rule, without host synchronisation except once, when the scratch
+ * space grows. */
+trb_status trb_film_write(trb_scene* scene, size_t n, const trb_sample* samples, const uint32_t* regions, float* film_rgbw);
+trb_status trb_film_write_device(trb_scene* scene, size_t n, const trb_sample* d_samples, const uint32_t* d_regions,
+                                 float* d_film_rgbw, void* cuda_stream);
+
 /* ≙ RenderTarget::get_render (render_target.rs:185-210): rgb/weight, clamp, sRGB,
  * (c*255) as u8; pixels with weight <= 0 stay 0. Host buffers; runs on the scene's GPU. */
 trb_status trb_film_to_srgb8(trb_scene* scene, const float* film_rgbw, uint8_t* rgb8);

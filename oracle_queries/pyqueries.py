@@ -3,7 +3,7 @@ TEST INFRASTRUCTURE, like oracle/pyoracle.py.
 
 ``QueryOracleScene`` is an ``OracleScene`` backed by that library (the detmath oracle with the ray queries added), so it has
 every oracle method plus ``intersect_records``, ``occluded``, ``illumination`` and the shading queries ``bsdf_eval``, ``bsdf_sample``,
-``light_sample``, ``light_pdf``, ``emitted`` and ``lights`` with the signatures of ``tray_rust_b200.api.Scene``.
+``light_sample``, ``light_pdf``, ``emitted`` and ``lights``, and ``film_write``, with the signatures of ``tray_rust_b200.api.Scene``.
 """
 import ctypes as C
 
@@ -25,6 +25,7 @@ def load():
         for name in ("orc_light_sample", "orc_light_pdf", "orc_emitted"):
             getattr(lib, name).argtypes = [vp, sz, vp, vp]
         lib.orc_scene_lights.argtypes = [vp, vp]
+        lib.orc_film_write.argtypes = [vp, sz, vp, vp, vp]
         lib._queries_ready = True
     return lib
 
@@ -100,3 +101,14 @@ class QueryOracleScene(O.OracleScene):
         out = np.zeros(n, np.uint32)
         self._check(self._lib.orc_scene_lights(self._h, F.ptr(out)))
         return out
+
+    def film_write(self, samples, regions, film=None):
+        """RenderTarget::write per non-empty region in Morton-list order (see api.Scene.film_write); film is added into in place."""
+        samples = np.ascontiguousarray(samples, dtype=F.SAMPLE_DTYPE)
+        regions = np.ascontiguousarray(regions, dtype=np.uint32)
+        assert len(samples) == len(regions)
+        if film is None:
+            film = np.zeros((self._desc.film.height, self._desc.film.width, 4), np.float32)
+        assert film.dtype == np.float32 and film.flags.c_contiguous and film.size == self._desc.film.height * self._desc.film.width * 4
+        self._check(self._lib.orc_film_write(self._h, len(samples), F.ptr(samples), F.ptr(regions), F.ptr(film)))
+        return film

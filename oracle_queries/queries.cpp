@@ -15,6 +15,9 @@
  *   orc_light_sample / orc_light_pdf  SceneShade::sample_incident and light_pdf (emitter.rs:164-204)
  *   orc_emitted                       SceneShade::radiance (emitter.rs:140-142)
  *   orc_scene_lights                  the light list of sample_one_light
+ * and the film half:
+ *   orc_film_write                    RenderTarget::write (render_target.rs:77-165), called once per region that has samples, regions
+ *                                     in the Morton block list's order, each region's samples in input order
  */
 #include "../oracle/oracle.cpp"
 
@@ -193,6 +196,22 @@ int orc_emitted(orc_scene* s, size_t n, const trb_emit_query* q, float* rgb) {
 /* the light list of sample_one_light: instance indices of the emitters in object order */
 int orc_scene_lights(const orc_scene* s, uint32_t* inst) {
     for (size_t k = 0; k < s->shade.lights.size(); ++k) inst[k] = s->shade.lights[k];
+    return TRB_OK;
+}
+
+/* ---- film writes: the samples grouped by region (index by * (width / 8) + bx; out-of-range indices skip the sample), then the
+ * existing RenderTarget::write once per non-empty region in the order of BlockQueue::new's Morton list, one thread, no atomics. */
+int orc_film_write(orc_scene* s, size_t n, const trb_sample* samples, const uint32_t* regions, float* film_rgbw) {
+    const uint32_t nbx = s->film.width / 8, nr = nbx * (s->film.height / 8);
+    std::vector<std::vector<ImageSample>> by_region(nr);
+    for (size_t i = 0; i < n; ++i)
+        if (regions[i] < nr) by_region[regions[i]].push_back(ImageSample{samples[i].x, samples[i].y, Col(samples[i].r, samples[i].g, samples[i].b)});
+    for (const auto& b : s->block_list(0, 0)) {
+        const std::vector<ImageSample>& v = by_region[b.second * nbx + b.first];
+        if (v.empty()) continue;
+        const int x0 = (int)b.first * 8, y0 = (int)b.second * 8;
+        s->rt.write(v, x0, y0, x0 + 8, y0 + 8, film_rgbw, false);
+    }
     return TRB_OK;
 }
 

@@ -16,6 +16,12 @@ over every traced ray (primary, shadow, MIS, continuation).
 Last, the five shading queries (trb_bsdf_eval, trb_bsdf_sample, trb_light_sample, trb_light_pdf, trb_emitted; device forms) on the
 records of those camera rays and on --rays synthetic records on the material zoo: Mqueries/s and the GB/s of the query, record and
 output bytes, with their share of the H100 SXM's 3.35 TB/s HBM3 peak.
+
+Then trb_film_write_device on C4's whole-frame camera samples (--width x --height at --film-spp, trb_render_samples with the regions
+of sample_regions()) into a device film: the whole call between CUDA events, and its two phases from torch.profiler's kernel
+times (sort = k_film_keys + CUB's radix sort + k_film_starts; gather = k_film_gather). Last, the worst case the order contract
+allows: 2^20 samples that all name one region, so each of that region's pixels sums them serially.
+--sections film runs only this part.
 """
 import argparse
 import json
@@ -45,8 +51,17 @@ def main():
     ap.add_argument("--tris", type=int, default=1_000_000)
     ap.add_argument("--width", type=int, default=1920)
     ap.add_argument("--height", type=int, default=1080)
+    ap.add_argument("--film-spp", type=int, default=8)
+    ap.add_argument("--sections", default="all", choices=["all", "film"])
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
+    if a.sections == "film":
+        res = {"device": device_info()}
+        film_writes(a, res)
+        if a.out:
+            os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+            json.dump(res, open(a.out, "w"), indent=1)
+        return
     import torch as T
     dev = T.device("cuda:0")
     g = api.Scene(SB.scene_c4(a.tris, 64, 64, 1).finish())
@@ -100,6 +115,7 @@ def main():
     print("  hit fraction %.3f, records equal trb_intersect's (t, inst): %s" % (res["hit_fraction"], res["records_match_trb_intersect"]))
     illumination_vs_render(a, res)
     shading_queries(a, res)
+    film_writes(a, res)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         json.dump(res, open(a.out, "w"), indent=1)
@@ -263,6 +279,62 @@ def shading_queries(a, res):
         for name, x in r["results"].items():
             print("  %-40s %8.3f ms  %8.1f Mqueries/s  %7.1f GB/s (%.1f%% of %.0f GB/s HBM)" % (name, x["ms"], x["mqueries_per_s"], x["gb_per_s"],
                                                                                            100 * x["hbm_fraction"], HBM_PEAK_GBS))
+
+
+def time_film_write(call, s, reps, T):
+    """median over reps of: the call's GPU time between CUDA events, and its sort / gather kernel times from torch.profiler"""
+    from torch.profiler import ProfilerActivity, profile
+    call()  # warm-up: grows the scene's sort scratch
+    s.synchronize()
+    tot, sort, gather = [], [], []
+    for _ in range(reps):
+        e0, e1 = T.cuda.Event(enable_timing=True), T.cuda.Event(enable_timing=True)
+        e0.record(s)
+        call()
+        e1.record(s)
+        s.synchronize()
+        tot.append(e0.elapsed_time(e1))
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            call()
+            s.synchronize()
+        k = [(e.key, getattr(e, "device_time_total", 0.0) / 1e3) for e in prof.key_averages()]  # us -> ms
+        gather.append(sum(ms for name, ms in k if "k_film_gather" in name))
+        sort.append(sum(ms for name, ms in k if "k_film_keys" in name or "k_film_starts" in name or "cub" in name.lower()))
+    return {"ms": float(np.median(tot)), "sort_ms": float(np.median(sort)), "gather_ms": float(np.median(gather))}
+
+
+def film_writes(a, res):
+    import torch as T
+    dev = T.device("cuda:0")
+    g = api.Scene(SB.scene_c4(a.tris, a.width, a.height, a.film_spp).finish())
+    g.update_frame(0, 0.0, 0.0)
+    samples, _ = g.render_samples(seed=1)
+    regions = g.sample_regions()
+    n = len(samples)
+    d_s = T.from_numpy(samples.view(np.float32).reshape(-1, 5).copy()).to(dev)
+    d_r = T.from_numpy(regions.view(np.int32).copy()).to(dev)
+    d_film = T.zeros((g.height, g.width, 4), dtype=T.float32, device=dev)
+    s = T.cuda.Stream()
+    s.wait_stream(T.cuda.current_stream())
+    frame = time_film_write(lambda: g.film_write_device(n, d_s.data_ptr(), d_r.data_ptr(), d_film.data_ptr(), s.cuda_stream), s, a.reps, T)
+    frame.update(samples=n, msamples_per_s=n / frame["ms"] / 1e3)
+    m = 1 << 20
+    rng = np.random.default_rng(0xF1)
+    one = np.zeros(m, F.SAMPLE_DTYPE)
+    bx, by = (a.width // 16) * 8, (a.height // 16) * 8
+    one["x"], one["y"] = rng.uniform(bx, bx + 8, m), rng.uniform(by, by + 8, m)
+    for k in ("r", "g", "b"):
+        one[k] = rng.uniform(0, 1, m)
+    d_s1 = T.from_numpy(one.view(np.float32).reshape(-1, 5).copy()).to(dev)
+    d_r1 = T.full((m,), (by // 8) * (a.width // 8) + bx // 8, dtype=T.int32, device=dev)
+    single = time_film_write(lambda: g.film_write_device(m, d_s1.data_ptr(), d_r1.data_ptr(), d_film.data_ptr(), s.cuda_stream), s, a.reps, T)
+    single.update(samples=m, msamples_per_s=m / single["ms"] / 1e3)
+    g.check_error()
+    res["film_write"] = {"c4_frame": frame, "one_region": single, "width": a.width, "height": a.height, "spp": a.film_spp}
+    print("  trb_film_write_device, median of %d:" % a.reps)
+    for name, x in (("C4 %dx%d, %d spp" % (a.width, a.height, a.film_spp), frame), ("one region", single)):
+        print("  %-40s %8.3f ms (sort %.3f, gather %.3f)  %8.1f M samples/s  (%d samples)" % (name, x["ms"], x["sort_ms"], x["gather_ms"],
+                                                                                            x["msamples_per_s"], x["samples"]))
 
 
 if __name__ == "__main__":

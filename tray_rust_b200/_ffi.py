@@ -211,6 +211,7 @@ TRB_SYMBOLS = [
     "trb_illumination", "trb_illumination_device",
     "trb_bsdf_eval", "trb_bsdf_eval_device", "trb_bsdf_sample", "trb_bsdf_sample_device", "trb_light_sample", "trb_light_sample_device",
     "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
+    "trb_film_write", "trb_film_write_device", "trb_camera_rays_device",
 ]
 
 _trb = None
@@ -261,6 +262,9 @@ def load_trb():
     lib.trb_emitted_device.argtypes = [vp, sz, vp, vp, vp]
     lib.trb_scene_lights.argtypes = [vp, vp]
     lib.trb_camera_rays.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp]
+    lib.trb_camera_rays_device.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp, vp]
+    lib.trb_film_write.argtypes = [vp, sz, vp, vp, vp]
+    lib.trb_film_write_device.argtypes = [vp, sz, vp, vp, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]

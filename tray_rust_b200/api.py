@@ -66,6 +66,17 @@ class _Base:
         self._check(getattr(self._lib, self._pfx + "block_list")(self._h, start, count, C.byref(m), F.ptr(xy), n))
         return xy
 
+    def sample_regions(self, **kw):
+        """The region (8x8 block index by * (width / 8) + bx) of every camera sample of the selection, in the order of
+        render_samples / camera_rays: what film_write needs to write those samples as the render does."""
+        cfg = _cfg(**kw)
+        xy = self.block_list(cfg.block_start, cfg.block_count)
+        if cfg.shard_count > 1:
+            ch = max(1, cfg.shard_chunk)
+            xy = xy[[(j // ch) % cfg.shard_count == cfg.shard_index for j in range(len(xy))]]
+        per_block = self._n_samples(cfg) // max(1, len(xy))
+        return np.repeat(xy[:, 1] * np.uint32(self.width // 8) + xy[:, 0], per_block).astype(np.uint32)
+
     def bvh(self, which=-1):
         nn, no = F.u32(), F.u32()
         f = getattr(self._lib, self._pfx + "scene_get_bvh")
@@ -192,6 +203,34 @@ class Scene(_Base):
         rays, xy = np.zeros(n, F.RAY_DTYPE), np.zeros((n, 2), np.float32)
         self._check(self._lib.trb_camera_rays(self._h, C.byref(cfg), n, F.ptr(rays), F.ptr(xy)))
         return rays, xy
+
+    def camera_rays_device(self, d_rays, d_xy, stream=None, **kw):
+        """trb_camera_rays_device: the camera rays (RAY_DTYPE, 32 B) and film positions (2 float32) of the selection into device
+        buffers of n = blocks * 64 * sample_count records (4-byte aligned), enqueued on `stream` (a cudaStream_t as an int; None =
+        default stream) without host synchronisation. Returns n."""
+        cfg = _cfg(**kw)
+        n = self._n_samples(cfg)
+        self._check(self._lib.trb_camera_rays_device(self._h, C.byref(cfg), n, d_rays, d_xy, stream))
+        return n
+
+    def film_write(self, samples, regions, film=None):
+        """trb_film_write: RenderTarget::write once per region that has samples, regions in Morton-list order, each region's
+        samples (SAMPLE_DTYPE) in input order; regions[i] is the 8x8 block index of sample i (sample_regions() for render_samples'
+        order; an index >= total_blocks skips the sample). `film` (height, width, 4) float32 is added into in place; a zero film
+        when None. Returns the film. Bit-reproducible: no float atomics."""
+        samples = np.ascontiguousarray(samples, dtype=F.SAMPLE_DTYPE)
+        regions = np.ascontiguousarray(regions, dtype=np.uint32)
+        assert len(samples) == len(regions)
+        if film is None:
+            film = np.zeros((self.height, self.width, 4), np.float32)
+        assert film.dtype == np.float32 and film.flags.c_contiguous and film.size == self.height * self.width * 4
+        self._check(self._lib.trb_film_write(self._h, len(samples), F.ptr(samples), F.ptr(regions), F.ptr(film)))
+        return film
+
+    def film_write_device(self, n, d_samples, d_regions, d_film, stream=None):
+        """trb_film_write_device: n samples (20 B), n uint32 regions and the RGBW film, device buffers 4-byte aligned, enqueued on
+        `stream` without host synchronisation (except once, when the scene's sort scratch grows)."""
+        self._check(self._lib.trb_film_write_device(self._h, n, d_samples, d_regions, d_film, stream))
 
     def intersect(self, rays):
         rays = np.ascontiguousarray(rays, dtype=F.RAY_DTYPE)

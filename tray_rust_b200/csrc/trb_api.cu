@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <memory>
 #include <thread>
+#include <cub/device/device_radix_sort.cuh>
 #include "trb_host.h"
 #include "trb_kernels.cuh"
 
@@ -262,9 +263,12 @@ struct trb_scene {
     uint32_t* d_ad_flags = nullptr;
     uint32_t* d_ad_count = nullptr;
     uint32_t* d_ad_spp = nullptr;
+    // caller film writes (trb_film_write): sort keys and sample order (double-buffered), region starts, CUB's temporary storage
+    void* d_film_scratch = nullptr;
+    size_t film_scratch_bytes = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
-                        (void*)d_ad_count, (void*)d_ad_spp}) if (p) cudaFree(p);
+                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -1033,6 +1037,76 @@ trb_status launch_light_pdf(trb_scene* s, size_t n, const trb_light_pdf_query* d
 trb_status launch_emitted(trb_scene* s, size_t n, const trb_emit_query* d_q, float* d_rgb, cudaStream_t st) {
     if (s->ds.has_anim || s->anim_emission) trb::k_emitted<true><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_rgb);
     else trb::k_emitted<false><<<shade_grid(s, n), 128, 0, st>>>(s->ds, n, d_q, d_rgb);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// ---- caller film writes (trb_film_write / trb_film_write_device; DESIGN.md §5) --------------------------------------------------
+// Argument checks, before anything is read: n < 2^32 (the sort and the region starts index with 32 bits), buffers present when
+// n > 0, device buffers 4-byte aligned.
+trb_status film_check(const trb_scene* s, size_t n, const void* samples, const void* regions, const void* film, bool device) {
+    if (!s) return fail(TRB_INVALID_ARG, "null argument");
+    if ((uint64_t)n >= (1ull << 32)) return fail(TRB_INVALID_ARG, "film writes take fewer than 2^32 samples");
+    if (n && (!samples || !regions || !film)) return fail(TRB_INVALID_ARG, "null argument");
+    if (device && n && ((reinterpret_cast<uintptr_t>(samples) | reinterpret_cast<uintptr_t>(regions) | reinterpret_cast<uintptr_t>(film)) & 3u))
+        return fail(TRB_INVALID_ARG, "device film-write buffers must be 4-byte aligned");
+    return TRB_OK;
+}
+
+// Enqueue one film write on `st`: keys, a stable radix sort of the sample order by region (CUB; its kernels are not counted in
+// g_launches), region starts, the gather. The scratch space is per scene and only grows; growing it drains the device once. There
+// is no splitting into passes: a split would change the order of the additions, so a write that does not fit is TRB_OOM.
+trb_status film_write_enqueue(trb_scene* s, uint32_t n, const trb_sample* d_samples, const uint32_t* d_regions, float* d_film, cudaStream_t st) {
+    const uint32_t nr = (s->film.width / 8) * (s->film.height / 8);
+    const int bits = 32 - __builtin_clz(nr); // keys are 0 .. nr (nr = out of range)
+    size_t temp = 0;
+    cub::DoubleBuffer<uint32_t> keys(nullptr, nullptr), order(nullptr, nullptr);
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, temp, keys, order, n, 0, bits, st));
+    const size_t a = ((size_t)n * 4 + 255) / 256 * 256, sb = ((size_t)(nr + 1) * 4 + 255) / 256 * 256;
+    const size_t need = 4 * a + sb + temp;
+    if (need > s->film_scratch_bytes) {
+        CU(cudaDeviceSynchronize()); // a write still in flight owns the old scratch
+        cudaFree(s->d_film_scratch);
+        s->d_film_scratch = nullptr; s->film_scratch_bytes = 0;
+        const cudaError_t e = cudaMalloc(&s->d_film_scratch, need);
+        if (e != cudaSuccess) { cudaGetLastError(); s->d_film_scratch = nullptr; CU(e); }
+        s->film_scratch_bytes = need;
+    }
+    char* base = static_cast<char*>(s->d_film_scratch);
+    uint32_t* k0 = reinterpret_cast<uint32_t*>(base);
+    uint32_t* o0 = reinterpret_cast<uint32_t*>(base + 2 * a);
+    keys = cub::DoubleBuffer<uint32_t>(k0, reinterpret_cast<uint32_t*>(base + a));
+    order = cub::DoubleBuffer<uint32_t>(o0, reinterpret_cast<uint32_t*>(base + 3 * a));
+    uint32_t* d_start = reinterpret_cast<uint32_t*>(base + 4 * a);
+    trb::k_film_keys<<<(unsigned)std::min<size_t>(((size_t)n + 255) / 256, (size_t)s->sm_count * 8), 256, 0, st>>>(n, d_regions, nr, k0, o0);
+    g_launches++;
+    CU(cudaGetLastError());
+    CU(cub::DeviceRadixSort::SortPairs(base + 4 * a + sb, temp, keys, order, n, 0, bits, st));
+    trb::k_film_starts<<<(nr + 1 + 255) / 256, 256, 0, st>>>(n, keys.Current(), nr, d_start);
+    g_launches++;
+    CU(cudaGetLastError());
+    trb::k_film_gather<<<nr, trb::FILM_WRITE_THREADS, 0, st>>>(s->ds, d_samples, order.Current(), d_start, d_film);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// k_camera_rays over the selection of cfg into device buffers of n = blocks * 64 * sample_count records, enqueued on st
+trb_status camera_rays_enqueue(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_ray* d_rays, float* d_xy, cudaStream_t st) {
+    uint32_t spp, first, count, nb;
+    const uint2* d_blocks = nullptr;
+    trb_status r = resolve_samples(s, cfg, spp, first, count);
+    if (r != TRB_OK) return r;
+    r = ensure_blocks(s, cfg, &d_blocks, &nb);
+    if (r != TRB_OK) return r;
+    if (n != (size_t)nb * 64 * count) return fail(TRB_INVALID_ARG, "ray buffer size must be blocks*64*sample_count");
+    if (n == 0) return TRB_OK;
+    trb::RenderParams rp{};
+    rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
+    const unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)s->sm_count * 8);
+    if (s->ds.has_anim) trb::k_camera_rays<true><<<grid, 256, 0, st>>>(s->ds, rp, d_rays, d_xy);
+    else trb::k_camera_rays<false><<<grid, 256, 0, st>>>(s->ds, rp, d_rays, d_xy);
     g_launches++;
     CU(cudaGetLastError());
     return TRB_OK;
@@ -1902,6 +1976,44 @@ trb_status trb_scene_lights(const trb_scene* s, uint32_t* inst) {
     uint32_t k = 0;
     for (uint32_t i = 0; i < (uint32_t)s->instances.size(); ++i) if (s->instances[i].kind != TRB_INST_RECEIVER) inst[k++] = i; // as trb_scene_create builds ds.lights
     return TRB_OK;
+}
+
+trb_status trb_film_write(trb_scene* s, size_t n, const trb_sample* samples, const uint32_t* regions, float* film_rgbw) {
+    const trb_status r = film_check(s, n, samples, regions, film_rgbw, false);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t film_bytes = (size_t)s->film.width * s->film.height * 4 * sizeof(float);
+    const size_t r_off = (n * sizeof(trb_sample) + 255) / 256 * 256, f_off = r_off + (n * sizeof(uint32_t) + 255) / 256 * 256;
+    char* d = nullptr;
+    CU(cudaMalloc(&d, f_off + film_bytes));
+    cudaError_t e = cudaMemcpy(d, samples, n * sizeof(trb_sample), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d + r_off, regions, n * sizeof(uint32_t), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(d + f_off, film_rgbw, film_bytes, cudaMemcpyHostToDevice);
+    trb_status st = TRB_OK;
+    if (e == cudaSuccess)
+        st = film_write_enqueue(s, (uint32_t)n, reinterpret_cast<const trb_sample*>(d), reinterpret_cast<const uint32_t*>(d + r_off),
+                                reinterpret_cast<float*>(d + f_off), 0);
+    if (e == cudaSuccess && st == TRB_OK) e = cudaMemcpy(film_rgbw, d + f_off, film_bytes, cudaMemcpyDeviceToHost);
+    if (st != TRB_OK) cudaDeviceSynchronize();
+    cudaFree(d);
+    if (st != TRB_OK) return st;
+    CU(e);
+    return TRB_OK;
+}
+
+trb_status trb_film_write_device(trb_scene* s, size_t n, const trb_sample* d_samples, const uint32_t* d_regions, float* d_film_rgbw, void* stream) {
+    const trb_status r = film_check(s, n, d_samples, d_regions, d_film_rgbw, true);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return film_write_enqueue(s, (uint32_t)n, d_samples, d_regions, d_film_rgbw, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_camera_rays_device(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_ray* d_rays, float* d_xy, void* stream) {
+    if (!s || !cfg || (n && (!d_rays || !d_xy))) return fail(TRB_INVALID_ARG, "null argument");
+    if (((reinterpret_cast<uintptr_t>(d_rays) | reinterpret_cast<uintptr_t>(d_xy)) & 3u)) return fail(TRB_INVALID_ARG, "device ray buffers must be 4-byte aligned");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    CU(cudaSetDevice(s->device));
+    return camera_rays_enqueue(s, cfg, n, d_rays, d_xy, static_cast<cudaStream_t>(stream));
 }
 
 trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {

@@ -3310,4 +3310,118 @@ __global__ void k_ad_pixel_spp(const __grid_constant__ DScene sc, const uint2* b
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Caller film writes (trb_film_write; DESIGN.md §5): RenderTarget::write (render_target.rs:77-165) once per region that has
+// samples, regions in Morton-list order, each region's samples in input order — without float atomics. The samples are
+// stable-sorted by region (CUB radix sort, launched from trb_api.cu), then one CTA per target 8x8 block gathers, for each of
+// its 64 pixels (one owner thread each), the sum S_r of every candidate region r in Morton order and adds it to the film.
+// ------------------------------------------------------------------------------------------
+// Sort keys: the sample's region, or n_regions for a region out of range (sorted last, never written); values: input positions.
+__global__ void k_film_keys(uint32_t n, const uint32_t* __restrict__ regions, uint32_t n_regions, uint32_t* __restrict__ keys,
+                            uint32_t* __restrict__ order) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const uint32_t r = regions[i];
+        keys[i] = r < n_regions ? r : n_regions;
+        order[i] = i;
+    }
+}
+
+// start[r] = the first sorted position whose key is >= r, for r in [0, n_regions]: region r's samples are [start[r], start[r + 1]).
+__global__ void k_film_starts(uint32_t n, const uint32_t* __restrict__ keys, uint32_t n_regions, uint32_t* __restrict__ start) {
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r <= n_regions; r += gridDim.x * blockDim.x) {
+        uint32_t lo = 0, hi = n;
+        while (lo < hi) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            if (keys[mid] < r) lo = mid + 1; else hi = mid;
+        }
+        start[r] = lo;
+    }
+}
+
+// morton.rs: the Morton code of block (x, y). Codes of distinct blocks differ, so ordering blocks by code is their order in
+// BlockQueue::new's stably sorted list (block_queue.rs:28-46).
+__device__ __forceinline__ uint32_t morton_block(uint32_t x, uint32_t y) {
+    auto part = [](uint32_t v) {
+        v &= 0x0000ffffu; v = (v ^ (v << 8)) & 0x00ff00ffu; v = (v ^ (v << 4)) & 0x0f0f0f0fu;
+        v = (v ^ (v << 2)) & 0x33333333u; return (v ^ (v << 1)) & 0x55555555u;
+    };
+    return (part(y) << 1) + part(x);
+}
+
+constexpr int FILM_WRITE_THREADS = 64; // one thread per pixel of the target block
+constexpr int FILM_CHUNK = 512;        // samples staged in shared memory at a time
+
+// One CTA per target 8x8 block. Candidate regions are those whose write range [start - fpw, start + 8 + fpw] (inclusive,
+// clipped to the image; render_target.rs:79-82) reaches the block: the 3x3 neighbours for fpw <= 7, 4x4 (two blocks to the
+// left and above) for fpw = 8. Per candidate with samples, each pixel inside its write range sums weight * c and weight over
+// the region's samples in input order (the lock-block test of render_target.rs:105-110 always applies here: caller positions
+// may be anywhere, NaN included), then adds that sum to its film value, as RenderTarget::write adds filtered_samples.
+__global__ void __launch_bounds__(FILM_WRITE_THREADS) k_film_gather(const __grid_constant__ DScene sc, const trb_sample* __restrict__ samples,
+                                                                    const uint32_t* __restrict__ order, const uint32_t* __restrict__ start,
+                                                                    float* __restrict__ film) {
+    __shared__ float s_table[256];
+    __shared__ float s_x[FILM_CHUNK], s_y[FILM_CHUNK], s_r[FILM_CHUNK], s_g[FILM_CHUNK], s_b[FILM_CHUNK];
+    __shared__ uint32_t s_cand[16], s_code[16];
+    __shared__ int s_ncand;
+    const uint32_t nbx = sc.width / 8, nby = sc.height / 8;
+    const uint32_t tbx = blockIdx.x % nbx, tby = blockIdx.x / nbx;
+    for (int i = threadIdx.x; i < 256; i += FILM_WRITE_THREADS) s_table[i] = sc.filter_table[i];
+    if (threadIdx.x == 0) { // the candidate regions with samples, sorted by Morton code (insertion sort of at most 16)
+        int nc = 0;
+        const uint32_t bx0 = (uint32_t)max((int)tbx - (8 + sc.fpw_x) / 8, 0), bx1 = min(tbx + (uint32_t)(7 + sc.fpw_x) / 8, nbx - 1);
+        const uint32_t by0 = (uint32_t)max((int)tby - (8 + sc.fpw_y) / 8, 0), by1 = min(tby + (uint32_t)(7 + sc.fpw_y) / 8, nby - 1);
+        for (uint32_t by = by0; by <= by1; ++by)
+            for (uint32_t bx = bx0; bx <= bx1; ++bx) {
+                const uint32_t r = by * nbx + bx;
+                if (start[r + 1] == start[r]) continue; // no samples: RenderTarget::write is not called for it
+                const uint32_t code = morton_block(bx, by);
+                int k = nc++;
+                for (; k > 0 && s_code[k - 1] > code; --k) { s_code[k] = s_code[k - 1]; s_cand[k] = s_cand[k - 1]; }
+                s_code[k] = code; s_cand[k] = r;
+            }
+        s_ncand = nc;
+    }
+    __syncthreads();
+    const int ix = (int)(tbx * 8 + (threadIdx.x & 7)), iy = (int)(tby * 8 + (threadIdx.x >> 3));
+    float* px = film + ((size_t)iy * sc.width + ix) * 4;
+    float f0 = px[0], f1 = px[1], f2 = px[2], f3v = px[3];
+    bool touched = false;
+    const int nc = s_ncand;
+    for (int c = 0; c < nc; ++c) {
+        const uint32_t r = s_cand[c];
+        const int rx = (int)(r % nbx) * 8, ry = (int)(r / nbx) * 8;
+        const int x_lo = max(rx - sc.fpw_x, 0), x_hi = min(rx + 8 + sc.fpw_x, (int)sc.width - 1);
+        const int y_lo = max(ry - sc.fpw_y, 0), y_hi = min(ry + 8 + sc.fpw_y, (int)sc.height - 1);
+        const bool in = ix >= x_lo && ix <= x_hi && iy >= y_lo && iy <= y_hi;
+        float a0 = 0.0f, a1 = 0.0f, a2 = 0.0f, a3 = 0.0f; // filtered_samples[px] (render_target.rs:112-114)
+        const uint32_t s0 = start[r], s1 = start[r + 1];
+        for (uint32_t b = s0; b < s1; b += FILM_CHUNK) {
+            const uint32_t cnt = min(s1 - b, (uint32_t)FILM_CHUNK);
+            __syncthreads();
+            for (uint32_t j = threadIdx.x; j < cnt; j += FILM_WRITE_THREADS) {
+                const trb_sample* sp = samples + order[b + j];
+                s_x[j] = sp->x; s_y[j] = sp->y; s_r[j] = sp->r; s_g[j] = sp->g; s_b[j] = sp->b;
+            }
+            __syncthreads();
+            if (!in) continue;
+            for (uint32_t j = 0; j < cnt; ++j) {
+                const float sx = s_x[j], sy = s_y[j];
+                if (!lock_block_takes(sx, ix, x_lo, x_hi, sc.fpw_x) || !lock_block_takes(sy, iy, y_lo, y_hi, sc.fpw_y)) continue;
+                const float fy = fabsf((float)iy - (sy - 0.5f)) * sc.filter_inv_h;
+                if (fy > sc.filter_h) continue; // sic: normalised distance vs width (A7)
+                const float fx = fabsf((float)ix - (sx - 0.5f)) * sc.filter_inv_w;
+                if (fx > sc.filter_w) continue;
+                const uint32_t fyi = min(f2u(fy * 16.0f), 15u), fxi = min(f2u(fx * 16.0f), 15u);
+                const float wgt = s_table[fyi * 16 + fxi];
+                a0 += wgt * s_r[j];
+                a1 += wgt * s_g[j];
+                a2 += wgt * s_b[j];
+                a3 += wgt;
+            }
+        }
+        if (in) { f0 += a0; f1 += a1; f2 += a2; f3v += a3; touched = true; } // pixels[px] += filtered_samples[px] (:153-161)
+    }
+    if (touched) { px[0] = f0; px[1] = f1; px[2] = f2; px[3] = f3v; }
+}
+
 } // namespace trb
