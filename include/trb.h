@@ -634,6 +634,12 @@ trb_status trb_film_write_device(trb_scene* scene, size_t n, const trb_sample* d
  * (c*255) as u8; pixels with weight <= 0 stay 0. Host buffers; runs on the scene's GPU. */
 trb_status trb_film_to_srgb8(trb_scene* scene, const float* film_rgbw, uint8_t* rgb8);
 
+/* The same conversion on the host, with no scene and no device: ≙ Image::get_srgb8 (film/image.rs:53-67), which the distributed
+ * master applies to the blocks its workers sent. film_rgbw holds width*height RGBW pixels, rgb8 receives width*height*3 bytes.
+ * The bytes equal trb_film_to_srgb8's for the same film, bit for bit (one per-pixel function compiled for both sides), including
+ * weights <= 0 or NaN (black), infinities and NaN colours. TRB_INVALID_ARG for null buffers with width*height > 0. */
+trb_status trb_host_film_to_srgb8(uint32_t width, uint32_t height, const float* film_rgbw, uint8_t* rgb8);
+
 /* ≙ image::save_buffer(path, &img, w, h, image::RGB(8)) for the frames written by main.rs:95-103 and by the distributed
  * master (exec/distrib/master.rs:137-142): an 8-bit RGB PNG (stored deflate blocks; host only, no device needed). */
 trb_status trb_write_png(const char* path, const uint8_t* rgb8, uint32_t width, uint32_t height);

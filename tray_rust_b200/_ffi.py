@@ -211,7 +211,7 @@ TRB_SYMBOLS = [
     "trb_illumination", "trb_illumination_device",
     "trb_bsdf_eval", "trb_bsdf_eval_device", "trb_bsdf_sample", "trb_bsdf_sample_device", "trb_light_sample", "trb_light_sample_device",
     "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
-    "trb_film_write", "trb_film_write_device", "trb_camera_rays_device",
+    "trb_film_write", "trb_film_write_device", "trb_camera_rays_device", "trb_host_film_to_srgb8",
 ]
 
 _trb = None
@@ -272,6 +272,7 @@ def load_trb():
     lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
     lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]
+    lib.trb_host_film_to_srgb8.argtypes = [u32, u32, vp, vp]
     lib.trb_block_list.argtypes = [vp, u32, u32, C.POINTER(u32), vp, u32]
     lib.trb_scene_get_bvh.argtypes = [vp, C.c_int, C.POINTER(u32), vp, C.POINTER(u32), vp]
     lib.trb_scene_get_transform.argtypes = [vp, u32, vp, vp]

@@ -35,6 +35,20 @@ def adaptive_schedule(min_spp, max_spp):
     return tuple(x.value for x in out)
 
 
+def film_to_srgb8(film):
+    """trb_host_film_to_srgb8: Image::get_srgb8 of an RGBW film of shape (height, width, 4) on the host, without a scene or a GPU.
+    Returns (height, width, 3) uint8, the same bytes as Scene.to_srgb8 of the same film."""
+    film = np.ascontiguousarray(film, dtype=np.float32)
+    if film.ndim != 3 or film.shape[2] != 4:
+        raise ValueError("film must have shape (height, width, 4)")
+    lib = F.load_trb()
+    out = np.zeros(film.shape[:2] + (3,), np.uint8)
+    rc = lib.trb_host_film_to_srgb8(film.shape[1], film.shape[0], F.ptr(film), F.ptr(out))
+    if rc != F.TRB_OK:
+        raise TrbError(rc, (lib.trb_last_error() or b"").decode())
+    return out
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
 

@@ -2033,6 +2033,13 @@ trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {
     return TRB_OK;
 }
 
+trb_status trb_host_film_to_srgb8(uint32_t width, uint32_t height, const float* film, uint8_t* rgb8) {
+    const size_t npx = (size_t)width * height;
+    if (npx && (!film || !rgb8)) return fail(TRB_INVALID_ARG, "null argument");
+    for (size_t i = 0; i < npx; ++i) trb::srgb8_pixel(film[4 * i], film[4 * i + 1], film[4 * i + 2], film[4 * i + 3], rgb8 + 3 * i);
+    return TRB_OK;
+}
+
 trb_status trb_block_list(const trb_scene* s, uint32_t start, uint32_t count, uint32_t* n_out, uint32_t* xy, uint32_t cap) {
     if (!s || !n_out) return fail(TRB_INVALID_ARG, "null argument");
     std::vector<uint32_t> b = morton_blocks(s->film.width, s->film.height, start, count);

@@ -7,7 +7,8 @@
 // beckmann.rs:35-46, src/bxdf/merl.rs:62-75); libdevice and glibc differ in the last ulp, so this
 // translation unit is compiled with --fmad=false and evaluates these fixed polynomial sequences
 // (Cephes single-precision kernels) instead, which makes every camera sample reproducible on any
-// IEEE machine. Written for sm_90a; nothing here is shared with oracle/.
+// IEEE machine. Written for sm_90a; nothing here is shared with oracle/. The TRB_DM functions compile for the host as well,
+// with the same operations, so host code that calls them (trb_host_film_to_srgb8) gets the device's bits.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -30,7 +31,14 @@ TRB_DM float bits_f32(uint32_t u) {
     float f; memcpy(&f, &u, 4); return f;
 #endif
 }
-__device__ __forceinline__ float pow2i(int k) { return __uint_as_float((uint32_t)(k + 127) << 23); }
+TRB_DM uint32_t f32_bits(float f) {
+#ifdef __CUDA_ARCH__
+    return __float_as_uint(f);
+#else
+    uint32_t u; memcpy(&u, &f, 4); return u;
+#endif
+}
+TRB_DM float pow2i(int k) { return bits_f32((uint32_t)(k + 127) << 23); }
 
 // Cody-Waite reduction to [-pi/4, pi/4]; quadrant in q. |x| <= 1e5.
 TRB_DM float reduce_pio2(float x, int& q) {
@@ -97,9 +105,9 @@ __device__ __forceinline__ float datan2(float y, float x) {
     if (x < 0.0f) a = TRB_PI - a;
     return y < 0.0f ? -a : a;
 }
-__device__ __forceinline__ float dexp(float x) {
+TRB_DM float dexp(float x) {
     if (x != x) return x;
-    if (x > 88.72283905206835f) return __int_as_float(0x7f800000);
+    if (x > 88.72283905206835f) return bits_f32(0x7f800000u);
     if (x < -87.33654475055310f) return 0.0f;
     float kf = floorf(1.44269504088896341f * x + 0.5f);
     float r = x - kf * 0.693359375f;
@@ -110,16 +118,16 @@ __device__ __forceinline__ float dexp(float x) {
     if (k > 127) { p = p * 2.0f; k -= 1; }
     return p * pow2i(k);
 }
-__device__ __forceinline__ float dlog(float x) {
+TRB_DM float dlog(float x) {
     if (x != x) return x;
-    if (x < 0.0f) return x - x + __int_as_float(0x7fc00000);
-    if (x == 0.0f) return __int_as_float(0xff800000);
-    if (x == __int_as_float(0x7f800000)) return x;
+    if (x < 0.0f) return x - x + bits_f32(0x7fc00000u);
+    if (x == 0.0f) return bits_f32(0xff800000u);
+    if (x == bits_f32(0x7f800000u)) return x;
     int e = 0;
     if (x < 1.17549435e-38f) { x = x * 8388608.0f; e = -23; }
-    uint32_t b = __float_as_uint(x);
+    uint32_t b = f32_bits(x);
     e += (int)((b >> 23) & 0xffu) - 126;
-    float m = __uint_as_float((b & 0x007fffffu) | 0x3f000000u);
+    float m = bits_f32((b & 0x007fffffu) | 0x3f000000u);
     if (m < 0.707106781186547524f) { e -= 1; m = m + m - 1.0f; }
     else { m = m - 1.0f; }
     float z = m * m;
@@ -131,7 +139,7 @@ __device__ __forceinline__ float dlog(float x) {
     z = z + 0.693359375f * fe;
     return z;
 }
-__device__ __forceinline__ float dpow(float x, float y) { return dexp(y * dlog(x)); }
+TRB_DM float dpow(float x, float y) { return dexp(y * dlog(x)); }
 
 // ---- counter RNG ---------------------------------------------------------------------
 __host__ __device__ __forceinline__ uint32_t mix32(uint32_t x) {
@@ -194,6 +202,32 @@ __host__ __device__ __forceinline__ float ld_sobol(uint32_t n, uint32_t scramble
         i ^= i >> 1;
     }
     return fminf((float)((scramble >> 8) & 0xffffffu) / 16777216.0f, 1.0f - TRB_EPS);
+}
+
+// Rust `f as usize` into 32 bits: truncation toward zero, saturating, NaN -> 0
+TRB_DM uint32_t f2u(float f) {
+#ifdef __CUDA_ARCH__
+    return __float2uint_rz(f);
+#else
+    return f != f || f <= 0.0f ? 0u : (f >= 4294967296.0f ? 0xffffffffu : (uint32_t)f);
+#endif
+}
+
+// One pixel of RenderTarget::get_render (render_target.rs:185-210) and of the master's Image::get_srgb8 (film/image.rs:53-67),
+// with Colorf::clamp and Colorf::to_srgb (color.rs:36-72): rgb / weight, clamped to [0, 1], sRGB, then (c * 255) as u8. A pixel
+// whose weight is not > 0 stays black. k_srgb8 (trb_film_to_srgb8) and trb_host_film_to_srgb8 both call this, so the device and
+// the host convert a film to the same bytes.
+TRB_DM void srgb8_pixel(float r, float g, float b, float w, uint8_t* o) {
+    o[0] = 0; o[1] = 0; o[2] = 0;
+    if (w > 0.0f) {
+        const float v[3] = {r / w, g / w, b / w};
+        for (int k = 0; k < 3; ++k) {
+            const float x = v[k] < 0.0f ? 0.0f : (v[k] > 1.0f ? 1.0f : v[k]);
+            const float s = x <= 0.0031308f ? 12.92f * x : (1.0f + 0.055f) * dpow(x, 1.0f / 2.4f) - 0.055f;
+            const float q = s * 255.0f;
+            o[k] = (uint8_t)f2u(q > 255.0f ? 255.0f : q);
+        }
+    }
 }
 
 } // namespace trb

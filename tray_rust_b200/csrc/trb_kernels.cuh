@@ -48,7 +48,6 @@ __device__ __forceinline__ f3 unit(f3 a) { float l = ieee_sqrt(len2(a)); return 
 __device__ __forceinline__ bool black(f3 c) { return c.x == 0.0f && c.y == 0.0f && c.z == 0.0f; }
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return x < lo ? lo : (x > hi ? hi : x); }
 __device__ __forceinline__ float lerpf(float t, float a, float b) { return a * (1.0f - t) + b * t; }
-__device__ __forceinline__ uint32_t f2u(float f) { return __float2uint_rz(f); } // saturating, NaN -> 0 (Rust `as usize`)
 __device__ __forceinline__ float finf() { return __int_as_float(0x7f800000); }
 
 // Transform application (src/linalg/transform.rs:150-254), m row-major 4x4
@@ -119,13 +118,6 @@ TRB_HD __forceinline__ bool box_hit(const float4 lo, const float4 hi, f3 o, f3 i
 // slot hit in that order (QUAD_EMPTY if none); the other hit slots come back farthest-first in e[0..2] so that the
 // caller pushes them in this order and they pop nearest-first. Each entry = entry distance << 32 | reference.
 // Host+device: trb_host_quad_check runs this very function against a literal bvh.rs:81-130 traversal.
-TRB_HD __forceinline__ uint32_t f32_bits(float f) {
-#ifdef __CUDA_ARCH__
-    return __float_as_uint(f);
-#else
-    uint32_t u; memcpy(&u, &f, 4); return u;
-#endif
-}
 struct QuadOut { uint32_t next; unsigned long long e0, e1, e2; bool p0, p1, p2; };
 TRB_HD __forceinline__ void quad_visit(const float4 q0, const float4 q1, const float4 q2, const float4 q3, const float4 q4, const float4 q5, const float4 q6,
                                        const float4 q7, f3 o, f3 inv, bool nx, bool ny, bool nz, float tmin, float tmax, QuadOut& out) {
@@ -3156,16 +3148,8 @@ __global__ void k_tlas_build(const __grid_constant__ FrameBuild fb) {
 __global__ void k_srgb8(size_t n, const float4* __restrict__ film, uint8_t* __restrict__ rgb8) {
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const float4 c = film[i];
-        uint8_t o[3] = {0, 0, 0};
-        if (c.w > 0.0f) {
-            const float v[3] = {c.x / c.w, c.y / c.w, c.z / c.w};
-            for (int k = 0; k < 3; ++k) {
-                const float x = clampf(v[k], 0.0f, 1.0f);
-                const float s = x <= 0.0031308f ? 12.92f * x : (1.0f + 0.055f) * dpow(x, 1.0f / 2.4f) - 0.055f;
-                const float q = s * 255.0f;
-                o[k] = (uint8_t)f2u(q > 255.0f ? 255.0f : q);
-            }
-        }
+        uint8_t o[3];
+        srgb8_pixel(c.x, c.y, c.z, c.w, o); // trb_detmath.cuh, shared with trb_host_film_to_srgb8
         rgb8[3 * i] = o[0]; rgb8[3 * i + 1] = o[1]; rgb8[3 * i + 2] = o[2];
     }
 }

@@ -1,0 +1,414 @@
+// trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
+//
+//   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D]
+//   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
+//   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
+//
+// Single node (main.rs:56-109): Scene::load_file, then for every frame of the inclusive range Exec::render (trb_render, which
+// includes update_frame), RenderTarget::get_render (trb_film_to_srgb8), write the image, clear the film.
+// Master (main.rs:111-146, exec/distrib/master.rs): reads the film section on the host only (no GPU needed), splits the Morton
+// block list B / W blocks per worker with the remainder on the last (master.rs:88-93, 217-224), connects to every worker, sends
+// each its Instructions, then collects Frames from all workers in one poll loop and adds each into its frame's image
+// (Image::add_blocks, film/image.rs:36-50) in arrival order. When all W workers have reported a frame it is converted
+// (Image::get_srgb8 == trb_host_film_to_srgb8) and written.
+// Worker: trb_worker's code (trb_distrib.hpp).
+//
+// Extensions over the reference: --seed, --spp and --device mean what they mean for trb_worker; a worker address is host[:port],
+// a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
+// frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
+// blocks) and binary PPM are written; JPEG is not built.
+// Where the reference master panics, hangs or silently misbehaves (a worker it cannot reach, a worker that hangs up early, a
+// malformed or out-of-range Frame, more workers than blocks), trb_tray exits with status 1 and a message naming the worker and
+// the frame. Without a CUDA device, single-node mode exits with status 3, like trb_worker.
+#include <netdb.h>
+#include <poll.h>
+#include <sys/stat.h>
+#include <algorithm>
+#include <cctype>
+#include <cerrno>
+#include <chrono>
+#include <cstdarg>
+#include "trb_distrib.hpp"
+#include "../../include/tray_exec.hpp"
+
+namespace {
+
+const char* USAGE =
+    "Usage:\n"
+    "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
+    "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
+    "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
+    "    trb_tray (-h | --help)\n"
+    "\n"
+    "Options:\n"
+    "  -o <path>               Output file (.png or .ppm) or directory (frames written as frame<#####>.png). Default './'.\n"
+    "  -n <number>             Accepted for compatibility with tray_rust; the GPU decides its own parallelism.\n"
+    "  --start-frame <number>  First frame to render, of the inclusive range [start, end]. Default: the scene's film.start_frame.\n"
+    "  --end-frame <number>    Last frame to render, of the inclusive range [start, end]. Default: the scene's film.end_frame.\n"
+    "  --master                Drive the workers in <workers>... (host or host:port, default port 63234) and save the frames.\n"
+    "  --worker                Listen for a master and render the blocks it assigns (the same program as trb_worker).\n"
+    "  --seed S                Random seed of the render (default 1).\n"
+    "  --spp N                 Samples per pixel, overriding the scene's film.samples.\n"
+    "  --device D              CUDA device to render on (default 0).\n"
+    "  -h, --help              Show this message.\n";
+
+int die(const char* fmt, ...) {
+    std::fputs("trb_tray: ", stderr);
+    va_list ap; va_start(ap, fmt); std::vfprintf(stderr, fmt, ap); va_end(ap);
+    std::fputc('\n', stderr);
+    return 1;
+}
+
+double seconds_since(std::chrono::steady_clock::time_point t0) { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); }
+
+bool parse_u64(const char* s, uint64_t& v) {
+    if (!s || !*s || *s == '-') return false;
+    char* e = nullptr; errno = 0;
+    const unsigned long long x = std::strtoull(s, &e, 10);
+    if (errno || *e) return false;
+    v = x; return true;
+}
+
+// -o: PathBuf::extension decides between a directory and one file (main.rs:60-73, 88-91)
+struct OutPath {
+    std::string path = "./";
+    bool is_dir = true;
+    bool ppm = false;
+    std::string file_for(uint64_t frame) const {
+        if (!is_dir) return path;
+        char name[32]; std::snprintf(name, sizeof name, "frame%05llu.png", (unsigned long long)frame);
+        return path + (path.back() == '/' ? "" : "/") + name;
+    }
+};
+
+// Path::extension: the part of the last component after its last '.', unless that dot starts the name; "." and ".." have none
+bool path_extension(const std::string& p, std::string& ext) {
+    size_t end = p.size();
+    while (end > 1 && p[end - 1] == '/') --end;
+    const size_t slash = p.rfind('/', end - 1);
+    const std::string name = p.substr(slash == std::string::npos ? 0 : slash + 1, end - (slash == std::string::npos ? 0 : slash + 1));
+    if (name.empty() || name == "." || name == "..") return false;
+    const size_t dot = name.rfind('.');
+    if (dot == std::string::npos || dot == 0) return false;
+    ext = name.substr(dot + 1);
+    return true;
+}
+
+// Checked before any scene load: an output the program cannot write is refused up front, where the reference renders every frame
+// and then prints "Error saving image" for each.
+bool resolve_out_path(const char* o, OutPath& out) {
+    if (!o) return true;
+    out.path = o;
+    std::string ext;
+    out.is_dir = !path_extension(out.path, ext);
+    if (out.is_dir) return true;
+    for (char& c : ext) c = (char)std::tolower((unsigned char)c);
+    if (ext == "png") return true;
+    if (ext == "ppm") { out.ppm = true; return true; }
+    if (ext == "jpg" || ext == "jpeg") die("cannot write '%s': JPEG output is not built; use .png or .ppm", o);
+    else die("cannot write '%s': unsupported image format '.%s'; use .png or .ppm", o, ext.c_str());
+    return false;
+}
+
+// std::fs::create_dir of the -o directory: one level; an existing one is fine
+bool create_out_dir(const OutPath& out, bool given) {
+    if (!given || !out.is_dir) return true;
+    if (::mkdir(out.path.c_str(), 0777) == 0 || errno == EEXIST) return true;
+    die("failed to create output directory '%s': %s", out.path.c_str(), std::strerror(errno));
+    return false;
+}
+
+// image::save_buffer(path, img, w, h, image::RGB(8)) for the two formats that are built
+bool save_image(const OutPath& out, const std::string& file, const uint8_t* rgb8, uint32_t w, uint32_t h) {
+    if (!out.ppm) {
+        if (trb_write_png(file.c_str(), rgb8, w, h) == TRB_OK) return true;
+        die("Error saving image '%s': %s", file.c_str(), trb_last_error());
+        return false;
+    }
+    FILE* f = std::fopen(file.c_str(), "wb");
+    bool ok = f != nullptr;
+    if (ok) {
+        ok = std::fprintf(f, "P6\n%u %u\n255\n", w, h) > 0 && std::fwrite(rgb8, 1, (size_t)w * h * 3, f) == (size_t)w * h * 3;
+        ok = std::fclose(f) == 0 && ok;
+    }
+    if (!ok) die("Error saving image '%s': %s", file.c_str(), std::strerror(errno));
+    return ok;
+}
+
+struct Args {
+    std::string scene;
+    std::vector<std::string> workers;
+    const char* out = nullptr;
+    bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false;
+    uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
+};
+
+// scene description (host only): the film section, frame range overrides applied
+struct Desc {
+    trb_scene_desc* d = nullptr;
+    ~Desc() { if (d) trb_desc_free(d); }
+};
+
+bool load_desc(const Args& a, uint32_t spp, Desc& desc, uint64_t& start, uint64_t& end) {
+    const trb_status rc = trb_desc_load_json(a.scene.c_str(), 0, 0, spp, &desc.d);
+    if (rc != TRB_OK) { die("cannot load scene '%s': %s", a.scene.c_str(), trb_last_error()); return false; }
+    start = a.has_start ? a.start : desc.d->film.start_frame;
+    end = a.has_end ? a.end : desc.d->film.end_frame;
+    if (end < start) { die("end frame %llu is before start frame %llu", (unsigned long long)end, (unsigned long long)start); return false; }
+    if (end > UINT32_MAX) { die("end frame %llu does not fit the renderer's 32-bit frame index", (unsigned long long)end); return false; }
+    return true;
+}
+
+// ---- single node (main.rs:56-109) -------------------------------------------------------------------------------------------
+int single_node(const Args& a, const OutPath& out) {
+    Desc desc;
+    uint64_t start = 0, end = 0;
+    if (!load_desc(a, (uint32_t)a.spp, desc, start, end)) return 1;
+    try {
+        tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
+        trb_desc_free(desc.d); desc.d = nullptr;
+        tray::RenderTarget rt = scene.make_render_target();
+        const auto dim = rt.dimensions();
+        tray::B200 exec;
+        tray::Config config;
+        config.seed = (uint32_t)a.seed;
+        const auto scene_start = std::chrono::steady_clock::now();
+        for (uint64_t i = start; i <= end; ++i) {
+            config.current_frame = i;
+            exec.render(scene, rt, config);
+            const std::vector<uint8_t> img = tray::get_render(scene, rt);
+            const std::string file = out.file_for(i);
+            if (!save_image(out, file, img.data(), (uint32_t)dim.first, (uint32_t)dim.second)) return 1;
+            rt.clear();
+            std::printf("Frame %llu: rendered to '%s'\n--------------------\n", (unsigned long long)i, file.c_str());
+            std::fflush(stdout);
+        }
+        std::printf("Rendering entire sequence took %.4fs\n", seconds_since(scene_start));
+    } catch (const tray::Error& e) {
+        std::fprintf(stderr, "trb_tray: status %d: %s\n", (int)e.status, e.what());
+        return e.status == TRB_NO_DEVICE ? 3 : 1;
+    }
+    return 0;
+}
+
+// ---- master (main.rs:111-146, exec/distrib/master.rs) -----------------------------------------------------------------------
+struct WorkerConn {
+    std::string name;             // host:port, as the messages print it
+    int fd = -1;
+    std::vector<uint8_t> buf;     // the Frame being read
+    size_t got = 0;
+    uint64_t expected = 8;        // the size header first, then the Frame's encoded_size
+    std::vector<bool> reported;   // per frame of the range
+    uint64_t n_reported = 0;
+};
+
+struct DistributedFrame {         // master.rs:24-46
+    std::vector<float> render;    // RGBW; empty until the first worker reports and after the frame is written
+    size_t num_reporting = 0;
+    std::chrono::steady_clock::time_point first_tile_recv;
+};
+
+struct Master {
+    std::vector<WorkerConn> workers;
+    ~Master() { for (WorkerConn& w : workers) if (w.fd >= 0) ::close(w.fd); }
+};
+
+// host[:port]; a bare host means exec::distrib::worker::PORT
+bool parse_worker(const std::string& s, std::string& host, std::string& port) {
+    port = std::to_string(trb_distrib::PORT);
+    if (std::count(s.begin(), s.end(), ':') == 1) {
+        host = s.substr(0, s.find(':')); port = s.substr(s.find(':') + 1);
+    } else {
+        host = s;
+    }
+    uint64_t p = 0;
+    return !host.empty() && parse_u64(port.c_str(), p) && p > 0 && p < 65536;
+}
+
+int connect_worker(const std::string& host, const std::string& port, std::string& err) {
+    addrinfo hints{}, *res = nullptr;
+    hints.ai_family = AF_UNSPEC; hints.ai_socktype = SOCK_STREAM;
+    const int g = ::getaddrinfo(host.c_str(), port.c_str(), &hints, &res);
+    if (g != 0) { err = ::gai_strerror(g); return -1; }
+    int fd = -1;
+    err = "no address";
+    for (addrinfo* ai = res; ai; ai = ai->ai_next) {
+        fd = ::socket(ai->ai_family, ai->ai_socktype | SOCK_CLOEXEC, ai->ai_protocol);
+        if (fd < 0) { err = std::strerror(errno); continue; }
+        if (::connect(fd, ai->ai_addr, ai->ai_addrlen) == 0) break;
+        err = std::strerror(errno);
+        ::close(fd); fd = -1;
+    }
+    ::freeaddrinfo(res);
+    return fd;
+}
+
+// which frame a message about worker `w` is about
+std::string frame_of(const WorkerConn& w, uint64_t start, uint64_t n_frames) {
+    char s[96];
+    if (w.got >= 16) { uint64_t f; std::memcpy(&f, &w.buf[8], 8); std::snprintf(s, sizeof s, "frame %llu", (unsigned long long)f); return s; }
+    for (uint64_t k = 0; k < n_frames; ++k)
+        if (!w.reported[k]) { std::snprintf(s, sizeof s, "frame %llu (its next unreported frame)", (unsigned long long)(start + k)); return s; }
+    return "after its last frame";
+}
+
+int master_node(const Args& a, const OutPath& out) {
+    Desc desc;
+    uint64_t start = 0, end = 0;
+    if (!load_desc(a, 0, desc, start, end)) return 1;
+    const uint32_t w = desc.d->film.width, h = desc.d->film.height;
+    trb_desc_free(desc.d); desc.d = nullptr;
+    if (w == 0 || h == 0 || w % 8 || h % 8) return die("image %ux%u is not evenly divided by blocks of (8, 8)", w, h); // block_queue.rs:29-31
+    const uint64_t n_frames = end - start + 1;
+    const uint64_t n_workers = a.workers.size();
+    const uint64_t n_blocks = (uint64_t)(w / 8) * (h / 8);
+    // block_count 0 means "all blocks" to a worker (block_queue.rs:39), so an idle worker would render the whole image again
+    if (n_workers > n_blocks) return die("%llu workers for %llu blocks: every worker needs at least one 8x8 block", (unsigned long long)n_workers, (unsigned long long)n_blocks);
+    const uint64_t blocks_per_worker = n_blocks / n_workers, blocks_remainder = n_blocks % n_workers; // master.rs:91-93
+    const uint64_t max_frame_bytes = trb_distrib::FRAME_HEADER_BYTES + 32ull * w * h; // 1x1 blocks over the whole image, each 16 + 16 bytes
+
+    Master m;
+    m.workers.resize(n_workers);
+    const auto scene_start = std::chrono::steady_clock::now();
+    for (uint64_t i = 0; i < n_workers; ++i) { // connect to every worker before sending anything (master.rs:99-113)
+        std::string host, port, err;
+        WorkerConn& wc = m.workers[i];
+        if (!parse_worker(a.workers[i], host, port)) return die("bad worker address '%s': use host or host:port", a.workers[i].c_str());
+        wc.name = host + ":" + port;
+        wc.reported.assign(n_frames, false);
+        wc.fd = connect_worker(host, port, err);
+        if (wc.fd < 0) return die("failed to contact worker %s: %s", wc.name.c_str(), err.c_str());
+    }
+    for (uint64_t i = 0; i < n_workers; ++i) { // master.rs:217-229
+        const uint64_t b_start = i * blocks_per_worker;
+        const uint64_t b_count = i == n_workers - 1 ? blocks_per_worker + blocks_remainder : blocks_per_worker;
+        const std::vector<uint8_t> bytes = trb_distrib::encode_instructions(a.scene, start, end, b_start, b_count);
+        if (!trb_distrib::write_all(m.workers[i].fd, bytes.data(), bytes.size()))
+            return die("failed to send instructions to worker %s: %s", m.workers[i].name.c_str(), std::strerror(errno));
+    }
+
+    std::vector<DistributedFrame> frames(n_frames);
+    std::vector<uint8_t> rgb8((size_t)w * h * 3);
+    uint64_t n_written = 0;
+    while (n_written < n_frames) {
+        std::vector<pollfd> pfd;
+        std::vector<size_t> who;
+        for (size_t i = 0; i < m.workers.size(); ++i)
+            if (m.workers[i].fd >= 0) { pfd.push_back(pollfd{m.workers[i].fd, POLLIN, 0}); who.push_back(i); }
+        if (::poll(pfd.data(), pfd.size(), -1) < 0) {
+            if (errno == EINTR) continue;
+            return die("poll: %s", std::strerror(errno));
+        }
+        for (size_t k = 0; k < pfd.size(); ++k) {
+            if (!pfd[k].revents) continue;
+            WorkerConn& wc = m.workers[who[k]];
+            if (wc.buf.size() < wc.expected) wc.buf.resize((size_t)wc.expected);
+            const ssize_t r = ::read(wc.fd, &wc.buf[wc.got], (size_t)(wc.expected - wc.got));
+            if (r < 0 && (errno == EINTR || errno == EAGAIN)) continue;
+            if (r <= 0) {
+                const std::string why = r < 0 ? std::strerror(errno) : "connection closed";
+                if (wc.got) return die("worker %s hung up in the middle of %s (%zu of %llu bytes received): %s", wc.name.c_str(),
+                                       frame_of(wc, start, n_frames).c_str(), wc.got, (unsigned long long)wc.expected, why.c_str());
+                return die("worker %s hung up before %s, having sent %llu of %llu frames: %s", wc.name.c_str(), frame_of(wc, start, n_frames).c_str(),
+                           (unsigned long long)wc.n_reported, (unsigned long long)n_frames, why.c_str());
+            }
+            wc.got += (size_t)r;
+            if (wc.got < wc.expected) continue;
+            if (wc.expected == 8) { // the size header (master.rs:249-262)
+                std::memcpy(&wc.expected, wc.buf.data(), 8);
+                if (wc.expected < trb_distrib::FRAME_HEADER_BYTES || wc.expected > max_frame_bytes)
+                    return die("worker %s sent an implausible Frame size %llu for %s (a %ux%u image's Frames hold %llu to %llu bytes)", wc.name.c_str(),
+                               (unsigned long long)wc.expected, frame_of(wc, start, n_frames).c_str(), w, h,
+                               (unsigned long long)trb_distrib::FRAME_HEADER_BYTES, (unsigned long long)max_frame_bytes);
+                continue;
+            }
+            trb_distrib::Frame f;
+            const std::string bad = trb_distrib::decode_frame(wc.buf, f);
+            const std::string what = frame_of(wc, start, n_frames);
+            if (!bad.empty()) return die("worker %s, %s: %s", wc.name.c_str(), what.c_str(), bad.c_str());
+            if (f.frame < start || f.frame > end)
+                return die("worker %s reported %s, outside the range [%llu, %llu]", wc.name.c_str(), what.c_str(), (unsigned long long)start, (unsigned long long)end);
+            const uint64_t fi = f.frame - start;
+            if (wc.reported[fi]) return die("worker %s reported %s twice", wc.name.c_str(), what.c_str());
+            if (f.block_w == 0 || f.block_h == 0 || f.block_w > w || f.block_h > h)
+                return die("worker %s, %s: block size (%llu, %llu) does not fit the %ux%u image", wc.name.c_str(), what.c_str(),
+                           (unsigned long long)f.block_w, (unsigned long long)f.block_h, w, h);
+            const uint64_t n_fb = f.blocks.size() / 2, stride = f.block_w * f.block_h * 4;
+            if (f.pixels.size() != n_fb * stride)
+                return die("worker %s, %s: %zu pixel floats for %llu blocks of (%llu, %llu), expected %llu", wc.name.c_str(), what.c_str(), f.pixels.size(),
+                           (unsigned long long)n_fb, (unsigned long long)f.block_w, (unsigned long long)f.block_h, (unsigned long long)(n_fb * stride));
+            for (uint64_t b = 0; b < n_fb; ++b) {
+                const uint64_t x0 = f.blocks[2 * b], y0 = f.blocks[2 * b + 1];
+                if (x0 > w - f.block_w || y0 > h - f.block_h)
+                    return die("worker %s, %s: block (%llu, %llu) of size (%llu, %llu) lies outside the %ux%u image", wc.name.c_str(), what.c_str(),
+                               (unsigned long long)x0, (unsigned long long)y0, (unsigned long long)f.block_w, (unsigned long long)f.block_h, w, h);
+            }
+            DistributedFrame& df = frames[fi];
+            if (df.num_reporting == 0) { df.render.assign((size_t)w * h * 4, 0.0f); df.first_tile_recv = std::chrono::steady_clock::now(); }
+            for (uint64_t b = 0; b < n_fb; ++b) { // Image::add_blocks (film/image.rs:36-50)
+                const float* px = &f.pixels[b * stride];
+                for (uint64_t by = 0; by < f.block_h; ++by)
+                    for (uint64_t bx = 0; bx < f.block_w; ++bx) {
+                        float* c = &df.render[4 * ((f.blocks[2 * b + 1] + by) * w + f.blocks[2 * b] + bx)];
+                        const float* p = &px[4 * (by * f.block_w + bx)];
+                        for (int i = 0; i < 4; ++i) c[i] += p[i];
+                    }
+            }
+            wc.reported[fi] = true; ++wc.n_reported;
+            wc.buf.clear(); wc.got = 0; wc.expected = 8;
+            if (wc.n_reported == n_frames) { ::close(wc.fd); wc.fd = -1; } // its last frame: the reference worker exits now
+            if (++df.num_reporting < n_workers) continue;
+            const double render_time = seconds_since(df.first_tile_recv); // master.rs:130-146
+            const std::string file = out.file_for(f.frame);
+            trb_host_film_to_srgb8(w, h, df.render.data(), rgb8.data());
+            if (!save_image(out, file, rgb8.data(), w, h)) return 1;
+            std::printf("Frame %llu: time between receiving first and last tile %.4fs\n", (unsigned long long)f.frame, render_time);
+            std::printf("Frame %llu: rendered to '%s'\n--------------------\n", (unsigned long long)f.frame, file.c_str());
+            std::fflush(stdout);
+            std::vector<float>().swap(df.render);
+            ++n_written;
+        }
+    }
+    std::printf("Rendering entire sequence took %.4fs\n", seconds_since(scene_start));
+    return 0;
+}
+
+} // namespace
+
+int main(int argc, char** argv) {
+    for (int i = 1; i < argc; ++i)
+        if (std::strcmp(argv[i], "--worker") == 0) return trb_distrib::worker_main(argc, argv);
+    Args a;
+    bool have_scene = false;
+    for (int i = 1; i < argc; ++i) {
+        const std::string s = argv[i];
+        const char* v = i + 1 < argc ? argv[i + 1] : nullptr;
+        auto number = [&](uint64_t& x, bool& has) {
+            if (!parse_u64(v, x)) { die("%s needs a non-negative integer", s.c_str()); return false; }
+            has = true; ++i; return true;
+        };
+        bool ok = true, unused = false;
+        if (s == "-h" || s == "--help") { std::fputs(USAGE, stdout); return 0; }
+        else if (s == "-o") { if (!v) return die("-o needs a path"); a.out = v; ++i; }
+        else if (s == "-n") { uint64_t n; ok = number(n, unused); }
+        else if (s == "--start-frame") ok = number(a.start, a.has_start);
+        else if (s == "--end-frame") ok = number(a.end, a.has_end);
+        else if (s == "--seed") ok = number(a.seed, a.has_seed) && a.seed <= UINT32_MAX;
+        else if (s == "--spp") ok = number(a.spp, a.has_spp) && a.spp <= UINT32_MAX;
+        else if (s == "--device") ok = number(a.device, a.has_device) && a.device <= INT32_MAX;
+        else if (s == "--master") a.master = true;
+        else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
+        else if (!have_scene) { a.scene = s; have_scene = true; }
+        else a.workers.push_back(s);
+        if (!ok) { std::fputs(USAGE, stderr); return 2; }
+    }
+    if (!have_scene) { std::fputs(USAGE, stderr); return 2; }
+    if (a.master && a.workers.empty()) return die("--master needs at least one worker address");
+    if (!a.master && !a.workers.empty()) return die("unexpected argument '%s' (worker addresses follow --master)", a.workers[0].c_str());
+    if (a.master && (a.has_seed || a.has_spp || a.has_device)) return die("--seed, --spp and --device are the workers' options: pass them to each worker");
+    if (a.has_start && a.has_end && a.end < a.start)
+        return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
+    OutPath out;
+    if (!resolve_out_path(a.out, out) || !create_out_dir(out, a.out != nullptr)) return 1;
+    return a.master ? master_node(a, out) : single_node(a, out);
+}
