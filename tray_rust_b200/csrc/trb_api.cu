@@ -61,10 +61,11 @@ struct HostMesh {
 uint32_t pow2_ceil(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 
 // Re-layout of the reference-order flat tree into child-pair records (trb_device.h DPair). Pure layout: no box,
-// child order or primitive order changes. Returns false if a leaf does not fit the 25-bit slot / 5-bit count fields.
+// child order or primitive order changes. Returns false if a leaf does not fit the 25-bit slot / 5-bit count fields, or,
+// `wide` (mesh levels only: REF_LEAF | first slot, the leaf's end is marked in its last DTri), if a leaf is empty or ends past 2^30.
 float bits_f(uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; }
 constexpr uint32_t QUAD_EMPTY_HOST = 0xffffffffu;
-bool pack_pairs(const std::vector<trb_bvh_node>& in, std::vector<trb::DPair>& out, trb::DBvh& hdr) {
+bool pack_pairs(const std::vector<trb_bvh_node>& in, std::vector<trb::DPair>& out, trb::DBvh& hdr, bool wide = false) {
     std::vector<uint32_t> rec_of(in.size(), 0);
     uint32_t n_rec = 0;
     for (size_t i = 0; i < in.size(); ++i) if (!(in[i].b & TRB_BVH_LEAF)) rec_of[i] = n_rec++;
@@ -72,6 +73,10 @@ bool pack_pairs(const std::vector<trb_bvh_node>& in, std::vector<trb::DPair>& ou
     auto ref_of = [&](uint32_t i) -> uint32_t {
         if (in[i].b & TRB_BVH_LEAF) {
             const uint32_t cnt = in[i].b & ~TRB_BVH_LEAF, first = in[i].a;
+            if (wide) {
+                if (cnt == 0 || (uint64_t)first + cnt > (1u << 30)) ok = false;
+                return trb::REF_LEAF | (first & ~trb::REF_TAG);
+            }
             if (cnt > 31 || first >= (1u << 25)) ok = false;
             return trb::REF_LEAF | (cnt << 25) | first;
         }
@@ -91,6 +96,13 @@ bool pack_pairs(const std::vector<trb_bvh_node>& in, std::vector<trb::DPair>& ou
     hdr.root_lo = make_float4(in[0].bmin[0], in[0].bmin[1], in[0].bmin[2], bits_f(ref_of(0)));
     hdr.root_hi = make_float4(in[0].bmax[0], in[0].bmax[1], in[0].bmax[2], 0.f);
     return ok;
+}
+// Whether every leaf of a mesh tree fits the narrow reference (count << 25 | first slot). A scene whose meshes all fit uses the
+// narrow form unless the option trace.wide_leaf asks for the wide one.
+bool leaves_fit_narrow(const std::vector<trb_bvh_node>& in) {
+    for (const trb_bvh_node& n : in)
+        if ((n.b & TRB_BVH_LEAF) && ((n.b & ~TRB_BVH_LEAF) > 31 || n.a >= (1u << 25))) return false;
+    return true;
 }
 
 // Collapse pairs of levels of the reference-order tree into DQuad records (trb_device.h). Layout only: boxes, child
@@ -163,6 +175,7 @@ struct Tuning {
     uint32_t sched = 6;        // trace: quorum of the phased loop (0 = flat state machine)
     int quads = 0;             // trace: DQuad two-level records
     int exact_box = 0;         // trace: test option — every ray takes the literal BBox::fast_intersect transcription (box_hit) instead of box_hit_finite
+    int wide_leaf = 0;         // trace: test option — 1: wide mesh leaf references for every scene; 0: only where a mesh leaf does not fit the narrow form
     int pipe = 36;             // trace: kernel variant. 0 = round-1 kernel; 1 = + box_hit_finite; 33 = + RayHome + fused non-node chains at 7 CTAs per SM; 34 / 35 / 36 / 37 = the same at 8 / 8 / 9 / 9 CTAs with 16 / 12 / 12 / 8 stack entries in shared memory
     int film_v2 = 1;           // film: per-warp private tiles (0 = shared-memory atomics)
     int sort = 0;              // ray queues: 0 = path order; 1 / 2 = counting sort by (octant, origin cell) / (cell, octant) before each trace round
@@ -181,6 +194,7 @@ int env_int(const char* name, int dflt) { const char* v = getenv(name); return v
 void tuning_from_env(Tuning& t) {
     t.refill = env_int("TRB_REFILL", t.refill); t.trace_grid = (unsigned)env_int("TRB_TRACE_GRID", (int)t.trace_grid);
     t.sched = (uint32_t)env_int("TRB_TRACE_SCHED", (int)t.sched); t.quads = env_int("TRB_TRACE_QUADS", t.quads); t.pipe = env_int("TRB_TRACE_PIPE", t.pipe);
+    t.wide_leaf = env_int("TRB_TRACE_WIDE_LEAF", t.wide_leaf);
     t.film_v2 = env_int("TRB_FILM_V2", t.film_v2); t.sort = env_int("TRB_SORT", t.sort); t.sort_bits = env_int("TRB_SORT_BITS", t.sort_bits);
     t.sort_min_round = env_int("TRB_SORT_MIN_ROUND", t.sort_min_round); t.shade_split = env_int("TRB_SHADE_SPLIT", t.shade_split); t.anim_table = env_int("TRB_ANIM_TABLE", t.anim_table); t.frame_device = env_int("TRB_FRAME_DEVICE", t.frame_device);
     if (getenv("TRB_PASS_PATHS")) t.pass_paths = strtoull(getenv("TRB_PASS_PATHS"), nullptr, 0);
@@ -210,6 +224,10 @@ struct trb_scene {
     std::vector<float> fov_floats;
     std::vector<trb_material> materials;
     std::vector<HostMesh> meshes;
+    std::vector<trb::DMesh> dmeshes;     // the device mesh headers (d_meshes), kept to re-pack the node records (trace.wide_leaf)
+    trb::DMesh* d_meshes = nullptr;
+    bool needs_wide = false;             // some mesh leaf does not fit the narrow reference (a mesh of more than 2^25 triangles)
+    bool wide_leaf = false;              // the mesh node records hold wide leaf references: the WIDE kernel instantiations run
     uint32_t spp_pow2 = 1;
     uint32_t n_anim = 0;                 // instances whose transform stack is keyframed (evaluated per path into WfState::xf_tab)
     bool frame_set = false; uint32_t last_frame = 0; float last_start = 0, last_end = 0; // the arguments of the last update_frame (re-run when an option changes what it builds)
@@ -360,6 +378,9 @@ trb_status validate(const trb_scene_desc* d) {
     for (uint32_t i = 0; i < d->n_meshes; ++i) {
         const trb_mesh& m = d->meshes[i];
         if (m.n_tris == 0 || m.n_verts == 0) return fail(TRB_INVALID_ARG, "empty mesh");
+        // the wide leaf references hold a 30-bit slot; the kernels index vertex attributes as 3 * index in 32 bits
+        if (m.n_tris > (1u << 30)) return fail(TRB_UNSUPPORTED, "mesh too large for the wide leaf encoding (2^30 triangles)");
+        if (m.n_verts > 0xffffffffu / 3) return fail(TRB_UNSUPPORTED, "mesh has too many vertices (more than (2^32 - 1) / 3)");
         if (!m.positions || !m.normals || !m.texcoords || !m.indices) return fail(TRB_INVALID_ARG, "Normals and texture coordinates are required!"); // mesh.rs:57-61
         for (size_t k = 0; k < 3 * (size_t)m.n_tris; ++k) if (m.indices[k] >= m.n_verts) return fail(TRB_INVALID_ARG, "mesh index out of range");
     }
@@ -399,14 +420,29 @@ trb_status resolve_samples(const trb_scene* s, const trb_render_cfg* cfg, uint32
     return TRB_OK;
 }
 
+// The instantiation of a kernel that traces through scene_trace for the scene's animation and mesh leaf form
+template <int MODE>
+auto simple_integrator_kernel(const trb_scene* s) {
+    const bool anim = s->ds.has_anim != 0;
+    if (s->wide_leaf) return anim ? trb::k_simple_integrator<MODE, true, true> : trb::k_simple_integrator<MODE, false, true>;
+    return anim ? trb::k_simple_integrator<MODE, true> : trb::k_simple_integrator<MODE, false>;
+}
+template <bool STATS>
+auto intersect_kernel(const trb_scene* s) {
+    const bool anim = s->ds.has_anim != 0;
+    if (s->wide_leaf) return anim ? trb::k_intersect<STATS, true, true> : trb::k_intersect<STATS, false, true>;
+    return anim ? trb::k_intersect<STATS, true> : trb::k_intersect<STATS, false>;
+}
+
 template <bool STATS, int MODE, bool ANIM>
 trb_status launch_render_t(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, cudaStream_t st) {
     const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
     const size_t smem = (size_t)T * T * sizeof(float4);
+    const auto kernel = s->wide_leaf ? trb::k_render<STATS, MODE, ANIM, true> : trb::k_render<STATS, MODE, ANIM>;
     int per_sm = 0;
-    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, trb::k_render<STATS, MODE, ANIM>, trb::RENDER_THREADS, smem));
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, trb::RENDER_THREADS, smem));
     const uint32_t grid = std::max(1u, std::min<uint32_t>(rp.n_blocks, (uint32_t)(std::max(1, per_sm) * s->sm_count)));
-    trb::k_render<STATS, MODE, ANIM><<<grid, trb::RENDER_THREADS, smem, st>>>(s->ds, rp, flags);
+    kernel<<<grid, trb::RENDER_THREADS, smem, st>>>(s->ds, rp, flags);
     g_launches++;
     CU(cudaGetLastError());
     return TRB_OK;
@@ -481,7 +517,13 @@ void launch_query_trace(trb_scene* s, const trb::RenderParams& rp, const trb::Wf
     const unsigned resident = stats ? 4u : (anim ? 8u : 9u); // as for renders: two rounds of what is resident per SM
     const unsigned tgrid = (unsigned)s->sm_count * (tu.trace_grid ? tu.trace_grid : 2u * resident);
     const uint32_t sched = std::max(1u, tu.sched);
-    if (anim) {
+    if (s->wide_leaf) { // PIPE bit 128: wide mesh leaf references
+        if (anim) {
+            if (stats) trb::k_wf_trace<true, 4, 16, true, true, false, 225><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+            else trb::k_wf_trace<false, 8, 12, true, true, false, 225><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+        } else if (stats) trb::k_wf_trace<true, 4, 16, false, true, false, 225><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+        else trb::k_wf_trace<false, 9, 12, false, true, false, 225><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
+    } else if (anim) {
         if (stats) trb::k_wf_trace<true, 4, 16, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
         else trb::k_wf_trace<false, 8, 12, true, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
     } else if (stats) trb::k_wf_trace<true, 4, 16, false, true, false, 97><<<tgrid, 128, 0, st>>>(s->ds, rp, wf, 0, tflags, tu.refill, sched, q_sorted);
@@ -544,6 +586,9 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
     const uint32_t sched = tu.sched;   // 0 = flat state machine; else the quorum of the phased loop (see k_wf_trace)
     const bool quads = tu.quads != 0;  // DQuad two-level records (never in the STATS variants: their counters are the reference's)
     const uint32_t tflags = flags | (tu.exact_box ? trb::WF_TRACE_FORCE_EXACT_BOX : 0u);
+    // a scene with wide mesh leaves runs the default trace variant only: the option-selected experimental ones have no wide form
+    if (s->wide_leaf && (sched == 0 || quads || tu.pipe == 0 || tu.pipe == 1 || (tu.pipe >= 33 && tu.pipe <= 35) || tu.pipe == 37))
+        return fail(TRB_UNSUPPORTED, "trace.quads, trace.sched 0 and the experimental trace.pipe variants do not read wide mesh leaves (trace.wide_leaf)");
     for (uint32_t round = 0; round < rounds; ++round) {
         const uint32_t* q_sorted = nullptr;
         if (tu.sort && (int)round >= tu.sort_min_round) { // counting sort of this round's rays by (type, octant, origin cell): DESIGN.md "Ray sorting"
@@ -567,7 +612,11 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
         // variants run the same code at their own occupancy, so the parity tests' counters cover it.
         const bool v2 = tu.pipe != 0;
         if (mode == 2 && round == 0) launch_query_trace(s, rp, wf, tflags, stats, q_sorted, st);
-        else if (anim) {
+        else if (s->wide_leaf) { // the default variant and its STATS and keyframed forms with PIPE bit 128 (wide mesh leaf references)
+            if (anim) { if (stats) TRB_TRACE_LAUNCH(true, 4, 16, true, true, false, 161); else TRB_TRACE_LAUNCH(false, 8, 12, true, true, false, 161); }
+            else if (stats) TRB_TRACE_LAUNCH(true, 4, 16, false, true, false, 161);
+            else TRB_TRACE_LAUNCH(false, 9, 12, false, true, false, 161);
+        } else if (anim) {
             if (stats) { if (v2) TRB_TRACE_LAUNCH(true, 4, 16, true, true, false, 33); else TRB_TRACE_LAUNCH(true, 4, 16, true, true, false, 0); }
             else if (!v2) TRB_TRACE_LAUNCH(false, 7, 16, true, true, false, 0);
             else if (tu.pipe == 33) TRB_TRACE_LAUNCH(false, 7, 16, true, true, false, 33);
@@ -608,11 +657,8 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
     if (s->integrator.type != TRB_INTEGRATOR_PATH) { // Whitted / NormalsDebug: one thread per camera sample, then the same film kernel
         const unsigned grid = (unsigned)std::min<size_t>((n_paths + 127) / 128, (size_t)s->sm_count * 8);
-        const bool anim = s->ds.has_anim != 0;
-        if (anim) { if (mode == 0) trb::k_simple_integrator<0, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
-                    else trb::k_simple_integrator<1, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr); }
-        else if (mode == 0) trb::k_simple_integrator<0, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
-        else trb::k_simple_integrator<1, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
+        const auto kernel = mode == 0 ? simple_integrator_kernel<0>(s) : simple_integrator_kernel<1>(s);
+        kernel<<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, nullptr);
         g_launches++;
         if (mode == 0) {
             const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
@@ -885,8 +931,7 @@ trb_status illum_passes(trb_scene* s, size_t n, const trb_illum_ray* d_rays, uin
         wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
         if (s->integrator.type != TRB_INTEGRATOR_PATH) {
             const unsigned grid = (unsigned)std::min<size_t>((wf.n_paths + 127) / 128, (size_t)s->sm_count * 8);
-            if (anim) trb::k_simple_integrator<2, true><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);
-            else trb::k_simple_integrator<2, false><<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);
+            simple_integrator_kernel<2>(s)<<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);
             g_launches++;
         } else {
             CU(cudaMemsetAsync(wf.counters, 0, 64 * trb::WF_CNT * sizeof(uint32_t), st));
@@ -1112,6 +1157,24 @@ trb_status camera_rays_enqueue(trb_scene* s, const trb_render_cfg* cfg, size_t n
     return TRB_OK;
 }
 
+// Packs every mesh's DPair records in one leaf form, narrow or wide (trb_device.h), into the buffers allocated when the scene was
+// created, and uploads the mesh headers. Kernels still in flight may read the records, so the device is drained first.
+trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
+    CU(cudaDeviceSynchronize());
+    for (size_t mi = 0; mi < s->meshes.size(); ++mi) {
+        std::vector<trb::DPair> pn;
+        trb::DBvh hdr{};
+        if (!pack_pairs(s->meshes[mi].nodes, pn, hdr, wide))
+            return fail(TRB_UNSUPPORTED, wide ? "mesh too large for the wide leaf encoding (2^30 triangles)" : "mesh too large for the leaf encoding (2^25 triangles)");
+        trb::DBvh& dh = s->dmeshes[mi].bvh;
+        if (!pn.empty()) CU(cudaMemcpy(const_cast<trb::DPair*>(dh.pairs), pn.data(), pn.size() * sizeof(trb::DPair), cudaMemcpyHostToDevice));
+        dh.root_lo = hdr.root_lo;
+    }
+    if (!s->dmeshes.empty()) CU(cudaMemcpy(s->d_meshes, s->dmeshes.data(), s->dmeshes.size() * sizeof(trb::DMesh), cudaMemcpyHostToDevice));
+    s->wide_leaf = wide;
+    return TRB_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -1137,6 +1200,11 @@ trb_status trb_scene_set_option(trb_scene* s, const char* name, long long value)
     }
     else if (k == "trace.pipe") t.pipe = (int)value;
     else if (k == "trace.exact_box") t.exact_box = (int)value;
+    else if (k == "trace.wide_leaf") { // re-pack the mesh node records when the form changes (a mesh that needs the wide form keeps it)
+        t.wide_leaf = (int)value;
+        const bool wide = s->needs_wide || value != 0;
+        if (wide != s->wide_leaf) { CU(cudaSetDevice(s->device)); return upload_mesh_nodes(s, wide); }
+    }
     else if (k == "film.v2") t.film_v2 = (int)value;
     else if (k == "sort.mode") t.sort = (int)value;
     else if (k == "sort.bits") t.sort_bits = (int)std::min<long long>(6, std::max<long long>(1, value));
@@ -1214,7 +1282,7 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     s->materials.assign(d->materials, d->materials + d->n_materials);
 
     // meshes: BVH<Triangle> with max_geom 16 (mesh.rs:44), then leaf-ordered triangle records
-    std::vector<trb::DMesh> dmeshes(d->n_meshes);
+    s->dmeshes.resize(d->n_meshes);
     s->meshes.resize(d->n_meshes);
     for (uint32_t mi = 0; mi < d->n_meshes; ++mi) {
         const trb_mesh& m = d->meshes[mi];
@@ -1223,55 +1291,68 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
         hm.nrm.assign(m.normals, m.normals + 3 * (size_t)m.n_verts);
         hm.uv.assign(m.texcoords, m.texcoords + 2 * (size_t)m.n_verts);
         hm.idx.assign(m.indices, m.indices + 3 * (size_t)m.n_tris);
+        auto vert = [&hm](size_t t, int k) { return &hm.pos[3 * (size_t)hm.idx[3 * t + k]]; };
         std::vector<Box3> tb(m.n_tris);
-        for (uint32_t t = 0; t < m.n_tris; ++t) { // Triangle::bounds (mesh.rs:128-134)
+        for (size_t t = 0; t < m.n_tris; ++t) { // Triangle::bounds (mesh.rs:128-134)
             Box3 b;
-            const float* pa = &hm.pos[3 * hm.idx[3 * t]];
+            const float* pa = vert(t, 0);
             for (int k = 0; k < 3; ++k) b.lo[k] = b.hi[k] = pa[k];
-            box_grow_pt(b, &hm.pos[3 * hm.idx[3 * t + 1]]);
-            box_grow_pt(b, &hm.pos[3 * hm.idx[3 * t + 2]]);
+            box_grow_pt(b, vert(t, 1));
+            box_grow_pt(b, vert(t, 2));
             tb[t] = b;
         }
-        BvhBuilder bb;
-        bb.build(tb, 16);
-        hm.nodes = bb.nodes; hm.order = bb.order;
+        {
+            BvhBuilder bb;
+            bb.build(tb, 16);
+            hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
+        }
+        std::vector<Box3>().swap(tb);
         for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
-        std::vector<trb::DPair> pn;
-        trb::DBvh hdr{};
-        if (!pack_pairs(hm.nodes, pn, hdr)) return fail(TRB_UNSUPPORTED, "mesh too large for the leaf encoding (2^25 triangles)");
         std::vector<trb::DTri> tris(m.n_tris);
-        for (uint32_t slot = 0; slot < m.n_tris; ++slot) {
+        for (size_t slot = 0; slot < m.n_tris; ++slot) {
             const uint32_t t = hm.order[slot];
-            const float* pa = &hm.pos[3 * hm.idx[3 * t]];
-            const float* pb = &hm.pos[3 * hm.idx[3 * t + 1]];
-            const float* pc = &hm.pos[3 * hm.idx[3 * t + 2]];
+            const float* pa = vert(t, 0);
+            const float* pb = vert(t, 1);
+            const float* pc = vert(t, 2);
             float tid; std::memcpy(&tid, &t, 4);
             tris[slot].v0 = make_float4(pa[0], pa[1], pa[2], tid);
             tris[slot].e0 = make_float4(pb[0] - pa[0], pb[1] - pa[1], pb[2] - pa[2], 0.f);
             tris[slot].e1 = make_float4(pc[0] - pa[0], pc[1] - pa[1], pc[2] - pa[2], 0.f);
             tris[slot].pad = make_float4(0.f, 0.f, 0.f, 0.f);
         }
-        std::vector<trb::DQuad> qn;
-        uint32_t qroot = 0;
-        if (!pack_quads(hm.nodes, qn, qroot)) return fail(TRB_UNSUPPORTED, "mesh too large for the leaf encoding (2^25 triangles)");
-        hdr.root_hi.w = bits_f(qroot);
-        trb::DQuad* dquads;
-        CU(s->arena.upload(qn.data(), qn.size(), &dquads));
-        hdr.quads = dquads;
-        trb::DMesh& dm = dmeshes[mi];
+        size_t n_rec = 0;
+        for (const trb_bvh_node& n : hm.nodes) { // the leaf mark on the last slot of every leaf, whichever form the scene uses
+            const uint32_t cnt = n.b & ~TRB_BVH_LEAF;
+            if (!(n.b & TRB_BVH_LEAF)) ++n_rec;
+            else if (cnt) tris[(size_t)n.a + cnt - 1].e0.w = bits_f(trb::TRI_LEAF_END);
+        }
+        trb::DMesh& dm = s->dmeshes[mi];
+        trb::DBvh& hdr = dm.bvh;
+        hdr.quads = nullptr;
+        hdr.root_hi = make_float4(hm.bounds.hi[0], hm.bounds.hi[1], hm.bounds.hi[2], bits_f(QUAD_EMPTY_HOST));
+        if (leaves_fit_narrow(hm.nodes)) { // DQuad records (trace.quads) hold narrow leaves only: a mesh that needs the wide form skips them
+            std::vector<trb::DQuad> qn;
+            uint32_t qroot = 0;
+            if (!pack_quads(hm.nodes, qn, qroot)) return fail(TRB_UNSUPPORTED, "mesh too large for the leaf encoding (2^25 triangles)");
+            hdr.root_hi.w = bits_f(qroot);
+            trb::DQuad* dquads;
+            CU(s->arena.upload(qn.data(), qn.size(), &dquads));
+            hdr.quads = dquads;
+        } else s->needs_wide = true;
         float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
         CU(s->arena.upload(hm.pos.data(), hm.pos.size(), &dp));
         CU(s->arena.upload(hm.nrm.data(), hm.nrm.size(), &dn));
         CU(s->arena.upload(hm.uv.data(), hm.uv.size(), &dt));
         CU(s->arena.upload(hm.idx.data(), hm.idx.size(), &di));
-        CU(s->arena.upload(pn.data(), pn.size(), &dnodes));
+        CU(s->arena.alloc(n_rec, &dnodes)); // filled by upload_mesh_nodes: both leaf forms have one record per interior node
         CU(s->arena.upload(tris.data(), tris.size(), &dtris));
         hdr.pairs = dnodes;
-        dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.bvh = hdr; dm.tris = dtris;
+        dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.tris = dtris;
         dm.n_nodes = (uint32_t)hm.nodes.size(); dm.n_tris = m.n_tris;
     }
-    trb::DMesh* d_meshes;
-    CU(s->arena.upload(dmeshes.data(), dmeshes.size(), &d_meshes));
+    CU(s->arena.alloc(s->dmeshes.size(), &s->d_meshes));
+    { const trb_status r = upload_mesh_nodes(s.get(), s->needs_wide || s->tune.wide_leaf != 0); if (r != TRB_OK) return r; }
+    trb::DMesh* d_meshes = s->d_meshes;
 
     // materials (precompute what Material::bsdf recomputes per hit from constant textures)
     std::vector<trb::DMaterial> dmats(d->n_materials);
@@ -1815,8 +1896,7 @@ trb_status trb_intersect_device(trb_scene* s, size_t n, const trb_ray* d_rays, t
     CU(cudaSetDevice(s->device));
     const unsigned grid = (unsigned)std::min<size_t>((n + 127) / 128, (size_t)s->sm_count * 16);
     g_launches++;
-    if (s->ds.has_anim) trb::k_intersect<false, true><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(s->ds, n, d_rays, d_hits, reinterpret_cast<trb::DStats*>(d_stats), s->d_error);
-    else trb::k_intersect<false, false><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(s->ds, n, d_rays, d_hits, reinterpret_cast<trb::DStats*>(d_stats), s->d_error);
+    intersect_kernel<false>(s)<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(s->ds, n, d_rays, d_hits, reinterpret_cast<trb::DStats*>(d_stats), s->d_error);
     CU(cudaGetLastError());
     return TRB_OK;
 }
@@ -1835,8 +1915,7 @@ trb_status trb_intersect(trb_scene* s, size_t n, const trb_ray* rays, trb_hit* h
     if (e == cudaSuccess) {
         cudaEventRecord(s->ev0, 0);
         const unsigned grid = (unsigned)std::min<size_t>((n + 127) / 128, (size_t)s->sm_count * 16);
-        if (s->ds.has_anim) trb::k_intersect<true, true><<<grid, 128>>>(s->ds, n, d_rays, d_hits, s->d_stats, s->d_error);
-        else trb::k_intersect<true, false><<<grid, 128>>>(s->ds, n, d_rays, d_hits, s->d_stats, s->d_error); // host variant always counts tests
+        intersect_kernel<true>(s)<<<grid, 128>>>(s->ds, n, d_rays, d_hits, s->d_stats, s->d_error); // host variant always counts tests
         cudaEventRecord(s->ev1, 0);
         e = cudaGetLastError();
     }

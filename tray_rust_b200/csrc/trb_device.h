@@ -19,7 +19,10 @@ constexpr uint32_t LEAF_BIT = 0x80000000u;
 // boxes, so one fetch (four 16-byte loads, two 32-byte sectors) feeds two box tests and the dependent-load
 // chain per ray is half as long. Topology, child order and every compare are unchanged (DESIGN.md
 // "Node layout"). A child reference is 2 tag bits + 30 payload bits:
-//   REF_INTERIOR | record index        REF_LEAF | count << 25 | first primitive slot
+//   REF_INTERIOR | record index        REF_LEAF | count << 25 | first primitive slot     (narrow leaves)
+//                                      REF_LEAF | first triangle slot (30 bits)          (wide mesh leaves)
+// A wide leaf ends at the triangle that carries TRI_LEAF_END (DTri). A scene uses one form for all its meshes, and the
+// host launches the kernel instantiations of that form (template flag WIDE); TLAS leaves are always narrow.
 struct DPair {
     float4 l_lo; // left  (= first child, index+1) min, w = left reference
     float4 l_hi; // left  max,                       w = right reference
@@ -51,10 +54,13 @@ static_assert(sizeof(DBvh) == 48, "DBvh layout");
 
 // One triangle in LEAF ORDER (slot k of the BLAS == ordered_geom[k]), padded to 64 B so that it is two aligned
 // 32-byte loads (one L1TEX tag lookup each) and never straddles a 128-byte line:
-// v0 = (pa.xyz, triangle index), e0 = pb-pa, e1 = pc-pa (the same single IEEE subtraction the
-// reference performs per test, mesh.rs:140, hoisted to load time).
+// v0 = (pa.xyz, triangle index), e0 = (pb-pa, leaf mark), e1 = (pc-pa, 0) (the same single IEEE subtraction the
+// reference performs per test, mesh.rs:140, hoisted to load time). The leaf mark is a bit pattern, never read as a
+// float: TRI_LEAF_END on the last slot of every mesh leaf, 0 elsewhere. The wide mesh leaf references (no count,
+// see DPair) walk a leaf up to the marked slot.
 struct alignas(64) DTri { float4 v0, e0, e1, pad; };
 static_assert(sizeof(DTri) == 64, "DTri layout");
+constexpr uint32_t TRI_LEAF_END = 0xffffffffu;
 
 struct DMesh {
     const float* positions; // 3 per vertex

@@ -337,7 +337,8 @@ __device__ __forceinline__ uint32_t trace_pop(TraceState& t, const Stack& stack)
     return ST_DONE;
 }
 // One transition: visit an interior node (two box tests), a leaf, the root, a pending instance, or leave a mesh.
-template <bool STATS, bool ANIM, class Stack>
+// WIDE: mesh leaf references carry no count (REF_LEAF | first slot); the leaf ends at the triangle marked TRI_LEAF_END.
+template <bool STATS, bool ANIM, bool WIDE = false, class Stack>
 __device__ __forceinline__ void trace_step(const DScene& sc, TraceState& t, const Stack& stack, Cnt& cnt, int* err) {
     const uint32_t cur = t.cur;
     const uint32_t tag = cur & REF_TAG;
@@ -369,7 +370,7 @@ __device__ __forceinline__ void trace_step(const DScene& sc, TraceState& t, cons
             for (uint32_t k = a + n; k-- > a;) stack.put(t.sp++, ST_INSTANCE | k); // pops as a, a+1, ... (bvh.rs:95-98)
         } else {
             const DTri* __restrict__ tris = t.tris;
-            for (uint32_t k = a; k < a + n; ++k) {
+            for (uint32_t k = WIDE ? (cur & ~REF_TAG) : a; WIDE || k < a + n; ++k) {
                 const float4 v0 = __ldg(&tris[k].v0), q0 = __ldg(&tris[k].e0), q1 = __ldg(&tris[k].e1);
                 if (STATS) cnt.tri++;
                 const f3 e0 = mk(q0.x, q0.y, q0.z), e1 = mk(q1.x, q1.y, q1.z);
@@ -389,6 +390,7 @@ __device__ __forceinline__ void trace_step(const DScene& sc, TraceState& t, cons
                     t.found = true;
                     if (t.any_hit) t.sp = 0;
                 }
+                if (WIDE && __float_as_uint(q0.w) == TRI_LEAF_END) break;
             }
         }
         next = trace_pop(t, stack);
@@ -611,16 +613,18 @@ __device__ __forceinline__ void accept_hit(TraceState& t, const RayHome* home, u
     } else { t.h_prim = prim; t.h_b1 = b1; t.h_b2 = b2; t.h_inst = inst; }
     t.found = true;
 }
-template <bool STATS, bool HOME = false>
+// WIDE: a mesh leaf reference is REF_LEAF | slot, and the next state is the next slot unless this triangle carries the leaf mark
+template <bool STATS, bool HOME = false, bool WIDE = false>
 __device__ __forceinline__ void step_triangle(TraceState& t, Cnt& cnt, const RayHome* home = nullptr) {
     const uint32_t cur = t.cur;
-    const uint32_t a = cur & 0x01ffffffu, n = (cur >> 25) & 31u;
+    const uint32_t a = WIDE ? (cur & ~REF_TAG) : (cur & 0x01ffffffu), n = (cur >> 25) & 31u;
     uint32_t next = n > 1 ? (REF_LEAF | ((n - 1) << 25) | (a + 1)) : ST_POP;
-    if (n != 0) {
+    if (WIDE || n != 0) {
         const DTri* __restrict__ tri = t.tris + a;
         float4 v0, q0, q1, qpad;
         ldg256(&tri->v0, v0, q0);
         ldg256(&tri->e1, q1, qpad);
+        if (WIDE) next = __float_as_uint(q0.w) == TRI_LEAF_END ? ST_POP : cur + 1;
         if (STATS) cnt.tri++;
         const f3 e0 = mk(q0.x, q0.y, q0.z), e1 = mk(q1.x, q1.y, q1.z);
         const f3 s0 = cross3(t.d, e1);
@@ -719,13 +723,13 @@ __device__ __forceinline__ void step_other(const DScene& sc, TraceState& t, cons
     t.cur = next;
 }
 
-template <bool STATS, bool ANIM>
+template <bool STATS, bool ANIM, bool WIDE = false>
 __device__ __noinline__ bool scene_trace(const DScene& sc, Ray& ray, HitRec& hit, bool any_hit, Cnt& cnt, int* err, float time) {
     TraceState t;
     unsigned long long stack_mem[STACK_DEPTH];
     const LocalStack stack{stack_mem};
     trace_init(sc, t, ray, any_hit, time);
-    while (t.cur != ST_DONE) trace_step<STATS, ANIM>(sc, t, stack, cnt, err);
+    while (t.cur != ST_DONE) trace_step<STATS, ANIM, WIDE>(sc, t, stack, cnt, err);
     ray.tmax = t.tmax;
     hit.t = t.tmax; hit.inst = t.h_inst; hit.prim = t.h_prim; hit.b1 = t.h_b1; hit.b2 = t.h_b2;
     return t.found;
@@ -1582,11 +1586,11 @@ __device__ __forceinline__ float camera_ray(const DScene& sc, float sx, float sy
     return frame_time;
 }
 
-template <bool STATS, bool ANIM>
+template <bool STATS, bool ANIM, bool WIDE = false>
 __device__ f3 radiance_of_sample(const DScene& sc, Ray ray, float time, uint32_t hpix_sample, bool ref_shadow, RayCounts& rc, Cnt& cnt, int* err) {
     HitRec hit;
     rc.primary++;
-    if (!scene_trace<STATS, ANIM>(sc, ray, hit, false, cnt, err, time)) return splat(0.0f); // multithreaded.rs:101-102
+    if (!scene_trace<STATS, ANIM, WIDE>(sc, ray, hit, false, cnt, err, time)) return splat(0.0f); // multithreaded.rs:101-102
     f3 illum = splat(0.0f), throughput = splat(1.0f);
     bool specular_bounce = false;
     uint32_t bounce = 0;
@@ -1601,13 +1605,13 @@ __device__ f3 radiance_of_sample(const DScene& sc, Ray ray, float time, uint32_t
             Ray sr; sr.o = o.org; sr.d = o.ds.shadow_d; sr.tmin = 0.001f; sr.tmax = 0.999f;
             HitRec sh;
             rc.shadow++;
-            occluded = scene_trace<STATS, ANIM>(sc, sr, sh, !ref_shadow, cnt, err, time);
+            occluded = scene_trace<STATS, ANIM, WIDE>(sc, sr, sh, !ref_shadow, cnt, err, time);
         }
         if (o.ds.has_mis) {
             Ray mr; mr.o = o.org; mr.d = o.ds.mis_d; mr.tmin = 0.001f; mr.tmax = finf();
             HitRec mh;
             rc.mis++;
-            if (scene_trace<STATS, ANIM>(sc, mr, mh, false, cnt, err, time)) mis_ok = mis_sees_light<ANIM>(sc, o.org, o.ds.mis_d, o.light, mh.inst, mh.t, time);
+            if (scene_trace<STATS, ANIM, WIDE>(sc, mr, mh, false, cnt, err, time)) mis_ok = mis_sees_light<ANIM>(sc, o.org, o.ds.mis_d, o.light, mh.inst, mh.t, time);
         }
         illum = illum + o.t_before * direct_resolve(o.ds.a, o.ds.b, occluded, mis_ok);
         throughput = o.throughput;
@@ -1615,7 +1619,7 @@ __device__ f3 radiance_of_sample(const DScene& sc, Ray ray, float time, uint32_t
         if (o.terminate) break;
         ray.o = o.org; ray.d = o.next_d; ray.tmin = 0.001f; ray.tmax = finf();
         rc.cont++;
-        if (!scene_trace<STATS, ANIM>(sc, ray, hit, false, cnt, err, time)) break;
+        if (!scene_trace<STATS, ANIM, WIDE>(sc, ray, hit, false, cnt, err, time)) break;
         surface_at<ANIM>(sc, ray, hit, s, time);
         bounce += 1;
     }
@@ -1695,7 +1699,7 @@ __device__ __forceinline__ void splat_sample(const DScene& sc, float4* tile, con
 constexpr int RENDER_THREADS = 128;
 constexpr int MAX_TILE = 25; // fpw <= 8
 
-template <bool STATS, int MODE, bool ANIM>
+template <bool STATS, int MODE, bool ANIM, bool WIDE = false>
 __global__ void __launch_bounds__(RENDER_THREADS) k_render(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, uint32_t flags) {
     extern __shared__ float4 tile[];           // T*T RGBW
     __shared__ float s_table[256];
@@ -1731,7 +1735,7 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_render(const __grid_constant
             Ray ray;
             const float time = camera_ray<ANIM>(sc, sx, sy, tm, ray);
             my_samples++;
-            f3 c = radiance_of_sample<STATS, ANIM>(sc, ray, time, rng_absorb(ps.hpix, si), ref_shadow, rc, cnt, rp.error_flag);
+            f3 c = radiance_of_sample<STATS, ANIM, WIDE>(sc, ray, time, rng_absorb(ps.hpix, si), ref_shadow, rc, cnt, rp.error_flag);
             c = mk(clampf(c.x, 0.0f, 1.0f), clampf(c.y, 0.0f, 1.0f), clampf(c.z, 0.0f, 1.0f)); // multithreaded.rs:99 (Q12)
             if (MODE == 1) {
                 trb_sample* out = reinterpret_cast<trb_sample*>(rp.samples_out) + ((size_t)item * 64 + pix) * rp.sample_count + (si - rp.sample_first);
@@ -2082,6 +2086,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(const __grid_constant__ 
                                                          uint32_t round, uint32_t flags, int WF_REFILL_IDLE, uint32_t sched, const uint32_t* __restrict__ q_sorted) {
     constexpr bool HOME = PHASED && (PIPE & 32) != 0; // RayHome: world ray and hit record live in the path state, not in registers
     constexpr bool QUERY = (PIPE & 64) != 0;          // ray queries (k_query_load): each ray's [min_t, max_t] is org.w and the direction entry's .w
+    constexpr bool WIDE = (PIPE & 128) != 0;          // wide mesh leaf references (trb_device.h DPair)
     uint32_t* cnt_r = wf.counters + round * WF_CNT;
     const uint32_t n_cont = cnt_r[WF_N_CONT], n_shadow = cnt_r[WF_N_SHADOW], n_mis = cnt_r[WF_N_MIS];
     const uint32_t total = n_cont + n_shadow + n_mis;
@@ -2177,14 +2182,14 @@ __global__ void __launch_bounds__(128, MINB) k_wf_trace(const __grid_constant__ 
                 if (m_o != 0 && (m_a == 0 || __popc(m_o) >= thr_o)) {
                     if (is_o) {
                         const RayHome home{&wf.org[p], type == 0 ? &wf.cont[p] : (type == 1 ? &wf.shadow[p] : &wf.mis[p]), &wf.hit[p], &wf.a[p].w, type};
-                        if ((t.cur & REF_TAG) == REF_LEAF && t.level_inst != TRB_MISS) step_triangle<STATS, HOME>(t, cnt, &home);
+                        if ((t.cur & REF_TAG) == REF_LEAF && t.level_inst != TRB_MISS) step_triangle<STATS, HOME, WIDE>(t, cnt, &home);
                         else step_other<STATS, ANIM, HOME>(sc, t, stack, cnt, &home);
                     }
                 }
             }
         } else {
             for (;;) {
-                if (have && t.cur != ST_DONE) trace_step<STATS, ANIM>(sc, t, stack, cnt, rp.error_flag);
+                if (have && t.cur != ST_DONE) trace_step<STATS, ANIM, WIDE>(sc, t, stack, cnt, rp.error_flag);
                 const unsigned running = __ballot_sync(0xffffffffu, have && t.cur != ST_DONE);
                 if (running == 0) break;
                 if (!exhausted && 32 - __popc(running) >= WF_REFILL_IDLE) break;
@@ -2409,7 +2414,7 @@ __device__ __noinline__ void light_sample_incident(const DScene& sc, uint32_t li
     seg = pw - p;
 }
 
-template <bool ANIM>
+template <bool ANIM, bool WIDE = false>
 __device__ f3 whitted_illum(const DScene& sc, const Ray& ray, uint32_t depth, const HitRec& hit, uint32_t node, uint32_t hs, float time, bool ref_shadow,
                             RayCounts& rc, Cnt& cnt, int* err) {
     Surf s;
@@ -2435,7 +2440,7 @@ __device__ f3 whitted_illum(const DScene& sc, const Ray& ray, uint32_t depth, co
             Ray sr; sr.o = s.p; sr.d = seg; sr.tmin = 0.001f; sr.tmax = 0.999f;
             HitRec sh;
             rc.shadow++;
-            if (!scene_trace<true, ANIM>(sc, sr, sh, !ref_shadow, cnt, err, time)) illum = illum + f * lrad * fabsf(dot3(wi, fr.n)) / pdf;
+            if (!scene_trace<true, ANIM, WIDE>(sc, sr, sh, !ref_shadow, cnt, err, time)) illum = illum + f * lrad * fabsf(dot3(wi, fr.n)) / pdf;
         }
     }
     if (depth < sc.max_depth) {
@@ -2452,8 +2457,8 @@ __device__ f3 whitted_illum(const DScene& sc, const Ray& ray, uint32_t depth, co
                 Ray r2; r2.o = fr.p; r2.d = wi; r2.tmin = 0.001f; r2.tmax = finf();
                 HitRec h2;
                 rc.cont++;
-                if (scene_trace<true, ANIM>(sc, r2, h2, false, cnt, err, time)) {
-                    const f3 li = whitted_illum<ANIM>(sc, r2, depth + 1, h2, 2 * node + (uint32_t)which, hs, time, ref_shadow, rc, cnt, err);
+                if (scene_trace<true, ANIM, WIDE>(sc, r2, h2, false, cnt, err, time)) {
+                    const f3 li = whitted_illum<ANIM, WIDE>(sc, r2, depth + 1, h2, 2 * node + (uint32_t)which, hs, time, ref_shadow, rc, cnt, err);
                     out = f * li * fabsf(dot3(wi, fr.n)) / pdf;
                 }
             }
@@ -2466,7 +2471,7 @@ __device__ f3 whitted_illum(const DScene& sc, const Ray& ray, uint32_t depth, co
 // One camera sample per thread for the Whitted / NormalsDebug integrators; radiance to wf.rad (MODE 0, then the film kernel) or to trb_sample records (MODE 1).
 // MODE 2 (illumination queries): path p is sample p % rp.spp of the caller's ray rays[p / rp.spp], whose key and sample index key the
 // streams; the unclamped radiance goes to rad[p] (then k_illum_reduce).
-template <int MODE, bool ANIM>
+template <int MODE, bool ANIM, bool WIDE = false>
 __global__ void __launch_bounds__(128) k_simple_integrator(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, float4* rad, uint32_t n_paths,
                                                            uint32_t integrator, uint32_t flags, const trb_illum_ray* __restrict__ rays) {
     RayCounts rc = {0, 0, 0, 0};
@@ -2492,14 +2497,14 @@ __global__ void __launch_bounds__(128) k_simple_integrator(const __grid_constant
         mine++; rc.primary++;
         HitRec hit;
         f3 c = splat(0.0f);
-        if (scene_trace<true, ANIM>(sc, ray, hit, false, cnt, rp.error_flag, time)) {
+        if (scene_trace<true, ANIM, WIDE>(sc, ray, hit, false, cnt, rp.error_flag, time)) {
             if (integrator == TRB_INTEGRATOR_NORMALS_DEBUG) { // (bsdf.n + 1) / 2
                 Surf s;
                 surface_at<ANIM>(sc, ray, hit, s, time);
                 Frame fr;
                 make_frame(s, fr);
                 c = (fr.n + splat(1.0f)) / 2.0f;
-            } else c = whitted_illum<ANIM>(sc, ray, 0, hit, 1, rng_absorb(hpix, si), time, (flags & 4u) != 0, rc, cnt, rp.error_flag);
+            } else c = whitted_illum<ANIM, WIDE>(sc, ray, 0, hit, 1, rng_absorb(hpix, si), time, (flags & 4u) != 0, rc, cnt, rp.error_flag);
         }
         if (MODE == 2) { rad[p] = make_float4(c.x, c.y, c.z, 1.0f); continue; }
         c = mk(clampf(c.x, 0.0f, 1.0f), clampf(c.y, 0.0f, 1.0f), clampf(c.z, 0.0f, 1.0f)); // multithreaded.rs:99 (Q12)
@@ -2826,7 +2831,7 @@ __global__ void k_camera_rays(const __grid_constant__ DScene sc, const __grid_co
 }
 
 // Scene::intersect over a ray batch (trb_intersect): one ray per thread, grid-stride.
-template <bool STATS, bool ANIM>
+template <bool STATS, bool ANIM, bool WIDE = false>
 __global__ void __launch_bounds__(128) k_intersect(const __grid_constant__ DScene sc, size_t n, const trb_ray* __restrict__ rays, trb_hit* __restrict__ hits,
                                                     DStats* stats, int* err) {
     Cnt cnt = {0, 0, 0};
@@ -2835,7 +2840,7 @@ __global__ void __launch_bounds__(128) k_intersect(const __grid_constant__ DScen
         const float4 a = __ldg(reinterpret_cast<const float4*>(rays + i)), b = __ldg(reinterpret_cast<const float4*>(rays + i) + 1);
         Ray r; r.o = mk(a.x, a.y, a.z); r.d = mk(a.w, b.x, b.y); r.tmin = b.z; r.tmax = b.w;
         HitRec h;
-        const bool hit = scene_trace<STATS, ANIM>(sc, r, h, false, cnt, err, sc.cam.shutter_open); // batch rays carry no time: the frame's shutter-open time
+        const bool hit = scene_trace<STATS, ANIM, WIDE>(sc, r, h, false, cnt, err, sc.cam.shutter_open); // batch rays carry no time: the frame's shutter-open time
         rc.primary++;
         uint4 o; o.x = __float_as_uint(r.tmax); o.y = hit ? h.inst : TRB_MISS; o.z = hit ? h.prim : 0u; o.w = 0u;
         *reinterpret_cast<uint4*>(hits + i) = o;

@@ -269,6 +269,44 @@ def random_triangle_mesh(n_tris, seed, lo=(-13, 1, -8), hi=(13, 23, 18), jitter=
     return v.reshape(-1, 3), normals, uv, idx
 
 
+def heightfield_mesh(grid, seed, lo=(-13, -8), hi=(13, 18), base=5.0, amplitude=2.5, waves=6):
+    """A grid x grid vertex heightfield y(x, z) over [lo, hi] in x and z, with shared vertices: 2 (grid - 1)^2 triangles from grid^2
+    vertices, 4200 x 4200 giving 35 263 202 triangles in about 0.6 GB of attributes (a triangle soup of that size would need
+    five times as much). The height is a sum of `waves` seeded sinusoids around `base`; normals are the analytic surface
+    normals, texcoords (i / (grid - 1), j / (grid - 1)). Vertex j * grid + i sits at (x_i, y, z_j); cell (i, j) is the
+    triangles (a, a + 1, a + grid + 1) and (a, a + grid + 1, a + grid) with a = j * grid + i."""
+    assert grid >= 2
+    rng = np.random.Generator(np.random.PCG64(seed))
+    fx, fz = rng.uniform(-1.2, 1.2, size=(2, waves))
+    phase = rng.uniform(0.0, 2.0 * math.pi, size=waves)
+    amp = amplitude * rng.uniform(0.3, 1.0, size=waves) / math.sqrt(waves)
+    xs, zs = np.linspace(lo[0], hi[0], grid), np.linspace(lo[1], hi[1], grid)
+    X, Z = np.meshgrid(xs, zs)  # [j, i]
+    H = np.full_like(X, base)
+    dx, dz = np.zeros_like(X), np.zeros_like(X)
+    for k in range(waves):
+        s = fx[k] * X + fz[k] * Z + phase[k]
+        H += amp[k] * np.sin(s)
+        c = amp[k] * np.cos(s)
+        dx += fx[k] * c
+        dz += fz[k] * c
+        del s, c
+    positions = np.stack([X, H, Z], axis=-1).astype(np.float32).reshape(-1, 3)
+    del X, Z, H
+    inv = 1.0 / np.sqrt(dx * dx + dz * dz + 1.0)
+    normals = np.stack([-dx * inv, inv, -dz * inv], axis=-1).astype(np.float32).reshape(-1, 3)
+    del dx, dz, inv
+    t = np.arange(grid, dtype=np.float32) / np.float32(grid - 1)
+    texcoords = np.empty((grid, grid, 2), np.float32)
+    texcoords[..., 0] = t[None, :]
+    texcoords[..., 1] = t[:, None]
+    a = (np.arange(grid - 1, dtype=np.uint32)[:, None] * np.uint32(grid) + np.arange(grid - 1, dtype=np.uint32)[None, :]).reshape(-1)
+    idx = np.empty((2 * len(a), 3), np.uint32)
+    idx[0::2, 0] = a; idx[0::2, 1] = a + 1; idx[0::2, 2] = a + grid + 1
+    idx[1::2, 0] = a; idx[1::2, 1] = a + grid + 1; idx[1::2, 2] = a + grid
+    return positions, normals, texcoords.reshape(-1, 2), idx
+
+
 def icosphere_mesh(subdiv, radius=1.0, noise=0.0, seed=0):
     """Closed triangle mesh with smooth vertex normals and spherical uvs (C3 bunny stand-in)."""
     t = (1.0 + math.sqrt(5.0)) / 2.0
@@ -316,6 +354,19 @@ def scene_c4(n_tris=1_000_000, width=1920, height=1080, spp=4096, seed=0x5EED1E5
     mats = cornell_walls(b)
     cornell_light(b, mats["white"])
     m = b.add_mesh(*random_triangle_mesh(n_tris, seed))
+    mat = b.add_material(F.MAT_MATTE, (0.74, 0.74, 0.73), roughness=1.0)
+    b.receiver(F.SHAPE_MESH, mat, [trs()], mesh=m)
+    b.add_camera([trs(t=(0, 12, -60))], fov=30.0)
+    return b
+
+
+def scene_heightfield(grid=4200, width=1920, height=1080, spp=4, seed=0x4E16F1D):
+    """A large shared-vertex mesh inside the Cornell walls: the heightfield_mesh grid (4200: 35 M triangles, more than the 2^25
+    a narrow mesh leaf reference can address, so the scene uses wide mesh leaves)."""
+    b = SceneBuilder(width, height, spp, 4, 8)
+    mats = cornell_walls(b)
+    cornell_light(b, mats["white"])
+    m = b.add_mesh(*heightfield_mesh(grid, seed))
     mat = b.add_material(F.MAT_MATTE, (0.74, 0.74, 0.73), roughness=1.0)
     b.receiver(F.SHAPE_MESH, mat, [trs()], mesh=m)
     b.add_camera([trs(t=(0, 12, -60))], fov=30.0)
