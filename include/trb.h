@@ -726,6 +726,23 @@ trb_status trb_scene_get_filter_table(const trb_scene* scene, float* table256);
 trb_status trb_host_build_bvh(const float* boxes6, uint32_t n, uint32_t max_geom, uint32_t* n_nodes,
                               trb_bvh_node* nodes, uint32_t* ordered);
 
+/* trb_host_build_bvh run on GPU `device`, with the same arguments and statuses and the same output (the same nodes in the
+ * same order, the same ordered_geom), bit for bit except that a bound which ties between -0.0 and +0.0 may carry the other
+ * zero. Host buffers; NULL nodes / ordered query sizes. n >= 2^31 is TRB_UNSUPPORTED; without a GPU the result is
+ * TRB_NO_DEVICE. Boxes on which the reference's build would split a node into an empty child (more than max_geom boxes
+ * whose centroids all fall in one bucket, from infinite or NaN coordinates) give TRB_INVALID_ARG. */
+trb_status trb_build_bvh(int device, const float* boxes6, uint32_t n, uint32_t max_geom, uint32_t* n_nodes,
+                         trb_bvh_node* nodes, uint32_t* ordered);
+
+/* trb_build_bvh with DEVICE buffers on GPU `device` (4-byte aligned): d_nodes has room for 2n - 1 nodes, d_ordered for
+ * n words, and the node count is written to the device word d_n_nodes. The work is enqueued on cuda_stream (a
+ * cudaStream_t; NULL = default stream), and no other stream is touched. The one exception to asynchrony: the build
+ * proceeds level by level over its nodes of more than 1024 boxes and reads the number of such nodes back, so it
+ * synchronises cuda_stream once per level (the call returns with the rest of the work enqueued). Scratch memory is
+ * allocated and freed stream-ordered on cuda_stream. Null buffers or n == 0: TRB_INVALID_ARG. */
+trb_status trb_build_bvh_device(int device, const float* d_boxes6, uint32_t n, uint32_t max_geom, uint32_t* d_n_nodes,
+                                trb_bvh_node* d_nodes, uint32_t* d_ordered, void* cuda_stream);
+
 /* Keyframe::transform (keyframe.rs:60-63): T * R * S and its inverse, row-major. */
 trb_status trb_host_keyframe_transform(const trb_keyframe* kf, float* mat16, float* inv16);
 

@@ -212,6 +212,7 @@ TRB_SYMBOLS = [
     "trb_bsdf_eval", "trb_bsdf_eval_device", "trb_bsdf_sample", "trb_bsdf_sample_device", "trb_light_sample", "trb_light_sample_device",
     "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
     "trb_film_write", "trb_film_write_device", "trb_camera_rays_device", "trb_host_film_to_srgb8",
+    "trb_build_bvh", "trb_build_bvh_device",
 ]
 
 _trb = None
@@ -281,6 +282,8 @@ def load_trb():
     lib.trb_desc_free.argtypes = [C.POINTER(SceneDesc)]
     lib.trb_desc_free.restype = None
     lib.trb_host_build_bvh.argtypes = [vp, u32, u32, C.POINTER(u32), vp, vp]
+    lib.trb_build_bvh.argtypes = [C.c_int, vp, u32, u32, C.POINTER(u32), vp, vp]
+    lib.trb_build_bvh_device.argtypes = [C.c_int, vp, u32, u32, vp, vp, vp, vp]
     lib.trb_host_keyframe_transform.argtypes = [C.POINTER(Keyframe), vp, vp]
     lib.trb_host_animated_transform.argtypes = [C.POINTER(SceneDesc), u32, u32, f32, vp, vp]
     lib.trb_host_animated_color.argtypes = [C.POINTER(SceneDesc), u32, u32, f32, vp]

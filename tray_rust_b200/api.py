@@ -49,6 +49,32 @@ def film_to_srgb8(film):
     return out
 
 
+def build_bvh(boxes, max_geom, device=0):
+    """trb_build_bvh: BVH::new over boxes of shape (n, 6) (min xyz, max xyz) with the reference's SAH build, run on GPU `device`.
+    Returns (nodes as NODE_DTYPE, ordered_geom as uint32), the bytes trb_host_build_bvh returns."""
+    boxes = np.ascontiguousarray(boxes, dtype=np.float32).reshape(-1, 6)
+    lib = F.load_trb()
+    nn = F.u32()
+    rc = lib.trb_build_bvh(device, F.ptr(boxes), len(boxes), max_geom, C.byref(nn), None, None)
+    if rc == F.TRB_OK:
+        nodes = np.zeros(nn.value, F.NODE_DTYPE)
+        order = np.zeros(len(boxes), np.uint32)
+        rc = lib.trb_build_bvh(device, F.ptr(boxes), len(boxes), max_geom, C.byref(nn), F.ptr(nodes), F.ptr(order))
+    if rc != F.TRB_OK:
+        raise TrbError(rc, (lib.trb_last_error() or b"").decode())
+    return nodes, order
+
+
+def build_bvh_device(d_boxes, n, max_geom, d_n_nodes, d_nodes, d_ordered, device=0, stream=None):
+    """trb_build_bvh_device: the same build over DEVICE buffers (pointers as ints): d_nodes with room for 2n - 1 nodes, d_ordered
+    for n uint32, and the node count written to the device word d_n_nodes. Enqueued on `stream` (a cudaStream_t as an int, e.g.
+    torch.cuda.Stream().cuda_stream; None = default stream), which it synchronises once per level of large nodes."""
+    lib = F.load_trb()
+    rc = lib.trb_build_bvh_device(device, d_boxes, n, max_geom, d_n_nodes, d_nodes, d_ordered, stream)
+    if rc != F.TRB_OK:
+        raise TrbError(rc, (lib.trb_last_error() or b"").decode())
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
 

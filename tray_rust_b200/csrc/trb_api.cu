@@ -10,6 +10,7 @@
 #include <cub/device/device_radix_sort.cuh>
 #include "trb_host.h"
 #include "trb_kernels.cuh"
+#include "trb_bvh_build.cuh"
 
 using namespace trbh;
 
@@ -189,6 +190,7 @@ struct Tuning {
     int shade_sort = 1;        // split shading: bucket the paths by material kind between k_wf_shade_a and _b / _c
     int shade_kind = 1;        // split shading with buckets: the matte bucket goes through _b / _c instantiations compiled for matte alone
     uint64_t pass_paths = 1ull << 24; // camera samples per wavefront pass (the frame is rendered in additive passes)
+    int build_device = 1;      // scene creation: mesh BVHs built on the device (trb_bvh_build.cuh); 0 = on the host, as when the build's scratch does not fit
 };
 int env_int(const char* name, int dflt) { const char* v = getenv(name); return v ? (int)strtol(v, nullptr, 0) : dflt; }
 void tuning_from_env(Tuning& t) {
@@ -198,6 +200,7 @@ void tuning_from_env(Tuning& t) {
     t.film_v2 = env_int("TRB_FILM_V2", t.film_v2); t.sort = env_int("TRB_SORT", t.sort); t.sort_bits = env_int("TRB_SORT_BITS", t.sort_bits);
     t.sort_min_round = env_int("TRB_SORT_MIN_ROUND", t.sort_min_round); t.shade_split = env_int("TRB_SHADE_SPLIT", t.shade_split); t.anim_table = env_int("TRB_ANIM_TABLE", t.anim_table); t.frame_device = env_int("TRB_FRAME_DEVICE", t.frame_device);
     if (getenv("TRB_PASS_PATHS")) t.pass_paths = strtoull(getenv("TRB_PASS_PATHS"), nullptr, 0);
+    t.build_device = env_int("TRB_BUILD_DEVICE", t.build_device);
 }
 
 } // namespace
@@ -1175,6 +1178,70 @@ trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
     return TRB_OK;
 }
 
+// BVH<Triangle> of one uploaded mesh (max_geom 16, mesh.rs:44) into hm.nodes / hm.order, and its leaf-ordered triangle records with
+// their leaf-end marks into dtris. The triangle boxes are computed on the device. The SAH build runs on the device, or on the host
+// (BvhBuilder over the boxes read back) when `on_device` is off or its scratch does not fit in free device memory, which keeps the
+// largest meshes loadable. Every scratch buffer is freed before returning.
+trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, uint32_t n, HostMesh& hm, trb::DTri* dtris) {
+    float* d_boxes = nullptr;
+    uint32_t* d_order = nullptr; // + one word: the node count
+    trb_bvh_node* d_nodes = nullptr;
+    const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
+    auto run = [&]() -> trb_status {
+        CU(cudaMalloc(&d_boxes, 24 * (size_t)n));
+        CU(cudaMalloc(&d_order, 4 * ((size_t)n + 1)));
+        trb::bvhb::k_tri_boxes<<<grid(n), 256>>>(dp, di, n, d_boxes);
+        ++g_launches;
+        size_t free_b = 0, total_b = 0;
+        CU(cudaMemGetInfo(&free_b, &total_b));
+        const size_t need = trb::bvhb::build_scratch_bytes(n) + (2 * (size_t)n - 1) * sizeof(trb_bvh_node) + ((size_t)64 << 20);
+        if (on_device && need <= free_b) {
+            CU(cudaMalloc(&d_nodes, (2 * (size_t)n - 1) * sizeof(trb_bvh_node)));
+            bool empty = false;
+            CU(trb::bvhb::build_device(d_boxes, n, 16, d_order + n, d_nodes, d_order, 0, &g_launches, &empty));
+            if (empty) return fail(TRB_INVALID_ARG, "mesh triangles with infinite coordinates: the SAH build would split a node into an empty child");
+            uint32_t nn = 0;
+            CU(cudaMemcpy(&nn, d_order + n, 4, cudaMemcpyDeviceToHost));
+            hm.nodes.resize(nn);
+            hm.order.resize(n);
+            CU(cudaMemcpy(hm.nodes.data(), d_nodes, (size_t)nn * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(hm.order.data(), d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
+        } else {
+            {
+                std::vector<Box3> tb(n);
+                CU(cudaMemcpy(tb.data(), d_boxes, 24 * (size_t)n, cudaMemcpyDeviceToHost));
+                BvhBuilder bb;
+                bb.build(tb, 16);
+                hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
+            }
+            CU(cudaMemcpy(d_order, hm.order.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
+        }
+        CU(cudaFree(d_boxes));
+        d_boxes = nullptr;
+        trb::bvhb::k_tri_pack<<<grid(n), 256>>>(dp, di, d_order, n, dtris);
+        ++g_launches;
+        if (!d_nodes) { // host build: the marks are set from the host tree, a chunk of nodes at a time
+            const size_t chunk = std::min<size_t>(hm.nodes.size(), (size_t)1 << 22);
+            CU(cudaMalloc(&d_nodes, chunk * sizeof(trb_bvh_node)));
+            for (size_t i = 0; i < hm.nodes.size(); i += chunk) {
+                const size_t k = std::min(chunk, hm.nodes.size() - i);
+                CU(cudaMemcpy(d_nodes, hm.nodes.data() + i, k * sizeof(trb_bvh_node), cudaMemcpyHostToDevice));
+                trb::bvhb::k_tri_leaf_marks<<<grid(k), 256>>>(d_nodes, (uint32_t)k, dtris);
+                ++g_launches;
+            }
+        } else {
+            trb::bvhb::k_tri_leaf_marks<<<grid(hm.nodes.size()), 256>>>(d_nodes, (uint32_t)hm.nodes.size(), dtris);
+            ++g_launches;
+        }
+        CU(cudaGetLastError());
+        CU(cudaDeviceSynchronize());
+        return TRB_OK;
+    };
+    const trb_status r = run();
+    cudaFree(d_boxes); cudaFree(d_order); cudaFree(d_nodes);
+    return r;
+}
+
 } // namespace
 
 extern "C" {
@@ -1291,41 +1358,16 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
         hm.nrm.assign(m.normals, m.normals + 3 * (size_t)m.n_verts);
         hm.uv.assign(m.texcoords, m.texcoords + 2 * (size_t)m.n_verts);
         hm.idx.assign(m.indices, m.indices + 3 * (size_t)m.n_tris);
-        auto vert = [&hm](size_t t, int k) { return &hm.pos[3 * (size_t)hm.idx[3 * t + k]]; };
-        std::vector<Box3> tb(m.n_tris);
-        for (size_t t = 0; t < m.n_tris; ++t) { // Triangle::bounds (mesh.rs:128-134)
-            Box3 b;
-            const float* pa = vert(t, 0);
-            for (int k = 0; k < 3; ++k) b.lo[k] = b.hi[k] = pa[k];
-            box_grow_pt(b, vert(t, 1));
-            box_grow_pt(b, vert(t, 2));
-            tb[t] = b;
-        }
-        {
-            BvhBuilder bb;
-            bb.build(tb, 16);
-            hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
-        }
-        std::vector<Box3>().swap(tb);
+        float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
+        CU(s->arena.upload(hm.pos.data(), hm.pos.size(), &dp));
+        CU(s->arena.upload(hm.nrm.data(), hm.nrm.size(), &dn));
+        CU(s->arena.upload(hm.uv.data(), hm.uv.size(), &dt));
+        CU(s->arena.upload(hm.idx.data(), hm.idx.size(), &di));
+        CU(s->arena.alloc(m.n_tris, &dtris));
+        { const trb_status r = build_mesh_bvh(s->tune.build_device != 0, dp, di, m.n_tris, hm, dtris); if (r != TRB_OK) return r; }
         for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
-        std::vector<trb::DTri> tris(m.n_tris);
-        for (size_t slot = 0; slot < m.n_tris; ++slot) {
-            const uint32_t t = hm.order[slot];
-            const float* pa = vert(t, 0);
-            const float* pb = vert(t, 1);
-            const float* pc = vert(t, 2);
-            float tid; std::memcpy(&tid, &t, 4);
-            tris[slot].v0 = make_float4(pa[0], pa[1], pa[2], tid);
-            tris[slot].e0 = make_float4(pb[0] - pa[0], pb[1] - pa[1], pb[2] - pa[2], 0.f);
-            tris[slot].e1 = make_float4(pc[0] - pa[0], pc[1] - pa[1], pc[2] - pa[2], 0.f);
-            tris[slot].pad = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
         size_t n_rec = 0;
-        for (const trb_bvh_node& n : hm.nodes) { // the leaf mark on the last slot of every leaf, whichever form the scene uses
-            const uint32_t cnt = n.b & ~TRB_BVH_LEAF;
-            if (!(n.b & TRB_BVH_LEAF)) ++n_rec;
-            else if (cnt) tris[(size_t)n.a + cnt - 1].e0.w = bits_f(trb::TRI_LEAF_END);
-        }
+        for (const trb_bvh_node& n : hm.nodes) if (!(n.b & TRB_BVH_LEAF)) ++n_rec;
         trb::DMesh& dm = s->dmeshes[mi];
         trb::DBvh& hdr = dm.bvh;
         hdr.quads = nullptr;
@@ -1339,13 +1381,7 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
             CU(s->arena.upload(qn.data(), qn.size(), &dquads));
             hdr.quads = dquads;
         } else s->needs_wide = true;
-        float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
-        CU(s->arena.upload(hm.pos.data(), hm.pos.size(), &dp));
-        CU(s->arena.upload(hm.nrm.data(), hm.nrm.size(), &dn));
-        CU(s->arena.upload(hm.uv.data(), hm.uv.size(), &dt));
-        CU(s->arena.upload(hm.idx.data(), hm.idx.size(), &di));
         CU(s->arena.alloc(n_rec, &dnodes)); // filled by upload_mesh_nodes: both leaf forms have one record per interior node
-        CU(s->arena.upload(tris.data(), tris.size(), &dtris));
         hdr.pairs = dnodes;
         dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.tris = dtris;
         dm.n_nodes = (uint32_t)hm.nodes.size(); dm.n_tris = m.n_tris;
@@ -2177,6 +2213,51 @@ trb_status trb_host_build_bvh(const float* boxes6, uint32_t n, uint32_t max_geom
     if (nodes) std::memcpy(nodes, bb.nodes.data(), bb.nodes.size() * sizeof(trb_bvh_node));
     if (ordered) std::memcpy(ordered, bb.order.data(), bb.order.size() * sizeof(uint32_t));
     return TRB_OK;
+}
+
+static trb_status bvh_device_check(int device, uint32_t n) {
+    if (n >= (1u << 31)) return fail(TRB_UNSUPPORTED, "more than 2^31 - 1 boxes");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(TRB_NO_DEVICE, "no CUDA device: tray_rust_b200 has no CPU fallback"); }
+    if (device < 0 || device >= ndev) return fail(TRB_INVALID_ARG, "device ordinal out of range");
+    CU(cudaSetDevice(device));
+    return TRB_OK;
+}
+
+trb_status trb_build_bvh_device(int device, const float* d_boxes6, uint32_t n, uint32_t max_geom, uint32_t* d_n_nodes, trb_bvh_node* d_nodes,
+                                uint32_t* d_ordered, void* cuda_stream) {
+    if (!d_boxes6 || n == 0 || !d_n_nodes || !d_nodes || !d_ordered) return fail(TRB_INVALID_ARG, "null buffer or empty geometry");
+    const trb_status c = bvh_device_check(device, n);
+    if (c != TRB_OK) return c;
+    bool empty = false;
+    CU(trb::bvhb::build_device(d_boxes6, n, max_geom, d_n_nodes, d_nodes, d_ordered, (cudaStream_t)cuda_stream, &g_launches, &empty));
+    if (empty) return fail(TRB_INVALID_ARG, "the SAH build would split a node into an empty child (infinite coordinates)");
+    return TRB_OK;
+}
+
+trb_status trb_build_bvh(int device, const float* boxes6, uint32_t n, uint32_t max_geom, uint32_t* n_nodes, trb_bvh_node* nodes, uint32_t* ordered) {
+    if (!boxes6 || n == 0 || !n_nodes) return fail(TRB_INVALID_ARG, "empty geometry"); // bvh.rs:35 assert!(!geometry.is_empty())
+    const trb_status c = bvh_device_check(device, n);
+    if (c != TRB_OK) return c;
+    float* d_boxes = nullptr;
+    uint32_t* d_order = nullptr; // + one word: the node count
+    trb_bvh_node* d_nodes = nullptr;
+    auto run = [&]() -> trb_status {
+        CU(cudaMalloc(&d_boxes, 24 * (size_t)n));
+        CU(cudaMalloc(&d_order, 4 * ((size_t)n + 1)));
+        CU(cudaMalloc(&d_nodes, (2 * (size_t)n - 1) * sizeof(trb_bvh_node)));
+        CU(cudaMemcpy(d_boxes, boxes6, 24 * (size_t)n, cudaMemcpyHostToDevice));
+        bool empty = false;
+        CU(trb::bvhb::build_device(d_boxes, n, max_geom, d_order + n, d_nodes, d_order, 0, &g_launches, &empty));
+        if (empty) return fail(TRB_INVALID_ARG, "the SAH build would split a node into an empty child (infinite coordinates)");
+        CU(cudaMemcpy(n_nodes, d_order + n, 4, cudaMemcpyDeviceToHost));
+        if (nodes) CU(cudaMemcpy(nodes, d_nodes, (size_t)*n_nodes * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
+        if (ordered) CU(cudaMemcpy(ordered, d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
+        return TRB_OK;
+    };
+    const trb_status r = run();
+    cudaFree(d_boxes); cudaFree(d_order); cudaFree(d_nodes);
+    return r;
 }
 
 trb_status trb_host_keyframe_transform(const trb_keyframe* kf, float* mat16, float* inv16) {
