@@ -345,6 +345,23 @@ trb_status trb_scene_info(const trb_scene* scene, uint32_t* width, uint32_t* hei
  * BVH<Instance> (max_geom 4) for the shutter interval and uploads it. */
 trb_status trb_scene_update_frame(trb_scene* scene, uint32_t frame, float start, float end);
 
+/* Replace the vertex attributes of mesh `mesh` (n_verts of the description, indices and triangle count unchanged). Each of
+ * positions (3 floats per vertex), normals (3) and texcoords (2) may be NULL to keep the current array. New positions rebuild
+ * the mesh's BVH<Triangle> (max_geom 16), its leaf-ordered triangle records and node records, and, if a frame has been set,
+ * re-run trb_scene_update_frame with its last arguments. Afterwards the scene equals one created from the description with
+ * these arrays, except that the mesh has no records for the trace.quads experiment (it then returns TRB_UNSUPPORTED).
+ * Drains the device before it overwrites anything that kernels read; returns when the update is complete.
+ * Statuses: a null scene or a mesh index out of range is TRB_INVALID_ARG; all three arrays NULL is TRB_OK and changes nothing.
+ * Positions that trb_scene_create would reject get its status and message (TRB_INVALID_ARG for triangles with infinite
+ * coordinates that make the build split a node into an empty child). A failed update leaves the scene as it was, with one
+ * exception: a CUDA error (a device fault, not a property of the input) reported once the node records are being written may leave
+ * it half updated. */
+trb_status trb_scene_update_mesh(trb_scene* scene, uint32_t mesh, const float* positions, const float* normals, const float* texcoords);
+/* The same from device buffers on the scene's GPU: the caller's arrays are read on cuda_stream (a cudaStream_t; NULL = default
+ * stream), so a producer on that stream needs no host copy. */
+trb_status trb_scene_update_mesh_device(trb_scene* scene, uint32_t mesh, const float* d_positions, const float* d_normals,
+                                        const float* d_texcoords, void* cuda_stream);
+
 /* -- the hot path ------------------------------------------------------------------ */
 
 /* ≙ Exec::render (exec/mod.rs:48; multithreaded.rs:55-70). Renders the selected

@@ -1,0 +1,14 @@
+/* A plain-C caller of the mesh update entry points (include/trb.h): it compiles and links against libtrb with nothing but the header,
+ * and prints the status of each entry point called with a null scene (checked before any device is touched). */
+#include <stdio.h>
+#include "trb.h"
+
+int main(void) {
+    float v[9] = {0, 0, 0, 1, 0, 0, 0, 1, 0};
+    printf("status trb_scene_update_mesh:null_scene %d\n", (int)trb_scene_update_mesh(NULL, 0, v, v, v));
+    printf("status trb_scene_update_mesh:null_all %d\n", (int)trb_scene_update_mesh(NULL, 0, NULL, NULL, NULL));
+    printf("status trb_scene_update_mesh_device:null_scene %d\n", (int)trb_scene_update_mesh_device(NULL, 0, v, NULL, NULL, NULL));
+    printf("status trb_scene_update_mesh_device:null_all %d\n", (int)trb_scene_update_mesh_device(NULL, 3, NULL, NULL, NULL, NULL));
+    printf("status TRB_INVALID_ARG %d\n", (int)TRB_INVALID_ARG);
+    return 0;
+}

@@ -213,6 +213,7 @@ TRB_SYMBOLS = [
     "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
     "trb_film_write", "trb_film_write_device", "trb_camera_rays_device", "trb_host_film_to_srgb8",
     "trb_build_bvh", "trb_build_bvh_device",
+    "trb_scene_update_mesh", "trb_scene_update_mesh_device",
 ]
 
 _trb = None
@@ -241,6 +242,8 @@ def load_trb():
     lib.trb_scene_destroy.restype = None
     lib.trb_scene_info.argtypes = [vp] + [C.POINTER(u32)] * 6
     lib.trb_scene_update_frame.argtypes = [vp, u32, f32, f32]
+    lib.trb_scene_update_mesh.argtypes = [vp, u32, vp, vp, vp]
+    lib.trb_scene_update_mesh_device.argtypes = [vp, u32, vp, vp, vp, vp]
     lib.trb_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]

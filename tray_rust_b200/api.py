@@ -184,6 +184,30 @@ class Scene(_Base):
         cfg = _cfg(**kw)
         self._check(self._lib.trb_render_device(self._h, C.byref(cfg), d_film_ptr, d_stats_ptr, stream))
 
+    def _mesh_verts(self, mesh):
+        if not 0 <= mesh < self._desc.n_meshes:
+            raise ValueError("mesh index %d out of range (%d meshes)" % (mesh, self._desc.n_meshes))
+        return self._desc.meshes[mesh].n_verts
+
+    def update_mesh(self, mesh, positions=None, normals=None, texcoords=None):
+        """trb_scene_update_mesh: replace mesh `mesh`'s positions (n_verts x 3), normals (n_verts x 3) and / or texcoords
+        (n_verts x 2); None keeps an array. New positions rebuild the mesh's BVH and refresh the current frame."""
+        nv = self._mesh_verts(mesh)
+        arrays = []
+        for name, a, k in (("positions", positions, 3), ("normals", normals, 3), ("texcoords", texcoords, 2)):
+            if a is not None:
+                a = np.ascontiguousarray(a, np.float32)
+                if a.size != nv * k or (a.ndim != 1 and a.shape != (nv, k)):
+                    raise ValueError("%s must have shape (%d, %d), got %s" % (name, nv, k, a.shape))
+            arrays.append(a)
+        self._check(self._lib.trb_scene_update_mesh(self._h, mesh, *(None if a is None else F.ptr(a) for a in arrays)))
+
+    def update_mesh_device(self, mesh, d_positions=None, d_normals=None, d_texcoords=None, stream=None):
+        """trb_scene_update_mesh_device: the same from device pointers (ints) holding float32 arrays of the mesh's vertex count,
+        read on `stream` (a cudaStream_t as an int; None = default stream)."""
+        self._mesh_verts(mesh)
+        self._check(self._lib.trb_scene_update_mesh_device(self._h, mesh, d_positions, d_normals, d_texcoords, stream))
+
     def set_option(self, name, value):
         """trb_scene_set_option: launch-shape options (never change results)."""
         self._check(self._lib.trb_scene_set_option(self._h, name.encode(), int(value)))

@@ -49,14 +49,19 @@ struct DeviceArena { // owns every cudaMalloc of a scene
         *out = static_cast<T*>(d);
         return e;
     }
+    void release(const void* p) { // frees one allocation of this arena (a mesh buffer that an update replaced)
+        for (size_t i = 0; i < ptrs.size(); ++i)
+            if (ptrs[i] == p) { cudaFree(ptrs[i]); ptrs[i] = ptrs.back(); ptrs.pop_back(); return; }
+    }
 };
 
 struct HostMesh {
-    std::vector<float> pos, nrm, uv;
-    std::vector<uint32_t> idx;
     std::vector<trb_bvh_node> nodes;
     std::vector<uint32_t> order;
     Box3 bounds;
+    uint32_t n_verts = 0;
+    bool narrow = true;    // every leaf fits the narrow reference (pack_pairs)
+    size_t pair_cap = 0;   // DPair records the mesh's record buffer holds
 };
 
 uint32_t pow2_ceil(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
@@ -230,6 +235,7 @@ struct trb_scene {
     std::vector<trb::DMesh> dmeshes;     // the device mesh headers (d_meshes), kept to re-pack the node records (trace.wide_leaf)
     trb::DMesh* d_meshes = nullptr;
     bool needs_wide = false;             // some mesh leaf does not fit the narrow reference (a mesh of more than 2^25 triangles)
+    bool quads_dropped = false;          // trb_scene_update_mesh rebuilt a mesh, which has no DQuad records (trace.quads) since
     bool wide_leaf = false;              // the mesh node records hold wide leaf references: the WIDE kernel instantiations run
     uint32_t spp_pow2 = 1;
     uint32_t n_anim = 0;                 // instances whose transform stack is keyframed (evaluated per path into WfState::xf_tab)
@@ -592,6 +598,7 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
     // a scene with wide mesh leaves runs the default trace variant only: the option-selected experimental ones have no wide form
     if (s->wide_leaf && (sched == 0 || quads || tu.pipe == 0 || tu.pipe == 1 || (tu.pipe >= 33 && tu.pipe <= 35) || tu.pipe == 37))
         return fail(TRB_UNSUPPORTED, "trace.quads, trace.sched 0 and the experimental trace.pipe variants do not read wide mesh leaves (trace.wide_leaf)");
+    if (quads && s->quads_dropped) return fail(TRB_UNSUPPORTED, "trace.quads reads DQuad records, which a mesh updated by trb_scene_update_mesh does not have");
     for (uint32_t round = 0; round < rounds; ++round) {
         const uint32_t* q_sorted = nullptr;
         if (tu.sort && (int)round >= tu.sort_min_round) { // counting sort of this round's rays by (type, octant, origin cell): DESIGN.md "Ray sorting"
@@ -1181,11 +1188,15 @@ trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
 // BVH<Triangle> of one uploaded mesh (max_geom 16, mesh.rs:44) into hm.nodes / hm.order, and its leaf-ordered triangle records with
 // their leaf-end marks into dtris. The triangle boxes are computed on the device. The SAH build runs on the device, or on the host
 // (BvhBuilder over the boxes read back) when `on_device` is off or its scratch does not fit in free device memory, which keeps the
-// largest meshes loadable. Every scratch buffer is freed before returning.
-trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, uint32_t n, HostMesh& hm, trb::DTri* dtris) {
+// largest meshes loadable. Every scratch buffer is freed before returning, except that with `keep` the device-built node array is
+// handed to the caller (*keep stays null after a host build). `ev_built` / `ev_read` (optional) are recorded on the default stream
+// once the tree is built and once it has been read back to the host (a host build records both after building).
+trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, uint32_t n, HostMesh& hm, trb::DTri* dtris,
+                          trb_bvh_node** keep = nullptr, cudaEvent_t ev_built = nullptr, cudaEvent_t ev_read = nullptr) {
     float* d_boxes = nullptr;
     uint32_t* d_order = nullptr; // + one word: the node count
     trb_bvh_node* d_nodes = nullptr;
+    bool built = false;          // d_nodes holds the device-built tree
     const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
     auto run = [&]() -> trb_status {
         CU(cudaMalloc(&d_boxes, 24 * (size_t)n));
@@ -1200,12 +1211,15 @@ trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, u
             bool empty = false;
             CU(trb::bvhb::build_device(d_boxes, n, 16, d_order + n, d_nodes, d_order, 0, &g_launches, &empty));
             if (empty) return fail(TRB_INVALID_ARG, "mesh triangles with infinite coordinates: the SAH build would split a node into an empty child");
+            built = true;
+            if (ev_built) CU(cudaEventRecord(ev_built, 0));
             uint32_t nn = 0;
             CU(cudaMemcpy(&nn, d_order + n, 4, cudaMemcpyDeviceToHost));
             hm.nodes.resize(nn);
             hm.order.resize(n);
             CU(cudaMemcpy(hm.nodes.data(), d_nodes, (size_t)nn * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
             CU(cudaMemcpy(hm.order.data(), d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
+            if (ev_read) CU(cudaEventRecord(ev_read, 0));
         } else {
             {
                 std::vector<Box3> tb(n);
@@ -1214,6 +1228,8 @@ trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, u
                 bb.build(tb, 16);
                 hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
             }
+            if (ev_built) CU(cudaEventRecord(ev_built, 0));
+            if (ev_read) CU(cudaEventRecord(ev_read, 0));
             CU(cudaMemcpy(d_order, hm.order.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
         }
         CU(cudaFree(d_boxes));
@@ -1238,13 +1254,179 @@ trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, u
         return TRB_OK;
     };
     const trb_status r = run();
+    if (r == TRB_OK && keep && built) { *keep = d_nodes; d_nodes = nullptr; }
     cudaFree(d_boxes); cudaFree(d_order); cudaFree(d_nodes);
     return r;
+}
+
+// DPair records of a device-built mesh tree (d_nodes, n nodes) in one leaf form, with pack_pairs' layout, on the default stream.
+// The interior nodes are ranked first (an exclusive scan of their flags); `records(n_rec, &out)` then supplies room for the n_rec
+// records. *fits_narrow: whether every leaf fits the narrow reference. Scratch is freed before returning.
+template <class Records>
+trb_status pack_pairs_device(const trb_bvh_node* d_nodes, uint32_t n, bool wide, Records records, bool* fits_narrow) {
+    uint32_t* d_rec = nullptr; // n + 1 ranks, then the narrow-misfit word
+    void* d_cub = nullptr;
+    const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
+    auto run = [&]() -> trb_status {
+        size_t cub_bytes = 0;
+        CU(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)n + 1));
+        CU(cudaMalloc(&d_rec, 4 * ((size_t)n + 2)));
+        CU(cudaMalloc(&d_cub, std::max<size_t>(1, cub_bytes)));
+        CU(cudaMemset(d_rec + n + 1, 0, 4));
+        trb::bvhb::k_pair_flags<<<grid((size_t)n + 1), 256>>>(d_nodes, n, d_rec);
+        ++g_launches;
+        CU(cub::DeviceScan::ExclusiveSum(d_cub, cub_bytes, d_rec, d_rec, (int)n + 1));
+        uint32_t n_rec = 0;
+        CU(cudaMemcpy(&n_rec, d_rec + n, 4, cudaMemcpyDeviceToHost));
+        trb::DPair* out = nullptr;
+        { const trb_status r = records(n_rec, &out); if (r != TRB_OK) return r; }
+        trb::bvhb::k_pair_pack<<<grid(n), 256>>>(d_nodes, n, d_rec, wide, out, d_rec + n + 1);
+        ++g_launches;
+        CU(cudaGetLastError());
+        uint32_t bad = 0;
+        CU(cudaMemcpy(&bad, d_rec + n + 1, 4, cudaMemcpyDeviceToHost));
+        *fits_narrow = bad == 0;
+        return TRB_OK;
+    };
+    const trb_status r = run();
+    cudaFree(d_rec); cudaFree(d_cub);
+    return r;
+}
+
+// trb_scene_update_mesh(_device): `device` says the caller's arrays are device memory, read on `st`. New positions are copied
+// into a fresh buffer and the tree and triangle records are built into fresh buffers, so a failed build or allocation leaves the
+// scene as it was; the live buffers are replaced only after the build succeeded and the device was drained. The node records are
+// written into the live record buffer when the new tree fits it, so a CUDA error from the packing on (a device fault, not a
+// property of the input) may leave the scene half updated. TRB_MESH_UPDATE_TIME=1 prints the phases, timed with CUDA events on the
+// default stream (every phase ends at a synchronisation point, so they are also wall time), to stderr: build, read-back (the tree to
+// the host), triangle records (k_tri_pack, k_tri_leaf_marks), pack (node records), frame refresh.
+trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float* nrm, const float* uv, bool device, cudaStream_t st) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (mi >= s->meshes.size()) return fail(TRB_INVALID_ARG, "mesh index out of range");
+    if (!pos && !nrm && !uv) return TRB_OK;
+    CU(cudaSetDevice(s->device));
+    HostMesh& hm = s->meshes[mi];
+    trb::DMesh& dm = s->dmeshes[mi];
+    const size_t nv = hm.n_verts;
+    auto copy_in = [&](const float* dst, const float* src, size_t n) -> cudaError_t {
+        if (!device) return cudaMemcpy(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyHostToDevice);
+        const cudaError_t e = cudaMemcpyAsync(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+        return e != cudaSuccess ? e : cudaStreamSynchronize(st);
+    };
+    struct PhaseEvents {
+        cudaEvent_t e[6] = {};
+        ~PhaseEvents() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+    } ev;
+    const bool timing = pos && getenv("TRB_MESH_UPDATE_TIME") != nullptr;
+    if (timing) for (cudaEvent_t& x : ev.e) CU(cudaEventCreate(&x));
+    auto mark = [&](int k) { if (timing) cudaEventRecord(ev.e[k], 0); };
+    auto report = [&]() {
+        if (!timing) return;
+        mark(5);
+        cudaEventSynchronize(ev.e[5]);
+        static const char* const phase[5] = {"build", "read-back", "triangle records", "pack", "frame refresh"};
+        for (int k = 0; k < 5; ++k) {
+            float ms = 0.f;
+            cudaEventElapsedTime(&ms, ev.e[k], ev.e[k + 1]);
+            fprintf(stderr, "trb_scene_update_mesh %s %.3f ms\n", phase[k], ms);
+        }
+    };
+    if (pos) {
+        float* d_pos = nullptr;
+        trb::DTri* d_tris = nullptr;
+        trb_bvh_node* d_nodes = nullptr; // the device-built tree (null after a host build)
+        HostMesh nm;
+        auto build = [&]() -> trb_status {
+            CU(s->arena.alloc(3 * nv, &d_pos));
+            CU(s->arena.alloc(dm.n_tris, &d_tris));
+            mark(0);
+            CU(copy_in(d_pos, pos, 3 * nv));
+            return build_mesh_bvh(s->tune.build_device != 0, d_pos, dm.indices, dm.n_tris, nm, d_tris, &d_nodes, ev.e[1], ev.e[2]);
+        };
+        { const trb_status r = build(); if (r != TRB_OK) { s->arena.release(d_pos); s->arena.release(d_tris); return r; } }
+        mark(3);
+        // the device is drained (build_mesh_bvh ends with a device synchronisation): nothing in flight reads what is replaced below
+        trb::DPair* pairs = const_cast<trb::DPair*>(dm.bvh.pairs);
+        size_t cap = hm.pair_cap;
+        auto records = [&](uint32_t n_rec, trb::DPair** out) -> trb_status {
+            if (n_rec > cap) { // the new tree has more interior nodes than the buffer holds: a larger one replaces it at the commit
+                trb::DPair* grown = nullptr;
+                CU(s->arena.alloc(n_rec, &grown));
+                pairs = grown; cap = n_rec;
+            }
+            *out = pairs;
+            return TRB_OK;
+        };
+        bool narrow = true;
+        trb_status r = TRB_OK;
+        if (d_nodes) {
+            r = pack_pairs_device(d_nodes, (uint32_t)nm.nodes.size(), s->wide_leaf, records, &narrow);
+            cudaFree(d_nodes);
+        } else { // host build: the records are packed on the host, as at creation. A tree that does not fit the scene's narrow form is
+                 // packed wide (the form changes below and every mesh is re-packed): either way the buffer is sized for its interior nodes
+            narrow = leaves_fit_narrow(nm.nodes);
+            std::vector<trb::DPair> pn;
+            trb::DBvh hdr{};
+            pack_pairs(nm.nodes, pn, hdr, s->wide_leaf || !narrow);
+            trb::DPair* out = nullptr;
+            r = records((uint32_t)pn.size(), &out);
+            if (r == TRB_OK && !pn.empty()) {
+                const cudaError_t e = cudaMemcpy(out, pn.data(), pn.size() * sizeof(trb::DPair), cudaMemcpyHostToDevice);
+                if (e != cudaSuccess) r = fail(TRB_CUDA, std::string("cudaMemcpy(node records): ") + cudaGetErrorString(e));
+            }
+        }
+        if (r != TRB_OK) {
+            s->arena.release(d_pos); s->arena.release(d_tris);
+            if (pairs != dm.bvh.pairs) s->arena.release(pairs);
+            return r;
+        }
+        mark(4);
+        // commit: positions, triangle records, tree and header
+        s->arena.release(dm.positions);
+        s->arena.release(dm.tris);
+        if (pairs != dm.bvh.pairs) s->arena.release(dm.bvh.pairs);
+        if (dm.bvh.quads) s->arena.release(dm.bvh.quads);
+        hm.nodes = std::move(nm.nodes); hm.order = std::move(nm.order);
+        hm.narrow = narrow; hm.pair_cap = cap;
+        for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
+        const trb_bvh_node& root = hm.nodes[0];
+        uint32_t root_ref = trb::REF_INTERIOR; // record 0
+        if (root.b & TRB_BVH_LEAF)
+            root_ref = s->wide_leaf ? (trb::REF_LEAF | (root.a & ~trb::REF_TAG)) : (trb::REF_LEAF | ((root.b & ~TRB_BVH_LEAF) << 25) | root.a);
+        dm.positions = d_pos; dm.tris = d_tris; dm.n_nodes = (uint32_t)hm.nodes.size();
+        dm.bvh.pairs = pairs; dm.bvh.quads = nullptr; // DQuad records (trace.quads) are built at creation only
+        dm.bvh.root_lo = make_float4(hm.bounds.lo[0], hm.bounds.lo[1], hm.bounds.lo[2], bits_f(root_ref));
+        dm.bvh.root_hi = make_float4(hm.bounds.hi[0], hm.bounds.hi[1], hm.bounds.hi[2], bits_f(QUAD_EMPTY_HOST));
+        s->quads_dropped = true;
+        s->needs_wide = false;
+        for (const HostMesh& m : s->meshes) if (!m.narrow) s->needs_wide = true;
+        const bool wide = s->needs_wide || s->tune.wide_leaf != 0;
+        if (wide != s->wide_leaf) { // the scene's leaf form changes with this tree: every mesh is re-packed, headers included
+            const trb_status rw = upload_mesh_nodes(s, wide);
+            if (rw != TRB_OK) return rw;
+        } else CU(cudaMemcpy(s->d_meshes + mi, &dm, sizeof dm, cudaMemcpyHostToDevice));
+    } else CU(cudaDeviceSynchronize()); // kernels in flight may read the attributes overwritten below
+    if (nrm) CU(copy_in(dm.normals, nrm, 3 * nv));
+    if (uv) CU(copy_in(dm.texcoords, uv, 2 * nv));
+    if (pos && s->frame_set) { // instance bounds and the TLAS over the new mesh bounds
+        const trb_status r = trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+        if (r != TRB_OK) return r;
+    }
+    report();
+    return TRB_OK;
 }
 
 } // namespace
 
 extern "C" {
+
+trb_status trb_scene_update_mesh(trb_scene* s, uint32_t mesh, const float* positions, const float* normals, const float* texcoords) {
+    return update_mesh(s, mesh, positions, normals, texcoords, false, nullptr);
+}
+trb_status trb_scene_update_mesh_device(trb_scene* s, uint32_t mesh, const float* d_positions, const float* d_normals, const float* d_texcoords,
+                                        void* cuda_stream) {
+    return update_mesh(s, mesh, d_positions, d_normals, d_texcoords, true, static_cast<cudaStream_t>(cuda_stream));
+}
 
 const char* trb_last_error(void) { return g_error.c_str(); }
 void trb_internal_set_error(const char* msg) { g_error = msg ? msg : ""; } // used by trb_loader.cpp
@@ -1354,15 +1536,12 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     for (uint32_t mi = 0; mi < d->n_meshes; ++mi) {
         const trb_mesh& m = d->meshes[mi];
         HostMesh& hm = s->meshes[mi];
-        hm.pos.assign(m.positions, m.positions + 3 * (size_t)m.n_verts);
-        hm.nrm.assign(m.normals, m.normals + 3 * (size_t)m.n_verts);
-        hm.uv.assign(m.texcoords, m.texcoords + 2 * (size_t)m.n_verts);
-        hm.idx.assign(m.indices, m.indices + 3 * (size_t)m.n_tris);
+        hm.n_verts = m.n_verts;
         float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
-        CU(s->arena.upload(hm.pos.data(), hm.pos.size(), &dp));
-        CU(s->arena.upload(hm.nrm.data(), hm.nrm.size(), &dn));
-        CU(s->arena.upload(hm.uv.data(), hm.uv.size(), &dt));
-        CU(s->arena.upload(hm.idx.data(), hm.idx.size(), &di));
+        CU(s->arena.upload(m.positions, 3 * (size_t)m.n_verts, &dp));
+        CU(s->arena.upload(m.normals, 3 * (size_t)m.n_verts, &dn));
+        CU(s->arena.upload(m.texcoords, 2 * (size_t)m.n_verts, &dt));
+        CU(s->arena.upload(m.indices, 3 * (size_t)m.n_tris, &di));
         CU(s->arena.alloc(m.n_tris, &dtris));
         { const trb_status r = build_mesh_bvh(s->tune.build_device != 0, dp, di, m.n_tris, hm, dtris); if (r != TRB_OK) return r; }
         for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
@@ -1380,8 +1559,9 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
             trb::DQuad* dquads;
             CU(s->arena.upload(qn.data(), qn.size(), &dquads));
             hdr.quads = dquads;
-        } else s->needs_wide = true;
+        } else { s->needs_wide = true; hm.narrow = false; }
         CU(s->arena.alloc(n_rec, &dnodes)); // filled by upload_mesh_nodes: both leaf forms have one record per interior node
+        hm.pair_cap = n_rec;
         hdr.pairs = dnodes;
         dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.tris = dtris;
         dm.n_nodes = (uint32_t)hm.nodes.size(); dm.n_tris = m.n_tris;

@@ -480,6 +480,39 @@ __global__ void k_tri_leaf_marks(const trb_bvh_node* __restrict__ nodes, uint32_
     if ((nd.b & TRB_BVH_LEAF) && cnt) tris[(size_t)nd.a + cnt - 1].e0.w = __uint_as_float(TRI_LEAF_END);
 }
 
+// ---- mesh helpers of trb_scene_update_mesh: the DPair records (trb_device.h) of a preorder tree still on the device
+// rec[i] = 1 for an interior node, rec[n] = 0; an exclusive scan then gives each interior node its record index and rec[n] the count
+__global__ void k_pair_flags(const trb_bvh_node* __restrict__ nodes, uint32_t n, uint32_t* __restrict__ rec) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    rec[i] = i < n && !(nodes[i].b & TRB_BVH_LEAF) ? 1u : 0u;
+}
+// One record per interior node in the layout of trb_api.cu's pack_pairs, leaves referenced in the narrow or the wide form.
+// *narrow_bad is set where a leaf does not fit the narrow reference, whichever form was asked for, so the caller learns which
+// form the tree needs. Every leaf fits the wide reference: a mesh holds at most 2^30 triangles and a leaf at least one.
+__device__ __forceinline__ uint32_t pair_ref(const trb_bvh_node& nd, uint32_t rec, bool wide) {
+    if (!(nd.b & TRB_BVH_LEAF)) return REF_INTERIOR | rec;
+    const uint32_t cnt = nd.b & ~TRB_BVH_LEAF, first = nd.a;
+    return wide ? (REF_LEAF | (first & ~REF_TAG)) : (REF_LEAF | (cnt << 25) | first);
+}
+__global__ void k_pair_pack(const trb_bvh_node* __restrict__ nodes, uint32_t n, const uint32_t* __restrict__ rec, bool wide,
+                            DPair* __restrict__ out, uint32_t* narrow_bad) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const trb_bvh_node nd = nodes[i];
+    if (nd.b & TRB_BVH_LEAF) {
+        if ((nd.b & ~TRB_BVH_LEAF) > 31 || nd.a >= (1u << 25)) *narrow_bad = 1u;
+        return;
+    }
+    const trb_bvh_node l = nodes[i + 1], r = nodes[nd.a];
+    DPair p;
+    p.l_lo = make_float4(l.bmin[0], l.bmin[1], l.bmin[2], __uint_as_float(pair_ref(l, rec[i + 1], wide)));
+    p.l_hi = make_float4(l.bmax[0], l.bmax[1], l.bmax[2], __uint_as_float(pair_ref(r, rec[nd.a], wide)));
+    p.r_lo = make_float4(r.bmin[0], r.bmin[1], r.bmin[2], __uint_as_float(nd.b));
+    p.r_hi = make_float4(r.bmax[0], r.bmax[1], r.bmax[2], 0.f);
+    out[rec[i]] = p;
+}
+
 // ---- host driver
 inline size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
 struct Scratch {
