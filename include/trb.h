@@ -362,6 +362,28 @@ trb_status trb_scene_update_mesh(trb_scene* scene, uint32_t mesh, const float* p
 trb_status trb_scene_update_mesh_device(trb_scene* scene, uint32_t mesh, const float* d_positions, const float* d_normals,
                                         const float* d_texcoords, void* cuda_stream);
 
+/* Scene edits: replace entries [first, first + count) of one array of the description. The structure of the scene (counts, index
+ * ranges, which instance is a light, which spline is keyframed) stays; only the values change. After a successful call the scene
+ * equals trb_scene_create on the description with those entries replaced and, if a frame has been set, that scene after
+ * trb_scene_update_frame with the last arguments given: TLAS, transforms, renders and their counters, Adaptive per-pixel counts,
+ * ray, illumination and shading queries, and the light list; films to rounding (they are added with atomics).
+ * Statuses: a null scene, a null array with count > 0, or a range past the end of the array (first + count computed in 64 bits) is
+ * TRB_INVALID_ARG; count 0 is TRB_OK and changes nothing, even with a null array. Each call drains the device before it overwrites
+ * anything that kernels read, and returns when the edit is complete. A failed call leaves the scene as it was, with one exception: a
+ * CUDA error (a device fault, not a property of the input) reported once the writes have begun may leave it half edited. */
+/* Replace keyframes[first .. first + count): the TRS control points of instance, group and camera transforms (trb_spline.ctrl_first
+ * indexes this array). Splines, knots and every other array keep their structure. If a frame has been set, it is rebuilt. */
+trb_status trb_scene_update_keyframes(trb_scene* scene, uint32_t first, uint32_t count, const trb_keyframe* keyframes);
+/* The same from a device array on the scene's GPU, read on cuda_stream (a cudaStream_t; NULL = default stream); returns when complete.
+ * A pointer that is not 4-byte aligned is TRB_INVALID_ARG. */
+trb_status trb_scene_update_keyframes_device(trb_scene* scene, uint32_t first, uint32_t count, const trb_keyframe* d_keyframes,
+                                             void* cuda_stream);
+/* Replace color_keys[first .. first + count): emission colours and their key times (AnimatedColor). The frame is not rebuilt. */
+trb_status trb_scene_update_color_keys(trb_scene* scene, uint32_t first, uint32_t count, const trb_color_key* keys);
+/* Replace materials[first .. first + count): type, colours, roughness, eta, MERL table, texture bindings. They are checked as
+ * trb_scene_create checks them, with its statuses and messages. The frame is not rebuilt. */
+trb_status trb_scene_update_materials(trb_scene* scene, uint32_t first, uint32_t count, const trb_material* materials);
+
 /* -- the hot path ------------------------------------------------------------------ */
 
 /* ≙ Exec::render (exec/mod.rs:48; multithreaded.rs:55-70). Renders the selected

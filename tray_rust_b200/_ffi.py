@@ -196,6 +196,10 @@ LIGHT_QUERY_DTYPE = np.dtype([("p", "<f4", 3), ("time", "<f4"), ("u", "<f4", 2),
 LIGHT_SAMPLE_DTYPE = np.dtype([("li", "<f4", 3), ("pdf", "<f4"), ("wi", "<f4", 3), ("delta", "<u4"), ("shadow", QUERY_RAY_DTYPE)])
 LIGHT_PDF_QUERY_DTYPE = np.dtype([("p", "<f4", 3), ("time", "<f4"), ("wi", "<f4", 3), ("light", "<u4")])
 EMIT_QUERY_DTYPE = np.dtype([("w", "<f4", 3), ("time", "<f4"), ("n", "<f4", 3), ("inst", "<u4")])
+KEYFRAME_DTYPE = np.dtype([("translation", "<f4", 3), ("rotation", "<f4", 4), ("scaling", "<f4", 3)])
+COLOR_KEY_DTYPE = np.dtype([("rgba", "<f4", 4), ("time", "<f4")])
+MATERIAL_DTYPE = np.dtype([("type", "<u4"), ("c0", "<f4", 3), ("c1", "<f4", 3), ("roughness", "<f4"), ("eta", "<f4"), ("merl", "<u4"),
+                           ("tex", "<u4", 4)])
 
 TRB_SYMBOLS = [
     "trb_scene_create", "trb_scene_load_json", "trb_scene_destroy", "trb_scene_info", "trb_scene_update_frame",
@@ -214,6 +218,7 @@ TRB_SYMBOLS = [
     "trb_film_write", "trb_film_write_device", "trb_camera_rays_device", "trb_host_film_to_srgb8",
     "trb_build_bvh", "trb_build_bvh_device",
     "trb_scene_update_mesh", "trb_scene_update_mesh_device",
+    "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
 ]
 
 _trb = None
@@ -244,6 +249,10 @@ def load_trb():
     lib.trb_scene_update_frame.argtypes = [vp, u32, f32, f32]
     lib.trb_scene_update_mesh.argtypes = [vp, u32, vp, vp, vp]
     lib.trb_scene_update_mesh_device.argtypes = [vp, u32, vp, vp, vp, vp]
+    lib.trb_scene_update_keyframes.argtypes = [vp, u32, u32, vp]
+    lib.trb_scene_update_keyframes_device.argtypes = [vp, u32, u32, vp, vp]
+    lib.trb_scene_update_color_keys.argtypes = [vp, u32, u32, vp]
+    lib.trb_scene_update_materials.argtypes = [vp, u32, u32, vp]
     lib.trb_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]

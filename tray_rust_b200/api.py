@@ -208,6 +208,38 @@ class Scene(_Base):
         self._mesh_verts(mesh)
         self._check(self._lib.trb_scene_update_mesh_device(self._h, mesh, d_positions, d_normals, d_texcoords, stream))
 
+    def _edit_range(self, name, first, count):
+        n = getattr(self._desc, "n_" + name)
+        if first < 0 or count < 0 or first + count > n:
+            raise ValueError("%s [%d, %d) out of range (%d entries)" % (name, first, first + count, n))
+
+    def _edit(self, name, dtype, first, a):
+        a = np.asarray(a)
+        if a.dtype != dtype or a.ndim != 1:
+            raise ValueError("%s must be a 1-d array of dtype %s, got %s %s" % (name, dtype, a.dtype, a.shape))
+        self._edit_range(name, first, len(a))
+        a = np.ascontiguousarray(a)
+        self._check(getattr(self._lib, "trb_scene_update_" + name)(self._h, first, len(a), F.ptr(a)))
+
+    def update_keyframes(self, first, keyframes):
+        """trb_scene_update_keyframes: replace keyframes[first:first + len(keyframes)] (F.KEYFRAME_DTYPE), the TRS control points of
+        instance, group and camera transforms; a frame already set is rebuilt."""
+        self._edit("keyframes", F.KEYFRAME_DTYPE, first, keyframes)
+
+    def update_keyframes_device(self, first, count, d_keyframes, stream=None):
+        """trb_scene_update_keyframes_device: the same from a device pointer (int) to `count` keyframes in F.KEYFRAME_DTYPE's layout,
+        read on `stream` (a cudaStream_t as an int; None = default stream)."""
+        self._edit_range("keyframes", first, count)
+        self._check(self._lib.trb_scene_update_keyframes_device(self._h, first, count, d_keyframes, stream))
+
+    def update_color_keys(self, first, keys):
+        """trb_scene_update_color_keys: replace color_keys[first:first + len(keys)] (F.COLOR_KEY_DTYPE), emission colours and times."""
+        self._edit("color_keys", F.COLOR_KEY_DTYPE, first, keys)
+
+    def update_materials(self, first, materials):
+        """trb_scene_update_materials: replace materials[first:first + len(materials)] (F.MATERIAL_DTYPE)."""
+        self._edit("materials", F.MATERIAL_DTYPE, first, materials)
+
     def set_option(self, name, value):
         """trb_scene_set_option: launch-shape options (never change results)."""
         self._check(self._lib.trb_scene_set_option(self._h, name.encode(), int(value)))

@@ -231,6 +231,7 @@ struct trb_scene {
     std::vector<trb_color_key> color_keys;
     std::vector<float> fov_floats;
     std::vector<trb_material> materials;
+    uint32_t n_merl = 0;                 // MERL tables of the description (a material edit is checked against it)
     std::vector<HostMesh> meshes;
     std::vector<trb::DMesh> dmeshes;     // the device mesh headers (d_meshes), kept to re-pack the node records (trace.wide_leaf)
     trb::DMesh* d_meshes = nullptr;
@@ -320,6 +321,14 @@ Box3 shape_bounds(const trb_scene& s, const trb_instance& in) {
     return b;
 }
 
+// One material of a description (trb_scene_create, trb_scene_update_materials)
+trb_status validate_material(const trb_material& m, uint32_t n_merl, uint32_t n_textures) {
+    if (m.type > TRB_MAT_MERL) return fail(TRB_INVALID_ARG, "unrecognized material type");
+    if (m.type == TRB_MAT_MERL && m.merl >= n_merl) return fail(TRB_INVALID_ARG, "merl table index out of range");
+    for (int k = 0; k < 4; ++k) if (m.tex[k] > n_textures) return fail(TRB_INVALID_ARG, "texture index out of range");
+    return TRB_OK;
+}
+
 trb_status validate(const trb_scene_desc* d) {
     if (!d) return fail(TRB_INVALID_ARG, "null scene description");
     if (d->abi_version != TRB_ABI_VERSION) return fail(TRB_INVALID_ARG, "trb_scene_desc.abi_version mismatch");
@@ -372,9 +381,8 @@ trb_status validate(const trb_scene_desc* d) {
         if ((uint64_t)c.spline_first + c.n_splines > d->n_splines) return fail(TRB_INVALID_ARG, "camera spline range out of bounds");
     }
     for (uint32_t i = 0; i < d->n_materials; ++i) {
-        if (d->materials[i].type > TRB_MAT_MERL) return fail(TRB_INVALID_ARG, "unrecognized material type");
-        if (d->materials[i].type == TRB_MAT_MERL && d->materials[i].merl >= d->n_merl) return fail(TRB_INVALID_ARG, "merl table index out of range");
-        for (int k = 0; k < 4; ++k) if (d->materials[i].tex[k] > d->n_textures) return fail(TRB_INVALID_ARG, "texture index out of range");
+        const trb_status r = validate_material(d->materials[i], d->n_merl, d->n_textures);
+        if (r != TRB_OK) return r;
     }
     uint64_t texels = 0;
     for (uint32_t i = 0; i < d->n_textures; ++i)
@@ -1025,6 +1033,56 @@ bool static_instance_records(const trb_scene* s, std::vector<trb::DInstance>& di
     return any_anim;
 }
 
+// The device record of a material: what Material::bsdf recomputes per hit from constant textures, precomputed
+trb::DMaterial device_material(const trb_material& m) {
+    trb::DMaterial o;
+    std::memset(&o, 0, sizeof o);
+    o.type = m.type;
+    for (int k = 0; k < 3; ++k) { o.c0[k] = m.c0[k]; o.c1[k] = m.c1[k]; }
+    o.roughness = m.roughness; o.eta = m.eta;
+    o.width = fmaxf(m.roughness, 0.000001f);         // Beckmann::new (beckmann.rs:19-22)
+    float sigma = kPi / 180.0f * m.roughness;        // OrenNayar::new (oren_nayar.rs:26-34), roughness in degrees
+    sigma *= sigma;
+    o.on_a = 1.0f - 0.5f * sigma / (sigma + 0.33f);
+    o.on_b = 0.45f * sigma / (sigma + 0.09f);
+    o.merl_off = m.type == TRB_MAT_MERL ? m.merl * TRB_MERL_TABLE_FLOATS : 0;
+    for (int k = 0; k < 4; ++k) o.tex[k] = m.tex[k];
+    return o;
+}
+
+// The material kinds of the hittable instances, which choose the shading kernels (launch_shade)
+void material_shape(trb_scene* s) {
+    uint32_t kinds = 0;
+    for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_EMITTER_POINT && in.material < s->materials.size()) kinds |= 1u << s->materials[in.material].type;
+    // two kinds are enough: with the material buckets the split kernels run one kind's code at a time, the fused kernel runs every
+    // kind a warp holds
+    s->mixed_materials = __builtin_popcount(kinds) >= 2 || (kinds & (1u << TRB_MAT_MERL)) != 0;
+    s->material_kinds = kinds;
+}
+
+// DScene::level_xf of spline k: Keyframe::transform of a one-control-point level (identity, unused, for keyframed splines)
+Xf level_transform(const trb_scene* s, size_t k) {
+    return s->splines[k].n_ctrl == 1 ? keyframe_xf(s->keyframes[s->splines[k].ctrl_first]) : xf_identity();
+}
+
+// Distinct keyframed splines by content (degree, knots, control keyframes compared bit for bit): uniq_of per spline (0xffffffff for
+// one-control-point levels), uniq_list a representative spline of each (DScene::spline_uniq, uniq_splines)
+void spline_dedup(const trb_scene* s, std::vector<uint32_t>& uniq_of, std::vector<uint32_t>& uniq_list) {
+    uniq_of.assign(s->splines.size(), 0xffffffffu);
+    uniq_list.clear();
+    auto same = [&](const trb_spline& a, const trb_spline& b) {
+        return a.degree == b.degree && a.n_ctrl == b.n_ctrl && a.n_knots == b.n_knots &&
+               memcmp(&s->keyframes[a.ctrl_first], &s->keyframes[b.ctrl_first], a.n_ctrl * sizeof(trb_keyframe)) == 0 &&
+               memcmp(&s->knots[a.knot_first], &s->knots[b.knot_first], a.n_knots * sizeof(float)) == 0;
+    };
+    for (size_t k = 0; k < s->splines.size(); ++k) {
+        if (s->splines[k].n_ctrl <= 1) continue;
+        for (size_t u = 0; u < uniq_list.size() && uniq_of[k] == 0xffffffffu; ++u)
+            if (same(s->splines[k], s->splines[uniq_list[u]])) uniq_of[k] = (uint32_t)u;
+        if (uniq_of[k] == 0xffffffffu) { uniq_of[k] = (uint32_t)uniq_list.size(); uniq_list.push_back((uint32_t)k); }
+    }
+}
+
 // ---- shading queries (trb_bsdf_eval / trb_bsdf_sample / trb_light_sample / trb_light_pdf / trb_emitted; DESIGN.md §5) ------------------
 // Argument checks: `a` and `b` are the input buffers (the light and emission queries have one and pass it twice), read with 16-byte
 // loads on the device; `out_align` is the device output's required alignment. `frame`: the query reads the instance matrices.
@@ -1416,9 +1474,117 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
     return TRB_OK;
 }
 
+// ---- description edits (trb_scene_update_keyframes / _color_keys / _materials; DESIGN.md §4 "Scene edits") ----------------------
+// The argument checks, before anything is read: entries [first, first + count) of an array of n. *done: nothing to do (count 0).
+trb_status edit_check(const trb_scene* s, uint32_t first, uint32_t count, const void* a, size_t n, bool device, bool* done) {
+    *done = false;
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (count == 0) { *done = true; return TRB_OK; }
+    if (!a) return fail(TRB_INVALID_ARG, "null array");
+    if ((uint64_t)first + count > n) return fail(TRB_INVALID_ARG, "edit range out of bounds");
+    if (device && (reinterpret_cast<uintptr_t>(a) & 3u)) return fail(TRB_INVALID_ARG, "device array must be 4-byte aligned");
+    return TRB_OK;
+}
+
+// The host mirror, the device keyframe table, the level transforms of the one-control-point splines whose point was edited and, when
+// a keyframed spline's control points were edited, the distinct-spline tables; then the frame, as update_frame built it
+trb_status update_keyframes(trb_scene* s, uint32_t first, uint32_t count, const trb_keyframe* kf) {
+    CU(cudaSetDevice(s->device));
+    CU(cudaDeviceSynchronize()); // kernels in flight may read what is overwritten below
+    std::copy(kf, kf + count, s->keyframes.begin() + first);
+    CU(cudaMemcpy(const_cast<trb_keyframe*>(s->ds.keyframes) + first, kf, count * sizeof(trb_keyframe), cudaMemcpyHostToDevice));
+    const uint64_t last = (uint64_t)first + count;
+    size_t lo = s->splines.size(), hi = 0;
+    bool keyed = false;
+    for (size_t k = 0; k < s->splines.size(); ++k) {
+        const trb_spline& sp = s->splines[k];
+        if (sp.ctrl_first >= last || (uint64_t)sp.ctrl_first + sp.n_ctrl <= first) continue;
+        if (sp.n_ctrl == 1) { lo = std::min(lo, k); hi = std::max(hi, k); }
+        else keyed = true;
+    }
+    if (lo <= hi) { // the span between the first and the last edited level
+        std::vector<Xf> level(hi - lo + 1);
+        for (size_t k = lo; k <= hi; ++k) level[k - lo] = level_transform(s, k);
+        CU(cudaMemcpy(const_cast<Xf*>(s->ds.level_xf) + lo, level.data(), level.size() * sizeof(Xf), cudaMemcpyHostToDevice));
+    }
+    if (keyed) {
+        std::vector<uint32_t> uniq_of, uniq_list;
+        spline_dedup(s, uniq_of, uniq_list);
+        CU(cudaMemcpy(const_cast<uint32_t*>(s->ds.spline_uniq), uniq_of.data(), uniq_of.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(const_cast<uint32_t*>(s->ds.uniq_splines), uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        s->ds.n_uniq_splines = (uint32_t)uniq_list.size();
+    }
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    return TRB_OK;
+}
+
+// The host mirror, the device colour-key table and the static emission of the instance records whose first key was edited. Only
+// the emission fields are written: the device frame path uploads the rest of the records once and then writes the matrices alone.
+trb_status update_color_keys(trb_scene* s, uint32_t first, uint32_t count, const trb_color_key* keys) {
+    CU(cudaSetDevice(s->device));
+    CU(cudaDeviceSynchronize());
+    std::copy(keys, keys + count, s->color_keys.begin() + first);
+    CU(cudaMemcpy(const_cast<trb_color_key*>(s->ds.color_keys) + first, keys, count * sizeof(trb_color_key), cudaMemcpyHostToDevice));
+    std::vector<trb::DInstance> di;
+    std::vector<uint32_t> anim_list;
+    static_instance_records(s, di, anim_list);
+    size_t lo = di.size(), hi = 0;
+    for (size_t i = 0; i < di.size(); ++i) {
+        const trb_instance& in = s->instances[i];
+        if (in.kind != TRB_INST_RECEIVER && in.emission_first >= first && in.emission_first - first < count) { lo = std::min(lo, i); hi = std::max(hi, i); }
+    }
+    if (lo <= hi)
+        CU(cudaMemcpy2D(s->d_instances[lo].emission, sizeof(trb::DInstance), di[lo].emission, sizeof(trb::DInstance), sizeof di[lo].emission,
+                        hi - lo + 1, cudaMemcpyHostToDevice));
+    return TRB_OK;
+}
+
+// Checked as trb_scene_create checks them; then the host mirror, the device records and the shading shape (material_shape)
+trb_status update_materials(trb_scene* s, uint32_t first, uint32_t count, const trb_material* m) {
+    for (uint32_t i = 0; i < count; ++i) {
+        const trb_status r = validate_material(m[i], s->n_merl, s->ds.n_textures);
+        if (r != TRB_OK) return r;
+    }
+    std::vector<trb::DMaterial> dm(count);
+    for (uint32_t i = 0; i < count; ++i) dm[i] = device_material(m[i]);
+    CU(cudaSetDevice(s->device));
+    CU(cudaDeviceSynchronize());
+    std::copy(m, m + count, s->materials.begin() + first);
+    CU(cudaMemcpy(const_cast<trb::DMaterial*>(s->ds.materials) + first, dm.data(), count * sizeof(trb::DMaterial), cudaMemcpyHostToDevice));
+    material_shape(s);
+    return TRB_OK;
+}
+
 } // namespace
 
 extern "C" {
+
+trb_status trb_scene_update_keyframes(trb_scene* s, uint32_t first, uint32_t count, const trb_keyframe* keyframes) {
+    bool done;
+    const trb_status r = edit_check(s, first, count, keyframes, s ? s->keyframes.size() : 0, false, &done);
+    return r != TRB_OK || done ? r : update_keyframes(s, first, count, keyframes);
+}
+trb_status trb_scene_update_keyframes_device(trb_scene* s, uint32_t first, uint32_t count, const trb_keyframe* d_keyframes, void* cuda_stream) {
+    bool done;
+    const trb_status r = edit_check(s, first, count, d_keyframes, s ? s->keyframes.size() : 0, true, &done);
+    if (r != TRB_OK || done) return r;
+    CU(cudaSetDevice(s->device));
+    const cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    std::vector<trb_keyframe> kf(count);
+    CU(cudaMemcpyAsync(kf.data(), d_keyframes, count * sizeof(trb_keyframe), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    return update_keyframes(s, first, count, kf.data());
+}
+trb_status trb_scene_update_color_keys(trb_scene* s, uint32_t first, uint32_t count, const trb_color_key* keys) {
+    bool done;
+    const trb_status r = edit_check(s, first, count, keys, s ? s->color_keys.size() : 0, false, &done);
+    return r != TRB_OK || done ? r : update_color_keys(s, first, count, keys);
+}
+trb_status trb_scene_update_materials(trb_scene* s, uint32_t first, uint32_t count, const trb_material* materials) {
+    bool done;
+    const trb_status r = edit_check(s, first, count, materials, s ? s->materials.size() : 0, false, &done);
+    return r != TRB_OK || done ? r : update_materials(s, first, count, materials);
+}
 
 trb_status trb_scene_update_mesh(trb_scene* s, uint32_t mesh, const float* positions, const float* normals, const float* texcoords) {
     return update_mesh(s, mesh, positions, normals, texcoords, false, nullptr);
@@ -1572,23 +1738,10 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
 
     // materials (precompute what Material::bsdf recomputes per hit from constant textures)
     std::vector<trb::DMaterial> dmats(d->n_materials);
-    for (uint32_t i = 0; i < d->n_materials; ++i) {
-        const trb_material& m = d->materials[i];
-        trb::DMaterial& o = dmats[i];
-        std::memset(&o, 0, sizeof o);
-        o.type = m.type;
-        for (int k = 0; k < 3; ++k) { o.c0[k] = m.c0[k]; o.c1[k] = m.c1[k]; }
-        o.roughness = m.roughness; o.eta = m.eta;
-        o.width = fmaxf(m.roughness, 0.000001f);         // Beckmann::new (beckmann.rs:19-22)
-        float sigma = kPi / 180.0f * m.roughness;        // OrenNayar::new (oren_nayar.rs:26-34), roughness in degrees
-        sigma *= sigma;
-        o.on_a = 1.0f - 0.5f * sigma / (sigma + 0.33f);
-        o.on_b = 0.45f * sigma / (sigma + 0.09f);
-        o.merl_off = m.type == TRB_MAT_MERL ? m.merl * TRB_MERL_TABLE_FLOATS : 0;
-        for (int k = 0; k < 4; ++k) o.tex[k] = m.tex[k];
-    }
+    for (uint32_t i = 0; i < d->n_materials; ++i) dmats[i] = device_material(d->materials[i]);
     trb::DMaterial* d_mats;
     CU(s->arena.upload(dmats.data(), dmats.size(), &d_mats));
+    s->n_merl = d->n_merl;
     float* d_merl = nullptr;
     CU(s->arena.alloc((size_t)d->n_merl * TRB_MERL_TABLE_FLOATS, &d_merl));
     for (uint32_t i = 0; i < d->n_merl; ++i)
@@ -1624,14 +1777,7 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     CU(s->arena.alloc(d->n_instances, &s->d_instances));
     CU(s->arena.alloc(d->n_instances, &s->d_anim_instances));
     for (const trb_instance& in : s->instances) if (!trbh::xf_is_static(s->splines.data(), in.spline_first, in.n_splines)) s->n_anim++;
-    {
-        uint32_t kinds = 0;
-        for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_EMITTER_POINT && in.material < s->materials.size()) kinds |= 1u << s->materials[in.material].type;
-        // two kinds are enough: with the material buckets the split kernels run one kind's code at a time, the fused kernel runs every
-        // kind a warp holds
-        s->mixed_materials = __builtin_popcount(kinds) >= 2 || (kinds & (1u << TRB_MAT_MERL)) != 0;
-        s->material_kinds = kinds;
-    }
+    material_shape(s.get());
     CU(s->arena.alloc(1, &s->d_counter));
     CU(s->arena.alloc(1, &s->d_error));
     CU(cudaMemset(s->d_error, 0, sizeof(int)));
@@ -1658,27 +1804,20 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
         if (!s->keyframes.empty()) CU(s->arena.upload(s->keyframes.data(), s->keyframes.size(), &d_kf));
         if (!s->knots.empty()) CU(s->arena.upload(s->knots.data(), s->knots.size(), &d_kn));
         if (!s->color_keys.empty()) CU(s->arena.upload(s->color_keys.data(), s->color_keys.size(), &d_ck));
-        std::vector<Xf> level(s->splines.size(), xf_identity());
-        for (size_t k = 0; k < s->splines.size(); ++k)
-            if (s->splines[k].n_ctrl == 1) level[k] = keyframe_xf(s->keyframes[s->splines[k].ctrl_first]);
+        std::vector<Xf> level(s->splines.size());
+        for (size_t k = 0; k < s->splines.size(); ++k) level[k] = level_transform(s.get(), k);
         Xf* d_lv = nullptr;
         if (!level.empty()) CU(s->arena.upload(level.data(), level.size(), &d_lv));
-        // distinct keyframed splines by content (degree, knots, control keyframes compared bit for bit)
-        std::vector<uint32_t> uniq_of(s->splines.size(), 0xffffffffu), uniq_list;
-        auto same = [&](const trb_spline& a, const trb_spline& b) {
-            return a.degree == b.degree && a.n_ctrl == b.n_ctrl && a.n_knots == b.n_knots &&
-                   memcmp(&s->keyframes[a.ctrl_first], &s->keyframes[b.ctrl_first], a.n_ctrl * sizeof(trb_keyframe)) == 0 &&
-                   memcmp(&s->knots[a.knot_first], &s->knots[b.knot_first], a.n_knots * sizeof(float)) == 0;
-        };
-        for (size_t k = 0; k < s->splines.size(); ++k) {
-            if (s->splines[k].n_ctrl <= 1) continue;
-            for (size_t u = 0; u < uniq_list.size() && uniq_of[k] == 0xffffffffu; ++u)
-                if (same(s->splines[k], s->splines[uniq_list[u]])) uniq_of[k] = (uint32_t)u;
-            if (uniq_of[k] == 0xffffffffu) { uniq_of[k] = (uint32_t)uniq_list.size(); uniq_list.push_back((uint32_t)k); }
-        }
+        std::vector<uint32_t> uniq_of, uniq_list;
+        spline_dedup(s.get(), uniq_of, uniq_list);
         uint32_t* d_uo = nullptr; uint32_t* d_ul = nullptr;
         if (!uniq_of.empty()) CU(s->arena.upload(uniq_of.data(), uniq_of.size(), &d_uo));
-        if (!uniq_list.empty()) CU(s->arena.upload(uniq_list.data(), uniq_list.size(), &d_ul));
+        // room for every keyframed spline: a keyframe edit can make splines that were equal distinct (trb_scene_update_keyframes)
+        const size_t n_keyed = (size_t)std::count_if(s->splines.begin(), s->splines.end(), [](const trb_spline& sp) { return sp.n_ctrl > 1; });
+        if (n_keyed) {
+            CU(s->arena.alloc(n_keyed, &d_ul));
+            CU(cudaMemcpy(d_ul, uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        }
         ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
         ds.splines = d_sp; ds.keyframes = d_kf; ds.knots = d_kn; ds.color_keys = d_ck; ds.level_xf = d_lv; ds.has_anim = 0;
     }

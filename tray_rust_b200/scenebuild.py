@@ -373,6 +373,20 @@ def scene_heightfield(grid=4200, width=1920, height=1080, spp=4, seed=0x4E16F1D)
     return b
 
 
+def scene_instances(k, seed, width=64, height=64, spp=4, radius=0.3):
+    """A Cornell box holding k small sphere receivers at seeded positions, each with a one-level static transform: the instance-heavy
+    scene of the scene-edit tests and benchmark (every receiver's keyframe is one entry of the description's keyframes)."""
+    b = SceneBuilder(width, height, spp, 2, 6)
+    mats = cornell_walls(b)
+    cornell_light(b, mats["white"])
+    mat = b.add_material(F.MAT_MATTE, (0.74, 0.74, 0.73), roughness=1.0)
+    rng = np.random.Generator(np.random.PCG64(seed))
+    for t in rng.uniform((-13, 1, -8), (13, 22, 18), size=(k, 3)):
+        b.receiver(F.SHAPE_SPHERE, mat, [trs(t=t, s=radius)], p0=1.0)
+    b.add_camera([trs(t=(0, 12, -60))], fov=30.0)
+    return b
+
+
 def scene_c3(width=800, height=600, spp=2048, subdiv=6, n_tris=69451):
     """SURVEY.md §8d C3 stand-in: Cornell box + a noisy icosphere cut to the Stanford bunny's 69 451 triangles (the bunny is not
     in the reference repo). The subdivision-6 icosphere has 81 920 faces; the lowest ones (a cap resting towards the floor) are
