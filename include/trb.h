@@ -363,7 +363,8 @@ trb_status trb_scene_update_mesh_device(trb_scene* scene, uint32_t mesh, const f
                                         const float* d_texcoords, void* cuda_stream);
 
 /* Scene edits: replace entries [first, first + count) of one array of the description. The structure of the scene (counts, index
- * ranges, which instance is a light, which spline is keyframed) stays; only the values change. After a successful call the scene
+ * ranges, which instance is a light, which spline is keyframed) stays; only the values change (trb_scene_replace_objects, below,
+ * changes the structure). After a successful call the scene
  * equals trb_scene_create on the description with those entries replaced and, if a frame has been set, that scene after
  * trb_scene_update_frame with the last arguments given: TLAS, transforms, renders and their counters, Adaptive per-pixel counts,
  * ray, illumination and shading queries, and the light list; films to rounding (they are added with atomics).
@@ -383,6 +384,34 @@ trb_status trb_scene_update_color_keys(trb_scene* scene, uint32_t first, uint32_
 /* Replace materials[first .. first + count): type, colours, roughness, eta, MERL table, texture bindings. They are checked as
  * trb_scene_create checks them, with its statuses and messages. The frame is not rebuilt. */
 trb_status trb_scene_update_materials(trb_scene* scene, uint32_t first, uint32_t count, const trb_material* materials);
+
+/* The object section of a trb_scene_desc: everything Scene::load_file builds from "camera(s)" and "objects"
+ * (scene.rs:185-260, 480-628). Same field meanings, same index conventions as in trb_scene_desc. */
+typedef struct trb_scene_objects {
+    uint32_t n_cameras;    const trb_camera* cameras;
+    uint32_t n_instances;  const trb_instance* instances;
+    uint32_t n_splines;    const trb_spline* splines;
+    uint32_t n_keyframes;  const trb_keyframe* keyframes;
+    uint32_t n_knots;      const float* knots;
+    uint32_t n_color_keys; const trb_color_key* color_keys;
+    uint32_t n_fov_floats; const float* fov_floats;
+} trb_scene_objects;
+
+/* Object replacement: replace the scene's cameras, instances, splines, keyframes, knots, colour keys and fov floats with the seven
+ * arrays of `objects`. Every count may differ from the scene's current one, in either direction, so objects, lights and cameras can
+ * be added and removed, instances bound to another mesh, material or shape, receivers turned into emitters and static transforms
+ * into keyframed ones. trb_instance.mesh and .material index the scene's existing meshes and materials, which stay as they are
+ * with their trees, as do the MERL tables, textures, film, integrator and options. After a successful call the scene equals
+ * trb_scene_create on the description with the seven arrays replaced and, if a frame has been set, that scene after
+ * trb_scene_update_frame with the last arguments given (the camera is selected as on a new scene's first frame), on everything the
+ * scene edits above list.
+ * The section is checked before anything is written, by the code that checks it in trb_scene_create, with the same statuses and
+ * messages; mesh and material indices are checked against the scene's counts. A null scene or null `objects`, or a null array with a
+ * non-zero count, is TRB_INVALID_ARG, as is a section none of whose cameras is active at the frame that has been set. The call
+ * drains the device before it frees or overwrites anything that kernels read, and returns when the replacement is complete. A
+ * failed call leaves the scene as it was, with one exception: a CUDA error (a device fault, not a property of the input) reported
+ * once the scene has been switched to the new section, while the frame is rebuilt, may leave it without a frame. */
+trb_status trb_scene_replace_objects(trb_scene* scene, const trb_scene_objects* objects);
 
 /* -- the hot path ------------------------------------------------------------------ */
 

@@ -97,6 +97,17 @@ class SceneDesc(C.Structure):
                 ("n_images", u32), ("images", C.POINTER(Image))]
 
 
+class SceneObjects(C.Structure):
+    """trb_scene_objects: the object section of a SceneDesc, with the same field names"""
+    _fields_ = [("n_cameras", u32), ("cameras", C.POINTER(Camera)),
+                ("n_instances", u32), ("instances", C.POINTER(Instance)),
+                ("n_splines", u32), ("splines", C.POINTER(Spline)),
+                ("n_keyframes", u32), ("keyframes", C.POINTER(Keyframe)),
+                ("n_knots", u32), ("knots", C.POINTER(f32)),
+                ("n_color_keys", u32), ("color_keys", C.POINTER(ColorKey)),
+                ("n_fov_floats", u32), ("fov_floats", C.POINTER(f32))]
+
+
 class RenderCfg(C.Structure):
     _fields_ = [("spp", u32), ("sample_first", u32), ("sample_count", u32), ("block_start", u32),
                 ("block_count", u32), ("current_frame", u32), ("seed", u32), ("flags", u32),
@@ -219,6 +230,7 @@ TRB_SYMBOLS = [
     "trb_build_bvh", "trb_build_bvh_device",
     "trb_scene_update_mesh", "trb_scene_update_mesh_device",
     "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
+    "trb_scene_replace_objects",
 ]
 
 _trb = None
@@ -253,6 +265,7 @@ def load_trb():
     lib.trb_scene_update_keyframes_device.argtypes = [vp, u32, u32, vp, vp]
     lib.trb_scene_update_color_keys.argtypes = [vp, u32, u32, vp]
     lib.trb_scene_update_materials.argtypes = [vp, u32, u32, vp]
+    lib.trb_scene_replace_objects.argtypes = [vp, C.POINTER(SceneObjects)]
     lib.trb_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]

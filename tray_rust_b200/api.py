@@ -240,6 +240,20 @@ class Scene(_Base):
         """trb_scene_update_materials: replace materials[first:first + len(materials)] (F.MATERIAL_DTYPE)."""
         self._edit("materials", F.MATERIAL_DTYPE, first, materials)
 
+    def replace_objects(self, objects):
+        """trb_scene_replace_objects: replace the cameras, instances, splines, keyframes, knots, colour keys and fov floats with the
+        section `objects` (F.SceneObjects, e.g. SceneBuilder.objects()); meshes, materials, textures, film and integrator stay. Counts
+        may change: this adds and removes objects, lights and cameras. A frame already set is rebuilt."""
+        self._check(self._lib.trb_scene_replace_objects(self._h, C.byref(objects)))
+        desc = F.SceneDesc.from_buffer_copy(self._desc)  # a copy: the caller's description (it may belong to the loader) stays as it is
+        for name, _ in F.SceneObjects._fields_:
+            setattr(desc, name, getattr(objects, name))
+        desc._keep = (self._desc, objects)  # the arrays both point into
+        self._desc = desc
+        ni, nl = F.u32(), F.u32()
+        self._check(self._lib.trb_scene_info(self._h, None, None, None, None, C.byref(ni), C.byref(nl)))
+        self.n_instances, self.n_lights = ni.value, nl.value
+
     def set_option(self, name, value):
         """trb_scene_set_option: launch-shape options (never change results)."""
         self._check(self._lib.trb_scene_set_option(self._h, name.encode(), int(value)))

@@ -329,57 +329,71 @@ trb_status validate_material(const trb_material& m, uint32_t n_merl, uint32_t n_
     return TRB_OK;
 }
 
+// The object section of a description (trb_scene_create, trb_scene_replace_objects); mesh and material indices against the counts given
+trb_status validate_objects(const trb_scene_objects& o, uint32_t n_meshes, uint32_t n_materials) {
+    if (o.n_instances == 0) return fail(TRB_INVALID_ARG, "Aborting: the scene does not have any objects!"); // scene.rs:134
+    if (o.n_cameras == 0) return fail(TRB_INVALID_ARG, "Error: A camera is required!");
+    if (!o.cameras || !o.instances || (o.n_splines && !o.splines) || (o.n_keyframes && !o.keyframes) || (o.n_knots && !o.knots) ||
+        (o.n_color_keys && !o.color_keys) || (o.n_fov_floats && !o.fov_floats))
+        return fail(TRB_INVALID_ARG, "null array with a non-zero count");
+    bool light = false;
+    for (uint32_t i = 0; i < o.n_instances; ++i) {
+        const trb_instance& in = o.instances[i];
+        if (in.kind > TRB_INST_EMITTER_POINT || in.shape > TRB_SHAPE_MESH) return fail(TRB_INVALID_ARG, "unknown instance kind/shape");
+        if (in.kind != TRB_INST_EMITTER_POINT && in.shape == TRB_SHAPE_NONE) return fail(TRB_INVALID_ARG, "instance without geometry");
+        if (in.kind == TRB_INST_EMITTER_AREA && in.shape == TRB_SHAPE_MESH)
+            return fail(TRB_INVALID_ARG, "Geometry of type 'mesh' is not sampleable and can't be used for area light geometry"); // scene.rs:577-579
+        if (in.shape == TRB_SHAPE_MESH && in.mesh >= n_meshes) return fail(TRB_INVALID_ARG, "mesh index out of range");
+        if (in.kind != TRB_INST_EMITTER_POINT && in.material >= n_materials) return fail(TRB_INVALID_ARG, "material index out of range");
+        if ((uint64_t)in.spline_first + in.n_splines > o.n_splines) return fail(TRB_INVALID_ARG, "spline range out of bounds");
+        if (in.kind != TRB_INST_RECEIVER) {
+            light = true;
+            if (in.n_emission == 0 || (uint64_t)in.emission_first + in.n_emission > o.n_color_keys) return fail(TRB_INVALID_ARG, "An emission color is required for emitters");
+        }
+    }
+    for (uint32_t k = 0; k < o.n_splines; ++k) { // BSpline::new's invariants (bspline 0.2.2) + the device evaluator's degree cap
+        const trb_spline& sp = o.splines[k];
+        if (sp.n_ctrl == 0 || (uint64_t)sp.ctrl_first + sp.n_ctrl > o.n_keyframes) return fail(TRB_INVALID_ARG, "spline control points out of bounds");
+        if (sp.n_ctrl > 1) {
+            if ((uint64_t)sp.knot_first + sp.n_knots > o.n_knots) return fail(TRB_INVALID_ARG, "spline knots out of bounds");
+            if (sp.n_ctrl <= sp.degree) return fail(TRB_INVALID_ARG, "Too few control points for curve"); // BSpline::new panics with this message
+            if ((uint64_t)sp.n_knots != (uint64_t)sp.n_ctrl + sp.degree + 1) return fail(TRB_INVALID_ARG, "Invalid B-spline: knots.len() != control_points.len() + degree + 1");
+            if (sp.degree > (uint32_t)trbh::kMaxSplineDegree) return fail(TRB_UNSUPPORTED, "B-spline degree above 5");
+            for (uint32_t i = 0; i < sp.n_knots; ++i) if (o.knots[sp.knot_first + i] != o.knots[sp.knot_first + i]) return fail(TRB_INVALID_ARG, "NaN knot in B-spline"); // BSpline::new sorts with partial_cmp().unwrap(): panics on NaN
+        }
+    }
+    if (!light) return fail(TRB_INVALID_ARG, "At least one light is required"); // multithreaded.rs:39
+    for (uint32_t i = 0; i < o.n_cameras; ++i) {
+        const trb_camera& c = o.cameras[i];
+        if (c.n_fov_ctrl) { // CameraFov::Animated (camera.rs:95-125)
+            if ((uint64_t)c.fov_ctrl_first + c.n_fov_ctrl > o.n_fov_floats || (uint64_t)c.fov_knot_first + c.n_fov_knots > o.n_fov_floats) return fail(TRB_INVALID_ARG, "fov spline out of bounds");
+            if (c.n_fov_ctrl <= c.fov_degree) return fail(TRB_INVALID_ARG, "Too few control points for curve");
+            if ((uint64_t)c.n_fov_knots != (uint64_t)c.n_fov_ctrl + c.fov_degree + 1) return fail(TRB_INVALID_ARG, "Invalid B-spline: knots.len() != control_points.len() + degree + 1");
+            for (uint32_t i = 0; i < c.n_fov_knots; ++i) if (o.fov_floats[c.fov_knot_first + i] != o.fov_floats[c.fov_knot_first + i]) return fail(TRB_INVALID_ARG, "NaN knot in B-spline");
+            if (c.fov_degree > (uint32_t)trbh::kMaxSplineDegree) return fail(TRB_UNSUPPORTED, "B-spline degree above 5");
+        }
+        if ((uint64_t)c.spline_first + c.n_splines > o.n_splines) return fail(TRB_INVALID_ARG, "camera spline range out of bounds");
+    }
+    return TRB_OK;
+}
+
+trb_scene_objects desc_objects(const trb_scene_desc& d) {
+    return {d.n_cameras, d.cameras, d.n_instances, d.instances, d.n_splines, d.splines, d.n_keyframes, d.keyframes,
+            d.n_knots, d.knots, d.n_color_keys, d.color_keys, d.n_fov_floats, d.fov_floats};
+}
+
 trb_status validate(const trb_scene_desc* d) {
     if (!d) return fail(TRB_INVALID_ARG, "null scene description");
     if (d->abi_version != TRB_ABI_VERSION) return fail(TRB_INVALID_ARG, "trb_scene_desc.abi_version mismatch");
     if (d->film.width == 0 || d->film.height == 0 || d->film.width % 8 || d->film.height % 8)
         return fail(TRB_INVALID_ARG, "Image not evenly divided by blocks of (8, 8)"); // block_queue.rs:29-31
     if (d->film.frames == 0) return fail(TRB_INVALID_ARG, "film.frames must be >= 1");
-    if (d->n_instances == 0) return fail(TRB_INVALID_ARG, "Aborting: the scene does not have any objects!"); // scene.rs:134
-    if (d->n_cameras == 0) return fail(TRB_INVALID_ARG, "Error: A camera is required!");
     if (d->integrator.type > TRB_INTEGRATOR_NORMALS_DEBUG) return fail(TRB_INVALID_ARG, "Unrecognized integrator type"); // scene.rs:313
     if (d->integrator.type == TRB_INTEGRATOR_PATH && d->integrator.max_depth > 57u) return fail(TRB_UNSUPPORTED, "max_depth > 57");
     if (d->integrator.type == TRB_INTEGRATOR_WHITTED && d->integrator.max_depth > 24u) return fail(TRB_UNSUPPORTED, "whitted max_depth > 24 (device recursion stack)");
     if (!(d->film.filter_w > 0.0f && d->film.filter_h > 0.0f)) return fail(TRB_INVALID_ARG, "filter width/height must be positive");
     if (floorf(d->film.filter_w / 0.5f) > 8.0f || floorf(d->film.filter_h / 0.5f) > 8.0f) return fail(TRB_UNSUPPORTED, "filter wider than 4 pixels");
-    bool light = false;
-    for (uint32_t i = 0; i < d->n_instances; ++i) {
-        const trb_instance& in = d->instances[i];
-        if (in.kind > TRB_INST_EMITTER_POINT || in.shape > TRB_SHAPE_MESH) return fail(TRB_INVALID_ARG, "unknown instance kind/shape");
-        if (in.kind != TRB_INST_EMITTER_POINT && in.shape == TRB_SHAPE_NONE) return fail(TRB_INVALID_ARG, "instance without geometry");
-        if (in.kind == TRB_INST_EMITTER_AREA && in.shape == TRB_SHAPE_MESH)
-            return fail(TRB_INVALID_ARG, "Geometry of type 'mesh' is not sampleable and can't be used for area light geometry"); // scene.rs:577-579
-        if (in.shape == TRB_SHAPE_MESH && in.mesh >= d->n_meshes) return fail(TRB_INVALID_ARG, "mesh index out of range");
-        if (in.kind != TRB_INST_EMITTER_POINT && in.material >= d->n_materials) return fail(TRB_INVALID_ARG, "material index out of range");
-        if ((uint64_t)in.spline_first + in.n_splines > d->n_splines) return fail(TRB_INVALID_ARG, "spline range out of bounds");
-        if (in.kind != TRB_INST_RECEIVER) {
-            light = true;
-            if (in.n_emission == 0 || (uint64_t)in.emission_first + in.n_emission > d->n_color_keys) return fail(TRB_INVALID_ARG, "An emission color is required for emitters");
-        }
-    }
-    for (uint32_t k = 0; k < d->n_splines; ++k) { // BSpline::new's invariants (bspline 0.2.2) + the device evaluator's degree cap
-        const trb_spline& sp = d->splines[k];
-        if (sp.n_ctrl == 0 || (uint64_t)sp.ctrl_first + sp.n_ctrl > d->n_keyframes) return fail(TRB_INVALID_ARG, "spline control points out of bounds");
-        if (sp.n_ctrl > 1) {
-            if ((uint64_t)sp.knot_first + sp.n_knots > d->n_knots) return fail(TRB_INVALID_ARG, "spline knots out of bounds");
-            if (sp.n_ctrl <= sp.degree) return fail(TRB_INVALID_ARG, "Too few control points for curve"); // BSpline::new panics with this message
-            if ((uint64_t)sp.n_knots != (uint64_t)sp.n_ctrl + sp.degree + 1) return fail(TRB_INVALID_ARG, "Invalid B-spline: knots.len() != control_points.len() + degree + 1");
-            if (sp.degree > (uint32_t)trbh::kMaxSplineDegree) return fail(TRB_UNSUPPORTED, "B-spline degree above 5");
-            for (uint32_t i = 0; i < sp.n_knots; ++i) if (d->knots[sp.knot_first + i] != d->knots[sp.knot_first + i]) return fail(TRB_INVALID_ARG, "NaN knot in B-spline"); // BSpline::new sorts with partial_cmp().unwrap(): panics on NaN
-        }
-    }
-    if (!light) return fail(TRB_INVALID_ARG, "At least one light is required"); // multithreaded.rs:39
-    for (uint32_t i = 0; i < d->n_cameras; ++i) {
-        const trb_camera& c = d->cameras[i];
-        if (c.n_fov_ctrl) { // CameraFov::Animated (camera.rs:95-125)
-            if ((uint64_t)c.fov_ctrl_first + c.n_fov_ctrl > d->n_fov_floats || (uint64_t)c.fov_knot_first + c.n_fov_knots > d->n_fov_floats) return fail(TRB_INVALID_ARG, "fov spline out of bounds");
-            if (c.n_fov_ctrl <= c.fov_degree) return fail(TRB_INVALID_ARG, "Too few control points for curve");
-            if ((uint64_t)c.n_fov_knots != (uint64_t)c.n_fov_ctrl + c.fov_degree + 1) return fail(TRB_INVALID_ARG, "Invalid B-spline: knots.len() != control_points.len() + degree + 1");
-            for (uint32_t i = 0; i < c.n_fov_knots; ++i) if (d->fov_floats[c.fov_knot_first + i] != d->fov_floats[c.fov_knot_first + i]) return fail(TRB_INVALID_ARG, "NaN knot in B-spline");
-            if (c.fov_degree > (uint32_t)trbh::kMaxSplineDegree) return fail(TRB_UNSUPPORTED, "B-spline degree above 5");
-        }
-        if ((uint64_t)c.spline_first + c.n_splines > d->n_splines) return fail(TRB_INVALID_ARG, "camera spline range out of bounds");
-    }
+    { const trb_status r = validate_objects(desc_objects(*d), d->n_meshes, d->n_materials); if (r != TRB_OK) return r; }
     for (uint32_t i = 0; i < d->n_materials; ++i) {
         const trb_status r = validate_material(d->materials[i], d->n_merl, d->n_textures);
         if (r != TRB_OK) return r;
@@ -1555,6 +1569,100 @@ trb_status update_materials(trb_scene* s, uint32_t first, uint32_t count, const 
     return TRB_OK;
 }
 
+
+// ---- the object section (trb_scene_create, trb_scene_replace_objects; DESIGN.md §4 "Object replacement") ------------------------
+// Makes `o`, already checked by validate_objects, the scene's object section: the host copy (knots sorted as BSpline::new sorts
+// them), the light list, the instance records without matrices (so that trb_emitted runs before the first update_frame), the
+// animation tables, and what the kernels' choice depends on (n_anim, material_shape, anim_emission). Needs the scene's meshes and
+// materials in place. The new device buffers are complete before DScene is switched over and the ones they replace are released, so
+// a failure leaves the scene as it was. The caller has drained the device.
+trb_status set_objects(trb_scene* s, const trb_scene_objects& o) {
+    std::vector<trb_camera> cameras(o.cameras, o.cameras + o.n_cameras);
+    std::vector<trb_instance> instances(o.instances, o.instances + o.n_instances);
+    std::vector<trb_spline> splines(o.splines, o.splines + o.n_splines);
+    std::vector<trb_keyframe> keyframes(o.keyframes, o.keyframes + o.n_keyframes);
+    std::vector<float> knots(o.knots, o.knots + o.n_knots), fov_floats(o.fov_floats, o.fov_floats + o.n_fov_floats);
+    std::vector<trb_color_key> color_keys(o.color_keys, o.color_keys + o.n_color_keys);
+    for (const trb_spline& sp : splines) // BSpline::new sorts its knots (bspline 0.2.2); ranges were bounds-checked by validate_objects()
+        if (sp.n_ctrl > 1) std::stable_sort(knots.begin() + sp.knot_first, knots.begin() + sp.knot_first + sp.n_knots);
+    for (const trb_camera& c : cameras)
+        if (c.n_fov_ctrl) std::stable_sort(fov_floats.begin() + c.fov_knot_first, fov_floats.begin() + c.fov_knot_first + c.n_fov_knots);
+    // the helpers below read the section from the scene: the current one is kept in the locals until the device buffers exist
+    auto swap_host = [&] {
+        s->cameras.swap(cameras); s->instances.swap(instances); s->splines.swap(splines); s->keyframes.swap(keyframes);
+        s->knots.swap(knots); s->fov_floats.swap(fov_floats); s->color_keys.swap(color_keys);
+    };
+    swap_host();
+    std::vector<uint32_t> lights;
+    for (uint32_t i = 0; i < o.n_instances; ++i) if (s->instances[i].kind != TRB_INST_RECEIVER) lights.push_back(i); // multithreaded.rs:33-38
+    std::vector<trb::DInstance> di;
+    std::vector<uint32_t> anim_list, uniq_of, uniq_list;
+    static_instance_records(s, di, anim_list);
+    std::vector<Xf> level(s->splines.size());
+    for (size_t k = 0; k < level.size(); ++k) level[k] = level_transform(s, k);
+    spline_dedup(s, uniq_of, uniq_list);
+    // room for every keyframed spline: a keyframe edit can make splines that were equal distinct (trb_scene_update_keyframes)
+    const size_t n_keyed = (size_t)std::count_if(s->splines.begin(), s->splines.end(), [](const trb_spline& sp) { return sp.n_ctrl > 1; });
+
+    DeviceArena fresh; // frees what it holds if an allocation or upload fails
+    uint32_t *d_lights = nullptr, *d_anim = nullptr, *d_uo = nullptr, *d_ul = nullptr;
+    trb::DInstance* d_inst = nullptr;
+    trb_spline* d_sp = nullptr; trb_keyframe* d_kf = nullptr; float* d_kn = nullptr; trb_color_key* d_ck = nullptr; Xf* d_lv = nullptr;
+    const trb_status r = [&]() -> trb_status {
+        CU(fresh.upload(lights.data(), lights.size(), &d_lights));
+        CU(fresh.upload(di.data(), di.size(), &d_inst));
+        CU(fresh.alloc(di.size(), &d_anim)); // update_frame fills it
+        if (!s->splines.empty()) CU(fresh.upload(s->splines.data(), s->splines.size(), &d_sp));
+        if (!s->keyframes.empty()) CU(fresh.upload(s->keyframes.data(), s->keyframes.size(), &d_kf));
+        if (!s->knots.empty()) CU(fresh.upload(s->knots.data(), s->knots.size(), &d_kn));
+        if (!s->color_keys.empty()) CU(fresh.upload(s->color_keys.data(), s->color_keys.size(), &d_ck));
+        if (!level.empty()) CU(fresh.upload(level.data(), level.size(), &d_lv));
+        if (!uniq_of.empty()) CU(fresh.upload(uniq_of.data(), uniq_of.size(), &d_uo));
+        if (n_keyed) {
+            CU(fresh.alloc(n_keyed, &d_ul));
+            CU(cudaMemcpy(d_ul, uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        }
+        return TRB_OK;
+    }();
+    if (r != TRB_OK) { swap_host(); return r; }
+
+    trb::DScene& ds = s->ds;
+    for (const void* p : {(const void*)ds.lights, (const void*)s->d_instances, (const void*)s->d_anim_instances, (const void*)ds.splines,
+                          (const void*)ds.keyframes, (const void*)ds.knots, (const void*)ds.color_keys, (const void*)ds.level_xf,
+                          (const void*)ds.spline_uniq, (const void*)ds.uniq_splines}) s->arena.release(p);
+    s->arena.ptrs.insert(s->arena.ptrs.end(), fresh.ptrs.begin(), fresh.ptrs.end());
+    fresh.ptrs.clear();
+    s->d_instances = d_inst; s->d_anim_instances = d_anim;
+    ds.instances = d_inst; ds.n_instances = o.n_instances; ds.lights = d_lights; ds.n_lights = (uint32_t)lights.size();
+    ds.splines = d_sp; ds.keyframes = d_kf; ds.knots = d_kn; ds.color_keys = d_ck; ds.level_xf = d_lv;
+    ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
+    ds.has_anim = 0; ds.anim_instances = nullptr; ds.n_anim_instances = 0; // update_frame sets them
+    s->n_anim = (uint32_t)anim_list.size();
+    material_shape(s);
+    s->anim_emission = false;
+    for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_RECEIVER && in.n_emission > 1) s->anim_emission = true;
+    return TRB_OK;
+}
+
+// Checked as trb_scene_create checks the section, and that the frame that has been set can be set again; then set_objects, the
+// state that was sized or built for the old section, and the frame
+trb_status replace_objects(trb_scene* s, const trb_scene_objects& o) {
+    const trb_status v = validate_objects(o, (uint32_t)s->meshes.size(), (uint32_t)s->materials.size());
+    if (v != TRB_OK) return v;
+    if (s->frame_set && o.cameras[0].active_at > s->last_frame) return fail(TRB_INVALID_ARG, "no camera is active at this frame");
+    CU(cudaSetDevice(s->device));
+    CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
+    const trb_status r = set_objects(s, o);
+    if (r != TRB_OK) return r;
+    // nothing of the old instance list's frame survives; the camera is selected as on a new scene's first frame (scene.rs:153-166)
+    s->frame_ready = false; s->instances_static_uploaded = false; s->host_frame_stale = false;
+    s->world.clear(); s->tlas_nodes.clear(); s->tlas_order.clear(); s->tlas_n_nodes = 0;
+    s->active_camera = -1;
+    if (s->wf.n_anim != s->n_anim) s->wf_capacity = 0; // WfState::xf_tab is sized by n_anim: ensure_wavefront allocates the state anew
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    return TRB_OK;
+}
+
 } // namespace
 
 extern "C" {
@@ -1592,6 +1700,12 @@ trb_status trb_scene_update_mesh(trb_scene* s, uint32_t mesh, const float* posit
 trb_status trb_scene_update_mesh_device(trb_scene* s, uint32_t mesh, const float* d_positions, const float* d_normals, const float* d_texcoords,
                                         void* cuda_stream) {
     return update_mesh(s, mesh, d_positions, d_normals, d_texcoords, true, static_cast<cudaStream_t>(cuda_stream));
+}
+
+trb_status trb_scene_replace_objects(trb_scene* s, const trb_scene_objects* objects) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (!objects) return fail(TRB_INVALID_ARG, "null objects");
+    return replace_objects(s, *objects);
 }
 
 const char* trb_last_error(void) { return g_error.c_str(); }
@@ -1683,17 +1797,6 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     s->sm_count = prop.multiProcessorCount;
     s->film = d->film; s->integrator = d->integrator;
     s->spp_pow2 = pow2_ceil(std::max(1u, d->film.samples));
-    s->cameras.assign(d->cameras, d->cameras + d->n_cameras);
-    s->instances.assign(d->instances, d->instances + d->n_instances);
-    s->splines.assign(d->splines, d->splines + d->n_splines);
-    s->keyframes.assign(d->keyframes, d->keyframes + d->n_keyframes);
-    s->knots.assign(d->knots, d->knots + d->n_knots);
-    for (const trb_spline& sp : s->splines) // BSpline::new sorts its knots (bspline 0.2.2); ranges were bounds-checked by validate()
-        if (sp.n_ctrl > 1) std::stable_sort(s->knots.begin() + sp.knot_first, s->knots.begin() + sp.knot_first + sp.n_knots);
-    s->color_keys.assign(d->color_keys, d->color_keys + d->n_color_keys);
-    if (d->n_fov_floats) s->fov_floats.assign(d->fov_floats, d->fov_floats + d->n_fov_floats);
-    for (const trb_camera& c : s->cameras)
-        if (c.n_fov_ctrl) std::stable_sort(s->fov_floats.begin() + c.fov_knot_first, s->fov_floats.begin() + c.fov_knot_first + c.n_fov_knots);
     s->materials.assign(d->materials, d->materials + d->n_materials);
 
     // meshes: BVH<Triangle> with max_geom 16 (mesh.rs:44), then leaf-ordered triangle records
@@ -1765,19 +1868,10 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
         CU(s->arena.upload(tx.data(), tx.size(), &d_tx));
         s->ds.images = d_img; s->ds.textures = d_tex; s->ds.texels = d_tx; s->ds.n_textures = d->n_textures;
     }
-    std::vector<uint32_t> lights;
-    for (uint32_t i = 0; i < d->n_instances; ++i) if (d->instances[i].kind != TRB_INST_RECEIVER) lights.push_back(i); // multithreaded.rs:33-38
-    uint32_t* d_lights;
-    CU(s->arena.upload(lights.data(), lights.size(), &d_lights));
-
     filter_table(d->film, s->table);
     float* d_table;
     CU(s->arena.upload(s->table, 256, &d_table));
 
-    CU(s->arena.alloc(d->n_instances, &s->d_instances));
-    CU(s->arena.alloc(d->n_instances, &s->d_anim_instances));
-    for (const trb_instance& in : s->instances) if (!trbh::xf_is_static(s->splines.data(), in.spline_first, in.n_splines)) s->n_anim++;
-    material_shape(s.get());
     CU(s->arena.alloc(1, &s->d_counter));
     CU(s->arena.alloc(1, &s->d_error));
     CU(cudaMemset(s->d_error, 0, sizeof(int)));
@@ -1788,8 +1882,7 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     CU(cudaEventCreate(&s->ev1));
 
     trb::DScene& ds = s->ds;
-    ds.instances = s->d_instances; ds.meshes = d_meshes; ds.materials = d_mats; ds.merl = d_merl; ds.lights = d_lights;
-    ds.n_instances = d->n_instances; ds.n_lights = (uint32_t)lights.size();
+    ds.meshes = d_meshes; ds.materials = d_mats; ds.merl = d_merl;
     ds.width = d->film.width; ds.height = d->film.height;
     ds.min_depth = d->integrator.min_depth; ds.max_depth = d->integrator.max_depth;
     ds.filter_w = d->film.filter_w; ds.filter_h = d->film.filter_h;
@@ -1798,36 +1891,7 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     // the per-pixel test accepts |d| <= w / inv_w; the lock-block filter of render_target.rs:104-109 can only reject beyond fpw - 0.5
     ds.film_block_filter = (d->film.filter_w / ds.filter_inv_w <= (float)ds.fpw_x && d->film.filter_h / ds.filter_inv_h <= (float)ds.fpw_y) ? 0u : 1u;
     ds.filter_table = d_table;
-    { // animation tables (evaluated per ray for keyframed instances / camera / emission)
-        trb_spline* d_sp = nullptr; trb_keyframe* d_kf = nullptr; float* d_kn = nullptr; trb_color_key* d_ck = nullptr;
-        if (!s->splines.empty()) CU(s->arena.upload(s->splines.data(), s->splines.size(), &d_sp));
-        if (!s->keyframes.empty()) CU(s->arena.upload(s->keyframes.data(), s->keyframes.size(), &d_kf));
-        if (!s->knots.empty()) CU(s->arena.upload(s->knots.data(), s->knots.size(), &d_kn));
-        if (!s->color_keys.empty()) CU(s->arena.upload(s->color_keys.data(), s->color_keys.size(), &d_ck));
-        std::vector<Xf> level(s->splines.size());
-        for (size_t k = 0; k < s->splines.size(); ++k) level[k] = level_transform(s.get(), k);
-        Xf* d_lv = nullptr;
-        if (!level.empty()) CU(s->arena.upload(level.data(), level.size(), &d_lv));
-        std::vector<uint32_t> uniq_of, uniq_list;
-        spline_dedup(s.get(), uniq_of, uniq_list);
-        uint32_t* d_uo = nullptr; uint32_t* d_ul = nullptr;
-        if (!uniq_of.empty()) CU(s->arena.upload(uniq_of.data(), uniq_of.size(), &d_uo));
-        // room for every keyframed spline: a keyframe edit can make splines that were equal distinct (trb_scene_update_keyframes)
-        const size_t n_keyed = (size_t)std::count_if(s->splines.begin(), s->splines.end(), [](const trb_spline& sp) { return sp.n_ctrl > 1; });
-        if (n_keyed) {
-            CU(s->arena.alloc(n_keyed, &d_ul));
-            CU(cudaMemcpy(d_ul, uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-        }
-        ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
-        ds.splines = d_sp; ds.keyframes = d_kf; ds.knots = d_kn; ds.color_keys = d_ck; ds.level_xf = d_lv; ds.has_anim = 0;
-    }
-    { // the instance records without matrices, so that trb_emitted runs before the first update_frame
-        std::vector<trb::DInstance> di;
-        std::vector<uint32_t> anim_list;
-        static_instance_records(s.get(), di, anim_list);
-        CU(cudaMemcpy(s->d_instances, di.data(), di.size() * sizeof(trb::DInstance), cudaMemcpyHostToDevice));
-        for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_RECEIVER && in.n_emission > 1) s->anim_emission = true;
-    }
+    { const trb_status r = set_objects(s.get(), desc_objects(*d)); if (r != TRB_OK) return r; }
     // Scene::load_file builds the BVH<Instance> for [0, scene_time] (scene.rs:141); the first render rebuilds it
     *out = s.release();
     return TRB_OK;
@@ -1896,6 +1960,10 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
     if (static_instance_records(s, di, anim_list)) any_anim = true;
     s->ds.has_anim = any_anim ? 1u : 0u;
     if (n + 1 > s->tlas_capacity) { // a tree over n instances has < n interior records and < 2n nodes
+        for (const void* p : {(const void*)s->d_tlas_quads, (const void*)s->d_tlas, (const void*)s->d_tlas_order, (const void*)s->d_tlas_nodes,
+                              (const void*)s->d_bounds, (const void*)s->d_build_f, (const void*)s->d_build_u, (const void*)s->d_build_counts})
+            s->arena.release(p); // grown after trb_scene_replace_objects added instances (the device was drained above)
+        s->tlas_capacity = 0; s->frame_ready = false;
         CU(s->arena.alloc(n + 1, &s->d_tlas_quads));
         CU(s->arena.alloc(n + 1, &s->d_tlas));
         CU(s->arena.alloc(n, &s->d_tlas_order));

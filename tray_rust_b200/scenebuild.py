@@ -152,14 +152,31 @@ class SceneBuilder:
         else:
             self.cameras.append((sf, ns, float(fov), float(shutter_size), active_at, 0, 0, 0, 0, 0))
 
-    # -- finish ---------------------------------------------------------------------------
-    def finish(self):
-        d = F.SceneDesc()
-        d.abi_version = F.TRB_ABI_VERSION
-        d.film = F.Film(**self.film)
-        d.integrator = F.Integrator(*self.integrator)
-        keep = self._keep
+    def remove_instance(self, i):
+        """Drop instance i with the splines, keyframes, knots and colour keys it owns, and renumber what the remaining instances, splines
+        and cameras reference: the builder is then the one that never added it. Returns the removed instance's tuple."""
+        inst = self.instances.pop(i)
+        sf, ns, ef, ne = inst[6:10]
+        gone = self.splines[sf:sf + ns]
 
+        def cut(items, ranges):
+            """delete [first, first + n) for each range; returns the new index of an old one"""
+            ranges = sorted(r for r in ranges if r[1])
+            for first, n in reversed(ranges):
+                del items[first:first + n]
+            return lambda idx: idx - sum(n for first, n in ranges if first < idx)
+        kf = cut(self.keyframes, [(sp[2], sp[1]) for sp in gone])
+        kn = cut(self.knots, [(sp[4], sp[3]) for sp in gone])
+        sp_ = cut(self.splines, [(sf, ns)])
+        ck = cut(self.color_keys, [(ef, ne)])
+        self.splines = [(d, nc, kf(cf), nk, kn(kf0)) for d, nc, cf, nk, kf0 in self.splines]
+        self.instances = [it[:6] + (sp_(it[6]), it[7], ck(it[8]), it[9]) for it in self.instances]
+        self.cameras = [(sp_(c[0]),) + c[1:] for c in self.cameras]
+        return inst
+
+    # -- finish ---------------------------------------------------------------------------
+    def _fill_objects(self, d, keep):
+        """the object section's seven arrays and counts into d (a SceneDesc or a SceneObjects: same field names)"""
         def arr(ctype, items, conv):
             a = (ctype * max(1, len(items)))()
             for i, it in enumerate(items):
@@ -185,6 +202,36 @@ class SceneBuilder:
             (o.kind, o.shape, o.p0, o.p1, o.mesh, o.material, o.spline_first, o.n_splines, o.emission_first, o.n_emission) = it
         d.instances = arr(F.Instance, self.instances, inst); d.n_instances = len(self.instances)
 
+        def cam(o, it):
+            (o.spline_first, o.n_splines, o.fov, o.shutter_size, o.active_at, o.fov_degree, o.n_fov_ctrl, o.fov_ctrl_first, o.n_fov_knots,
+             o.fov_knot_first) = it
+        d.cameras = arr(F.Camera, self.cameras, cam); d.n_cameras = len(self.cameras)
+        ff = (F.f32 * max(1, len(self.fov_floats)))(*self.fov_floats); keep.append(ff)
+        d.fov_floats = ff; d.n_fov_floats = len(self.fov_floats)
+
+    def objects(self):
+        """The builder's object section (trb_scene_objects) for Scene.replace_objects: after b.receiver(...) on the builder a scene was
+        created from, scene.replace_objects(b.objects()) adds that receiver to the scene."""
+        o = F.SceneObjects()
+        o._keep = []
+        self._fill_objects(o, o._keep)
+        return o
+
+    def finish(self):
+        d = F.SceneDesc()
+        d.abi_version = F.TRB_ABI_VERSION
+        d.film = F.Film(**self.film)
+        d.integrator = F.Integrator(*self.integrator)
+        keep = self._keep
+
+        def arr(ctype, items, conv):
+            a = (ctype * max(1, len(items)))()
+            for i, it in enumerate(items):
+                conv(a[i], it)
+            keep.append(a)
+            return a
+        self._fill_objects(d, keep)
+
         def mesh(o, it):
             p, n, t, i = it
             o.n_verts, o.n_tris = len(p), len(i)
@@ -202,13 +249,6 @@ class SceneBuilder:
             mt[i] = t.ctypes.data_as(C.POINTER(F.f32))
         keep.append(mt); keep.append(self.merl)
         d.merl_tables = mt; d.n_merl = len(self.merl)
-
-        def cam(o, it):
-            (o.spline_first, o.n_splines, o.fov, o.shutter_size, o.active_at, o.fov_degree, o.n_fov_ctrl, o.fov_ctrl_first, o.n_fov_knots,
-             o.fov_knot_first) = it
-        d.cameras = arr(F.Camera, self.cameras, cam); d.n_cameras = len(self.cameras)
-        ff = (F.f32 * max(1, len(self.fov_floats)))(*self.fov_floats); keep.append(ff)
-        d.fov_floats = ff; d.n_fov_floats = len(self.fov_floats)
 
         def tex(o, it):
             o.first_image, o.n_images = it
