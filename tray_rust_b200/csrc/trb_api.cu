@@ -196,7 +196,24 @@ struct Tuning {
     int shade_kind = 1;        // split shading with buckets: the matte bucket goes through _b / _c instantiations compiled for matte alone
     uint64_t pass_paths = 1ull << 24; // camera samples per wavefront pass (the frame is rendered in additive passes)
     int build_device = 1;      // scene creation: mesh BVHs built on the device (trb_bvh_build.cuh); 0 = on the host, as when the build's scratch does not fit
+    long long tlas_min = -1;   // frame: test option — the instance count from which the device frame path builds the instance tree with the level
+                               // builder instead of one thread; -1 = kTlasLevelMin. The tree does not depend on it
+    int frame_time = 0;        // TRB_FRAME_TIME=1: trb_scene_update_frame prints its phases to stderr
+    int tlas_small = 8;        // frame: the level builder's serial-subtree threshold (TRB_FRAME_TLAS_SMALL; swept below; the tree does not depend on it)
 };
+// The instance tree of a frame (device path). One thread (k_tlas_build) is two launches and no synchronisation but the final
+// read-back; the level builder (bvhb::build_device) is tens of launches and a stream synchronisation per level, and overtakes it
+// once the serial build costs more than those. tools/tlas_bench.py, scene_instances(k), NVIDIA H100 80GB HBM3 at a 700 W limit, median
+// of five update_frame calls alternating the two, two calls of the tool, one-thread / level builder in ms: k = 10: 0.19-0.44 / 0.57-0.82;
+// 100: 0.78-0.88 / 1.30-1.70; 10^3: 6.62-6.83 / 1.90-2.22; 10^4: 87.0-87.9 / 2.44-2.60; 10^5: 1167 / 3.95-4.09. The one-thread build
+// grows by about 6.5 us per instance and the level builder by a level (about 0.1 ms) per doubling, so the two meet near 200 instances;
+// the level builder runs from 256, where interpolation puts it at 1.4 ms against 1.8 ms.
+constexpr uint32_t kTlasLevelMin = 256;
+// Tuning::tlas_small, the level builder's serial-subtree threshold for the instance tree (meshes use bvhb::SMALL = 1024, but a thousand
+// boxes cost one thread about 6 ms, the k = 10^3 figure above, which a frame cannot hide). Swept with
+// TRB_FRAME_TLAS_SMALL under tools/tlas_bench.py on an NVIDIA H100 80GB HBM3 at a 700 W limit, update_frame in ms at 10^3 / 10^5 instances:
+// 8: 1.79 / 3.32; 16: 2.28 / 4.00; 32: 3.36 / 5.13; 64: 5.49 / 8.71; 128: 8.49 / 17.1; 1024: 19.3 / 178. At 8 the level loop (17 levels,
+// 2.29 ms at 10^5) outweighs the serial subtrees (0.30 ms); at 32 it is the reverse (1.79 / 2.42 ms).
 int env_int(const char* name, int dflt) { const char* v = getenv(name); return v ? (int)strtol(v, nullptr, 0) : dflt; }
 void tuning_from_env(Tuning& t) {
     t.refill = env_int("TRB_REFILL", t.refill); t.trace_grid = (unsigned)env_int("TRB_TRACE_GRID", (int)t.trace_grid);
@@ -206,6 +223,8 @@ void tuning_from_env(Tuning& t) {
     t.sort_min_round = env_int("TRB_SORT_MIN_ROUND", t.sort_min_round); t.shade_split = env_int("TRB_SHADE_SPLIT", t.shade_split); t.anim_table = env_int("TRB_ANIM_TABLE", t.anim_table); t.frame_device = env_int("TRB_FRAME_DEVICE", t.frame_device);
     if (getenv("TRB_PASS_PATHS")) t.pass_paths = strtoull(getenv("TRB_PASS_PATHS"), nullptr, 0);
     t.build_device = env_int("TRB_BUILD_DEVICE", t.build_device);
+    t.tlas_min = env_int("TRB_FRAME_TLAS_MIN", (int)t.tlas_min); t.frame_time = env_int("TRB_FRAME_TIME", t.frame_time);
+    t.tlas_small = std::max(4, env_int("TRB_FRAME_TLAS_SMALL", t.tlas_small)); // the level kernels have no case for fewer than five boxes
 }
 
 } // namespace
@@ -240,6 +259,8 @@ struct trb_scene {
     bool wide_leaf = false;              // the mesh node records hold wide leaf references: the WIDE kernel instantiations run
     uint32_t spp_pow2 = 1;
     uint32_t n_anim = 0;                 // instances whose transform stack is keyframed (evaluated per path into WfState::xf_tab)
+    std::vector<uint32_t> anim_list;     // those instances, and whether any instance's transform or emission depends on time: properties
+    bool inst_any_anim = false;          // of the object section (static_instance_records), kept so that a frame need not rebuild the records
     bool frame_set = false; uint32_t last_frame = 0; float last_start = 0, last_end = 0; // the arguments of the last update_frame (re-run when an option changes what it builds)
     uint32_t material_kinds = 0;         // bit k: some hittable instance's material is of kind k (TRB_MAT_*)
     bool mixed_materials = false;        // the hittable instances use >= 2 material kinds or a MERL table: the split shade kernels with material buckets win (Tuning::shade_split = -1)
@@ -267,6 +288,8 @@ struct trb_scene {
     float* d_build_f = nullptr;
     uint32_t* d_build_u = nullptr;
     uint32_t* d_build_counts = nullptr;
+    char* d_build_level = nullptr;       // the level builder's scratch, top tree and scan storage (LevelScratch) for tlas_capacity - 1 instances,
+                                         // allocated with the first frame that runs it and released where the capacity grows
     uint32_t tlas_n_nodes = 0;
     bool instances_static_uploaded = false, host_frame_stale = false;
     std::vector<BlockList> block_lists;
@@ -1597,7 +1620,7 @@ trb_status set_objects(trb_scene* s, const trb_scene_objects& o) {
     for (uint32_t i = 0; i < o.n_instances; ++i) if (s->instances[i].kind != TRB_INST_RECEIVER) lights.push_back(i); // multithreaded.rs:33-38
     std::vector<trb::DInstance> di;
     std::vector<uint32_t> anim_list, uniq_of, uniq_list;
-    static_instance_records(s, di, anim_list);
+    const bool inst_any_anim = static_instance_records(s, di, anim_list);
     std::vector<Xf> level(s->splines.size());
     for (size_t k = 0; k < level.size(); ++k) level[k] = level_transform(s, k);
     spline_dedup(s, uniq_of, uniq_list);
@@ -1638,6 +1661,7 @@ trb_status set_objects(trb_scene* s, const trb_scene_objects& o) {
     ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
     ds.has_anim = 0; ds.anim_instances = nullptr; ds.n_anim_instances = 0; // update_frame sets them
     s->n_anim = (uint32_t)anim_list.size();
+    s->anim_list.swap(anim_list); s->inst_any_anim = inst_any_anim;
     material_shape(s);
     s->anim_emission = false;
     for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_RECEIVER && in.n_emission > 1) s->anim_emission = true;
@@ -1725,6 +1749,11 @@ trb_status trb_scene_set_option(trb_scene* s, const char* name, long long value)
         int& field = k == "trace.quads" ? t.quads : t.frame_device;
         const bool changed = (field != 0) != (value != 0);
         field = (int)value;
+        if (changed && s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    }
+    else if (k == "frame.tlas_min") { // which builder makes the instance tree: rebuild the current frame with the one now chosen
+        const bool changed = t.tlas_min != value;
+        t.tlas_min = value;
         if (changed && s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
     }
     else if (k == "trace.pipe") t.pipe = (int)value;
@@ -1911,12 +1940,38 @@ trb_status trb_scene_info(const trb_scene* s, uint32_t* w, uint32_t* h, uint32_t
     return TRB_OK;
 }
 
+namespace {
+// The level builder's memory for frames of up to n instances (the scene's instance capacity), carved from trb_scene::d_build_level: the build's scratch and top tree
+// (bvhb::OwnedScratch), then the record ranks (one per node and one past the end), the narrow-misfit word and the scan's storage
+struct LevelScratch {
+    trb::bvhb::OwnedScratch own; uint32_t* rec; uint32_t* narrow_bad; void* cub; size_t cub_bytes; size_t bytes;
+    LevelScratch(uint32_t n, uint32_t small, char* base) {
+        size_t off = 0;
+        auto take = [&](size_t b) { char* p = base ? base + off : nullptr; off += trb::bvhb::align_up(b); return p; };
+        own.base = take(trb::bvhb::scratch_layout(n, nullptr, small).bytes);
+        own.tn = (trb::bvhb::TNode*)take(trb::bvhb::top_cap(n) * sizeof(trb::bvhb::TNode));
+        rec = (uint32_t*)take(4 * (2 * (size_t)n + 1));
+        narrow_bad = (uint32_t*)take(4);
+        cub_bytes = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, 2 * (int)n);
+        cub = take(cub_bytes);
+        bytes = off;
+    }
+};
+// TRB_FRAME_TIME=1: the phases of the device frame path, timed with CUDA events on the default stream, to stderr
+struct FrameEvents {
+    cudaEvent_t e[6] = {};
+    ~FrameEvents() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+};
+} // namespace
+
 trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, float end) {
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     CU(cudaSetDevice(s->device));
     // A frame boundary: passes enqueued with trb_render_device may still be reading the instances / TLAS this call
     // overwrites, so the device is drained first (the reference's update_frame likewise runs between renders, scene.rs:152).
     CU(cudaDeviceSynchronize());
+    const auto t_host = std::chrono::steady_clock::now();
     s->frame_set = true; s->last_frame = frame; s->last_start = start; s->last_end = end;
     // camera selection (scene.rs:153-166)
     int cam;
@@ -1955,15 +2010,18 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
 
     // instance transforms + bounds, then BVH<Instance>::rebuild(shutter_open, shutter_close) (scene.rs:175, bvh.rs:61-78)
     const size_t n = s->instances.size();
-    std::vector<trb::DInstance> di;
-    std::vector<uint32_t> anim_list;
-    if (static_instance_records(s, di, anim_list)) any_anim = true;
+    const bool device_path = s->tune.frame_device && !s->tune.quads;
+    const std::vector<uint32_t>& anim_list = s->anim_list;
+    std::vector<trb::DInstance> di; // the static records, where this frame uploads them: a frame on the device writes the matrices alone
+    if (!device_path || !s->instances_static_uploaded) { std::vector<uint32_t> unused; static_instance_records(s, di, unused); }
+    if (s->inst_any_anim) any_anim = true;
     s->ds.has_anim = any_anim ? 1u : 0u;
     if (n + 1 > s->tlas_capacity) { // a tree over n instances has < n interior records and < 2n nodes
         for (const void* p : {(const void*)s->d_tlas_quads, (const void*)s->d_tlas, (const void*)s->d_tlas_order, (const void*)s->d_tlas_nodes,
-                              (const void*)s->d_bounds, (const void*)s->d_build_f, (const void*)s->d_build_u, (const void*)s->d_build_counts})
+                              (const void*)s->d_bounds, (const void*)s->d_build_f, (const void*)s->d_build_u, (const void*)s->d_build_counts,
+                              (const void*)s->d_build_level})
             s->arena.release(p); // grown after trb_scene_replace_objects added instances (the device was drained above)
-        s->tlas_capacity = 0; s->frame_ready = false;
+        s->tlas_capacity = 0; s->frame_ready = false; s->d_build_level = nullptr;
         CU(s->arena.alloc(n + 1, &s->d_tlas_quads));
         CU(s->arena.alloc(n + 1, &s->d_tlas));
         CU(s->arena.alloc(n, &s->d_tlas_order));
@@ -1979,8 +2037,32 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
     s->ds.anim_instances = s->d_anim_instances; s->ds.n_anim_instances = (uint32_t)anim_list.size();
     s->ds.tlas = s->d_tlas_hdr; s->ds.tlas_pairs = s->d_tlas; s->ds.tlas_quads = s->d_tlas_quads; s->ds.tlas_order = s->d_tlas_order;
 
-    if (s->tune.frame_device && !s->tune.quads) {
-        // ---- device path: transforms, animation bounds, SAH build and record packing all on the GPU (k_frame_instances, k_tlas_build)
+    if (device_path) {
+        // ---- device path: transforms, animation bounds, SAH build and record packing all on the GPU (k_frame_instances, then
+        // k_tlas_build or, from tlas_min instances, the level builder)
+        const long long tlas_min = s->tune.tlas_min < 0 ? (long long)kTlasLevelMin : s->tune.tlas_min;
+        const bool level = n > 0 && (long long)n >= tlas_min;
+        FrameEvents ev;
+        const bool timing = s->tune.frame_time != 0;
+        if (timing) for (cudaEvent_t& x : ev.e) CU(cudaEventCreate(&x));
+        const unsigned long long launches0 = g_launches;
+        trb::bvhb::BuildTrace trace;
+        auto mark = [&](int k) { if (timing) cudaEventRecord(ev.e[k], 0); };
+        auto report = [&](float host_ms) {
+            if (!timing) return;
+            cudaEventSynchronize(ev.e[5]);
+            auto ms = [&](int a, int b) { float t = 0.f; cudaEventElapsedTime(&t, ev.e[a], ev.e[b]); return t; };
+            fprintf(stderr, "trb_scene_update_frame instances %zu builder %s\n", n, level ? "level" : "one-thread");
+            fprintf(stderr, "trb_scene_update_frame host before the first launch %.3f ms\n", host_ms);
+            fprintf(stderr, "trb_scene_update_frame k_frame_instances %.3f ms\n", ms(0, 1));
+            if (level) {
+                fprintf(stderr, "trb_scene_update_frame level loop %.3f ms\n", ms(1, 2));
+                fprintf(stderr, "trb_scene_update_frame serial subtrees %.3f ms\n", ms(2, 3));
+                fprintf(stderr, "trb_scene_update_frame numbering and emit %.3f ms\n", ms(3, 4));
+                fprintf(stderr, "trb_scene_update_frame record packing %.3f ms\n", ms(4, 5));
+            } else fprintf(stderr, "trb_scene_update_frame k_tlas_build %.3f ms\n", ms(1, 5));
+            fprintf(stderr, "trb_scene_update_frame levels %u launches %llu\n", trace.levels, g_launches - launches0);
+        };
         if (!s->instances_static_uploaded) { CU(cudaMemcpy(s->d_instances, di.data(), n * sizeof(trb::DInstance), cudaMemcpyHostToDevice)); s->instances_static_uploaded = true; }
         trb::FrameBuild fb{};
         fb.instances = s->d_instances; fb.bounds = reinterpret_cast<trbh::Box3*>(s->d_bounds); fb.n = (uint32_t)n;
@@ -1988,12 +2070,46 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
         fb.cx = s->d_build_f; fb.cy = s->d_build_f + n; fb.cz = s->d_build_f + 2 * n;
         fb.idx = s->d_build_u; fb.task = s->d_build_u + n; fb.rec_of = s->d_build_u + 4 * n + 4;
         fb.nodes = s->d_tlas_nodes; fb.order = s->d_tlas_order; fb.counts = s->d_build_counts; fb.pairs = s->d_tlas; fb.hdr = s->d_tlas_hdr;
+        // sized like the other frame buffers, by the capacity: a later frame of more instances within it runs in the same memory
+        const uint32_t cap_n = (uint32_t)(s->tlas_capacity - 1), small = (uint32_t)s->tune.tlas_small;
+        if (level && !s->d_build_level) CU(s->arena.alloc(LevelScratch(cap_n, small, nullptr).bytes, &s->d_build_level));
+        const float host_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t_host).count();
+        mark(0);
         trb::k_frame_instances<<<(unsigned)((n + 63) / 64), 64>>>(s->ds, fb);
-        trb::k_tlas_build<<<1, 1>>>(fb);
-        g_launches += 2;
-        CU(cudaGetLastError());
-        uint32_t counts[3] = {0, 0, 0};
-        CU(cudaMemcpy(counts, s->d_build_counts, sizeof counts, cudaMemcpyDeviceToHost)); // also the frame's only synchronisation point
+        ++g_launches;
+        mark(1);
+        uint32_t counts[4] = {0, 0, 0, 0};
+        static const char* const not_buildable = "the instance tree cannot be built: an instance's bounds are infinite, NaN or beyond 2^126";
+        if (!level) {
+            trb::k_tlas_build<<<1, 1>>>(fb);
+            ++g_launches;
+            CU(cudaGetLastError());
+        } else {
+            const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
+            const LevelScratch ls(cap_n, small, s->d_build_level);
+            const uint32_t n32 = (uint32_t)n;
+            bool empty = false;
+            uint32_t n_nodes = 0;
+            trace.after_levels = ev.e[2]; trace.after_small = ev.e[3];
+            // bounds the build would not end on are refused inside it, before any serial subtree runs (trb_host.h bvh_bound_buildable)
+            CU(trb::bvhb::build_device(s->d_bounds, n32, 4u /* scene.rs:141 */, s->d_build_counts, s->d_tlas_nodes, s->d_tlas_order, 0, &g_launches, &empty,
+                                       small, &ls.own, &n_nodes, &trace, true));
+            if (empty) { s->frame_ready = false; return fail(TRB_INVALID_ARG, not_buildable); }
+            mark(4);
+            // the child-pair records and the header, as k_tlas_build's tail writes them
+            CU(cudaMemsetAsync(ls.narrow_bad, 0, 4, 0));
+            trb::bvhb::k_pair_flags<<<grid((size_t)n_nodes + 1), 256>>>(s->d_tlas_nodes, n_nodes, ls.rec);
+            size_t cub_bytes = ls.cub_bytes;
+            CU(cub::DeviceScan::ExclusiveSum(ls.cub, cub_bytes, ls.rec, ls.rec, (int)n_nodes + 1, 0));
+            trb::bvhb::k_pair_pack<<<grid(n_nodes), 256>>>(s->d_tlas_nodes, n_nodes, ls.rec, false, s->d_tlas, ls.narrow_bad);
+            trb::bvhb::k_tlas_header<<<1, 1>>>(s->d_tlas_nodes, ls.rec, n_nodes, n32, ls.narrow_bad, s->d_tlas, s->d_tlas_hdr, s->d_build_counts);
+            g_launches += 3;
+            CU(cudaGetLastError());
+        }
+        mark(5);
+        CU(cudaMemcpy(counts, s->d_build_counts, sizeof counts, cudaMemcpyDeviceToHost)); // also the frame's last synchronisation point
+        report(host_ms);
+        if (counts[3]) { s->frame_ready = false; return fail(TRB_INVALID_ARG, not_buildable); }
         if (!counts[2]) return fail(TRB_UNSUPPORTED, "too many instances for the leaf encoding");
         s->tlas_n_nodes = counts[0];
         s->host_frame_stale = true; // world transforms / TLAS nodes are fetched from the device when a getter asks for them

@@ -23,6 +23,17 @@
 // Centroid bounds are reduced as plain values: their zero signs never reach a result (c - cmin and cmax - cmin give the
 // same bucket for either sign, and the axis and coincidence tests compare magnitudes).
 //
+// The frame's instance tree (trb_scene_update_frame) is also built by one device thread running trbh::bvh_build_arrays
+// (k_tlas_build), whose fminf / fmaxf are min.f32 / max.f32: a NaN operand is skipped and -0.0 orders below +0.0. The two rules
+// differ only where a fold meets both zeros, and an instance bound is never -0: arvo_bounds starts each bound from the composed
+// translation and adds products to it, a sum is -0 only when both operands are, and the translation entry of keyframe_xf and of
+// every xf_compose of such transforms contains the term 1 * (+0) or ends in a term that is itself never -0 (DESIGN.md §4
+// "`update_frame` on the device" has the induction). So this builder reproduces that kernel's bytes with the one rule above, which
+// tests/test_tlas_build_gpu.py checks builder against builder, together with the absence of -0 bounds.
+//
+// The serial-subtree threshold (`small`, at least 4: the level kernels have no n == 1 and n < 5 cases) is an argument of the
+// build: both phases run the same algorithm, so the tree does not depend on it. Meshes pass SMALL.
+//
 // Partition as a closed form (partition.rs:9-38). Let pred(x) = bucket(x) <= best, P the number of elements of [b, e) with
 // pred true, L the positions of [b, b+P) with pred false in ascending order and R the positions of [b+P, e) with pred
 // true in descending order; |L| = |R| because both equal P minus the trues in [b, b+P). The two-ended loop swaps L[k]
@@ -42,7 +53,7 @@
 namespace trb {
 namespace bvhb {
 
-constexpr uint32_t SMALL = 1024;   // a node of at most SMALL elements is one thread's serial subtree
+constexpr uint32_t SMALL = 1024;   // meshes: a node of at most SMALL elements is one thread's serial subtree
 constexpr uint32_t NONE = 0xffffffffu;
 enum : uint32_t { K_SAH = 0, K_LEAF = 1, K_KEEP = 2, K_PART = 3 }; // open node: undecided SAH, leaf, split in place, partition
 enum : uint32_t { T_LEAF = 0, T_INTERIOR = 1, T_SMALL = 2 };        // top-tree node kinds
@@ -92,7 +103,7 @@ __device__ __forceinline__ float dec_hi(unsigned long long key, const float* box
 }
 
 struct Bin { unsigned long long lo[3], hi[3]; uint32_t cnt, pad; };
-struct Open {                                  // a node of more than SMALL elements, open at this level
+struct Open {                                  // a node of more than `small` elements, open at this level
     uint32_t begin, end, tn, kind;             // range of idx[], top-tree node, decision
     uint32_t axis, best, mid, pad;             // mid: first slot of the second child
     float cmin, cmax;
@@ -121,10 +132,10 @@ __global__ void k_bvh_init(const float* __restrict__ boxes, uint32_t n, float* _
     idx[i] = i;
 }
 
-__global__ void k_bvh_root(uint32_t n, TNode* tn, Open* op, uint32_t* small_list, Counters* cnt) {
+__global__ void k_bvh_root(uint32_t n, uint32_t small, TNode* tn, Open* op, uint32_t* small_list, Counters* cnt) {
     TNode& t = tn[0];
     t.begin = 0; t.end = n; t.pre = 0;
-    if (n > SMALL) { t.kind = T_INTERIOR; open_init(op[0], 0, n, 0); *cnt = Counters{1, 1, 0, 0}; }
+    if (n > small) { t.kind = T_INTERIOR; open_init(op[0], 0, n, 0); *cnt = Counters{1, 1, 0, 0}; }
     else { t.kind = T_SMALL; small_list[0] = 0; *cnt = Counters{1, 0, 1, 0}; }
 }
 
@@ -266,7 +277,7 @@ __global__ void k_bvh_swap(uint32_t n, const uint32_t* __restrict__ seg, const O
 }
 
 // leaves take their bounds; interior nodes get two children, each opened at the next level or left to a serial subtree
-__global__ void k_bvh_children(const Open* __restrict__ op, uint32_t n_open, TNode* tn, Open* next, uint32_t* small_list, Counters* cnt,
+__global__ void k_bvh_children(const Open* __restrict__ op, uint32_t n_open, uint32_t small, TNode* tn, Open* next, uint32_t* small_list, Counters* cnt,
                                const uint32_t* __restrict__ idx, const float* __restrict__ boxes) {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n_open) return;
@@ -285,7 +296,7 @@ __global__ void k_bvh_children(const Open* __restrict__ op, uint32_t n_open, TNo
     for (int i = 0; i < 2; ++i) {
         TNode& ch = tn[l + i];
         ch.begin = b[i]; ch.end = b[i + 1];
-        if (b[i + 1] - b[i] > SMALL) { ch.kind = T_INTERIOR; open_init(next[atomicAdd(&cnt->n_next, 1u)], b[i], b[i + 1], l + i); }
+        if (b[i + 1] - b[i] > small) { ch.kind = T_INTERIOR; open_init(next[atomicAdd(&cnt->n_next, 1u)], b[i], b[i + 1], l + i); }
         else { ch.kind = T_SMALL; small_list[atomicAdd(&cnt->n_small, 1u)] = l + i; }
     }
 }
@@ -513,16 +524,32 @@ __global__ void k_pair_pack(const trb_bvh_node* __restrict__ nodes, uint32_t n, 
     out[rec[i]] = p;
 }
 
+// ---- instance-tree helpers of trb_scene_update_frame (the level builder's counterpart of k_tlas_build's head and tail)
+// *bad = 1 where some bound fails trbh::bvh_bound_buildable
+__global__ void k_bounds_check(const float* __restrict__ bounds, size_t n_floats, uint32_t* bad) {
+    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    if (i < n_floats && !trbh::bvh_bound_buildable(bounds[i])) *bad = 1u;
+}
+// the traversal header and the frame's counts {n_nodes, n_order, pack ok, 0: the build accepted the bounds}, after k_pair_pack in the narrow form
+__global__ void k_tlas_header(const trb_bvh_node* __restrict__ nodes, const uint32_t* __restrict__ rec, uint32_t n_nodes, uint32_t n_order,
+                              const uint32_t* __restrict__ narrow_bad, DPair* pairs, DBvh* hdr, uint32_t* counts) {
+    const trb_bvh_node root = nodes[0];
+    hdr->pairs = pairs;
+    hdr->root_lo = make_float4(root.bmin[0], root.bmin[1], root.bmin[2], __uint_as_float(pair_ref(root, rec[0], false)));
+    hdr->root_hi = make_float4(root.bmax[0], root.bmax[1], root.bmax[2], 0.f);
+    counts[0] = n_nodes; counts[1] = n_order; counts[2] = *narrow_bad ? 0u : 1u; counts[3] = 0u;
+}
+
 // ---- host driver
 inline size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
 struct Scratch {
     float* cen; uint32_t* seg; unsigned long long* f; uint32_t* tmp; uint32_t* small_list; trb_bvh_node* snodes;
     Open* open[2]; Counters* cnt; void* cub; size_t cub_bytes; size_t bytes;
 };
-inline uint32_t open_cap(uint32_t n) { return n / (SMALL + 1) + 1; } // open nodes are disjoint and hold more than SMALL elements each
+inline uint32_t open_cap(uint32_t n, uint32_t small = SMALL) { return n / (small + 1) + 1; } // open nodes are disjoint and hold more than `small` elements each
 // Carves the scratch of an n-box build from `base` (base = nullptr: only sizes it). f and tmp are adjacent: after the level
 // loop their 12n + 8 bytes hold the serial subtrees' task stacks (3n words).
-inline Scratch scratch_layout(uint32_t n, char* base) {
+inline Scratch scratch_layout(uint32_t n, char* base, uint32_t small = SMALL) {
     Scratch s{};
     size_t off = 0;
     auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += align_up(bytes); return p; };
@@ -533,8 +560,8 @@ inline Scratch scratch_layout(uint32_t n, char* base) {
     s.tmp = (uint32_t*)take((size_t)n * 4);
     s.small_list = (uint32_t*)take((size_t)n * 4);
     s.snodes = (trb_bvh_node*)take(2 * (size_t)n * sizeof(trb_bvh_node));
-    s.open[0] = (Open*)take(open_cap(n) * sizeof(Open));
-    s.open[1] = (Open*)take(open_cap(n) * sizeof(Open));
+    s.open[0] = (Open*)take(open_cap(n, small) * sizeof(Open));
+    s.open[1] = (Open*)take(open_cap(n, small) * sizeof(Open));
     s.cnt = (Counters*)take(sizeof(Counters));
     cub::DeviceScan::ExclusiveSum(nullptr, s.cub_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)n + 1);
     s.cub = take(s.cub_bytes);
@@ -542,36 +569,57 @@ inline Scratch scratch_layout(uint32_t n, char* base) {
     return s;
 }
 // device bytes an n-box build allocates, besides its nodes and order outputs (the top tree is small and grows on demand)
-inline size_t build_scratch_bytes(uint32_t n) { return scratch_layout(n, nullptr).bytes + (size_t)(4 * open_cap(n) + 64) * sizeof(TNode); }
+inline size_t build_scratch_bytes(uint32_t n, uint32_t small = SMALL) {
+    return scratch_layout(n, nullptr, small).bytes + (size_t)(4 * open_cap(n, small) + 64) * sizeof(TNode);
+}
+// A build that must not allocate runs in memory its caller keeps: `base` of scratch_layout(n, nullptr, small).bytes and a top tree of
+// top_cap(n) nodes, which no build outgrows (the top tree is a binary tree whose leaves hold disjoint, non-empty ranges of the n boxes).
+inline size_t top_cap(uint32_t n) { return 2 * (size_t)n; }
+struct OwnedScratch { char* base; TNode* tn; };
+// What a caller timing the build's phases gets back: events recorded after the level loop and after the serial subtrees (recorded
+// only when non-null), and the number of levels.
+struct BuildTrace { cudaEvent_t after_levels = nullptr, after_small = nullptr; uint32_t levels = 0; };
 
 #define BVHB_TRY(call) do { const cudaError_t e_ = (call); if (e_ != cudaSuccess) { err = e_; goto done; } } while (0)
 
-// Builds the BVH of the n boxes at d_boxes (6 floats each) on `st`: nodes to d_nodes (room for 2n - 1), their count to the
-// device word d_n_nodes, ordered_geom to d_order. Synchronises `st` once per level of nodes larger than SMALL and once at the
-// end. *empty is set where the reference's build would split a node into a child of no elements (a node of more than
-// max_geom boxes whose centroids all fall in one bucket, which infinite coordinates cause): the reference and the host
-// builder never finish such a build, so the output is then not a tree and the caller reports an error.
+// Builds the BVH of the n boxes at d_boxes (6 floats each) on `st`: nodes to d_nodes (room for 2n - 1),
+// their count to the device word d_n_nodes (and to *h_n_nodes when given), ordered_geom to d_order. Nodes of more than `small` (>= 4)
+// boxes are split level by level, the rest by one thread each. Synchronises `st` once per level and once at the end. Scratch is
+// `own` when given, else allocated on `st` for this call and freed. *empty is set where the reference's build would split a node into
+// a child of no elements (a node of more than max_geom boxes whose centroids all fall in one bucket, which infinite coordinates cause):
+// the reference and the host builder never finish such a build, so the output is then not a tree and the caller reports an error.
+// With `refuse`, *empty is also set, and no serial subtree is started, where more than max_geom boxes hold a bound that fails
+// trbh::bvh_bound_buildable: the serial subtrees, like bvh_build_arrays, never end on a split that keeps every element on one side.
 inline cudaError_t build_device(const float* d_boxes, uint32_t n, uint32_t max_geom, uint32_t* d_n_nodes, trb_bvh_node* d_nodes,
-                                uint32_t* d_order, cudaStream_t st, unsigned long long* launches, bool* empty) {
+                                uint32_t* d_order, cudaStream_t st, unsigned long long* launches, bool* empty, uint32_t small = SMALL,
+                                const OwnedScratch* own = nullptr, uint32_t* h_n_nodes = nullptr, BuildTrace* trace = nullptr, bool refuse = false) {
     cudaError_t err = cudaSuccess;
-    char* base = nullptr;
-    TNode* tn = nullptr;
-    Scratch s = scratch_layout(n, nullptr);
-    uint32_t cap = 4 * open_cap(n) + 64, n_tree = 1, n_open, n_small;
+    char* base = own ? own->base : nullptr;
+    TNode* tn = own ? own->tn : nullptr;
+    Scratch s = scratch_layout(n, nullptr, small);
+    size_t cap = own ? top_cap(n) : 4 * (size_t)open_cap(n, small) + 64;
+    uint32_t n_tree = 1, n_open, n_small, h_nodes = 0;
     std::vector<uint32_t> lvl{0u, 1u}; // the top tree's levels: level L is nodes [lvl[L], lvl[L + 1])
     Counters hc{};
     auto grid = [](size_t k, unsigned b) { return (unsigned)((k + b - 1) / b); };
-    BVHB_TRY(cudaMallocAsync((void**)&base, s.bytes, st));
-    BVHB_TRY(cudaMallocAsync((void**)&tn, cap * sizeof(TNode), st));
-    s = scratch_layout(n, base);
+    if (!own) {
+        BVHB_TRY(cudaMallocAsync((void**)&base, s.bytes, st));
+        BVHB_TRY(cudaMallocAsync((void**)&tn, cap * sizeof(TNode), st));
+    }
+    s = scratch_layout(n, base, small);
     k_bvh_init<<<grid(n, 256), 256, 0, st>>>(d_boxes, n, s.cen, d_order);
-    k_bvh_root<<<1, 1, 0, st>>>(n, tn, s.open[0], s.small_list, s.cnt);
+    k_bvh_root<<<1, 1, 0, st>>>(n, small, tn, s.open[0], s.small_list, s.cnt);
     *launches += 2;
-    n_open = n > SMALL ? 1 : 0;
+    if (refuse && n > max_geom) { // the flag is read with the first level's counters, or before the serial subtrees when there is no level
+        k_bounds_check<<<grid(6 * (size_t)n, 256), 256, 0, st>>>(d_boxes, 6 * (size_t)n, &s.cnt->empty);
+        ++*launches;
+    }
+    n_open = n > small ? 1 : 0;
     *empty = false;
     for (int cur = 0; n_open && !hc.empty; cur ^= 1) {
-        if (n_tree + 2 * n_open > cap) { // room for this level's children
-            const uint32_t ncap = std::max(2 * cap, n_tree + 2 * n_open);
+        if (n_tree + 2 * (size_t)n_open > cap) { // room for this level's children
+            if (own) { err = cudaErrorInvalidValue; goto done; } // top_cap(n) nodes hold every top tree
+            const size_t ncap = std::max(2 * cap, n_tree + 2 * (size_t)n_open);
             TNode* t2 = nullptr;
             BVHB_TRY(cudaMallocAsync((void**)&t2, ncap * sizeof(TNode), st));
             BVHB_TRY(cudaMemcpyAsync(t2, tn, n_tree * sizeof(TNode), cudaMemcpyDeviceToDevice, st));
@@ -590,19 +638,22 @@ inline cudaError_t build_device(const float* d_boxes, uint32_t n, uint32_t max_g
         k_bvh_ranks<<<grid(n, 256), 256, 0, st>>>(n, s.seg, op, s.f, s.tmp);
         k_bvh_swap<<<grid(n, 256), 256, 0, st>>>(n, s.seg, op, s.f, s.tmp, d_order);
         BVHB_TRY(cudaMemsetAsync(&s.cnt->n_next, 0, 4, st));
-        k_bvh_children<<<grid(n_open, 128), 128, 0, st>>>(op, n_open, tn, s.open[cur ^ 1], s.small_list, s.cnt, d_order, d_boxes);
+        k_bvh_children<<<grid(n_open, 128), 128, 0, st>>>(op, n_open, small, tn, s.open[cur ^ 1], s.small_list, s.cnt, d_order, d_boxes);
         *launches += 10;
         BVHB_TRY(cudaGetLastError());
         BVHB_TRY(cudaMemcpyAsync(&hc, s.cnt, sizeof hc, cudaMemcpyDeviceToHost, st));
         BVHB_TRY(cudaStreamSynchronize(st));
         n_tree = hc.n_tree; n_open = hc.n_next;
         lvl.push_back(n_tree);
+        if (trace) trace->levels++;
     }
     BVHB_TRY(cudaMemcpyAsync(&hc, s.cnt, sizeof hc, cudaMemcpyDeviceToHost, st));
     BVHB_TRY(cudaStreamSynchronize(st));
     if (hc.empty) { *empty = true; goto done; } // nodes are left open: there is no tree to number
+    if (trace && trace->after_levels) BVHB_TRY(cudaEventRecord(trace->after_levels, st));
     n_small = hc.n_small;
     if (n_small) k_bvh_small<<<grid(n_small, 64), 64, 0, st>>>(s.small_list, n_small, tn, s.cnt, max_geom, d_boxes, s.cen, n, d_order, (uint32_t*)s.f, s.snodes);
+    if (trace && trace->after_small) BVHB_TRY(cudaEventRecord(trace->after_small, st));
     while (lvl.size() > 1 && lvl[lvl.size() - 2] == lvl.back()) lvl.pop_back(); // a last level that opened no node
     for (size_t L = lvl.size() - 1; L-- > 0;) k_bvh_size<<<grid(lvl[L + 1] - lvl[L], 128), 128, 0, st>>>(tn, lvl[L], lvl[L + 1]);
     for (size_t L = 0; L + 1 < lvl.size(); ++L) k_bvh_pre<<<grid(lvl[L + 1] - lvl[L], 128), 128, 0, st>>>(tn, lvl[L], lvl[L + 1]);
@@ -612,12 +663,16 @@ inline cudaError_t build_device(const float* d_boxes, uint32_t n, uint32_t max_g
     *launches += 3 + 3 * (lvl.size() - 1);
     BVHB_TRY(cudaGetLastError());
     BVHB_TRY(cudaMemcpyAsync(d_n_nodes, &tn[0].size, 4, cudaMemcpyDeviceToDevice, st));
+    if (h_n_nodes) BVHB_TRY(cudaMemcpyAsync(&h_nodes, &tn[0].size, 4, cudaMemcpyDeviceToHost, st));
     BVHB_TRY(cudaMemcpyAsync(&hc, s.cnt, sizeof hc, cudaMemcpyDeviceToHost, st));
     BVHB_TRY(cudaStreamSynchronize(st));
     *empty = hc.empty != 0;
+    if (h_n_nodes) *h_n_nodes = h_nodes;
 done:
-    if (tn) { const cudaError_t e = cudaFreeAsync(tn, st); if (err == cudaSuccess) err = e; }
-    if (base) { const cudaError_t e = cudaFreeAsync(base, st); if (err == cudaSuccess) err = e; }
+    if (!own) {
+        if (tn) { const cudaError_t e = cudaFreeAsync(tn, st); if (err == cudaSuccess) err = e; }
+        if (base) { const cudaError_t e = cudaFreeAsync(base, st); if (err == cudaSuccess) err = e; }
+    }
     return err;
 }
 #undef BVHB_TRY

@@ -261,6 +261,15 @@ TRB_HD inline void bvh_build_arrays(BvhBuildArrays& B) {
     }
 }
 
+// When bvh_build_arrays ends. A split that returns `begin` or `end` never shrinks its range: the first child is then empty (n = 0:
+// no leaf case matches, and it splits into itself again) or the whole range, and either repeats for ever while the task stack grows
+// past its array. It happens exactly where a node of more than max_geom elements has all its centroids in one bucket, which takes a
+// centroid extent that is infinite or NaN: with a finite extent of at least kEps the element at cmin lands in bucket 0 and the one at
+// cmax in bucket 11, and every split candidate (0..10) separates them. Bounds of magnitude at most 2^126 keep every centroid, and
+// the difference of any two, finite. Trees of at most four elements never reach the buckets. The frame's instance tree is
+// therefore built only over bounds that pass this test (or over at most four instances); the reference never finishes otherwise.
+TRB_HD inline bool bvh_bound_buildable(float v) { return fabsf(v) <= 8.507059173023462e37f; } // 2^126; false for NaN
+
 struct BvhBuilder { // host convenience over bvh_build_arrays
     std::vector<trb_bvh_node> nodes;
     std::vector<uint32_t> order; // ordered_geom

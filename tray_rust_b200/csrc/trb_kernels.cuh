@@ -3069,8 +3069,8 @@ __global__ void __launch_bounds__(128) k_emitted(const __grid_constant__ DScene 
 // Scene::update_frame on the device (SURVEY 8f N1; scene.rs:152-176, bvh.rs:61-78): per instance the world transform at the
 // shutter-open time and its bounds over the shutter interval (animation_bounds, animated_transform.rs:57-70: 128 time
 // samples when every stacked level is keyframed, one box otherwise — Q22), then BVH<Instance>::rebuild with the reference's
-// SAH builder (the same bvh_build_arrays the host runs, one thread: a TLAS has tens of instances) and the child-pair
-// records the trace kernel walks. Nothing is uploaded per frame but the camera block inside the kernel parameters.
+// SAH builder (the same bvh_build_arrays the host runs, on one thread for the tens of instances of most scenes; the level builder
+// of trb_bvh_build.cuh writes the same bytes for scenes of many instances) and the child-pair records the trace kernel walks. Nothing is uploaded per frame but the camera block inside the kernel parameters.
 // ------------------------------------------------------------------------------------------
 struct FrameBuild {
     DInstance* instances;          // in/out: static fields set at scene creation; inv / mat written here
@@ -3079,7 +3079,7 @@ struct FrameBuild {
     float shutter_open, shutter_close;
     // TLAS build
     float* cx; float* cy; float* cz; uint32_t* idx; uint32_t* task; uint32_t* rec_of; // scratch
-    trb_bvh_node* nodes; uint32_t* order; uint32_t* counts; // out: reference-order nodes, ordered_geom, {n_nodes, n_order, pack ok}
+    trb_bvh_node* nodes; uint32_t* order; uint32_t* counts; // out: reference-order nodes, ordered_geom, {n_nodes, n_order, pack ok, bounds not buildable}
     DPair* pairs; DBvh* hdr;                                // out: traversal records + header
 };
 __device__ __forceinline__ trbh::Box3 shape_bounds_dev(const DScene& sc, const DInstance& in) {
@@ -3118,6 +3118,10 @@ __global__ void __launch_bounds__(64) k_frame_instances(const __grid_constant__ 
 }
 __global__ void k_tlas_build(const __grid_constant__ FrameBuild fb) {
     if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    bool buildable = true; // trb_host.h bvh_bound_buildable: the build below would not end otherwise
+    if (fb.n > 4u) for (uint32_t i = 0; i < 6u * fb.n; ++i) buildable = buildable && trbh::bvh_bound_buildable(reinterpret_cast<const float*>(fb.bounds)[i]);
+    fb.counts[3] = buildable ? 0u : 1u;
+    if (!buildable) return;
     trbh::BvhBuildArrays B{fb.bounds, fb.n, 4u, fb.cx, fb.cy, fb.cz, fb.idx, fb.task, fb.nodes, fb.order, 0u, 0u}; // max_geom 4 (scene.rs:141)
     trbh::bvh_build_arrays(B);
     // child-pair records (trb_device.h DPair): pure re-layout of the reference-order tree

@@ -413,16 +413,21 @@ def scene_heightfield(grid=4200, width=1920, height=1080, spp=4, seed=0x4E16F1D)
     return b
 
 
-def scene_instances(k, seed, width=64, height=64, spp=4, radius=0.3):
+def scene_instances(k, seed, width=64, height=64, spp=4, radius=0.3, mesh=False):
     """A Cornell box holding k small sphere receivers at seeded positions, each with a one-level static transform: the instance-heavy
-    scene of the scene-edit tests and benchmark (every receiver's keyframe is one entry of the description's keyframes)."""
+    scene of the scene-edit tests and benchmark (every receiver's keyframe is one entry of the description's keyframes). With `mesh`
+    the receivers are k instances of one shared 80-triangle icosphere instead, at the same positions."""
     b = SceneBuilder(width, height, spp, 2, 6)
     mats = cornell_walls(b)
     cornell_light(b, mats["white"])
     mat = b.add_material(F.MAT_MATTE, (0.74, 0.74, 0.73), roughness=1.0)
+    shared = b.add_mesh(*icosphere_mesh(1)) if mesh else 0
     rng = np.random.Generator(np.random.PCG64(seed))
     for t in rng.uniform((-13, 1, -8), (13, 22, 18), size=(k, 3)):
-        b.receiver(F.SHAPE_SPHERE, mat, [trs(t=t, s=radius)], p0=1.0)
+        if mesh:
+            b.receiver(F.SHAPE_MESH, mat, [trs(t=t, s=radius)], mesh=shared)
+        else:
+            b.receiver(F.SHAPE_SPHERE, mat, [trs(t=t, s=radius)], p0=1.0)
     b.add_camera([trs(t=(0, 12, -60))], fov=30.0)
     return b
 
