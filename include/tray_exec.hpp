@@ -71,6 +71,11 @@ class Scene {
     void update_frame(size_t frame, float start, float end) { check(trb_scene_update_frame(s_, (uint32_t)frame, start, end)); } // scene.rs:152
     // the scene's cameras and objects replaced in place; meshes, materials and textures stay built (trb_scene_replace_objects)
     void replace_objects(const trb_scene_objects& objects) { check(trb_scene_replace_objects(s_, &objects)); }
+    // the scene's meshes added, removed, reordered and rebuilt in place, with the object section too when `objects` is given
+    // (trb_scene_replace_meshes)
+    void replace_meshes(const trb_scene_meshes& meshes, const trb_scene_objects* objects = nullptr) {
+        check(trb_scene_replace_meshes(s_, &meshes, objects));
+    }
     RenderTarget make_render_target() const { uint32_t w, h; check(trb_scene_info(s_, &w, &h, nullptr, nullptr, nullptr, nullptr)); return RenderTarget(w, h); }
     uint32_t spp() const { uint32_t v; check(trb_scene_info(s_, nullptr, nullptr, &v, nullptr, nullptr, nullptr)); return v; }
     trb_scene* handle() const { return s_; }

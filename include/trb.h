@@ -413,6 +413,35 @@ typedef struct trb_scene_objects {
  * once the scene has been switched to the new section, while the frame is rebuilt, may leave it without a frame. */
 trb_status trb_scene_replace_objects(trb_scene* scene, const trb_scene_objects* objects);
 
+/* The mesh section of a trb_scene_desc, as trb_scene_replace_meshes takes it: mesh i of the new list is the scene's current mesh
+ * keep[i], which keeps its buffers and trees, or, where keep[i] is TRB_MESH_NEW, the arrays of meshes[i] (read only there). */
+#define TRB_MESH_NEW 0xffffffffu
+typedef struct trb_scene_meshes {
+    uint32_t n_meshes;
+    const trb_mesh* meshes;   /* meshes[i] is read only where keep[i] == TRB_MESH_NEW */
+    const uint32_t* keep;     /* keep[i]: index of the scene's current mesh that becomes mesh i, or TRB_MESH_NEW */
+} trb_scene_meshes;
+
+/* Mesh replacement: replace the scene's meshes with the list `meshes` describes, of any length. A kept mesh (keep[i] an index of the
+ * current list) may move to another index and is neither uploaded nor built again; a new one is uploaded and its BVH<Triangle>
+ * (max_geom 16) built as trb_scene_create builds it; a current mesh that no keep entry names is released. With `objects` the object
+ * section is replaced in the same call, as trb_scene_replace_objects replaces it (what renumbered meshes need); with `objects` NULL
+ * the instances stay and their mesh indices index the new list. After a successful call the scene equals trb_scene_create on the
+ * description with the mesh section (and the object section, if given) replaced and, if a frame has been set, that scene after
+ * trb_scene_update_frame with the last arguments given, on everything the scene edits above list.
+ * Statuses: a null scene or null `meshes`, a null keep with n_meshes > 0, a null meshes array where some keep[i] is TRB_MESH_NEW, a
+ * keep entry past the current list or naming a mesh twice, an instance whose mesh index is past the new list, or a section none of
+ * whose cameras is active at the frame that has been set is TRB_INVALID_ARG. New meshes and `objects` are checked by the code that
+ * checks them in trb_scene_create, with its statuses and messages. Every new buffer is built before the scene is switched over, so a
+ * failed call leaves the scene as it was, with one exception: a CUDA error (a device fault, not a property of the input) reported
+ * once the scene has been switched, while node records are re-packed or the frame is rebuilt. Drains the device before it frees or
+ * overwrites anything kernels read; returns when the replacement is complete. */
+trb_status trb_scene_replace_meshes(trb_scene* scene, const trb_scene_meshes* meshes, const trb_scene_objects* objects);
+/* The same with the four arrays of each new mesh in device memory on the scene's GPU, read on cuda_stream (a cudaStream_t; NULL =
+ * default stream); `meshes`, its two arrays and `objects` stay host memory. The indices are checked on the device. */
+trb_status trb_scene_replace_meshes_device(trb_scene* scene, const trb_scene_meshes* meshes, const trb_scene_objects* objects,
+                                           void* cuda_stream);
+
 /* -- the hot path ------------------------------------------------------------------ */
 
 /* ≙ Exec::render (exec/mod.rs:48; multithreaded.rs:55-70). Renders the selected

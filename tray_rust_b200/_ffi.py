@@ -108,6 +108,14 @@ class SceneObjects(C.Structure):
                 ("n_fov_floats", u32), ("fov_floats", C.POINTER(f32))]
 
 
+MESH_NEW = 0xFFFFFFFF
+
+
+class SceneMeshes(C.Structure):
+    """trb_scene_meshes: mesh i of the new list is the scene's current mesh keep[i], or meshes[i] where keep[i] is MESH_NEW"""
+    _fields_ = [("n_meshes", u32), ("meshes", C.POINTER(Mesh)), ("keep", C.POINTER(u32))]
+
+
 class RenderCfg(C.Structure):
     _fields_ = [("spp", u32), ("sample_first", u32), ("sample_count", u32), ("block_start", u32),
                 ("block_count", u32), ("current_frame", u32), ("seed", u32), ("flags", u32),
@@ -230,7 +238,7 @@ TRB_SYMBOLS = [
     "trb_build_bvh", "trb_build_bvh_device",
     "trb_scene_update_mesh", "trb_scene_update_mesh_device",
     "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
-    "trb_scene_replace_objects",
+    "trb_scene_replace_objects", "trb_scene_replace_meshes", "trb_scene_replace_meshes_device",
 ]
 
 _trb = None
@@ -266,6 +274,8 @@ def load_trb():
     lib.trb_scene_update_color_keys.argtypes = [vp, u32, u32, vp]
     lib.trb_scene_update_materials.argtypes = [vp, u32, u32, vp]
     lib.trb_scene_replace_objects.argtypes = [vp, C.POINTER(SceneObjects)]
+    lib.trb_scene_replace_meshes.argtypes = [vp, C.POINTER(SceneMeshes), C.POINTER(SceneObjects)]
+    lib.trb_scene_replace_meshes_device.argtypes = [vp, C.POINTER(SceneMeshes), C.POINTER(SceneObjects), vp]
     lib.trb_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]

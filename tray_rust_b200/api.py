@@ -245,10 +245,36 @@ class Scene(_Base):
         section `objects` (F.SceneObjects, e.g. SceneBuilder.objects()); meshes, materials, textures, film and integrator stay. Counts
         may change: this adds and removes objects, lights and cameras. A frame already set is rebuilt."""
         self._check(self._lib.trb_scene_replace_objects(self._h, C.byref(objects)))
+        self._replaced(objects)
+
+    def replace_meshes(self, section, objects=None):
+        """trb_scene_replace_meshes: replace the mesh list with `section` (F.SceneMeshes, e.g. SceneBuilder.meshes()): kept meshes
+        (keep[i], an index of the current list) stay built, MESH_NEW entries are uploaded and built, unnamed meshes are released. With
+        `objects` (F.SceneObjects) the object section is replaced too; without, the instances' mesh indices index the new list. A
+        frame already set is rebuilt."""
+        self._check(self._lib.trb_scene_replace_meshes(self._h, C.byref(section), None if objects is None else C.byref(objects)))
+        self._replaced(objects, section)
+
+    def replace_meshes_device(self, section, objects=None, stream=None):
+        """trb_scene_replace_meshes_device: the same with the new meshes' four arrays as device pointers on the scene's GPU, read on
+        `stream` (a cudaStream_t as an int; None = default stream)."""
+        self._check(self._lib.trb_scene_replace_meshes_device(self._h, C.byref(section), None if objects is None else C.byref(objects), stream))
+        self._replaced(objects, section)
+
+    def _replaced(self, objects=None, section=None):
+        """the description after a replacement: the object section and / or the mesh list (kept meshes keep their entries)"""
         desc = F.SceneDesc.from_buffer_copy(self._desc)  # a copy: the caller's description (it may belong to the loader) stays as it is
-        for name, _ in F.SceneObjects._fields_:
+        for name, _ in F.SceneObjects._fields_ if objects is not None else ():
             setattr(desc, name, getattr(objects, name))
-        desc._keep = (self._desc, objects)  # the arrays both point into
+        meshes = None
+        if section is not None:
+            n = section.n_meshes
+            meshes = (F.Mesh * max(1, n))()
+            for i in range(n):
+                k = section.keep[i]
+                meshes[i] = section.meshes[i] if k == F.MESH_NEW else self._desc.meshes[k]
+            desc.meshes, desc.n_meshes = meshes, n
+        desc._keep = (self._desc, objects, section, meshes)  # the arrays they point into
         self._desc = desc
         ni, nl = F.u32(), F.u32()
         self._check(self._lib.trb_scene_info(self._h, None, None, None, None, C.byref(ni), C.byref(nl)))

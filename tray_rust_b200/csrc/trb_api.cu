@@ -405,6 +405,19 @@ trb_scene_objects desc_objects(const trb_scene_desc& d) {
             d.n_knots, d.knots, d.n_color_keys, d.color_keys, d.n_fov_floats, d.fov_floats};
 }
 
+// One mesh of a description (trb_scene_create, trb_scene_replace_meshes). Device arrays (`device`) are not read here: their indices
+// are checked on the device once copied (setup_mesh), with the same message.
+trb_status validate_mesh(const trb_mesh& m, bool device) {
+    if (m.n_tris == 0 || m.n_verts == 0) return fail(TRB_INVALID_ARG, "empty mesh");
+    // the wide leaf references hold a 30-bit slot; the kernels index vertex attributes as 3 * index in 32 bits
+    if (m.n_tris > (1u << 30)) return fail(TRB_UNSUPPORTED, "mesh too large for the wide leaf encoding (2^30 triangles)");
+    if (m.n_verts > 0xffffffffu / 3) return fail(TRB_UNSUPPORTED, "mesh has too many vertices (more than (2^32 - 1) / 3)");
+    if (!m.positions || !m.normals || !m.texcoords || !m.indices) return fail(TRB_INVALID_ARG, "Normals and texture coordinates are required!"); // mesh.rs:57-61
+    if (!device)
+        for (size_t k = 0; k < 3 * (size_t)m.n_tris; ++k) if (m.indices[k] >= m.n_verts) return fail(TRB_INVALID_ARG, "mesh index out of range");
+    return TRB_OK;
+}
+
 trb_status validate(const trb_scene_desc* d) {
     if (!d) return fail(TRB_INVALID_ARG, "null scene description");
     if (d->abi_version != TRB_ABI_VERSION) return fail(TRB_INVALID_ARG, "trb_scene_desc.abi_version mismatch");
@@ -430,13 +443,8 @@ trb_status validate(const trb_scene_desc* d) {
     }
     if (texels >= (1ull << 32)) return fail(TRB_UNSUPPORTED, "more than 2^32 texels of image textures");
     for (uint32_t i = 0; i < d->n_meshes; ++i) {
-        const trb_mesh& m = d->meshes[i];
-        if (m.n_tris == 0 || m.n_verts == 0) return fail(TRB_INVALID_ARG, "empty mesh");
-        // the wide leaf references hold a 30-bit slot; the kernels index vertex attributes as 3 * index in 32 bits
-        if (m.n_tris > (1u << 30)) return fail(TRB_UNSUPPORTED, "mesh too large for the wide leaf encoding (2^30 triangles)");
-        if (m.n_verts > 0xffffffffu / 3) return fail(TRB_UNSUPPORTED, "mesh has too many vertices (more than (2^32 - 1) / 3)");
-        if (!m.positions || !m.normals || !m.texcoords || !m.indices) return fail(TRB_INVALID_ARG, "Normals and texture coordinates are required!"); // mesh.rs:57-61
-        for (size_t k = 0; k < 3 * (size_t)m.n_tris; ++k) if (m.indices[k] >= m.n_verts) return fail(TRB_INVALID_ARG, "mesh index out of range");
+        const trb_status r = validate_mesh(d->meshes[i], false);
+        if (r != TRB_OK) return r;
     }
     return TRB_OK;
 }
@@ -1262,18 +1270,25 @@ trb_status camera_rays_enqueue(trb_scene* s, const trb_render_cfg* cfg, size_t n
     return TRB_OK;
 }
 
-// Packs every mesh's DPair records in one leaf form, narrow or wide (trb_device.h), into the buffers allocated when the scene was
-// created, and uploads the mesh headers. Kernels still in flight may read the records, so the device is drained first.
+// One mesh's DPair records in one leaf form, narrow or wide (trb_device.h), packed from its host tree into its record buffer, and
+// the root reference into its header (dh.root_lo)
+trb_status pack_mesh_nodes(const HostMesh& hm, trb::DBvh& dh, bool wide) {
+    std::vector<trb::DPair> pn;
+    trb::DBvh hdr{};
+    if (!pack_pairs(hm.nodes, pn, hdr, wide))
+        return fail(TRB_UNSUPPORTED, wide ? "mesh too large for the wide leaf encoding (2^30 triangles)" : "mesh too large for the leaf encoding (2^25 triangles)");
+    if (!pn.empty()) CU(cudaMemcpy(const_cast<trb::DPair*>(dh.pairs), pn.data(), pn.size() * sizeof(trb::DPair), cudaMemcpyHostToDevice));
+    dh.root_lo = hdr.root_lo;
+    return TRB_OK;
+}
+
+// Packs every mesh's DPair records in one leaf form into the buffers allocated when the mesh was set up (setup_mesh), and uploads
+// the mesh headers. Kernels still in flight may read the records, so the device is drained first.
 trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
     CU(cudaDeviceSynchronize());
     for (size_t mi = 0; mi < s->meshes.size(); ++mi) {
-        std::vector<trb::DPair> pn;
-        trb::DBvh hdr{};
-        if (!pack_pairs(s->meshes[mi].nodes, pn, hdr, wide))
-            return fail(TRB_UNSUPPORTED, wide ? "mesh too large for the wide leaf encoding (2^30 triangles)" : "mesh too large for the leaf encoding (2^25 triangles)");
-        trb::DBvh& dh = s->dmeshes[mi].bvh;
-        if (!pn.empty()) CU(cudaMemcpy(const_cast<trb::DPair*>(dh.pairs), pn.data(), pn.size() * sizeof(trb::DPair), cudaMemcpyHostToDevice));
-        dh.root_lo = hdr.root_lo;
+        const trb_status r = pack_mesh_nodes(s->meshes[mi], s->dmeshes[mi].bvh, wide);
+        if (r != TRB_OK) return r;
     }
     if (!s->dmeshes.empty()) CU(cudaMemcpy(s->d_meshes, s->dmeshes.data(), s->dmeshes.size() * sizeof(trb::DMesh), cudaMemcpyHostToDevice));
     s->wide_leaf = wide;
@@ -1386,6 +1401,65 @@ trb_status pack_pairs_device(const trb_bvh_node* d_nodes, uint32_t n, bool wide,
     const trb_status r = run();
     cudaFree(d_rec); cudaFree(d_cub);
     return r;
+}
+
+// One mesh of a description into fresh buffers of `arena` (trb_scene_create, trb_scene_replace_meshes), checked by validate_mesh: the
+// four arrays uploaded or, with `device`, copied from the caller's device arrays on `st` and the indices checked there
+// (k_mesh_index_check, flag read before anything else is built); BVH<Triangle> with max_geom 16 (mesh.rs:44) and the leaf-ordered
+// triangle records (build_mesh_bvh); the bounds; DQuad records (trace.quads) where every leaf fits the narrow reference; and room
+// for one DPair record per interior node (both leaf forms have one), which pack_mesh_nodes fills in the scene's form.
+trb_status setup_mesh(trb_scene* s, DeviceArena& arena, const trb_mesh& m, bool device, cudaStream_t st, HostMesh& hm, trb::DMesh& dm) {
+    hm.n_verts = m.n_verts;
+    float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
+    const size_t nv = m.n_verts, ni = 3 * (size_t)m.n_tris;
+    if (!device) {
+        CU(arena.upload(m.positions, 3 * nv, &dp));
+        CU(arena.upload(m.normals, 3 * nv, &dn));
+        CU(arena.upload(m.texcoords, 2 * nv, &dt));
+        CU(arena.upload(m.indices, ni, &di));
+    } else {
+        CU(arena.alloc(3 * nv, &dp)); CU(arena.alloc(3 * nv, &dn)); CU(arena.alloc(2 * nv, &dt)); CU(arena.alloc(ni, &di));
+        uint32_t* d_bad = nullptr;
+        CU(arena.alloc(1, &d_bad));
+        CU(cudaMemcpyAsync(dp, m.positions, 3 * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(dn, m.normals, 3 * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(dt, m.texcoords, 2 * nv * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(di, m.indices, ni * sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemsetAsync(d_bad, 0, sizeof(uint32_t), st));
+        const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>((ni / 4 + 255) / 256, (size_t)s->sm_count * 8));
+        trb::bvhb::k_mesh_index_check<<<blocks, 256, 0, st>>>(di, ni, m.n_verts, d_bad);
+        ++g_launches;
+        CU(cudaGetLastError());
+        uint32_t bad = 0;
+        CU(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        arena.release(d_bad);
+        if (bad) return fail(TRB_INVALID_ARG, "mesh index out of range");
+    }
+    CU(arena.alloc(m.n_tris, &dtris));
+    { const trb_status r = build_mesh_bvh(s->tune.build_device != 0, dp, di, m.n_tris, hm, dtris); if (r != TRB_OK) return r; }
+    for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
+    size_t n_rec = 0;
+    for (const trb_bvh_node& n : hm.nodes) if (!(n.b & TRB_BVH_LEAF)) ++n_rec;
+    trb::DBvh& hdr = dm.bvh;
+    hdr.quads = nullptr;
+    hdr.root_hi = make_float4(hm.bounds.hi[0], hm.bounds.hi[1], hm.bounds.hi[2], bits_f(QUAD_EMPTY_HOST));
+    hm.narrow = leaves_fit_narrow(hm.nodes);
+    if (hm.narrow) { // DQuad records (trace.quads) hold narrow leaves only: a mesh that needs the wide form skips them
+        std::vector<trb::DQuad> qn;
+        uint32_t qroot = 0;
+        if (!pack_quads(hm.nodes, qn, qroot)) return fail(TRB_UNSUPPORTED, "mesh too large for the leaf encoding (2^25 triangles)");
+        hdr.root_hi.w = bits_f(qroot);
+        trb::DQuad* dquads;
+        CU(arena.upload(qn.data(), qn.size(), &dquads));
+        hdr.quads = dquads;
+    }
+    CU(arena.alloc(n_rec, &dnodes));
+    hm.pair_cap = n_rec;
+    hdr.pairs = dnodes;
+    dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.tris = dtris;
+    dm.n_nodes = (uint32_t)hm.nodes.size(); dm.n_tris = m.n_tris;
+    return TRB_OK;
 }
 
 // trb_scene_update_mesh(_device): `device` says the caller's arrays are device memory, read on `st`. New positions are copied
@@ -1598,91 +1672,200 @@ trb_status update_materials(trb_scene* s, uint32_t first, uint32_t count, const 
 // them), the light list, the instance records without matrices (so that trb_emitted runs before the first update_frame), the
 // animation tables, and what the kernels' choice depends on (n_anim, material_shape, anim_emission). Needs the scene's meshes and
 // materials in place. The new device buffers are complete before DScene is switched over and the ones they replace are released, so
-// a failure leaves the scene as it was. The caller has drained the device.
-trb_status set_objects(trb_scene* s, const trb_scene_objects& o) {
-    std::vector<trb_camera> cameras(o.cameras, o.cameras + o.n_cameras);
-    std::vector<trb_instance> instances(o.instances, o.instances + o.n_instances);
-    std::vector<trb_spline> splines(o.splines, o.splines + o.n_splines);
-    std::vector<trb_keyframe> keyframes(o.keyframes, o.keyframes + o.n_keyframes);
-    std::vector<float> knots(o.knots, o.knots + o.n_knots), fov_floats(o.fov_floats, o.fov_floats + o.n_fov_floats);
-    std::vector<trb_color_key> color_keys(o.color_keys, o.color_keys + o.n_color_keys);
-    for (const trb_spline& sp : splines) // BSpline::new sorts its knots (bspline 0.2.2); ranges were bounds-checked by validate_objects()
-        if (sp.n_ctrl > 1) std::stable_sort(knots.begin() + sp.knot_first, knots.begin() + sp.knot_first + sp.n_knots);
-    for (const trb_camera& c : cameras)
-        if (c.n_fov_ctrl) std::stable_sort(fov_floats.begin() + c.fov_knot_first, fov_floats.begin() + c.fov_knot_first + c.n_fov_knots);
-    // the helpers below read the section from the scene: the current one is kept in the locals until the device buffers exist
+// a failure leaves the scene as it was. set_objects is stage_objects, which builds all of that without touching the scene, then
+// commit_objects, which switches the scene over; the caller has drained the device before the commit.
+struct StagedObjects {
+    std::vector<trb_camera> cameras;
+    std::vector<trb_instance> instances;
+    std::vector<trb_spline> splines;
+    std::vector<trb_keyframe> keyframes;
+    std::vector<float> knots, fov_floats;
+    std::vector<trb_color_key> color_keys;
+    std::vector<uint32_t> anim_list;
+    bool inst_any_anim = false;
+    uint32_t n_lights = 0, n_uniq = 0;
+    DeviceArena fresh; // frees what it holds unless committed
+    uint32_t *d_lights = nullptr, *d_anim = nullptr, *d_uo = nullptr, *d_ul = nullptr;
+    trb::DInstance* d_inst = nullptr;
+    trb_spline* d_sp = nullptr; trb_keyframe* d_kf = nullptr; float* d_kn = nullptr; trb_color_key* d_ck = nullptr; Xf* d_lv = nullptr;
+};
+
+trb_status stage_objects(trb_scene* s, const trb_scene_objects& o, StagedObjects& g) {
+    g.cameras.assign(o.cameras, o.cameras + o.n_cameras);
+    g.instances.assign(o.instances, o.instances + o.n_instances);
+    g.splines.assign(o.splines, o.splines + o.n_splines);
+    g.keyframes.assign(o.keyframes, o.keyframes + o.n_keyframes);
+    g.knots.assign(o.knots, o.knots + o.n_knots); g.fov_floats.assign(o.fov_floats, o.fov_floats + o.n_fov_floats);
+    g.color_keys.assign(o.color_keys, o.color_keys + o.n_color_keys);
+    for (const trb_spline& sp : g.splines) // BSpline::new sorts its knots (bspline 0.2.2); ranges were bounds-checked by validate_objects()
+        if (sp.n_ctrl > 1) std::stable_sort(g.knots.begin() + sp.knot_first, g.knots.begin() + sp.knot_first + sp.n_knots);
+    for (const trb_camera& c : g.cameras)
+        if (c.n_fov_ctrl) std::stable_sort(g.fov_floats.begin() + c.fov_knot_first, g.fov_floats.begin() + c.fov_knot_first + c.n_fov_knots);
+    // the helpers below read the section from the scene: it is swapped in while they run and swapped out again before returning
     auto swap_host = [&] {
-        s->cameras.swap(cameras); s->instances.swap(instances); s->splines.swap(splines); s->keyframes.swap(keyframes);
-        s->knots.swap(knots); s->fov_floats.swap(fov_floats); s->color_keys.swap(color_keys);
+        s->cameras.swap(g.cameras); s->instances.swap(g.instances); s->splines.swap(g.splines); s->keyframes.swap(g.keyframes);
+        s->knots.swap(g.knots); s->fov_floats.swap(g.fov_floats); s->color_keys.swap(g.color_keys);
     };
     swap_host();
     std::vector<uint32_t> lights;
     for (uint32_t i = 0; i < o.n_instances; ++i) if (s->instances[i].kind != TRB_INST_RECEIVER) lights.push_back(i); // multithreaded.rs:33-38
     std::vector<trb::DInstance> di;
-    std::vector<uint32_t> anim_list, uniq_of, uniq_list;
-    const bool inst_any_anim = static_instance_records(s, di, anim_list);
+    std::vector<uint32_t> uniq_of, uniq_list;
+    g.inst_any_anim = static_instance_records(s, di, g.anim_list);
     std::vector<Xf> level(s->splines.size());
     for (size_t k = 0; k < level.size(); ++k) level[k] = level_transform(s, k);
     spline_dedup(s, uniq_of, uniq_list);
     // room for every keyframed spline: a keyframe edit can make splines that were equal distinct (trb_scene_update_keyframes)
     const size_t n_keyed = (size_t)std::count_if(s->splines.begin(), s->splines.end(), [](const trb_spline& sp) { return sp.n_ctrl > 1; });
-
-    DeviceArena fresh; // frees what it holds if an allocation or upload fails
-    uint32_t *d_lights = nullptr, *d_anim = nullptr, *d_uo = nullptr, *d_ul = nullptr;
-    trb::DInstance* d_inst = nullptr;
-    trb_spline* d_sp = nullptr; trb_keyframe* d_kf = nullptr; float* d_kn = nullptr; trb_color_key* d_ck = nullptr; Xf* d_lv = nullptr;
+    g.n_lights = (uint32_t)lights.size(); g.n_uniq = (uint32_t)uniq_list.size();
     const trb_status r = [&]() -> trb_status {
-        CU(fresh.upload(lights.data(), lights.size(), &d_lights));
-        CU(fresh.upload(di.data(), di.size(), &d_inst));
-        CU(fresh.alloc(di.size(), &d_anim)); // update_frame fills it
-        if (!s->splines.empty()) CU(fresh.upload(s->splines.data(), s->splines.size(), &d_sp));
-        if (!s->keyframes.empty()) CU(fresh.upload(s->keyframes.data(), s->keyframes.size(), &d_kf));
-        if (!s->knots.empty()) CU(fresh.upload(s->knots.data(), s->knots.size(), &d_kn));
-        if (!s->color_keys.empty()) CU(fresh.upload(s->color_keys.data(), s->color_keys.size(), &d_ck));
-        if (!level.empty()) CU(fresh.upload(level.data(), level.size(), &d_lv));
-        if (!uniq_of.empty()) CU(fresh.upload(uniq_of.data(), uniq_of.size(), &d_uo));
+        CU(g.fresh.upload(lights.data(), lights.size(), &g.d_lights));
+        CU(g.fresh.upload(di.data(), di.size(), &g.d_inst));
+        CU(g.fresh.alloc(di.size(), &g.d_anim)); // update_frame fills it
+        if (!s->splines.empty()) CU(g.fresh.upload(s->splines.data(), s->splines.size(), &g.d_sp));
+        if (!s->keyframes.empty()) CU(g.fresh.upload(s->keyframes.data(), s->keyframes.size(), &g.d_kf));
+        if (!s->knots.empty()) CU(g.fresh.upload(s->knots.data(), s->knots.size(), &g.d_kn));
+        if (!s->color_keys.empty()) CU(g.fresh.upload(s->color_keys.data(), s->color_keys.size(), &g.d_ck));
+        if (!level.empty()) CU(g.fresh.upload(level.data(), level.size(), &g.d_lv));
+        if (!uniq_of.empty()) CU(g.fresh.upload(uniq_of.data(), uniq_of.size(), &g.d_uo));
         if (n_keyed) {
-            CU(fresh.alloc(n_keyed, &d_ul));
-            CU(cudaMemcpy(d_ul, uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+            CU(g.fresh.alloc(n_keyed, &g.d_ul));
+            CU(cudaMemcpy(g.d_ul, uniq_list.data(), uniq_list.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
         }
         return TRB_OK;
     }();
-    if (r != TRB_OK) { swap_host(); return r; }
+    swap_host();
+    return r;
+}
 
+// Needs the scene's meshes and materials in place (material_shape reads the materials)
+void commit_objects(trb_scene* s, StagedObjects& g) {
+    s->cameras.swap(g.cameras); s->instances.swap(g.instances); s->splines.swap(g.splines); s->keyframes.swap(g.keyframes);
+    s->knots.swap(g.knots); s->fov_floats.swap(g.fov_floats); s->color_keys.swap(g.color_keys);
     trb::DScene& ds = s->ds;
     for (const void* p : {(const void*)ds.lights, (const void*)s->d_instances, (const void*)s->d_anim_instances, (const void*)ds.splines,
                           (const void*)ds.keyframes, (const void*)ds.knots, (const void*)ds.color_keys, (const void*)ds.level_xf,
                           (const void*)ds.spline_uniq, (const void*)ds.uniq_splines}) s->arena.release(p);
-    s->arena.ptrs.insert(s->arena.ptrs.end(), fresh.ptrs.begin(), fresh.ptrs.end());
-    fresh.ptrs.clear();
-    s->d_instances = d_inst; s->d_anim_instances = d_anim;
-    ds.instances = d_inst; ds.n_instances = o.n_instances; ds.lights = d_lights; ds.n_lights = (uint32_t)lights.size();
-    ds.splines = d_sp; ds.keyframes = d_kf; ds.knots = d_kn; ds.color_keys = d_ck; ds.level_xf = d_lv;
-    ds.spline_uniq = d_uo; ds.uniq_splines = d_ul; ds.n_uniq_splines = (uint32_t)uniq_list.size();
+    s->arena.ptrs.insert(s->arena.ptrs.end(), g.fresh.ptrs.begin(), g.fresh.ptrs.end());
+    g.fresh.ptrs.clear();
+    s->d_instances = g.d_inst; s->d_anim_instances = g.d_anim;
+    ds.instances = g.d_inst; ds.n_instances = (uint32_t)s->instances.size(); ds.lights = g.d_lights; ds.n_lights = g.n_lights;
+    ds.splines = g.d_sp; ds.keyframes = g.d_kf; ds.knots = g.d_kn; ds.color_keys = g.d_ck; ds.level_xf = g.d_lv;
+    ds.spline_uniq = g.d_uo; ds.uniq_splines = g.d_ul; ds.n_uniq_splines = g.n_uniq;
     ds.has_anim = 0; ds.anim_instances = nullptr; ds.n_anim_instances = 0; // update_frame sets them
-    s->n_anim = (uint32_t)anim_list.size();
-    s->anim_list.swap(anim_list); s->inst_any_anim = inst_any_anim;
+    s->n_anim = (uint32_t)g.anim_list.size();
+    s->anim_list.swap(g.anim_list); s->inst_any_anim = g.inst_any_anim;
     material_shape(s);
     s->anim_emission = false;
     for (const trb_instance& in : s->instances) if (in.kind != TRB_INST_RECEIVER && in.n_emission > 1) s->anim_emission = true;
+}
+
+trb_status set_objects(trb_scene* s, const trb_scene_objects& o) {
+    StagedObjects g;
+    const trb_status r = stage_objects(s, o, g);
+    if (r != TRB_OK) return r;
+    commit_objects(s, g);
     return TRB_OK;
 }
 
-// Checked as trb_scene_create checks the section, and that the frame that has been set can be set again; then set_objects, the
-// state that was sized or built for the old section, and the frame
-trb_status replace_objects(trb_scene* s, const trb_scene_objects& o) {
-    const trb_status v = validate_objects(o, (uint32_t)s->meshes.size(), (uint32_t)s->materials.size());
-    if (v != TRB_OK) return v;
-    if (s->frame_set && o.cameras[0].active_at > s->last_frame) return fail(TRB_INVALID_ARG, "no camera is active at this frame");
-    CU(cudaSetDevice(s->device));
-    CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
-    const trb_status r = set_objects(s, o);
-    if (r != TRB_OK) return r;
-    // nothing of the old instance list's frame survives; the camera is selected as on a new scene's first frame (scene.rs:153-166)
+// After a new object section was committed: nothing of the old instance list's frame survives, and the camera is selected as on a
+// new scene's first frame (scene.rs:153-166). The caller re-runs the frame that had been set.
+void objects_replaced(trb_scene* s) {
     s->frame_ready = false; s->instances_static_uploaded = false; s->host_frame_stale = false;
     s->world.clear(); s->tlas_nodes.clear(); s->tlas_order.clear(); s->tlas_n_nodes = 0;
     s->active_camera = -1;
     if (s->wf.n_anim != s->n_anim) s->wf_capacity = 0; // WfState::xf_tab is sized by n_anim: ensure_wavefront allocates the state anew
+}
+
+// The checks of a new object section against a scene whose meshes will number n_meshes: trb_scene_create's, and that the frame that
+// has been set can be set again
+trb_status check_objects(const trb_scene* s, const trb_scene_objects& o, uint32_t n_meshes) {
+    const trb_status v = validate_objects(o, n_meshes, (uint32_t)s->materials.size());
+    if (v != TRB_OK) return v;
+    if (s->frame_set && o.cameras[0].active_at > s->last_frame) return fail(TRB_INVALID_ARG, "no camera is active at this frame");
+    return TRB_OK;
+}
+
+// Checked as trb_scene_create checks the section; then set_objects, the state that was sized or built for the old section, and the frame
+trb_status replace_objects(trb_scene* s, const trb_scene_objects& o) {
+    const trb_status v = check_objects(s, o, (uint32_t)s->meshes.size());
+    if (v != TRB_OK) return v;
+    CU(cudaSetDevice(s->device));
+    CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
+    const trb_status r = set_objects(s, o);
+    if (r != TRB_OK) return r;
+    objects_replaced(s);
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    return TRB_OK;
+}
+
+// ---- the mesh section (trb_scene_replace_meshes; DESIGN.md §4 "Mesh replacement") -----------------------------------------------
+// Checks everything first (keep entries, new meshes as creation checks them, the object section or the current instances against the
+// new mesh count); builds every new mesh, the new header array and the staged object section into fresh buffers; and only then drains
+// the device, switches the scene over and releases what was replaced. Kept meshes move with their buffers, trees and records; their
+// records are re-packed only when the scene's leaf form changes with the new list.
+trb_status replace_meshes(trb_scene* s, const trb_scene_meshes& sec, const trb_scene_objects* o, bool device, cudaStream_t st) {
+    const uint32_t n = sec.n_meshes, n_old = (uint32_t)s->meshes.size();
+    if (n && !sec.keep) return fail(TRB_INVALID_ARG, "null keep array with a non-zero mesh count");
+    std::vector<char> named(n_old, 0);
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t k = sec.keep[i];
+        if (k == TRB_MESH_NEW) { if (!sec.meshes) return fail(TRB_INVALID_ARG, "null meshes array with a new mesh"); continue; }
+        if (k >= n_old) return fail(TRB_INVALID_ARG, "kept mesh index out of range");
+        if (named[k]) return fail(TRB_INVALID_ARG, "a mesh is kept twice");
+        named[k] = 1;
+    }
+    if (o) { const trb_status v = check_objects(s, *o, n); if (v != TRB_OK) return v; }
+    else
+        for (const trb_instance& in : s->instances)
+            if (in.shape == TRB_SHAPE_MESH && in.mesh >= n) return fail(TRB_INVALID_ARG, "mesh index out of range");
+    for (uint32_t i = 0; i < n; ++i)
+        if (sec.keep[i] == TRB_MESH_NEW) { const trb_status v = validate_mesh(sec.meshes[i], device); if (v != TRB_OK) return v; }
+    CU(cudaSetDevice(s->device));
+
+    // build: new meshes, the leaf form of the new list, new meshes' node records in it, the header array, the object section
+    DeviceArena fresh; // frees what it holds if anything below fails
+    std::vector<HostMesh> built(n);
+    std::vector<trb::DMesh> dmeshes(n);
+    bool needs_wide = false;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t k = sec.keep[i];
+        if (k != TRB_MESH_NEW) { dmeshes[i] = s->dmeshes[k]; needs_wide |= !s->meshes[k].narrow; continue; }
+        const trb_status r = setup_mesh(s, fresh, sec.meshes[i], device, st, built[i], dmeshes[i]);
+        if (r != TRB_OK) return r;
+        needs_wide |= !built[i].narrow;
+    }
+    const bool wide = needs_wide || s->tune.wide_leaf != 0, repack = wide != s->wide_leaf;
+    if (!repack) // otherwise every mesh is packed below, once the kept ones' records are no longer read
+        for (uint32_t i = 0; i < n; ++i)
+            if (sec.keep[i] == TRB_MESH_NEW) { const trb_status r = pack_mesh_nodes(built[i], dmeshes[i].bvh, wide); if (r != TRB_OK) return r; }
+    trb::DMesh* d_meshes = nullptr;
+    CU(fresh.upload(dmeshes.data(), dmeshes.size(), &d_meshes));
+    StagedObjects g;
+    if (o) { const trb_status r = stage_objects(s, *o, g); if (r != TRB_OK) return r; }
+
+    // switch: passes enqueued by the _device calls may still read the buffers released here
+    CU(cudaDeviceSynchronize());
+    for (uint32_t k = 0; k < n_old; ++k) {
+        if (named[k]) continue;
+        const trb::DMesh& dm = s->dmeshes[k];
+        for (const void* p : {(const void*)dm.positions, (const void*)dm.normals, (const void*)dm.texcoords, (const void*)dm.indices,
+                              (const void*)dm.tris, (const void*)dm.bvh.pairs, (const void*)dm.bvh.quads})
+            if (p) s->arena.release(p);
+    }
+    s->arena.release(s->d_meshes);
+    s->arena.ptrs.insert(s->arena.ptrs.end(), fresh.ptrs.begin(), fresh.ptrs.end());
+    fresh.ptrs.clear();
+    std::vector<HostMesh> meshes(n);
+    for (uint32_t i = 0; i < n; ++i) meshes[i] = std::move(sec.keep[i] == TRB_MESH_NEW ? built[i] : s->meshes[sec.keep[i]]);
+    s->meshes.swap(meshes); s->dmeshes.swap(dmeshes);
+    s->d_meshes = d_meshes; s->ds.meshes = d_meshes;
+    s->needs_wide = needs_wide;
+    s->quads_dropped = false; // a narrow mesh without DQuad records was rebuilt by trb_scene_update_mesh
+    for (uint32_t i = 0; i < n; ++i) if (s->meshes[i].narrow && !s->dmeshes[i].bvh.quads) s->quads_dropped = true;
+    if (o) { commit_objects(s, g); objects_replaced(s); }
+    else { s->instances_static_uploaded = false; s->frame_ready = false; } // the instances' mesh bounds changed
+    if (repack) { const trb_status r = upload_mesh_nodes(s, wide); if (r != TRB_OK) return r; }
     if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
     return TRB_OK;
 }
@@ -1730,6 +1913,17 @@ trb_status trb_scene_replace_objects(trb_scene* s, const trb_scene_objects* obje
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     if (!objects) return fail(TRB_INVALID_ARG, "null objects");
     return replace_objects(s, *objects);
+}
+
+trb_status trb_scene_replace_meshes(trb_scene* s, const trb_scene_meshes* meshes, const trb_scene_objects* objects) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (!meshes) return fail(TRB_INVALID_ARG, "null meshes");
+    return replace_meshes(s, *meshes, objects, false, nullptr);
+}
+trb_status trb_scene_replace_meshes_device(trb_scene* s, const trb_scene_meshes* meshes, const trb_scene_objects* objects, void* cuda_stream) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (!meshes) return fail(TRB_INVALID_ARG, "null meshes");
+    return replace_meshes(s, *meshes, objects, true, static_cast<cudaStream_t>(cuda_stream));
 }
 
 const char* trb_last_error(void) { return g_error.c_str(); }
@@ -1832,37 +2026,9 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     s->dmeshes.resize(d->n_meshes);
     s->meshes.resize(d->n_meshes);
     for (uint32_t mi = 0; mi < d->n_meshes; ++mi) {
-        const trb_mesh& m = d->meshes[mi];
-        HostMesh& hm = s->meshes[mi];
-        hm.n_verts = m.n_verts;
-        float *dp, *dn, *dt; uint32_t* di; trb::DPair* dnodes; trb::DTri* dtris;
-        CU(s->arena.upload(m.positions, 3 * (size_t)m.n_verts, &dp));
-        CU(s->arena.upload(m.normals, 3 * (size_t)m.n_verts, &dn));
-        CU(s->arena.upload(m.texcoords, 2 * (size_t)m.n_verts, &dt));
-        CU(s->arena.upload(m.indices, 3 * (size_t)m.n_tris, &di));
-        CU(s->arena.alloc(m.n_tris, &dtris));
-        { const trb_status r = build_mesh_bvh(s->tune.build_device != 0, dp, di, m.n_tris, hm, dtris); if (r != TRB_OK) return r; }
-        for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
-        size_t n_rec = 0;
-        for (const trb_bvh_node& n : hm.nodes) if (!(n.b & TRB_BVH_LEAF)) ++n_rec;
-        trb::DMesh& dm = s->dmeshes[mi];
-        trb::DBvh& hdr = dm.bvh;
-        hdr.quads = nullptr;
-        hdr.root_hi = make_float4(hm.bounds.hi[0], hm.bounds.hi[1], hm.bounds.hi[2], bits_f(QUAD_EMPTY_HOST));
-        if (leaves_fit_narrow(hm.nodes)) { // DQuad records (trace.quads) hold narrow leaves only: a mesh that needs the wide form skips them
-            std::vector<trb::DQuad> qn;
-            uint32_t qroot = 0;
-            if (!pack_quads(hm.nodes, qn, qroot)) return fail(TRB_UNSUPPORTED, "mesh too large for the leaf encoding (2^25 triangles)");
-            hdr.root_hi.w = bits_f(qroot);
-            trb::DQuad* dquads;
-            CU(s->arena.upload(qn.data(), qn.size(), &dquads));
-            hdr.quads = dquads;
-        } else { s->needs_wide = true; hm.narrow = false; }
-        CU(s->arena.alloc(n_rec, &dnodes)); // filled by upload_mesh_nodes: both leaf forms have one record per interior node
-        hm.pair_cap = n_rec;
-        hdr.pairs = dnodes;
-        dm.positions = dp; dm.normals = dn; dm.texcoords = dt; dm.indices = di; dm.tris = dtris;
-        dm.n_nodes = (uint32_t)hm.nodes.size(); dm.n_tris = m.n_tris;
+        const trb_status r = setup_mesh(s.get(), s->arena, d->meshes[mi], false, nullptr, s->meshes[mi], s->dmeshes[mi]);
+        if (r != TRB_OK) return r;
+        if (!s->meshes[mi].narrow) s->needs_wide = true;
     }
     CU(s->arena.alloc(s->dmeshes.size(), &s->d_meshes));
     { const trb_status r = upload_mesh_nodes(s.get(), s->needs_wide || s->tune.wide_leaf != 0); if (r != TRB_OK) return r; }

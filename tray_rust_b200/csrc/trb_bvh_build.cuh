@@ -490,6 +490,20 @@ __global__ void k_tri_leaf_marks(const trb_bvh_node* __restrict__ nodes, uint32_
     const uint32_t cnt = nd.b & ~TRB_BVH_LEAF;
     if ((nd.b & TRB_BVH_LEAF) && cnt) tris[(size_t)nd.a + cnt - 1].e0.w = __uint_as_float(TRI_LEAF_END);
 }
+// *bad = 1 where some of the n indices is >= n_verts: trb_scene_create's "mesh index out of range" for indices that are already on the
+// device (trb_scene_replace_meshes_device), read once where they are. idx is a cudaMalloc'd buffer, so 16-byte aligned: vector loads
+// over the body, a scalar tail, and one atomic per warp that found an index out of range. Grid-stride; blockDim a multiple of 32.
+__global__ void k_mesh_index_check(const uint32_t* __restrict__ idx, size_t n, uint32_t n_verts, uint32_t* bad) {
+    const size_t n4 = n / 4, stride = (size_t)gridDim.x * blockDim.x, t = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    const uint4* __restrict__ v = reinterpret_cast<const uint4*>(idx);
+    bool out = false;
+    for (size_t i = t; i < n4; i += stride) {
+        const uint4 q = v[i];
+        out |= (q.x >= n_verts) | (q.y >= n_verts) | (q.z >= n_verts) | (q.w >= n_verts);
+    }
+    for (size_t i = 4 * n4 + t; i < n; i += stride) out |= idx[i] >= n_verts;
+    if (__any_sync(0xffffffffu, out) && (threadIdx.x & 31) == 0) atomicOr(bad, 1u);
+}
 
 // ---- mesh helpers of trb_scene_update_mesh: the DPair records (trb_device.h) of a preorder tree still on the device
 // rec[i] = 1 for an interior node, rec[n] = 0; an exclusive scan then gives each interior node its record index and rec[n] the count

@@ -61,6 +61,7 @@ class SceneBuilder:
         self.fov_floats = []
         self.textures, self.images = [], []
         self._keep = []
+        self._given = []  # the mesh list a scene was last given (finish(), meshes_section())
 
     # -- transforms ---------------------------------------------------------------------
     def _add_xf(self, levels):
@@ -102,14 +103,31 @@ class SceneBuilder:
         self.merl.append(t)
         return len(self.merl) - 1
 
-    def add_mesh(self, positions, normals, texcoords, indices):
+    @staticmethod
+    def _mesh(positions, normals, texcoords, indices):
         p = np.ascontiguousarray(positions, dtype=np.float32).reshape(-1, 3)
         n = np.ascontiguousarray(normals, dtype=np.float32).reshape(-1, 3)
         t = np.ascontiguousarray(texcoords, dtype=np.float32).reshape(-1, 2)
         i = np.ascontiguousarray(indices, dtype=np.uint32).reshape(-1, 3)
         assert len(p) == len(n) == len(t)
-        self.meshes.append((p, n, t, i))
+        return p, n, t, i
+
+    def add_mesh(self, positions, normals, texcoords, indices):
+        self.meshes.append(self._mesh(positions, normals, texcoords, indices))
         return len(self.meshes) - 1
+
+    def set_mesh(self, i, positions, normals, texcoords, indices):
+        """Replace mesh i's arrays (any vertex and triangle counts); the next meshes() section builds it anew."""
+        self.meshes[i] = self._mesh(positions, normals, texcoords, indices)
+
+    def remove_mesh(self, i):
+        """Drop mesh i and renumber the mesh instances above it: the builder is then the one that never added it. Refused (ValueError)
+        while an instance still uses mesh i. Returns the removed arrays."""
+        users = [k for k, it in enumerate(self.instances) if it[1] == F.SHAPE_MESH and it[4] == i]
+        if users:
+            raise ValueError("mesh %d is used by instances %s" % (i, users))
+        self.instances = [it[:4] + (it[4] - 1,) + it[5:] if it[1] == F.SHAPE_MESH and it[4] > i else it for it in self.instances]
+        return self.meshes.pop(i)
 
     def add_instance(self, kind, shape, material, xf, p0=0.0, p1=0.0, mesh=0, emission=None):
         sf, ns = self._add_xf(xf)
@@ -217,6 +235,34 @@ class SceneBuilder:
         self._fill_objects(o, o._keep)
         return o
 
+    def _fill_meshes(self, d, keep):
+        """the mesh list's count and trb_mesh array into d (a SceneDesc or a SceneMeshes: same field names); the builder remembers the
+        list as the one a scene was last given, which meshes() compares against"""
+        a = (F.Mesh * max(1, len(self.meshes)))()
+        for o, (p, n, t, i) in zip(a, self.meshes):
+            o.n_verts, o.n_tris = len(p), len(i)
+            o.positions = p.ctypes.data_as(C.POINTER(F.f32)); o.normals = n.ctypes.data_as(C.POINTER(F.f32))
+            o.texcoords = t.ctypes.data_as(C.POINTER(F.f32)); o.indices = i.ctypes.data_as(C.POINTER(F.u32))
+        keep += [a, list(self.meshes)]
+        d.meshes = a; d.n_meshes = len(self.meshes)
+        self._given = list(self.meshes)
+
+    def meshes_section(self):
+        """The builder's mesh list (trb_scene_meshes) for Scene.replace_meshes: mesh i keeps the scene's mesh j when it is the same
+        arrays the scene was last given as mesh j (by finish() or an earlier section; set_mesh makes new ones), otherwise it is new."""
+        given = {id(m): j for j, m in enumerate(self._given)}
+        keep = []
+        for m in self.meshes:
+            j = given.pop(id(m), None)
+            keep.append(F.MESH_NEW if j is None else j)
+        s = F.SceneMeshes()
+        s._keep = []
+        self._fill_meshes(s, s._keep)
+        k = (F.u32 * max(1, len(keep)))(*keep)
+        s._keep.append(k)
+        s.keep = k
+        return s
+
     def finish(self):
         d = F.SceneDesc()
         d.abi_version = F.TRB_ABI_VERSION
@@ -231,14 +277,7 @@ class SceneBuilder:
             keep.append(a)
             return a
         self._fill_objects(d, keep)
-
-        def mesh(o, it):
-            p, n, t, i = it
-            o.n_verts, o.n_tris = len(p), len(i)
-            o.positions = p.ctypes.data_as(C.POINTER(F.f32)); o.normals = n.ctypes.data_as(C.POINTER(F.f32))
-            o.texcoords = t.ctypes.data_as(C.POINTER(F.f32)); o.indices = i.ctypes.data_as(C.POINTER(F.u32))
-        d.meshes = arr(F.Mesh, self.meshes, mesh); d.n_meshes = len(self.meshes)
-        keep.append(self.meshes)
+        self._fill_meshes(d, keep)
 
         def mat(o, it):
             o.type = it[0]; o.c0[:] = it[1]; o.c1[:] = it[2]; o.roughness = it[3]; o.eta = it[4]; o.merl = it[5]
