@@ -76,6 +76,15 @@ class Scene {
     void replace_meshes(const trb_scene_meshes& meshes, const trb_scene_objects* objects = nullptr) {
         check(trb_scene_replace_meshes(s_, &meshes, objects));
     }
+    // the scene's film and / or integrator replaced in place; a null pointer keeps the current one (trb_scene_replace_settings)
+    void replace_settings(const trb_film* film, const trb_integrator* integrator = nullptr) {
+        check(trb_scene_replace_settings(s_, film, integrator));
+    }
+    // the scene's materials, MERL tables, textures and images replaced in place, with the object section too when `objects` is given
+    // (trb_scene_replace_materials)
+    void replace_materials(const trb_scene_materials& materials, const trb_scene_objects* objects = nullptr) {
+        check(trb_scene_replace_materials(s_, &materials, objects));
+    }
     RenderTarget make_render_target() const { uint32_t w, h; check(trb_scene_info(s_, &w, &h, nullptr, nullptr, nullptr, nullptr)); return RenderTarget(w, h); }
     uint32_t spp() const { uint32_t v; check(trb_scene_info(s_, nullptr, nullptr, &v, nullptr, nullptr, nullptr)); return v; }
     trb_scene* handle() const { return s_; }

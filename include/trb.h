@@ -442,6 +442,45 @@ trb_status trb_scene_replace_meshes(trb_scene* scene, const trb_scene_meshes* me
 trb_status trb_scene_replace_meshes_device(trb_scene* scene, const trb_scene_meshes* meshes, const trb_scene_objects* objects,
                                            void* cuda_stream);
 
+/* Settings replacement: replace the scene's film (`film`) and / or integrator (`integrator`); NULL keeps the current one. A new film
+ * rebuilds the filter table (trb_scene_get_filter_table), the device film and its host staging, the block lists and the Adaptive
+ * sampler's state, and sets the rounded spp from film.samples; a new integrator sets the type and depths and raises the context's
+ * stack limit for Whitted and NormalsDebug as trb_scene_create does (it is never lowered). After a successful call the scene equals
+ * trb_scene_create on the description with the film and integrator replaced and, if a frame has been set, that scene after
+ * trb_scene_update_frame with the last arguments given (the camera's pixel transform follows the film size), on everything the scene
+ * edits above list. Statuses: a null scene is TRB_INVALID_ARG; the film and integrator are checked by the code that checks them in
+ * trb_scene_create, with its statuses and messages. A failed call leaves the scene as it was, with one exception: a CUDA error (a
+ * device fault, not a property of the input) reported while the frame is rebuilt. Drains the device before it frees anything kernels
+ * read; returns when the replacement is complete. The replicas of a trb_group are edited one by one (trb_group_scene); the group
+ * renders refuse replicas of different film sizes with TRB_INVALID_ARG. */
+trb_status trb_scene_replace_settings(trb_scene* scene, const trb_film* film, const trb_integrator* integrator);
+
+/* The material section of a trb_scene_desc, as trb_scene_replace_materials takes it. Same field meanings, same index conventions. */
+typedef struct trb_scene_materials {
+    uint32_t n_materials; const trb_material* materials;
+    uint32_t n_merl;      const float* const* merl_tables; /* each TRB_MERL_TABLE_FLOATS floats */
+    uint32_t n_textures;  const trb_texture* textures;
+    uint32_t n_images;    const trb_image* images;
+} trb_scene_materials;
+
+/* Material replacement: replace the scene's materials, MERL tables, textures and images with the section `materials`, of any counts.
+ * With `objects` the object section is replaced in the same call, as trb_scene_replace_objects replaces it (what renumbered materials
+ * need); with `objects` NULL the instances stay and their material indices index the new list. The shading kernels (fused or split)
+ * and the texture coordinates follow the new section as on a new scene. After a successful call the scene equals trb_scene_create on
+ * the description with the material section (and the object section, if given) replaced and, if a frame has been set, that scene
+ * after trb_scene_update_frame with the last arguments given, on everything the scene edits above list.
+ * Statuses: a null scene or null `materials`, a null array with a non-zero count, a null MERL table, an instance whose material index
+ * is past the new list, or a section none of whose cameras is active at the frame that has been set is TRB_INVALID_ARG. The section
+ * and `objects` are checked by the code that checks them in trb_scene_create, with its statuses and messages. Every new buffer is
+ * built before the scene is switched over, so a failed call leaves the scene as it was, with one exception: a CUDA error (a device
+ * fault, not a property of the input) reported while the frame is rebuilt. Drains the device before it frees anything kernels read;
+ * returns when the replacement is complete. */
+trb_status trb_scene_replace_materials(trb_scene* scene, const trb_scene_materials* materials, const trb_scene_objects* objects);
+/* The same with the MERL tables and each image's rgba8 in device memory on the scene's GPU, read on cuda_stream (a cudaStream_t;
+ * NULL = default stream) with device-to-device copies; `materials`, its arrays of structs and `objects` stay host memory. */
+trb_status trb_scene_replace_materials_device(trb_scene* scene, const trb_scene_materials* materials, const trb_scene_objects* objects,
+                                              void* cuda_stream);
+
 /* -- the hot path ------------------------------------------------------------------ */
 
 /* ≙ Exec::render (exec/mod.rs:48; multithreaded.rs:55-70). Renders the selected

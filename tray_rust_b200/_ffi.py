@@ -116,6 +116,14 @@ class SceneMeshes(C.Structure):
     _fields_ = [("n_meshes", u32), ("meshes", C.POINTER(Mesh)), ("keep", C.POINTER(u32))]
 
 
+class SceneMaterials(C.Structure):
+    """trb_scene_materials: the material section of a SceneDesc (materials, MERL tables, textures, images), with the same field names"""
+    _fields_ = [("n_materials", u32), ("materials", C.POINTER(Material)),
+                ("n_merl", u32), ("merl_tables", C.POINTER(C.POINTER(f32))),
+                ("n_textures", u32), ("textures", C.POINTER(Texture)),
+                ("n_images", u32), ("images", C.POINTER(Image))]
+
+
 class RenderCfg(C.Structure):
     _fields_ = [("spp", u32), ("sample_first", u32), ("sample_count", u32), ("block_start", u32),
                 ("block_count", u32), ("current_frame", u32), ("seed", u32), ("flags", u32),
@@ -239,6 +247,7 @@ TRB_SYMBOLS = [
     "trb_scene_update_mesh", "trb_scene_update_mesh_device",
     "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
     "trb_scene_replace_objects", "trb_scene_replace_meshes", "trb_scene_replace_meshes_device",
+    "trb_scene_replace_settings", "trb_scene_replace_materials", "trb_scene_replace_materials_device",
 ]
 
 _trb = None
@@ -276,6 +285,9 @@ def load_trb():
     lib.trb_scene_replace_objects.argtypes = [vp, C.POINTER(SceneObjects)]
     lib.trb_scene_replace_meshes.argtypes = [vp, C.POINTER(SceneMeshes), C.POINTER(SceneObjects)]
     lib.trb_scene_replace_meshes_device.argtypes = [vp, C.POINTER(SceneMeshes), C.POINTER(SceneObjects), vp]
+    lib.trb_scene_replace_settings.argtypes = [vp, C.POINTER(Film), C.POINTER(Integrator)]
+    lib.trb_scene_replace_materials.argtypes = [vp, C.POINTER(SceneMaterials), C.POINTER(SceneObjects)]
+    lib.trb_scene_replace_materials_device.argtypes = [vp, C.POINTER(SceneMaterials), C.POINTER(SceneObjects), vp]
     lib.trb_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_device.argtypes = [vp, C.POINTER(RenderCfg), vp, vp, vp]
     lib.trb_intersect.argtypes = [vp, sz, vp, vp, C.POINTER(Stats)]

@@ -261,11 +261,44 @@ class Scene(_Base):
         self._check(self._lib.trb_scene_replace_meshes_device(self._h, C.byref(section), None if objects is None else C.byref(objects), stream))
         self._replaced(objects, section)
 
-    def _replaced(self, objects=None, section=None):
-        """the description after a replacement: the object section and / or the mesh list (kept meshes keep their entries)"""
+    def replace_settings(self, film=None, integrator=None):
+        """trb_scene_replace_settings: replace the film (F.Film, or a dict of its fields like SceneBuilder.film) and / or the integrator
+        (F.Integrator, or a (type, min_depth, max_depth) tuple like SceneBuilder.integrator); None keeps the current one. A frame
+        already set is rebuilt."""
+        if isinstance(film, dict):
+            film = F.Film(**film)
+        if isinstance(integrator, tuple):
+            integrator = F.Integrator(*integrator)
+        self._check(self._lib.trb_scene_replace_settings(self._h, None if film is None else C.byref(film),
+                                                           None if integrator is None else C.byref(integrator)))
+        self._replaced(film=film, integrator=integrator)
+
+    def replace_materials(self, section, objects=None):
+        """trb_scene_replace_materials: replace the materials, MERL tables, textures and images with `section` (F.SceneMaterials, e.g.
+        SceneBuilder.materials_section()). With `objects` (F.SceneObjects) the object section is replaced too; without, the instances'
+        material indices index the new list. A frame already set is rebuilt."""
+        self._check(self._lib.trb_scene_replace_materials(self._h, C.byref(section), None if objects is None else C.byref(objects)))
+        self._replaced(objects, materials=section)
+
+    def replace_materials_device(self, section, objects=None, stream=None):
+        """trb_scene_replace_materials_device: the same with the MERL tables and each image's rgba8 as device pointers on the scene's
+        GPU, read on `stream` (a cudaStream_t as an int; None = default stream)."""
+        self._check(self._lib.trb_scene_replace_materials_device(self._h, C.byref(section), None if objects is None else C.byref(objects),
+                                                                 stream))
+        self._replaced(objects, materials=section)
+
+    def _replaced(self, objects=None, section=None, materials=None, film=None, integrator=None):
+        """the description after a replacement: the object section, the mesh list (kept meshes keep their entries), the material section,
+        the film and / or the integrator"""
         desc = F.SceneDesc.from_buffer_copy(self._desc)  # a copy: the caller's description (it may belong to the loader) stays as it is
         for name, _ in F.SceneObjects._fields_ if objects is not None else ():
             setattr(desc, name, getattr(objects, name))
+        for name, _ in F.SceneMaterials._fields_ if materials is not None else ():
+            setattr(desc, name, getattr(materials, name))
+        if film is not None:
+            desc.film = film
+        if integrator is not None:
+            desc.integrator = integrator
         meshes = None
         if section is not None:
             n = section.n_meshes
@@ -274,11 +307,11 @@ class Scene(_Base):
                 k = section.keep[i]
                 meshes[i] = section.meshes[i] if k == F.MESH_NEW else self._desc.meshes[k]
             desc.meshes, desc.n_meshes = meshes, n
-        desc._keep = (self._desc, objects, section, meshes)  # the arrays they point into
+        desc._keep = (self._desc, objects, section, meshes, materials)  # the arrays they point into
         self._desc = desc
-        ni, nl = F.u32(), F.u32()
-        self._check(self._lib.trb_scene_info(self._h, None, None, None, None, C.byref(ni), C.byref(nl)))
-        self.n_instances, self.n_lights = ni.value, nl.value
+        w, hh, spp, nb, ni, nl = (F.u32() for _ in range(6))
+        self._check(self._lib.trb_scene_info(self._h, *(C.byref(x) for x in (w, hh, spp, nb, ni, nl))))
+        self.width, self.height, self.spp, self.total_blocks, self.n_instances, self.n_lights = (x.value for x in (w, hh, spp, nb, ni, nl))
 
     def set_option(self, name, value):
         """trb_scene_set_option: launch-shape options (never change results)."""

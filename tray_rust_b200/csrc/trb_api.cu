@@ -418,30 +418,47 @@ trb_status validate_mesh(const trb_mesh& m, bool device) {
     return TRB_OK;
 }
 
-trb_status validate(const trb_scene_desc* d) {
-    if (!d) return fail(TRB_INVALID_ARG, "null scene description");
-    if (d->abi_version != TRB_ABI_VERSION) return fail(TRB_INVALID_ARG, "trb_scene_desc.abi_version mismatch");
-    if (d->film.width == 0 || d->film.height == 0 || d->film.width % 8 || d->film.height % 8)
+// The film and the integrator of a description (trb_scene_create, trb_scene_replace_settings)
+trb_status validate_settings(const trb_film& f, const trb_integrator& in) {
+    if (f.width == 0 || f.height == 0 || f.width % 8 || f.height % 8)
         return fail(TRB_INVALID_ARG, "Image not evenly divided by blocks of (8, 8)"); // block_queue.rs:29-31
-    if (d->film.frames == 0) return fail(TRB_INVALID_ARG, "film.frames must be >= 1");
-    if (d->integrator.type > TRB_INTEGRATOR_NORMALS_DEBUG) return fail(TRB_INVALID_ARG, "Unrecognized integrator type"); // scene.rs:313
-    if (d->integrator.type == TRB_INTEGRATOR_PATH && d->integrator.max_depth > 57u) return fail(TRB_UNSUPPORTED, "max_depth > 57");
-    if (d->integrator.type == TRB_INTEGRATOR_WHITTED && d->integrator.max_depth > 24u) return fail(TRB_UNSUPPORTED, "whitted max_depth > 24 (device recursion stack)");
-    if (!(d->film.filter_w > 0.0f && d->film.filter_h > 0.0f)) return fail(TRB_INVALID_ARG, "filter width/height must be positive");
-    if (floorf(d->film.filter_w / 0.5f) > 8.0f || floorf(d->film.filter_h / 0.5f) > 8.0f) return fail(TRB_UNSUPPORTED, "filter wider than 4 pixels");
-    { const trb_status r = validate_objects(desc_objects(*d), d->n_meshes, d->n_materials); if (r != TRB_OK) return r; }
-    for (uint32_t i = 0; i < d->n_materials; ++i) {
-        const trb_status r = validate_material(d->materials[i], d->n_merl, d->n_textures);
+    if (f.frames == 0) return fail(TRB_INVALID_ARG, "film.frames must be >= 1");
+    if (in.type > TRB_INTEGRATOR_NORMALS_DEBUG) return fail(TRB_INVALID_ARG, "Unrecognized integrator type"); // scene.rs:313
+    if (in.type == TRB_INTEGRATOR_PATH && in.max_depth > 57u) return fail(TRB_UNSUPPORTED, "max_depth > 57");
+    if (in.type == TRB_INTEGRATOR_WHITTED && in.max_depth > 24u) return fail(TRB_UNSUPPORTED, "whitted max_depth > 24 (device recursion stack)");
+    if (!(f.filter_w > 0.0f && f.filter_h > 0.0f)) return fail(TRB_INVALID_ARG, "filter width/height must be positive");
+    if (floorf(f.filter_w / 0.5f) > 8.0f || floorf(f.filter_h / 0.5f) > 8.0f) return fail(TRB_UNSUPPORTED, "filter wider than 4 pixels");
+    return TRB_OK;
+}
+
+trb_scene_materials desc_materials(const trb_scene_desc& d) {
+    return {d.n_materials, d.materials, d.n_merl, d.merl_tables, d.n_textures, d.textures, d.n_images, d.images};
+}
+
+// The material section of a description (trb_scene_create, trb_scene_replace_materials): materials against its own MERL and texture
+// counts, texture image ranges, images and the texel limit. Images in device memory are checked the same way (their pixels are not read).
+trb_status validate_materials(const trb_scene_materials& m) {
+    for (uint32_t i = 0; i < m.n_materials; ++i) {
+        const trb_status r = validate_material(m.materials[i], m.n_merl, m.n_textures);
         if (r != TRB_OK) return r;
     }
     uint64_t texels = 0;
-    for (uint32_t i = 0; i < d->n_textures; ++i)
-        if (d->textures[i].n_images == 0 || (uint64_t)d->textures[i].first_image + d->textures[i].n_images > d->n_images) return fail(TRB_INVALID_ARG, "texture image range out of bounds");
-    for (uint32_t i = 0; i < d->n_images; ++i) {
-        if (d->images[i].width == 0 || d->images[i].height == 0 || !d->images[i].rgba8) return fail(TRB_INVALID_ARG, "empty image");
-        texels += (uint64_t)d->images[i].width * d->images[i].height;
+    for (uint32_t i = 0; i < m.n_textures; ++i)
+        if (m.textures[i].n_images == 0 || (uint64_t)m.textures[i].first_image + m.textures[i].n_images > m.n_images) return fail(TRB_INVALID_ARG, "texture image range out of bounds");
+    for (uint32_t i = 0; i < m.n_images; ++i) {
+        if (m.images[i].width == 0 || m.images[i].height == 0 || !m.images[i].rgba8) return fail(TRB_INVALID_ARG, "empty image");
+        texels += (uint64_t)m.images[i].width * m.images[i].height;
     }
     if (texels >= (1ull << 32)) return fail(TRB_UNSUPPORTED, "more than 2^32 texels of image textures");
+    return TRB_OK;
+}
+
+trb_status validate(const trb_scene_desc* d) {
+    if (!d) return fail(TRB_INVALID_ARG, "null scene description");
+    if (d->abi_version != TRB_ABI_VERSION) return fail(TRB_INVALID_ARG, "trb_scene_desc.abi_version mismatch");
+    { const trb_status r = validate_settings(d->film, d->integrator); if (r != TRB_OK) return r; }
+    { const trb_status r = validate_objects(desc_objects(*d), d->n_meshes, d->n_materials); if (r != TRB_OK) return r; }
+    { const trb_status r = validate_materials(desc_materials(*d)); if (r != TRB_OK) return r; }
     for (uint32_t i = 0; i < d->n_meshes; ++i) {
         const trb_status r = validate_mesh(d->meshes[i], false);
         if (r != TRB_OK) return r;
@@ -1777,10 +1794,10 @@ void objects_replaced(trb_scene* s) {
     if (s->wf.n_anim != s->n_anim) s->wf_capacity = 0; // WfState::xf_tab is sized by n_anim: ensure_wavefront allocates the state anew
 }
 
-// The checks of a new object section against a scene whose meshes will number n_meshes: trb_scene_create's, and that the frame that
-// has been set can be set again
-trb_status check_objects(const trb_scene* s, const trb_scene_objects& o, uint32_t n_meshes) {
-    const trb_status v = validate_objects(o, n_meshes, (uint32_t)s->materials.size());
+// The checks of a new object section against a scene whose meshes and materials will number n_meshes and n_materials:
+// trb_scene_create's, and that the frame that has been set can be set again
+trb_status check_objects(const trb_scene* s, const trb_scene_objects& o, uint32_t n_meshes, uint32_t n_materials) {
+    const trb_status v = validate_objects(o, n_meshes, n_materials);
     if (v != TRB_OK) return v;
     if (s->frame_set && o.cameras[0].active_at > s->last_frame) return fail(TRB_INVALID_ARG, "no camera is active at this frame");
     return TRB_OK;
@@ -1788,7 +1805,7 @@ trb_status check_objects(const trb_scene* s, const trb_scene_objects& o, uint32_
 
 // Checked as trb_scene_create checks the section; then set_objects, the state that was sized or built for the old section, and the frame
 trb_status replace_objects(trb_scene* s, const trb_scene_objects& o) {
-    const trb_status v = check_objects(s, o, (uint32_t)s->meshes.size());
+    const trb_status v = check_objects(s, o, (uint32_t)s->meshes.size(), (uint32_t)s->materials.size());
     if (v != TRB_OK) return v;
     CU(cudaSetDevice(s->device));
     CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
@@ -1815,7 +1832,7 @@ trb_status replace_meshes(trb_scene* s, const trb_scene_meshes& sec, const trb_s
         if (named[k]) return fail(TRB_INVALID_ARG, "a mesh is kept twice");
         named[k] = 1;
     }
-    if (o) { const trb_status v = check_objects(s, *o, n); if (v != TRB_OK) return v; }
+    if (o) { const trb_status v = check_objects(s, *o, n, (uint32_t)s->materials.size()); if (v != TRB_OK) return v; }
     else
         for (const trb_instance& in : s->instances)
             if (in.shape == TRB_SHAPE_MESH && in.mesh >= n) return fail(TRB_INVALID_ARG, "mesh index out of range");
@@ -1866,6 +1883,172 @@ trb_status replace_meshes(trb_scene* s, const trb_scene_meshes& sec, const trb_s
     if (o) { commit_objects(s, g); objects_replaced(s); }
     else { s->instances_static_uploaded = false; s->frame_ready = false; } // the instances' mesh bounds changed
     if (repack) { const trb_status r = upload_mesh_nodes(s, wide); if (r != TRB_OK) return r; }
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    return TRB_OK;
+}
+
+// ---- film, integrator and material section (trb_scene_create, trb_scene_replace_settings / _materials; DESIGN.md §4 "Settings
+// replacement" and "Material replacement") ---------------------------------------------------------------------------------------
+// Each part is staged into fresh buffers without touching the scene, then committed once the device has been drained, so creation
+// and replacement run the same code and a failed replacement leaves the scene as it was.
+
+// k_simple_integrator (Whitted and NormalsDebug) is recursive, so its stack is the context's limit, not a size ptxas computed: the
+// reference's recursion is kept as device recursion (one frame per ray depth), and even NormalsDebug's one scene_trace call (kernel
+// frame + scene_trace's, about 1.8 KB on sm_90a) needs more than CUDA's default 1 KB. The limit is raised, never lowered.
+trb_status raise_stack_limit(const trb_integrator& in) {
+    if (in.type != TRB_INTEGRATOR_WHITTED && in.type != TRB_INTEGRATOR_NORMALS_DEBUG) return TRB_OK;
+    size_t have = 0;
+    CU(cudaDeviceGetLimit(&have, cudaLimitStackSize));
+    const size_t need = 4096 + (size_t)2048 * (in.max_depth + 2);
+    if (have < need) CU(cudaDeviceSetLimit(cudaLimitStackSize, need));
+    return TRB_OK;
+}
+
+// The film's filter table (host and device), the device film of trb_render and its pinned host staging
+struct StagedFilm {
+    trb_film film{};
+    float table[256];
+    DeviceArena fresh; // frees what it holds unless committed
+    float* d_table = nullptr;
+    float4* d_film = nullptr;
+    float* h_staging = nullptr; // pinned; freed unless committed
+    ~StagedFilm() { if (h_staging) cudaFreeHost(h_staging); }
+};
+
+trb_status stage_film(const trb_film& f, StagedFilm& g) {
+    g.film = f;
+    filter_table(f, g.table);
+    const size_t npx = (size_t)f.width * f.height;
+    CU(g.fresh.upload(g.table, 256, &g.d_table));
+    CU(g.fresh.alloc(npx, &g.d_film));
+    CU(cudaMallocHost(&g.h_staging, npx * 4 * sizeof(float)));
+    return TRB_OK;
+}
+
+// Also retires what was made for the old film: the Morton block lists (keyed by the selection, not by the film size) and the Adaptive
+// sampler's per-pixel and per-block state (sized by the pixel count; ensure_adaptive allocates it anew). The caller has drained the device.
+void commit_film(trb_scene* s, StagedFilm& g) {
+    trb::DScene& ds = s->ds;
+    s->arena.release(ds.filter_table); s->arena.release(s->d_film);
+    s->arena.ptrs.insert(s->arena.ptrs.end(), g.fresh.ptrs.begin(), g.fresh.ptrs.end());
+    g.fresh.ptrs.clear();
+    if (s->h_film_staging) cudaFreeHost(s->h_film_staging);
+    s->h_film_staging = g.h_staging; g.h_staging = nullptr;
+    s->d_film = g.d_film;
+    const trb_film& f = g.film;
+    s->film = f;
+    std::memcpy(s->table, g.table, sizeof s->table);
+    s->spp_pow2 = pow2_ceil(std::max(1u, f.samples));
+    ds.width = f.width; ds.height = f.height;
+    ds.filter_w = f.filter_w; ds.filter_h = f.filter_h;
+    ds.filter_inv_w = 1.0f / f.filter_w; ds.filter_inv_h = 1.0f / f.filter_h;
+    ds.fpw_x = (int)floorf(f.filter_w / 0.5f); ds.fpw_y = (int)floorf(f.filter_h / 0.5f); // render_target.rs:48-49
+    // the per-pixel test accepts |d| <= w / inv_w; the lock-block filter of render_target.rs:104-109 can only reject beyond fpw - 0.5
+    ds.film_block_filter = (f.filter_w / ds.filter_inv_w <= (float)ds.fpw_x && f.filter_h / ds.filter_inv_h <= (float)ds.fpw_y) ? 0u : 1u;
+    ds.filter_table = g.d_table;
+    for (BlockList& b : s->block_lists) cudaFree(b.dev);
+    s->block_lists.clear();
+    for (void** p : {(void**)&s->d_ad_state, (void**)&s->d_ad_list[0], (void**)&s->d_ad_list[1], (void**)&s->d_ad_index[0],
+                     (void**)&s->d_ad_index[1], (void**)&s->d_ad_flags, (void**)&s->d_ad_count, (void**)&s->d_ad_spp}) {
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+    }
+}
+
+// The material records, MERL tables and image textures, and the counts they are checked against
+struct StagedMaterials {
+    std::vector<trb_material> materials;
+    uint32_t n_merl = 0, n_textures = 0;
+    DeviceArena fresh; // frees what it holds unless committed
+    trb::DMaterial* d_mats = nullptr;
+    float* d_merl = nullptr;
+    trb::DImage* d_img = nullptr; trb::DTexture* d_tex = nullptr; uchar4* d_tx = nullptr;
+};
+
+// `m` checked by validate_materials. With `device` the MERL tables and the images' texels are device memory on the scene's GPU,
+// copied on `st`; otherwise host memory.
+trb_status stage_materials(const trb_scene_materials& m, bool device, cudaStream_t st, StagedMaterials& g) {
+    g.materials.assign(m.materials, m.materials + m.n_materials);
+    g.n_merl = m.n_merl; g.n_textures = m.n_textures;
+    // precompute what Material::bsdf recomputes per hit from constant textures
+    std::vector<trb::DMaterial> dmats(m.n_materials);
+    for (uint32_t i = 0; i < m.n_materials; ++i) dmats[i] = device_material(m.materials[i]);
+    CU(g.fresh.upload(dmats.data(), dmats.size(), &g.d_mats));
+    auto copy = [&](void* dst, const void* src, size_t bytes) {
+        return device ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) : cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
+    };
+    CU(g.fresh.alloc((size_t)m.n_merl * TRB_MERL_TABLE_FLOATS, &g.d_merl));
+    for (uint32_t i = 0; i < m.n_merl; ++i)
+        CU(copy(g.d_merl + (size_t)i * TRB_MERL_TABLE_FLOATS, m.merl_tables[i], sizeof(float) * TRB_MERL_TABLE_FLOATS));
+    // image textures: every frame's RGBA8 texels in one array (texture/image.rs)
+    std::vector<trb::DImage> dimg(m.n_images);
+    std::vector<trb::DTexture> dtex(m.n_textures);
+    size_t n_tx = 0;
+    for (uint32_t i = 0; i < m.n_images; ++i) {
+        const trb_image& im = m.images[i];
+        dimg[i].width = im.width; dimg[i].height = im.height; dimg[i].offset = (uint32_t)n_tx; dimg[i].time = im.time;
+        n_tx += (size_t)im.width * im.height;
+    }
+    for (uint32_t i = 0; i < m.n_textures; ++i) { dtex[i].first_image = m.textures[i].first_image; dtex[i].n_images = m.textures[i].n_images; }
+    CU(g.fresh.upload(dimg.data(), dimg.size(), &g.d_img));
+    CU(g.fresh.upload(dtex.data(), dtex.size(), &g.d_tex));
+    CU(g.fresh.alloc(n_tx, &g.d_tx));
+    for (uint32_t i = 0; i < m.n_images; ++i)
+        CU(copy(g.d_tx + dimg[i].offset, m.images[i].rgba8, (size_t)m.images[i].width * m.images[i].height * 4));
+    if (device) CU(cudaStreamSynchronize(st));
+    return TRB_OK;
+}
+
+// Also the shading shape (material_shape), which needs the object section in place. The caller has drained the device.
+void commit_materials(trb_scene* s, StagedMaterials& g) {
+    trb::DScene& ds = s->ds;
+    for (const void* p : {(const void*)ds.materials, (const void*)ds.merl, (const void*)ds.images, (const void*)ds.textures,
+                          (const void*)ds.texels}) s->arena.release(p);
+    s->arena.ptrs.insert(s->arena.ptrs.end(), g.fresh.ptrs.begin(), g.fresh.ptrs.end());
+    g.fresh.ptrs.clear();
+    s->materials.swap(g.materials); s->n_merl = g.n_merl;
+    ds.materials = g.d_mats; ds.merl = g.d_merl;
+    ds.images = g.d_img; ds.textures = g.d_tex; ds.texels = g.d_tx; ds.n_textures = g.n_textures;
+    material_shape(s);
+}
+
+// trb_scene_replace_settings: checked as trb_scene_create checks the film and the integrator; the new film staged and the stack limit
+// raised before the device is drained and anything switched; then the frame, whose camera depends on the film size
+trb_status replace_settings(trb_scene* s, const trb_film* film, const trb_integrator* integrator) {
+    const trb_integrator in = integrator ? *integrator : s->integrator;
+    { const trb_status v = validate_settings(film ? *film : s->film, in); if (v != TRB_OK) return v; }
+    CU(cudaSetDevice(s->device));
+    StagedFilm g;
+    if (film) { const trb_status r = stage_film(*film, g); if (r != TRB_OK) return r; }
+    if (integrator) { const trb_status r = raise_stack_limit(in); if (r != TRB_OK) return r; }
+    CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
+    if (film) commit_film(s, g);
+    s->integrator = in;
+    s->ds.min_depth = in.min_depth; s->ds.max_depth = in.max_depth;
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
+    return TRB_OK;
+}
+
+// trb_scene_replace_materials(_device): checks everything first (null arrays, the section as creation checks it, the object section or
+// the current instances against the new material count), stages the section and the object section, and only then drains the device
+// and switches the scene over
+trb_status replace_materials(trb_scene* s, const trb_scene_materials& m, const trb_scene_objects* o, bool device, cudaStream_t st) {
+    if ((m.n_materials && !m.materials) || (m.n_merl && !m.merl_tables) || (m.n_textures && !m.textures) || (m.n_images && !m.images))
+        return fail(TRB_INVALID_ARG, "null array with a non-zero count");
+    for (uint32_t i = 0; i < m.n_merl; ++i) if (!m.merl_tables[i]) return fail(TRB_INVALID_ARG, "null MERL table");
+    { const trb_status v = validate_materials(m); if (v != TRB_OK) return v; }
+    if (o) { const trb_status v = check_objects(s, *o, (uint32_t)s->meshes.size(), m.n_materials); if (v != TRB_OK) return v; }
+    else
+        for (const trb_instance& in : s->instances)
+            if (in.kind != TRB_INST_EMITTER_POINT && in.material >= m.n_materials) return fail(TRB_INVALID_ARG, "material index out of range");
+    CU(cudaSetDevice(s->device));
+    StagedMaterials g;
+    { const trb_status r = stage_materials(m, device, st, g); if (r != TRB_OK) return r; }
+    StagedObjects go;
+    if (o) { const trb_status r = stage_objects(s, *o, go); if (r != TRB_OK) return r; }
+    CU(cudaDeviceSynchronize()); // passes enqueued by the _device calls may still read the buffers released below
+    commit_materials(s, g);
+    if (o) { commit_objects(s, go); objects_replaced(s); }
     if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
     return TRB_OK;
 }
@@ -1924,6 +2107,23 @@ trb_status trb_scene_replace_meshes_device(trb_scene* s, const trb_scene_meshes*
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     if (!meshes) return fail(TRB_INVALID_ARG, "null meshes");
     return replace_meshes(s, *meshes, objects, true, static_cast<cudaStream_t>(cuda_stream));
+}
+
+trb_status trb_scene_replace_settings(trb_scene* s, const trb_film* film, const trb_integrator* integrator) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    return replace_settings(s, film, integrator);
+}
+
+trb_status trb_scene_replace_materials(trb_scene* s, const trb_scene_materials* materials, const trb_scene_objects* objects) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (!materials) return fail(TRB_INVALID_ARG, "null materials");
+    return replace_materials(s, *materials, objects, false, nullptr);
+}
+trb_status trb_scene_replace_materials_device(trb_scene* s, const trb_scene_materials* materials, const trb_scene_objects* objects,
+                                              void* cuda_stream) {
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (!materials) return fail(TRB_INVALID_ARG, "null materials");
+    return replace_materials(s, *materials, objects, true, static_cast<cudaStream_t>(cuda_stream));
 }
 
 const char* trb_last_error(void) { return g_error.c_str(); }
@@ -2006,21 +2206,11 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     std::unique_ptr<trb_scene> s(new trb_scene);
     s->device = device;
     tuning_from_env(s->tune);
-    // k_simple_integrator (Whitted and NormalsDebug) is recursive, so its stack is the context's limit, not a size ptxas computed: the
-    // reference's recursion is kept as device recursion (one frame per ray depth), and even NormalsDebug's one scene_trace call
-    // (kernel frame + scene_trace's, about 1.8 KB on sm_90a) needs more than CUDA's default 1 KB
-    if (d->integrator.type == TRB_INTEGRATOR_WHITTED || d->integrator.type == TRB_INTEGRATOR_NORMALS_DEBUG) {
-        size_t have = 0;
-        CU(cudaDeviceGetLimit(&have, cudaLimitStackSize));
-        const size_t need = 4096 + (size_t)2048 * (d->integrator.max_depth + 2);
-        if (have < need) CU(cudaDeviceSetLimit(cudaLimitStackSize, need));
-    }
+    { const trb_status r = raise_stack_limit(d->integrator); if (r != TRB_OK) return r; }
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
     s->sm_count = prop.multiProcessorCount;
-    s->film = d->film; s->integrator = d->integrator;
-    s->spp_pow2 = pow2_ceil(std::max(1u, d->film.samples));
-    s->materials.assign(d->materials, d->materials + d->n_materials);
+    s->integrator = d->integrator;
 
     // meshes: BVH<Triangle> with max_geom 16 (mesh.rs:44), then leaf-ordered triangle records
     s->dmeshes.resize(d->n_meshes);
@@ -2032,60 +2222,26 @@ trb_status trb_scene_create(const trb_scene_desc* d, int device, trb_scene** out
     }
     CU(s->arena.alloc(s->dmeshes.size(), &s->d_meshes));
     { const trb_status r = upload_mesh_nodes(s.get(), s->needs_wide || s->tune.wide_leaf != 0); if (r != TRB_OK) return r; }
-    trb::DMesh* d_meshes = s->d_meshes;
-
-    // materials (precompute what Material::bsdf recomputes per hit from constant textures)
-    std::vector<trb::DMaterial> dmats(d->n_materials);
-    for (uint32_t i = 0; i < d->n_materials; ++i) dmats[i] = device_material(d->materials[i]);
-    trb::DMaterial* d_mats;
-    CU(s->arena.upload(dmats.data(), dmats.size(), &d_mats));
-    s->n_merl = d->n_merl;
-    float* d_merl = nullptr;
-    CU(s->arena.alloc((size_t)d->n_merl * TRB_MERL_TABLE_FLOATS, &d_merl));
-    for (uint32_t i = 0; i < d->n_merl; ++i)
-        CU(cudaMemcpy(d_merl + (size_t)i * TRB_MERL_TABLE_FLOATS, d->merl_tables[i], sizeof(float) * TRB_MERL_TABLE_FLOATS, cudaMemcpyHostToDevice));
-
-    { // image textures: every frame's RGBA8 texels in one array (texture/image.rs)
-        std::vector<trb::DImage> dimg(d->n_images);
-        std::vector<trb::DTexture> dtex(d->n_textures);
-        std::vector<uchar4> tx;
-        for (uint32_t i = 0; i < d->n_images; ++i) {
-            const trb_image& im = d->images[i];
-            dimg[i].width = im.width; dimg[i].height = im.height; dimg[i].offset = (uint32_t)tx.size(); dimg[i].time = im.time;
-            const size_t n = (size_t)im.width * im.height;
-            tx.resize(tx.size() + n);
-            std::memcpy(tx.data() + dimg[i].offset, im.rgba8, n * 4);
-        }
-        for (uint32_t i = 0; i < d->n_textures; ++i) { dtex[i].first_image = d->textures[i].first_image; dtex[i].n_images = d->textures[i].n_images; }
-        trb::DImage* d_img = nullptr; trb::DTexture* d_tex = nullptr; uchar4* d_tx = nullptr;
-        CU(s->arena.upload(dimg.data(), dimg.size(), &d_img));
-        CU(s->arena.upload(dtex.data(), dtex.size(), &d_tex));
-        CU(s->arena.upload(tx.data(), tx.size(), &d_tx));
-        s->ds.images = d_img; s->ds.textures = d_tex; s->ds.texels = d_tx; s->ds.n_textures = d->n_textures;
+    s->ds.meshes = s->d_meshes;
+    {
+        StagedMaterials g;
+        const trb_status r = stage_materials(desc_materials(*d), false, nullptr, g);
+        if (r != TRB_OK) return r;
+        commit_materials(s.get(), g);
     }
-    filter_table(d->film, s->table);
-    float* d_table;
-    CU(s->arena.upload(s->table, 256, &d_table));
-
+    {
+        StagedFilm g;
+        const trb_status r = stage_film(d->film, g);
+        if (r != TRB_OK) return r;
+        commit_film(s.get(), g);
+    }
     CU(s->arena.alloc(1, &s->d_counter));
     CU(s->arena.alloc(1, &s->d_error));
     CU(cudaMemset(s->d_error, 0, sizeof(int)));
     CU(s->arena.alloc(1, &s->d_stats));
-    CU(s->arena.alloc((size_t)d->film.width * d->film.height, &s->d_film));
-    CU(cudaMallocHost(&s->h_film_staging, (size_t)d->film.width * d->film.height * 4 * sizeof(float)));
     CU(cudaEventCreate(&s->ev0));
     CU(cudaEventCreate(&s->ev1));
-
-    trb::DScene& ds = s->ds;
-    ds.meshes = d_meshes; ds.materials = d_mats; ds.merl = d_merl;
-    ds.width = d->film.width; ds.height = d->film.height;
-    ds.min_depth = d->integrator.min_depth; ds.max_depth = d->integrator.max_depth;
-    ds.filter_w = d->film.filter_w; ds.filter_h = d->film.filter_h;
-    ds.filter_inv_w = 1.0f / d->film.filter_w; ds.filter_inv_h = 1.0f / d->film.filter_h;
-    ds.fpw_x = (int)floorf(d->film.filter_w / 0.5f); ds.fpw_y = (int)floorf(d->film.filter_h / 0.5f); // render_target.rs:48-49
-    // the per-pixel test accepts |d| <= w / inv_w; the lock-block filter of render_target.rs:104-109 can only reject beyond fpw - 0.5
-    ds.film_block_filter = (d->film.filter_w / ds.filter_inv_w <= (float)ds.fpw_x && d->film.filter_h / ds.filter_inv_h <= (float)ds.fpw_y) ? 0u : 1u;
-    ds.filter_table = d_table;
+    s->ds.min_depth = d->integrator.min_depth; s->ds.max_depth = d->integrator.max_depth;
     { const trb_status r = set_objects(s.get(), desc_objects(*d)); if (r != TRB_OK) return r; }
     // Scene::load_file builds the BVH<Instance> for [0, scene_time] (scene.rs:141); the first render rebuilds it
     *out = s.release();
@@ -3336,6 +3492,9 @@ namespace {
 trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
     if (!g || !cfg || !film) return fail(TRB_INVALID_ARG, "null argument");
     const int n = (int)g->scenes.size();
+    for (const trb_scene* s : g->scenes) // the film reduce is sized by replica 0 (trb_scene_replace_settings edits one replica at a time)
+        if (s->film.width != g->scenes[0]->film.width || s->film.height != g->scenes[0]->film.height)
+            return fail(TRB_INVALID_ARG, "the group's replicas have different film sizes");
     if (n == 1) return ad ? trb_render_adaptive(g->scenes[0], cfg, ad, film, pixel_spp, stats) : trb_render(g->scenes[0], cfg, film, stats);
     if (ad) {
         trbh::AdSchedule sch;

@@ -263,21 +263,18 @@ class SceneBuilder:
         s.keep = k
         return s
 
-    def finish(self):
-        d = F.SceneDesc()
-        d.abi_version = F.TRB_ABI_VERSION
-        d.film = F.Film(**self.film)
-        d.integrator = F.Integrator(*self.integrator)
-        keep = self._keep
-
+    def _fill_materials(self, d, keep):
+        """the material section's four arrays and counts into d (a SceneDesc or a SceneMaterials: same field names). The MERL tables and
+        images are passed as the builder holds them: numpy arrays, or torch CUDA tensors for Scene.replace_materials_device"""
         def arr(ctype, items, conv):
             a = (ctype * max(1, len(items)))()
             for i, it in enumerate(items):
                 conv(a[i], it)
             keep.append(a)
             return a
-        self._fill_objects(d, keep)
-        self._fill_meshes(d, keep)
+
+        def addr(t):
+            return t.data_ptr() if hasattr(t, "data_ptr") else t.ctypes.data
 
         def mat(o, it):
             o.type = it[0]; o.c0[:] = it[1]; o.c1[:] = it[2]; o.roughness = it[3]; o.eta = it[4]; o.merl = it[5]
@@ -285,8 +282,8 @@ class SceneBuilder:
         d.materials = arr(F.Material, self.materials, mat); d.n_materials = len(self.materials)
         mt = (C.POINTER(F.f32) * max(1, len(self.merl)))()
         for i, t in enumerate(self.merl):
-            mt[i] = t.ctypes.data_as(C.POINTER(F.f32))
-        keep.append(mt); keep.append(self.merl)
+            mt[i] = C.cast(addr(t), C.POINTER(F.f32))
+        keep.append(mt); keep.append(list(self.merl))
         d.merl_tables = mt; d.n_merl = len(self.merl)
 
         def tex(o, it):
@@ -296,9 +293,60 @@ class SceneBuilder:
         def image(o, it):
             px, t = it
             o.height, o.width = px.shape[0], px.shape[1]
-            o.rgba8 = px.ctypes.data_as(C.POINTER(C.c_uint8)); o.time = t
+            o.rgba8 = C.cast(addr(px), C.POINTER(C.c_uint8)); o.time = t
         d.images = arr(F.Image, self.images, image); d.n_images = len(self.images)
-        keep.append(self.images)
+        keep.append(list(self.images))
+
+    def materials_section(self):
+        """The builder's material section (trb_scene_materials) for Scene.replace_materials: its materials, MERL tables, textures and
+        images, as finish() would give them."""
+        s = F.SceneMaterials()
+        s._keep = []
+        self._fill_materials(s, s._keep)
+        return s
+
+    def remove_material(self, i):
+        """Drop material i and renumber the instances that use the materials above it: the builder is then the one that never added it.
+        Refused (ValueError) while an instance other than a point light (which has no material) uses material i. Returns the removed
+        material."""
+        users = [k for k, it in enumerate(self.instances) if it[0] != F.INST_EMITTER_POINT and it[5] == i]
+        if users:
+            raise ValueError("material %d is used by instances %s" % (i, users))
+        self.instances = [it[:5] + (it[5] - 1,) + it[6:] if it[0] != F.INST_EMITTER_POINT and it[5] > i else it for it in self.instances]
+        return self.materials.pop(i)
+
+    def remove_texture(self, i):
+        """Drop texture i (the value add_texture returned is i + 1) with its images, and renumber the materials' texture bindings and the
+        other textures' image ranges: the builder is then the one that never added it. Refused (ValueError) while a material is bound to
+        it. Returns the removed texture's frames [(pixels, time), ...]."""
+        users = [k for k, m in enumerate(self.materials) if i + 1 in tuple(m[6])]
+        if users:
+            raise ValueError("texture %d is used by materials %s" % (i, users))
+        first, n = self.textures.pop(i)
+        frames = self.images[first:first + n]
+        del self.images[first:first + n]
+        self.textures = [(f - n if f > first else f, k) for f, k in self.textures]
+        self.materials = [m[:6] + (tuple(t - 1 if t > i + 1 else t for t in m[6]),) for m in self.materials]
+        return frames
+
+    def remove_merl_table(self, i):
+        """Drop MERL table i and renumber the MERL materials that use the tables above it: the builder is then the one that never added
+        it. Refused (ValueError) while a MERL material uses table i. Returns the removed table."""
+        users = [k for k, m in enumerate(self.materials) if m[0] == F.MAT_MERL and m[5] == i]
+        if users:
+            raise ValueError("MERL table %d is used by materials %s" % (i, users))
+        self.materials = [m[:5] + (m[5] - 1,) + m[6:] if m[0] == F.MAT_MERL and m[5] > i else m for m in self.materials]
+        return self.merl.pop(i)
+
+    def finish(self):
+        d = F.SceneDesc()
+        d.abi_version = F.TRB_ABI_VERSION
+        d.film = F.Film(**self.film)
+        d.integrator = F.Integrator(*self.integrator)
+        keep = self._keep
+        self._fill_objects(d, keep)
+        self._fill_meshes(d, keep)
+        self._fill_materials(d, keep)
         d._keep = keep
         return d
 
