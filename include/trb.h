@@ -362,6 +362,23 @@ trb_status trb_scene_update_mesh(trb_scene* scene, uint32_t mesh, const float* p
 trb_status trb_scene_update_mesh_device(trb_scene* scene, uint32_t mesh, const float* d_positions, const float* d_normals,
                                         const float* d_texcoords, void* cuda_stream);
 
+/* Refit mesh `mesh` to new vertex positions: the mesh's BVH<Triangle> keeps the partition its build chose (same nodes, order,
+ * second_child, axis, geom_offset, ngeom and ordered_geom) and each node's box becomes the fold of bvh.rs:143 over that node's
+ * triangles at the new positions: BBox::new() unioned with Triangle::bounds of each of them (a bound tied between -0.0 and +0.0 may
+ * carry either sign; NaN components are dropped as fminf / fmaxf drop them). The triangle and node records are rewritten on the device
+ * and, if a frame has been set, trb_scene_update_frame is re-run with its last arguments; renders, counters and queries then follow
+ * the reference's traversal over that tree. The mesh then has no records for the trace.quads experiment (it returns TRB_UNSUPPORTED).
+ * Arguments, the stream rule and the statuses are trb_scene_update_mesh's; positions NULL is exactly its attribute copy. The refit
+ * depends on no value of the positions, so it does not fail on them: positions that a rebuild refuses refit fine. The frame it re-runs
+ * keeps trb_scene_update_frame's rule, which refuses infinite or NaN instance bounds among more than four instances; the mesh is then
+ * refit and the call returns that status with no frame set. Otherwise a failed call leaves the scene as it was, except for a CUDA
+ * error (a device fault), which may leave it half refit. A refit tree is correct however far the mesh has moved, but slower to trace
+ * as it deforms: trb_scene_update_mesh rebuilds it. */
+trb_status trb_scene_refit_mesh(trb_scene* scene, uint32_t mesh, const float* positions, const float* normals, const float* texcoords);
+/* The same from device buffers on the scene's GPU, read on cuda_stream (a cudaStream_t; NULL = default stream); returns when complete. */
+trb_status trb_scene_refit_mesh_device(trb_scene* scene, uint32_t mesh, const float* d_positions, const float* d_normals,
+                                       const float* d_texcoords, void* cuda_stream);
+
 /* Scene edits: replace entries [first, first + count) of one array of the description. The structure of the scene (counts, index
  * ranges, which instance is a light, which spline is keyframed) stays; only the values change (trb_scene_replace_objects, below,
  * changes the structure). After a successful call the scene

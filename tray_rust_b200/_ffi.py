@@ -244,7 +244,7 @@ TRB_SYMBOLS = [
     "trb_light_pdf", "trb_light_pdf_device", "trb_emitted", "trb_emitted_device", "trb_scene_lights",
     "trb_film_write", "trb_film_write_device", "trb_camera_rays_device", "trb_host_film_to_srgb8",
     "trb_build_bvh", "trb_build_bvh_device",
-    "trb_scene_update_mesh", "trb_scene_update_mesh_device",
+    "trb_scene_update_mesh", "trb_scene_update_mesh_device", "trb_scene_refit_mesh", "trb_scene_refit_mesh_device",
     "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
     "trb_scene_replace_objects", "trb_scene_replace_meshes", "trb_scene_replace_meshes_device",
     "trb_scene_replace_settings", "trb_scene_replace_materials", "trb_scene_replace_materials_device",
@@ -278,6 +278,8 @@ def load_trb():
     lib.trb_scene_update_frame.argtypes = [vp, u32, f32, f32]
     lib.trb_scene_update_mesh.argtypes = [vp, u32, vp, vp, vp]
     lib.trb_scene_update_mesh_device.argtypes = [vp, u32, vp, vp, vp, vp]
+    lib.trb_scene_refit_mesh.argtypes = [vp, u32, vp, vp, vp]
+    lib.trb_scene_refit_mesh_device.argtypes = [vp, u32, vp, vp, vp, vp]
     lib.trb_scene_update_keyframes.argtypes = [vp, u32, u32, vp]
     lib.trb_scene_update_keyframes_device.argtypes = [vp, u32, u32, vp, vp]
     lib.trb_scene_update_color_keys.argtypes = [vp, u32, u32, vp]

@@ -189,9 +189,8 @@ class Scene(_Base):
             raise ValueError("mesh index %d out of range (%d meshes)" % (mesh, self._desc.n_meshes))
         return self._desc.meshes[mesh].n_verts
 
-    def update_mesh(self, mesh, positions=None, normals=None, texcoords=None):
-        """trb_scene_update_mesh: replace mesh `mesh`'s positions (n_verts x 3), normals (n_verts x 3) and / or texcoords
-        (n_verts x 2); None keeps an array. New positions rebuild the mesh's BVH and refresh the current frame."""
+    def _mesh_arrays(self, mesh, positions, normals, texcoords):
+        """the three arrays as float32 pointers (None kept), each checked against the mesh's vertex count"""
         nv = self._mesh_verts(mesh)
         arrays = []
         for name, a, k in (("positions", positions, 3), ("normals", normals, 3), ("texcoords", texcoords, 2)):
@@ -200,7 +199,26 @@ class Scene(_Base):
                 if a.size != nv * k or (a.ndim != 1 and a.shape != (nv, k)):
                     raise ValueError("%s must have shape (%d, %d), got %s" % (name, nv, k, a.shape))
             arrays.append(a)
+        return arrays
+
+    def update_mesh(self, mesh, positions=None, normals=None, texcoords=None):
+        """trb_scene_update_mesh: replace mesh `mesh`'s positions (n_verts x 3), normals (n_verts x 3) and / or texcoords
+        (n_verts x 2); None keeps an array. New positions rebuild the mesh's BVH and refresh the current frame."""
+        arrays = self._mesh_arrays(mesh, positions, normals, texcoords)
         self._check(self._lib.trb_scene_update_mesh(self._h, mesh, *(None if a is None else F.ptr(a) for a in arrays)))
+
+    def refit_mesh(self, mesh, positions, normals=None, texcoords=None):
+        """trb_scene_refit_mesh: move mesh `mesh`'s vertices to `positions` (n_verts x 3) keeping its BVH's partition (the boxes are
+        recomputed bottom-up on the device) and refresh the current frame; normals (n_verts x 3) and texcoords (n_verts x 2) may be
+        replaced in the same call. Cheaper than update_mesh, but the tree's quality drops as the mesh deforms."""
+        arrays = self._mesh_arrays(mesh, positions, normals, texcoords)
+        self._check(self._lib.trb_scene_refit_mesh(self._h, mesh, *(None if a is None else F.ptr(a) for a in arrays)))
+
+    def refit_mesh_device(self, mesh, d_positions, d_normals=None, d_texcoords=None, stream=None):
+        """trb_scene_refit_mesh_device: the same from device pointers (ints) holding float32 arrays of the mesh's vertex count,
+        read on `stream` (a cudaStream_t as an int; None = default stream)."""
+        self._mesh_verts(mesh)
+        self._check(self._lib.trb_scene_refit_mesh_device(self._h, mesh, d_positions, d_normals, d_texcoords, stream))
 
     def update_mesh_device(self, mesh, d_positions=None, d_normals=None, d_texcoords=None, stream=None):
         """trb_scene_update_mesh_device: the same from device pointers (ints) holding float32 arrays of the mesh's vertex count,

@@ -62,6 +62,11 @@ struct HostMesh {
     uint32_t n_verts = 0;
     bool narrow = true;    // every leaf fits the narrow reference (pack_pairs)
     size_t pair_cap = 0;   // DPair records the mesh's record buffer holds
+    // trb_scene_refit_mesh: the boxes of `nodes` are stale once a refit rewrote the device records (refresh_host_tree reads them back
+    // when a host reader needs them). d_refit holds, per record, its parent link (k_refit_parents) and then its arrival counter; it
+    // follows the topology, so a rebuild or a removal of the mesh releases it.
+    bool stale = false;
+    uint32_t* d_refit = nullptr;
 };
 
 uint32_t pow2_ceil(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
@@ -1299,11 +1304,33 @@ trb_status pack_mesh_nodes(const HostMesh& hm, trb::DBvh& dh, bool wide) {
     return TRB_OK;
 }
 
+// The boxes of a refit mesh's host tree, read back from its device records (either leaf form: only the boxes are read). Record k
+// belongs to the k-th interior node in preorder and holds the boxes of its two children; the root box is hm.bounds.
+trb_status refresh_host_tree(HostMesh& hm, const trb::DMesh& dm) {
+    if (!hm.stale) return TRB_OK;
+    std::vector<trb::DPair> pn((hm.nodes.size() - 1) / 2); // a binary tree of n nodes has (n - 1) / 2 interior ones
+    if (!pn.empty()) CU(cudaMemcpy(pn.data(), dm.bvh.pairs, pn.size() * sizeof(trb::DPair), cudaMemcpyDeviceToHost));
+    auto set = [](trb_bvh_node& n, const float4& lo, const float4& hi) {
+        n.bmin[0] = lo.x; n.bmin[1] = lo.y; n.bmin[2] = lo.z; n.bmax[0] = hi.x; n.bmax[1] = hi.y; n.bmax[2] = hi.z;
+    };
+    set(hm.nodes[0], make_float4(hm.bounds.lo[0], hm.bounds.lo[1], hm.bounds.lo[2], 0.f), make_float4(hm.bounds.hi[0], hm.bounds.hi[1], hm.bounds.hi[2], 0.f));
+    size_t k = 0;
+    for (size_t i = 0; i < hm.nodes.size(); ++i) {
+        if (hm.nodes[i].b & TRB_BVH_LEAF) continue;
+        const trb::DPair& p = pn[k++];
+        set(hm.nodes[i + 1], p.l_lo, p.l_hi);
+        set(hm.nodes[hm.nodes[i].a], p.r_lo, p.r_hi);
+    }
+    hm.stale = false;
+    return TRB_OK;
+}
+
 // Packs every mesh's DPair records in one leaf form into the buffers allocated when the mesh was set up (setup_mesh), and uploads
 // the mesh headers. Kernels still in flight may read the records, so the device is drained first.
 trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
     CU(cudaDeviceSynchronize());
     for (size_t mi = 0; mi < s->meshes.size(); ++mi) {
+        { const trb_status r = refresh_host_tree(s->meshes[mi], s->dmeshes[mi]); if (r != TRB_OK) return r; }
         const trb_status r = pack_mesh_nodes(s->meshes[mi], s->dmeshes[mi].bvh, wide);
         if (r != TRB_OK) return r;
     }
@@ -1479,6 +1506,22 @@ trb_status setup_mesh(trb_scene* s, DeviceArena& arena, const trb_mesh& m, bool 
     return TRB_OK;
 }
 
+// n floats of a caller's array into a mesh buffer: from host memory, or from device memory read on `st` (complete on return)
+cudaError_t mesh_copy_in(const float* dst, const float* src, size_t n, bool device, cudaStream_t st) {
+    if (!device) return cudaMemcpy(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyHostToDevice);
+    const cudaError_t e = cudaMemcpyAsync(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
+    return e != cudaSuccess ? e : cudaStreamSynchronize(st);
+}
+// The attribute half of trb_scene_update_mesh and trb_scene_refit_mesh: normals and / or texcoords copied in place. The caller has
+// drained the device.
+trb_status copy_mesh_attributes(trb_scene* s, uint32_t mi, const float* nrm, const float* uv, bool device, cudaStream_t st) {
+    const trb::DMesh& dm = s->dmeshes[mi];
+    const size_t nv = s->meshes[mi].n_verts;
+    if (nrm) CU(mesh_copy_in(dm.normals, nrm, 3 * nv, device, st));
+    if (uv) CU(mesh_copy_in(dm.texcoords, uv, 2 * nv, device, st));
+    return TRB_OK;
+}
+
 // trb_scene_update_mesh(_device): `device` says the caller's arrays are device memory, read on `st`. New positions are copied
 // into a fresh buffer and the tree and triangle records are built into fresh buffers, so a failed build or allocation leaves the
 // scene as it was; the live buffers are replaced only after the build succeeded and the device was drained. The node records are
@@ -1494,11 +1537,7 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
     HostMesh& hm = s->meshes[mi];
     trb::DMesh& dm = s->dmeshes[mi];
     const size_t nv = hm.n_verts;
-    auto copy_in = [&](const float* dst, const float* src, size_t n) -> cudaError_t {
-        if (!device) return cudaMemcpy(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyHostToDevice);
-        const cudaError_t e = cudaMemcpyAsync(const_cast<float*>(dst), src, n * sizeof(float), cudaMemcpyDeviceToDevice, st);
-        return e != cudaSuccess ? e : cudaStreamSynchronize(st);
-    };
+    auto copy_in = [&](const float* dst, const float* src, size_t n) { return mesh_copy_in(dst, src, n, device, st); };
     struct PhaseEvents {
         cudaEvent_t e[6] = {};
         ~PhaseEvents() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
@@ -1572,8 +1611,9 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
         s->arena.release(dm.tris);
         if (pairs != dm.bvh.pairs) s->arena.release(dm.bvh.pairs);
         if (dm.bvh.quads) s->arena.release(dm.bvh.quads);
+        if (hm.d_refit) s->arena.release(hm.d_refit); // the refit's parent links follow the old topology
         hm.nodes = std::move(nm.nodes); hm.order = std::move(nm.order);
-        hm.narrow = narrow; hm.pair_cap = cap;
+        hm.narrow = narrow; hm.pair_cap = cap; hm.stale = false; hm.d_refit = nullptr;
         for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = hm.nodes[0].bmin[k]; hm.bounds.hi[k] = hm.nodes[0].bmax[k]; }
         const trb_bvh_node& root = hm.nodes[0];
         uint32_t root_ref = trb::REF_INTERIOR; // record 0
@@ -1592,13 +1632,57 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
             if (rw != TRB_OK) return rw;
         } else CU(cudaMemcpy(s->d_meshes + mi, &dm, sizeof dm, cudaMemcpyHostToDevice));
     } else CU(cudaDeviceSynchronize()); // kernels in flight may read the attributes overwritten below
-    if (nrm) CU(copy_in(dm.normals, nrm, 3 * nv));
-    if (uv) CU(copy_in(dm.texcoords, uv, 2 * nv));
+    { const trb_status r = copy_mesh_attributes(s, mi, nrm, uv, device, st); if (r != TRB_OK) return r; }
     if (pos && s->frame_set) { // instance bounds and the TLAS over the new mesh bounds
         const trb_status r = trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end);
         if (r != TRB_OK) return r;
     }
     report();
+    return TRB_OK;
+}
+
+// trb_scene_refit_mesh(_device): new positions through the mesh's kept tree (DESIGN.md §4 "Mesh refits"). Without positions it is
+// update_mesh's attribute copy. With them: the device is drained, the positions are copied in place, the triangle records rewritten
+// (k_refit_tris) and the node boxes recomputed bottom-up in the records (k_refit_nodes, after k_refit_parents on a mesh's first refit),
+// all on `st`; the root box (the header's 24 bytes) is the only read-back. The host tree is marked stale instead of being copied back.
+// Nothing here depends on the values of the positions, so the call fails only on a CUDA error.
+trb_status refit_mesh(trb_scene* s, uint32_t mi, const float* pos, const float* nrm, const float* uv, bool device, cudaStream_t st) {
+    if (!pos) return update_mesh(s, mi, nullptr, nrm, uv, device, st);
+    if (!s) return fail(TRB_INVALID_ARG, "null scene");
+    if (mi >= s->meshes.size()) return fail(TRB_INVALID_ARG, "mesh index out of range");
+    CU(cudaSetDevice(s->device));
+    HostMesh& hm = s->meshes[mi];
+    trb::DMesh& dm = s->dmeshes[mi];
+    const uint32_t n_rec = (uint32_t)((hm.nodes.size() - 1) / 2);
+    const auto grid = [](size_t k) { return (unsigned)std::max<size_t>(1, (k + 255) / 256); };
+    CU(cudaDeviceSynchronize()); // kernels in flight read the positions, triangle records, node records and header rewritten below
+    if (!hm.d_refit) {
+        uint32_t* links = nullptr;
+        CU(s->arena.alloc(2 * (size_t)n_rec, &links));
+        hm.d_refit = links;
+        trb::bvhb::k_refit_parents<<<grid(n_rec), 256, 0, st>>>(dm.bvh.pairs, n_rec, hm.d_refit);
+        ++g_launches;
+    }
+    CU(mesh_copy_in(dm.positions, pos, 3 * (size_t)hm.n_verts, device, st));
+    if (dm.bvh.quads) { s->arena.release(dm.bvh.quads); dm.bvh.quads = nullptr; } // DQuad records (trace.quads) are built at creation only
+    dm.bvh.root_hi.w = bits_f(QUAD_EMPTY_HOST);
+    s->quads_dropped = true;
+    trb::DMesh* d_dm = s->d_meshes + mi;
+    CU(cudaMemcpyAsync(d_dm, &dm, sizeof dm, cudaMemcpyHostToDevice, st));
+    if (n_rec) CU(cudaMemsetAsync(hm.d_refit + n_rec, 0, 4 * (size_t)n_rec, st));
+    trb::bvhb::k_refit_tris<<<grid(dm.n_tris), 256, 0, st>>>(dm.positions, dm.indices, dm.n_tris, const_cast<trb::DTri*>(dm.tris));
+    trb::bvhb::k_refit_nodes<<<grid(n_rec), 256, 0, st>>>(const_cast<trb::DPair*>(dm.bvh.pairs), n_rec, hm.d_refit, hm.d_refit + n_rec,
+                                                          s->wide_leaf, dm.tris, dm.indices, dm.positions, &d_dm->bvh);
+    g_launches += 2;
+    CU(cudaGetLastError());
+    trb::DBvh hdr{};
+    CU(cudaMemcpyAsync(&hdr, &d_dm->bvh, sizeof hdr, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    dm.bvh.root_lo = hdr.root_lo; dm.bvh.root_hi = hdr.root_hi;
+    for (int k = 0; k < 3; ++k) { hm.bounds.lo[k] = (&hdr.root_lo.x)[k]; hm.bounds.hi[k] = (&hdr.root_hi.x)[k]; }
+    hm.stale = true;
+    { const trb_status r = copy_mesh_attributes(s, mi, nrm, uv, device, st); if (r != TRB_OK) return r; }
+    if (s->frame_set) return trb_scene_update_frame(s, s->last_frame, s->last_start, s->last_end); // instance bounds and the TLAS
     return TRB_OK;
 }
 
@@ -1867,7 +1951,7 @@ trb_status replace_meshes(trb_scene* s, const trb_scene_meshes& sec, const trb_s
         if (named[k]) continue;
         const trb::DMesh& dm = s->dmeshes[k];
         for (const void* p : {(const void*)dm.positions, (const void*)dm.normals, (const void*)dm.texcoords, (const void*)dm.indices,
-                              (const void*)dm.tris, (const void*)dm.bvh.pairs, (const void*)dm.bvh.quads})
+                              (const void*)dm.tris, (const void*)dm.bvh.pairs, (const void*)dm.bvh.quads, (const void*)s->meshes[k].d_refit})
             if (p) s->arena.release(p);
     }
     s->arena.release(s->d_meshes);
@@ -2090,6 +2174,13 @@ trb_status trb_scene_update_mesh(trb_scene* s, uint32_t mesh, const float* posit
 trb_status trb_scene_update_mesh_device(trb_scene* s, uint32_t mesh, const float* d_positions, const float* d_normals, const float* d_texcoords,
                                         void* cuda_stream) {
     return update_mesh(s, mesh, d_positions, d_normals, d_texcoords, true, static_cast<cudaStream_t>(cuda_stream));
+}
+trb_status trb_scene_refit_mesh(trb_scene* s, uint32_t mesh, const float* positions, const float* normals, const float* texcoords) {
+    return refit_mesh(s, mesh, positions, normals, texcoords, false, nullptr);
+}
+trb_status trb_scene_refit_mesh_device(trb_scene* s, uint32_t mesh, const float* d_positions, const float* d_normals, const float* d_texcoords,
+                                       void* cuda_stream) {
+    return refit_mesh(s, mesh, d_positions, d_normals, d_texcoords, true, static_cast<cudaStream_t>(cuda_stream));
 }
 
 trb_status trb_scene_replace_objects(trb_scene* s, const trb_scene_objects* objects) {
@@ -3002,7 +3093,16 @@ trb_status trb_scene_get_bvh(const trb_scene* s, int which, uint32_t* n_nodes, t
             nn = &dev_nodes; oo = &dev_order;
         } else { nn = &s->tlas_nodes; oo = &s->tlas_order; }
     }
-    else { if ((size_t)which >= s->meshes.size()) return fail(TRB_INVALID_ARG, "mesh index out of range"); nn = &s->meshes[which].nodes; oo = &s->meshes[which].order; }
+    else {
+        if ((size_t)which >= s->meshes.size()) return fail(TRB_INVALID_ARG, "mesh index out of range");
+        if (s->meshes[which].stale) { // a refit left the boxes on the device: refreshing the host copy does not change the scene
+            trb_scene* ms = const_cast<trb_scene*>(s);
+            CU(cudaSetDevice(s->device));
+            const trb_status r = refresh_host_tree(ms->meshes[which], ms->dmeshes[which]);
+            if (r != TRB_OK) return r;
+        }
+        nn = &s->meshes[which].nodes; oo = &s->meshes[which].order;
+    }
     *n_nodes = (uint32_t)nn->size(); *n_ordered = (uint32_t)oo->size();
     if (nodes) std::memcpy(nodes, nn->data(), nn->size() * sizeof(trb_bvh_node));
     if (ordered) std::memcpy(ordered, oo->data(), oo->size() * sizeof(uint32_t));

@@ -538,6 +538,105 @@ __global__ void k_pair_pack(const trb_bvh_node* __restrict__ nodes, uint32_t n, 
     out[rec[i]] = p;
 }
 
+// ---- mesh helpers of trb_scene_refit_mesh: new positions through the kept tree (DESIGN.md §4 "Mesh refits")
+// The leaf-ordered triangle records from new positions with k_tri_pack's arithmetic. Each slot keeps its triangle index and its
+// leaf-end mark, so the tree's ordered_geom is never needed on the device.
+__global__ void k_refit_tris(const float* __restrict__ pos, const uint32_t* __restrict__ tri, uint32_t n_tris, DTri* tris) {
+    const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
+    if (slot >= n_tris) return;
+    const uint32_t t = __float_as_uint(tris[slot].v0.w);
+    const float mark = tris[slot].e0.w;
+    const float* pa = pos + 3 * (size_t)tri[3 * (size_t)t];
+    const float* pb = pos + 3 * (size_t)tri[3 * (size_t)t + 1];
+    const float* pc = pos + 3 * (size_t)tri[3 * (size_t)t + 2];
+    DTri r;
+    r.v0 = make_float4(pa[0], pa[1], pa[2], __uint_as_float(t));
+    r.e0 = make_float4(pb[0] - pa[0], pb[1] - pa[1], pb[2] - pa[2], mark);
+    r.e1 = make_float4(pc[0] - pa[0], pc[1] - pa[1], pc[2] - pa[2], 0.f);
+    r.pad = make_float4(0.f, 0.f, 0.f, 0.f);
+    tris[slot] = r;
+}
+// The parent of every record as (parent record << 1 | side), side 0 for the first child (l), 1 for the second (r); the root record 0
+// has none. Records number the interior nodes in preorder (pack_pairs), so n_rec < 2^30 and the link fits 31 bits.
+__global__ void k_refit_parents(const DPair* __restrict__ pairs, uint32_t n_rec, uint32_t* __restrict__ parent) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_rec) return;
+    if (r == 0) parent[0] = NONE;
+    const uint32_t lref = __float_as_uint(pairs[r].l_lo.w), rref = __float_as_uint(pairs[r].l_hi.w);
+    if ((lref & REF_TAG) == REF_INTERIOR) parent[lref & ~REF_TAG] = r << 1;
+    if ((rref & REF_TAG) == REF_INTERIOR) parent[rref & ~REF_TAG] = r << 1 | 1u;
+}
+// The fold of bvh.rs:143 over one leaf: BBox::new() grown with Triangle::bounds (mesh.rs:128-134) of each of its triangles, in slot
+// order, from the mesh's positions. A narrow reference carries the count, a wide one runs to the slot marked TRI_LEAF_END.
+__device__ __forceinline__ trbh::Box3 refit_leaf_box(uint32_t ref, bool wide, const DTri* __restrict__ tris, const uint32_t* __restrict__ tri,
+                                                     const float* __restrict__ pos) {
+    trbh::Box3 b;
+    for (int c = 0; c < 3; ++c) { b.lo[c] = INFINITY; b.hi[c] = -INFINITY; }
+    const uint32_t first = wide ? (ref & ~REF_TAG) : (ref & ((1u << 25) - 1u)), cnt = wide ? NONE : (ref >> 25) & 31u;
+    for (uint32_t j = 0; j < cnt; ++j) {
+        const uint32_t slot = first + j, t = __float_as_uint(tris[slot].v0.w);
+        trbh::Box3 tb;
+        for (int v = 0; v < 3; ++v) {
+            const float* p = pos + 3 * (size_t)tri[3 * (size_t)t + v];
+            for (int c = 0; c < 3; ++c) {
+                if (v == 0) tb.lo[c] = tb.hi[c] = p[c];
+                else { tb.lo[c] = hmin(tb.lo[c], p[c]); tb.hi[c] = hmax(tb.hi[c], p[c]); }
+            }
+        }
+        hgrow(b, tb);
+        if (wide && __float_as_uint(tris[slot].e0.w) == TRI_LEAF_END) break;
+    }
+    return b;
+}
+__device__ __forceinline__ void refit_store(DPair* pairs, uint32_t rec, uint32_t side, const trbh::Box3& b) {
+    float* f = reinterpret_cast<float*>(pairs + rec) + 8 * side; // side 0: l_lo / l_hi, side 1: r_lo / r_hi; the w words stay
+    for (int c = 0; c < 3; ++c) { f[c] = b.lo[c]; f[4 + c] = b.hi[c]; }
+}
+// Node boxes, bottom-up, in place in the DPair records (Karras 2012). The thread of record r writes the boxes of r's leaf children and
+// then arrives at r once per box written; the box of an interior child is written into r by the thread that completed that child,
+// which then arrives at r once. The arrival that brings r's counter to 2 owns r: it unions r's two boxes (first child first) into the
+// box of r's node, writes it into the parent's slot, and arrives there. Every box is therefore written once, by one thread, from
+// operands that are final when it reads them, and the result does not depend on the schedule.
+// Ordering: each box is stored, then __threadfence() (release), then the arrival's atomicAdd. The owning arrival issues
+// __threadfence() (acquire) before it reads the record, and reads it with ld.global.cg (from L2, never a stale L1 line).
+// The root record's box goes into the mesh header (root_lo / root_hi xyz; the w words stay). A tree that is one leaf has no record:
+// thread 0 folds that leaf into the header. `count` holds n_rec zeros.
+__global__ void k_refit_nodes(DPair* pairs, uint32_t n_rec, const uint32_t* __restrict__ parent, uint32_t* count, bool wide,
+                              const DTri* __restrict__ tris, const uint32_t* __restrict__ tri, const float* __restrict__ pos, DBvh* hdr) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    auto store_root = [&](const trbh::Box3& b) {
+        float* lo = reinterpret_cast<float*>(&hdr->root_lo);
+        float* hi = reinterpret_cast<float*>(&hdr->root_hi);
+        for (int c = 0; c < 3; ++c) { lo[c] = b.lo[c]; hi[c] = b.hi[c]; }
+    };
+    if (n_rec == 0) {
+        if (r == 0) store_root(refit_leaf_box(__float_as_uint(hdr->root_lo.w), wide, tris, tri, pos));
+        return;
+    }
+    if (r >= n_rec) return;
+    const uint32_t lref = __float_as_uint(pairs[r].l_lo.w), rref = __float_as_uint(pairs[r].l_hi.w);
+    uint32_t arrivals = 0;
+    if ((lref & REF_TAG) == REF_LEAF) { refit_store(pairs, r, 0, refit_leaf_box(lref, wide, tris, tri, pos)); ++arrivals; }
+    if ((rref & REF_TAG) == REF_LEAF) { refit_store(pairs, r, 1, refit_leaf_box(rref, wide, tris, tri, pos)); ++arrivals; }
+    if (arrivals == 0) return;
+    __threadfence();
+    uint32_t node = r;
+    if (atomicAdd(&count[node], arrivals) + arrivals != 2u) return;
+    for (;;) {
+        __threadfence();
+        const float4 llo = __ldcg(&pairs[node].l_lo), lhi = __ldcg(&pairs[node].l_hi), rlo = __ldcg(&pairs[node].r_lo), rhi = __ldcg(&pairs[node].r_hi);
+        trbh::Box3 b;
+        b.lo[0] = hmin(llo.x, rlo.x); b.lo[1] = hmin(llo.y, rlo.y); b.lo[2] = hmin(llo.z, rlo.z);
+        b.hi[0] = hmax(lhi.x, rhi.x); b.hi[1] = hmax(lhi.y, rhi.y); b.hi[2] = hmax(lhi.z, rhi.z);
+        if (node == 0) { store_root(b); return; }
+        const uint32_t p = parent[node];
+        refit_store(pairs, p >> 1, p & 1u, b);
+        __threadfence();
+        node = p >> 1;
+        if (atomicAdd(&count[node], 1u) != 1u) return;
+    }
+}
+
 // ---- instance-tree helpers of trb_scene_update_frame (the level builder's counterpart of k_tlas_build's head and tail)
 // *bad = 1 where some bound fails trbh::bvh_bound_buildable
 __global__ void k_bounds_check(const float* __restrict__ bounds, size_t n_floats, uint32_t* bad) {
