@@ -752,6 +752,53 @@ trb_status trb_camera_rays(trb_scene* scene, const trb_render_cfg* cfg, size_t n
 trb_status trb_render_samples(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_sample* samples,
                               trb_stats* stats);
 
+/* -- AOVs: denoiser guide images and per-pixel depth / object id from the render's own primary hits (DESIGN.md §4 "AOVs") --------
+ * For every camera sample of a render, one record from the sample's primary hit (the trb_camera_rays ray, traced by Scene::intersect):
+ *   depth   the hit's t, as trb_intersect_records gives it for that ray; +inf on a miss
+ *   inst    the instance hit, or TRB_MISS
+ *   n       the unit world-space shading normal of the BSDF frame (bsdf.rs:38-44, what NormalsDebug shows as (n + 1) / 2); not flipped
+ *           toward the camera; 0 on a miss
+ *   albedo  Material::bsdf's lobes at the hit, textured: the sum, in lobe order, of each lobe's colour times its Fresnel factor at
+ *           normal incidence (diffuse lobes 1, reflection F(1), transmission 1 - F(1)); MERL: pi * BSDF::eval(n, n, all lobes). Each
+ *           channel clamped to [0, 1]. Emission is not part of it. 0 on a miss.
+ * 32 bytes. */
+typedef struct trb_aov_sample {
+    float albedo[3];
+    float depth;
+    float n[3];
+    uint32_t inst;
+} trb_aov_sample;
+
+/* AOV outputs of a film render; any may be NULL (not rendered).
+ *   albedo_w, normal_w  RGBW films (width*height*4 floats, the colour film's layout). Each sample adds w * value and w with the colour
+ *                       film's weights (RenderTarget::write: filter table, filter_pixel_width window, 2x2 lock blocks); a miss adds w
+ *                       with a zero value, so their W equals the colour film's W up to float addition order. Added into.
+ *   nearest             width*height uint64: each sample does atomicMin(pixel, float_bits(depth) << 32 | inst) on the pixel it was
+ *                       taken for. Initialise it to all ones; a pixel whose samples all missed holds 0x7f800000ffffffff. The result
+ *                       does not depend on the order of samples, passes or calls. */
+typedef struct trb_aov_film {
+    float* albedo_w;
+    float* normal_w;
+    uint64_t* nearest;
+} trb_aov_film;
+
+/* trb_render that also renders the AOVs into the HOST buffers of `aov` (same sizes as above; nearest is read and written). The colour
+ * film, samples and every trb_stats counter equal trb_render's with the same cfg. Path integrator on the wavefront only: Whitted,
+ * NormalsDebug and TRB_RENDER_MEGAKERNEL give TRB_UNSUPPORTED. The first AOV render allocates 32 B of AOV record per path in flight
+ * (TRB_OOM if that does not fit); plain renders never do. Blocking. */
+trb_status trb_render_aov(trb_scene* scene, const trb_render_cfg* cfg, float* film_rgbw, const trb_aov_film* aov, trb_stats* stats);
+
+/* trb_render_aov with the contract of trb_render_device: the film and the outputs of `d_aov` (a host struct of DEVICE pointers) are
+ * device buffers on the scene's GPU, enqueued on cuda_stream without host synchronisation. TRB_INVALID_ARG for a film or an AOV
+ * film that is not 16-byte aligned, or a nearest buffer that is not 8-byte aligned. */
+trb_status trb_render_aov_device(trb_scene* scene, const trb_render_cfg* cfg, float* d_film_rgbw, const trb_aov_film* d_aov,
+                                 trb_stats* d_stats, void* cuda_stream);
+
+/* trb_render_samples that also writes each camera sample's AOV record into the HOST buffer aov[n], in the same order. samples[] and
+ * the stats equal trb_render_samples'. The statuses of trb_render_samples and trb_render_aov. */
+trb_status trb_render_samples_aov(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov,
+                                  trb_stats* stats);
+
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
  * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */

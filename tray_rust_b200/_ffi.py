@@ -199,6 +199,11 @@ class Sample(C.Structure):
     _fields_ = [("x", f32), ("y", f32), ("r", f32), ("g", f32), ("b", f32)]
 
 
+class AovFilm(C.Structure):
+    """trb_aov_film: the AOV outputs of a film render (any may be NULL)"""
+    _fields_ = [("albedo_w", C.c_void_p), ("normal_w", C.c_void_p), ("nearest", C.c_void_p)]
+
+
 class BvhNode(C.Structure):
     _fields_ = [("bmin", f32 * 3), ("bmax", f32 * 3), ("a", u32), ("b", u32)]
 
@@ -225,6 +230,7 @@ LIGHT_PDF_QUERY_DTYPE = np.dtype([("p", "<f4", 3), ("time", "<f4"), ("wi", "<f4"
 EMIT_QUERY_DTYPE = np.dtype([("w", "<f4", 3), ("time", "<f4"), ("n", "<f4", 3), ("inst", "<u4")])
 KEYFRAME_DTYPE = np.dtype([("translation", "<f4", 3), ("rotation", "<f4", 4), ("scaling", "<f4", 3)])
 COLOR_KEY_DTYPE = np.dtype([("rgba", "<f4", 4), ("time", "<f4")])
+AOV_SAMPLE_DTYPE = np.dtype([("albedo", "<f4", 3), ("depth", "<f4"), ("n", "<f4", 3), ("inst", "<u4")])  # trb_aov_sample, 32 B
 MATERIAL_DTYPE = np.dtype([("type", "<u4"), ("c0", "<f4", 3), ("c1", "<f4", 3), ("roughness", "<f4"), ("eta", "<f4"), ("merl", "<u4"),
                            ("tex", "<u4", 4)])
 
@@ -248,6 +254,7 @@ TRB_SYMBOLS = [
     "trb_scene_update_keyframes", "trb_scene_update_keyframes_device", "trb_scene_update_color_keys", "trb_scene_update_materials",
     "trb_scene_replace_objects", "trb_scene_replace_meshes", "trb_scene_replace_meshes_device",
     "trb_scene_replace_settings", "trb_scene_replace_materials", "trb_scene_replace_materials_device",
+    "trb_render_aov", "trb_render_aov_device", "trb_render_samples_aov",
 ]
 
 _trb = None
@@ -316,6 +323,9 @@ def load_trb():
     lib.trb_film_write.argtypes = [vp, sz, vp, vp, vp]
     lib.trb_film_write_device.argtypes = [vp, sz, vp, vp, vp, vp]
     lib.trb_render_samples.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, C.POINTER(Stats)]
+    lib.trb_render_aov.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), C.POINTER(Stats)]
+    lib.trb_render_aov_device.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp]
+    lib.trb_render_samples_aov.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

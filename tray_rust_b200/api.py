@@ -75,6 +75,12 @@ def build_bvh_device(d_boxes, n, max_geom, d_n_nodes, d_nodes, d_ordered, device
         raise TrbError(rc, (lib.trb_last_error() or b"").decode())
 
 
+def decode_nearest(nearest):
+    """The (depth float32, inst uint32) of a ``nearest`` AOV buffer: its high and low 32 bits (trb_aov_film)."""
+    nearest = np.ascontiguousarray(nearest, dtype=np.uint64)
+    return (nearest >> np.uint64(32)).astype(np.uint32).view(np.float32), (nearest & np.uint64(0xffffffff)).astype(np.uint32)
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
 
@@ -183,6 +189,49 @@ class Scene(_Base):
     def render_device(self, d_film_ptr, d_stats_ptr=None, stream=None, **kw):
         cfg = _cfg(**kw)
         self._check(self._lib.trb_render_device(self._h, C.byref(cfg), d_film_ptr, d_stats_ptr, stream))
+
+    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, **kw):
+        """trb_render_aov: the colour film and the AOVs of the same render (DESIGN.md §4 "AOVs"), all accumulated into.
+        albedo / normal: True (allocate, zero), False / None (not rendered) or a float32 (height, width, 4) film; nearest: True
+        (allocate, all ones), False / None or a uint64 (height, width) array. Returns (film, aovs, Stats) where aovs maps "albedo_w",
+        "normal_w" and "nearest" to the arrays rendered."""
+        cfg = _cfg(**kw)
+        if film is None:
+            film = np.zeros((self.height, self.width, 4), np.float32)
+        aovs = {}
+        for name, a, shape, dtype, fill in (("albedo_w", albedo, (self.height, self.width, 4), np.float32, 0),
+                                            ("normal_w", normal, (self.height, self.width, 4), np.float32, 0),
+                                            ("nearest", nearest, (self.height, self.width), np.uint64, np.iinfo(np.uint64).max)):
+            if a is True:
+                a = np.full(shape, fill, dtype)
+            if a is None or a is False:
+                continue
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+            aovs[name] = a
+        if not isinstance(film, np.ndarray) or film.dtype != np.float32 or film.shape != (self.height, self.width, 4) or not film.flags.c_contiguous:
+            raise ValueError("film must be a C-contiguous float32 array of shape %s" % ((self.height, self.width, 4),))
+        out = F.AovFilm(*(aovs[k].ctypes.data if k in aovs else None for k in ("albedo_w", "normal_w", "nearest")))
+        st = F.Stats()
+        self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
+        return film, aovs, st
+
+    def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, **kw):
+        """trb_render_aov_device: device films of height*width*4 float32 (16-byte aligned) and a device nearest buffer of height*width
+        uint64 (8-byte aligned; initialise it to all ones), pointers as ints, any AOV None. Enqueued on `stream` (a cudaStream_t as an
+        int; None = default stream) without host synchronisation. Never updates the frame."""
+        cfg = _cfg(**kw)
+        out = F.AovFilm(d_albedo, d_normal, d_nearest)
+        self._check(self._lib.trb_render_aov_device(self._h, C.byref(cfg), d_film, C.byref(out), d_stats, stream))
+
+    def render_samples_aov(self, **kw):
+        """trb_render_samples_aov: (samples as render_samples, AOV records as AOV_SAMPLE_DTYPE in the same order, Stats)."""
+        cfg = _cfg(**kw)
+        n = self._n_samples(cfg)
+        out, aov = np.zeros(n, F.SAMPLE_DTYPE), np.zeros(n, F.AOV_SAMPLE_DTYPE)
+        st = F.Stats()
+        self._check(self._lib.trb_render_samples_aov(self._h, C.byref(cfg), n, F.ptr(out), F.ptr(aov), C.byref(st)))
+        return out, aov, st
 
     def _mesh_verts(self, mesh):
         if not 0 <= mesh < self._desc.n_meshes:

@@ -322,9 +322,13 @@ struct trb_scene {
     // caller film writes (trb_film_write): sort keys and sample order (double-buffered), region starts, CUB's temporary storage
     void* d_film_scratch = nullptr;
     size_t film_scratch_bytes = 0;
+    // AOV records of a film render's pass (trb_render_aov*), allocated by the first AOV render at the path-state capacity: per path
+    // (albedo, depth) in d_aov[p] and (n, inst bits) in d_aov[aov_capacity + p], 32 bytes
+    float4* d_aov = nullptr;
+    size_t aov_capacity = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
-                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch}) if (p) cudaFree(p);
+                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -531,6 +535,26 @@ trb_status launch_render_t(trb_scene* s, const trb::RenderParams& rp, uint32_t f
     CU(cudaGetLastError());
     return TRB_OK;
 }
+// The AOVs a render asks for (DESIGN.md §4 "AOVs"): samples = the caller's device records (per-sample mode), else the film outputs
+// (any may be nullptr)
+struct AovRequest { trb_aov_sample* samples; float4* albedo_w; float4* normal_w; unsigned long long* nearest; };
+
+// the path-indexed AOV records of film passes, at the path-state capacity
+trb_status ensure_aov(trb_scene* s) {
+    if (s->aov_capacity >= s->wf_capacity) return TRB_OK;
+    CU(cudaDeviceSynchronize()); // a pass still in flight owns the old buffer
+    if (s->d_aov) cudaFree(s->d_aov);
+    s->d_aov = nullptr; s->aov_capacity = 0;
+    const cudaError_t err = cudaMalloc(reinterpret_cast<void**>(&s->d_aov), s->wf_capacity * 2 * sizeof(float4));
+    if (err != cudaSuccess) {
+        s->d_aov = nullptr;
+        cudaGetLastError();
+        return fail(err == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(err));
+    }
+    s->aov_capacity = s->wf_capacity;
+    return TRB_OK;
+}
+
 trb_status ensure_wavefront(trb_scene* s, size_t n_paths) {
     if (n_paths <= s->wf_capacity) return TRB_OK;
     CU(cudaDeviceSynchronize()); // a pass still in flight owns the old buffers
@@ -659,7 +683,8 @@ void launch_shade(trb_scene* s, const trb::RenderParams& rp, const trb::WfState&
 // The bounce rounds of a wavefront pass whose round-0 paths are in place (k_wf_generate or k_illum_load, then the transform
 // table): per round the optional ray sort, the trace, the shade kernels (DESIGN.md "Execution shape"). mode as launch_shade; the
 // illumination queries' round 0 traces each ray's own [min_t, max_t] (launch_query_trace).
-trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb::WfState& wf, uint32_t flags, int mode, cudaStream_t st) {
+trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb::WfState& wf, uint32_t flags, int mode, cudaStream_t st,
+                            const AovRequest* aov = nullptr) {
     const Tuning& tu = s->tune;
     const bool stats = (flags & TRB_RENDER_STATS) != 0, anim = s->ds.has_anim != 0;
     const uint32_t rounds = s->integrator.max_depth + 2; // bounces 0..max_depth, plus the round that only resolves
@@ -723,6 +748,15 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
         }
 #undef TRB_TRACE_LAUNCH
         if (ev.first) { CU(cudaEventRecord(ev.second, st)); s->trace_events.push_back(ev); }
+        if (aov && round == 0) { // the primary hits, before the round-0 shade overwrites them
+            const unsigned agrid = (unsigned)std::min<size_t>((wf.n_paths + 127) / 128, (size_t)s->sm_count * 16);
+            float4* lo = mode == 1 ? reinterpret_cast<float4*>(aov->samples) : s->d_aov;
+            float4* hi = mode == 1 ? lo + 1 : s->d_aov + s->aov_capacity;
+            const uint32_t step = mode == 1 ? 2u : 1u;
+            if (anim) trb::k_wf_aov<true><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
+            else trb::k_wf_aov<false><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
+            g_launches++;
+        }
         if (mode == 0) launch_shade<0>(s, rp, wf, round, st);
         else if (mode == 1) launch_shade<1>(s, rp, wf, round, st);
         else launch_shade<2>(s, rp, wf, round, st);
@@ -733,7 +767,7 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
 
 // One wavefront pass over rp's blocks x samples: generate, then (trace, shade) per bounce round, then the film
 // (DESIGN.md "Execution shape"). n_paths = blocks * 64 * sample_count must fit the allocated path state.
-trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st) {
+trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st, const AovRequest* aov = nullptr) {
     const size_t n_paths = (size_t)rp.n_blocks * 64 * rp.sample_count;
     if (n_paths > s->wf_capacity || n_paths >= (1ull << 30)) return fail(TRB_INVALID_ARG, "pass larger than the wavefront state");
     const Tuning& tu = s->tune;
@@ -765,7 +799,7 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     else trb::k_wf_generate<false><<<gen_grid, 256, 0, st>>>(s->ds, rp, wf);
     g_launches++;
     launch_anim_table(s, wf, n_paths, rp.ad_state != nullptr, st);
-    const trb_status r = wavefront_rounds(s, rp, wf, flags, mode, st);
+    const trb_status r = wavefront_rounds(s, rp, wf, flags, mode, st, aov);
     if (r != TRB_OK) return r;
     if (mode == 0 && rp.film) { // (an Adaptive parity dump has no film: its records are written by k_ad_decide)
         const int T = 9 + 2 * std::max(s->ds.fpw_x, s->ds.fpw_y);
@@ -776,6 +810,23 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
         } else if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, rp, wf);
         else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, rp, wf);
         g_launches++;
+        if (aov) { // the colour film's kernel over each half of the AOV records in place of the radiance: the same weights and order
+            trb::RenderParams ra = rp;
+            trb::WfState wa = wf;
+            const std::pair<float4*, float4*> films[2] = {{aov->albedo_w, s->d_aov}, {aov->normal_w, s->d_aov + s->aov_capacity}};
+            for (const auto& f : films) {
+                if (!f.first) continue;
+                ra.film = f.first; wa.rad = f.second;
+                if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                g_launches++;
+            }
+            if (aov->nearest) {
+                const unsigned ngrid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
+                trb::k_wf_nearest<<<ngrid, 256, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, (uint32_t)n_paths, aov->nearest);
+                g_launches++;
+            }
+        }
     }
     CU(cudaGetLastError());
     return TRB_OK;
@@ -786,7 +837,7 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
 // samples (fewer if device memory is short): all selected blocks x a sample sub-range, or — for images with more than
 // pass_paths / 64 blocks — a block sub-range x one sample. A camera sample's radiance is a pure function of
 // (scene, seed, pixel, sample index), so the split changes nothing but the order of the film's float additions.
-trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int mode, cudaStream_t st) {
+trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int mode, cudaStream_t st, const AovRequest* aov = nullptr) {
     const uint32_t nb = rp.n_blocks, first = rp.sample_first, count = rp.sample_count;
     const uint2* blocks = rp.blocks;
     const uint64_t total = (uint64_t)nb * 64 * count;
@@ -801,6 +852,10 @@ trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int
         while ((r = ensure_wavefront(s, (size_t)want)) == TRB_OOM && want > (1u << 16) && mode == 0) want = ((want / 2 + 63) / 64) * 64;
         if (r != TRB_OK) return r;
     }
+    if (aov && mode == 0) {
+        const trb_status r = ensure_aov(s);
+        if (r != TRB_OK) return r;
+    }
     const uint64_t cap = std::max<uint64_t>(want, 64);  // paths per pass actually used (a larger state left by an earlier call is not required)
     uint32_t bp, sp;
     if ((uint64_t)nb * 64 <= cap) { bp = nb; sp = (uint32_t)std::min<uint64_t>(count, cap / ((uint64_t)nb * 64)); }
@@ -809,7 +864,7 @@ trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int
         for (uint32_t s0 = 0; s0 < count; s0 += sp) {
             rp.blocks = blocks + b0; rp.n_blocks = std::min(bp, nb - b0);
             rp.sample_first = first + s0; rp.sample_count = std::min(sp, count - s0);
-            trb_status r = launch_wavefront(s, rp, flags, mode, st);
+            trb_status r = launch_wavefront(s, rp, flags, mode, st, aov);
             if (r != TRB_OK) return r;
         }
     return TRB_OK;
@@ -916,8 +971,8 @@ trb_status adaptive_pixel_spp_out(trb_scene* s, const uint2* d_blocks, uint32_t 
     return TRB_OK;
 }
 
-trb_status launch_render(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st) {
-    if (!(flags & TRB_RENDER_MEGAKERNEL) || s->integrator.type != TRB_INTEGRATOR_PATH) return render_passes(s, rp, flags, mode, st);
+trb_status launch_render(trb_scene* s, const trb::RenderParams& rp, uint32_t flags, int mode, cudaStream_t st, const AovRequest* aov = nullptr) {
+    if (!(flags & TRB_RENDER_MEGAKERNEL) || s->integrator.type != TRB_INTEGRATOR_PATH) return render_passes(s, rp, flags, mode, st, aov);
     const bool stats = (flags & TRB_RENDER_STATS) != 0;
     CU(cudaMemsetAsync(rp.work_counter, 0, sizeof(uint32_t), st));
     if (s->ds.has_anim) {
@@ -2574,8 +2629,9 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
     return TRB_OK;
 }
 
-trb_status trb_render_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, trb_stats* d_stats, void* stream) {
-    if (!s || !cfg || !d_film) return fail(TRB_INVALID_ARG, "null argument");
+namespace {
+// trb_render_device's body; aov: the AOV outputs of trb_render_aov_device (nullptr: none)
+trb_status render_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, trb_stats* d_stats, cudaStream_t st, const AovRequest* aov) {
     if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
     CU(cudaSetDevice(s->device));
     uint32_t spp, first, count, nb;
@@ -2589,11 +2645,34 @@ trb_status trb_render_device(trb_scene* s, const trb_render_cfg* cfg, float* d_f
     rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
     rp.work_counter = s->d_counter; rp.film = reinterpret_cast<float4*>(d_film); rp.stats = reinterpret_cast<trb::DStats*>(d_stats);
     rp.error_flag = s->d_error;
-    return launch_render(s, rp, cfg->flags, 0, static_cast<cudaStream_t>(stream));
+    return launch_render(s, rp, cfg->flags, 0, st, aov);
 }
 
-trb_status trb_render(trb_scene* s, const trb_render_cfg* cfg, float* film, trb_stats* stats) {
-    if (!s || !cfg || !film) return fail(TRB_INVALID_ARG, "null argument");
+// The AOV renders run the path integrator's wavefront only (DESIGN.md §4 "AOVs")
+trb_status aov_supported(const trb_scene* s, const trb_render_cfg* cfg) {
+    if (s->integrator.type != TRB_INTEGRATOR_PATH) return fail(TRB_UNSUPPORTED, "AOVs are rendered by the path integrator only");
+    if (cfg->flags & TRB_RENDER_MEGAKERNEL) return fail(TRB_UNSUPPORTED, "AOVs are rendered on the wavefront pipeline only, not with TRB_RENDER_MEGAKERNEL");
+    return TRB_OK;
+}
+
+// a device buffer freed with the scope
+struct DeviceBuffer {
+    void* p = nullptr;
+    ~DeviceBuffer() { if (p) cudaFree(p); }
+};
+
+// additive, like film::Image::add_pixels (image.rs:21-33); a 33 MB read-modify-write: split over a few host threads
+void add_film(float* film, const float* src, size_t n) {
+    const unsigned nt = n >= (1u << 20) ? std::min(8u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
+    auto add = [film, src](size_t a, size_t b) { for (size_t i = a; i < b; ++i) film[i] += src[i]; };
+    std::vector<std::thread> th;
+    for (unsigned k = 1; k < nt; ++k) th.emplace_back(add, n * k / nt, n * (k + 1) / nt);
+    add(0, n / nt);
+    for (auto& t : th) t.join();
+}
+
+// trb_render's body; aov: the host AOV outputs of trb_render_aov (nullptr: none)
+trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats) {
     CU(cudaSetDevice(s->device));
     float update_ms = 0.f;
     if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) { // Exec::render: scene.update_frame first (multithreaded.rs:57-60)
@@ -2606,23 +2685,33 @@ trb_status trb_render(trb_scene* s, const trb_render_cfg* cfg, float* film, trb_
     const size_t npx = (size_t)s->film.width * s->film.height;
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
+    DeviceBuffer d_albedo, d_normal, d_nearest; // the AOV outputs on the device: films from zero (added into the caller's), nearest from the caller's
+    AovRequest req{nullptr, nullptr, nullptr, nullptr};
+    if (aov) {
+        if (aov->albedo_w) { CU(cudaMalloc(&d_albedo.p, npx * sizeof(float4))); CU(cudaMemsetAsync(d_albedo.p, 0, npx * sizeof(float4), 0)); }
+        if (aov->normal_w) { CU(cudaMalloc(&d_normal.p, npx * sizeof(float4))); CU(cudaMemsetAsync(d_normal.p, 0, npx * sizeof(float4), 0)); }
+        if (aov->nearest) { CU(cudaMalloc(&d_nearest.p, npx * sizeof(uint64_t))); CU(cudaMemcpy(d_nearest.p, aov->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice)); }
+        req = {nullptr, static_cast<float4*>(d_albedo.p), static_cast<float4*>(d_normal.p), static_cast<unsigned long long*>(d_nearest.p)};
+    }
+    const bool with_aov = aov && (aov->albedo_w || aov->normal_w || aov->nearest);
     CU(cudaEventRecord(s->ev0, 0));
-    trb_status r = trb_render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), nullptr);
+    trb_status r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, with_aov ? &req : nullptr);
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev1, 0));
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, 0));
     CU(cudaStreamSynchronize(0));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
-    { // additive, like film::Image::add_pixels (image.rs:21-33); a 33 MB read-modify-write: split over a few host threads
-        const size_t n = npx * 4;
-        const unsigned nt = n >= (1u << 20) ? std::min(8u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
-        const float* src = s->h_film_staging;
-        auto add = [film, src](size_t a, size_t b) { for (size_t i = a; i < b; ++i) film[i] += src[i]; };
-        std::vector<std::thread> th;
-        for (unsigned k = 1; k < nt; ++k) th.emplace_back(add, n * k / nt, n * (k + 1) / nt);
-        add(0, n / nt);
-        for (auto& t : th) t.join();
+    add_film(film, s->h_film_staging, npx * 4);
+    if (with_aov) {
+        std::vector<float> h;
+        for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, d_albedo.p}, std::pair<float*, void*>{aov->normal_w, d_normal.p}}) {
+            if (!dst) continue;
+            h.resize(npx * 4);
+            CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
+            add_film(dst, h.data(), npx * 4);
+        }
+        if (aov->nearest) CU(cudaMemcpy(aov->nearest, d_nearest.p, npx * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     }
     if (stats) {
         trb::DStats h;
@@ -2635,9 +2724,8 @@ trb_status trb_render(trb_scene* s, const trb_render_cfg* cfg, float* film, trb_
     return TRB_OK;
 }
 
-trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_stats* stats) {
-    if (!s || !cfg || !samples) return fail(TRB_INVALID_ARG, "null argument");
-    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+// trb_render_samples' body; aov: the host AOV records of trb_render_samples_aov (nullptr: none)
+trb_status render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov, trb_stats* stats) {
     CU(cudaSetDevice(s->device));
     uint32_t spp, first, count, nb;
     const uint2* d_blocks = nullptr;
@@ -2649,17 +2737,28 @@ trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n,
     if (n == 0) return TRB_OK;
     trb_sample* d_out = nullptr;
     CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
+    DeviceBuffer d_aov;
+    if (aov) {
+        const cudaError_t e = cudaMalloc(&d_aov.p, n * sizeof(trb_aov_sample));
+        if (e != cudaSuccess) {
+            cudaFree(d_out);
+            cudaGetLastError();
+            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(e));
+        }
+    }
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     trb::RenderParams rp{};
     rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
     rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
+    const AovRequest req{static_cast<trb_aov_sample*>(d_aov.p), nullptr, nullptr, nullptr};
     CU(cudaEventRecord(s->ev0, 0));
-    r = launch_render(s, rp, cfg->flags, 1, 0);
+    r = launch_render(s, rp, cfg->flags, 1, 0, aov ? &req : nullptr);
     if (r != TRB_OK) { cudaFree(d_out); return r; }
     CU(cudaEventRecord(s->ev1, 0));
     cudaError_t e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
     cudaFree(d_out);
     CU(e);
+    if (aov) CU(cudaMemcpy(aov, d_aov.p, n * sizeof(trb_aov_sample), cudaMemcpyDeviceToHost));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
     if (stats) {
@@ -2670,6 +2769,52 @@ trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n,
         CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
     }
     return TRB_OK;
+}
+} // namespace
+
+trb_status trb_render_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !d_film) return fail(TRB_INVALID_ARG, "null argument");
+    return render_device(s, cfg, d_film, d_stats, static_cast<cudaStream_t>(stream), nullptr);
+}
+
+trb_status trb_render(trb_scene* s, const trb_render_cfg* cfg, float* film, trb_stats* stats) {
+    if (!s || !cfg || !film) return fail(TRB_INVALID_ARG, "null argument");
+    return render_host(s, cfg, film, nullptr, stats);
+}
+
+trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_stats* stats) {
+    if (!s || !cfg || !samples) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    return render_samples(s, cfg, n, samples, nullptr, stats);
+}
+
+trb_status trb_render_aov_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, const trb_aov_film* d_aov, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !d_film || !d_aov) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    const trb_status r = aov_supported(s, cfg);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_film) | reinterpret_cast<uintptr_t>(d_aov->albedo_w) | reinterpret_cast<uintptr_t>(d_aov->normal_w)) & 15u) ||
+        (reinterpret_cast<uintptr_t>(d_aov->nearest) & 7u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest)};
+    const bool with_aov = d_aov->albedo_w || d_aov->normal_w || d_aov->nearest;
+    return render_device(s, cfg, d_film, d_stats, static_cast<cudaStream_t>(stream), with_aov ? &req : nullptr);
+}
+
+trb_status trb_render_aov(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats) {
+    if (!s || !cfg || !film || !aov) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_status r = aov_supported(s, cfg);
+    if (r != TRB_OK) return r;
+    return render_host(s, cfg, film, aov, stats);
+}
+
+trb_status trb_render_samples_aov(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov, trb_stats* stats) {
+    if (!s || !cfg || !samples || !aov) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    const trb_status r = aov_supported(s, cfg);
+    if (r != TRB_OK) return r;
+    return render_samples(s, cfg, n, samples, aov, stats);
 }
 
 trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {

@@ -2737,6 +2737,69 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constan
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// AOVs (DESIGN.md §4 "AOVs"): one trb_aov_sample per camera sample from its primary hit, computed between the round-0 trace and the
+// round-0 shade from the path state those two kernels share. The films are written by the colour film's own kernel (k_wf_film_v2 or
+// k_wf_film) over the records' two halves, nearest by k_wf_nearest.
+// ------------------------------------------------------------------------------------------
+// Albedo of Material::bsdf's lobes (lobe_of, allocation order): colour x Fresnel factor at normal incidence, summed left to right,
+// each channel clamped to [0, 1]. MERL has no colour term: pi * BSDF::eval(n, n) over all lobes.
+__device__ __noinline__ f3 aov_albedo(const DScene& sc, const Mat& m, const Frame& fr) {
+    f3 acc = splat(0.0f);
+    if (m.type == TRB_MAT_MERL) acc = bsdf_eval(sc, m, fr, fr.n, fr.n, BX_ALL) * TRB_PI;
+    else {
+        const f3 F = fresnel(m, 1.0f);
+#pragma unroll 1
+        for (int i = 0; i < 2; ++i) {
+            int kind; uint32_t type; f3 col;
+            if (!lobe_of(m, i, kind, type, col)) continue;
+            if (kind == LK_LAMBERT || kind == LK_OREN_NAYAR) acc = acc + col;
+            else if (type & BX_TRANSMISSION) acc = acc + col * (splat(1.0f) - F);
+            else acc = acc + col * F;
+        }
+    }
+    return mk(clampf(acc.x, 0.0f, 1.0f), clampf(acc.y, 0.0f, 1.0f), clampf(acc.z, 0.0f, 1.0f));
+}
+
+// Per path of the pass (round 0: every path, path p = sample p of the pass): the camera ray (org, cont), its hit t (cont.w) and hit
+// record, the path's time (thr.w) and keyframed transforms. Writes the record's two halves, (albedo, depth) to lo[p * step] and
+// (n, inst bits) to hi[p * step]: step 2 with hi = lo + 1 is a trb_aov_sample array, step 1 two float4 arrays the film kernels read
+// as they read wf.rad. Reads nothing the shade kernels write and writes nothing they read.
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_wf_aov(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, float4* __restrict__ lo_out,
+                                                float4* __restrict__ hi_out, uint32_t step) {
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < wf.n_paths; p += gridDim.x * blockDim.x) {
+        const uint4 h4 = wf.hit[p];
+        float4 lo = make_float4(0.0f, 0.0f, 0.0f, finf()), hi = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(TRB_MISS));
+        if (h4.x != TRB_MISS) {
+            const float4 o4 = wf.org[p], c4 = wf.cont[p];
+            const float time = wf.thr[p].w;
+            Ray ray; ray.o = mk(o4.x, o4.y, o4.z); ray.d = mk(c4.x, c4.y, c4.z); ray.tmin = 0.0f; ray.tmax = c4.w;
+            HitRec h; h.t = c4.w; h.inst = h4.x; h.prim = h4.y; h.b1 = __uint_as_float(h4.z); h.b2 = __uint_as_float(h4.w);
+            Surf s;
+            surface_at<ANIM>(sc, ray, h, s, time, wf_xf_row<ANIM>(wf, p));
+            Frame fr;
+            make_frame(s, fr);
+            Mat m;
+            load_mat_at(sc, __ldg(&sc.instances[h.inst].material), s.u, s.v, time, m);
+            const f3 a = aov_albedo(sc, m, fr);
+            lo = make_float4(a.x, a.y, a.z, c4.w);
+            hi = make_float4(fr.n.x, fr.n.y, fr.n.z, __uint_as_float(h4.x));
+        }
+        lo_out[(size_t)p * step] = lo;
+        hi_out[(size_t)p * step] = hi;
+    }
+}
+
+// nearest: per camera sample of the pass, atomicMin(float_bits(depth) << 32 | inst) on the pixel the sample was taken for
+__global__ void __launch_bounds__(256) k_wf_nearest(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const float4* __restrict__ lo,
+                                                    const float4* __restrict__ hi, uint32_t n, unsigned long long* __restrict__ nearest) {
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const SampleId id = sample_id(sc, rp, p);
+        atomicMin(&nearest[id.pixel], ((unsigned long long)__float_as_uint(lo[p].w) << 32) | __float_as_uint(hi[p].w));
+    }
+}
+
 // LowDiscrepancy::get_samples + get_samples_1d + Camera::generate_ray only (parity of S2 / C)
 // k_wf_film without shared-memory atomics (opt-in: TRB_FILM_V2=1; validated by tools/film_check.py). Each of the CTA's
 // four warps splats into its OWN copy of the tile. Inside a warp the 32 lanes are 32 different pixels walking the footprint
