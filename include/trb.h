@@ -799,6 +799,66 @@ trb_status trb_render_aov_device(trb_scene* scene, const trb_render_cfg* cfg, fl
 trb_status trb_render_samples_aov(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov,
                                   trb_stats* stats);
 
+/* -- Denoising: an edge-avoiding a-trous filter over two half renders and their AOVs (DESIGN.md §4 "Denoising") -----------------
+ * SVGF's spatial filter (Schied et al. 2017, §4.4-4.5; Dammertz et al. 2010) with the variance taken from two half-buffers and the
+ * colour demodulated by the albedo. Render samples [0, n) of a frame into colour_a and [n, 2n) into colour_b (trb_render_cfg's
+ * sample_first / sample_count), with albedo_w, normal_w and nearest accumulated over both (trb_render_aov). All five are the scene's
+ * film layout: width*height RGBW float films, width*height uint64 nearest. Per pixel p, float32, left to right, never contracted:
+ *   W     = A.w + B.w. W <= 0: the output is (0, 0, 0, 0) and p is never a neighbour (blocks a block-range render did not render).
+ *   c     = (A.rgb + B.rgb) / W,  c_a = A.rgb / A.w,  c_b = B.rgb / B.w
+ *   d     = max(albedo_w.rgb / albedo_w.w, TRB_DENOISE_EPS_ALBEDO) per channel;  e = c / d,  e_a = c_a / d,  e_b = c_b / d
+ *   v     = (L(e_a) - L(e_b))^2 * 0.25,  L(x) = 0.2126 x.r + 0.7152 x.g + 0.0722 x.b
+ *   m     = normal_w.rgb / normal_w.w, len2 = m.x^2 + m.y^2 + m.z^2; n = m / sqrt(len2) per component, or "no normal" if len2 == 0
+ *   z     = the float in nearest's high 32 bits (+inf: a miss)
+ *   Unless c, albedo, m, len2, e and v are all finite and z is neither NaN nor -inf, p is copied through: (c, 1), never a neighbour.
+ *   dz    = (gx, gy), per axis the central difference (z[+1] - z[-1]) * 0.5 when both neighbours are inside the image with finite z,
+ *           else z[+1] - z or z - z[-1] for the one that is, else 0; 0 when z is infinite
+ * Iteration i = 0 .. N-1, step s = 2^i, over the valid pixels, from (e, v):
+ *   g     = sum k(dx) k(dy) v(q) / sum k(dx) k(dy) over the 3x3 q = p + (dx, dy) inside the image and valid, k = (1/4, 1/2, 1/4)
+ *   for the 25 taps q = p + s (dx, dy), dy then dx from -2 to 2, inside the image and valid, h = (1/16, 1/4, 3/8, 1/4, 1/16):
+ *     w_l = exp(-(|L(e(p)) - L(e(q))| / (sigma_luminance * sqrt(g) + TRB_DENOISE_EPS_LUMINANCE)))
+ *     w_n = max(0, n_p . n_q) squared log2(normal_power) times; 1 when neither has a normal, 0 when one has
+ *     w_z = exp(-(|z_p - z_q| / (sigma_depth * |gx * s dx + gy * s dy| + TRB_DENOISE_EPS_DEPTH))); 1 when both z are infinite,
+ *           0 when one is
+ *     w   = h(dx) h(dy) * w_l * w_n * w_z
+ *   e'(p) = sum w e(q) / sum w,  v'(p) = sum w^2 v(q) / (sum w)^2
+ * The output of a valid pixel is (e_N * d, 1): an RGBW film that trb_film_to_srgb8 and trb_host_film_to_srgb8 take as it is. Every NaN
+ * the output holds is written as 0x7fffffff, whatever NaN the inputs carried. exp is
+ * the library's deterministic exp; sums run in tap order without atomics, so the output is bit-reproducible. */
+#define TRB_DENOISE_EPS_ALBEDO 1e-3f
+#define TRB_DENOISE_EPS_LUMINANCE 1e-6f
+#define TRB_DENOISE_EPS_DEPTH 1e-2f
+
+/* The five inputs, all required: host pointers for trb_denoise, device pointers for trb_denoise_device. */
+typedef struct trb_denoise_input {
+    const float* colour_a;
+    const float* colour_b;
+    const float* albedo_w;
+    const float* normal_w;
+    const uint64_t* nearest;
+} trb_denoise_input;
+
+/* NULL means the defaults: 5 iterations (0-10; 0 = demodulate and remodulate only), normal_power 128 (a power of two, 1-1024),
+ * sigma_luminance 4 and sigma_depth 1 (finite, > 0). Anything else is TRB_INVALID_ARG. */
+typedef struct trb_denoise_params {
+    uint32_t iterations;
+    uint32_t normal_power;
+    float sigma_luminance;
+    float sigma_depth;
+} trb_denoise_params;
+
+/* Denoise HOST films into the HOST RGBW film out_rgbw (width*height*4 floats, overwritten). The inputs are staged per call; blocking.
+ * The scene keeps 72 bytes of scratch per pixel, allocated by its first denoise (TRB_OOM if that does not fit) and released when
+ * trb_scene_replace_settings changes the film; renders never allocate it. TRB_INVALID_ARG for a null argument, bad parameters or an
+ * output that overlaps an input. */
+trb_status trb_denoise(trb_scene* scene, const trb_denoise_input* in, const trb_denoise_params* params, float* out_rgbw);
+
+/* trb_denoise with DEVICE buffers on the scene's GPU (films and output 16-byte aligned, nearest 8-byte aligned; TRB_INVALID_ARG
+ * otherwise), enqueued on cuda_stream (a cudaStream_t; NULL = default stream) under trb_render_device's one-stream rule. No host
+ * synchronisation, except once when the scratch grows. */
+trb_status trb_denoise_device(trb_scene* scene, const trb_denoise_input* d_in, const trb_denoise_params* params, float* d_out_rgbw,
+                              void* cuda_stream);
+
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
  * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */

@@ -103,3 +103,12 @@ for d in (SB.scene_animated(32, 32, 2).finish(), SB.scene_materials_zoo(32, 32, 
     _, aovs, _ = g.render_aov(seed=3, flags=F.RENDER_NO_UPDATE)
     print("aov ok", int((aov["inst"] != F.MISS).sum()), float(aovs["albedo_w"][..., 3].sum()))
     g.close()
+# the denoiser (k_dn_prepare, k_dn_atrous): a block-range render leaves zero-weight pixels; every iteration count's step reaches the
+# borders of a 40 x 24 image
+g = api.Scene(SB.scene_c4(5000, 40, 24, 4).finish())
+g.update_frame(0, 0.0, 0.0)
+den, film, aovs, _ = g.render_denoised(4, seed=3, block_start=2, block_count=10)
+for it in (0, 1, 10):
+    d = g.denoise(film, film, aovs, iterations=it)
+print("denoise ok", float(den[..., :3].sum()), int((den[..., 3] == 0).sum()))
+g.close()

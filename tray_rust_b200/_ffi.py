@@ -204,6 +204,20 @@ class AovFilm(C.Structure):
     _fields_ = [("albedo_w", C.c_void_p), ("normal_w", C.c_void_p), ("nearest", C.c_void_p)]
 
 
+class DenoiseInput(C.Structure):
+    """trb_denoise_input: the two half films, the albedo and normal films and the nearest buffer (all required)"""
+    _fields_ = [("colour_a", C.c_void_p), ("colour_b", C.c_void_p), ("albedo_w", C.c_void_p), ("normal_w", C.c_void_p),
+                ("nearest", C.c_void_p)]
+
+
+class DenoiseParams(C.Structure):
+    """trb_denoise_params (NULL: DENOISE_DEFAULTS)"""
+    _fields_ = [("iterations", u32), ("normal_power", u32), ("sigma_luminance", f32), ("sigma_depth", f32)]
+
+
+DENOISE_DEFAULTS = dict(iterations=5, normal_power=128, sigma_luminance=4.0, sigma_depth=1.0)
+
+
 class BvhNode(C.Structure):
     _fields_ = [("bmin", f32 * 3), ("bmax", f32 * 3), ("a", u32), ("b", u32)]
 
@@ -255,6 +269,7 @@ TRB_SYMBOLS = [
     "trb_scene_replace_objects", "trb_scene_replace_meshes", "trb_scene_replace_meshes_device",
     "trb_scene_replace_settings", "trb_scene_replace_materials", "trb_scene_replace_materials_device",
     "trb_render_aov", "trb_render_aov_device", "trb_render_samples_aov",
+    "trb_denoise", "trb_denoise_device",
 ]
 
 _trb = None
@@ -326,6 +341,8 @@ def load_trb():
     lib.trb_render_aov.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), C.POINTER(Stats)]
     lib.trb_render_aov_device.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp]
     lib.trb_render_samples_aov.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp, C.POINTER(Stats)]
+    lib.trb_denoise.argtypes = [vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseParams), vp]
+    lib.trb_denoise_device.argtypes = [vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseParams), vp, vp]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

@@ -81,6 +81,14 @@ def decode_nearest(nearest):
     return (nearest >> np.uint64(32)).astype(np.uint32).view(np.float32), (nearest & np.uint64(0xffffffff)).astype(np.uint32)
 
 
+def _denoise_params(params):
+    unknown = set(params) - set(F.DENOISE_DEFAULTS)
+    if unknown:
+        raise TypeError("unknown denoise parameters: %s" % sorted(unknown))
+    p = dict(F.DENOISE_DEFAULTS, **params)
+    return F.DenoiseParams(p["iterations"], p["normal_power"], p["sigma_luminance"], p["sigma_depth"])
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
 
@@ -232,6 +240,53 @@ class Scene(_Base):
         st = F.Stats()
         self._check(self._lib.trb_render_samples_aov(self._h, C.byref(cfg), n, F.ptr(out), F.ptr(aov), C.byref(st)))
         return out, aov, st
+
+    def denoise(self, colour_a, colour_b, aovs, out=None, **params):
+        """trb_denoise (DESIGN.md §4 "Denoising"): the two half films of a frame, (height, width, 4) float32, and the AOVs rendered
+        over both (a dict with "albedo_w", "normal_w" and "nearest", as render_aov returns it). params: iterations, normal_power,
+        sigma_luminance, sigma_depth; a missing one takes its default (F.DENOISE_DEFAULTS). Returns the denoised RGBW film (into
+        `out` when given). Scene.render_denoised renders the inputs and calls this."""
+        film_shape = (self.height, self.width, 4)
+        ins = [("colour_a", colour_a, film_shape, np.float32), ("colour_b", colour_b, film_shape, np.float32),
+               ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32), ("normal_w", aovs.get("normal_w"), film_shape, np.float32),
+               ("nearest", aovs.get("nearest"), (self.height, self.width), np.uint64)]
+        if out is None:
+            out = np.zeros(film_shape, np.float32)
+        for name, a, shape, dtype in ins + [("out", out, film_shape, np.float32)]:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        d_in, prm = F.DenoiseInput(*(a.ctypes.data for _, a, _, _ in ins)), _denoise_params(params)
+        self._check(self._lib.trb_denoise(self._h, C.byref(d_in), C.byref(prm), F.ptr(out)))
+        return out
+
+    def denoise_device(self, d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest, d_out, stream=None, **params):
+        """trb_denoise_device: device pointers as ints (films and d_out height*width*4 float32, 16-byte aligned; d_nearest
+        height*width uint64, 8-byte aligned), enqueued on `stream` (a cudaStream_t as an int; None = default stream). params as for
+        denoise."""
+        d_in, prm = F.DenoiseInput(d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest), _denoise_params(params)
+        self._check(self._lib.trb_denoise_device(self._h, C.byref(d_in), C.byref(prm), d_out, stream))
+
+    def render_denoised(self, spp=0, denoise=None, **kw):
+        """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:
+        samples [0, spp/2) and [spp/2, spp) are rendered into two films by render_aov, with the albedo, normal and nearest AOVs
+        accumulated over both, and denoised with the parameters in the dict `denoise` (None: the defaults). kw: render_aov's
+        (seed, current_frame, flags, block_start, block_count). Returns (denoised, film, aovs, (stats_a, stats_b)), where film is
+        the sum of the two halves, the noisy spp-sample film. Raises ValueError below 2 spp."""
+        n = 1
+        while n < (spp or self.spp):
+            n *= 2
+        if n < 2:
+            raise ValueError("a denoised render needs at least 2 samples per pixel (two half renders); got %d" % (spp or self.spp))
+        for k in ("spp", "sample_first", "sample_count"):
+            if k in kw:
+                raise ValueError("render_denoised chooses %s itself" % k)
+        half = n // 2
+        a, aovs, st_a = self.render_aov(spp=n, sample_first=0, sample_count=half, **kw)
+        kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
+        b, _, st_b = self.render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
+                                     sample_count=half, **kw)
+        out = self.denoise(a, b, aovs, **(denoise or {}))
+        return out, a + b, aovs, (st_a, st_b)
 
     def _mesh_verts(self, mesh):
         if not 0 <= mesh < self._desc.n_meshes:

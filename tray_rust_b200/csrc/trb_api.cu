@@ -7,10 +7,12 @@
 #include <cstdlib>
 #include <memory>
 #include <thread>
+#include <tuple>
 #include <cub/device/device_radix_sort.cuh>
 #include "trb_host.h"
 #include "trb_kernels.cuh"
 #include "trb_bvh_build.cuh"
+#include "trb_denoise.cuh"
 
 using namespace trbh;
 
@@ -326,9 +328,12 @@ struct trb_scene {
     // (albedo, depth) in d_aov[p] and (n, inst bits) in d_aov[aov_capacity + p], 32 bytes
     float4* d_aov = nullptr;
     size_t aov_capacity = 0;
+    // denoiser scratch (trb_denoise*; trb::DnScratch), allocated by the first denoise for the film's pixel count and released with the film
+    void* d_denoise = nullptr;
+    size_t denoise_pixels = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
-                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov}) if (p) cudaFree(p);
+                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, d_denoise}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -2088,10 +2093,11 @@ void commit_film(trb_scene* s, StagedFilm& g) {
     for (BlockList& b : s->block_lists) cudaFree(b.dev);
     s->block_lists.clear();
     for (void** p : {(void**)&s->d_ad_state, (void**)&s->d_ad_list[0], (void**)&s->d_ad_list[1], (void**)&s->d_ad_index[0],
-                     (void**)&s->d_ad_index[1], (void**)&s->d_ad_flags, (void**)&s->d_ad_count, (void**)&s->d_ad_spp}) {
+                     (void**)&s->d_ad_index[1], (void**)&s->d_ad_flags, (void**)&s->d_ad_count, (void**)&s->d_ad_spp, &s->d_denoise}) {
         if (*p) cudaFree(*p);
         *p = nullptr;
     }
+    s->denoise_pixels = 0;
 }
 
 // The material records, MERL tables and image textures, and the counts they are checked against
@@ -2815,6 +2821,108 @@ trb_status trb_render_samples_aov(trb_scene* s, const trb_render_cfg* cfg, size_
     const trb_status r = aov_supported(s, cfg);
     if (r != TRB_OK) return r;
     return render_samples(s, cfg, n, samples, aov, stats);
+}
+
+namespace {
+// trb_denoise_params, NULL meaning the defaults (include/trb.h "Denoising"); checked before anything else, so no scene is needed
+trb_status denoise_params(const trb_denoise_params* p, trb::DnParams& out) {
+    const trb_denoise_params d = p ? *p : trb_denoise_params{5, 128, 4.0f, 1.0f};
+    if (d.iterations > 10) return fail(TRB_INVALID_ARG, "denoise iterations must be 0 to 10");
+    if (d.normal_power < 1 || d.normal_power > 1024 || (d.normal_power & (d.normal_power - 1)))
+        return fail(TRB_INVALID_ARG, "denoise normal_power must be a power of two from 1 to 1024");
+    if (!(d.sigma_luminance > 0.0f) || !std::isfinite(d.sigma_luminance)) return fail(TRB_INVALID_ARG, "denoise sigma_luminance must be finite and > 0");
+    if (!(d.sigma_depth > 0.0f) || !std::isfinite(d.sigma_depth)) return fail(TRB_INVALID_ARG, "denoise sigma_depth must be finite and > 0");
+    out.iterations = d.iterations;
+    out.normal_squarings = (uint32_t)__builtin_ctz(d.normal_power);
+    out.sigma_l = d.sigma_luminance; out.sigma_z = d.sigma_depth;
+    return TRB_OK;
+}
+
+// The argument checks of both forms: parameters, null pointers, an output overlapping an input
+trb_status denoise_check(const trb_scene* s, const trb_denoise_input* in, const trb_denoise_params* params, const float* out, trb::DnParams& prm) {
+    const trb_status r = denoise_params(params, prm);
+    if (r != TRB_OK) return r;
+    if (!s || !in || !out || !in->colour_a || !in->colour_b || !in->albedo_w || !in->normal_w || !in->nearest) return fail(TRB_INVALID_ARG, "null argument");
+    prm.width = (int)s->film.width; prm.height = (int)s->film.height;
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    const uintptr_t o0 = reinterpret_cast<uintptr_t>(out), o1 = o0 + npx * sizeof(float4);
+    const std::pair<const void*, size_t> ins[5] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
+                                                   {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                                                   {in->nearest, npx * sizeof(uint64_t)}};
+    for (const auto& [p, bytes] : ins) {
+        const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+        if (a < o1 && o0 < a + bytes) return fail(TRB_INVALID_ARG, "the denoise output overlaps an input");
+    }
+    return TRB_OK;
+}
+
+// Enqueue the 1 + N denoise launches on `st`. The scratch is per scene and sized by the film; growing it drains the device once.
+trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_denoise_input& in, float* d_out, cudaStream_t st) {
+    const size_t npx = (size_t)prm.width * prm.height;
+    if (npx == 0) return TRB_OK;
+    if (s->denoise_pixels < npx) {
+        if (s->d_denoise) {
+            CU(cudaDeviceSynchronize()); // a denoise still in flight owns the old scratch
+            cudaFree(s->d_denoise);
+        }
+        s->d_denoise = nullptr; s->denoise_pixels = 0;
+        const cudaError_t e = cudaMalloc(&s->d_denoise, npx * trb::DN_BYTES_PER_PIXEL);
+        if (e != cudaSuccess) {
+            cudaGetLastError(); s->d_denoise = nullptr;
+            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("denoise scratch: ") + cudaGetErrorString(e));
+        }
+        s->denoise_pixels = npx;
+    }
+    float4* base = static_cast<float4*>(s->d_denoise);
+    const trb::DnScratch sc{base, base + npx, {base + 2 * npx, base + 3 * npx}, reinterpret_cast<float2*>(base + 4 * npx)};
+    float4* out = reinterpret_cast<float4*>(d_out);
+    const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    trb::k_dn_prepare<<<grid, block, 0, st>>>(prm, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
+                                              reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                              reinterpret_cast<const unsigned long long*>(in.nearest), sc, out);
+    g_launches++;
+    CU(cudaGetLastError());
+    for (uint32_t i = 0; i < prm.iterations; ++i) {
+        const bool last = i + 1 == prm.iterations;
+        trb::k_dn_atrous<<<grid, block, 0, st>>>(prm, 1 << i, sc.guide, sc.grad, sc.divisor, sc.ev[i & 1], last ? nullptr : sc.ev[(i + 1) & 1],
+                                                 last ? out : nullptr);
+        g_launches++;
+        CU(cudaGetLastError());
+    }
+    return TRB_OK;
+}
+} // namespace
+
+trb_status trb_denoise_device(trb_scene* s, const trb_denoise_input* d_in, const trb_denoise_params* params, float* d_out, void* stream) {
+    trb::DnParams prm{};
+    const trb_status r = denoise_check(s, d_in, params, d_out, prm);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
+          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out)) & 15u) || (reinterpret_cast<uintptr_t>(d_in->nearest) & 7u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    CU(cudaSetDevice(s->device));
+    return denoise_enqueue(s, prm, *d_in, d_out, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_denoise(trb_scene* s, const trb_denoise_input* in, const trb_denoise_params* params, float* out) {
+    trb::DnParams prm{};
+    trb_status r = denoise_check(s, in, params, out, prm);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_out;
+    for (auto [d, h, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
+                               {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
+        CU(cudaMalloc(&d->p, bytes));
+        CU(cudaMemcpy(d->p, h, bytes, cudaMemcpyHostToDevice));
+    }
+    CU(cudaMalloc(&d_out.p, fb));
+    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
+                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
+    r = denoise_enqueue(s, prm, d_in, static_cast<float*>(d_out.p), 0);
+    if (r != TRB_OK) return r;
+    CU(cudaMemcpy(out, d_out.p, fb, cudaMemcpyDeviceToHost));
+    return TRB_OK;
 }
 
 trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {

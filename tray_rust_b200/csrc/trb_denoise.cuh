@@ -1,0 +1,171 @@
+// trb_denoise.cuh — the denoiser of trb_denoise / trb_denoise_device (include/trb.h "Denoising", DESIGN.md §4 "Denoising"): SVGF's
+// edge-avoiding a-trous filter over the demodulated colour of two half renders, guided by their albedo, normal and nearest-hit films.
+// Two kernels: k_dn_prepare reads the inputs once into a guide record per pixel and the first (e, v) buffer; k_dn_atrous runs one
+// iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film. Float32 in the header's order, no
+// atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
+#pragma once
+#include "trb_detmath.cuh"
+#include "../../include/trb.h"
+
+namespace trb {
+
+struct DnParams {
+    int width, height;
+    uint32_t iterations;
+    uint32_t normal_squarings;   // log2(normal_power)
+    float sigma_l, sigma_z;
+};
+
+// The scene's scratch for n pixels, 72 bytes each: guide (n, z) with z = NaN marking a pixel that is not filtered, the albedo divisor d,
+// two (e, v) buffers, and the depth gradient
+struct DnScratch {
+    float4* guide;
+    float4* divisor;
+    float4* ev[2];
+    float2* grad;
+};
+constexpr size_t DN_BYTES_PER_PIXEL = 4 * sizeof(float4) + sizeof(float2);
+
+__device__ __forceinline__ bool dn_finite(float x) { return fabsf(x) < __int_as_float(0x7f800000); }
+__device__ __forceinline__ float dn_lum(float r, float g, float b) { return 0.2126f * r + 0.7152f * g + 0.0722f * b; }
+// every NaN the output holds is written as 0x7fffffff, whatever its inputs carried
+__device__ __forceinline__ float4 dn_out(float r, float g, float b, float w) {
+    const float qnan = __int_as_float(0x7fffffff);
+    return make_float4(r == r ? r : qnan, g == g ? g : qnan, b == b ? b : qnan, w);
+}
+__device__ __forceinline__ float dn_depth(const unsigned long long* nearest, int i) { return __uint_as_float((uint32_t)(nearest[i] >> 32)); }
+
+// one axis of the depth gradient: central, one-sided, or 0 (z finite)
+__device__ __forceinline__ float dn_grad(float z, bool has_lo, float zlo, bool has_hi, float zhi) {
+    has_lo = has_lo && dn_finite(zlo);
+    has_hi = has_hi && dn_finite(zhi);
+    if (has_lo && has_hi) return (zhi - zlo) * 0.5f;
+    if (has_hi) return zhi - z;
+    if (has_lo) return z - zlo;
+    return 0.0f;
+}
+
+__global__ void __launch_bounds__(256) k_dn_prepare(const DnParams prm, const float4* __restrict__ ca, const float4* __restrict__ cb,
+                                                    const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                    const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int i = y * prm.width + x;
+    const float4 A = ca[i], B = cb[i];
+    const float W = A.w + B.w;
+    if (W <= 0.0f) {
+        out[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        return;
+    }
+    const float c0 = (A.x + B.x) / W, c1 = (A.y + B.y) / W, c2 = (A.z + B.z) / W;
+    const float4 al = alb[i], nw = nrm[i];
+    const float a0 = al.x / al.w, a1 = al.y / al.w, a2 = al.z / al.w;
+    const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
+    const float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
+    const float la = dn_lum(A.x / A.w / d0, A.y / A.w / d1, A.z / A.w / d2), lb = dn_lum(B.x / B.w / d0, B.y / B.w / d1, B.z / B.w / d2);
+    const float dl = la - lb;
+    const float v = dl * dl * 0.25f;
+    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
+    const float z = dn_depth(nearest, i);
+    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
+                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && dn_finite(v) &&
+                    z == z && z != __int_as_float(0xff800000);
+    if (!ok) {
+        out[i] = dn_out(c0, c1, c2, 1.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        return;
+    }
+    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    if (len2 != 0.0f) {
+        const float l = sqrtf(len2);
+        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    }
+    float gx = 0.0f, gy = 0.0f;
+    if (dn_finite(z)) {
+        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
+        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
+        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
+    }
+    sc.guide[i] = make_float4(n0, n1, n2, z);
+    sc.grad[i] = make_float2(gx, gy);
+    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
+    sc.ev[0][i] = make_float4(e0, e1, e2, v);
+    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+}
+
+// One a-trous iteration at step s from ev_in to ev_out, or, the last one, remodulated into out (ev_out unused)
+__global__ void __launch_bounds__(256) k_dn_atrous(const DnParams prm, int s, const float4* __restrict__ guide, const float2* __restrict__ grad,
+                                                   const float4* __restrict__ divisor, const float4* __restrict__ ev_in,
+                                                   float4* __restrict__ ev_out, float4* __restrict__ out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int W = prm.width, H = prm.height, i = y * W + x;
+    const float4 gp = guide[i];
+    if (gp.w != gp.w) return; // not filtered: k_dn_prepare wrote its output
+    const float4 ep = ev_in[i];
+    const float lp = dn_lum(ep.x, ep.y, ep.z);
+    float gs = 0.0f, gk = 0.0f;
+    for (int dy = -1; dy <= 1; ++dy)
+        for (int dx = -1; dx <= 1; ++dx) {
+            const int qx = x + dx, qy = y + dy;
+            if (qx < 0 || qx >= W || qy < 0 || qy >= H) continue;
+            const int q = qy * W + qx;
+            if (guide[q].w != guide[q].w) continue;
+            const float k = (dx == 0 ? 0.5f : 0.25f) * (dy == 0 ? 0.5f : 0.25f);
+            gk = gk + k;
+            gs = gs + k * ev_in[q].w;
+        }
+    const float denom_l = prm.sigma_l * sqrtf(gs / gk) + TRB_DENOISE_EPS_LUMINANCE;
+    const float2 g = grad[i];
+    const bool p_inf = !dn_finite(gp.w), p_nrm = gp.x != 0.0f || gp.y != 0.0f || gp.z != 0.0f;
+    const float h[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
+    float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, sw = 0.0f, sv = 0.0f;
+#pragma unroll
+    for (int dy = -2; dy <= 2; ++dy) {
+        const int qy = y + s * dy;
+        if (qy < 0 || qy >= H) continue;
+#pragma unroll
+        for (int dx = -2; dx <= 2; ++dx) {
+            const int qx = x + s * dx;
+            if (qx < 0 || qx >= W) continue;
+            const int q = qy * W + qx;
+            const float4 gq = guide[q];
+            if (gq.w != gq.w) continue;
+            const float4 eq = ev_in[q];
+            const float wl = dexp(-(fabsf(lp - dn_lum(eq.x, eq.y, eq.z)) / denom_l));
+            float wn;
+            const bool q_nrm = gq.x != 0.0f || gq.y != 0.0f || gq.z != 0.0f;
+            if (p_nrm != q_nrm) wn = 0.0f;
+            else if (!p_nrm) wn = 1.0f;
+            else {
+                const float dot = gp.x * gq.x + gp.y * gq.y + gp.z * gq.z;
+                wn = dot > 0.0f ? dot : 0.0f;
+                for (uint32_t k = 0; k < prm.normal_squarings; ++k) wn = wn * wn;
+            }
+            float wz;
+            const bool q_inf = !dn_finite(gq.w);
+            if (p_inf != q_inf) wz = 0.0f;
+            else if (p_inf) wz = 1.0f;
+            else wz = dexp(-(fabsf(gp.w - gq.w) / (prm.sigma_z * fabsf(g.x * (float)(s * dx) + g.y * (float)(s * dy)) + TRB_DENOISE_EPS_DEPTH)));
+            float w = h[dx + 2] * h[dy + 2];
+            w = w * wl;
+            w = w * wn;
+            w = w * wz;
+            s0 = s0 + w * eq.x; s1 = s1 + w * eq.y; s2 = s2 + w * eq.z;
+            sw = sw + w;
+            sv = sv + w * w * eq.w;
+        }
+    }
+    const float e0 = s0 / sw, e1 = s1 / sw, e2 = s2 / sw;
+    if (out) {
+        const float4 d = divisor[i];
+        out[i] = dn_out(e0 * d.x, e1 * d.y, e2 * d.z, 1.0f);
+    } else {
+        ev_out[i] = make_float4(e0, e1, e2, sv / (sw * sw));
+    }
+}
+
+} // namespace trb

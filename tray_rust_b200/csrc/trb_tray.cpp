@@ -1,6 +1,6 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
-//   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D]
+//   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
 //
@@ -13,7 +13,9 @@
 // (Image::get_srgb8 == trb_host_film_to_srgb8) and written.
 // Worker: trb_worker's code (trb_distrib.hpp).
 //
-// Extensions over the reference: --seed, --spp and --device mean what they mean for trb_worker; a worker address is host[:port],
+// Extensions over the reference: --seed, --spp and --device mean what they mean for trb_worker; --denoise renders every frame as two
+// half-sample renders with AOVs and writes the denoised image (trb_denoise; single node, path integrator, 2 spp or more, refused
+// before anything renders otherwise: the wire format carries no AOVs); a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -28,6 +30,7 @@
 #include <cerrno>
 #include <chrono>
 #include <cstdarg>
+#include <memory>
 #include "trb_distrib.hpp"
 #include "../../include/tray_exec.hpp"
 
@@ -36,6 +39,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
+    "             [--denoise]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -50,6 +54,8 @@ const char* USAGE =
     "  --seed S                Random seed of the render (default 1).\n"
     "  --spp N                 Samples per pixel, overriding the scene's film.samples.\n"
     "  --device D              CUDA device to render on (default 0).\n"
+    "  --denoise               Render each frame's samples as two halves with albedo, normal and depth, and write the denoised\n"
+    "                          image. Single node only, path integrator, at least 2 samples per pixel.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -139,7 +145,7 @@ struct Args {
     std::string scene;
     std::vector<std::string> workers;
     const char* out = nullptr;
-    bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false;
+    bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
 };
 
@@ -159,11 +165,37 @@ bool load_desc(const Args& a, uint32_t spp, Desc& desc, uint64_t& start, uint64_
     return true;
 }
 
+uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
+
+// --denoise: samples [0, n/2) and [n/2, n) of the frame into two films, the AOVs over both, then trb_denoise (DESIGN.md §4 "Denoising")
+struct DenoisedFrame {
+    std::vector<float> a, b, albedo, normal, out;
+    std::vector<uint64_t> nearest;
+    explicit DenoisedFrame(size_t npx) : a(npx * 4), b(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame) {
+        std::fill(a.begin(), a.end(), 0.0f); std::fill(b.begin(), b.end(), 0.0f);
+        std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
+        std::fill(nearest.begin(), nearest.end(), ~0ull);
+        trb_render_cfg cfg{};
+        cfg.spp = spp; cfg.seed = seed; cfg.current_frame = frame; cfg.sample_count = spp / 2;
+        const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
+        tray::check(trb_render_aov(s, &cfg, a.data(), &aov, nullptr)); // includes Scene::update_frame
+        cfg.sample_first = spp / 2; cfg.flags = TRB_RENDER_NO_UPDATE;
+        tray::check(trb_render_aov(s, &cfg, b.data(), &aov, nullptr));
+        const trb_denoise_input in{a.data(), b.data(), albedo.data(), normal.data(), nearest.data()};
+        tray::check(trb_denoise(s, &in, nullptr, out.data()));
+    }
+};
+
 // ---- single node (main.rs:56-109) -------------------------------------------------------------------------------------------
 int single_node(const Args& a, const OutPath& out) {
     Desc desc;
     uint64_t start = 0, end = 0;
     if (!load_desc(a, (uint32_t)a.spp, desc, start, end)) return 1;
+    const uint32_t spp = pow2_at_least(std::max(1u, desc.d->film.samples));
+    if (a.denoise && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("--denoise needs the path integrator: the scene's integrator renders no albedo, normal or depth");
+    if (a.denoise && spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders); the scene has %u", spp);
     try {
         tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
         trb_desc_free(desc.d); desc.d = nullptr;
@@ -173,10 +205,19 @@ int single_node(const Args& a, const OutPath& out) {
         tray::Config config;
         config.seed = (uint32_t)a.seed;
         const auto scene_start = std::chrono::steady_clock::now();
+        std::unique_ptr<DenoisedFrame> dn;
+        if (a.denoise) dn.reset(new DenoisedFrame((size_t)dim.first * dim.second));
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
-            exec.render(scene, rt, config);
-            const std::vector<uint8_t> img = tray::get_render(scene, rt);
+            std::vector<uint8_t> img;
+            if (dn) {
+                dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
+                img.resize((size_t)dim.first * dim.second * 3);
+                tray::check(trb_film_to_srgb8(scene.handle(), dn->out.data(), img.data()));
+            } else {
+                exec.render(scene, rt, config);
+                img = tray::get_render(scene, rt);
+            }
             const std::string file = out.file_for(i);
             if (!save_image(out, file, img.data(), (uint32_t)dim.first, (uint32_t)dim.second)) return 1;
             rt.clear();
@@ -376,8 +417,13 @@ int master_node(const Args& a, const OutPath& out) {
 } // namespace
 
 int main(int argc, char** argv) {
-    for (int i = 1; i < argc; ++i)
-        if (std::strcmp(argv[i], "--worker") == 0) return trb_distrib::worker_main(argc, argv);
+    bool worker = false, denoise = false;
+    for (int i = 1; i < argc; ++i) {
+        worker = worker || std::strcmp(argv[i], "--worker") == 0;
+        denoise = denoise || std::strcmp(argv[i], "--denoise") == 0;
+    }
+    if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
     for (int i = 1; i < argc; ++i) {
@@ -397,6 +443,7 @@ int main(int argc, char** argv) {
         else if (s == "--spp") ok = number(a.spp, a.has_spp) && a.spp <= UINT32_MAX;
         else if (s == "--device") ok = number(a.device, a.has_device) && a.device <= INT32_MAX;
         else if (s == "--master") a.master = true;
+        else if (s == "--denoise") a.denoise = true;
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -406,6 +453,8 @@ int main(int argc, char** argv) {
     if (a.master && a.workers.empty()) return die("--master needs at least one worker address");
     if (!a.master && !a.workers.empty()) return die("unexpected argument '%s' (worker addresses follow --master)", a.workers[0].c_str());
     if (a.master && (a.has_seed || a.has_spp || a.has_device)) return die("--seed, --spp and --device are the workers' options: pass them to each worker");
+    if (a.master && a.denoise) return die("--denoise is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.denoise && a.has_spp && a.spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders)");
     if (a.has_start && a.has_end && a.end < a.start)
         return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
     OutPath out;
