@@ -859,6 +859,93 @@ trb_status trb_denoise(trb_scene* scene, const trb_denoise_input* in, const trb_
 trb_status trb_denoise_device(trb_scene* scene, const trb_denoise_input* d_in, const trb_denoise_params* params, float* d_out_rgbw,
                               void* cuda_stream);
 
+/* -- Temporal denoising: reproject each pixel's history through the scene's motion and accumulate the half-buffers over frames -----
+ * (DESIGN.md §4 "Temporal denoising"). SVGF's temporal half (Schied et al. 2017, §4.1-4.2) over trb_denoise's inputs, with the
+ * variance still taken from the two halves: two half histories blended with the same weights are two independent estimates of one
+ * mean, so (L(ē_a) - L(ē_b))^2 / 4 stays the variance of their mean, and it shrinks as the history grows.
+ *
+ * A trb_denoise_history belongs to one scene (another scene is TRB_INVALID_ARG). It is empty after create and after reset, and it
+ * takes the film size of the first call that uses it: a later call with another film size (trb_scene_replace_settings) is
+ * TRB_INVALID_ARG until it is reset. Per pixel it holds H_a, H_b (the demodulated accumulated halves), the unit normal n, the depth
+ * z, the instance inst and len (frames accumulated), or "none"; two such sets, each call reading one and writing the other. It also
+ * holds a snapshot of the frame it was written at: the inverse of the camera's cam_world at shutter-open, tan(fov / 2), the film size,
+ * every instance's world transform at shutter-open (object -> world), the instance count, and the scene's object generation, a counter
+ * that trb_scene_replace_objects and trb_scene_replace_meshes with an object section (the calls that renumber instances) increment.
+ * A history of another generation is treated as empty.
+ *
+ * The inputs are trb_denoise's, rendered at the scene's current frame (the last update_frame; a render with current_frame sets it).
+ * Per pixel p = (x, y), float32, left to right, never contracted: validity, e, e_a, e_b, v, d, n, z and dz are trb_denoise's. A pixel
+ * trb_denoise does not filter is written as trb_denoise writes it, stores "none", has motion (NaN, NaN) and history_length 0.
+ * Otherwise, with i = the low 32 bits of nearest:
+ *   1. o, dir = camera_ray's arithmetic through (x + 0.5, y + 0.5) with the current frame's cam_world at shutter-open (not a keyframed
+ *      camera's per-ray transform): pc = px_to_cam . (x + 0.5, y + 0.5, 0), dir = cam_world (vector) . unit(tan * pc.x, tan * pc.y,
+ *      1 * pc.z), o = cam_world (point) . 0; p_w = o + z * dir per component.
+ *   2. Motion, when the history is not empty, its generation is the scene's, i is below the snapshot's and the scene's instance count
+ *      and z is finite: p_o = inv_cur[i] . p_w, p' = mat_prev[i] . p_o, q = cam_inv_prev . p' (points, applied as the trace kernels
+ *      apply an instance's inverse: divided by w when |w - 1| < FLT_EPSILON). If q.z > 0:
+ *        X = q.x / (q.z * tan_prev), Y = q.y / (q.z * tan_prev)
+ *        r = ((X - X0) / (X1 - X0) * w_prev, (Y - Y1) / (Y0 - Y1) * h_prev), with a = (float)w_prev / (float)h_prev and
+ *            (X0, X1, Y0, Y1) = a > 1 ? (-a, a, -1, 1) : (-1, 1, -1 / a, 1 / a): the inverse of camera_ray's raster -> camera
+ *            mapping up to rounding, since camera space directions are (tan X, tan Y, 1) up to scale
+ *        motion = r - (x + 0.5, y + 0.5); |q| = sqrt(q.x^2 + q.y^2 + q.z^2) is the depth the previous frame's ray would record.
+ *      Otherwise motion is (NaN, NaN) and there is no history.
+ *   3. c = r - 0.5, f = (floor(c.x), floor(c.y)), a = c - f. Taps t = f + (0,0), (1,0), (0,1), (1,1) in that order, with weights
+ *      (1 - a.x) * (1 - a.y), a.x * (1 - a.y), (1 - a.x) * a.y, a.x * a.y. A tap counts when it is inside the image (tested on the
+ *      float coordinates), is not "none", has inst == i, |z_t - |q|| <= depth_tolerance * |q|, and n_t . n >= normal_threshold when
+ *      both have a normal (passing when neither has one, failing when one has). S = the sum of the counted weights in tap order; if
+ *      S > 0, H_a' = (sum of w * H_a in tap order) / S per channel, H_b' likewise, len_prev = the largest len of a counted tap with
+ *      w > 0. S <= 0: no history.
+ *   4. n' = min(len_prev + 1, max_history), or 1 without history. n' == 1: ē_a = e_a, ē_b = e_b, and e, v are trb_denoise's (so the
+ *      output is trb_denoise's, bit for bit). Otherwise alpha = 1 / (float)n', per channel
+ *        ē_a = alpha * e_a + (1 - alpha) * H_a',  ē_b likewise,  ē = alpha * e + (1 - alpha) * ((H_a' + H_b') * 0.5)
+ *        v = (L(ē_a) - L(ē_b))^2 * 0.25
+ *   5. (ē, v) replaces (e, v) in trb_denoise's a-trous iterations; the output is remodulated by d as there.
+ *   6. A filtered pixel with finite z stores (ē_a, ē_b, n, z, i, n'); every other pixel stores "none". The snapshot becomes the
+ *      current frame's.
+ * Every NaN written to rgbw or motion is 0x7fffffff. Motion covers rigid instance transforms and the camera, not the deformation of
+ * trb_scene_update_mesh / trb_scene_refit_mesh: the depth and normal tests reject what moved too far, and what they accept may ghost.
+ * Misses have no history. */
+typedef struct trb_denoise_history trb_denoise_history;
+
+/* NULL means: trb_denoise's defaults for `spatial`, max_history 8 (1-255), depth_tolerance 0.05 (finite, > 0), normal_threshold 0.9
+ * (in [-1, 1]). `spatial` takes trb_denoise's ranges. Anything out of range is TRB_INVALID_ARG. These defaults have not been tuned. */
+typedef struct trb_denoise_temporal_params {
+    trb_denoise_params spatial;
+    uint32_t max_history;
+    float depth_tolerance;
+    float normal_threshold;
+    uint32_t pad; /* ignored */
+} trb_denoise_temporal_params;
+
+/* rgbw (width*height*4 floats) is required; motion (width*height*2 floats) and history_length (width*height uint32) may be NULL. */
+typedef struct trb_denoise_temporal_output {
+    float* rgbw;
+    float* motion;
+    uint32_t* history_length;
+} trb_denoise_temporal_output;
+
+/* An empty history for `scene`'s temporal denoising. Its per-pixel buffers (96 bytes per pixel) and the instance snapshot (64 bytes
+ * per instance, twice) are allocated by its first call and grown where a call needs more (draining the device once, TRB_OOM if it does
+ * not fit). Destroy it before its scene. */
+trb_status trb_denoise_history_create(trb_scene* scene, trb_denoise_history** out);
+trb_status trb_denoise_history_destroy(trb_denoise_history* history);
+/* Empty the history and forget its film size; the next call filters as trb_denoise does. */
+trb_status trb_denoise_history_reset(trb_denoise_history* history);
+
+/* Denoise a frame with its history: HOST inputs and outputs, staged per call; blocking. Parameters are checked first (no scene is
+ * needed to refuse them); then TRB_INVALID_ARG for a null scene, history, input or out->rgbw, a history of another scene or film size,
+ * a scene without a frame, or an output overlapping an input or another output; TRB_OOM when scratch or history does not fit. A call
+ * that fails leaves the history as it was. */
+trb_status trb_denoise_temporal(trb_scene* scene, trb_denoise_history* history, const trb_denoise_input* in,
+                                const trb_denoise_temporal_params* params, const trb_denoise_temporal_output* out);
+
+/* trb_denoise_temporal with DEVICE buffers (films and rgbw 16-byte, nearest and motion 8-byte, history_length 4-byte aligned;
+ * TRB_INVALID_ARG otherwise), enqueued on cuda_stream under trb_render_device's one-stream rule: 1 + iterations kernel launches and
+ * one copy of the instance transforms. No host synchronisation, except once when the scratch or the history grows. */
+trb_status trb_denoise_temporal_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_input* d_in,
+                                       const trb_denoise_temporal_params* params, const trb_denoise_temporal_output* d_out,
+                                       void* cuda_stream);
+
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
  * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */

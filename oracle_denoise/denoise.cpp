@@ -6,6 +6,8 @@
  *                no scene: width and height are arguments. Statuses: TRB_INVALID_ARG for a null pointer or the parameters
  *                trb_denoise refuses.
  *
+ * oracle_temporal/temporal.cpp includes this file whole for denoise_params, denoise_prepare and denoise_filter.
+ *
  * Nothing here is shared with the library's kernels (tray_rust_b200/csrc/trb_denoise.cuh): the per-pixel state is a plain struct,
  * validity is a bool, and every iteration is a fresh pass over the image.
  */
@@ -40,23 +42,27 @@ float axis_gradient(float z, bool lo_in, float zlo, bool hi_in, float zhi) {
     return 0.0f;
 }
 
-}  // namespace
-
-extern "C" {
-
-int orc_denoise(uint32_t width, uint32_t height, const trb_denoise_input* in, const trb_denoise_params* params, float* out) {
-    trb_denoise_params p = {5, 128, 4.0f, 1.0f};
+/* The parameters (NULL: the defaults) into p and log2(normal_power); false where trb_denoise refuses them */
+bool denoise_params(const trb_denoise_params* params, trb_denoise_params& p, int& squarings) {
+    p = trb_denoise_params{5, 128, 4.0f, 1.0f};
     if (params) p = *params;
-    if (p.iterations > 10) return TRB_INVALID_ARG;
-    int squarings = -1;
+    if (p.iterations > 10) return false;
+    squarings = -1;
     for (int k = 0; k <= 10; ++k)
         if (p.normal_power == (1u << k)) squarings = k;
-    if (squarings < 0) return TRB_INVALID_ARG;
-    if (!(p.sigma_luminance > 0.0f) || !fin(p.sigma_luminance) || !(p.sigma_depth > 0.0f) || !fin(p.sigma_depth)) return TRB_INVALID_ARG;
-    if (!in || !out || !in->colour_a || !in->colour_b || !in->albedo_w || !in->normal_w || !in->nearest) return TRB_INVALID_ARG;
-    const long W = width, H = height, N = W * H;
-    std::vector<Px> px(N);
-    std::vector<float> e(N * 3), v(N);
+    if (squarings < 0) return false;
+    return p.sigma_luminance > 0.0f && fin(p.sigma_luminance) && p.sigma_depth > 0.0f && fin(p.sigma_depth);
+}
+
+/* The per-pixel rules before the first iteration: px, e (3 per pixel) and v; ea and eb (3 per pixel, may be NULL) receive the
+ * demodulated halves e_a and e_b */
+void denoise_prepare(long W, long H, const trb_denoise_input* in, std::vector<Px>& px, std::vector<float>& e, std::vector<float>& v,
+                     std::vector<float>* ea_all, std::vector<float>* eb_all) {
+    const long N = W * H;
+    px.assign(N, Px());
+    e.assign(N * 3, 0.0f); v.assign(N, 0.0f);
+    if (ea_all) ea_all->assign(N * 3, 0.0f);
+    if (eb_all) eb_all->assign(N * 3, 0.0f);
     for (long y = 0; y < H; ++y)
         for (long x = 0; x < W; ++x) {
             const long i = y * W + x;
@@ -79,6 +85,8 @@ int orc_denoise(uint32_t width, uint32_t height, const trb_denoise_input* in, co
                 eb[k] = B[k] / B[3] / q.d[k];
                 m[k] = nw[k] / nw[3];
                 ok = ok && fin(m[k]) && fin(e[3 * i + k]);
+                if (ea_all) (*ea_all)[3 * i + k] = ea[k];
+                if (eb_all) (*eb_all)[3 * i + k] = eb[k];
             }
             const float dl = lum(ea) - lum(eb);
             v[i] = dl * dl * 0.25f;
@@ -97,6 +105,12 @@ int orc_denoise(uint32_t width, uint32_t height, const trb_denoise_input* in, co
                 q.gy = axis_gradient(q.z, y > 0, y > 0 ? depth_of(in->nearest[i - W]) : 0.0f, y + 1 < H, y + 1 < H ? depth_of(in->nearest[i + W]) : 0.0f);
             }
         }
+}
+
+/* The a-trous iterations from (e, v) and the output film */
+void denoise_filter(long W, long H, const trb_denoise_params& p, int squarings, const std::vector<Px>& px, std::vector<float> e,
+                    std::vector<float> v, float* out) {
+    const long N = W * H;
     const float h[5] = {1.0f / 16.0f, 1.0f / 4.0f, 3.0f / 8.0f, 1.0f / 4.0f, 1.0f / 16.0f};
     const float k3[3] = {0.25f, 0.5f, 0.25f};
     std::vector<float> e2(N * 3), v2(N);
@@ -165,6 +179,21 @@ int orc_denoise(uint32_t width, uint32_t height, const trb_denoise_input* in, co
         }
         o[3] = 1.0f;
     }
+}
+
+}  // namespace
+
+extern "C" {
+
+int orc_denoise(uint32_t width, uint32_t height, const trb_denoise_input* in, const trb_denoise_params* params, float* out) {
+    trb_denoise_params p;
+    int squarings;
+    if (!denoise_params(params, p, squarings)) return TRB_INVALID_ARG;
+    if (!in || !out || !in->colour_a || !in->colour_b || !in->albedo_w || !in->normal_w || !in->nearest) return TRB_INVALID_ARG;
+    std::vector<Px> px;
+    std::vector<float> e, v;
+    denoise_prepare(width, height, in, px, e, v, nullptr, nullptr);
+    denoise_filter(width, height, p, squarings, px, std::move(e), std::move(v), out);
     return TRB_OK;
 }
 

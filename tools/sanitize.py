@@ -112,3 +112,13 @@ for it in (0, 1, 10):
     d = g.denoise(film, film, aovs, iterations=it)
 print("denoise ok", float(den[..., :3].sum()), int((den[..., 3] == 0).sum()))
 g.close()
+# the temporal denoiser (k_dn_temporal): three frames of the keyframed scene with motion and history lengths, taps reaching the borders,
+# then a history reset
+g = api.Scene(SB.scene_animated(40, 24, 2).finish())
+hist = api.DenoiseHistory(g)
+for k in range(3):
+    den, film, aovs, _ = g.render_denoised_temporal(hist, 2, seed=3, current_frame=k)
+    _, motion, hl = g.denoise_temporal(hist, film, film, aovs, motion=True, history_length=True, iterations=1)
+hist.reset()
+print("denoise temporal ok", float(den[..., :3].sum()), int(hl.max()), int(np.isnan(motion).sum()))
+g.close()

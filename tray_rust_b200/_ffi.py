@@ -218,6 +218,19 @@ class DenoiseParams(C.Structure):
 DENOISE_DEFAULTS = dict(iterations=5, normal_power=128, sigma_luminance=4.0, sigma_depth=1.0)
 
 
+class DenoiseTemporalParams(C.Structure):
+    """trb_denoise_temporal_params (NULL: DENOISE_DEFAULTS and DENOISE_TEMPORAL_DEFAULTS)"""
+    _fields_ = [("spatial", DenoiseParams), ("max_history", u32), ("depth_tolerance", f32), ("normal_threshold", f32), ("pad", u32)]
+
+
+class DenoiseTemporalOutput(C.Structure):
+    """trb_denoise_temporal_output: rgbw (required), motion and history_length (may be NULL)"""
+    _fields_ = [("rgbw", C.c_void_p), ("motion", C.c_void_p), ("history_length", C.c_void_p)]
+
+
+DENOISE_TEMPORAL_DEFAULTS = dict(max_history=8, depth_tolerance=0.05, normal_threshold=0.9)
+
+
 class BvhNode(C.Structure):
     _fields_ = [("bmin", f32 * 3), ("bmax", f32 * 3), ("a", u32), ("b", u32)]
 
@@ -270,6 +283,8 @@ TRB_SYMBOLS = [
     "trb_scene_replace_settings", "trb_scene_replace_materials", "trb_scene_replace_materials_device",
     "trb_render_aov", "trb_render_aov_device", "trb_render_samples_aov",
     "trb_denoise", "trb_denoise_device",
+    "trb_denoise_history_create", "trb_denoise_history_destroy", "trb_denoise_history_reset", "trb_denoise_temporal",
+    "trb_denoise_temporal_device",
 ]
 
 _trb = None
@@ -343,6 +358,12 @@ def load_trb():
     lib.trb_render_samples_aov.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_denoise.argtypes = [vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseParams), vp]
     lib.trb_denoise_device.argtypes = [vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseParams), vp, vp]
+    lib.trb_denoise_history_create.argtypes = [vp, C.POINTER(vp)]
+    lib.trb_denoise_history_destroy.argtypes = [vp]
+    lib.trb_denoise_history_reset.argtypes = [vp]
+    lib.trb_denoise_temporal.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseTemporalParams), C.POINTER(DenoiseTemporalOutput)]
+    lib.trb_denoise_temporal_device.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseTemporalParams),
+                                                C.POINTER(DenoiseTemporalOutput), vp]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

@@ -89,6 +89,42 @@ def _denoise_params(params):
     return F.DenoiseParams(p["iterations"], p["normal_power"], p["sigma_luminance"], p["sigma_depth"])
 
 
+def _temporal_params(params):
+    unknown = set(params) - set(F.DENOISE_DEFAULTS) - set(F.DENOISE_TEMPORAL_DEFAULTS)
+    if unknown:
+        raise TypeError("unknown temporal denoise parameters: %s" % sorted(unknown))
+    t = dict(F.DENOISE_TEMPORAL_DEFAULTS, **{k: v for k, v in params.items() if k in F.DENOISE_TEMPORAL_DEFAULTS})
+    spatial = _denoise_params({k: v for k, v in params.items() if k in F.DENOISE_DEFAULTS})
+    return F.DenoiseTemporalParams(spatial, t["max_history"], t["depth_tolerance"], t["normal_threshold"], 0)
+
+
+class DenoiseHistory:
+    """trb_denoise_history (DESIGN.md §4 "Temporal denoising"): the per-pixel history and frame snapshot of one scene's temporal
+    denoise. Empty when created and after reset(); close() (or the scene's close) releases it."""
+
+    def __init__(self, scene):
+        self._lib = scene._lib
+        self._scene = scene
+        h = C.c_void_p()
+        scene._check(self._lib.trb_denoise_history_create(scene._h, C.byref(h)))
+        self._h = h
+        scene._histories.append(self)
+
+    def reset(self):
+        self._scene._check(self._lib.trb_denoise_history_reset(self._h))
+
+    def close(self):
+        if self._h is not None:
+            self._lib.trb_denoise_history_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class _Base:
     """Shared helpers; subclasses provide self._lib, self._h, self._pfx and self._check."""
 
@@ -163,6 +199,7 @@ class Scene(_Base):
         self._desc = desc  # keep arrays alive
         h = C.c_void_p()
         self._h = None
+        self._histories = []  # DenoiseHistory objects, released before the scene
         self._check(self._lib.trb_scene_create(C.byref(desc), device, C.byref(h)))
         self._h = h
         self.device = device
@@ -176,6 +213,8 @@ class Scene(_Base):
 
     def close(self):
         if self._h is not None:
+            for hist in getattr(self, "_histories", []):
+                hist.close()
             self._lib.trb_scene_destroy(self._h)
             self._h = None
 
@@ -265,6 +304,68 @@ class Scene(_Base):
         denoise."""
         d_in, prm = F.DenoiseInput(d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest), _denoise_params(params)
         self._check(self._lib.trb_denoise_device(self._h, C.byref(d_in), C.byref(prm), d_out, stream))
+
+    def denoise_temporal(self, history, colour_a, colour_b, aovs, out=None, motion=False, history_length=False, **params):
+        """trb_denoise_temporal (DESIGN.md §4 "Temporal denoising"): denoise's inputs, rendered at the scene's current frame, with the
+        DenoiseHistory `history`, which it reads and then holds this frame. params: denoise's plus max_history, depth_tolerance and
+        normal_threshold (F.DENOISE_TEMPORAL_DEFAULTS). Returns the denoised RGBW film (into `out` when given), or a tuple of it with
+        the (height, width, 2) float32 motion and the (height, width) uint32 history length where `motion` / `history_length` ask
+        for them (True, or an array to write into)."""
+        film_shape = (self.height, self.width, 4)
+        ins = [("colour_a", colour_a, film_shape, np.float32), ("colour_b", colour_b, film_shape, np.float32),
+               ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32), ("normal_w", aovs.get("normal_w"), film_shape, np.float32),
+               ("nearest", aovs.get("nearest"), (self.height, self.width), np.uint64)]
+        if out is None:
+            out = np.zeros(film_shape, np.float32)
+        outs = [("out", out, film_shape, np.float32)]
+        if motion is True:
+            motion = np.zeros((self.height, self.width, 2), np.float32)
+        if history_length is True:
+            history_length = np.zeros((self.height, self.width), np.uint32)
+        if motion is not False and motion is not None:
+            outs.append(("motion", motion, (self.height, self.width, 2), np.float32))
+        if history_length is not False and history_length is not None:
+            outs.append(("history_length", history_length, (self.height, self.width), np.uint32))
+        for name, a, shape, dtype in ins + outs:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseInput(*(a.ctypes.data for _, a, _, _ in ins)), _temporal_params(params)
+        o = F.DenoiseTemporalOutput(out.ctypes.data, got["motion"].ctypes.data if "motion" in got else None,
+                                    got["history_length"].ctypes.data if "history_length" in got else None)
+        self._check(self._lib.trb_denoise_temporal(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o)))
+        if len(outs) == 1:
+            return out
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_temporal_device(self, history, d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest, d_out, d_motion=None,
+                                d_history_length=None, stream=None, **params):
+        """trb_denoise_temporal_device: denoise_device's pointers (ints) plus d_motion (height*width*2 float32, 8-byte aligned) and
+        d_history_length (height*width uint32), either None; enqueued on `stream`. params as for denoise_temporal."""
+        d_in, prm = F.DenoiseInput(d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest), _temporal_params(params)
+        o = F.DenoiseTemporalOutput(d_out, d_motion, d_history_length)
+        self._check(self._lib.trb_denoise_temporal_device(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o), stream))
+
+    def render_denoised_temporal(self, history, spp=0, seed=1, current_frame=0, denoise=None, **kw):
+        """render_denoised for frame `current_frame` of an animation, denoised with `history` (denoise_temporal; the dict `denoise`
+        holds its parameters). The two halves are rendered with seed (seed + current_frame) mod 2^32, so that consecutive frames draw
+        independent samples (a frame's radiance is a pure function of scene, seed, pixel and sample). Returns render_denoised's tuple."""
+        frame_seed = (seed + current_frame) % (1 << 32)
+        n = 1
+        while n < (spp or self.spp):
+            n *= 2
+        if n < 2:
+            raise ValueError("a denoised render needs at least 2 samples per pixel (two half renders); got %d" % (spp or self.spp))
+        for k in ("spp", "sample_first", "sample_count"):
+            if k in kw:
+                raise ValueError("render_denoised_temporal chooses %s itself" % k)
+        half = n // 2
+        a, aovs, st_a = self.render_aov(spp=n, sample_first=0, sample_count=half, seed=frame_seed, current_frame=current_frame, **kw)
+        kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
+        b, _, st_b = self.render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
+                                     sample_count=half, seed=frame_seed, current_frame=current_frame, **kw)
+        out = self.denoise_temporal(history, a, b, aovs, **(denoise or {}))
+        return out, a + b, aovs, (st_a, st_b)
 
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:

@@ -331,6 +331,10 @@ struct trb_scene {
     // denoiser scratch (trb_denoise*; trb::DnScratch), allocated by the first denoise for the film's pixel count and released with the film
     void* d_denoise = nullptr;
     size_t denoise_pixels = 0;
+    // temporal denoising (trb_denoise_temporal*): the inverse of the camera's cam_world at the current frame's shutter-open, and the
+    // object generation, counted up by the calls that renumber instances (replace_objects, replace_meshes with an object section)
+    float cam_inv[16] = {};
+    uint64_t object_generation = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
                         (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, d_denoise}) if (p) cudaFree(p);
@@ -2247,18 +2251,24 @@ trb_status trb_scene_refit_mesh_device(trb_scene* s, uint32_t mesh, const float*
 trb_status trb_scene_replace_objects(trb_scene* s, const trb_scene_objects* objects) {
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     if (!objects) return fail(TRB_INVALID_ARG, "null objects");
-    return replace_objects(s, *objects);
+    const trb_status r = replace_objects(s, *objects);
+    if (r == TRB_OK) s->object_generation++;
+    return r;
 }
 
 trb_status trb_scene_replace_meshes(trb_scene* s, const trb_scene_meshes* meshes, const trb_scene_objects* objects) {
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     if (!meshes) return fail(TRB_INVALID_ARG, "null meshes");
-    return replace_meshes(s, *meshes, objects, false, nullptr);
+    const trb_status r = replace_meshes(s, *meshes, objects, false, nullptr);
+    if (r == TRB_OK && objects) s->object_generation++;
+    return r;
 }
 trb_status trb_scene_replace_meshes_device(trb_scene* s, const trb_scene_meshes* meshes, const trb_scene_objects* objects, void* cuda_stream) {
     if (!s) return fail(TRB_INVALID_ARG, "null scene");
     if (!meshes) return fail(TRB_INVALID_ARG, "null meshes");
-    return replace_meshes(s, *meshes, objects, true, static_cast<cudaStream_t>(cuda_stream));
+    const trb_status r = replace_meshes(s, *meshes, objects, true, static_cast<cudaStream_t>(cuda_stream));
+    if (r == TRB_OK && objects) s->object_generation++;
+    return r;
 }
 
 trb_status trb_scene_replace_settings(trb_scene* s, const trb_film* film, const trb_integrator* integrator) {
@@ -2479,6 +2489,7 @@ trb_status trb_scene_update_frame(trb_scene* s, uint32_t frame, float start, flo
     bool any_anim = !cam_static;
     std::memcpy(s->ds.cam.px_to_cam, px_to_cam.m, 64);
     std::memcpy(s->ds.cam.cam_mat, cam_world.fwd.m, 64);
+    std::memcpy(s->cam_inv, cam_world.inv.m, 64);
     std::memcpy(s->ds.cam.scaling, scaling, 12);
     s->ds.cam.shutter_open = s->shutter_open; s->ds.cam.shutter_close = s->shutter_close;
 
@@ -2856,10 +2867,8 @@ trb_status denoise_check(const trb_scene* s, const trb_denoise_input* in, const 
     return TRB_OK;
 }
 
-// Enqueue the 1 + N denoise launches on `st`. The scratch is per scene and sized by the film; growing it drains the device once.
-trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_denoise_input& in, float* d_out, cudaStream_t st) {
-    const size_t npx = (size_t)prm.width * prm.height;
-    if (npx == 0) return TRB_OK;
+// The scene's denoise scratch for the film's npx pixels. The scratch is per scene and sized by the film; growing it drains the device once.
+trb_status denoise_scratch(trb_scene* s, size_t npx, trb::DnScratch& sc) {
     if (s->denoise_pixels < npx) {
         if (s->d_denoise) {
             CU(cudaDeviceSynchronize()); // a denoise still in flight owns the old scratch
@@ -2874,14 +2883,13 @@ trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_den
         s->denoise_pixels = npx;
     }
     float4* base = static_cast<float4*>(s->d_denoise);
-    const trb::DnScratch sc{base, base + npx, {base + 2 * npx, base + 3 * npx}, reinterpret_cast<float2*>(base + 4 * npx)};
-    float4* out = reinterpret_cast<float4*>(d_out);
+    sc = trb::DnScratch{base, base + npx, {base + 2 * npx, base + 3 * npx}, reinterpret_cast<float2*>(base + 4 * npx)};
+    return TRB_OK;
+}
+
+// The N a-trous launches after k_dn_prepare or k_dn_temporal wrote the scratch
+trb_status denoise_atrous(const trb::DnParams& prm, const trb::DnScratch& sc, float4* out, cudaStream_t st) {
     const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
-    trb::k_dn_prepare<<<grid, block, 0, st>>>(prm, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
-                                              reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
-                                              reinterpret_cast<const unsigned long long*>(in.nearest), sc, out);
-    g_launches++;
-    CU(cudaGetLastError());
     for (uint32_t i = 0; i < prm.iterations; ++i) {
         const bool last = i + 1 == prm.iterations;
         trb::k_dn_atrous<<<grid, block, 0, st>>>(prm, 1 << i, sc.guide, sc.grad, sc.divisor, sc.ev[i & 1], last ? nullptr : sc.ev[(i + 1) & 1],
@@ -2890,6 +2898,23 @@ trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_den
         CU(cudaGetLastError());
     }
     return TRB_OK;
+}
+
+// Enqueue the 1 + N denoise launches on `st`
+trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_denoise_input& in, float* d_out, cudaStream_t st) {
+    const size_t npx = (size_t)prm.width * prm.height;
+    if (npx == 0) return TRB_OK;
+    trb::DnScratch sc;
+    const trb_status r = denoise_scratch(s, npx, sc);
+    if (r != TRB_OK) return r;
+    float4* out = reinterpret_cast<float4*>(d_out);
+    const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    trb::k_dn_prepare<<<grid, block, 0, st>>>(prm, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
+                                              reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                              reinterpret_cast<const unsigned long long*>(in.nearest), sc, out);
+    g_launches++;
+    CU(cudaGetLastError());
+    return denoise_atrous(prm, sc, out, st);
 }
 } // namespace
 
@@ -2922,6 +2947,222 @@ trb_status trb_denoise(trb_scene* s, const trb_denoise_input* in, const trb_deno
     r = denoise_enqueue(s, prm, d_in, static_cast<float*>(d_out.p), 0);
     if (r != TRB_OK) return r;
     CU(cudaMemcpy(out, d_out.p, fb, cudaMemcpyDeviceToHost));
+    return TRB_OK;
+}
+
+// ---- temporal denoising (include/trb.h "Temporal denoising", DESIGN.md §4) -------------------------------------------------------
+// Two per-pixel history sets (trb::DnHistory, 48 B per pixel each) and two instance snapshots (64 B per instance each); `cur` is the
+// set the next call reads. The host fields describe the frame the read set was written at.
+struct trb_denoise_history {
+    trb_scene* scene = nullptr;
+    int device = 0;
+    void* d_px = nullptr;          // 2 sets x 3 float4 arrays of px_capacity pixels
+    size_t px_capacity = 0;
+    float* d_mats = nullptr;       // 2 sets x mat_capacity x 16 floats
+    size_t mat_capacity = 0;
+    uint32_t cur = 0;
+    bool bound = false;            // the film size is taken (first call after create / reset)
+    uint32_t width = 0, height = 0;
+    bool has_prev = false;         // the read set holds a frame
+    float cam_inv[16] = {}, tan_fov = 0;
+    uint32_t n_instances = 0;
+    uint64_t generation = 0;
+    ~trb_denoise_history() {
+        if (d_px) cudaFree(d_px);
+        if (d_mats) cudaFree(d_mats);
+    }
+    trb::DnHistory set(uint32_t k) const {
+        float4* base = static_cast<float4*>(d_px) + (size_t)k * 3 * px_capacity;
+        return trb::DnHistory{base, base + px_capacity, base + 2 * px_capacity};
+    }
+};
+
+trb_status trb_denoise_history_create(trb_scene* s, trb_denoise_history** out) {
+    if (!s || !out) return fail(TRB_INVALID_ARG, "null argument");
+    trb_denoise_history* h = new (std::nothrow) trb_denoise_history();
+    if (!h) return fail(TRB_OOM, "denoise history");
+    h->scene = s; h->device = s->device;
+    *out = h;
+    return TRB_OK;
+}
+
+trb_status trb_denoise_history_destroy(trb_denoise_history* h) {
+    if (!h) return TRB_OK;
+    cudaSetDevice(h->device);
+    delete h; // cudaFree waits for the calls still reading the buffers
+    return TRB_OK;
+}
+
+trb_status trb_denoise_history_reset(trb_denoise_history* h) {
+    if (!h) return fail(TRB_INVALID_ARG, "null history");
+    h->has_prev = false; h->bound = false; h->width = h->height = 0;
+    return TRB_OK;
+}
+
+namespace {
+bool spans_overlap(const void* a, size_t abytes, const void* b, size_t bbytes) {
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+    return a && b && a0 < b0 + bbytes && b0 < a0 + abytes;
+}
+
+// trb_denoise_temporal_params, NULL meaning the defaults; checked before anything else
+trb_status temporal_params(const trb_denoise_temporal_params* p, trb::DnParams& prm, trb::DnTemporal& tp) {
+    const trb_status r = denoise_params(p ? &p->spatial : nullptr, prm);
+    if (r != TRB_OK) return r;
+    const uint32_t max_history = p ? p->max_history : 8u;
+    const float depth_tolerance = p ? p->depth_tolerance : 0.05f, normal_threshold = p ? p->normal_threshold : 0.9f;
+    if (max_history < 1 || max_history > 255) return fail(TRB_INVALID_ARG, "temporal denoise max_history must be 1 to 255");
+    if (!(depth_tolerance > 0.0f) || !std::isfinite(depth_tolerance)) return fail(TRB_INVALID_ARG, "temporal denoise depth_tolerance must be finite and > 0");
+    if (!(normal_threshold >= -1.0f && normal_threshold <= 1.0f)) return fail(TRB_INVALID_ARG, "temporal denoise normal_threshold must be in [-1, 1]");
+    tp.max_history = max_history; tp.depth_tolerance = depth_tolerance; tp.normal_threshold = normal_threshold;
+    return TRB_OK;
+}
+
+// The checks of both forms after the parameters: null pointers, the history's scene and film size, a frame, overlapping outputs
+trb_status temporal_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_input* in, const trb_denoise_temporal_params* params,
+                          const trb_denoise_temporal_output* out, trb::DnParams& prm, trb::DnTemporal& tp) {
+    trb_status r = temporal_params(params, prm, tp);
+    if (r != TRB_OK) return r;
+    if (!s || !h || !in || !out || !out->rgbw) return fail(TRB_INVALID_ARG, "null argument");
+    r = denoise_check(s, in, params ? &params->spatial : nullptr, out->rgbw, prm);
+    if (r != TRB_OK) return r;
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    const std::pair<const void*, size_t> ins[5] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
+                                                   {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                                                   {in->nearest, npx * sizeof(uint64_t)}};
+    const std::pair<const void*, size_t> outs[3] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)},
+                                                    {out->history_length, npx * sizeof(uint32_t)}};
+    for (int k = 1; k < 3; ++k) {
+        for (const auto& [p, bytes] : ins)
+            if (spans_overlap(outs[k].first, outs[k].second, p, bytes)) return fail(TRB_INVALID_ARG, "a temporal denoise output overlaps an input");
+        for (int j = 0; j < k; ++j)
+            if (spans_overlap(outs[k].first, outs[k].second, outs[j].first, outs[j].second))
+                return fail(TRB_INVALID_ARG, "two temporal denoise outputs overlap");
+    }
+    if (h->scene != s) return fail(TRB_INVALID_ARG, "the denoise history belongs to another scene");
+    if (h->bound && (h->width != s->film.width || h->height != s->film.height))
+        return fail(TRB_INVALID_ARG, "the denoise history was written at another film size: reset it");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "update_frame must be called before a temporal denoise");
+    return TRB_OK;
+}
+
+// A device buffer of `bytes`; a failure is TRB_OOM (out of memory) or TRB_CUDA and leaves *p unset
+trb_status history_alloc(void** p, size_t bytes, const char* what) {
+    const cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) return TRB_OK;
+    cudaGetLastError(); *p = nullptr;
+    return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+// k_dn_temporal and the a-trous launches on `st`, then the history's switch to the set just written
+trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_input& in,
+                            const trb_denoise_temporal_output& out, cudaStream_t st) {
+    const size_t npx = (size_t)prm.width * prm.height, n = s->instances.size();
+    if (npx == 0) return TRB_OK;
+    trb::DnScratch sc;
+    trb_status r = denoise_scratch(s, npx, sc);
+    if (r != TRB_OK) return r;
+    // the pixel sets are bound to one film size, so they only grow while the history is empty: nothing to keep. A new buffer is
+    // allocated before the old one is released, so a failure leaves the history as it was.
+    if (h->px_capacity < npx) {
+        void* p = nullptr;
+        r = history_alloc(&p, 2 * 3 * npx * sizeof(float4), "denoise history");
+        if (r != TRB_OK) return r;
+        if (h->d_px) { CU(cudaDeviceSynchronize()); cudaFree(h->d_px); } // a call still in flight owns the old sets
+        h->d_px = p; h->px_capacity = npx; h->has_prev = false;
+    }
+    if (h->mat_capacity < n) { // both snapshots, the read one copied to its place in the new buffer
+        void* p = nullptr;
+        r = history_alloc(&p, 2 * n * 16 * sizeof(float), "denoise history snapshot");
+        if (r != TRB_OK) return r;
+        if (h->d_mats) {
+            CU(cudaDeviceSynchronize());
+            const size_t rows = std::min<size_t>(h->n_instances, h->mat_capacity);
+            if (rows)
+                CU(cudaMemcpy(static_cast<float*>(p) + (size_t)h->cur * n * 16, h->d_mats + (size_t)h->cur * h->mat_capacity * 16, rows * 64,
+                              cudaMemcpyDeviceToDevice));
+            cudaFree(h->d_mats);
+        }
+        h->d_mats = static_cast<float*>(p); h->mat_capacity = n;
+    }
+    // the current frame, and the snapshot the read set was written at
+    std::memcpy(tp.px_to_cam, s->ds.cam.px_to_cam, 64);
+    std::memcpy(tp.cam_mat, s->ds.cam.cam_mat, 64);
+    std::memcpy(tp.scaling, s->ds.cam.scaling, 12);
+    tp.n_cur = (uint32_t)n;
+    std::memcpy(tp.cam_inv_prev, h->cam_inv, 64);
+    tp.tan_prev = h->tan_fov;
+    tp.w_prev = (float)prm.width; tp.h_prev = (float)prm.height;
+    const float aspect = (float)s->film.width / (float)s->film.height; // camera_setup's screen window
+    if (aspect > 1.0f) { tp.x0 = -aspect; tp.x1 = aspect; tp.y0 = -1.0f; tp.y1 = 1.0f; }
+    else { tp.x0 = -1.0f; tp.x1 = 1.0f; tp.y0 = -1.0f / aspect; tp.y1 = 1.0f / aspect; }
+    tp.n_prev = h->n_instances;
+    tp.has_prev = h->has_prev && h->generation == s->object_generation ? 1u : 0u;
+    const uint32_t rd = h->cur, wr = h->cur ^ 1u;
+    float* mats_rd = h->d_mats + (size_t)rd * h->mat_capacity * 16;
+    float* mats_wr = h->d_mats + (size_t)wr * h->mat_capacity * 16;
+    // this frame's object -> world matrices into the write snapshot: DInstance.mat, 64-byte rows at the records' 208-byte pitch
+    CU(cudaMemcpy2DAsync(mats_wr, 64, reinterpret_cast<const char*>(s->d_instances) + offsetof(trb::DInstance, mat), sizeof(trb::DInstance), 64, n,
+                         cudaMemcpyDeviceToDevice, st));
+    float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
+    const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    trb::k_dn_temporal<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
+                                               reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                               reinterpret_cast<const unsigned long long*>(in.nearest), sc, rgbw, s->d_instances, mats_rd,
+                                               h->set(rd), h->set(wr), reinterpret_cast<float2*>(out.motion), out.history_length);
+    g_launches++;
+    CU(cudaGetLastError());
+    r = denoise_atrous(prm, sc, rgbw, st);
+    if (r != TRB_OK) return r;
+    h->cur = wr; h->has_prev = true; h->bound = true; h->width = s->film.width; h->height = s->film.height;
+    std::memcpy(h->cam_inv, s->cam_inv, 64);
+    h->tan_fov = s->ds.cam.scaling[0];
+    h->n_instances = (uint32_t)n;
+    h->generation = s->object_generation;
+    return TRB_OK;
+}
+} // namespace
+
+trb_status trb_denoise_temporal_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_input* d_in, const trb_denoise_temporal_params* params,
+                                       const trb_denoise_temporal_output* d_out, void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    const trb_status r = temporal_check(s, h, d_in, params, d_out, prm, tp);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
+          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
+        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
+        (reinterpret_cast<uintptr_t>(d_out->history_length) & 3u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length 4-byte");
+    CU(cudaSetDevice(s->device));
+    return temporal_enqueue(s, h, prm, tp, *d_in, *d_out, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_denoise_temporal(trb_scene* s, trb_denoise_history* h, const trb_denoise_input* in, const trb_denoise_temporal_params* params,
+                                const trb_denoise_temporal_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    trb_status r = temporal_check(s, h, in, params, out, prm, tp);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_rgbw, d_motion, d_len;
+    for (auto [d, hp, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
+                                {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
+        CU(cudaMalloc(&d->p, bytes));
+        CU(cudaMemcpy(d->p, hp, bytes, cudaMemcpyHostToDevice));
+    }
+    CU(cudaMalloc(&d_rgbw.p, fb));
+    if (out->motion) CU(cudaMalloc(&d_motion.p, npx * sizeof(float2)));
+    if (out->history_length) CU(cudaMalloc(&d_len.p, npx * sizeof(uint32_t)));
+    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
+                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
+    const trb_denoise_temporal_output d_out{static_cast<float*>(d_rgbw.p), static_cast<float*>(d_motion.p), static_cast<uint32_t*>(d_len.p)};
+    r = temporal_enqueue(s, h, prm, tp, d_in, d_out, 0);
+    if (r != TRB_OK) return r;
+    CU(cudaMemcpy(out->rgbw, d_rgbw.p, fb, cudaMemcpyDeviceToHost));
+    if (out->motion) CU(cudaMemcpy(out->motion, d_motion.p, npx * sizeof(float2), cudaMemcpyDeviceToHost));
+    if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return TRB_OK;
 }
 

@@ -1,10 +1,12 @@
 // trb_denoise.cuh — the denoiser of trb_denoise / trb_denoise_device (include/trb.h "Denoising", DESIGN.md §4 "Denoising"): SVGF's
 // edge-avoiding a-trous filter over the demodulated colour of two half renders, guided by their albedo, normal and nearest-hit films.
-// Two kernels: k_dn_prepare reads the inputs once into a guide record per pixel and the first (e, v) buffer; k_dn_atrous runs one
-// iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film. Float32 in the header's order, no
+// Three kernels: k_dn_prepare reads the inputs once into a guide record per pixel and the first (e, v) buffer; k_dn_atrous runs one
+// iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film; k_dn_temporal takes k_dn_prepare's place
+// for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer. Float32 in the header's order, no
 // atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
 #pragma once
 #include "trb_detmath.cuh"
+#include "trb_kernels.cuh"
 #include "../../include/trb.h"
 
 namespace trb {
@@ -166,6 +168,156 @@ __global__ void __launch_bounds__(256) k_dn_atrous(const DnParams prm, int s, co
     } else {
         ev_out[i] = make_float4(e0, e1, e2, sv / (sw * sw));
     }
+}
+
+// ---- temporal denoising (trb_denoise_temporal*, include/trb.h "Temporal denoising") ---------------------------------------------
+// The current frame's camera and the history's snapshot of the frame it was written at; has_prev = 0 for an empty history or one of
+// another object generation
+struct DnTemporal {
+    float px_to_cam[16], cam_mat[16], scaling[3];
+    uint32_t n_cur;
+    float cam_inv_prev[16];
+    float tan_prev, w_prev, h_prev, x0, x1, y0, y1; // the previous film's size and screen window (camera_setup's)
+    uint32_t n_prev, has_prev;
+    uint32_t max_history;
+    float depth_tolerance, normal_threshold;
+};
+
+// One history set, 48 bytes per pixel: (H_a, z), (H_b, inst bits), (n, len bits); len == 0 is "none"
+struct DnHistory {
+    float4* a;
+    float4* b;
+    float4* n;
+};
+constexpr size_t DN_HISTORY_BYTES_PER_PIXEL = 3 * sizeof(float4);
+
+// k_dn_prepare's reads and writes, plus the reprojected history blended into (ē, v) before the a-trous iterations (1 + N launches as
+// for trb_denoise). mat_prev: the snapshot's object -> world matrices, 16 floats per instance; the current inverses are read from the
+// frame's instance records.
+__global__ void __launch_bounds__(256) k_dn_temporal(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ ca,
+                                                     const float4* __restrict__ cb, const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                     const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
+                                                     const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory hin,
+                                                     const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int i = y * prm.width + x;
+    const float qnan = __int_as_float(0x7fffffff);
+    const float4 A = ca[i], B = cb[i];
+    const float W = A.w + B.w;
+    if (W <= 0.0f) {
+        out[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        return;
+    }
+    const float c0 = (A.x + B.x) / W, c1 = (A.y + B.y) / W, c2 = (A.z + B.z) / W;
+    const float4 al = alb[i], nw = nrm[i];
+    const float a0 = al.x / al.w, a1 = al.y / al.w, a2 = al.z / al.w;
+    const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
+    float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
+    float ea0 = A.x / A.w / d0, ea1 = A.y / A.w / d1, ea2 = A.z / A.w / d2;
+    float eb0 = B.x / B.w / d0, eb1 = B.y / B.w / d1, eb2 = B.z / B.w / d2;
+    const float dl = dn_lum(ea0, ea1, ea2) - dn_lum(eb0, eb1, eb2);
+    float v = dl * dl * 0.25f;
+    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
+    const unsigned long long key = nearest[i];
+    const float z = __uint_as_float((uint32_t)(key >> 32));
+    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
+                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && dn_finite(v) &&
+                    z == z && z != __int_as_float(0xff800000);
+    if (!ok) {
+        out[i] = dn_out(c0, c1, c2, 1.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        return;
+    }
+    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    if (len2 != 0.0f) {
+        const float l = sqrtf(len2);
+        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    }
+    float gx = 0.0f, gy = 0.0f;
+    if (dn_finite(z)) {
+        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
+        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
+        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
+    }
+    // 1-3: reconstruct, reproject into the snapshot's frame, gather the history taps
+    const uint32_t id = (uint32_t)key;
+    float mx = qnan, my = qnan, S = 0.0f, ha0 = 0.0f, ha1 = 0.0f, ha2 = 0.0f, hb0 = 0.0f, hb1 = 0.0f, hb2 = 0.0f;
+    uint32_t len_prev = 0;
+    if (tp.has_prev && id < tp.n_prev && id < tp.n_cur && dn_finite(z)) {
+        const f3 pc = xf_point(tp.px_to_cam, mk((float)x + 0.5f, (float)y + 0.5f, 0.0f));
+        const f3 dir = xf_vector(tp.cam_mat, unit(mk(tp.scaling[0], tp.scaling[1], tp.scaling[2]) * pc));
+        const f3 o = xf_point(tp.cam_mat, splat(0.0f));
+        const f3 pw = mk(o.x + z * dir.x, o.y + z * dir.y, o.z + z * dir.z);
+        const f3 q = xf_point(tp.cam_inv_prev, xf_point(mat_prev + 16 * (size_t)id, xf_point(inst[id].inv, pw)));
+        if (q.z > 0.0f) {
+            const float X = q.x / (q.z * tp.tan_prev), Y = q.y / (q.z * tp.tan_prev);
+            const float rx = (X - tp.x0) / (tp.x1 - tp.x0) * tp.w_prev, ry = (Y - tp.y1) / (tp.y0 - tp.y1) * tp.h_prev;
+            mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
+            const float ql = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z);
+            const float cx = rx - 0.5f, cy = ry - 0.5f, fx = floorf(cx), fy = floorf(cy), ax = cx - fx, ay = cy - fy;
+            const bool p_nrm = n0 != 0.0f || n1 != 0.0f || n2 != 0.0f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float tx = fx + (float)(k & 1), ty = fy + (float)(k >> 1);
+                const float w = ((k & 1) ? ax : 1.0f - ax) * ((k >> 1) ? ay : 1.0f - ay);
+                if (!(tx >= 0.0f && tx <= tp.w_prev - 1.0f && ty >= 0.0f && ty <= tp.h_prev - 1.0f)) continue;
+                const int j = (int)ty * prm.width + (int)tx;
+                const float4 tn = hin.n[j];
+                const uint32_t tlen = __float_as_uint(tn.w);
+                if (tlen == 0u) continue;
+                const float4 ta = hin.a[j], tb = hin.b[j];
+                if (__float_as_uint(tb.w) != id) continue;
+                if (!(fabsf(ta.w - ql) <= tp.depth_tolerance * ql)) continue;
+                const bool t_nrm = tn.x != 0.0f || tn.y != 0.0f || tn.z != 0.0f;
+                if (t_nrm != p_nrm) continue;
+                if (p_nrm && !(tn.x * n0 + tn.y * n1 + tn.z * n2 >= tp.normal_threshold)) continue;
+                S = S + w;
+                ha0 = ha0 + w * ta.x; ha1 = ha1 + w * ta.y; ha2 = ha2 + w * ta.z;
+                hb0 = hb0 + w * tb.x; hb1 = hb1 + w * tb.y; hb2 = hb2 + w * tb.z;
+                if (w > 0.0f && tlen > len_prev) len_prev = tlen;
+            }
+        }
+    }
+    // 4: blend
+    uint32_t np = 1;
+    if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    if (np > 1) {
+        ha0 = ha0 / S; ha1 = ha1 / S; ha2 = ha2 / S;
+        hb0 = hb0 / S; hb1 = hb1 / S; hb2 = hb2 / S;
+        const float alpha = 1.0f / (float)np, beta = 1.0f - alpha;
+        e0 = alpha * e0 + beta * ((ha0 + hb0) * 0.5f);
+        e1 = alpha * e1 + beta * ((ha1 + hb1) * 0.5f);
+        e2 = alpha * e2 + beta * ((ha2 + hb2) * 0.5f);
+        ea0 = alpha * ea0 + beta * ha0; ea1 = alpha * ea1 + beta * ha1; ea2 = alpha * ea2 + beta * ha2;
+        eb0 = alpha * eb0 + beta * hb0; eb1 = alpha * eb1 + beta * hb1; eb2 = alpha * eb2 + beta * hb2;
+        const float dt = dn_lum(ea0, ea1, ea2) - dn_lum(eb0, eb1, eb2);
+        v = dt * dt * 0.25f;
+    }
+    // 5-6: the a-trous inputs as k_dn_prepare writes them, and the new history
+    sc.guide[i] = make_float4(n0, n1, n2, z);
+    sc.grad[i] = make_float2(gx, gy);
+    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
+    sc.ev[0][i] = make_float4(e0, e1, e2, v);
+    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+    if (dn_finite(z)) {
+        hout.a[i] = make_float4(ea0, ea1, ea2, z);
+        hout.b[i] = make_float4(eb0, eb1, eb2, __uint_as_float(id));
+        hout.n[i] = make_float4(n0, n1, n2, __uint_as_float(np));
+    } else {
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    if (motion) motion[i] = make_float2(mx == mx ? mx : qnan, my == my ? my : qnan);
+    if (hlen) hlen[i] = np;
 }
 
 } // namespace trb

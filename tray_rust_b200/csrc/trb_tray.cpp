@@ -1,6 +1,7 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
+//            [--denoise-temporal]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
 //
@@ -15,7 +16,8 @@
 //
 // Extensions over the reference: --seed, --spp and --device mean what they mean for trb_worker; --denoise renders every frame as two
 // half-sample renders with AOVs and writes the denoised image (trb_denoise; single node, path integrator, 2 spp or more, refused
-// before anything renders otherwise: the wire format carries no AOVs); a worker address is host[:port],
+// before anything renders otherwise: the wire format carries no AOVs); --denoise-temporal renders the frames in order with one
+// history and seed (S + frame) mod 2^32, denoising each with trb_denoise_temporal (refused where --denoise is, and with --denoise); a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -39,7 +41,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise]\n"
+    "             [--denoise | --denoise-temporal]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -56,6 +58,8 @@ const char* USAGE =
     "  --device D              CUDA device to render on (default 0).\n"
     "  --denoise               Render each frame's samples as two halves with albedo, normal and depth, and write the denoised\n"
     "                          image. Single node only, path integrator, at least 2 samples per pixel.\n"
+    "  --denoise-temporal      As --denoise, accumulating each pixel's history over the frame range through the scene's motion;\n"
+    "                          frame k is rendered with seed S + k.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -145,7 +149,8 @@ struct Args {
     std::string scene;
     std::vector<std::string> workers;
     const char* out = nullptr;
-    bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false;
+    bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
+         denoise_temporal = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
 };
 
@@ -167,12 +172,13 @@ bool load_desc(const Args& a, uint32_t spp, Desc& desc, uint64_t& start, uint64_
 
 uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 
-// --denoise: samples [0, n/2) and [n/2, n) of the frame into two films, the AOVs over both, then trb_denoise (DESIGN.md §4 "Denoising")
+// --denoise: samples [0, n/2) and [n/2, n) of the frame into two films, the AOVs over both, then trb_denoise (DESIGN.md §4 "Denoising");
+// --denoise-temporal: the same with trb_denoise_temporal and the history of the frames before (DESIGN.md §4 "Temporal denoising")
 struct DenoisedFrame {
     std::vector<float> a, b, albedo, normal, out;
     std::vector<uint64_t> nearest;
     explicit DenoisedFrame(size_t npx) : a(npx * 4), b(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame) {
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history = nullptr) {
         std::fill(a.begin(), a.end(), 0.0f); std::fill(b.begin(), b.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
@@ -183,7 +189,12 @@ struct DenoisedFrame {
         cfg.sample_first = spp / 2; cfg.flags = TRB_RENDER_NO_UPDATE;
         tray::check(trb_render_aov(s, &cfg, b.data(), &aov, nullptr));
         const trb_denoise_input in{a.data(), b.data(), albedo.data(), normal.data(), nearest.data()};
-        tray::check(trb_denoise(s, &in, nullptr, out.data()));
+        if (history) {
+            const trb_denoise_temporal_output o{out.data(), nullptr, nullptr};
+            tray::check(trb_denoise_temporal(s, history, &in, nullptr, &o));
+        } else {
+            tray::check(trb_denoise(s, &in, nullptr, out.data()));
+        }
     }
 };
 
@@ -193,9 +204,11 @@ int single_node(const Args& a, const OutPath& out) {
     uint64_t start = 0, end = 0;
     if (!load_desc(a, (uint32_t)a.spp, desc, start, end)) return 1;
     const uint32_t spp = pow2_at_least(std::max(1u, desc.d->film.samples));
-    if (a.denoise && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
-        return die("--denoise needs the path integrator: the scene's integrator renders no albedo, normal or depth");
-    if (a.denoise && spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders); the scene has %u", spp);
+    const bool denoise = a.denoise || a.denoise_temporal;
+    const char* flag = a.denoise_temporal ? "--denoise-temporal" : "--denoise";
+    if (denoise && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("%s needs the path integrator: the scene's integrator renders no albedo, normal or depth", flag);
+    if (denoise && spp < 2) return die("%s needs at least 2 samples per pixel (two half renders); the scene has %u", flag, spp);
     try {
         tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
         trb_desc_free(desc.d); desc.d = nullptr;
@@ -206,12 +219,16 @@ int single_node(const Args& a, const OutPath& out) {
         config.seed = (uint32_t)a.seed;
         const auto scene_start = std::chrono::steady_clock::now();
         std::unique_ptr<DenoisedFrame> dn;
-        if (a.denoise) dn.reset(new DenoisedFrame((size_t)dim.first * dim.second));
+        if (denoise) dn.reset(new DenoisedFrame((size_t)dim.first * dim.second));
+        trb_denoise_history* history = nullptr;
+        if (a.denoise_temporal) tray::check(trb_denoise_history_create(scene.handle(), &history));
+        const std::unique_ptr<trb_denoise_history, trb_status (*)(trb_denoise_history*)> history_owner(history, trb_denoise_history_destroy);
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (dn) {
-                dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
+                if (history) dn->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history);
+                else dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(scene.handle(), dn->out.data(), img.data()));
             } else {
@@ -417,12 +434,15 @@ int master_node(const Args& a, const OutPath& out) {
 } // namespace
 
 int main(int argc, char** argv) {
-    bool worker = false, denoise = false;
+    bool worker = false, denoise = false, denoise_temporal = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         denoise = denoise || std::strcmp(argv[i], "--denoise") == 0;
+        denoise_temporal = denoise_temporal || std::strcmp(argv[i], "--denoise-temporal") == 0;
     }
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && denoise_temporal)
+        return die("--denoise-temporal is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -444,6 +464,7 @@ int main(int argc, char** argv) {
         else if (s == "--device") ok = number(a.device, a.has_device) && a.device <= INT32_MAX;
         else if (s == "--master") a.master = true;
         else if (s == "--denoise") a.denoise = true;
+        else if (s == "--denoise-temporal") a.denoise_temporal = true;
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -455,6 +476,10 @@ int main(int argc, char** argv) {
     if (a.master && (a.has_seed || a.has_spp || a.has_device)) return die("--seed, --spp and --device are the workers' options: pass them to each worker");
     if (a.master && a.denoise) return die("--denoise is not available with --master: the wire format carries no albedo, normal or depth");
     if (a.denoise && a.has_spp && a.spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders)");
+    if (a.denoise && a.denoise_temporal) return die("--denoise and --denoise-temporal exclude each other: choose one");
+    if (a.master && a.denoise_temporal)
+        return die("--denoise-temporal is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.denoise_temporal && a.has_spp && a.spp < 2) return die("--denoise-temporal needs at least 2 samples per pixel (two half renders)");
     if (a.has_start && a.has_end && a.end < a.start)
         return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
     OutPath out;
