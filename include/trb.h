@@ -946,6 +946,70 @@ trb_status trb_denoise_temporal_device(trb_scene* scene, trb_denoise_history* hi
                                        const trb_denoise_temporal_params* params, const trb_denoise_temporal_output* d_out,
                                        void* cuda_stream);
 
+/* -- Temporal gradients: re-shade last frame's samples in this frame and shorten the history where the shading changed -------------
+ * (DESIGN.md §4 "Temporal gradients"). A-SVGF's temporal gradients (Schied, Peters, Dachsbacher 2018) on top of trb_denoise_temporal:
+ * a sample's radiance is a pure function of (scene, seed, key, sample), so one sample of the previous frame traced again in the
+ * current scene with the same random numbers differs from its recorded value only where the shading changed.
+ *
+ * Strata: the film is cut into 3x3 strata from (0, 0), the last column and row possibly smaller; gw = ceil(W / 3), gh = ceil(H / 3),
+ * S = gw * gh, stratum s = (s mod gw, s div gw). Its representative pixel is (min(3 sx + 1, W - 1), min(3 sy + 1, H - 1)).
+ * The history gains one gradient record per stratum, in two sets read and written like the pixel sets: the hit's instance i and its
+ * object-space point p_o, the camera ray (o, d, time), its key (the pixel index) and L_prev, the luminance L(x) = 0.2126 x.r +
+ * 0.7152 x.g + 0.0722 x.b of the sample's radiance clamped to [0, 1] per channel; plus the frame's cam_world at shutter-open, its
+ * shutter_open and the call's seed. The records are valid only if the previous call on the history was a gradient call of the same
+ * object generation and film size; otherwise (first call, after reset, after trb_denoise_temporal, after replace_objects) there are
+ * no gradients and lambda is 0 everywhere. Per call, float32, left to right, never contracted:
+ *   1. Re-shade. For each valid record j (i below both instance counts): p_w' = mat_cur[i] . p_o, q = cam_inv_cur . p_w' (points as
+ *      in "Temporal denoising"). Kept if q.z > 0, r = ((X - X0) / (X1 - X0) * W, (Y - Y1) / (Y0 - Y1) * H) with X = q.x / (q.z tan),
+ *      Y = q.y / (q.z tan) lies in [0, W) x [0, H), the current nearest at pixel floor(r) has instance i, and |z - dist| <=
+ *      depth_tolerance * z with dist = sqrt(v.x^2 + v.y^2 + v.z^2), v = p_w' - o_cur, o_cur = cam_world_cur . 0. Target stratum
+ *      t = floor(r) / 3 per axis; its winner is the smallest (float bits of dist) << 32 | j (a 64-bit atomicMin, so scheduling
+ *      does not matter). The winner's illumination ray: the recorded (o, d) if cam_world and mat[i] at shutter-open are both bit
+ *      for bit the snapshot's, else o = o_cur, d = unit(p_w' - o_cur) (Vector::normalized); [0, +inf); time = rec.time +
+ *      (shutter_open_cur - shutter_open_prev) (exactly rec.time when the shutter did not move); key and sample 0 from the record,
+ *      traced by trb_illumination at the record's seed with TRB_QUERY_CLAMP and spp 1. L_cur = L(its radiance). The target gets
+ *      delta = L_cur - L_prev, m = max(L_cur, L_prev), c = 1; a stratum without a winner gets (0, 0, 0).
+ *   2. Reconstruct: `iterations` a-trous passes k = 0 .. N-1 on the stratum grid, step 2^k strata, taps dy then dx from -2 to 2 inside
+ *      the grid with h = (1/16, 1/4, 3/8, 1/4, 1/16). A tap q counts when c_q > 0 and, for q != p, the representative pixels of p
+ *      and q have the same instance (the low 32 bits of nearest) and their normals (normal_w.rgb / normal_w.w, unit as in
+ *      trb_denoise; none if its length is 0 or not finite) both lack one or have n_p . n_q >= normal_threshold. W = sum h(dx) h(dy)
+ *      over counted taps; W > 0: delta' = sum w delta / W, m' = sum w m / W, c' = 1; else (0, 0, 0). Then
+ *      lambda = c > 0 && m > 0 ? min(1, |delta| / m) : 0.
+ *   3. Blend: "Temporal denoising" with one change at step 4, lambda taken from the pixel's stratum: where there is history,
+ *      len_adj = (uint32)floorf((1 - lambda) * (float)len_prev) and n' = min(len_adj + 1, max_history). Lambda 0 gives
+ *      trb_denoise_temporal's pixel, lambda 1 trb_denoise's (n' = 1). The history stores n'.
+ *   4. Record: in stratum s the pixel k = h mod (cw * ch) (row-major in the stratum, cw x ch its size), h = rng_absorb(rng_absorb(
+ *      rng_absorb(rng_seed(seed), s), 0xfffffffe), 0) (the counter hash of the sample streams); its camera ray as trb_camera_rays
+ *      generates sample 0 of 1 (with the ray's time), its hit as trb_intersect_records returns it (p_o = inv[i] . p at
+ *      shutter-open) and L as step 1 computes it at `seed`. A miss leaves the record invalid.
+ * Cost: about 2 S illumination samples and S ray queries per call on top of trb_denoise_temporal. */
+typedef struct trb_denoise_gradient_params {
+    trb_denoise_temporal_params temporal; /* as trb_denoise_temporal: same ranges and defaults */
+    uint32_t iterations;                  /* gradient a-trous passes on the stratum grid: 0-6, default 3 */
+    uint32_t pad[3];                      /* ignored */
+} trb_denoise_gradient_params;            /* NULL: all defaults */
+
+/* trb_denoise_temporal_output's three buffers, plus lambda (width*height floats, may be NULL): each pixel's lambda. */
+typedef struct trb_denoise_gradient_output {
+    float* rgbw;
+    float* motion;
+    uint32_t* history_length;
+    float* lambda;
+} trb_denoise_gradient_output;
+
+/* trb_denoise_temporal with temporal gradients: the same inputs, history, checks and statuses (parameters first, and a failed call
+ * leaves the history as it was), plus TRB_INVALID_ARG for iterations above 6 or a lambda output that overlaps another buffer.
+ * `seed` seeds this frame's gradient samples (render_denoised_temporal passes the frame's seed). HOST buffers; blocking. The
+ * history grows by 128 bytes of records and 328 bytes of per-call buffers per stratum. */
+trb_status trb_denoise_temporal_gradient(trb_scene* scene, trb_denoise_history* history, const trb_denoise_input* in,
+                                         const trb_denoise_gradient_params* params, uint32_t seed, const trb_denoise_gradient_output* out);
+
+/* The same with DEVICE buffers (the alignment of trb_denoise_temporal_device, lambda 4-byte aligned), enqueued on cuda_stream under
+ * trb_render_device's one-stream rule. No host synchronisation, except when scratch, history or the wavefront state grows. */
+trb_status trb_denoise_temporal_gradient_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_input* d_in,
+                                                const trb_denoise_gradient_params* params, uint32_t seed,
+                                                const trb_denoise_gradient_output* d_out, void* cuda_stream);
+
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
  * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */

@@ -122,3 +122,13 @@ for k in range(3):
 hist.reset()
 print("denoise temporal ok", float(den[..., :3].sum()), int(hl.max()), int(np.isnan(motion).sum()))
 g.close()
+# the temporal gradients (k_gr_*, k_dn_temporal_grad): four frames of the keyframed scene with every output, the records re-shaded
+# from the second frame on, the last with no a-trous pass, then a reset
+g = api.Scene(SB.scene_animated(40, 24, 2).finish())
+hist = api.DenoiseHistory(g)
+for k in range(4):
+    den, film, aovs, _ = g.render_denoised_temporal(hist, 2, seed=3, current_frame=k, gradients=True)
+_, motion, hl, lam = g.denoise_temporal_gradient(hist, film, film, aovs, 9, motion=True, history_length=True, lam=True, gradient_iterations=0)
+hist.reset()
+print("denoise gradient ok", float(den[..., :3].sum()), int(hl.max()), float(lam.max()))
+g.close()

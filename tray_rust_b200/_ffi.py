@@ -231,6 +231,20 @@ class DenoiseTemporalOutput(C.Structure):
 DENOISE_TEMPORAL_DEFAULTS = dict(max_history=8, depth_tolerance=0.05, normal_threshold=0.9)
 
 
+class DenoiseGradientParams(C.Structure):
+    """trb_denoise_gradient_params (NULL: the temporal defaults and DENOISE_GRADIENT_DEFAULTS)"""
+    _fields_ = [("temporal", DenoiseTemporalParams), ("iterations", u32), ("pad", u32 * 3)]
+
+
+class DenoiseGradientOutput(C.Structure):
+    """trb_denoise_gradient_output: rgbw (required), motion, history_length and lambda (may be NULL)"""
+    _fields_ = [("rgbw", C.c_void_p), ("motion", C.c_void_p), ("history_length", C.c_void_p), ("lambda_", C.c_void_p)]
+
+
+# Python name of trb_denoise_gradient_params.iterations: `iterations` already names the spatial filter's
+DENOISE_GRADIENT_DEFAULTS = dict(gradient_iterations=3)
+
+
 class BvhNode(C.Structure):
     _fields_ = [("bmin", f32 * 3), ("bmax", f32 * 3), ("a", u32), ("b", u32)]
 
@@ -284,7 +298,7 @@ TRB_SYMBOLS = [
     "trb_render_aov", "trb_render_aov_device", "trb_render_samples_aov",
     "trb_denoise", "trb_denoise_device",
     "trb_denoise_history_create", "trb_denoise_history_destroy", "trb_denoise_history_reset", "trb_denoise_temporal",
-    "trb_denoise_temporal_device",
+    "trb_denoise_temporal_device", "trb_denoise_temporal_gradient", "trb_denoise_temporal_gradient_device",
 ]
 
 _trb = None
@@ -364,6 +378,10 @@ def load_trb():
     lib.trb_denoise_temporal.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseTemporalParams), C.POINTER(DenoiseTemporalOutput)]
     lib.trb_denoise_temporal_device.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseTemporalParams),
                                                 C.POINTER(DenoiseTemporalOutput), vp]
+    lib.trb_denoise_temporal_gradient.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseGradientParams), u32,
+                                                  C.POINTER(DenoiseGradientOutput)]
+    lib.trb_denoise_temporal_gradient_device.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseGradientParams), u32,
+                                                         C.POINTER(DenoiseGradientOutput), vp]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

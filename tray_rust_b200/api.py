@@ -98,6 +98,15 @@ def _temporal_params(params):
     return F.DenoiseTemporalParams(spatial, t["max_history"], t["depth_tolerance"], t["normal_threshold"], 0)
 
 
+def _gradient_params(params):
+    unknown = set(params) - set(F.DENOISE_DEFAULTS) - set(F.DENOISE_TEMPORAL_DEFAULTS) - set(F.DENOISE_GRADIENT_DEFAULTS)
+    if unknown:
+        raise TypeError("unknown temporal gradient denoise parameters: %s" % sorted(unknown))
+    g = dict(F.DENOISE_GRADIENT_DEFAULTS, **{k: v for k, v in params.items() if k in F.DENOISE_GRADIENT_DEFAULTS})
+    temporal = _temporal_params({k: v for k, v in params.items() if k not in F.DENOISE_GRADIENT_DEFAULTS})
+    return F.DenoiseGradientParams(temporal, g["gradient_iterations"])
+
+
 class DenoiseHistory:
     """trb_denoise_history (DESIGN.md §4 "Temporal denoising"): the per-pixel history and frame snapshot of one scene's temporal
     denoise. Empty when created and after reset(); close() (or the scene's close) releases it."""
@@ -305,6 +314,51 @@ class Scene(_Base):
         d_in, prm = F.DenoiseInput(d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest), _denoise_params(params)
         self._check(self._lib.trb_denoise_device(self._h, C.byref(d_in), C.byref(prm), d_out, stream))
 
+    def _temporal_arrays(self, colour_a, colour_b, aovs, out, extra):
+        """The five input arrays and the output arrays of a temporal denoise, checked; extra: (name, array or True/False/None,
+        shape) of the optional outputs. Returns (ins, outs) as (name, array, shape, dtype) lists."""
+        film_shape = (self.height, self.width, 4)
+        ins = [("colour_a", colour_a, film_shape, np.float32), ("colour_b", colour_b, film_shape, np.float32),
+               ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32), ("normal_w", aovs.get("normal_w"), film_shape, np.float32),
+               ("nearest", aovs.get("nearest"), (self.height, self.width), np.uint64)]
+        outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
+        for name, a, shape, dtype in extra:
+            if a is True:
+                a = np.zeros(shape, dtype)
+            if a is not False and a is not None:
+                outs.append((name, a, shape, dtype))
+        for name, a, shape, dtype in ins + outs:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        return ins, outs
+
+    def denoise_temporal_gradient(self, history, colour_a, colour_b, aovs, seed, out=None, motion=False, history_length=False, lam=False,
+                                  **params):
+        """trb_denoise_temporal_gradient (DESIGN.md §4 "Temporal gradients"): denoise_temporal with temporal gradients. `seed` seeds
+        this frame's gradient samples (render_denoised_temporal passes the frame's seed). params: denoise_temporal's plus
+        gradient_iterations (trb_denoise_gradient_params.iterations, 0-6, default 3). Returns the denoised RGBW film, or a tuple of it
+        with motion, history_length and the (height, width) float32 per-pixel lambda, in that order, where asked for."""
+        h, w = self.height, self.width
+        ins, outs = self._temporal_arrays(colour_a, colour_b, aovs, out,
+                                          [("motion", motion, (h, w, 2), np.float32), ("history_length", history_length, (h, w), np.uint32),
+                                           ("lambda", lam, (h, w), np.float32)])
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseInput(*(a.ctypes.data for _, a, _, _ in ins)), _gradient_params(params)
+        o = F.DenoiseGradientOutput(*(got[k].ctypes.data if k in got else None for k in ("out", "motion", "history_length", "lambda")))
+        self._check(self._lib.trb_denoise_temporal_gradient(self._h, history._h, C.byref(d_in), C.byref(prm), seed % (1 << 32), C.byref(o)))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_temporal_gradient_device(self, history, d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest, seed, d_out, d_motion=None,
+                                         d_history_length=None, d_lambda=None, stream=None, **params):
+        """trb_denoise_temporal_gradient_device: denoise_temporal_device's pointers plus d_lambda (height*width float32, 4-byte
+        aligned, or None); enqueued on `stream`. params as for denoise_temporal_gradient."""
+        d_in, prm = F.DenoiseInput(d_colour_a, d_colour_b, d_albedo, d_normal, d_nearest), _gradient_params(params)
+        o = F.DenoiseGradientOutput(d_out, d_motion, d_history_length, d_lambda)
+        self._check(self._lib.trb_denoise_temporal_gradient_device(self._h, history._h, C.byref(d_in), C.byref(prm), seed % (1 << 32),
+                                                                   C.byref(o), stream))
+
     def denoise_temporal(self, history, colour_a, colour_b, aovs, out=None, motion=False, history_length=False, **params):
         """trb_denoise_temporal (DESIGN.md §4 "Temporal denoising"): denoise's inputs, rendered at the scene's current frame, with the
         DenoiseHistory `history`, which it reads and then holds this frame. params: denoise's plus max_history, depth_tolerance and
@@ -346,10 +400,11 @@ class Scene(_Base):
         o = F.DenoiseTemporalOutput(d_out, d_motion, d_history_length)
         self._check(self._lib.trb_denoise_temporal_device(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o), stream))
 
-    def render_denoised_temporal(self, history, spp=0, seed=1, current_frame=0, denoise=None, **kw):
+    def render_denoised_temporal(self, history, spp=0, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
         """render_denoised for frame `current_frame` of an animation, denoised with `history` (denoise_temporal; the dict `denoise`
         holds its parameters). The two halves are rendered with seed (seed + current_frame) mod 2^32, so that consecutive frames draw
-        independent samples (a frame's radiance is a pure function of scene, seed, pixel and sample). Returns render_denoised's tuple."""
+        independent samples (a frame's radiance is a pure function of scene, seed, pixel and sample). With `gradients`, the frame is
+        denoised by denoise_temporal_gradient with that frame seed. Returns render_denoised's tuple."""
         frame_seed = (seed + current_frame) % (1 << 32)
         n = 1
         while n < (spp or self.spp):
@@ -364,7 +419,10 @@ class Scene(_Base):
         kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
         b, _, st_b = self.render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
                                      sample_count=half, seed=frame_seed, current_frame=current_frame, **kw)
-        out = self.denoise_temporal(history, a, b, aovs, **(denoise or {}))
+        if gradients:
+            out = self.denoise_temporal_gradient(history, a, b, aovs, frame_seed, **(denoise or {}))
+        else:
+            out = self.denoise_temporal(history, a, b, aovs, **(denoise or {}))
         return out, a + b, aovs, (st_a, st_b)
 
     def render_denoised(self, spp=0, denoise=None, **kw):

@@ -2967,9 +2967,17 @@ struct trb_denoise_history {
     float cam_inv[16] = {}, tan_fov = 0;
     uint32_t n_instances = 0;
     uint64_t generation = 0;
+    // temporal gradients: two record sets and the per-call stratum buffers (trb::GrBuffers) for gr_capacity strata; the records of
+    // the read set are valid only after a gradient call, and were written at gr_seed, gr_shutter_open and gr_cam_mat
+    void* d_gr = nullptr;
+    size_t gr_capacity = 0;
+    bool gr_valid = false;
+    uint32_t gr_seed = 0;
+    float gr_shutter_open = 0, gr_cam_mat[16] = {};
     ~trb_denoise_history() {
         if (d_px) cudaFree(d_px);
         if (d_mats) cudaFree(d_mats);
+        if (d_gr) cudaFree(d_gr);
     }
     trb::DnHistory set(uint32_t k) const {
         float4* base = static_cast<float4*>(d_px) + (size_t)k * 3 * px_capacity;
@@ -2995,7 +3003,7 @@ trb_status trb_denoise_history_destroy(trb_denoise_history* h) {
 
 trb_status trb_denoise_history_reset(trb_denoise_history* h) {
     if (!h) return fail(TRB_INVALID_ARG, "null history");
-    h->has_prev = false; h->bound = false; h->width = h->height = 0;
+    h->has_prev = false; h->bound = false; h->width = h->height = 0; h->gr_valid = false;
     return TRB_OK;
 }
 
@@ -3054,9 +3062,109 @@ trb_status history_alloc(void** p, size_t bytes, const char* what) {
     return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 
-// k_dn_temporal and the a-trous launches on `st`, then the history's switch to the set just written
+// The gradient buffers of G strata, carved out of one allocation at 256-byte offsets: two record sets (64 B per stratum each), the
+// winner slots, the re-shade rays and radiance, the record query and illumination rays, their hits and radiance, two (delta, m, c)
+// buffers, the stratum guides and lambda: 456 B per stratum
+struct GrBuffers {
+    float4* rec[2];
+    unsigned long long* slot;
+    trb_illum_ray* reshade;
+    float* reshade_rgb;
+    trb_query_ray* qrays;
+    trb_illum_ray* irays;
+    trb_intersection* hits;
+    float* rgb;
+    float4* dm[2];
+    float4* guide;
+    float* lam;
+};
+size_t gr_layout(size_t G, char* base, GrBuffers* b) {
+    size_t off = 0;
+    auto take = [&](size_t bytes) { char* p = base ? base + off : nullptr; off += (bytes + 255) & ~(size_t)255; return p; };
+    char* r0 = take(G * 64); char* r1 = take(G * 64); char* sl = take(G * 8); char* rs = take(G * sizeof(trb_illum_ray));
+    char* rsc = take(G * 12); char* q = take(G * sizeof(trb_query_ray)); char* il = take(G * sizeof(trb_illum_ray));
+    char* hi = take(G * sizeof(trb_intersection)); char* rgb = take(G * 12); char* d0 = take(G * 16); char* d1 = take(G * 16);
+    char* gd = take(G * 16); char* lm = take(G * 4);
+    if (b) *b = GrBuffers{{reinterpret_cast<float4*>(r0), reinterpret_cast<float4*>(r1)}, reinterpret_cast<unsigned long long*>(sl),
+                          reinterpret_cast<trb_illum_ray*>(rs), reinterpret_cast<float*>(rsc), reinterpret_cast<trb_query_ray*>(q),
+                          reinterpret_cast<trb_illum_ray*>(il), reinterpret_cast<trb_intersection*>(hi), reinterpret_cast<float*>(rgb),
+                          {reinterpret_cast<float4*>(d0), reinterpret_cast<float4*>(d1)}, reinterpret_cast<float4*>(gd), reinterpret_cast<float*>(lm)};
+    return off;
+}
+
+// A gradient call's own arguments (trb_denoise_temporal_gradient*)
+struct GradCall {
+    uint32_t iterations;
+    uint32_t seed;
+    float* lambda;   // per-pixel output, may be null
+};
+
+// Steps 1-2 of "Temporal gradients": re-shade the read set's records in this frame, reconstruct lambda on the stratum grid into b.lam
+trb_status gradient_lambda(trb_scene* s, trb_denoise_history* h, const GradCall& gc, const trb::DnTemporal& tp, const GrBuffers& b,
+                           const float* mats_rd, const trb_denoise_input& in, bool valid, cudaStream_t st) {
+    const uint32_t W = s->film.width, H = s->film.height, gw = (W + 2) / 3, gh = (H + 2) / 3, S = gw * gh;
+    const unsigned grid = (unsigned)std::min<size_t>((S + 255) / 256, (size_t)s->sm_count * 8);
+    trb::GrFrame f{};
+    std::memcpy(f.cam_mat, s->ds.cam.cam_mat, 64);
+    std::memcpy(f.cam_inv, s->cam_inv, 64);
+    f.tan_cur = s->ds.cam.scaling[0];
+    f.x0 = tp.x0; f.x1 = tp.x1; f.y0 = tp.y0; f.y1 = tp.y1; f.w = (float)W; f.h = (float)H;
+    f.width = W; f.height = H; f.gw = gw; f.gh = gh;
+    f.n_cur = tp.n_cur; f.n_prev = valid ? tp.n_prev : 0u;
+    f.cam_same = std::memcmp(h->gr_cam_mat, s->ds.cam.cam_mat, 64) == 0 ? 1u : 0u;
+    f.dt = s->shutter_open - h->gr_shutter_open;
+    f.depth_tolerance = tp.depth_tolerance; f.normal_threshold = tp.normal_threshold;
+    const float4* rec = b.rec[h->cur];
+    const unsigned long long* nearest = reinterpret_cast<const unsigned long long*>(in.nearest);
+    CU(cudaMemsetAsync(b.slot, 0xff, (size_t)S * 8, st));
+    if (valid) {
+        trb::k_gr_project<<<grid, 256, 0, st>>>(f, rec, s->d_instances, nearest, b.slot);
+        g_launches++;
+    }
+    trb::k_gr_resolve<<<grid, 256, 0, st>>>(f, rec, s->d_instances, mats_rd, b.slot, reinterpret_cast<const float4*>(in.normal_w), nearest, b.reshade,
+                                            b.guide);
+    g_launches++;
+    CU(cudaGetLastError());
+    if (valid) {
+        const trb_status r = illum_passes(s, S, b.reshade, 1, h->gr_seed, b.reshade_rgb, TRB_QUERY_CLAMP, nullptr, st);
+        if (r != TRB_OK) return r;
+    } else {
+        CU(cudaMemsetAsync(b.reshade_rgb, 0, (size_t)S * 12, st));
+    }
+    trb::k_gr_delta<<<grid, 256, 0, st>>>(S, rec, b.slot, b.reshade_rgb, b.dm[0], gc.iterations == 0 ? b.lam : nullptr);
+    g_launches++;
+    for (uint32_t i = 0; i < gc.iterations; ++i) {
+        const bool last = i + 1 == gc.iterations;
+        trb::k_gr_atrous<<<grid, 256, 0, st>>>(gw, gh, 1 << i, tp.normal_threshold, b.guide, b.dm[i & 1], last ? nullptr : b.dm[(i + 1) & 1],
+                                               last ? b.lam : nullptr);
+        g_launches++;
+    }
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// Step 4: this frame's samples into the write set's records
+trb_status gradient_record(trb_scene* s, const GradCall& gc, const GrBuffers& b, uint32_t wr, cudaStream_t st) {
+    const uint32_t W = s->film.width, H = s->film.height, gw = (W + 2) / 3, gh = (H + 2) / 3, S = gw * gh;
+    const unsigned grid = (unsigned)std::min<size_t>((S + 255) / 256, (size_t)s->sm_count * 8);
+    if (s->ds.has_anim) trb::k_gr_record<true><<<grid, 256, 0, st>>>(s->ds, gw, gh, gc.seed, b.qrays, b.irays);
+    else trb::k_gr_record<false><<<grid, 256, 0, st>>>(s->ds, gw, gh, gc.seed, b.qrays, b.irays);
+    g_launches++;
+    CU(cudaGetLastError());
+    trb_status r = query_passes(s, S, b.qrays, b.hits, nullptr, 0u, nullptr, st);
+    if (r != TRB_OK) return r;
+    r = illum_passes(s, S, b.irays, 1, gc.seed, b.rgb, TRB_QUERY_CLAMP, nullptr, st);
+    if (r != TRB_OK) return r;
+    trb::k_gr_store<<<grid, 256, 0, st>>>(S, b.hits, b.irays, b.rgb, s->d_instances, b.rec[wr]);
+    g_launches++;
+    CU(cudaGetLastError());
+    return TRB_OK;
+}
+
+// k_dn_temporal (or, with gc, the gradient steps around k_dn_temporal_grad) and the a-trous launches on `st`, then the history's
+// switch to the set just written
 trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_input& in,
-                            const trb_denoise_temporal_output& out, cudaStream_t st) {
+                            const trb_denoise_temporal_output& out, cudaStream_t st, const GradCall* gc = nullptr) {
     const size_t npx = (size_t)prm.width * prm.height, n = s->instances.size();
     if (npx == 0) return TRB_OK;
     trb::DnScratch sc;
@@ -3085,6 +3193,14 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
         }
         h->d_mats = static_cast<float*>(p); h->mat_capacity = n;
     }
+    const size_t S = (size_t)((prm.width + 2) / 3) * ((prm.height + 2) / 3);
+    if (gc && h->gr_capacity < S) { // like the pixel sets: bound to one film size, so the records are not kept
+        void* p = nullptr;
+        r = history_alloc(&p, gr_layout(S, nullptr, nullptr), "denoise history gradients");
+        if (r != TRB_OK) return r;
+        if (h->d_gr) { CU(cudaDeviceSynchronize()); cudaFree(h->d_gr); }
+        h->d_gr = p; h->gr_capacity = S; h->gr_valid = false;
+    }
     // the current frame, and the snapshot the read set was written at
     std::memcpy(tp.px_to_cam, s->ds.cam.px_to_cam, 64);
     std::memcpy(tp.cam_mat, s->ds.cam.cam_mat, 64);
@@ -3106,14 +3222,36 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
                          cudaMemcpyDeviceToDevice, st));
     float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
     const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
-    trb::k_dn_temporal<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
-                                               reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
-                                               reinterpret_cast<const unsigned long long*>(in.nearest), sc, rgbw, s->d_instances, mats_rd,
-                                               h->set(rd), h->set(wr), reinterpret_cast<float2*>(out.motion), out.history_length);
-    g_launches++;
-    CU(cudaGetLastError());
-    r = denoise_atrous(prm, sc, rgbw, st);
-    if (r != TRB_OK) return r;
+    if (!gc) {
+        trb::k_dn_temporal<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
+                                                   reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                                   reinterpret_cast<const unsigned long long*>(in.nearest), sc, rgbw, s->d_instances, mats_rd,
+                                                   h->set(rd), h->set(wr), reinterpret_cast<float2*>(out.motion), out.history_length);
+        g_launches++;
+        CU(cudaGetLastError());
+        r = denoise_atrous(prm, sc, rgbw, st);
+        if (r != TRB_OK) return r;
+        h->gr_valid = false;
+    } else {
+        GrBuffers b;
+        gr_layout(h->gr_capacity, static_cast<char*>(h->d_gr), &b);
+        const bool valid = tp.has_prev && h->gr_valid;
+        r = gradient_lambda(s, h, *gc, tp, b, mats_rd, in, valid, st);
+        if (r != TRB_OK) return r;
+        trb::k_dn_temporal_grad<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
+                                                        reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                                        reinterpret_cast<const unsigned long long*>(in.nearest), sc, rgbw, s->d_instances, mats_rd,
+                                                        h->set(rd), h->set(wr), reinterpret_cast<float2*>(out.motion), out.history_length, b.lam,
+                                                        (uint32_t)((prm.width + 2) / 3), gc->lambda);
+        g_launches++;
+        CU(cudaGetLastError());
+        r = denoise_atrous(prm, sc, rgbw, st);
+        if (r != TRB_OK) return r;
+        r = gradient_record(s, *gc, b, wr, st);
+        if (r != TRB_OK) return r;
+        h->gr_valid = true; h->gr_seed = gc->seed; h->gr_shutter_open = s->shutter_open;
+        std::memcpy(h->gr_cam_mat, s->ds.cam.cam_mat, 64);
+    }
     h->cur = wr; h->has_prev = true; h->bound = true; h->width = s->film.width; h->height = s->film.height;
     std::memcpy(h->cam_inv, s->cam_inv, 64);
     h->tan_fov = s->ds.cam.scaling[0];
@@ -3163,6 +3301,85 @@ trb_status trb_denoise_temporal(trb_scene* s, trb_denoise_history* h, const trb_
     CU(cudaMemcpy(out->rgbw, d_rgbw.p, fb, cudaMemcpyDeviceToHost));
     if (out->motion) CU(cudaMemcpy(out->motion, d_motion.p, npx * sizeof(float2), cudaMemcpyDeviceToHost));
     if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return TRB_OK;
+}
+
+namespace {
+// trb_denoise_gradient_params, NULL meaning the defaults; checked before anything else
+trb_status gradient_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_input* in, const trb_denoise_gradient_params* params,
+                          const trb_denoise_gradient_output* out, trb::DnParams& prm, trb::DnTemporal& tp, GradCall& gc) {
+    const uint32_t iterations = params ? params->iterations : 3u;
+    trb_status r = temporal_params(params ? &params->temporal : nullptr, prm, tp);
+    if (r != TRB_OK) return r;
+    if (iterations > 6) return fail(TRB_INVALID_ARG, "temporal gradient iterations must be 0 to 6");
+    if (!out) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_denoise_temporal_output o{out->rgbw, out->motion, out->history_length};
+    r = temporal_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp);
+    if (r != TRB_OK) return r;
+    if (out->lambda) {
+        const size_t npx = (size_t)s->film.width * s->film.height;
+        const std::pair<const void*, size_t> others[8] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
+                                                          {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                                                          {in->nearest, npx * sizeof(uint64_t)}, {out->rgbw, npx * sizeof(float4)},
+                                                          {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
+        for (const auto& [p, bytes] : others)
+            if (spans_overlap(out->lambda, npx * sizeof(float), p, bytes)) return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
+    }
+    gc.iterations = iterations;
+    gc.lambda = out->lambda;
+    return TRB_OK;
+}
+} // namespace
+
+trb_status trb_denoise_temporal_gradient_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_input* d_in,
+                                                const trb_denoise_gradient_params* params, uint32_t seed, const trb_denoise_gradient_output* d_out,
+                                                void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    const trb_status r = gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
+          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
+        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
+        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->lambda)) & 3u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and lambda 4-byte");
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const trb_denoise_temporal_output o{d_out->rgbw, d_out->motion, d_out->history_length};
+    return temporal_enqueue(s, h, prm, tp, *d_in, o, static_cast<cudaStream_t>(stream), &gc);
+}
+
+trb_status trb_denoise_temporal_gradient(trb_scene* s, trb_denoise_history* h, const trb_denoise_input* in, const trb_denoise_gradient_params* params,
+                                         uint32_t seed, const trb_denoise_gradient_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    trb_status r = gradient_check(s, h, in, params, out, prm, tp, gc);
+    if (r != TRB_OK) return r;
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_rgbw, d_motion, d_len, d_lam;
+    for (auto [d, hp, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
+                                {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
+        CU(cudaMalloc(&d->p, bytes));
+        CU(cudaMemcpy(d->p, hp, bytes, cudaMemcpyHostToDevice));
+    }
+    CU(cudaMalloc(&d_rgbw.p, fb));
+    if (out->motion) CU(cudaMalloc(&d_motion.p, npx * sizeof(float2)));
+    if (out->history_length) CU(cudaMalloc(&d_len.p, npx * sizeof(uint32_t)));
+    if (out->lambda) CU(cudaMalloc(&d_lam.p, npx * sizeof(float)));
+    gc.lambda = static_cast<float*>(d_lam.p);
+    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
+                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
+    const trb_denoise_temporal_output d_out{static_cast<float*>(d_rgbw.p), static_cast<float*>(d_motion.p), static_cast<uint32_t*>(d_len.p)};
+    r = temporal_enqueue(s, h, prm, tp, d_in, d_out, 0, &gc);
+    if (r != TRB_OK) { cudaDeviceSynchronize(); return r; }
+    CU(cudaMemcpy(out->rgbw, d_rgbw.p, fb, cudaMemcpyDeviceToHost));
+    if (out->motion) CU(cudaMemcpy(out->motion, d_motion.p, npx * sizeof(float2), cudaMemcpyDeviceToHost));
+    if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (out->lambda) CU(cudaMemcpy(out->lambda, d_lam.p, npx * sizeof(float), cudaMemcpyDeviceToHost));
     return TRB_OK;
 }
 

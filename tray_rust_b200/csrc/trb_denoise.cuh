@@ -194,15 +194,24 @@ constexpr size_t DN_HISTORY_BYTES_PER_PIXEL = 3 * sizeof(float4);
 // k_dn_prepare's reads and writes, plus the reprojected history blended into (ē, v) before the a-trous iterations (1 + N launches as
 // for trb_denoise). mat_prev: the snapshot's object -> world matrices, 16 floats per instance; the current inverses are read from the
 // frame's instance records.
-__global__ void __launch_bounds__(256) k_dn_temporal(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ ca,
-                                                     const float4* __restrict__ cb, const float4* __restrict__ alb, const float4* __restrict__ nrm,
-                                                     const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
-                                                     const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory hin,
-                                                     const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen) {
+// The body of k_dn_temporal (GRAD false) and k_dn_temporal_grad (GRAD true: step 4 shortens the history by the pixel's stratum's
+// lambda, include/trb.h "Temporal gradients", and lam_out receives it). lam_s: S lambdas on the stratum grid of gw columns.
+template <bool GRAD>
+__device__ __forceinline__ void dn_temporal_px(const DnParams prm, const DnTemporal& tp, const float4* __restrict__ ca, const float4* __restrict__ cb,
+                                               const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                               const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
+                                               const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory hin,
+                                               const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen,
+                                               const float* __restrict__ lam_s, uint32_t gw, float* __restrict__ lam_out) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= prm.width || y >= prm.height) return;
     const int i = y * prm.width + x;
     const float qnan = __int_as_float(0x7fffffff);
+    float lam = 0.0f;
+    if (GRAD) {
+        lam = lam_s[(uint32_t)(y / 3) * gw + (uint32_t)(x / 3)];
+        if (lam_out) lam_out[i] = lam;
+    }
     const float4 A = ca[i], B = cb[i];
     const float W = A.w + B.w;
     if (W <= 0.0f) {
@@ -290,7 +299,14 @@ __global__ void __launch_bounds__(256) k_dn_temporal(const DnParams prm, const _
     }
     // 4: blend
     uint32_t np = 1;
-    if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    if (GRAD) {
+        if (S > 0.0f) {
+            const uint32_t len_adj = (uint32_t)floorf((1.0f - lam) * (float)len_prev);
+            np = len_adj + 1 < tp.max_history ? len_adj + 1 : tp.max_history;
+        }
+    } else {
+        if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    }
     if (np > 1) {
         ha0 = ha0 / S; ha1 = ha1 / S; ha2 = ha2 / S;
         hb0 = hb0 / S; hb1 = hb1 / S; hb2 = hb2 / S;
@@ -318,6 +334,231 @@ __global__ void __launch_bounds__(256) k_dn_temporal(const DnParams prm, const _
     }
     if (motion) motion[i] = make_float2(mx == mx ? mx : qnan, my == my ? my : qnan);
     if (hlen) hlen[i] = np;
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ ca,
+                                                     const float4* __restrict__ cb, const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                     const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
+                                                     const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory hin,
+                                                     const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen) {
+    dn_temporal_px<false>(prm, tp, ca, cb, alb, nrm, nearest, sc, out, inst, mat_prev, hin, hout, motion, hlen, nullptr, 0u, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal_grad(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ ca,
+                                                          const float4* __restrict__ cb, const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                          const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
+                                                          const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory hin,
+                                                          const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen,
+                                                          const float* __restrict__ lam_s, uint32_t gw, float* __restrict__ lam_out) {
+    dn_temporal_px<true>(prm, tp, ca, cb, alb, nrm, nearest, sc, out, inst, mat_prev, hin, hout, motion, hlen, lam_s, gw, lam_out);
+}
+
+// ---- temporal gradients (trb_denoise_temporal_gradient*, include/trb.h "Temporal gradients") --------------------------------------
+// One gradient record per 3x3 stratum, 64 bytes: (p_o, inst bits) (o, time) (d, key bits) (L, 0, 0, 0); inst == TRB_MISS: none
+struct GrRecords {
+    float4* r;       // 4 float4 per stratum
+};
+constexpr uint32_t GR_STRATUM = 3;
+constexpr uint32_t GR_PICK_STREAM = 0xfffffffeu;
+
+// The current frame (camera at shutter-open, film size, stratum grid) and the snapshot the records were written at
+struct GrFrame {
+    float cam_mat[16], cam_inv[16];
+    float tan_cur, x0, x1, y0, y1, w, h;
+    uint32_t width, height, gw, gh;
+    uint32_t n_cur, n_prev;
+    uint32_t cam_same;      // the current cam_mat is bit-identical to the snapshot's
+    float dt;               // shutter_open_cur - shutter_open_prev
+    float depth_tolerance, normal_threshold;
+};
+
+__device__ __forceinline__ float gr_lum(float r, float g, float b) { return 0.2126f * r + 0.7152f * g + 0.0722f * b; }
+
+// Step 1, forward projection: record j of the read set to the raster of the current frame; the winner of each target stratum is the
+// smallest (float bits of the distance << 32 | j)
+__global__ void __launch_bounds__(256) k_gr_project(const __grid_constant__ GrFrame f, const float4* __restrict__ rec,
+                                                    const DInstance* __restrict__ inst, const unsigned long long* __restrict__ nearest,
+                                                    unsigned long long* __restrict__ slot) {
+    const uint32_t S = f.gw * f.gh;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < S; j += gridDim.x * blockDim.x) {
+        const float4 r0 = rec[4 * (size_t)j];
+        const uint32_t id = __float_as_uint(r0.w);
+        if (id == TRB_MISS || id >= f.n_cur || id >= f.n_prev) continue;
+        const f3 pw = xf_point(inst[id].mat, mk(r0.x, r0.y, r0.z));
+        const f3 q = xf_point(f.cam_inv, pw);
+        if (!(q.z > 0.0f)) continue;
+        const float X = q.x / (q.z * f.tan_cur), Y = q.y / (q.z * f.tan_cur);
+        const float rx = (X - f.x0) / (f.x1 - f.x0) * f.w, ry = (Y - f.y1) / (f.y0 - f.y1) * f.h;
+        if (!(rx >= 0.0f && rx < f.w && ry >= 0.0f && ry < f.h)) continue;
+        const uint32_t px = (uint32_t)rx, py = (uint32_t)ry;
+        if (px >= f.width || py >= f.height) continue;
+        const unsigned long long key = nearest[(size_t)py * f.width + px];
+        if ((uint32_t)key != id) continue;
+        const float z = __uint_as_float((uint32_t)(key >> 32));
+        const f3 o = xf_point(f.cam_mat, splat(0.0f));
+        const f3 v = mk(pw.x - o.x, pw.y - o.y, pw.z - o.z);
+        const float dist = sqrtf(v.x * v.x + v.y * v.y + v.z * v.z);
+        if (!(fabsf(z - dist) <= f.depth_tolerance * z)) continue;
+        const uint32_t t = (py / GR_STRATUM) * f.gw + px / GR_STRATUM;
+        atomicMin(slot + t, ((unsigned long long)__float_as_uint(dist) << 32) | j);
+    }
+}
+
+// Step 1, the winner's illumination ray (the recorded one when camera and instance did not move, else from the camera to p_w'), and
+// each stratum's guide for the reconstruction: its representative pixel's unit normal (0 if none) and instance
+__global__ void __launch_bounds__(256) k_gr_resolve(const __grid_constant__ GrFrame f, const float4* __restrict__ rec, const DInstance* __restrict__ inst,
+                                                    const float* __restrict__ mat_prev, const unsigned long long* __restrict__ slot,
+                                                    const float4* __restrict__ nrm, const unsigned long long* __restrict__ nearest,
+                                                    trb_illum_ray* __restrict__ rays, float4* __restrict__ guide) {
+    const uint32_t S = f.gw * f.gh;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < S; t += gridDim.x * blockDim.x) {
+        const uint32_t sx = t % f.gw, sy = t / f.gw;
+        const uint32_t rx = min(sx * GR_STRATUM + 1, f.width - 1), ry = min(sy * GR_STRATUM + 1, f.height - 1);
+        const size_t rp = (size_t)ry * f.width + rx;
+        const float4 nw = nrm[rp];
+        const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+        const float l2 = m0 * m0 + m1 * m1 + m2 * m2;
+        float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+        if (dn_finite(l2) && l2 != 0.0f) {
+            const float l = sqrtf(l2);
+            n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+        }
+        guide[t] = make_float4(n0, n1, n2, __uint_as_float((uint32_t)nearest[rp]));
+        const unsigned long long w = slot[t];
+        trb_illum_ray r;
+        if (w == ~0ull) { // no winner: a ray that hits nothing
+            r.o[0] = r.o[1] = r.o[2] = 0.0f;
+            r.d[0] = r.d[1] = r.d[2] = 0.5773502691896258f;
+            r.min_t = 0.0f; r.max_t = 0.0f; r.time = 0.0f; r.key = 0u; r.sample = 0u;
+        } else {
+            const uint32_t j = (uint32_t)w;
+            const float4 r0 = rec[4 * (size_t)j], r1 = rec[4 * (size_t)j + 1], r2 = rec[4 * (size_t)j + 2];
+            const uint32_t id = __float_as_uint(r0.w);
+            bool same = f.cam_same != 0u;
+            const float* mc = inst[id].mat;
+            const float* mp = mat_prev + 16 * (size_t)id;
+            for (int k = 0; k < 16 && same; ++k) same = __float_as_uint(mc[k]) == __float_as_uint(mp[k]);
+            if (same) {
+                r.o[0] = r1.x; r.o[1] = r1.y; r.o[2] = r1.z;
+                r.d[0] = r2.x; r.d[1] = r2.y; r.d[2] = r2.z;
+            } else {
+                const f3 pw = xf_point(mc, mk(r0.x, r0.y, r0.z));
+                const f3 o = xf_point(f.cam_mat, splat(0.0f));
+                const f3 d = unit(mk(pw.x - o.x, pw.y - o.y, pw.z - o.z));
+                r.o[0] = o.x; r.o[1] = o.y; r.o[2] = o.z;
+                r.d[0] = d.x; r.d[1] = d.y; r.d[2] = d.z;
+            }
+            r.min_t = 0.0f; r.max_t = finf();
+            r.time = r1.w + f.dt;
+            r.key = __float_as_uint(r2.w); r.sample = 0u;
+        }
+        r.pad = 0u;
+        rays[t] = r;
+    }
+}
+
+// Step 1, each stratum's (delta, m, c): the re-shaded luminance against the recorded one where there is a winner, else 0
+__global__ void __launch_bounds__(256) k_gr_delta(uint32_t S, const float4* __restrict__ rec, const unsigned long long* __restrict__ slot,
+                                                  const float* __restrict__ rgb, float4* __restrict__ dm, float* __restrict__ lam_s) {
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < S; t += gridDim.x * blockDim.x) {
+        const unsigned long long w = slot[t];
+        float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (w != ~0ull) {
+            const float lc = gr_lum(rgb[3 * (size_t)t], rgb[3 * (size_t)t + 1], rgb[3 * (size_t)t + 2]);
+            const float lp = rec[4 * (size_t)(uint32_t)w + 3].x;
+            v = make_float4(lc - lp, lc > lp ? lc : lp, 1.0f, 0.0f);
+        }
+        dm[t] = v;
+        if (lam_s) lam_s[t] = v.z > 0.0f && v.y > 0.0f ? fminf(1.0f, fabsf(v.x) / v.y) : 0.0f; // no a-trous pass
+    }
+}
+
+// Step 2, one a-trous pass at a step of s strata over (delta, m, c); the last one (lam_s non-null) writes lambda instead
+__global__ void __launch_bounds__(256) k_gr_atrous(uint32_t gw, uint32_t gh, int s, float normal_threshold, const float4* __restrict__ guide,
+                                                   const float4* __restrict__ dm_in, float4* __restrict__ dm_out, float* __restrict__ lam_s) {
+    const uint32_t S = gw * gh;
+    const float h[5] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f};
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < S; t += gridDim.x * blockDim.x) {
+        const int x = (int)(t % gw), y = (int)(t / gw);
+        const float4 gp = guide[t];
+        const bool p_nrm = gp.x != 0.0f || gp.y != 0.0f || gp.z != 0.0f;
+        float W = 0.0f, sd = 0.0f, sm = 0.0f;
+#pragma unroll
+        for (int dy = -2; dy <= 2; ++dy) {
+            const int qy = y + s * dy;
+            if (qy < 0 || qy >= (int)gh) continue;
+#pragma unroll
+            for (int dx = -2; dx <= 2; ++dx) {
+                const int qx = x + s * dx;
+                if (qx < 0 || qx >= (int)gw) continue;
+                const uint32_t q = (uint32_t)qy * gw + (uint32_t)qx;
+                const float4 v = dm_in[q];
+                if (!(v.z > 0.0f)) continue;
+                if (q != t) {
+                    const float4 gq = guide[q];
+                    if (__float_as_uint(gq.w) != __float_as_uint(gp.w)) continue;
+                    const bool q_nrm = gq.x != 0.0f || gq.y != 0.0f || gq.z != 0.0f;
+                    if (q_nrm != p_nrm) continue;
+                    if (p_nrm && !(gp.x * gq.x + gp.y * gq.y + gp.z * gq.z >= normal_threshold)) continue;
+                }
+                const float w = h[dx + 2] * h[dy + 2];
+                W = W + w;
+                sd = sd + w * v.x;
+                sm = sm + w * v.y;
+            }
+        }
+        float4 o = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (W > 0.0f) o = make_float4(sd / W, sm / W, 1.0f, 0.0f);
+        if (lam_s) lam_s[t] = o.z > 0.0f && o.y > 0.0f ? fminf(1.0f, fabsf(o.x) / o.y) : 0.0f;
+        else dm_out[t] = o;
+    }
+}
+
+// Step 4, this frame's samples: one pixel per stratum picked by the draw (seed, s, GR_PICK_STREAM, 0), its camera ray as
+// k_camera_rays generates sample 0 of 1, as a query ray (for the hit) and an illumination ray (for L)
+template <bool ANIM>
+__global__ void __launch_bounds__(256) k_gr_record(const __grid_constant__ DScene sc, uint32_t gw, uint32_t gh, uint32_t seed,
+                                                   trb_query_ray* __restrict__ qrays, trb_illum_ray* __restrict__ irays) {
+    const uint32_t S = gw * gh, W = (uint32_t)sc.width, H = (uint32_t)sc.height;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < S; t += gridDim.x * blockDim.x) {
+        const uint32_t sx = t % gw, sy = t / gw;
+        const uint32_t cw = min(GR_STRATUM, W - sx * GR_STRATUM), ch = min(GR_STRATUM, H - sy * GR_STRATUM);
+        const uint32_t k = rng_absorb(rng_absorb(rng_absorb(rng_seed(seed), t), GR_PICK_STREAM), 0u) % (cw * ch);
+        const uint32_t px = sx * GR_STRATUM + k % cw, py = sy * GR_STRATUM + k / cw, pixel = py * W + px;
+        const PixelStreams ps = pixel_streams(seed, pixel);
+        const uint32_t ip = permute_index(0u, 1u, ps.kpos);
+        const float fx = ld_vdc(ip, ps.scr0) + (float)px, fy = ld_sobol(ip, ps.scr1) + (float)py;
+        const float tm = ld_vdc(permute_index(0u, 1u, ps.ktime), ps.scrt);
+        Ray r;
+        const float time = camera_ray<ANIM>(sc, fx, fy, tm, r);
+        trb_query_ray q;
+        q.o[0] = r.o.x; q.o[1] = r.o.y; q.o[2] = r.o.z; q.d[0] = r.d.x; q.d[1] = r.d.y; q.d[2] = r.d.z;
+        q.min_t = r.tmin; q.max_t = r.tmax; q.time = time; q.pad[0] = q.pad[1] = q.pad[2] = 0u;
+        qrays[t] = q;
+        trb_illum_ray l;
+        l.o[0] = r.o.x; l.o[1] = r.o.y; l.o[2] = r.o.z; l.d[0] = r.d.x; l.d[1] = r.d.y; l.d[2] = r.d.z;
+        l.min_t = r.tmin; l.max_t = r.tmax; l.time = time; l.key = pixel; l.sample = 0u; l.pad = 0u;
+        irays[t] = l;
+    }
+}
+
+// Step 4, the records of the write set: the hit's instance and object-space point (shutter-open inverse), the ray and L
+__global__ void __launch_bounds__(256) k_gr_store(uint32_t S, const trb_intersection* __restrict__ hits, const trb_illum_ray* __restrict__ irays,
+                                                  const float* __restrict__ rgb, const DInstance* __restrict__ inst, float4* __restrict__ rec) {
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < S; t += gridDim.x * blockDim.x) {
+        const trb_intersection& hit = hits[t];
+        const trb_illum_ray& l = irays[t];
+        float4* o = rec + 4 * (size_t)t;
+        if (hit.inst == TRB_MISS) {
+            o[0] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(TRB_MISS));
+            continue;
+        }
+        const f3 po = xf_point(inst[hit.inst].inv, mk(hit.p[0], hit.p[1], hit.p[2]));
+        o[0] = make_float4(po.x, po.y, po.z, __uint_as_float(hit.inst));
+        o[1] = make_float4(l.o[0], l.o[1], l.o[2], l.time);
+        o[2] = make_float4(l.d[0], l.d[1], l.d[2], __uint_as_float(l.key));
+        o[3] = make_float4(gr_lum(rgb[3 * (size_t)t], rgb[3 * (size_t)t + 1], rgb[3 * (size_t)t + 2]), 0.0f, 0.0f, 0.0f);
+    }
 }
 
 } // namespace trb

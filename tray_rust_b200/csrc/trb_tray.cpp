@@ -1,7 +1,7 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
-//            [--denoise-temporal]
+//            [--denoise-temporal [--temporal-gradients]]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
 //
@@ -17,7 +17,8 @@
 // Extensions over the reference: --seed, --spp and --device mean what they mean for trb_worker; --denoise renders every frame as two
 // half-sample renders with AOVs and writes the denoised image (trb_denoise; single node, path integrator, 2 spp or more, refused
 // before anything renders otherwise: the wire format carries no AOVs); --denoise-temporal renders the frames in order with one
-// history and seed (S + frame) mod 2^32, denoising each with trb_denoise_temporal (refused where --denoise is, and with --denoise); a worker address is host[:port],
+// history and seed (S + frame) mod 2^32, denoising each with trb_denoise_temporal (refused where --denoise is, and with --denoise);
+// --temporal-gradients, only with --denoise-temporal, denoises with trb_denoise_temporal_gradient at the frame's seed; a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -41,7 +42,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise | --denoise-temporal]\n"
+    "             [--denoise | --denoise-temporal [--temporal-gradients]]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -60,6 +61,8 @@ const char* USAGE =
     "                          image. Single node only, path integrator, at least 2 samples per pixel.\n"
     "  --denoise-temporal      As --denoise, accumulating each pixel's history over the frame range through the scene's motion;\n"
     "                          frame k is rendered with seed S + k.\n"
+    "  --temporal-gradients    With --denoise-temporal only: re-shade a sample of each 3x3 pixel block of the previous frame in\n"
+    "                          this one and shorten the history where the lighting changed (animated lights). Single node only.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -150,7 +153,7 @@ struct Args {
     std::vector<std::string> workers;
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
-         denoise_temporal = false;
+         denoise_temporal = false, temporal_gradients = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
 };
 
@@ -178,7 +181,7 @@ struct DenoisedFrame {
     std::vector<float> a, b, albedo, normal, out;
     std::vector<uint64_t> nearest;
     explicit DenoisedFrame(size_t npx) : a(npx * 4), b(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history = nullptr) {
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history = nullptr, bool gradients = false) {
         std::fill(a.begin(), a.end(), 0.0f); std::fill(b.begin(), b.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
@@ -189,7 +192,10 @@ struct DenoisedFrame {
         cfg.sample_first = spp / 2; cfg.flags = TRB_RENDER_NO_UPDATE;
         tray::check(trb_render_aov(s, &cfg, b.data(), &aov, nullptr));
         const trb_denoise_input in{a.data(), b.data(), albedo.data(), normal.data(), nearest.data()};
-        if (history) {
+        if (history && gradients) {
+            const trb_denoise_gradient_output o{out.data(), nullptr, nullptr, nullptr};
+            tray::check(trb_denoise_temporal_gradient(s, history, &in, nullptr, seed, &o));
+        } else if (history) {
             const trb_denoise_temporal_output o{out.data(), nullptr, nullptr};
             tray::check(trb_denoise_temporal(s, history, &in, nullptr, &o));
         } else {
@@ -227,7 +233,7 @@ int single_node(const Args& a, const OutPath& out) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (dn) {
-                if (history) dn->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history);
+                if (history) dn->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.temporal_gradients);
                 else dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(scene.handle(), dn->out.data(), img.data()));
@@ -434,15 +440,18 @@ int master_node(const Args& a, const OutPath& out) {
 } // namespace
 
 int main(int argc, char** argv) {
-    bool worker = false, denoise = false, denoise_temporal = false;
+    bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
+        temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
         denoise = denoise || std::strcmp(argv[i], "--denoise") == 0;
         denoise_temporal = denoise_temporal || std::strcmp(argv[i], "--denoise-temporal") == 0;
     }
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_temporal)
         return die("--denoise-temporal is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && temporal_gradients)
+        return die("--temporal-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -465,6 +474,7 @@ int main(int argc, char** argv) {
         else if (s == "--master") a.master = true;
         else if (s == "--denoise") a.denoise = true;
         else if (s == "--denoise-temporal") a.denoise_temporal = true;
+        else if (s == "--temporal-gradients") a.temporal_gradients = true;
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -479,6 +489,9 @@ int main(int argc, char** argv) {
     if (a.denoise && a.denoise_temporal) return die("--denoise and --denoise-temporal exclude each other: choose one");
     if (a.master && a.denoise_temporal)
         return die("--denoise-temporal is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.master && a.temporal_gradients)
+        return die("--temporal-gradients is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.temporal_gradients && !a.denoise_temporal) return die("--temporal-gradients needs --denoise-temporal");
     if (a.denoise_temporal && a.has_spp && a.spp < 2) return die("--denoise-temporal needs at least 2 samples per pixel (two half renders)");
     if (a.has_start && a.has_end && a.end < a.start)
         return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
