@@ -904,7 +904,8 @@ trb_status trb_denoise_device(trb_scene* scene, const trb_denoise_input* d_in, c
  *      current frame's.
  * Every NaN written to rgbw or motion is 0x7fffffff. Motion covers rigid instance transforms and the camera, not the deformation of
  * trb_scene_update_mesh / trb_scene_refit_mesh: the depth and normal tests reject what moved too far, and what they accept may ghost.
- * Misses have no history. */
+ * Misses have no history. A history last written by trb_denoise_moments* holds moments, not halves: these calls treat it as empty
+ * (as for another object generation), so the first one after it filters as trb_denoise does. */
 typedef struct trb_denoise_history trb_denoise_history;
 
 /* NULL means: trb_denoise's defaults for `spatial`, max_history 8 (1-255), depth_tolerance 0.05 (finite, > 0), normal_threshold 0.9
@@ -957,7 +958,8 @@ trb_status trb_denoise_temporal_device(trb_scene* scene, trb_denoise_history* hi
  * object-space point p_o, the camera ray (o, d, time), its key (the pixel index) and L_prev, the luminance L(x) = 0.2126 x.r +
  * 0.7152 x.g + 0.0722 x.b of the sample's radiance clamped to [0, 1] per channel; plus the frame's cam_world at shutter-open, its
  * shutter_open and the call's seed. The records are valid only if the previous call on the history was a gradient call of the same
- * object generation and film size; otherwise (first call, after reset, after trb_denoise_temporal, after replace_objects) there are
+ * object generation and film size; otherwise (first call, after reset, after trb_denoise_temporal or trb_denoise_moments, after
+ * replace_objects) there are
  * no gradients and lambda is 0 everywhere. Per call, float32, left to right, never contracted:
  *   1. Re-shade. For each valid record j (i below both instance counts): p_w' = mat_cur[i] . p_o, q = cam_inv_cur . p_w' (points as
  *      in "Temporal denoising"). Kept if q.z > 0, r = ((X - X0) / (X1 - X0) * W, (Y - Y1) / (Y0 - Y1) * H) with X = q.x / (q.z tan),
@@ -1009,6 +1011,72 @@ trb_status trb_denoise_temporal_gradient(trb_scene* scene, trb_denoise_history* 
 trb_status trb_denoise_temporal_gradient_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_input* d_in,
                                                 const trb_denoise_gradient_params* params, uint32_t seed,
                                                 const trb_denoise_gradient_output* d_out, void* cuda_stream);
+
+/* -- Moment denoising: one film per frame, the variance from temporally accumulated luminance moments -------------------------------
+ * (DESIGN.md §4 "Moment denoising"). SVGF's variance estimate (Schied et al. 2017, §4.2-4.3) in place of the two half films: each
+ * pixel accumulates the first two moments of its luminance over its reprojected history, and where that history is shorter than
+ * TRB_DENOISE_MOMENTS_MIN_HISTORY frames the variance is estimated spatially over a 7x7 window instead. So a frame needs one render at
+ * any sample count, 1 spp included: colour is trb_render_aov's film of the frame's whole sample range, albedo_w, normal_w and nearest
+ * its AOVs. The history is a trb_denoise_history as in "Temporal denoising" (same scene, film size, snapshot and generation rules);
+ * its per-pixel sets hold (ē, z), (mu1, mu2, inst) and (n, n') in the same 96 bytes per pixel. A history last written by the other
+ * family (trb_denoise_temporal* against trb_denoise_moments*) is treated as empty, as for another object generation.
+ * Per pixel p = (x, y), float32, left to right, never contracted, L(x) = 0.2126 x.r + 0.7152 x.g + 0.0722 x.b:
+ *   1. W = colour.w. W <= 0: the output is (0, 0, 0, 0), p is never a neighbour. c = colour.rgb / W; d, m, len2, n, z and dz are
+ *      trb_denoise's; e = c / d, l = L(e). Unless c, albedo, m, len2 and e are all finite and z is neither NaN nor -inf, p is copied
+ *      through as (c, 1) and is never a neighbour. Such pixels and W <= 0 ones store "none", have motion (NaN, NaN), history_length 0
+ *      and variance NaN.
+ *   2. Reprojection: steps 1-3 of "Temporal denoising", unchanged (the same motion, taps and instance, depth and normal tests), with
+ *      H' = (sum of w * ē_t in tap order) / S per channel, M1' = (sum of w * mu1_t) / S, M2' = (sum of w * mu2_t) / S and len_prev.
+ *   3. n' = min(len_prev + 1, max_history), or 1 without history. n' > 1: alpha = 1 / (float)n',
+ *        ē = alpha * e + (1 - alpha) * H' per channel,  mu1 = alpha * l + (1 - alpha) * M1',  mu2 = alpha * (l * l) + (1 - alpha) * M2'
+ *      n' == 1: ē = e, mu1 = l, mu2 = l * l. (The colour and the moments share the weight 1 / n'.)
+ *   4. n' >= TRB_DENOISE_MOMENTS_MIN_HISTORY: v = max(0, mu2 - mu1 * mu1). Otherwise, over the 7x7 taps q = p + (dx, dy), dy then dx
+ *      from -TRB_DENOISE_MOMENTS_RADIUS to TRB_DENOISE_MOMENTS_RADIUS, inside the image and filtered (p's own tap included, so the sum
+ *      is > 0), with ē, mu1, mu2 of step 3 at q:
+ *        w_l = exp(-(|L(ē_p) - L(ē_q)| / (sigma_luminance + TRB_DENOISE_EPS_LUMINANCE)))
+ *        w_n, w_z = trb_denoise's at step s = 1 (w_z's denominator sigma_depth * |gx * dx + gy * dy| + TRB_DENOISE_EPS_DEPTH)
+ *        w = w_l * w_n * w_z;  Sw, S1 = sum w * mu1, S2 = sum w * mu2 in tap order
+ *        v = max(0, S2 / Sw - (S1 / Sw) * (S1 / Sw)) * (4 / (float)n')   (SVGF's boost of short histories)
+ *   5. (ē, v) goes into trb_denoise's a-trous iterations; the output is remodulated by d as there (iterations 0: ē * d).
+ *   6. A filtered pixel with finite z stores (ē, z), (mu1, mu2, i), (n, n'); every other pixel stores "none". The snapshot becomes the
+ *      current frame's. Gradient records (trb_denoise_temporal_gradient) become invalid.
+ * max_history 1 makes every call a single-frame spatial denoiser of one film (n' = 1 everywhere). Every NaN written to rgbw, motion
+ * or variance is 0x7fffffff. The scene's denoise scratch grows to 88 bytes per pixel for moment calls (72 for every other denoise). */
+#define TRB_DENOISE_MOMENTS_MIN_HISTORY 4
+#define TRB_DENOISE_MOMENTS_RADIUS 3
+
+/* One colour film of the frame at any sample count and its AOVs, all required: host pointers for trb_denoise_moments, device
+ * pointers for trb_denoise_moments_device. The scene's film layout, as trb_denoise_input. */
+typedef struct trb_denoise_frame {
+    const float* colour;
+    const float* albedo_w;
+    const float* normal_w;
+    const uint64_t* nearest;
+} trb_denoise_frame;
+
+/* rgbw (width*height*4 floats) is required; motion (width*height*2 floats), history_length (width*height uint32) and variance
+ * (width*height floats: each pixel's v of step 4, the variance the a-trous iterations start from) may be NULL. */
+typedef struct trb_denoise_moments_output {
+    float* rgbw;
+    float* motion;
+    uint32_t* history_length;
+    float* variance;
+} trb_denoise_moments_output;
+
+/* Denoise a frame of one film with its history: HOST inputs and outputs, staged per call; blocking. The parameters are
+ * trb_denoise_temporal's, checked first (no scene is needed to refuse them); then TRB_INVALID_ARG for a null scene, history, input
+ * member or out->rgbw, a history of another scene or film size, a scene without a frame, or an output overlapping an input or another
+ * output; TRB_OOM when scratch or history does not fit. A call that fails leaves the history as it was. */
+trb_status trb_denoise_moments(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* in,
+                               const trb_denoise_temporal_params* params, const trb_denoise_moments_output* out);
+
+/* trb_denoise_moments with DEVICE buffers (colour, albedo_w, normal_w and rgbw 16-byte, nearest and motion 8-byte, history_length and
+ * variance 4-byte aligned; TRB_INVALID_ARG otherwise), enqueued on cuda_stream under trb_render_device's one-stream rule: 2 +
+ * iterations kernel launches and one copy of the instance transforms. No host synchronisation, except once when the scratch or the
+ * history grows. */
+trb_status trb_denoise_moments_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* d_in,
+                                      const trb_denoise_temporal_params* params, const trb_denoise_moments_output* d_out,
+                                      void* cuda_stream);
 
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus

@@ -46,6 +46,71 @@ bool temporal_params(const trb_denoise_temporal_params* params, trb_denoise_para
            t.normal_threshold <= 1.0f;
 }
 
+/* Steps 1-3 of the contract for the valid pixel P at (x, y) with instance id: the motion (left as it is without one), S, the
+ * tap-weighted sums sa and sb of the history's ha and hb (3 each, not yet divided by S) and len_prev. oracle_moments/moments.cpp
+ * calls it over a history whose ha holds ē and hb (mu1, mu2, 0). */
+void temporal_gather(long W, long H, long x, long y, const Px& P, uint32_t id, const orc_temporal_frame* f, const orc_denoise_history* h,
+                     const TemporalPrm& t, float& mx, float& my, float& S, float* sa, float* sb, uint32_t& len_prev) {
+    if (!(h->has_prev && id < h->n_instances && id < f->n_instances && fin(P.z))) return;
+    const M4 cam_mat = m4_of(f->cam_mat), px_to_cam = m4_of(f->px_to_cam), cam_inv_prev = m4_of(h->cam_inv);
+    const float aspect = (float)W / (float)H;
+    float X0 = -1.0f, X1 = 1.0f, Y0 = -1.0f / aspect, Y1 = 1.0f / aspect;
+    if (aspect > 1.0f) { X0 = -aspect; X1 = aspect; Y0 = -1.0f; Y1 = 1.0f; }
+    const V3 pc = Transform::mul_point(px_to_cam, V3((float)x + 0.5f, (float)y + 0.5f, 0.0f));
+    const V3 dir = Transform::mul_vector(cam_mat, normalized(V3(f->scaling[0], f->scaling[1], f->scaling[2]) * pc));
+    const V3 o = Transform::mul_point(cam_mat, V3(0.0f));
+    const V3 pw(o.x + P.z * dir.x, o.y + P.z * dir.y, o.z + P.z * dir.z);
+    const V3 po = Transform::mul_point(m4_of(f->inv + 16 * (size_t)id), pw);
+    const V3 pp = Transform::mul_point(m4_of(h->mats.data() + 16 * (size_t)id), po);
+    const V3 q = Transform::mul_point(cam_inv_prev, pp);
+    if (!(q.z > 0.0f)) return;
+    const float X = q.x / (q.z * h->tan_fov), Y = q.y / (q.z * h->tan_fov);
+    const float rx = (X - X0) / (X1 - X0) * (float)W, ry = (Y - Y1) / (Y0 - Y1) * (float)H;
+    mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
+    const float ql = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
+    const float cx = rx - 0.5f, cy = ry - 0.5f, fx = std::floor(cx), fy = std::floor(cy), ax = cx - fx, ay = cy - fy;
+    const int ox[4] = {0, 1, 0, 1}, oy[4] = {0, 0, 1, 1};
+    const float wts[4] = {(1.0f - ax) * (1.0f - ay), ax * (1.0f - ay), (1.0f - ax) * ay, ax * ay};
+    for (int k = 0; k < 4; ++k) {
+        const float tx = fx + (float)ox[k], ty = fy + (float)oy[k];
+        if (!(tx >= 0.0f && tx <= (float)W - 1.0f && ty >= 0.0f && ty <= (float)H - 1.0f)) continue;
+        const long j = (long)ty * W + (long)tx;
+        if (h->len[j] == 0 || h->inst[j] != id) continue;
+        if (!(std::fabs(h->z[j] - ql) <= t.depth_tolerance * ql)) continue;
+        const float* tn = &h->n[3 * j];
+        const bool t_nrm = tn[0] != 0.0f || tn[1] != 0.0f || tn[2] != 0.0f;
+        if (t_nrm != P.has_n) continue;
+        if (P.has_n && !(tn[0] * P.n[0] + tn[1] * P.n[1] + tn[2] * P.n[2] >= t.normal_threshold)) continue;
+        const float w = wts[k];
+        S = S + w;
+        for (int c = 0; c < 3; ++c) {
+            sa[c] = sa[c] + w * h->ha[3 * j + c];
+            sb[c] = sb[c] + w * h->hb[3 * j + c];
+        }
+        if (w > 0.0f && h->len[j] > len_prev) len_prev = h->len[j];
+    }
+}
+
+/* The frame of an oracle scene after orc_scene_update_frame: the camera's cam_world and every instance's transform at shutter-open,
+ * from the oracle's own matrices (inv and mat hold the instances' matrices, which f points at); false without a frame */
+bool scene_frame(orc_scene* s, orc_temporal_frame& f, std::vector<float>& inv, std::vector<float>& mat) {
+    if (!s || s->active_camera < 0) { g_err = "update_frame must be called before a temporal denoise"; return false; }
+    const Camera& cam = s->cameras[s->active_camera];
+    const Transform cw = cam.cam_world.transform(cam.shutter_open);
+    const size_t n = s->geom.instances.size();
+    inv.assign(16 * n, 0.0f); mat.assign(16 * n, 0.0f);
+    for (size_t k = 0; k < n; ++k) {
+        const Transform t = s->geom.instances[k].transform.transform(cam.shutter_open);
+        std::memcpy(&mat[16 * k], t.mat.m, 64); std::memcpy(&inv[16 * k], t.inv.m, 64);
+    }
+    std::memcpy(f.px_to_cam, cam.px_to_cam.mat.m, 64);
+    std::memcpy(f.cam_mat, cw.mat.m, 64);
+    std::memcpy(f.cam_inv, cw.inv.m, 64);
+    f.scaling[0] = cam.scaling.x; f.scaling[1] = cam.scaling.y; f.scaling[2] = cam.scaling.z;
+    f.n_instances = (uint32_t)n; f.inv = inv.data(); f.mat = mat.data();
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -67,10 +132,6 @@ int orc_denoise_temporal_frame(uint32_t width, uint32_t height, const orc_tempor
     std::vector<float> e, v, ea, eb;
     denoise_prepare(W, H, in, px, e, v, &ea, &eb);
     const float qnan = dm_from_bits(0x7fffffffu);
-    const M4 cam_mat = m4_of(f->cam_mat), px_to_cam = m4_of(f->px_to_cam), cam_inv_prev = m4_of(h->cam_inv);
-    const float aspect = (float)width / (float)height;
-    float X0 = -1.0f, X1 = 1.0f, Y0 = -1.0f / aspect, Y1 = 1.0f / aspect;
-    if (aspect > 1.0f) { X0 = -aspect; X1 = aspect; Y0 = -1.0f; Y1 = 1.0f; }
     std::vector<float> nha(N * 3), nhb(N * 3), nn(N * 3), nz(N);
     std::vector<uint32_t> ninst(N), nlen(N, 0u);
     for (long y = 0; y < H; ++y)
@@ -84,42 +145,7 @@ int orc_denoise_temporal_frame(uint32_t width, uint32_t height, const orc_tempor
                 float S = 0.0f, sa[3] = {0, 0, 0}, sb[3] = {0, 0, 0};
                 uint32_t len_prev = 0;
                 /* 1-3 */
-                if (h->has_prev && id < h->n_instances && id < f->n_instances && fin(P.z)) {
-                    const V3 pc = Transform::mul_point(px_to_cam, V3((float)x + 0.5f, (float)y + 0.5f, 0.0f));
-                    const V3 dir = Transform::mul_vector(cam_mat, normalized(V3(f->scaling[0], f->scaling[1], f->scaling[2]) * pc));
-                    const V3 o = Transform::mul_point(cam_mat, V3(0.0f));
-                    const V3 pw(o.x + P.z * dir.x, o.y + P.z * dir.y, o.z + P.z * dir.z);
-                    const V3 po = Transform::mul_point(m4_of(f->inv + 16 * (size_t)id), pw);
-                    const V3 pp = Transform::mul_point(m4_of(h->mats.data() + 16 * (size_t)id), po);
-                    const V3 q = Transform::mul_point(cam_inv_prev, pp);
-                    if (q.z > 0.0f) {
-                        const float X = q.x / (q.z * h->tan_fov), Y = q.y / (q.z * h->tan_fov);
-                        const float rx = (X - X0) / (X1 - X0) * (float)W, ry = (Y - Y1) / (Y0 - Y1) * (float)H;
-                        mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
-                        const float ql = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
-                        const float cx = rx - 0.5f, cy = ry - 0.5f, fx = std::floor(cx), fy = std::floor(cy), ax = cx - fx, ay = cy - fy;
-                        const int ox[4] = {0, 1, 0, 1}, oy[4] = {0, 0, 1, 1};
-                        const float wts[4] = {(1.0f - ax) * (1.0f - ay), ax * (1.0f - ay), (1.0f - ax) * ay, ax * ay};
-                        for (int k = 0; k < 4; ++k) {
-                            const float tx = fx + (float)ox[k], ty = fy + (float)oy[k];
-                            if (!(tx >= 0.0f && tx <= (float)W - 1.0f && ty >= 0.0f && ty <= (float)H - 1.0f)) continue;
-                            const long j = (long)ty * W + (long)tx;
-                            if (h->len[j] == 0 || h->inst[j] != id) continue;
-                            if (!(std::fabs(h->z[j] - ql) <= t.depth_tolerance * ql)) continue;
-                            const float* tn = &h->n[3 * j];
-                            const bool t_nrm = tn[0] != 0.0f || tn[1] != 0.0f || tn[2] != 0.0f;
-                            if (t_nrm != P.has_n) continue;
-                            if (P.has_n && !(tn[0] * P.n[0] + tn[1] * P.n[1] + tn[2] * P.n[2] >= t.normal_threshold)) continue;
-                            const float w = wts[k];
-                            S = S + w;
-                            for (int c = 0; c < 3; ++c) {
-                                sa[c] = sa[c] + w * h->ha[3 * j + c];
-                                sb[c] = sb[c] + w * h->hb[3 * j + c];
-                            }
-                            if (w > 0.0f && h->len[j] > len_prev) len_prev = h->len[j];
-                        }
-                    }
-                }
+                temporal_gather(W, H, x, y, P, id, f, h, t, mx, my, S, sa, sb, len_prev);
                 /* 4 */
                 np = S > 0.0f ? std::min(len_prev + 1, t.max_history) : 1u;
                 if (np > 1) {
@@ -155,21 +181,9 @@ int orc_denoise_temporal_frame(uint32_t width, uint32_t height, const orc_tempor
 
 int orc_denoise_temporal(orc_scene* s, orc_denoise_history* h, const trb_denoise_input* in, const trb_denoise_temporal_params* params,
                          float* rgbw, float* motion, uint32_t* history_length) {
-    if (!s || s->active_camera < 0) { g_err = "update_frame must be called before a temporal denoise"; return TRB_INVALID_ARG; }
-    const Camera& cam = s->cameras[s->active_camera];
-    const Transform cw = cam.cam_world.transform(cam.shutter_open);
-    const size_t n = s->geom.instances.size();
-    std::vector<float> inv(16 * n), mat(16 * n);
-    for (size_t k = 0; k < n; ++k) {
-        const Transform t = s->geom.instances[k].transform.transform(cam.shutter_open);
-        std::memcpy(&mat[16 * k], t.mat.m, 64); std::memcpy(&inv[16 * k], t.inv.m, 64);
-    }
     orc_temporal_frame f;
-    std::memcpy(f.px_to_cam, cam.px_to_cam.mat.m, 64);
-    std::memcpy(f.cam_mat, cw.mat.m, 64);
-    std::memcpy(f.cam_inv, cw.inv.m, 64);
-    f.scaling[0] = cam.scaling.x; f.scaling[1] = cam.scaling.y; f.scaling[2] = cam.scaling.z;
-    f.n_instances = (uint32_t)n; f.inv = inv.data(); f.mat = mat.data();
+    std::vector<float> inv, mat;
+    if (!scene_frame(s, f, inv, mat)) return TRB_INVALID_ARG;
     return orc_denoise_temporal_frame(s->film.width, s->film.height, &f, h, in, params, rgbw, motion, history_length);
 }
 

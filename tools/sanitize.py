@@ -132,3 +132,13 @@ _, motion, hl, lam = g.denoise_temporal_gradient(hist, film, film, aovs, 9, moti
 hist.reset()
 print("denoise gradient ok", float(den[..., :3].sum()), int(hl.max()), float(lam.max()))
 g.close()
+# the moment denoiser (k_dn_temporal_moments, k_dn_moments_variance): six 1-spp frames of the keyframed scene with every output, so
+# both variance branches and the 7x7 taps at the borders run, the last with no a-trous pass, then a reset
+g = api.Scene(SB.scene_animated(40, 24, 1).finish())
+hist = api.DenoiseHistory(g)
+for k in range(6):
+    den, film, aovs, _ = g.render_denoised_moments(hist, 1, seed=3, current_frame=k)
+_, motion, hl, var = g.denoise_moments(hist, film, aovs, motion=True, history_length=True, variance=True, iterations=0)
+hist.reset()
+print("denoise moments ok", float(den[..., :3].sum()), int(hl.max()), float(np.nanmax(var)))
+g.close()

@@ -245,6 +245,22 @@ class DenoiseGradientOutput(C.Structure):
 DENOISE_GRADIENT_DEFAULTS = dict(gradient_iterations=3)
 
 
+class DenoiseFrame(C.Structure):
+    """trb_denoise_frame: one colour film at any spp, the albedo and normal films and the nearest buffer (all required)"""
+    _fields_ = [("colour", C.c_void_p), ("albedo_w", C.c_void_p), ("normal_w", C.c_void_p), ("nearest", C.c_void_p)]
+
+
+class DenoiseMomentsOutput(C.Structure):
+    """trb_denoise_moments_output: rgbw (required), motion, history_length and variance (may be NULL)"""
+    _fields_ = [("rgbw", C.c_void_p), ("motion", C.c_void_p), ("history_length", C.c_void_p), ("variance", C.c_void_p)]
+
+
+# include/trb.h "Moment denoising": the history length from which a pixel's own moments give its variance, and the spatial
+# estimate's window radius (7x7)
+DENOISE_MOMENTS_MIN_HISTORY = 4
+DENOISE_MOMENTS_RADIUS = 3
+
+
 class BvhNode(C.Structure):
     _fields_ = [("bmin", f32 * 3), ("bmax", f32 * 3), ("a", u32), ("b", u32)]
 
@@ -299,6 +315,7 @@ TRB_SYMBOLS = [
     "trb_denoise", "trb_denoise_device",
     "trb_denoise_history_create", "trb_denoise_history_destroy", "trb_denoise_history_reset", "trb_denoise_temporal",
     "trb_denoise_temporal_device", "trb_denoise_temporal_gradient", "trb_denoise_temporal_gradient_device",
+    "trb_denoise_moments", "trb_denoise_moments_device",
 ]
 
 _trb = None
@@ -382,6 +399,9 @@ def load_trb():
                                                   C.POINTER(DenoiseGradientOutput)]
     lib.trb_denoise_temporal_gradient_device.argtypes = [vp, vp, C.POINTER(DenoiseInput), C.POINTER(DenoiseGradientParams), u32,
                                                          C.POINTER(DenoiseGradientOutput), vp]
+    lib.trb_denoise_moments.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseTemporalParams), C.POINTER(DenoiseMomentsOutput)]
+    lib.trb_denoise_moments_device.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseTemporalParams),
+                                               C.POINTER(DenoiseMomentsOutput), vp]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

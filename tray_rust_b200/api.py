@@ -425,6 +425,56 @@ class Scene(_Base):
             out = self.denoise_temporal(history, a, b, aovs, **(denoise or {}))
         return out, a + b, aovs, (st_a, st_b)
 
+    def denoise_moments(self, history, colour, aovs, out=None, motion=False, history_length=False, variance=False, **params):
+        """trb_denoise_moments (DESIGN.md §4 "Moment denoising"): one colour film of the frame at any spp, (height, width, 4)
+        float32, and the AOVs of the same render (render_aov's dict), rendered at the scene's current frame, with the DenoiseHistory
+        `history`. The variance comes from the luminance moments accumulated in the history, or a 7x7 spatial estimate where it is
+        short. params: denoise_temporal's. Returns the denoised RGBW film (into `out` when given), or a tuple of it with the motion,
+        the history length and the (height, width) float32 variance, in that order, where asked for (True, or an array)."""
+        h, w = self.height, self.width
+        film_shape = (h, w, 4)
+        ins = [("colour", colour, film_shape, np.float32), ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32),
+               ("normal_w", aovs.get("normal_w"), film_shape, np.float32), ("nearest", aovs.get("nearest"), (h, w), np.uint64)]
+        outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
+        for name, a, shape, dtype in (("motion", motion, (h, w, 2), np.float32), ("history_length", history_length, (h, w), np.uint32),
+                                      ("variance", variance, (h, w), np.float32)):
+            if a is True:
+                a = np.zeros(shape, dtype)
+            if a is not False and a is not None:
+                outs.append((name, a, shape, dtype))
+        for name, a, shape, dtype in ins + outs:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins)), _temporal_params(params)
+        o = F.DenoiseMomentsOutput(*(got[k].ctypes.data if k in got else None for k in ("out", "motion", "history_length", "variance")))
+        self._check(self._lib.trb_denoise_moments(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o)))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_moments_device(self, history, d_colour, d_albedo, d_normal, d_nearest, d_out, d_motion=None, d_history_length=None,
+                               d_variance=None, stream=None, **params):
+        """trb_denoise_moments_device: device pointers as ints (d_colour, d_albedo, d_normal and d_out height*width*4 float32,
+        16-byte aligned; d_nearest height*width uint64 and d_motion height*width*2 float32, 8-byte aligned; d_history_length
+        height*width uint32 and d_variance height*width float32, 4-byte aligned; the last three may be None), enqueued on `stream`.
+        params as for denoise_moments."""
+        d_in, prm = F.DenoiseFrame(d_colour, d_albedo, d_normal, d_nearest), _temporal_params(params)
+        o = F.DenoiseMomentsOutput(d_out, d_motion, d_history_length, d_variance)
+        self._check(self._lib.trb_denoise_moments_device(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o), stream))
+
+    def render_denoised_moments(self, history, spp=0, seed=1, current_frame=0, denoise=None, **kw):
+        """Frame `current_frame` of an animation rendered once by render_aov at `spp` (0: the scene's; 1 is enough) with seed
+        (seed + current_frame) mod 2^32, and denoised with `history` by denoise_moments (the dict `denoise` holds its parameters).
+        Returns (denoised, film, aovs, stats)."""
+        for k in ("sample_first", "sample_count"):
+            if k in kw:
+                raise ValueError("render_denoised_moments renders the whole sample range; %s is not taken" % k)
+        frame_seed = (seed + current_frame) % (1 << 32)
+        film, aovs, st = self.render_aov(spp=spp, seed=frame_seed, current_frame=current_frame, **kw)
+        out = self.denoise_moments(history, film, aovs, **(denoise or {}))
+        return out, film, aovs, st
+
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:
         samples [0, spp/2) and [spp/2, spp) are rendered into two films by render_aov, with the albedo, normal and nearest AOVs

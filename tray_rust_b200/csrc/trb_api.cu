@@ -328,9 +328,11 @@ struct trb_scene {
     // (albedo, depth) in d_aov[p] and (n, inst bits) in d_aov[aov_capacity + p], 32 bytes
     float4* d_aov = nullptr;
     size_t aov_capacity = 0;
-    // denoiser scratch (trb_denoise*; trb::DnScratch), allocated by the first denoise for the film's pixel count and released with the film
+    // denoiser scratch (trb_denoise*; trb::DnScratch), allocated by the first denoise for the film's pixel count and released with the film;
+    // denoise_moments: it also holds the moment records of trb_denoise_moments* (trb::DN_MOMENTS_BYTES_PER_PIXEL)
     void* d_denoise = nullptr;
     size_t denoise_pixels = 0;
+    bool denoise_moments = false;
     // temporal denoising (trb_denoise_temporal*): the inverse of the camera's cam_world at the current frame's shutter-open, and the
     // object generation, counted up by the calls that renumber instances (replace_objects, replace_meshes with an object section)
     float cam_inv[16] = {};
@@ -2867,23 +2869,26 @@ trb_status denoise_check(const trb_scene* s, const trb_denoise_input* in, const 
     return TRB_OK;
 }
 
-// The scene's denoise scratch for the film's npx pixels. The scratch is per scene and sized by the film; growing it drains the device once.
-trb_status denoise_scratch(trb_scene* s, size_t npx, trb::DnScratch& sc) {
-    if (s->denoise_pixels < npx) {
+// The scene's denoise scratch for the film's npx pixels, and with `mom` the moment records after it. The scratch is per scene and sized
+// by the film; growing it drains the device once.
+trb_status denoise_scratch(trb_scene* s, size_t npx, trb::DnScratch& sc, float4** mom = nullptr) {
+    const size_t mom_off = (npx * trb::DN_BYTES_PER_PIXEL + 15) & ~(size_t)15;
+    if (s->denoise_pixels < npx || (mom && !s->denoise_moments)) {
         if (s->d_denoise) {
             CU(cudaDeviceSynchronize()); // a denoise still in flight owns the old scratch
             cudaFree(s->d_denoise);
         }
-        s->d_denoise = nullptr; s->denoise_pixels = 0;
-        const cudaError_t e = cudaMalloc(&s->d_denoise, npx * trb::DN_BYTES_PER_PIXEL);
+        s->d_denoise = nullptr; s->denoise_pixels = 0; s->denoise_moments = false;
+        const cudaError_t e = cudaMalloc(&s->d_denoise, mom ? mom_off + npx * sizeof(float4) : npx * trb::DN_BYTES_PER_PIXEL);
         if (e != cudaSuccess) {
             cudaGetLastError(); s->d_denoise = nullptr;
             return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("denoise scratch: ") + cudaGetErrorString(e));
         }
-        s->denoise_pixels = npx;
+        s->denoise_pixels = npx; s->denoise_moments = mom != nullptr;
     }
     float4* base = static_cast<float4*>(s->d_denoise);
     sc = trb::DnScratch{base, base + npx, {base + 2 * npx, base + 3 * npx}, reinterpret_cast<float2*>(base + 4 * npx)};
+    if (mom) *mom = reinterpret_cast<float4*>(static_cast<char*>(s->d_denoise) + mom_off);
     return TRB_OK;
 }
 
@@ -2967,6 +2972,7 @@ struct trb_denoise_history {
     float cam_inv[16] = {}, tan_fov = 0;
     uint32_t n_instances = 0;
     uint64_t generation = 0;
+    bool moments = false;          // the read set was written by trb_denoise_moments* (moments), not trb_denoise_temporal* (halves)
     // temporal gradients: two record sets and the per-call stratum buffers (trb::GrBuffers) for gr_capacity strata; the records of
     // the read set are valid only after a gradient call, and were written at gr_seed, gr_shutter_open and gr_cam_mat
     void* d_gr = nullptr;
@@ -3026,6 +3032,27 @@ trb_status temporal_params(const trb_denoise_temporal_params* p, trb::DnParams& 
     return TRB_OK;
 }
 
+using Span = std::pair<const void*, size_t>;
+
+// The checks shared by the half-film and moment calls after their parameters and null pointers: outputs outs[first..] overlapping an
+// input or an earlier output, the history's scene and film size, a frame
+trb_status history_call_check(const trb_scene* s, const trb_denoise_history* h, const Span* ins, size_t nin, const Span* outs, size_t nout,
+                              size_t first) {
+    for (size_t k = first; k < nout; ++k) {
+        for (size_t j = 0; j < nin; ++j)
+            if (spans_overlap(outs[k].first, outs[k].second, ins[j].first, ins[j].second))
+                return fail(TRB_INVALID_ARG, k == 0 ? "the denoise output overlaps an input" : "a temporal denoise output overlaps an input");
+        for (size_t j = 0; j < k; ++j)
+            if (spans_overlap(outs[k].first, outs[k].second, outs[j].first, outs[j].second))
+                return fail(TRB_INVALID_ARG, "two temporal denoise outputs overlap");
+    }
+    if (h->scene != s) return fail(TRB_INVALID_ARG, "the denoise history belongs to another scene");
+    if (h->bound && (h->width != s->film.width || h->height != s->film.height))
+        return fail(TRB_INVALID_ARG, "the denoise history was written at another film size: reset it");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "update_frame must be called before a temporal denoise");
+    return TRB_OK;
+}
+
 // The checks of both forms after the parameters: null pointers, the history's scene and film size, a frame, overlapping outputs
 trb_status temporal_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_input* in, const trb_denoise_temporal_params* params,
                           const trb_denoise_temporal_output* out, trb::DnParams& prm, trb::DnTemporal& tp) {
@@ -3035,22 +3062,29 @@ trb_status temporal_check(const trb_scene* s, const trb_denoise_history* h, cons
     r = denoise_check(s, in, params ? &params->spatial : nullptr, out->rgbw, prm);
     if (r != TRB_OK) return r;
     const size_t npx = (size_t)s->film.width * s->film.height;
-    const std::pair<const void*, size_t> ins[5] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
-                                                   {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
-                                                   {in->nearest, npx * sizeof(uint64_t)}};
-    const std::pair<const void*, size_t> outs[3] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)},
-                                                    {out->history_length, npx * sizeof(uint32_t)}};
-    for (int k = 1; k < 3; ++k) {
-        for (const auto& [p, bytes] : ins)
-            if (spans_overlap(outs[k].first, outs[k].second, p, bytes)) return fail(TRB_INVALID_ARG, "a temporal denoise output overlaps an input");
-        for (int j = 0; j < k; ++j)
-            if (spans_overlap(outs[k].first, outs[k].second, outs[j].first, outs[j].second))
-                return fail(TRB_INVALID_ARG, "two temporal denoise outputs overlap");
+    const Span ins[5] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)},
+                         {in->normal_w, npx * sizeof(float4)}, {in->nearest, npx * sizeof(uint64_t)}};
+    const Span outs[3] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
+    return history_call_check(s, h, ins, 5, outs, 3, 1); // denoise_check tested rgbw
+}
+
+// The host forms' staging: each span copied into a new device buffer (inputs), or a device buffer for each non-null span (outputs)
+trb_status stage_in(const Span* hs, size_t n, DeviceBuffer* d) {
+    for (size_t k = 0; k < n; ++k) {
+        CU(cudaMalloc(&d[k].p, hs[k].second));
+        CU(cudaMemcpy(d[k].p, hs[k].first, hs[k].second, cudaMemcpyHostToDevice));
     }
-    if (h->scene != s) return fail(TRB_INVALID_ARG, "the denoise history belongs to another scene");
-    if (h->bound && (h->width != s->film.width || h->height != s->film.height))
-        return fail(TRB_INVALID_ARG, "the denoise history was written at another film size: reset it");
-    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "update_frame must be called before a temporal denoise");
+    return TRB_OK;
+}
+trb_status stage_out(const Span* hs, size_t n, DeviceBuffer* d) {
+    for (size_t k = 0; k < n; ++k)
+        if (hs[k].first) CU(cudaMalloc(&d[k].p, hs[k].second));
+    return TRB_OK;
+}
+// ... and the outputs copied back
+trb_status unstage_out(const Span* hs, size_t n, const DeviceBuffer* d) {
+    for (size_t k = 0; k < n; ++k)
+        if (hs[k].first) CU(cudaMemcpy(const_cast<void*>(hs[k].first), d[k].p, hs[k].second, cudaMemcpyDeviceToHost));
     return TRB_OK;
 }
 
@@ -3161,15 +3195,19 @@ trb_status gradient_record(trb_scene* s, const GradCall& gc, const GrBuffers& b,
     return TRB_OK;
 }
 
-// k_dn_temporal (or, with gc, the gradient steps around k_dn_temporal_grad) and the a-trous launches on `st`, then the history's
-// switch to the set just written
-trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_input& in,
-                            const trb_denoise_temporal_output& out, cudaStream_t st, const GradCall* gc = nullptr) {
+// The sets and snapshots of a history call: the one read, the one written, and the matrices of each
+struct HistorySets {
+    uint32_t rd, wr;
+    float* mats_rd;
+};
+
+// What a history call does before its kernels, for npx > 0 pixels: grow the history (and, with gc, its gradient buffers) where
+// needed, fill tp's current frame and the read set's snapshot (has_prev only for a history of the call's family, `moments`), and copy
+// this frame's instance transforms into the write snapshot on `st`
+trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnParams& prm, trb::DnTemporal& tp, bool moments, const GradCall* gc,
+                         HistorySets& hs, cudaStream_t st) {
     const size_t npx = (size_t)prm.width * prm.height, n = s->instances.size();
-    if (npx == 0) return TRB_OK;
-    trb::DnScratch sc;
-    trb_status r = denoise_scratch(s, npx, sc);
-    if (r != TRB_OK) return r;
+    trb_status r;
     // the pixel sets are bound to one film size, so they only grow while the history is empty: nothing to keep. A new buffer is
     // allocated before the old one is released, so a failure leaves the history as it was.
     if (h->px_capacity < npx) {
@@ -3213,13 +3251,40 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
     if (aspect > 1.0f) { tp.x0 = -aspect; tp.x1 = aspect; tp.y0 = -1.0f; tp.y1 = 1.0f; }
     else { tp.x0 = -1.0f; tp.x1 = 1.0f; tp.y0 = -1.0f / aspect; tp.y1 = 1.0f / aspect; }
     tp.n_prev = h->n_instances;
-    tp.has_prev = h->has_prev && h->generation == s->object_generation ? 1u : 0u;
-    const uint32_t rd = h->cur, wr = h->cur ^ 1u;
-    float* mats_rd = h->d_mats + (size_t)rd * h->mat_capacity * 16;
-    float* mats_wr = h->d_mats + (size_t)wr * h->mat_capacity * 16;
+    tp.has_prev = h->has_prev && h->generation == s->object_generation && h->moments == moments ? 1u : 0u;
+    hs.rd = h->cur; hs.wr = h->cur ^ 1u;
+    hs.mats_rd = h->d_mats + (size_t)hs.rd * h->mat_capacity * 16;
+    float* mats_wr = h->d_mats + (size_t)hs.wr * h->mat_capacity * 16;
     // this frame's object -> world matrices into the write snapshot: DInstance.mat, 64-byte rows at the records' 208-byte pitch
     CU(cudaMemcpy2DAsync(mats_wr, 64, reinterpret_cast<const char*>(s->d_instances) + offsetof(trb::DInstance, mat), sizeof(trb::DInstance), 64, n,
                          cudaMemcpyDeviceToDevice, st));
+    return TRB_OK;
+}
+
+// After a history call's kernels: the history switches to the set just written, and the snapshot becomes the current frame's
+void history_commit(trb_scene* s, trb_denoise_history* h, const HistorySets& hs, bool moments) {
+    h->cur = hs.wr; h->has_prev = true; h->bound = true; h->width = s->film.width; h->height = s->film.height;
+    std::memcpy(h->cam_inv, s->cam_inv, 64);
+    h->tan_fov = s->ds.cam.scaling[0];
+    h->n_instances = (uint32_t)s->instances.size();
+    h->generation = s->object_generation;
+    h->moments = moments;
+}
+
+// k_dn_temporal (or, with gc, the gradient steps around k_dn_temporal_grad) and the a-trous launches on `st`, then the history's
+// switch to the set just written
+trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_input& in,
+                            const trb_denoise_temporal_output& out, cudaStream_t st, const GradCall* gc = nullptr) {
+    const size_t npx = (size_t)prm.width * prm.height;
+    if (npx == 0) return TRB_OK;
+    trb::DnScratch sc;
+    trb_status r = denoise_scratch(s, npx, sc);
+    if (r != TRB_OK) return r;
+    HistorySets hs;
+    r = history_begin(s, h, prm, tp, false, gc, hs, st);
+    if (r != TRB_OK) return r;
+    const uint32_t rd = hs.rd, wr = hs.wr;
+    const float* mats_rd = hs.mats_rd;
     float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
     const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
     if (!gc) {
@@ -3252,11 +3317,7 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
         h->gr_valid = true; h->gr_seed = gc->seed; h->gr_shutter_open = s->shutter_open;
         std::memcpy(h->gr_cam_mat, s->ds.cam.cam_mat, 64);
     }
-    h->cur = wr; h->has_prev = true; h->bound = true; h->width = s->film.width; h->height = s->film.height;
-    std::memcpy(h->cam_inv, s->cam_inv, 64);
-    h->tan_fov = s->ds.cam.scaling[0];
-    h->n_instances = (uint32_t)n;
-    h->generation = s->object_generation;
+    history_commit(s, h, hs, false);
     return TRB_OK;
 }
 } // namespace
@@ -3284,24 +3345,16 @@ trb_status trb_denoise_temporal(trb_scene* s, trb_denoise_history* h, const trb_
     if (r != TRB_OK) return r;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_rgbw, d_motion, d_len;
-    for (auto [d, hp, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
-                                {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
-        CU(cudaMalloc(&d->p, bytes));
-        CU(cudaMemcpy(d->p, hp, bytes, cudaMemcpyHostToDevice));
-    }
-    CU(cudaMalloc(&d_rgbw.p, fb));
-    if (out->motion) CU(cudaMalloc(&d_motion.p, npx * sizeof(float2)));
-    if (out->history_length) CU(cudaMalloc(&d_len.p, npx * sizeof(uint32_t)));
-    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
-                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
-    const trb_denoise_temporal_output d_out{static_cast<float*>(d_rgbw.p), static_cast<float*>(d_motion.p), static_cast<uint32_t*>(d_len.p)};
+    const Span ins[5] = {{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
+    const Span outs[3] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
+    DeviceBuffer d_ins[5], d_outs[3];
+    if ((r = stage_in(ins, 5, d_ins)) != TRB_OK || (r = stage_out(outs, 3, d_outs)) != TRB_OK) return r;
+    const trb_denoise_input d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
+                                 static_cast<const float*>(d_ins[3].p), static_cast<const uint64_t*>(d_ins[4].p)};
+    const trb_denoise_temporal_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p)};
     r = temporal_enqueue(s, h, prm, tp, d_in, d_out, 0);
     if (r != TRB_OK) return r;
-    CU(cudaMemcpy(out->rgbw, d_rgbw.p, fb, cudaMemcpyDeviceToHost));
-    if (out->motion) CU(cudaMemcpy(out->motion, d_motion.p, npx * sizeof(float2), cudaMemcpyDeviceToHost));
-    if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    return TRB_OK;
+    return unstage_out(outs, 3, d_outs);
 }
 
 namespace {
@@ -3381,6 +3434,91 @@ trb_status trb_denoise_temporal_gradient(trb_scene* s, trb_denoise_history* h, c
     if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     if (out->lambda) CU(cudaMemcpy(out->lambda, d_lam.p, npx * sizeof(float), cudaMemcpyDeviceToHost));
     return TRB_OK;
+}
+
+// ---- moment denoising (include/trb.h "Moment denoising", DESIGN.md §4) -----------------------------------------------------------
+namespace {
+// The checks of both forms after the parameters: null pointers, overlapping outputs, the history's scene and film size, a frame
+trb_status moments_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_temporal_params* params,
+                         const trb_denoise_moments_output* out, trb::DnParams& prm, trb::DnTemporal& tp) {
+    trb_status r = temporal_params(params, prm, tp);
+    if (r != TRB_OK) return r;
+    if (!s || !h || !in || !out || !out->rgbw || !in->colour || !in->albedo_w || !in->normal_w || !in->nearest)
+        return fail(TRB_INVALID_ARG, "null argument");
+    prm.width = (int)s->film.width; prm.height = (int)s->film.height;
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    const Span ins[4] = {{in->colour, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                         {in->nearest, npx * sizeof(uint64_t)}};
+    const Span outs[4] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
+                          {out->variance, npx * sizeof(float)}};
+    return history_call_check(s, h, ins, 4, outs, 4, 0);
+}
+
+// k_dn_temporal_moments, k_dn_moments_variance and the a-trous launches on `st`, then the history's switch to the set just written
+trb_status moments_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_frame& in,
+                           const trb_denoise_moments_output& out, cudaStream_t st) {
+    const size_t npx = (size_t)prm.width * prm.height;
+    if (npx == 0) return TRB_OK;
+    trb::DnScratch sc;
+    float4* mom = nullptr;
+    trb_status r = denoise_scratch(s, npx, sc, &mom);
+    if (r != TRB_OK) return r;
+    HistorySets hs;
+    r = history_begin(s, h, prm, tp, true, nullptr, hs, st);
+    if (r != TRB_OK) return r;
+    float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
+    const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    trb::k_dn_temporal_moments<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour), reinterpret_cast<const float4*>(in.albedo_w),
+                                                       reinterpret_cast<const float4*>(in.normal_w), reinterpret_cast<const unsigned long long*>(in.nearest),
+                                                       sc, mom, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd), h->set(hs.wr),
+                                                       reinterpret_cast<float2*>(out.motion), out.history_length);
+    g_launches++;
+    trb::k_dn_moments_variance<<<grid, block, 0, st>>>(prm, sc.guide, sc.grad, mom, sc.ev[0], out.variance);
+    g_launches++;
+    CU(cudaGetLastError());
+    r = denoise_atrous(prm, sc, rgbw, st);
+    if (r != TRB_OK) return r;
+    h->gr_valid = false;
+    history_commit(s, h, hs, true);
+    return TRB_OK;
+}
+} // namespace
+
+trb_status trb_denoise_moments_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* d_in, const trb_denoise_temporal_params* params,
+                                      const trb_denoise_moments_output* d_out, void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    const trb_status r = moments_check(s, h, d_in, params, d_out, prm, tp);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_in->colour) | reinterpret_cast<uintptr_t>(d_in->albedo_w) | reinterpret_cast<uintptr_t>(d_in->normal_w) |
+          reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
+        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
+        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->variance)) & 3u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and variance 4-byte");
+    CU(cudaSetDevice(s->device));
+    return moments_enqueue(s, h, prm, tp, *d_in, *d_out, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_denoise_moments(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_temporal_params* params,
+                               const trb_denoise_moments_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    trb_status r = moments_check(s, h, in, params, out, prm, tp);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    const Span ins[4] = {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
+    const Span outs[4] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
+                          {out->variance, npx * sizeof(float)}};
+    DeviceBuffer d_ins[4], d_outs[4];
+    if ((r = stage_in(ins, 4, d_ins)) != TRB_OK || (r = stage_out(outs, 4, d_outs)) != TRB_OK) return r;
+    const trb_denoise_frame d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
+                                 static_cast<const uint64_t*>(d_ins[3].p)};
+    const trb_denoise_moments_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p),
+                                          static_cast<float*>(d_outs[3].p)};
+    r = moments_enqueue(s, h, prm, tp, d_in, d_out, 0);
+    if (r != TRB_OK) return r;
+    return unstage_out(outs, 4, d_outs);
 }
 
 trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {

@@ -2,7 +2,8 @@
 // edge-avoiding a-trous filter over the demodulated colour of two half renders, guided by their albedo, normal and nearest-hit films.
 // Three kernels: k_dn_prepare reads the inputs once into a guide record per pixel and the first (e, v) buffer; k_dn_atrous runs one
 // iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film; k_dn_temporal takes k_dn_prepare's place
-// for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer. Float32 in the header's order, no
+// for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer; k_dn_temporal_moments and
+// k_dn_moments_variance take it for trb_denoise_moments*, one film with the variance from luminance moments. Float32 in the header's order, no
 // atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
 #pragma once
 #include "trb_detmath.cuh"
@@ -191,6 +192,53 @@ struct DnHistory {
 };
 constexpr size_t DN_HISTORY_BYTES_PER_PIXEL = 3 * sizeof(float4);
 
+// Steps 1-3 of "Temporal denoising" for pixel (x, y) with depth z, instance id and unit normal n (0 if none): the motion (NaN where
+// none), S, the tap-weighted sums of the a and b records' first three channels (divided by S by the caller) and len_prev. Shared by
+// the half-film kernels (a, b = H_a, H_b) and k_dn_temporal_moments (a = H, b = (M1, M2, 0)).
+__device__ __forceinline__ void dn_reproject(const DnParams& prm, const DnTemporal& tp, int x, int y, float z, uint32_t id, float n0, float n1,
+                                             float n2, const DInstance* __restrict__ inst, const float* __restrict__ mat_prev, const DnHistory& hin,
+                                             float& mx, float& my, float& S, float& ha0, float& ha1, float& ha2, float& hb0, float& hb1,
+                                             float& hb2, uint32_t& len_prev) {
+    const float qnan = __int_as_float(0x7fffffff);
+    mx = qnan; my = qnan; S = 0.0f; ha0 = 0.0f; ha1 = 0.0f; ha2 = 0.0f; hb0 = 0.0f; hb1 = 0.0f; hb2 = 0.0f;
+    len_prev = 0;
+    if (tp.has_prev && id < tp.n_prev && id < tp.n_cur && dn_finite(z)) {
+        const f3 pc = xf_point(tp.px_to_cam, mk((float)x + 0.5f, (float)y + 0.5f, 0.0f));
+        const f3 dir = xf_vector(tp.cam_mat, unit(mk(tp.scaling[0], tp.scaling[1], tp.scaling[2]) * pc));
+        const f3 o = xf_point(tp.cam_mat, splat(0.0f));
+        const f3 pw = mk(o.x + z * dir.x, o.y + z * dir.y, o.z + z * dir.z);
+        const f3 q = xf_point(tp.cam_inv_prev, xf_point(mat_prev + 16 * (size_t)id, xf_point(inst[id].inv, pw)));
+        if (q.z > 0.0f) {
+            const float X = q.x / (q.z * tp.tan_prev), Y = q.y / (q.z * tp.tan_prev);
+            const float rx = (X - tp.x0) / (tp.x1 - tp.x0) * tp.w_prev, ry = (Y - tp.y1) / (tp.y0 - tp.y1) * tp.h_prev;
+            mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
+            const float ql = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z);
+            const float cx = rx - 0.5f, cy = ry - 0.5f, fx = floorf(cx), fy = floorf(cy), ax = cx - fx, ay = cy - fy;
+            const bool p_nrm = n0 != 0.0f || n1 != 0.0f || n2 != 0.0f;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float tx = fx + (float)(k & 1), ty = fy + (float)(k >> 1);
+                const float w = ((k & 1) ? ax : 1.0f - ax) * ((k >> 1) ? ay : 1.0f - ay);
+                if (!(tx >= 0.0f && tx <= tp.w_prev - 1.0f && ty >= 0.0f && ty <= tp.h_prev - 1.0f)) continue;
+                const int j = (int)ty * prm.width + (int)tx;
+                const float4 tn = hin.n[j];
+                const uint32_t tlen = __float_as_uint(tn.w);
+                if (tlen == 0u) continue;
+                const float4 ta = hin.a[j], tb = hin.b[j];
+                if (__float_as_uint(tb.w) != id) continue;
+                if (!(fabsf(ta.w - ql) <= tp.depth_tolerance * ql)) continue;
+                const bool t_nrm = tn.x != 0.0f || tn.y != 0.0f || tn.z != 0.0f;
+                if (t_nrm != p_nrm) continue;
+                if (p_nrm && !(tn.x * n0 + tn.y * n1 + tn.z * n2 >= tp.normal_threshold)) continue;
+                S = S + w;
+                ha0 = ha0 + w * ta.x; ha1 = ha1 + w * ta.y; ha2 = ha2 + w * ta.z;
+                hb0 = hb0 + w * tb.x; hb1 = hb1 + w * tb.y; hb2 = hb2 + w * tb.z;
+                if (w > 0.0f && tlen > len_prev) len_prev = tlen;
+            }
+        }
+    }
+}
+
 // k_dn_prepare's reads and writes, plus the reprojected history blended into (ē, v) before the a-trous iterations (1 + N launches as
 // for trb_denoise). mat_prev: the snapshot's object -> world matrices, 16 floats per instance; the current inverses are read from the
 // frame's instance records.
@@ -260,43 +308,9 @@ __device__ __forceinline__ void dn_temporal_px(const DnParams prm, const DnTempo
     }
     // 1-3: reconstruct, reproject into the snapshot's frame, gather the history taps
     const uint32_t id = (uint32_t)key;
-    float mx = qnan, my = qnan, S = 0.0f, ha0 = 0.0f, ha1 = 0.0f, ha2 = 0.0f, hb0 = 0.0f, hb1 = 0.0f, hb2 = 0.0f;
-    uint32_t len_prev = 0;
-    if (tp.has_prev && id < tp.n_prev && id < tp.n_cur && dn_finite(z)) {
-        const f3 pc = xf_point(tp.px_to_cam, mk((float)x + 0.5f, (float)y + 0.5f, 0.0f));
-        const f3 dir = xf_vector(tp.cam_mat, unit(mk(tp.scaling[0], tp.scaling[1], tp.scaling[2]) * pc));
-        const f3 o = xf_point(tp.cam_mat, splat(0.0f));
-        const f3 pw = mk(o.x + z * dir.x, o.y + z * dir.y, o.z + z * dir.z);
-        const f3 q = xf_point(tp.cam_inv_prev, xf_point(mat_prev + 16 * (size_t)id, xf_point(inst[id].inv, pw)));
-        if (q.z > 0.0f) {
-            const float X = q.x / (q.z * tp.tan_prev), Y = q.y / (q.z * tp.tan_prev);
-            const float rx = (X - tp.x0) / (tp.x1 - tp.x0) * tp.w_prev, ry = (Y - tp.y1) / (tp.y0 - tp.y1) * tp.h_prev;
-            mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
-            const float ql = sqrtf(q.x * q.x + q.y * q.y + q.z * q.z);
-            const float cx = rx - 0.5f, cy = ry - 0.5f, fx = floorf(cx), fy = floorf(cy), ax = cx - fx, ay = cy - fy;
-            const bool p_nrm = n0 != 0.0f || n1 != 0.0f || n2 != 0.0f;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float tx = fx + (float)(k & 1), ty = fy + (float)(k >> 1);
-                const float w = ((k & 1) ? ax : 1.0f - ax) * ((k >> 1) ? ay : 1.0f - ay);
-                if (!(tx >= 0.0f && tx <= tp.w_prev - 1.0f && ty >= 0.0f && ty <= tp.h_prev - 1.0f)) continue;
-                const int j = (int)ty * prm.width + (int)tx;
-                const float4 tn = hin.n[j];
-                const uint32_t tlen = __float_as_uint(tn.w);
-                if (tlen == 0u) continue;
-                const float4 ta = hin.a[j], tb = hin.b[j];
-                if (__float_as_uint(tb.w) != id) continue;
-                if (!(fabsf(ta.w - ql) <= tp.depth_tolerance * ql)) continue;
-                const bool t_nrm = tn.x != 0.0f || tn.y != 0.0f || tn.z != 0.0f;
-                if (t_nrm != p_nrm) continue;
-                if (p_nrm && !(tn.x * n0 + tn.y * n1 + tn.z * n2 >= tp.normal_threshold)) continue;
-                S = S + w;
-                ha0 = ha0 + w * ta.x; ha1 = ha1 + w * ta.y; ha2 = ha2 + w * ta.z;
-                hb0 = hb0 + w * tb.x; hb1 = hb1 + w * tb.y; hb2 = hb2 + w * tb.z;
-                if (w > 0.0f && tlen > len_prev) len_prev = tlen;
-            }
-        }
-    }
+    float mx, my, S, ha0, ha1, ha2, hb0, hb1, hb2;
+    uint32_t len_prev;
+    dn_reproject(prm, tp, x, y, z, id, n0, n1, n2, inst, mat_prev, hin, mx, my, S, ha0, ha1, ha2, hb0, hb1, hb2, len_prev);
     // 4: blend
     uint32_t np = 1;
     if (GRAD) {
@@ -351,6 +365,167 @@ __global__ void __launch_bounds__(256) k_dn_temporal_grad(const DnParams prm, co
                                                           const DnHistory hout, float2* __restrict__ motion, uint32_t* __restrict__ hlen,
                                                           const float* __restrict__ lam_s, uint32_t gw, float* __restrict__ lam_out) {
     dn_temporal_px<true>(prm, tp, ca, cb, alb, nrm, nearest, sc, out, inst, mat_prev, hin, hout, motion, hlen, lam_s, gw, lam_out);
+}
+
+// ---- moment denoising (trb_denoise_moments*, include/trb.h "Moment denoising") ---------------------------------------------------
+// One moment record per pixel, 16 bytes: (L(ē), mu1, mu2, n' bits), read by k_dn_moments_variance for the pixel and its 7x7 taps.
+// Moment calls take the scene's scratch to DN_MOMENTS_BYTES_PER_PIXEL, the records after the 72 bytes of DnScratch (16-byte aligned).
+constexpr size_t DN_MOMENTS_BYTES_PER_PIXEL = DN_BYTES_PER_PIXEL + sizeof(float4);
+
+// Steps 1-3 and 6 of "Moment denoising": trb_denoise's pixel over one film, the history reprojected and gathered as in "Temporal
+// denoising" (dn_reproject; a set's records are (ē, z), (mu1, mu2, 0, inst bits), (n, n' bits)) and the blend of the colour and the
+// luminance moments. Writes the guide, gradient and divisor as k_dn_prepare does, ev[0] = (ē, 0) (k_dn_moments_variance fills in v),
+// the moment record, the history, motion and history length.
+__global__ void __launch_bounds__(256) k_dn_temporal_moments(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ col,
+                                                             const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                             const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ mom,
+                                                             float4* __restrict__ out, const DInstance* __restrict__ inst, const float* __restrict__ mat_prev,
+                                                             const DnHistory hin, const DnHistory hout, float2* __restrict__ motion,
+                                                             uint32_t* __restrict__ hlen) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int i = y * prm.width + x;
+    const float qnan = __int_as_float(0x7fffffff);
+    const float4 A = col[i];
+    const float W = A.w;
+    if (W <= 0.0f) {
+        out[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        return;
+    }
+    const float c0 = A.x / W, c1 = A.y / W, c2 = A.z / W;
+    const float4 al = alb[i], nw = nrm[i];
+    const float a0 = al.x / al.w, a1 = al.y / al.w, a2 = al.z / al.w;
+    const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
+    float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
+    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
+    const unsigned long long key = nearest[i];
+    const float z = __uint_as_float((uint32_t)(key >> 32));
+    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
+                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && z == z &&
+                    z != __int_as_float(0xff800000);
+    if (!ok) {
+        out[i] = dn_out(c0, c1, c2, 1.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        return;
+    }
+    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    if (len2 != 0.0f) {
+        const float l = sqrtf(len2);
+        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    }
+    float gx = 0.0f, gy = 0.0f;
+    if (dn_finite(z)) {
+        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
+        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
+        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
+    }
+    const float l = dn_lum(e0, e1, e2);
+    // 2: reconstruct, reproject, gather H' and the moments (hb0, hb1)
+    const uint32_t id = (uint32_t)key;
+    float mx, my, S, h0, h1, h2, M1, M2, M3;
+    uint32_t len_prev;
+    dn_reproject(prm, tp, x, y, z, id, n0, n1, n2, inst, mat_prev, hin, mx, my, S, h0, h1, h2, M1, M2, M3, len_prev);
+    // 3: blend colour and moments with the same 1 / n'
+    uint32_t np = 1;
+    if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    float mu1 = l, mu2 = l * l;
+    if (np > 1) {
+        h0 = h0 / S; h1 = h1 / S; h2 = h2 / S;
+        M1 = M1 / S; M2 = M2 / S;
+        const float alpha = 1.0f / (float)np, beta = 1.0f - alpha;
+        e0 = alpha * e0 + beta * h0; e1 = alpha * e1 + beta * h1; e2 = alpha * e2 + beta * h2;
+        mu1 = alpha * l + beta * M1;
+        mu2 = alpha * (l * l) + beta * M2;
+    }
+    sc.guide[i] = make_float4(n0, n1, n2, z);
+    sc.grad[i] = make_float2(gx, gy);
+    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
+    sc.ev[0][i] = make_float4(e0, e1, e2, 0.0f);
+    mom[i] = make_float4(dn_lum(e0, e1, e2), mu1, mu2, __uint_as_float(np));
+    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+    // 6: the new history
+    if (dn_finite(z)) {
+        hout.a[i] = make_float4(e0, e1, e2, z);
+        hout.b[i] = make_float4(mu1, mu2, 0.0f, __uint_as_float(id));
+        hout.n[i] = make_float4(n0, n1, n2, __uint_as_float(np));
+    } else {
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    if (motion) motion[i] = make_float2(mx == mx ? mx : qnan, my == my ? my : qnan);
+    if (hlen) hlen[i] = np;
+}
+
+// Step 4 of "Moment denoising": each filtered pixel's variance, mu2 - mu1^2 from its own moments once n' >= MIN_HISTORY, else the
+// 7x7 edge-stopped estimate over its neighbours' moments boosted by 4 / n'. Writes v into ev[0].w (and var, NaN where not filtered).
+__global__ void __launch_bounds__(256) k_dn_moments_variance(const DnParams prm, const float4* __restrict__ guide, const float2* __restrict__ grad,
+                                                             const float4* __restrict__ mom, float4* __restrict__ ev, float* __restrict__ var) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int W = prm.width, H = prm.height, i = y * W + x;
+    const float4 gp = guide[i];
+    if (gp.w != gp.w) { // not filtered
+        if (var) var[i] = __int_as_float(0x7fffffff);
+        return;
+    }
+    const float4 mp = mom[i];
+    const uint32_t np = __float_as_uint(mp.w);
+    float v;
+    if (np >= TRB_DENOISE_MOMENTS_MIN_HISTORY) {
+        v = mp.z - mp.y * mp.y;
+        v = v > 0.0f ? v : 0.0f;
+    } else {
+        const float2 g = grad[i];
+        const bool p_inf = !dn_finite(gp.w), p_nrm = gp.x != 0.0f || gp.y != 0.0f || gp.z != 0.0f;
+        const float denom_l = prm.sigma_l + TRB_DENOISE_EPS_LUMINANCE;
+        float sw = 0.0f, s1 = 0.0f, s2 = 0.0f;
+        for (int dy = -TRB_DENOISE_MOMENTS_RADIUS; dy <= TRB_DENOISE_MOMENTS_RADIUS; ++dy) {
+            const int qy = y + dy;
+            if (qy < 0 || qy >= H) continue;
+            for (int dx = -TRB_DENOISE_MOMENTS_RADIUS; dx <= TRB_DENOISE_MOMENTS_RADIUS; ++dx) {
+                const int qx = x + dx;
+                if (qx < 0 || qx >= W) continue;
+                const int q = qy * W + qx;
+                const float4 gq = guide[q];
+                if (gq.w != gq.w) continue;
+                const float4 mq = mom[q];
+                const float wl = dexp(-(fabsf(mp.x - mq.x) / denom_l));
+                float wn;
+                const bool q_nrm = gq.x != 0.0f || gq.y != 0.0f || gq.z != 0.0f;
+                if (p_nrm != q_nrm) wn = 0.0f;
+                else if (!p_nrm) wn = 1.0f;
+                else {
+                    const float dot = gp.x * gq.x + gp.y * gq.y + gp.z * gq.z;
+                    wn = dot > 0.0f ? dot : 0.0f;
+                    for (uint32_t k = 0; k < prm.normal_squarings; ++k) wn = wn * wn;
+                }
+                float wz;
+                const bool q_inf = !dn_finite(gq.w);
+                if (p_inf != q_inf) wz = 0.0f;
+                else if (p_inf) wz = 1.0f;
+                else wz = dexp(-(fabsf(gp.w - gq.w) / (prm.sigma_z * fabsf(g.x * (float)dx + g.y * (float)dy) + TRB_DENOISE_EPS_DEPTH)));
+                float w = wl * wn;
+                w = w * wz;
+                sw = sw + w;
+                s1 = s1 + w * mq.y;
+                s2 = s2 + w * mq.z;
+            }
+        }
+        const float m1 = s1 / sw, m2 = s2 / sw;
+        v = m2 - m1 * m1;
+        v = v > 0.0f ? v : 0.0f;
+        v = v * (4.0f / (float)np);
+    }
+    reinterpret_cast<float*>(ev + i)[3] = v;
+    if (var) var[i] = v;
 }
 
 // ---- temporal gradients (trb_denoise_temporal_gradient*, include/trb.h "Temporal gradients") --------------------------------------

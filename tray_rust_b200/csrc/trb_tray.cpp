@@ -18,7 +18,9 @@
 // half-sample renders with AOVs and writes the denoised image (trb_denoise; single node, path integrator, 2 spp or more, refused
 // before anything renders otherwise: the wire format carries no AOVs); --denoise-temporal renders the frames in order with one
 // history and seed (S + frame) mod 2^32, denoising each with trb_denoise_temporal (refused where --denoise is, and with --denoise);
-// --temporal-gradients, only with --denoise-temporal, denoises with trb_denoise_temporal_gradient at the frame's seed; a worker address is host[:port],
+// --temporal-gradients, only with --denoise-temporal, denoises with trb_denoise_temporal_gradient at the frame's seed; --denoise-moments
+// renders each frame once with AOVs (1 spp allowed), in order, with one history and seed (S + frame) mod 2^32, denoising it with
+// trb_denoise_moments (single node, path integrator, refused with the other denoise flags); a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -42,7 +44,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise | --denoise-temporal [--temporal-gradients]]\n"
+    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -63,6 +65,9 @@ const char* USAGE =
     "                          frame k is rendered with seed S + k.\n"
     "  --temporal-gradients    With --denoise-temporal only: re-shade a sample of each 3x3 pixel block of the previous frame in\n"
     "                          this one and shorten the history where the lighting changed (animated lights). Single node only.\n"
+    "  --denoise-moments       Render each frame once with albedo, normal and depth (1 sample per pixel is enough) and denoise it\n"
+    "                          with a history of luminance moments over the frame range; frame k is rendered with seed S + k.\n"
+    "                          Single node only, path integrator.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -153,7 +158,7 @@ struct Args {
     std::vector<std::string> workers;
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
-         denoise_temporal = false, temporal_gradients = false;
+         denoise_temporal = false, temporal_gradients = false, denoise_moments = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
 };
 
@@ -204,6 +209,26 @@ struct DenoisedFrame {
     }
 };
 
+// --denoise-moments: the frame's whole sample range into one film with its AOVs, then trb_denoise_moments with the history of the
+// frames before (DESIGN.md §4 "Moment denoising")
+struct MomentsFrame {
+    std::vector<float> colour, albedo, normal, out;
+    std::vector<uint64_t> nearest;
+    explicit MomentsFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history) {
+        std::fill(colour.begin(), colour.end(), 0.0f);
+        std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
+        std::fill(nearest.begin(), nearest.end(), ~0ull);
+        trb_render_cfg cfg{};
+        cfg.spp = spp; cfg.seed = seed; cfg.current_frame = frame;
+        const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
+        tray::check(trb_render_aov(s, &cfg, colour.data(), &aov, nullptr)); // includes Scene::update_frame
+        const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
+        const trb_denoise_moments_output o{out.data(), nullptr, nullptr, nullptr};
+        tray::check(trb_denoise_moments(s, history, &in, nullptr, &o));
+    }
+};
+
 // ---- single node (main.rs:56-109) -------------------------------------------------------------------------------------------
 int single_node(const Args& a, const OutPath& out) {
     Desc desc;
@@ -215,6 +240,8 @@ int single_node(const Args& a, const OutPath& out) {
     if (denoise && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
         return die("%s needs the path integrator: the scene's integrator renders no albedo, normal or depth", flag);
     if (denoise && spp < 2) return die("%s needs at least 2 samples per pixel (two half renders); the scene has %u", flag, spp);
+    if (a.denoise_moments && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("--denoise-moments needs the path integrator: the scene's integrator renders no albedo, normal or depth");
     try {
         tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
         trb_desc_free(desc.d); desc.d = nullptr;
@@ -227,12 +254,18 @@ int single_node(const Args& a, const OutPath& out) {
         std::unique_ptr<DenoisedFrame> dn;
         if (denoise) dn.reset(new DenoisedFrame((size_t)dim.first * dim.second));
         trb_denoise_history* history = nullptr;
-        if (a.denoise_temporal) tray::check(trb_denoise_history_create(scene.handle(), &history));
+        std::unique_ptr<MomentsFrame> mf;
+        if (a.denoise_moments) mf.reset(new MomentsFrame((size_t)dim.first * dim.second));
+        if (a.denoise_temporal || a.denoise_moments) tray::check(trb_denoise_history_create(scene.handle(), &history));
         const std::unique_ptr<trb_denoise_history, trb_status (*)(trb_denoise_history*)> history_owner(history, trb_denoise_history_destroy);
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
             std::vector<uint8_t> img;
-            if (dn) {
+            if (mf) {
+                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history);
+                img.resize((size_t)dim.first * dim.second * 3);
+                tray::check(trb_film_to_srgb8(scene.handle(), mf->out.data(), img.data()));
+            } else if (dn) {
                 if (history) dn->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.temporal_gradients);
                 else dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
                 img.resize((size_t)dim.first * dim.second * 3);
@@ -440,18 +473,21 @@ int master_node(const Args& a, const OutPath& out) {
 } // namespace
 
 int main(int argc, char** argv) {
-    bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false;
+    bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
         denoise = denoise || std::strcmp(argv[i], "--denoise") == 0;
         denoise_temporal = denoise_temporal || std::strcmp(argv[i], "--denoise-temporal") == 0;
+        denoise_moments = denoise_moments || std::strcmp(argv[i], "--denoise-moments") == 0;
     }
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_temporal)
         return die("--denoise-temporal is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && temporal_gradients)
         return die("--temporal-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && denoise_moments)
+        return die("--denoise-moments is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -475,6 +511,7 @@ int main(int argc, char** argv) {
         else if (s == "--denoise") a.denoise = true;
         else if (s == "--denoise-temporal") a.denoise_temporal = true;
         else if (s == "--temporal-gradients") a.temporal_gradients = true;
+        else if (s == "--denoise-moments") a.denoise_moments = true;
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -484,6 +521,10 @@ int main(int argc, char** argv) {
     if (a.master && a.workers.empty()) return die("--master needs at least one worker address");
     if (!a.master && !a.workers.empty()) return die("unexpected argument '%s' (worker addresses follow --master)", a.workers[0].c_str());
     if (a.master && (a.has_seed || a.has_spp || a.has_device)) return die("--seed, --spp and --device are the workers' options: pass them to each worker");
+    if (a.master && a.denoise_moments)
+        return die("--denoise-moments is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.denoise_moments && (a.denoise || a.denoise_temporal || a.temporal_gradients))
+        return die("--denoise-moments excludes --denoise, --denoise-temporal and --temporal-gradients: choose one denoiser");
     if (a.master && a.denoise) return die("--denoise is not available with --master: the wire format carries no albedo, normal or depth");
     if (a.denoise && a.has_spp && a.spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders)");
     if (a.denoise && a.denoise_temporal) return die("--denoise and --denoise-temporal exclude each other: choose one");
