@@ -656,7 +656,6 @@ void launch_shade(trb_scene* s, const trb::RenderParams& rp, const trb::WfState&
     const Tuning& tu = s->tune;
     const bool anim = s->ds.has_anim != 0;
     const unsigned shade_grid = (unsigned)s->sm_count * 4;
-    constexpr int MB = MODE == 2 ? 2 : 0; // k_wf_shade_b: the renders' two modes shade alike
     // per scene (shade_split < 0): split when the scene mixes material kinds, and also when it is all matte — the matte instantiations of
     // _b / _c carry less code and fewer live values than the fused kernel; other one-kind scenes stay fused
     const bool split_auto = s->mixed_materials || (tu.shade_sort && tu.shade_kind && s->material_kinds == (1u << TRB_MAT_MATTE));
@@ -667,15 +666,15 @@ void launch_shade(trb_scene* s, const trb::RenderParams& rp, const trb::WfState&
         const uint32_t rest = tu.shade_sort ? (s->material_kinds & ~own) : all;
         if (anim) {
             trb::k_wf_shade_a<MODE, true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round);
-            if (own) trb::k_wf_shade_b<true, 4, TRB_MAT_MATTE, MB><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, own);
-            if (rest) trb::k_wf_shade_b<true, 3, -1, MB><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+            if (own) trb::k_wf_shade_b<true, 4, TRB_MAT_MATTE><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_b<true, 3><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
             if (own) trb::k_wf_shade_c<MODE, true, 6, TRB_MAT_MATTE><<<(unsigned)s->sm_count * 6, 128, 0, st>>>(s->ds, rp, wf, round, own);
             if (rest) trb::k_wf_shade_c<MODE, true, 4><<<shade_grid, 128, 0, st>>>(s->ds, rp, wf, round, rest);
         } else {
             const unsigned ga = (unsigned)s->sm_count * 6, gb = (unsigned)s->sm_count * 5, gc = (unsigned)s->sm_count * 6;
             trb::k_wf_shade_a<MODE, false, 6><<<ga, 128, 0, st>>>(s->ds, rp, wf, round);
-            if (own) trb::k_wf_shade_b<false, 5, TRB_MAT_MATTE, MB><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, own);
-            if (rest) trb::k_wf_shade_b<false, 5, -1, MB><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, rest);
+            if (own) trb::k_wf_shade_b<false, 5, TRB_MAT_MATTE><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, own);
+            if (rest) trb::k_wf_shade_b<false, 5><<<gb, 128, 0, st>>>(s->ds, rp, wf, round, rest);
             if (own) trb::k_wf_shade_c<MODE, false, 6, TRB_MAT_MATTE><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, own);
             if (rest) trb::k_wf_shade_c<MODE, false, 6><<<gc, 128, 0, st>>>(s->ds, rp, wf, round, rest);
         }
@@ -785,6 +784,7 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
     trb::WfState wf = s->wf;
     wf.n_paths = (uint32_t)n_paths; // Adaptive passes: the worst case (the stride of the q_mid lists); their kernels read the live count on the device
     wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
+    if (!tu.sort) wf.bounds = nullptr; // the origin boxes only size the ray sort's grid: no box updates when sorting is off
     if (s->integrator.type != TRB_INTEGRATOR_PATH) { // Whitted / NormalsDebug: one thread per camera sample, then the same film kernel
         const unsigned grid = (unsigned)std::min<size_t>((n_paths + 127) / 128, (size_t)s->sm_count * 8);
         const auto kernel = mode == 0 ? simple_integrator_kernel<0>(s) : simple_integrator_kernel<1>(s);
@@ -1080,6 +1080,7 @@ trb_status illum_passes(trb_scene* s, size_t n, const trb_illum_ray* d_rays, uin
         trb::WfState wf = s->wf;
         wf.n_paths = (uint32_t)(m * spp);
         wf.mid_keyed = s->tune.shade_sort ? 1u : 0u;
+        if (!s->tune.sort) wf.bounds = nullptr; // as launch_wavefront
         if (s->integrator.type != TRB_INTEGRATOR_PATH) {
             const unsigned grid = (unsigned)std::min<size_t>((wf.n_paths + 127) / 128, (size_t)s->sm_count * 8);
             simple_integrator_kernel<2>(s)<<<grid, 128, 0, st>>>(s->ds, rp, wf.rad, wf.n_paths, s->integrator.type, flags, d_rays + b);

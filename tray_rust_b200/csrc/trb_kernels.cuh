@@ -2066,7 +2066,7 @@ __global__ void __launch_bounds__(256) k_wf_generate(const __grid_constant__ DSc
         wf.counters[WF_N_ACTIVE] = n; wf.counters[WF_N_CONT] = n;
         if (rp.stats) { atomicAdd(&rp.stats->camera_samples, (unsigned long long)n); }
     }
-    if (blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid
+    if (wf.bounds && blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid (nullptr: sorting off)
         uint32_t* b = wf.bounds + threadIdx.x * 8;
         b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
     }
@@ -2366,7 +2366,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade(const __grid_constant__ 
         wf_push(wf.q_mis, &cnt_n[WF_N_MIS], push_mis, p);
         wf_push(act_next, &cnt_n[WF_N_ACTIVE], push_active && !push_ending, p);
         wf_push(ending_next, &cnt_n[WF_N_ENDING], push_ending, p);
-        wf_bounds_add(wf.bounds + (round + 1) * 8, push_active, new_org);
+        if (wf.bounds) wf_bounds_add(wf.bounds + (round + 1) * 8, push_active, new_org); // ray sorting's origin boxes (nullptr: sorting off)
     }
 }
 
@@ -2523,9 +2523,10 @@ __global__ void __launch_bounds__(128) k_simple_integrator(const __grid_constant
 //   k_wf_shade_c  BSDF sample, throughput, Russian roulette -> continuation ray; decides whether the path goes on
 // Every value is computed by the same device functions in the same order as in the fused kernel: bit-identical results.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void load_frame(const WfState& wf, uint32_t p, Frame& fr, uint32_t& inst, float& u, float& v) {
+// the shading frame k_wf_shade_a left: f_p.w the hit's material index, f_n.w / f_t.w the hit's (u, v), f_b.w the path's stream hash
+__device__ __forceinline__ void load_frame(const WfState& wf, uint32_t p, Frame& fr, uint32_t& material, uint32_t& hs, float& u, float& v) {
     const float4 a = wf.f_p[p], n = wf.f_n[p], t = wf.f_t[p], b = wf.f_b[p];
-    fr.p = mk(a.x, a.y, a.z); inst = __float_as_uint(a.w); u = n.w; v = t.w;
+    fr.p = mk(a.x, a.y, a.z); material = __float_as_uint(a.w); u = n.w; v = t.w; hs = __float_as_uint(b.w);
     fr.n = mk(n.x, n.y, n.z); fr.tan = mk(t.x, t.y, t.z); fr.bitan = mk(b.x, b.y, b.z);
 }
 
@@ -2571,6 +2572,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
                 const uint4 h4 = wf.hit[p];
                 if (h4.x == TRB_MISS) done = true; // primary miss: black sample (multithreaded.rs:101-102); later: `None => break`
                 else {
+                    const uint32_t material = __ldg(&sc.instances[h4.x].material); // handed to _b / _c in f_p.w
                     Ray ray; ray.o = org; ray.d = mk(c4.x, c4.y, c4.z); ray.tmin = 0.0f; ray.tmax = c4.w;
                     HitRec h; h.t = c4.w; h.inst = h4.x; h.prim = h4.y; h.b1 = __uint_as_float(h4.z); h.b2 = __uint_as_float(h4.w);
                     Surf s;
@@ -2581,13 +2583,14 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
                     bounce_emission<ANIM>(sc, h.inst, ray.d, first_ng, round, (fl & WF_F_SPECULAR) != 0, mk(th4.x, th4.y, th4.z), time, illum);
                     Frame fr;
                     make_frame(s, fr);
-                    wf.f_p[p] = make_float4(fr.p.x, fr.p.y, fr.p.z, __uint_as_float(h.inst));
+                    const uint32_t hs = MODE == 2 ? __float_as_uint(il4.w) : wf_stream<MODE>(sc, rp, wf, p); // handed to _b / _c in f_b.w
+                    wf.f_p[p] = make_float4(fr.p.x, fr.p.y, fr.p.z, __uint_as_float(material));
                     wf.f_n[p] = make_float4(fr.n.x, fr.n.y, fr.n.z, s.u); // .w: the hit's (u, v) for image textures
                     wf.f_t[p] = make_float4(fr.tan.x, fr.tan.y, fr.tan.z, s.v);
-                    wf.f_b[p] = make_float4(fr.bitan.x, fr.bitan.y, fr.bitan.z, 0.0f);
+                    wf.f_b[p] = make_float4(fr.bitan.x, fr.bitan.y, fr.bitan.z, __uint_as_float(hs));
                     wf.illum[p] = make_float4(illum.x, illum.y, illum.z, MODE == 2 ? il4.w : 0.0f);
                     push_mid = true;
-                    if (wf.mid_keyed) mid_key = __ldg(&sc.materials[__ldg(&sc.instances[h.inst].material)].type) & (WF_MID_BUCKETS - 1u);
+                    if (wf.mid_keyed) mid_key = __ldg(&sc.materials[material].type) & (WF_MID_BUCKETS - 1u);
                 }
             }
             if (done) finish_sample(sc, rp, wf, p, illum, MODE);
@@ -2597,9 +2600,9 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_a(const __grid_constant_
 }
 
 // KIND >= 0: the instantiation compiled for that material kind alone; it drains that kind's bucket. KIND = -1: any kind; drains the
-// buckets of `bucket_mask` (the kinds the scene uses that have no instantiation of their own). MODE 2: illumination queries (the
-// stream hash the path carries); the renders' modes 0 and 1 shade alike and share MODE 0.
-template <bool ANIM, int MINB, int KIND = -1, int MODE = 0>
+// buckets of `bucket_mask` (the kinds the scene uses that have no instantiation of their own). Every mode shades alike here: the
+// stream hash comes with the frame.
+template <bool ANIM, int MINB, int KIND = -1>
 __global__ void __launch_bounds__(128, MINB) k_wf_shade_b(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
                                                      uint32_t round, uint32_t bucket_mask) {
     uint32_t* cnt_r = wf.counters + round * WF_CNT;
@@ -2620,13 +2623,12 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_b(const __grid_constant_
         bool push_shadow = false, push_mis = false;
         if (i < n) {
             p = q_mid[i];
-            Frame fr; uint32_t inst; float tu, tv;
-            load_frame(wf, p, fr, inst, tu, tv);
+            Frame fr; uint32_t material, hs; float tu, tv;
+            load_frame(wf, p, fr, material, hs, tu, tv);
             const float4 c4 = wf.cont[p], th4 = wf.thr[p];
             const f3 wo = -mk(c4.x, c4.y, c4.z);
             Mat m;
-            load_mat_at(sc, __ldg(&sc.instances[inst].material), tu, tv, th4.w, m);
-            const uint32_t hs = wf_stream<MODE>(sc, rp, wf, p);
+            load_mat_at(sc, material, tu, tv, th4.w, m);
             DirectSetup ds; uint32_t light;
             bounce_direct<ANIM, KIND>(sc, m, fr, wo, round, hs, th4.w, ds, light, wf_xf_row<ANIM>(wf, p), rp.ld_offset);
             push_shadow = ds.has_shadow; push_mis = ds.has_mis;
@@ -2666,13 +2668,12 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
         f3 new_org = splat(0.0f);
         if (i < n) {
             p = q_mid[i];
-            Frame fr; uint32_t inst; float tu, tv;
-            load_frame(wf, p, fr, inst, tu, tv);
+            Frame fr; uint32_t material, hs; float tu, tv;
+            load_frame(wf, p, fr, material, hs, tu, tv);
             const float4 c4 = wf.cont[p], th4 = wf.thr[p];
             const f3 wo = -mk(c4.x, c4.y, c4.z);
             Mat m;
-            load_mat_at(sc, __ldg(&sc.instances[inst].material), tu, tv, th4.w, m);
-            const uint32_t hs = wf_stream<MODE>(sc, rp, wf, p);
+            load_mat_at(sc, material, tu, tv, th4.w, m);
             ScatterOut so;
             bounce_scatter<KIND>(sc, m, fr, wo, round, hs, mk(th4.x, th4.y, th4.z), so, rp.ld_offset);
             const uint32_t fb = __float_as_uint(wf.org[p].w); // WF_F_SHADOW | WF_F_MIS from k_wf_shade_b
@@ -2690,7 +2691,7 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
         }
         wf_push(wf.q_cont, &cnt_n[WF_N_CONT], push_cont, p);
         wf_push(act_next, &cnt_n[WF_N_ACTIVE], push_active, p);
-        wf_bounds_add(wf.bounds + (round + 1) * 8, push_active, new_org);
+        if (wf.bounds) wf_bounds_add(wf.bounds + (round + 1) * 8, push_active, new_org); // ray sorting's origin boxes (nullptr: sorting off)
     }
     }
 }
@@ -2990,7 +2991,7 @@ __global__ void __launch_bounds__(256) k_illum_load(const __grid_constant__ WfSt
         wf.counters[WF_N_ACTIVE] = n; wf.counters[WF_N_CONT] = n;
         if (stats) atomicAdd(&stats->camera_samples, (unsigned long long)n);
     }
-    if (blockIdx.x == 0 && threadIdx.x < 64) {
+    if (wf.bounds && blockIdx.x == 0 && threadIdx.x < 64) {
         uint32_t* b = wf.bounds + threadIdx.x * 8;
         b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
     }
@@ -3271,7 +3272,7 @@ __global__ void __launch_bounds__(256) k_wf_generate_ad(const __grid_constant__ 
         if (lane == 0 && m && rp.stats) atomicAdd(&rp.stats->camera_samples, (unsigned long long)__popc(m));
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) { wf.counters[WF_N_ACTIVE] = n; wf.counters[WF_N_PATHS] = n; } // shade round 0 walks every path of the pass
-    if (blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid
+    if (wf.bounds && blockIdx.x == 0 && threadIdx.x < 64) { // empty origin boxes for every round's sort grid (nullptr: sorting off)
         uint32_t* b = wf.bounds + threadIdx.x * 8;
         b[0] = b[1] = b[2] = b[3] = 0xffffffffu; b[4] = b[5] = b[6] = b[7] = 0u;
     }
