@@ -959,7 +959,7 @@ trb_status trb_denoise_temporal_device(trb_scene* scene, trb_denoise_history* hi
  * 0.7152 x.g + 0.0722 x.b of the sample's radiance clamped to [0, 1] per channel; plus the frame's cam_world at shutter-open, its
  * shutter_open and the call's seed. The records are valid only if the previous call on the history was a gradient call of the same
  * object generation and film size; otherwise (first call, after reset, after trb_denoise_temporal or trb_denoise_moments, after
- * replace_objects) there are
+ * replace_objects, after trb_denoise_moments_gradient, whose history is of the moment family) there are
  * no gradients and lambda is 0 everywhere. Per call, float32, left to right, never contracted:
  *   1. Re-shade. For each valid record j (i below both instance counts): p_w' = mat_cur[i] . p_o, q = cam_inv_cur . p_w' (points as
  *      in "Temporal denoising"). Kept if q.z > 0, r = ((X - X0) / (X1 - X0) * W, (Y - Y1) / (Y0 - Y1) * H) with X = q.x / (q.z tan),
@@ -1077,6 +1077,45 @@ trb_status trb_denoise_moments(trb_scene* scene, trb_denoise_history* history, c
 trb_status trb_denoise_moments_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* d_in,
                                       const trb_denoise_temporal_params* params, const trb_denoise_moments_output* d_out,
                                       void* cuda_stream);
+
+/* -- Moment gradients: temporal gradients on the moment denoiser, so a 1-spp history drops where the lighting changed -------------
+ * (DESIGN.md §4 "Moment gradients"). A-SVGF (Schied, Peters, Dachsbacher 2018) is SVGF at one sample per pixel with temporal
+ * gradients: "Moment denoising" with the lambda of "Temporal gradients". Per call:
+ *   - steps 1, 2 and 4 of "Temporal gradients" run unchanged: re-shade the previous records at the previous seed, reconstruct lambda
+ *     on the 3x3 stratum grid (normal_w and nearest of the frame), and record this frame's samples at `seed`;
+ *   - "Moment denoising" runs with one change at step 3: where there is history, n' = min((uint32)floorf((1 - lambda) *
+ *     (float)len_prev) + 1, max_history) with lambda taken from the pixel's stratum, and ē, mu1 and mu2 blend with that 1 / n'.
+ *     A shortened history falls below TRB_DENOISE_MOMENTS_MIN_HISTORY exactly where the lighting changed, so step 4's 7x7 spatial
+ *     variance with its 4 / n' boost takes over there. Lambda 0 everywhere gives trb_denoise_moments's pixel bit for bit, lambda 1
+ *     its max_history 1 pixel.
+ * The records are valid only if the previous call on the history was a moment gradient call of the same object generation and film
+ * size; otherwise (first call, after reset, after replace_objects, trb_denoise_moments or any half-film call) lambda is 0
+ * everywhere. A half-film call (trb_denoise_temporal*, trb_denoise_temporal_gradient*) after a moment gradient call finds no
+ * history, as after trb_denoise_moments. The history and scratch sizes are those of the two calls combined: 96 bytes per pixel,
+ * 456 bytes per stratum and 88 bytes per pixel of scratch. */
+
+/* trb_denoise_moments_output's four buffers, plus lambda (width*height floats, may be NULL): each pixel's lambda. */
+typedef struct trb_denoise_moments_gradient_output {
+    float* rgbw;
+    float* motion;
+    uint32_t* history_length;
+    float* variance;
+    float* lambda;
+} trb_denoise_moments_gradient_output;
+
+/* trb_denoise_moments with temporal gradients: the same inputs, history, checks and statuses (the parameters first, with no scene
+ * needed, and a failed call leaves the history as it was), plus TRB_INVALID_ARG for iterations above 6 or a lambda output that
+ * overlaps another buffer. `seed` seeds this frame's gradient samples (render_denoised_moments(gradients=True) passes the frame's
+ * seed). HOST buffers; blocking. */
+trb_status trb_denoise_moments_gradient(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* in,
+                                        const trb_denoise_gradient_params* params, uint32_t seed,
+                                        const trb_denoise_moments_gradient_output* out);
+
+/* The same with DEVICE buffers (the alignment of trb_denoise_moments_device, lambda 4-byte aligned), enqueued on cuda_stream under
+ * trb_render_device's one-stream rule. No host synchronisation, except when scratch, history or the wavefront state grows. */
+trb_status trb_denoise_moments_gradient_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* d_in,
+                                               const trb_denoise_gradient_params* params, uint32_t seed,
+                                               const trb_denoise_moments_gradient_output* d_out, void* cuda_stream);
 
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus

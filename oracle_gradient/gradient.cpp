@@ -186,6 +186,50 @@ void reconstruct(uint32_t W, uint32_t H, const std::vector<uint64_t>& slot, cons
     }
 }
 
+/* Steps 1-3 of "Temporal denoising" for the valid pixel P at (x, y) with instance id: the motion (left as it is without one), S, the
+ * tap-weighted sums sa and sb of the history's ha and hb (3 each, not yet divided by S) and len_prev. oracle_moment_gradient calls it
+ * over a history whose ha holds ē and hb (mu1, mu2, 0). */
+void gradient_gather(long W, long H, long x, long y, const Px& P, uint32_t id, const orc_gradient_frame* f, const orc_gradient_history* h,
+                     const GradPrm& t, float& mx, float& my, float& S, float* sa, float* sb, uint32_t& len_prev) {
+    if (!(h->has_prev && id < h->n_instances && id < f->n_instances && fin(P.z))) return;
+    const M4 cam_mat = gm4(f->cam_mat), px_to_cam = gm4(f->px_to_cam), cam_inv_prev = gm4(h->cam_inv);
+    float X0, X1, Y0, Y1;
+    window((uint32_t)W, (uint32_t)H, X0, X1, Y0, Y1);
+    const V3 pc = Transform::mul_point(px_to_cam, V3((float)x + 0.5f, (float)y + 0.5f, 0.0f));
+    const V3 dir = Transform::mul_vector(cam_mat, normalized(V3(f->scaling[0], f->scaling[1], f->scaling[2]) * pc));
+    const V3 o = Transform::mul_point(cam_mat, V3(0.0f));
+    const V3 pw(o.x + P.z * dir.x, o.y + P.z * dir.y, o.z + P.z * dir.z);
+    const V3 po = Transform::mul_point(gm4(f->inv + 16 * (size_t)id), pw);
+    const V3 pp = Transform::mul_point(gm4(h->mats.data() + 16 * (size_t)id), po);
+    const V3 q = Transform::mul_point(cam_inv_prev, pp);
+    if (!(q.z > 0.0f)) return;
+    const float X = q.x / (q.z * h->tan_fov), Y = q.y / (q.z * h->tan_fov);
+    const float rx = (X - X0) / (X1 - X0) * (float)W, ry = (Y - Y1) / (Y0 - Y1) * (float)H;
+    mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
+    const float ql = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
+    const float cx = rx - 0.5f, cy = ry - 0.5f, fx = std::floor(cx), fy = std::floor(cy), ax = cx - fx, ay = cy - fy;
+    const int ox[4] = {0, 1, 0, 1}, oy[4] = {0, 0, 1, 1};
+    const float wts[4] = {(1.0f - ax) * (1.0f - ay), ax * (1.0f - ay), (1.0f - ax) * ay, ax * ay};
+    for (int k = 0; k < 4; ++k) {
+        const float tx = fx + (float)ox[k], ty = fy + (float)oy[k];
+        if (!(tx >= 0.0f && tx <= (float)W - 1.0f && ty >= 0.0f && ty <= (float)H - 1.0f)) continue;
+        const long j = (long)ty * W + (long)tx;
+        if (h->len[j] == 0 || h->inst[j] != id) continue;
+        if (!(std::fabs(h->z[j] - ql) <= t.depth_tolerance * ql)) continue;
+        const float* tn = &h->n[3 * j];
+        const bool t_nrm = tn[0] != 0.0f || tn[1] != 0.0f || tn[2] != 0.0f;
+        if (t_nrm != P.has_n) continue;
+        if (P.has_n && !(tn[0] * P.n[0] + tn[1] * P.n[1] + tn[2] * P.n[2] >= t.normal_threshold)) continue;
+        const float w = wts[k];
+        S = S + w;
+        for (int c = 0; c < 3; ++c) {
+            sa[c] = sa[c] + w * h->ha[3 * j + c];
+            sb[c] = sb[c] + w * h->hb[3 * j + c];
+        }
+        if (w > 0.0f && h->len[j] > len_prev) len_prev = h->len[j];
+    }
+}
+
 /* "Temporal denoising" with step 3's lambda (lam_s per stratum; lam_px per pixel out) */
 void temporal_lambda(uint32_t width, uint32_t height, const orc_gradient_frame* f, orc_gradient_history* h, const trb_denoise_input* in,
                      const trb_denoise_params& p, int squarings, const GradPrm& t, const float* lam_s, float* rgbw, float* motion,
@@ -195,9 +239,6 @@ void temporal_lambda(uint32_t width, uint32_t height, const orc_gradient_frame* 
     std::vector<float> e, v, ea, eb;
     denoise_prepare(W, H, in, px, e, v, &ea, &eb);
     const float qnan = dm_from_bits(0x7fffffffu);
-    const M4 cam_mat = gm4(f->cam_mat), px_to_cam = gm4(f->px_to_cam), cam_inv_prev = gm4(h->cam_inv);
-    float X0, X1, Y0, Y1;
-    window(width, height, X0, X1, Y0, Y1);
     std::vector<float> nha(N * 3), nhb(N * 3), nn(N * 3), nz(N);
     std::vector<uint32_t> ninst(N), nlen(N, 0u);
     for (long y = 0; y < H; ++y)
@@ -212,42 +253,7 @@ void temporal_lambda(uint32_t width, uint32_t height, const orc_gradient_frame* 
                 const uint32_t id = (uint32_t)in->nearest[i];
                 float S = 0.0f, sa[3] = {0, 0, 0}, sb[3] = {0, 0, 0};
                 uint32_t len_prev = 0;
-                if (h->has_prev && id < h->n_instances && id < f->n_instances && fin(P.z)) {
-                    const V3 pc = Transform::mul_point(px_to_cam, V3((float)x + 0.5f, (float)y + 0.5f, 0.0f));
-                    const V3 dir = Transform::mul_vector(cam_mat, normalized(V3(f->scaling[0], f->scaling[1], f->scaling[2]) * pc));
-                    const V3 o = Transform::mul_point(cam_mat, V3(0.0f));
-                    const V3 pw(o.x + P.z * dir.x, o.y + P.z * dir.y, o.z + P.z * dir.z);
-                    const V3 po = Transform::mul_point(gm4(f->inv + 16 * (size_t)id), pw);
-                    const V3 pp = Transform::mul_point(gm4(h->mats.data() + 16 * (size_t)id), po);
-                    const V3 q = Transform::mul_point(cam_inv_prev, pp);
-                    if (q.z > 0.0f) {
-                        const float X = q.x / (q.z * h->tan_fov), Y = q.y / (q.z * h->tan_fov);
-                        const float rx = (X - X0) / (X1 - X0) * (float)W, ry = (Y - Y1) / (Y0 - Y1) * (float)H;
-                        mx = rx - ((float)x + 0.5f); my = ry - ((float)y + 0.5f);
-                        const float ql = std::sqrt(q.x * q.x + q.y * q.y + q.z * q.z);
-                        const float cx = rx - 0.5f, cy = ry - 0.5f, fx = std::floor(cx), fy = std::floor(cy), ax = cx - fx, ay = cy - fy;
-                        const int ox[4] = {0, 1, 0, 1}, oy[4] = {0, 0, 1, 1};
-                        const float wts[4] = {(1.0f - ax) * (1.0f - ay), ax * (1.0f - ay), (1.0f - ax) * ay, ax * ay};
-                        for (int k = 0; k < 4; ++k) {
-                            const float tx = fx + (float)ox[k], ty = fy + (float)oy[k];
-                            if (!(tx >= 0.0f && tx <= (float)W - 1.0f && ty >= 0.0f && ty <= (float)H - 1.0f)) continue;
-                            const long j = (long)ty * W + (long)tx;
-                            if (h->len[j] == 0 || h->inst[j] != id) continue;
-                            if (!(std::fabs(h->z[j] - ql) <= t.depth_tolerance * ql)) continue;
-                            const float* tn = &h->n[3 * j];
-                            const bool t_nrm = tn[0] != 0.0f || tn[1] != 0.0f || tn[2] != 0.0f;
-                            if (t_nrm != P.has_n) continue;
-                            if (P.has_n && !(tn[0] * P.n[0] + tn[1] * P.n[1] + tn[2] * P.n[2] >= t.normal_threshold)) continue;
-                            const float w = wts[k];
-                            S = S + w;
-                            for (int c = 0; c < 3; ++c) {
-                                sa[c] = sa[c] + w * h->ha[3 * j + c];
-                                sb[c] = sb[c] + w * h->hb[3 * j + c];
-                            }
-                            if (w > 0.0f && h->len[j] > len_prev) len_prev = h->len[j];
-                        }
-                    }
-                }
+                gradient_gather(W, H, x, y, P, id, f, h, t, mx, my, S, sa, sb, len_prev);
                 np = 1u;
                 if (S > 0.0f) np = std::min((uint32_t)std::floor((1.0f - lam) * (float)len_prev) + 1u, t.max_history);
                 if (np > 1) {
@@ -276,6 +282,92 @@ void temporal_lambda(uint32_t width, uint32_t height, const orc_gradient_frame* 
     h->n_instances = f->n_instances;
     h->mats.assign(f->mat, f->mat + 16 * (size_t)f->n_instances);
     h->has_prev = true; h->bound = true; h->width = width; h->height = height;
+}
+
+}  // namespace
+
+namespace {
+
+/* The frame of an oracle scene after orc_scene_update_frame (the camera's active one): cam_world and every instance's transform at
+ * shutter-open, from the oracle's own matrices (inv and mat hold the instances' matrices, which f points at) */
+void scene_gradient_frame(orc_scene* s, orc_gradient_frame& f, std::vector<float>& inv, std::vector<float>& mat) {
+    const Camera& cam = s->cameras[s->active_camera];
+    const Transform cw = cam.cam_world.transform(cam.shutter_open);
+    const size_t n = s->geom.instances.size();
+    inv.assign(16 * n, 0.0f); mat.assign(16 * n, 0.0f);
+    for (size_t k = 0; k < n; ++k) {
+        const Transform tr = s->geom.instances[k].transform.transform(cam.shutter_open);
+        std::memcpy(&mat[16 * k], tr.mat.m, 64); std::memcpy(&inv[16 * k], tr.inv.m, 64);
+    }
+    std::memcpy(f.px_to_cam, cam.px_to_cam.mat.m, 64);
+    std::memcpy(f.cam_mat, cw.mat.m, 64);
+    std::memcpy(f.cam_inv, cw.inv.m, 64);
+    f.scaling[0] = cam.scaling.x; f.scaling[1] = cam.scaling.y; f.scaling[2] = cam.scaling.z;
+    f.n_instances = (uint32_t)n; f.inv = inv.data(); f.mat = mat.data(); f.shutter_open = cam.shutter_open;
+}
+
+/* Steps 1-2 with the scene: the history's records re-shaded by orc_illumination, lambda per stratum (0 without valid records) */
+void scene_lambda(orc_scene* s, const orc_gradient_history* h, const orc_gradient_frame& f, const float* normal_w, const uint64_t* nearest,
+                  const GradPrm& t, std::vector<float>& lam) {
+    const uint32_t W = s->film.width, H = s->film.height, S = ((W + 2) / 3) * ((H + 2) / 3);
+    lam.assign(S, 0.0f);
+    if (h->has_prev && h->gr_valid) {
+        std::vector<uint64_t> slot;
+        project(W, H, &f, h->n_instances, h->rec.data(), S, nearest, t.depth_tolerance, slot);
+        const bool cam_same = std::memcmp(h->gr_cam_mat, f.cam_mat, 64) == 0;
+        std::vector<trb_illum_ray> rays;
+        std::vector<uint32_t> tgt;
+        for (uint32_t k = 0; k < S; ++k)
+            if (slot[k] != ~0ull) {
+                rays.push_back(reshade_ray(&f, h->rec[(uint32_t)slot[k]], h->mats.data(), cam_same, f.shutter_open - h->gr_shutter_open));
+                tgt.push_back(k);
+            }
+        std::vector<float> rgb(3 * rays.size()), lc(S, 0.0f);
+        if (!rays.empty()) orc_illumination(s, rays.size(), rays.data(), 1, h->gr_seed, rgb.data(), 1, nullptr);
+        for (size_t k = 0; k < rays.size(); ++k) lc[tgt[k]] = glum(rgb[3 * k], rgb[3 * k + 1], rgb[3 * k + 2]);
+        reconstruct(W, H, slot, h->rec.data(), lc.data(), normal_w, nearest, t.normal_threshold, t.iterations, nullptr, lam.data());
+    } else {
+        std::vector<uint64_t> slot(S, ~0ull);
+        std::vector<float> lc(S, 0.0f);
+        reconstruct(W, H, slot, nullptr, lc.data(), normal_w, nearest, t.normal_threshold, t.iterations, nullptr, lam.data());
+    }
+}
+
+/* Step 4 with the scene: this frame's samples at `seed` into the history's records, which become valid */
+void scene_record(orc_scene* s, orc_gradient_history* h, const orc_gradient_frame& f, uint32_t seed) {
+    const uint32_t W = s->film.width, H = s->film.height, gw = (W + 2) / 3, gh = (H + 2) / 3, S = gw * gh;
+    const Camera& cam = s->cameras[s->active_camera];
+    std::vector<trb_query_ray> q(S);
+    std::vector<trb_illum_ray> il(S);
+    for (uint32_t k = 0; k < S; ++k) {
+        const uint32_t sx = k % gw, sy = k / gw, cwd = std::min(3u, W - 3 * sx), chd = std::min(3u, H - 3 * sy);
+        const uint32_t pick = dm_rng(seed, k, 0xfffffffeu, 0u) % (cwd * chd);
+        const uint32_t px = 3 * sx + pick % cwd, py = 3 * sy + pick / cwd, pixel = py * W + px;
+        const PixelStreams st = pixel_streams(seed, pixel);
+        const uint32_t ip = dm_permute(0, 1, st.kpos);
+        const float fx = van_der_corput(ip, st.scr0) + (float)px, fy = sobol(ip, st.scr1) + (float)py;
+        const float tm = van_der_corput(dm_permute(0, 1, st.ktime), st.scrt);
+        const Ray r = cam.generate_ray(fx, fy, tm);
+        q[k] = trb_query_ray{{r.o.x, r.o.y, r.o.z}, {r.d.x, r.d.y, r.d.z}, r.min_t, r.max_t, r.time, {0, 0, 0}};
+        il[k] = trb_illum_ray{{r.o.x, r.o.y, r.o.z}, {r.d.x, r.d.y, r.d.z}, r.min_t, r.max_t, r.time, pixel, 0, 0};
+    }
+    std::vector<trb_intersection> hits(S);
+    std::vector<float> rgb(3 * (size_t)S);
+    orc_intersect_records(s, S, q.data(), hits.data(), nullptr);
+    orc_illumination(s, S, il.data(), 1, seed, rgb.data(), 1, nullptr);
+    h->rec.assign(S, orc_gradient_record{});
+    for (uint32_t k = 0; k < S; ++k) {
+        orc_gradient_record& r = h->rec[k];
+        r.inst = hits[k].inst;
+        if (r.inst == TRB_MISS) continue;
+        const V3 po = Transform::mul_point(gm4(f.inv + 16 * (size_t)r.inst), V3(hits[k].p[0], hits[k].p[1], hits[k].p[2]));
+        r.p_o[0] = po.x; r.p_o[1] = po.y; r.p_o[2] = po.z;
+        for (int c = 0; c < 3; ++c) { r.o[c] = il[k].o[c]; r.d[c] = il[k].d[c]; }
+        r.time = il[k].time; r.key = il[k].key;
+        r.lum = glum(rgb[3 * k], rgb[3 * k + 1], rgb[3 * k + 2]);
+    }
+    h->gr_valid = true; h->gr_seed = seed; h->gr_shutter_open = f.shutter_open;
+    std::memcpy(h->gr_cam_mat, f.cam_mat, 64);
 }
 
 }  // namespace
@@ -328,78 +420,15 @@ int orc_denoise_temporal_gradient(orc_scene* s, orc_gradient_history* h, const t
     GradPrm t;
     if (!gradient_params(params, p, squarings, t)) return TRB_INVALID_ARG;
     if (!s || s->active_camera < 0) { g_err = "update_frame must be called before a temporal denoise"; return TRB_INVALID_ARG; }
-    const uint32_t W = s->film.width, H = s->film.height, gw = (W + 2) / 3, gh = (H + 2) / 3, S = gw * gh;
+    const uint32_t W = s->film.width, H = s->film.height;
     if (h->bound && (h->width != W || h->height != H)) return TRB_INVALID_ARG;
-    const Camera& cam = s->cameras[s->active_camera];
-    const Transform cw = cam.cam_world.transform(cam.shutter_open);
-    const size_t n = s->geom.instances.size();
-    std::vector<float> inv(16 * n), mat(16 * n);
-    for (size_t k = 0; k < n; ++k) {
-        const Transform tr = s->geom.instances[k].transform.transform(cam.shutter_open);
-        std::memcpy(&mat[16 * k], tr.mat.m, 64); std::memcpy(&inv[16 * k], tr.inv.m, 64);
-    }
     orc_gradient_frame f;
-    std::memcpy(f.px_to_cam, cam.px_to_cam.mat.m, 64);
-    std::memcpy(f.cam_mat, cw.mat.m, 64);
-    std::memcpy(f.cam_inv, cw.inv.m, 64);
-    f.scaling[0] = cam.scaling.x; f.scaling[1] = cam.scaling.y; f.scaling[2] = cam.scaling.z;
-    f.n_instances = (uint32_t)n; f.inv = inv.data(); f.mat = mat.data(); f.shutter_open = cam.shutter_open;
-    /* 1-2 */
-    std::vector<float> lam(S, 0.0f);
-    if (h->has_prev && h->gr_valid) {
-        std::vector<uint64_t> slot;
-        project(W, H, &f, h->n_instances, h->rec.data(), S, in->nearest, t.depth_tolerance, slot);
-        const bool cam_same = std::memcmp(h->gr_cam_mat, f.cam_mat, 64) == 0;
-        std::vector<trb_illum_ray> rays;
-        std::vector<uint32_t> tgt;
-        for (uint32_t k = 0; k < S; ++k)
-            if (slot[k] != ~0ull) {
-                rays.push_back(reshade_ray(&f, h->rec[(uint32_t)slot[k]], h->mats.data(), cam_same, f.shutter_open - h->gr_shutter_open));
-                tgt.push_back(k);
-            }
-        std::vector<float> rgb(3 * rays.size()), lc(S, 0.0f);
-        if (!rays.empty()) orc_illumination(s, rays.size(), rays.data(), 1, h->gr_seed, rgb.data(), 1, nullptr);
-        for (size_t k = 0; k < rays.size(); ++k) lc[tgt[k]] = glum(rgb[3 * k], rgb[3 * k + 1], rgb[3 * k + 2]);
-        reconstruct(W, H, slot, h->rec.data(), lc.data(), in->normal_w, in->nearest, t.normal_threshold, t.iterations, nullptr, lam.data());
-    } else {
-        std::vector<uint64_t> slot(S, ~0ull);
-        std::vector<float> lc(S, 0.0f);
-        reconstruct(W, H, slot, nullptr, lc.data(), in->normal_w, in->nearest, t.normal_threshold, t.iterations, nullptr, lam.data());
-    }
-    /* 3 */
+    std::vector<float> inv, mat;
+    scene_gradient_frame(s, f, inv, mat);
+    std::vector<float> lam;
+    scene_lambda(s, h, f, in->normal_w, in->nearest, t, lam);
     temporal_lambda(W, H, &f, h, in, p, squarings, t, lam.data(), rgbw, motion, history_length, lam_px);
-    /* 4 */
-    std::vector<trb_query_ray> q(S);
-    std::vector<trb_illum_ray> il(S);
-    for (uint32_t k = 0; k < S; ++k) {
-        const uint32_t sx = k % gw, sy = k / gw, cwd = std::min(3u, W - 3 * sx), chd = std::min(3u, H - 3 * sy);
-        const uint32_t pick = dm_rng(seed, k, 0xfffffffeu, 0u) % (cwd * chd);
-        const uint32_t px = 3 * sx + pick % cwd, py = 3 * sy + pick / cwd, pixel = py * W + px;
-        const PixelStreams st = pixel_streams(seed, pixel);
-        const uint32_t ip = dm_permute(0, 1, st.kpos);
-        const float fx = van_der_corput(ip, st.scr0) + (float)px, fy = sobol(ip, st.scr1) + (float)py;
-        const float tm = van_der_corput(dm_permute(0, 1, st.ktime), st.scrt);
-        const Ray r = cam.generate_ray(fx, fy, tm);
-        q[k] = trb_query_ray{{r.o.x, r.o.y, r.o.z}, {r.d.x, r.d.y, r.d.z}, r.min_t, r.max_t, r.time, {0, 0, 0}};
-        il[k] = trb_illum_ray{{r.o.x, r.o.y, r.o.z}, {r.d.x, r.d.y, r.d.z}, r.min_t, r.max_t, r.time, pixel, 0, 0};
-    }
-    std::vector<trb_intersection> hits(S);
-    std::vector<float> rgb(3 * (size_t)S);
-    orc_intersect_records(s, S, q.data(), hits.data(), nullptr);
-    orc_illumination(s, S, il.data(), 1, seed, rgb.data(), 1, nullptr);
-    h->rec.assign(S, orc_gradient_record{});
-    for (uint32_t k = 0; k < S; ++k) {
-        orc_gradient_record& r = h->rec[k];
-        r.inst = hits[k].inst;
-        if (r.inst == TRB_MISS) continue;
-        const V3 po = Transform::mul_point(gm4(&inv[16 * (size_t)r.inst]), V3(hits[k].p[0], hits[k].p[1], hits[k].p[2]));
-        r.p_o[0] = po.x; r.p_o[1] = po.y; r.p_o[2] = po.z;
-        for (int c = 0; c < 3; ++c) { r.o[c] = il[k].o[c]; r.d[c] = il[k].d[c]; }
-        r.time = il[k].time; r.key = il[k].key;
-        r.lum = glum(rgb[3 * k], rgb[3 * k + 1], rgb[3 * k + 2]);
-    }
-    h->gr_valid = true; h->gr_seed = seed; h->gr_shutter_open = f.shutter_open;
-    std::memcpy(h->gr_cam_mat, f.cam_mat, 64);
+    scene_record(s, h, f, seed);
     return TRB_OK;
 }
 

@@ -142,3 +142,14 @@ _, motion, hl, var = g.denoise_moments(hist, film, aovs, motion=True, history_le
 hist.reset()
 print("denoise moments ok", float(den[..., :3].sum()), int(hl.max()), float(np.nanmax(var)))
 g.close()
+# the moment gradients (k_gr_*, k_dn_temporal_moments_grad): five 1-spp frames of the keyframed scene, the records re-shaded from the
+# second frame on, the last with every output and no a-trous pass, then a reset
+g = api.Scene(SB.scene_animated(40, 24, 1).finish())
+hist = api.DenoiseHistory(g)
+for k in range(5):
+    den, film, aovs, _ = g.render_denoised_moments(hist, 1, seed=3, current_frame=k, gradients=True)
+_, motion, hl, var, lam = g.denoise_moments_gradient(hist, film, aovs, 9, motion=True, history_length=True, variance=True, lam=True,
+                                                     gradient_iterations=0)
+hist.reset()
+print("denoise moment gradient ok", float(den[..., :3].sum()), int(hl.max()), float(lam.max()))
+g.close()

@@ -255,6 +255,12 @@ class DenoiseMomentsOutput(C.Structure):
     _fields_ = [("rgbw", C.c_void_p), ("motion", C.c_void_p), ("history_length", C.c_void_p), ("variance", C.c_void_p)]
 
 
+class DenoiseMomentsGradientOutput(C.Structure):
+    """trb_denoise_moments_gradient_output: rgbw (required), motion, history_length, variance and lambda (may be NULL)"""
+    _fields_ = [("rgbw", C.c_void_p), ("motion", C.c_void_p), ("history_length", C.c_void_p), ("variance", C.c_void_p),
+                ("lambda_", C.c_void_p)]
+
+
 # include/trb.h "Moment denoising": the history length from which a pixel's own moments give its variance, and the spatial
 # estimate's window radius (7x7)
 DENOISE_MOMENTS_MIN_HISTORY = 4
@@ -315,7 +321,7 @@ TRB_SYMBOLS = [
     "trb_denoise", "trb_denoise_device",
     "trb_denoise_history_create", "trb_denoise_history_destroy", "trb_denoise_history_reset", "trb_denoise_temporal",
     "trb_denoise_temporal_device", "trb_denoise_temporal_gradient", "trb_denoise_temporal_gradient_device",
-    "trb_denoise_moments", "trb_denoise_moments_device",
+    "trb_denoise_moments", "trb_denoise_moments_device", "trb_denoise_moments_gradient", "trb_denoise_moments_gradient_device",
 ]
 
 _trb = None
@@ -402,6 +408,10 @@ def load_trb():
     lib.trb_denoise_moments.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseTemporalParams), C.POINTER(DenoiseMomentsOutput)]
     lib.trb_denoise_moments_device.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseTemporalParams),
                                                C.POINTER(DenoiseMomentsOutput), vp]
+    lib.trb_denoise_moments_gradient.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseGradientParams), u32,
+                                                 C.POINTER(DenoiseMomentsGradientOutput)]
+    lib.trb_denoise_moments_gradient_device.argtypes = [vp, vp, C.POINTER(DenoiseFrame), C.POINTER(DenoiseGradientParams), u32,
+                                                        C.POINTER(DenoiseMomentsGradientOutput), vp]
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]

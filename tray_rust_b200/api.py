@@ -431,20 +431,7 @@ class Scene(_Base):
         `history`. The variance comes from the luminance moments accumulated in the history, or a 7x7 spatial estimate where it is
         short. params: denoise_temporal's. Returns the denoised RGBW film (into `out` when given), or a tuple of it with the motion,
         the history length and the (height, width) float32 variance, in that order, where asked for (True, or an array)."""
-        h, w = self.height, self.width
-        film_shape = (h, w, 4)
-        ins = [("colour", colour, film_shape, np.float32), ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32),
-               ("normal_w", aovs.get("normal_w"), film_shape, np.float32), ("nearest", aovs.get("nearest"), (h, w), np.uint64)]
-        outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
-        for name, a, shape, dtype in (("motion", motion, (h, w, 2), np.float32), ("history_length", history_length, (h, w), np.uint32),
-                                      ("variance", variance, (h, w), np.float32)):
-            if a is True:
-                a = np.zeros(shape, dtype)
-            if a is not False and a is not None:
-                outs.append((name, a, shape, dtype))
-        for name, a, shape, dtype in ins + outs:
-            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
-                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        ins, outs = self._moments_arrays(colour, aovs, out, motion, history_length, variance)
         got = {name: a for name, a, _, _ in outs}
         d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins)), _temporal_params(params)
         o = F.DenoiseMomentsOutput(*(got[k].ctypes.data if k in got else None for k in ("out", "motion", "history_length", "variance")))
@@ -452,6 +439,51 @@ class Scene(_Base):
         if len(outs) == 1:
             return outs[0][1]
         return tuple(a for _, a, _, _ in outs)
+
+    def _moments_arrays(self, colour, aovs, out, motion, history_length, variance, lam=False):
+        """The four input arrays and the output arrays of a moment denoise, checked (motion, history_length, variance and lam:
+        True, False/None or an array). Returns (ins, outs) as (name, array, shape, dtype) lists."""
+        h, w = self.height, self.width
+        film_shape = (h, w, 4)
+        ins = [("colour", colour, film_shape, np.float32), ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32),
+               ("normal_w", aovs.get("normal_w"), film_shape, np.float32), ("nearest", aovs.get("nearest"), (h, w), np.uint64)]
+        outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
+        for name, a, shape, dtype in (("motion", motion, (h, w, 2), np.float32), ("history_length", history_length, (h, w), np.uint32),
+                                      ("variance", variance, (h, w), np.float32), ("lambda", lam, (h, w), np.float32)):
+            if a is True:
+                a = np.zeros(shape, dtype)
+            if a is not False and a is not None:
+                outs.append((name, a, shape, dtype))
+        for name, a, shape, dtype in ins + outs:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        return ins, outs
+
+    def denoise_moments_gradient(self, history, colour, aovs, seed, out=None, motion=False, history_length=False, variance=False, lam=False,
+                                 **params):
+        """trb_denoise_moments_gradient (DESIGN.md §4 "Moment gradients"): denoise_moments with temporal gradients, so a history is
+        shortened where the lighting under it changed. `seed` seeds this frame's gradient samples (render_denoised_moments passes
+        the frame's seed). params: denoise_moments's plus gradient_iterations (0-6, default 3). Returns the denoised RGBW film, or
+        a tuple of it with the motion, the history length, the variance and the (height, width) float32 per-pixel lambda, in that
+        order, where asked for (True, or an array)."""
+        ins, outs = self._moments_arrays(colour, aovs, out, motion, history_length, variance, lam)
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins)), _gradient_params(params)
+        o = F.DenoiseMomentsGradientOutput(*(got[k].ctypes.data if k in got else None
+                                             for k in ("out", "motion", "history_length", "variance", "lambda")))
+        self._check(self._lib.trb_denoise_moments_gradient(self._h, history._h, C.byref(d_in), C.byref(prm), seed % (1 << 32), C.byref(o)))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_moments_gradient_device(self, history, d_colour, d_albedo, d_normal, d_nearest, seed, d_out, d_motion=None,
+                                        d_history_length=None, d_variance=None, d_lambda=None, stream=None, **params):
+        """trb_denoise_moments_gradient_device: denoise_moments_device's pointers plus d_lambda (height*width float32, 4-byte
+        aligned, or None); enqueued on `stream`. params as for denoise_moments_gradient."""
+        d_in, prm = F.DenoiseFrame(d_colour, d_albedo, d_normal, d_nearest), _gradient_params(params)
+        o = F.DenoiseMomentsGradientOutput(d_out, d_motion, d_history_length, d_variance, d_lambda)
+        self._check(self._lib.trb_denoise_moments_gradient_device(self._h, history._h, C.byref(d_in), C.byref(prm), seed % (1 << 32),
+                                                                  C.byref(o), stream))
 
     def denoise_moments_device(self, history, d_colour, d_albedo, d_normal, d_nearest, d_out, d_motion=None, d_history_length=None,
                                d_variance=None, stream=None, **params):
@@ -463,16 +495,20 @@ class Scene(_Base):
         o = F.DenoiseMomentsOutput(d_out, d_motion, d_history_length, d_variance)
         self._check(self._lib.trb_denoise_moments_device(self._h, history._h, C.byref(d_in), C.byref(prm), C.byref(o), stream))
 
-    def render_denoised_moments(self, history, spp=0, seed=1, current_frame=0, denoise=None, **kw):
+    def render_denoised_moments(self, history, spp=0, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
         """Frame `current_frame` of an animation rendered once by render_aov at `spp` (0: the scene's; 1 is enough) with seed
         (seed + current_frame) mod 2^32, and denoised with `history` by denoise_moments (the dict `denoise` holds its parameters).
-        Returns (denoised, film, aovs, stats)."""
+        With `gradients`, the frame is denoised by denoise_moments_gradient with that frame seed. Returns (denoised, film, aovs,
+        stats)."""
         for k in ("sample_first", "sample_count"):
             if k in kw:
                 raise ValueError("render_denoised_moments renders the whole sample range; %s is not taken" % k)
         frame_seed = (seed + current_frame) % (1 << 32)
         film, aovs, st = self.render_aov(spp=spp, seed=frame_seed, current_frame=current_frame, **kw)
-        out = self.denoise_moments(history, film, aovs, **(denoise or {}))
+        if gradients:
+            out = self.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
+        else:
+            out = self.denoise_moments(history, film, aovs, **(denoise or {}))
         return out, film, aovs, st
 
     def render_denoised(self, spp=0, denoise=None, **kw):

@@ -3127,16 +3127,17 @@ size_t gr_layout(size_t G, char* base, GrBuffers* b) {
     return off;
 }
 
-// A gradient call's own arguments (trb_denoise_temporal_gradient*)
+// A gradient call's own arguments (trb_denoise_temporal_gradient*, trb_denoise_moments_gradient*)
 struct GradCall {
     uint32_t iterations;
     uint32_t seed;
     float* lambda;   // per-pixel output, may be null
 };
 
-// Steps 1-2 of "Temporal gradients": re-shade the read set's records in this frame, reconstruct lambda on the stratum grid into b.lam
+// Steps 1-2 of "Temporal gradients": re-shade the read set's records in this frame, reconstruct lambda on the stratum grid into b.lam.
+// nearest and normal_w are the frame's AOVs (trb_denoise_input's or trb_denoise_frame's).
 trb_status gradient_lambda(trb_scene* s, trb_denoise_history* h, const GradCall& gc, const trb::DnTemporal& tp, const GrBuffers& b,
-                           const float* mats_rd, const trb_denoise_input& in, bool valid, cudaStream_t st) {
+                           const float* mats_rd, const uint64_t* nearest_in, const float* normal_w, bool valid, cudaStream_t st) {
     const uint32_t W = s->film.width, H = s->film.height, gw = (W + 2) / 3, gh = (H + 2) / 3, S = gw * gh;
     const unsigned grid = (unsigned)std::min<size_t>((S + 255) / 256, (size_t)s->sm_count * 8);
     trb::GrFrame f{};
@@ -3150,13 +3151,13 @@ trb_status gradient_lambda(trb_scene* s, trb_denoise_history* h, const GradCall&
     f.dt = s->shutter_open - h->gr_shutter_open;
     f.depth_tolerance = tp.depth_tolerance; f.normal_threshold = tp.normal_threshold;
     const float4* rec = b.rec[h->cur];
-    const unsigned long long* nearest = reinterpret_cast<const unsigned long long*>(in.nearest);
+    const unsigned long long* nearest = reinterpret_cast<const unsigned long long*>(nearest_in);
     CU(cudaMemsetAsync(b.slot, 0xff, (size_t)S * 8, st));
     if (valid) {
         trb::k_gr_project<<<grid, 256, 0, st>>>(f, rec, s->d_instances, nearest, b.slot);
         g_launches++;
     }
-    trb::k_gr_resolve<<<grid, 256, 0, st>>>(f, rec, s->d_instances, mats_rd, b.slot, reinterpret_cast<const float4*>(in.normal_w), nearest, b.reshade,
+    trb::k_gr_resolve<<<grid, 256, 0, st>>>(f, rec, s->d_instances, mats_rd, b.slot, reinterpret_cast<const float4*>(normal_w), nearest, b.reshade,
                                             b.guide);
     g_launches++;
     CU(cudaGetLastError());
@@ -3176,6 +3177,12 @@ trb_status gradient_lambda(trb_scene* s, trb_denoise_history* h, const GradCall&
     }
     CU(cudaGetLastError());
     return TRB_OK;
+}
+
+// After step 4: the write set's records are valid, written at the call's seed and this frame's shutter_open and camera
+void gradient_commit(const trb_scene* s, trb_denoise_history* h, const GradCall& gc) {
+    h->gr_valid = true; h->gr_seed = gc.seed; h->gr_shutter_open = s->shutter_open;
+    std::memcpy(h->gr_cam_mat, s->ds.cam.cam_mat, 64);
 }
 
 // Step 4: this frame's samples into the write set's records
@@ -3302,7 +3309,7 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
         GrBuffers b;
         gr_layout(h->gr_capacity, static_cast<char*>(h->d_gr), &b);
         const bool valid = tp.has_prev && h->gr_valid;
-        r = gradient_lambda(s, h, *gc, tp, b, mats_rd, in, valid, st);
+        r = gradient_lambda(s, h, *gc, tp, b, mats_rd, in.nearest, in.normal_w, valid, st);
         if (r != TRB_OK) return r;
         trb::k_dn_temporal_grad<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour_a), reinterpret_cast<const float4*>(in.colour_b),
                                                         reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
@@ -3315,8 +3322,7 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
         if (r != TRB_OK) return r;
         r = gradient_record(s, *gc, b, wr, st);
         if (r != TRB_OK) return r;
-        h->gr_valid = true; h->gr_seed = gc->seed; h->gr_shutter_open = s->shutter_open;
-        std::memcpy(h->gr_cam_mat, s->ds.cam.cam_mat, 64);
+        gradient_commit(s, h, *gc);
     }
     history_commit(s, h, hs, false);
     return TRB_OK;
@@ -3455,9 +3461,10 @@ trb_status moments_check(const trb_scene* s, const trb_denoise_history* h, const
     return history_call_check(s, h, ins, 4, outs, 4, 0);
 }
 
-// k_dn_temporal_moments, k_dn_moments_variance and the a-trous launches on `st`, then the history's switch to the set just written
+// k_dn_temporal_moments (or, with gc, the gradient steps around k_dn_temporal_moments_grad), k_dn_moments_variance and the a-trous
+// launches on `st`, then the history's switch to the set just written
 trb_status moments_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_frame& in,
-                           const trb_denoise_moments_output& out, cudaStream_t st) {
+                           const trb_denoise_moments_output& out, cudaStream_t st, const GradCall* gc = nullptr) {
     const size_t npx = (size_t)prm.width * prm.height;
     if (npx == 0) return TRB_OK;
     trb::DnScratch sc;
@@ -3465,21 +3472,39 @@ trb_status moments_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& 
     trb_status r = denoise_scratch(s, npx, sc, &mom);
     if (r != TRB_OK) return r;
     HistorySets hs;
-    r = history_begin(s, h, prm, tp, true, nullptr, hs, st);
+    r = history_begin(s, h, prm, tp, true, gc, hs, st);
     if (r != TRB_OK) return r;
     float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
     const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
-    trb::k_dn_temporal_moments<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour), reinterpret_cast<const float4*>(in.albedo_w),
-                                                       reinterpret_cast<const float4*>(in.normal_w), reinterpret_cast<const unsigned long long*>(in.nearest),
-                                                       sc, mom, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd), h->set(hs.wr),
-                                                       reinterpret_cast<float2*>(out.motion), out.history_length);
+    GrBuffers b{};
+    if (!gc) {
+        trb::k_dn_temporal_moments<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour), reinterpret_cast<const float4*>(in.albedo_w),
+                                                           reinterpret_cast<const float4*>(in.normal_w), reinterpret_cast<const unsigned long long*>(in.nearest),
+                                                           sc, mom, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd), h->set(hs.wr),
+                                                           reinterpret_cast<float2*>(out.motion), out.history_length);
+    } else {
+        gr_layout(h->gr_capacity, static_cast<char*>(h->d_gr), &b);
+        r = gradient_lambda(s, h, *gc, tp, b, hs.mats_rd, in.nearest, in.normal_w, tp.has_prev && h->gr_valid, st);
+        if (r != TRB_OK) return r;
+        trb::k_dn_temporal_moments_grad<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour),
+                                                                reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                                                reinterpret_cast<const unsigned long long*>(in.nearest), sc, mom, rgbw, s->d_instances,
+                                                                hs.mats_rd, h->set(hs.rd), h->set(hs.wr), reinterpret_cast<float2*>(out.motion),
+                                                                out.history_length, b.lam, (uint32_t)((prm.width + 2) / 3), gc->lambda);
+    }
     g_launches++;
     trb::k_dn_moments_variance<<<grid, block, 0, st>>>(prm, sc.guide, sc.grad, mom, sc.ev[0], out.variance);
     g_launches++;
     CU(cudaGetLastError());
     r = denoise_atrous(prm, sc, rgbw, st);
     if (r != TRB_OK) return r;
-    h->gr_valid = false;
+    if (gc) {
+        r = gradient_record(s, *gc, b, hs.wr, st);
+        if (r != TRB_OK) return r;
+        gradient_commit(s, h, *gc);
+    } else {
+        h->gr_valid = false;
+    }
     history_commit(s, h, hs, true);
     return TRB_OK;
 }
@@ -3520,6 +3545,77 @@ trb_status trb_denoise_moments(trb_scene* s, trb_denoise_history* h, const trb_d
     r = moments_enqueue(s, h, prm, tp, d_in, d_out, 0);
     if (r != TRB_OK) return r;
     return unstage_out(outs, 4, d_outs);
+}
+
+// ---- moment gradients (include/trb.h "Moment gradients", DESIGN.md §4) -------------------------------------------------------------
+namespace {
+// trb_denoise_gradient_params (NULL meaning the defaults) first, then moments_check and the lambda output's overlaps
+trb_status moments_gradient_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_gradient_params* params,
+                                  const trb_denoise_moments_gradient_output* out, trb::DnParams& prm, trb::DnTemporal& tp, GradCall& gc) {
+    const uint32_t iterations = params ? params->iterations : 3u;
+    trb_status r = temporal_params(params ? &params->temporal : nullptr, prm, tp);
+    if (r != TRB_OK) return r;
+    if (iterations > 6) return fail(TRB_INVALID_ARG, "temporal gradient iterations must be 0 to 6");
+    if (!out) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_denoise_moments_output o{out->rgbw, out->motion, out->history_length, out->variance};
+    r = moments_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp);
+    if (r != TRB_OK) return r;
+    if (out->lambda) {
+        const size_t npx = (size_t)s->film.width * s->film.height;
+        const Span others[8] = {{in->colour, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                                {in->nearest, npx * sizeof(uint64_t)}, {out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)},
+                                {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)}};
+        for (const auto& [p, bytes] : others)
+            if (spans_overlap(out->lambda, npx * sizeof(float), p, bytes)) return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
+    }
+    gc.iterations = iterations;
+    gc.lambda = out->lambda;
+    return TRB_OK;
+}
+} // namespace
+
+trb_status trb_denoise_moments_gradient_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* d_in, const trb_denoise_gradient_params* params,
+                                               uint32_t seed, const trb_denoise_moments_gradient_output* d_out, void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    const trb_status r = moments_gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    if (r != TRB_OK) return r;
+    if (((reinterpret_cast<uintptr_t>(d_in->colour) | reinterpret_cast<uintptr_t>(d_in->albedo_w) | reinterpret_cast<uintptr_t>(d_in->normal_w) |
+          reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
+        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
+        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->variance) |
+          reinterpret_cast<uintptr_t>(d_out->lambda)) & 3u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length, variance and lambda 4-byte");
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const trb_denoise_moments_output o{d_out->rgbw, d_out->motion, d_out->history_length, d_out->variance};
+    return moments_enqueue(s, h, prm, tp, *d_in, o, static_cast<cudaStream_t>(stream), &gc);
+}
+
+trb_status trb_denoise_moments_gradient(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_gradient_params* params,
+                                        uint32_t seed, const trb_denoise_moments_gradient_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    trb_status r = moments_gradient_check(s, h, in, params, out, prm, tp, gc);
+    if (r != TRB_OK) return r;
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    const Span ins[4] = {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
+    const Span outs[5] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
+                          {out->variance, npx * sizeof(float)}, {out->lambda, npx * sizeof(float)}};
+    DeviceBuffer d_ins[4], d_outs[5];
+    if ((r = stage_in(ins, 4, d_ins)) != TRB_OK || (r = stage_out(outs, 5, d_outs)) != TRB_OK) return r;
+    const trb_denoise_frame d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
+                                 static_cast<const uint64_t*>(d_ins[3].p)};
+    const trb_denoise_moments_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p),
+                                          static_cast<float*>(d_outs[3].p)};
+    gc.lambda = static_cast<float*>(d_outs[4].p);
+    r = moments_enqueue(s, h, prm, tp, d_in, d_out, 0, &gc);
+    if (r != TRB_OK) { cudaDeviceSynchronize(); return r; }
+    return unstage_out(outs, 5, d_outs);
 }
 
 trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {

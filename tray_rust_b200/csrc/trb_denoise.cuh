@@ -3,7 +3,8 @@
 // Three kernels: k_dn_prepare reads the inputs once into a guide record per pixel and the first (e, v) buffer; k_dn_atrous runs one
 // iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film; k_dn_temporal takes k_dn_prepare's place
 // for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer; k_dn_temporal_moments and
-// k_dn_moments_variance take it for trb_denoise_moments*, one film with the variance from luminance moments. Float32 in the header's order, no
+// k_dn_moments_variance take it for trb_denoise_moments* (k_dn_temporal_moments_grad for trb_denoise_moments_gradient*), one film with
+// the variance from luminance moments. Float32 in the header's order, no
 // atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
 #pragma once
 #include "trb_detmath.cuh"
@@ -376,16 +377,26 @@ constexpr size_t DN_MOMENTS_BYTES_PER_PIXEL = DN_BYTES_PER_PIXEL + sizeof(float4
 // denoising" (dn_reproject; a set's records are (ē, z), (mu1, mu2, 0, inst bits), (n, n' bits)) and the blend of the colour and the
 // luminance moments. Writes the guide, gradient and divisor as k_dn_prepare does, ev[0] = (ē, 0) (k_dn_moments_variance fills in v),
 // the moment record, the history, motion and history length.
-__global__ void __launch_bounds__(256) k_dn_temporal_moments(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ col,
-                                                             const float4* __restrict__ alb, const float4* __restrict__ nrm,
-                                                             const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ mom,
-                                                             float4* __restrict__ out, const DInstance* __restrict__ inst, const float* __restrict__ mat_prev,
-                                                             const DnHistory hin, const DnHistory hout, float2* __restrict__ motion,
-                                                             uint32_t* __restrict__ hlen) {
+// The body of k_dn_temporal_moments (GRAD false) and k_dn_temporal_moments_grad (GRAD true: step 3 shortens the history by the
+// pixel's stratum's lambda, include/trb.h "Moment gradients", and lam_out receives it). lam_s: S lambdas on the stratum grid of gw
+// columns. tp is taken by value: by reference, k_dn_temporal_moments compiled to other SASS than its body had as a kernel of its own.
+template <bool GRAD>
+__device__ __forceinline__ void dn_temporal_moments_px(const DnParams prm, const DnTemporal tp, const float4* __restrict__ col,
+                                                       const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                       const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ mom,
+                                                       float4* __restrict__ out, const DInstance* __restrict__ inst,
+                                                       const float* __restrict__ mat_prev, const DnHistory hin, const DnHistory hout,
+                                                       float2* __restrict__ motion, uint32_t* __restrict__ hlen, const float* __restrict__ lam_s,
+                                                       uint32_t gw, float* __restrict__ lam_out) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= prm.width || y >= prm.height) return;
     const int i = y * prm.width + x;
     const float qnan = __int_as_float(0x7fffffff);
+    float lam = 0.0f;
+    if (GRAD) {
+        lam = lam_s[(uint32_t)(y / 3) * gw + (uint32_t)(x / 3)];
+        if (lam_out) lam_out[i] = lam;
+    }
     const float4 A = col[i];
     const float W = A.w;
     if (W <= 0.0f) {
@@ -436,7 +447,14 @@ __global__ void __launch_bounds__(256) k_dn_temporal_moments(const DnParams prm,
     dn_reproject(prm, tp, x, y, z, id, n0, n1, n2, inst, mat_prev, hin, mx, my, S, h0, h1, h2, M1, M2, M3, len_prev);
     // 3: blend colour and moments with the same 1 / n'
     uint32_t np = 1;
-    if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    if (GRAD) {
+        if (S > 0.0f) {
+            const uint32_t len_adj = (uint32_t)floorf((1.0f - lam) * (float)len_prev);
+            np = len_adj + 1 < tp.max_history ? len_adj + 1 : tp.max_history;
+        }
+    } else {
+        if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    }
     float mu1 = l, mu2 = l * l;
     if (np > 1) {
         h0 = h0 / S; h1 = h1 / S; h2 = h2 / S;
@@ -462,6 +480,26 @@ __global__ void __launch_bounds__(256) k_dn_temporal_moments(const DnParams prm,
     }
     if (motion) motion[i] = make_float2(mx == mx ? mx : qnan, my == my ? my : qnan);
     if (hlen) hlen[i] = np;
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal_moments(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ col,
+                                                             const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                             const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ mom,
+                                                             float4* __restrict__ out, const DInstance* __restrict__ inst, const float* __restrict__ mat_prev,
+                                                             const DnHistory hin, const DnHistory hout, float2* __restrict__ motion,
+                                                             uint32_t* __restrict__ hlen) {
+    dn_temporal_moments_px<false>(prm, tp, col, alb, nrm, nearest, sc, mom, out, inst, mat_prev, hin, hout, motion, hlen, nullptr, 0u, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal_moments_grad(const DnParams prm, const __grid_constant__ DnTemporal tp,
+                                                                  const float4* __restrict__ col, const float4* __restrict__ alb,
+                                                                  const float4* __restrict__ nrm, const unsigned long long* __restrict__ nearest,
+                                                                  DnScratch sc, float4* __restrict__ mom, float4* __restrict__ out,
+                                                                  const DInstance* __restrict__ inst, const float* __restrict__ mat_prev,
+                                                                  const DnHistory hin, const DnHistory hout, float2* __restrict__ motion,
+                                                                  uint32_t* __restrict__ hlen, const float* __restrict__ lam_s, uint32_t gw,
+                                                                  float* __restrict__ lam_out) {
+    dn_temporal_moments_px<true>(prm, tp, col, alb, nrm, nearest, sc, mom, out, inst, mat_prev, hin, hout, motion, hlen, lam_s, gw, lam_out);
 }
 
 // Step 4 of "Moment denoising": each filtered pixel's variance, mu2 - mu1^2 from its own moments once n' >= MIN_HISTORY, else the

@@ -1,7 +1,7 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
-//            [--denoise-temporal [--temporal-gradients]]
+//            [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
 //
@@ -20,7 +20,8 @@
 // history and seed (S + frame) mod 2^32, denoising each with trb_denoise_temporal (refused where --denoise is, and with --denoise);
 // --temporal-gradients, only with --denoise-temporal, denoises with trb_denoise_temporal_gradient at the frame's seed; --denoise-moments
 // renders each frame once with AOVs (1 spp allowed), in order, with one history and seed (S + frame) mod 2^32, denoising it with
-// trb_denoise_moments (single node, path integrator, refused with the other denoise flags); a worker address is host[:port],
+// trb_denoise_moments (single node, path integrator, refused with the other denoise flags); --moment-gradients, only with
+// --denoise-moments, denoises with trb_denoise_moments_gradient at the frame's seed; a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -44,7 +45,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments]\n"
+    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -68,6 +69,8 @@ const char* USAGE =
     "  --denoise-moments       Render each frame once with albedo, normal and depth (1 sample per pixel is enough) and denoise it\n"
     "                          with a history of luminance moments over the frame range; frame k is rendered with seed S + k.\n"
     "                          Single node only, path integrator.\n"
+    "  --moment-gradients      With --denoise-moments only: re-shade a sample of each 3x3 pixel block of the previous frame in\n"
+    "                          this one and shorten the moment history where the lighting changed. Single node only.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -158,7 +161,7 @@ struct Args {
     std::vector<std::string> workers;
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
-         denoise_temporal = false, temporal_gradients = false, denoise_moments = false;
+         denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
 };
 
@@ -210,12 +213,13 @@ struct DenoisedFrame {
 };
 
 // --denoise-moments: the frame's whole sample range into one film with its AOVs, then trb_denoise_moments with the history of the
-// frames before (DESIGN.md §4 "Moment denoising")
+// frames before (DESIGN.md §4 "Moment denoising"); --moment-gradients: trb_denoise_moments_gradient at the frame's seed instead
+// (DESIGN.md §4 "Moment gradients")
 struct MomentsFrame {
     std::vector<float> colour, albedo, normal, out;
     std::vector<uint64_t> nearest;
     explicit MomentsFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history) {
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history, bool gradients) {
         std::fill(colour.begin(), colour.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
@@ -224,8 +228,13 @@ struct MomentsFrame {
         const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
         tray::check(trb_render_aov(s, &cfg, colour.data(), &aov, nullptr)); // includes Scene::update_frame
         const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
-        const trb_denoise_moments_output o{out.data(), nullptr, nullptr, nullptr};
-        tray::check(trb_denoise_moments(s, history, &in, nullptr, &o));
+        if (gradients) {
+            const trb_denoise_moments_gradient_output o{out.data(), nullptr, nullptr, nullptr, nullptr};
+            tray::check(trb_denoise_moments_gradient(s, history, &in, nullptr, seed, &o));
+        } else {
+            const trb_denoise_moments_output o{out.data(), nullptr, nullptr, nullptr};
+            tray::check(trb_denoise_moments(s, history, &in, nullptr, &o));
+        }
     }
 };
 
@@ -262,7 +271,7 @@ int single_node(const Args& a, const OutPath& out) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (mf) {
-                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history);
+                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(scene.handle(), mf->out.data(), img.data()));
             } else if (dn) {
@@ -473,13 +482,15 @@ int master_node(const Args& a, const OutPath& out) {
 } // namespace
 
 int main(int argc, char** argv) {
-    bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false;
+    bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false,
+         moment_gradients = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
         denoise = denoise || std::strcmp(argv[i], "--denoise") == 0;
         denoise_temporal = denoise_temporal || std::strcmp(argv[i], "--denoise-temporal") == 0;
         denoise_moments = denoise_moments || std::strcmp(argv[i], "--denoise-moments") == 0;
+        moment_gradients = moment_gradients || std::strcmp(argv[i], "--moment-gradients") == 0;
     }
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_temporal)
@@ -488,6 +499,8 @@ int main(int argc, char** argv) {
         return die("--temporal-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_moments)
         return die("--denoise-moments is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && moment_gradients)
+        return die("--moment-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -512,6 +525,7 @@ int main(int argc, char** argv) {
         else if (s == "--denoise-temporal") a.denoise_temporal = true;
         else if (s == "--temporal-gradients") a.temporal_gradients = true;
         else if (s == "--denoise-moments") a.denoise_moments = true;
+        else if (s == "--moment-gradients") a.moment_gradients = true;
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -525,6 +539,9 @@ int main(int argc, char** argv) {
         return die("--denoise-moments is not available with --master: the wire format carries no albedo, normal or depth");
     if (a.denoise_moments && (a.denoise || a.denoise_temporal || a.temporal_gradients))
         return die("--denoise-moments excludes --denoise, --denoise-temporal and --temporal-gradients: choose one denoiser");
+    if (a.master && a.moment_gradients)
+        return die("--moment-gradients is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.moment_gradients && !a.denoise_moments) return die("--moment-gradients needs --denoise-moments");
     if (a.master && a.denoise) return die("--denoise is not available with --master: the wire format carries no albedo, normal or depth");
     if (a.denoise && a.has_spp && a.spp < 2) return die("--denoise needs at least 2 samples per pixel (two half renders)");
     if (a.denoise && a.denoise_temporal) return die("--denoise and --denoise-temporal exclude each other: choose one");
