@@ -1197,6 +1197,30 @@ trb_status trb_render_samples_adaptive(trb_scene* scene, const trb_render_cfg* c
 trb_status trb_render_adaptive_device(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* d_film_rgbw,
                                       uint32_t* d_pixel_spp, trb_stats* d_stats, void* cuda_stream);
 
+/* -- AOVs of Adaptive renders (DESIGN.md §4 "Adaptive AOVs") -------------------------------------------------------------
+ * trb_render_adaptive that also renders the AOVs (trb_aov_sample, trb_aov_film) of every sample it takes into the HOST buffers of
+ * `aov`: albedo_w and normal_w are added into with the colour film's weights, so their W equals the colour film's W up to float
+ * addition order; nearest is read and written (initialise it to all ones); any of the three may be NULL. The colour film,
+ * pixel_spp and every trb_stats counter equal trb_render_adaptive's with the same arguments. Statuses: trb_render_adaptive's
+ * (TRB_INVALID_ARG for a non-zero spp, sample_first or sample_count, or max < min after rounding; TRB_UNSUPPORTED for the
+ * Whitted / NormalsDebug integrators and TRB_RENDER_MEGAKERNEL), which include trb_render_aov's. The first AOV render allocates
+ * 32 B of AOV record per path in flight, as trb_render_aov does. Blocking. */
+trb_status trb_render_adaptive_aov(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                                   const trb_aov_film* aov, uint32_t* pixel_spp, trb_stats* stats);
+
+/* trb_render_adaptive_aov with the contract of trb_render_adaptive_device: the film, d_pixel_spp, d_stats and the outputs of
+ * `d_aov` (a host struct of DEVICE pointers) are device buffers on the scene's GPU; every round is enqueued on cuda_stream without
+ * host synchronisation, and update_frame is never called. TRB_INVALID_ARG for a film or an AOV film that is not 16-byte aligned,
+ * or a nearest buffer that is not 8-byte aligned, as trb_render_aov_device. */
+trb_status trb_render_adaptive_aov_device(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* d_film_rgbw,
+                                          const trb_aov_film* d_aov, uint32_t* d_pixel_spp, trb_stats* d_stats, void* cuda_stream);
+
+/* trb_render_samples_adaptive that also writes the AOV record of every (block, pixel, slot) into the HOST buffer aov[n], in the
+ * same layout: n = blocks*64*max_per_pixel, slots a pixel did not take are zero. samples[], pixel_spp and the stats equal
+ * trb_render_samples_adaptive's. Does not update the frame. */
+trb_status trb_render_samples_adaptive_aov(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, size_t n,
+                                           trb_sample* samples, trb_aov_sample* aov, uint32_t* pixel_spp, trb_stats* stats);
+
 /* trb_render_sharded with the Adaptive sampler: this rank's shard (interleaved chunks, or the reference's contiguous
  * ranges with cfg->shard_count == 0xffffffff) runs the Adaptive rounds into the device film, then ONE reduce to `root`,
  * whose host film_rgbw the summed film is ADDED to. pixel_spp (width*height, or NULL) receives the counts of this rank's

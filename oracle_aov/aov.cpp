@@ -12,20 +12,7 @@
  *                           samples (may be NULL) and stats receive orc_render_samples' records and counters of the same selection.
  */
 #include "../oracle_refit/refit.cpp"
-
-static Col aov_albedo(const BSDF& b) {
-    Col acc(0.0f);
-    for (int i = 0; i < b.n_lobes; ++i) {
-        const Lobe& l = b.lobes[i];
-        switch (l.kind) {
-            case L_LAMBERT: case L_OREN_NAYAR: acc = acc + l.c; break;
-            case L_SPEC_REFL: case L_TORRANCE_SPARROW: acc = acc + l.c * l.fresnel.eval(1.0f); break;
-            case L_SPEC_TRANS: case L_MICROFACET_TRANS: acc = acc + l.c * (Col(1.0f) - l.fresnel.eval(1.0f)); break;
-            case L_MERL: acc = b.eval(b.n, b.n, BX_ALL) * PI; break;
-        }
-    }
-    return acc.clamp();
-}
+#include "aov_albedo.h"
 
 extern "C" {
 

@@ -322,6 +322,7 @@ TRB_SYMBOLS = [
     "trb_denoise_history_create", "trb_denoise_history_destroy", "trb_denoise_history_reset", "trb_denoise_temporal",
     "trb_denoise_temporal_device", "trb_denoise_temporal_gradient", "trb_denoise_temporal_gradient_device",
     "trb_denoise_moments", "trb_denoise_moments_device", "trb_denoise_moments_gradient", "trb_denoise_moments_gradient_device",
+    "trb_render_adaptive_aov", "trb_render_adaptive_aov_device", "trb_render_samples_adaptive_aov",
 ]
 
 _trb = None
@@ -415,6 +416,9 @@ def load_trb():
     lib.trb_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
     lib.trb_render_samples_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, vp, vp]
+    lib.trb_render_adaptive_aov.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, C.POINTER(Stats)]
+    lib.trb_render_adaptive_aov_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, vp]
+    lib.trb_render_samples_adaptive_aov.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, vp, C.POINTER(Stats)]
     lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
     lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]

@@ -252,6 +252,13 @@ class Scene(_Base):
         (allocate, all ones), False / None or a uint64 (height, width) array. Returns (film, aovs, Stats) where aovs maps "albedo_w",
         "normal_w" and "nearest" to the arrays rendered."""
         cfg = _cfg(**kw)
+        film, aovs, out = self._aov_outputs(film, albedo, normal, nearest)
+        st = F.Stats()
+        self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
+        return film, aovs, st
+
+    def _aov_outputs(self, film, albedo, normal, nearest):
+        """The host film and AOV arrays of render_aov / render_adaptive_aov, checked or allocated: (film, aovs, AovFilm)."""
         if film is None:
             film = np.zeros((self.height, self.width, 4), np.float32)
         aovs = {}
@@ -267,10 +274,7 @@ class Scene(_Base):
             aovs[name] = a
         if not isinstance(film, np.ndarray) or film.dtype != np.float32 or film.shape != (self.height, self.width, 4) or not film.flags.c_contiguous:
             raise ValueError("film must be a C-contiguous float32 array of shape %s" % ((self.height, self.width, 4),))
-        out = F.AovFilm(*(aovs[k].ctypes.data if k in aovs else None for k in ("albedo_w", "normal_w", "nearest")))
-        st = F.Stats()
-        self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
-        return film, aovs, st
+        return film, aovs, F.AovFilm(*(aovs[k].ctypes.data if k in aovs else None for k in ("albedo_w", "normal_w", "nearest")))
 
     def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, **kw):
         """trb_render_aov_device: device films of height*width*4 float32 (16-byte aligned) and a device nearest buffer of height*width
@@ -511,6 +515,19 @@ class Scene(_Base):
             out = self.denoise_moments(history, film, aovs, **(denoise or {}))
         return out, film, aovs, st
 
+    def render_denoised_adaptive(self, history, min_spp, max_spp, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
+        """render_denoised_moments with the Adaptive sampler (DESIGN.md §4 "Adaptive AOVs"): frame `current_frame` rendered once by
+        render_adaptive_aov(min_spp, max_spp) with seed (seed + current_frame) mod 2^32, and denoised with `history` by
+        denoise_moments, or with `gradients` by denoise_moments_gradient with that frame seed. For a single image pass
+        denoise={"max_history": 1}. Returns (denoised, film, aovs, pixel_spp, stats)."""
+        frame_seed = (seed + current_frame) % (1 << 32)
+        film, aovs, pixel_spp, st = self.render_adaptive_aov(min_spp, max_spp, seed=frame_seed, current_frame=current_frame, **kw)
+        if gradients:
+            out = self.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
+        else:
+            out = self.denoise_moments(history, film, aovs, **(denoise or {}))
+        return out, film, aovs, pixel_spp, st
+
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:
         samples [0, spp/2) and [spp/2, spp) are rendered into two films by render_aov, with the albedo, normal and nearest AOVs
@@ -732,6 +749,38 @@ class Scene(_Base):
         self._check(self._lib.trb_render_samples_adaptive(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), n, F.ptr(out), F.ptr(spp),
                                                           C.byref(st)))
         return out, spp, st
+
+    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, **kw):
+        """trb_render_adaptive_aov: render_adaptive with the AOVs of the samples it takes (DESIGN.md §4 "Adaptive AOVs"), all
+        accumulated into; albedo / normal / nearest as for render_aov. Returns (film, aovs, pixel_spp, Stats)."""
+        cfg = _cfg(**kw)
+        film, aovs, out = self._aov_outputs(film, albedo, normal, nearest)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_adaptive_aov(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), C.byref(out),
+                                                      F.ptr(spp), C.byref(st)))
+        return film, aovs, spp, st
+
+    def render_adaptive_aov_device(self, min_spp, max_spp, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_pixel_spp=None, d_stats=None,
+                                   stream=None, **kw):
+        """trb_render_adaptive_aov_device: render_adaptive_device's pointers plus the AOV buffers of render_aov_device (any None).
+        Enqueued on `stream` without host synchronisation. Never updates the frame."""
+        cfg = _cfg(**kw)
+        out = F.AovFilm(d_albedo, d_normal, d_nearest)
+        self._check(self._lib.trb_render_adaptive_aov_device(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), d_film, C.byref(out),
+                                                             d_pixel_spp, d_stats, stream))
+
+    def render_samples_adaptive_aov(self, min_spp, max_spp, **kw):
+        """trb_render_samples_adaptive_aov: (samples as render_samples_adaptive, AOV records as AOV_SAMPLE_DTYPE in the same layout,
+        unused slots zero; pixel_spp; Stats)."""
+        cfg = _cfg(**kw)
+        n = self._n_selected_blocks(cfg) * 64 * adaptive_schedule(min_spp, max_spp)[3]
+        out, aov = np.zeros(n, F.SAMPLE_DTYPE), np.zeros(n, F.AOV_SAMPLE_DTYPE)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_samples_adaptive_aov(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), n, F.ptr(out), F.ptr(aov),
+                                                              F.ptr(spp), C.byref(st)))
+        return out, aov, spp, st
 
     def camera_rays(self, **kw):
         cfg = _cfg(**kw)

@@ -763,7 +763,10 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
             float4* lo = mode == 1 ? reinterpret_cast<float4*>(aov->samples) : s->d_aov;
             float4* hi = mode == 1 ? lo + 1 : s->d_aov + s->aov_capacity;
             const uint32_t step = mode == 1 ? 2u : 1u;
-            if (anim) trb::k_wf_aov<true><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
+            if (rp.ad_state) { // Adaptive pass (always mode 0): the paths the pass really holds
+                if (anim) trb::k_wf_aov_ad<true><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi);
+                else trb::k_wf_aov_ad<false><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi);
+            } else if (anim) trb::k_wf_aov<true><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
             else trb::k_wf_aov<false><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
             g_launches++;
         }
@@ -828,13 +831,17 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
             for (const auto& f : films) {
                 if (!f.first) continue;
                 ra.film = f.first; wa.rad = f.second;
-                if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                if (rp.ad_state) { // Adaptive: the live blocks and the pixels that sampled this round, as for the colour film
+                    if (tu.film_v2) trb::k_wf_film_v2<true><<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                    else trb::k_wf_film<true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                } else if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
                 else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
                 g_launches++;
             }
             if (aov->nearest) {
                 const unsigned ngrid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
-                trb::k_wf_nearest<<<ngrid, 256, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, (uint32_t)n_paths, aov->nearest);
+                if (rp.ad_state) trb::k_wf_nearest_ad<<<ngrid, 256, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, aov->nearest);
+                else trb::k_wf_nearest<<<ngrid, 256, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, (uint32_t)n_paths, aov->nearest);
                 g_launches++;
             }
         }
@@ -913,9 +920,10 @@ trb_status ensure_adaptive(trb_scene* s) {
 // synchronisation: the host cannot know how many blocks a round keeps, so it enqueues every round of the schedule with the
 // passes the whole selection would need, and each pass clamps itself to the round's live block count, which k_ad_init /
 // k_ad_compact keep on the device (DESIGN.md §5 "Adaptive rounds"). Afterwards d_spp[y * width + x] holds the sample count
-// of each selected pixel (d_spp: width*height u32, or nullptr).
+// of each selected pixel (d_spp: width*height u32, or nullptr). aov (nullptr: none): the AOV films of rp's film, or with
+// rp.film == nullptr the AOV records in samples_out's slot layout (DESIGN.md §4 "Adaptive AOVs").
 trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb::RenderParams rp, const uint2* d_blocks, uint32_t nb, uint32_t flags,
-                                  cudaStream_t st, uint32_t* d_spp) {
+                                  cudaStream_t st, uint32_t* d_spp, const AovRequest* aov = nullptr) {
     trb_status r = ensure_adaptive(s);
     if (r != TRB_OK) return r;
     const uint64_t per_block = (uint64_t)64 * std::max(sch.min, sch.step); // paths of one block in the largest round
@@ -926,6 +934,7 @@ trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb
         while ((r = ensure_wavefront(s, (size_t)want)) == TRB_OOM && want / 2 >= per_block && want > (1u << 16)) want = ((want / 2 + 63) / 64) * 64;
         if (r != TRB_OK) return r;
     }
+    if (aov && (r = ensure_aov(s)) != TRB_OK) return r;
     const uint64_t cap = want;
     rp.ad_state = s->d_ad_state;
     rp.ad_min = sch.min; rp.ad_max = sch.max; rp.ad_step = sch.step; rp.ad_max_per_pixel = sch.max_per_pixel;
@@ -942,9 +951,13 @@ trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb
         const uint32_t bp = (uint32_t)std::max<uint64_t>(1, cap / ((uint64_t)64 * count));
         for (uint32_t b0 = 0; b0 < nb; b0 += bp) { // worst case: the whole selection is still live; passes past the live count exit at once
             rp.blocks = s->d_ad_list[cur] + b0; rp.n_blocks = std::min(bp, nb - b0); rp.ad_block_index = s->d_ad_index[cur] + b0; rp.ad_b0 = b0;
-            r = launch_wavefront(s, rp, flags, 0, st);
+            r = launch_wavefront(s, rp, flags, 0, st, aov);
             if (r != TRB_OK) return r;
             const unsigned dgrid = (unsigned)std::min<size_t>(((size_t)rp.n_blocks * 64 + 127) / 128, (size_t)s->sm_count * 16);
+            if (aov && aov->samples) {
+                trb::k_ad_aov_slots<<<dgrid, 128, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, aov->samples);
+                g_launches++;
+            }
             trb::k_ad_decide<<<dgrid, 128, 0, st>>>(s->ds, rp, s->wf, s->d_ad_flags + b0);
             g_launches++;
         }
@@ -2691,6 +2704,36 @@ void add_film(float* film, const float* src, size_t n) {
     for (auto& t : th) t.join();
 }
 
+// The device side of a host AOV render (trb_render_aov, trb_render_adaptive_aov): films from zero, added into the caller's
+// afterwards; nearest from the caller's
+struct HostAov {
+    DeviceBuffer albedo, normal, nearest;
+    AovRequest req{nullptr, nullptr, nullptr, nullptr};
+    const trb_aov_film* aov = nullptr; // nullptr: no AOV output asked for
+    trb_status stage(const trb_aov_film* a, size_t npx) {
+        if (!a || !(a->albedo_w || a->normal_w || a->nearest)) return TRB_OK;
+        aov = a;
+        if (a->albedo_w) { CU(cudaMalloc(&albedo.p, npx * sizeof(float4))); CU(cudaMemsetAsync(albedo.p, 0, npx * sizeof(float4), 0)); }
+        if (a->normal_w) { CU(cudaMalloc(&normal.p, npx * sizeof(float4))); CU(cudaMemsetAsync(normal.p, 0, npx * sizeof(float4), 0)); }
+        if (a->nearest) { CU(cudaMalloc(&nearest.p, npx * sizeof(uint64_t))); CU(cudaMemcpy(nearest.p, a->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice)); }
+        req = {nullptr, static_cast<float4*>(albedo.p), static_cast<float4*>(normal.p), static_cast<unsigned long long*>(nearest.p)};
+        return TRB_OK;
+    }
+    const AovRequest* request() const { return aov ? &req : nullptr; }
+    trb_status unstage(size_t npx) {
+        if (!aov) return TRB_OK;
+        std::vector<float> h;
+        for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, albedo.p}, std::pair<float*, void*>{aov->normal_w, normal.p}}) {
+            if (!dst) continue;
+            h.resize(npx * 4);
+            CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
+            add_film(dst, h.data(), npx * 4);
+        }
+        if (aov->nearest) CU(cudaMemcpy(aov->nearest, nearest.p, npx * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        return TRB_OK;
+    }
+};
+
 // trb_render's body; aov: the host AOV outputs of trb_render_aov (nullptr: none)
 trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats) {
     CU(cudaSetDevice(s->device));
@@ -2705,17 +2748,11 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     const size_t npx = (size_t)s->film.width * s->film.height;
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
-    DeviceBuffer d_albedo, d_normal, d_nearest; // the AOV outputs on the device: films from zero (added into the caller's), nearest from the caller's
-    AovRequest req{nullptr, nullptr, nullptr, nullptr};
-    if (aov) {
-        if (aov->albedo_w) { CU(cudaMalloc(&d_albedo.p, npx * sizeof(float4))); CU(cudaMemsetAsync(d_albedo.p, 0, npx * sizeof(float4), 0)); }
-        if (aov->normal_w) { CU(cudaMalloc(&d_normal.p, npx * sizeof(float4))); CU(cudaMemsetAsync(d_normal.p, 0, npx * sizeof(float4), 0)); }
-        if (aov->nearest) { CU(cudaMalloc(&d_nearest.p, npx * sizeof(uint64_t))); CU(cudaMemcpy(d_nearest.p, aov->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice)); }
-        req = {nullptr, static_cast<float4*>(d_albedo.p), static_cast<float4*>(d_normal.p), static_cast<unsigned long long*>(d_nearest.p)};
-    }
-    const bool with_aov = aov && (aov->albedo_w || aov->normal_w || aov->nearest);
+    HostAov ha;
+    trb_status r = ha.stage(aov, npx);
+    if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
-    trb_status r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, with_aov ? &req : nullptr);
+    r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, ha.request());
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev1, 0));
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, 0));
@@ -2723,16 +2760,7 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
     add_film(film, s->h_film_staging, npx * 4);
-    if (with_aov) {
-        std::vector<float> h;
-        for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, d_albedo.p}, std::pair<float*, void*>{aov->normal_w, d_normal.p}}) {
-            if (!dst) continue;
-            h.resize(npx * 4);
-            CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
-            add_film(dst, h.data(), npx * 4);
-        }
-        if (aov->nearest) CU(cudaMemcpy(aov->nearest, d_nearest.p, npx * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    }
+    if ((r = ha.unstage(npx)) != TRB_OK) return r;
     if (stats) {
         trb::DStats h;
         CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
@@ -3646,8 +3674,10 @@ trb_status trb_host_adaptive_decide(const trb_adaptive* ad, const float* lum, si
     return TRB_OK;
 }
 
-trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
-    if (!s || !cfg || !ad || !film) return fail(TRB_INVALID_ARG, "null argument");
+namespace {
+// trb_render_adaptive's body; aov: the host AOV outputs of trb_render_adaptive_aov (nullptr: none)
+trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, uint32_t* pixel_spp,
+                                trb_stats* stats) {
     trbh::AdSchedule sch;
     trb_status r = adaptive_check(s, cfg, ad, sch);
     if (r != TRB_OK) return r;
@@ -3668,13 +3698,15 @@ trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const tr
     const size_t npx = (size_t)s->film.width * s->film.height;
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
+    HostAov ha;
+    if ((r = ha.stage(aov, npx)) != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     if (nb) { // an empty selection renders nothing (block_queue.rs:42-44)
         r = ensure_adaptive(s);
         if (r != TRB_OK) return r;
         trb::RenderParams rp{};
         rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = s->d_film; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-        r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr);
+        r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr, ha.request());
         if (r != TRB_OK) return r;
     }
     CU(cudaEventRecord(s->ev1, 0));
@@ -3683,6 +3715,7 @@ trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const tr
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
     for (size_t i = 0; i < npx * 4; ++i) film[i] += s->h_film_staging[i]; // additive, like trb_render
+    if ((r = ha.unstage(npx)) != TRB_OK) return r;
     r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
     if (r != TRB_OK) return r;
     if (stats) {
@@ -3696,9 +3729,9 @@ trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const tr
     return TRB_OK;
 }
 
-trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, uint32_t* pixel_spp,
-                                       trb_stats* stats) {
-    if (!s || !cfg || !ad || !samples) return fail(TRB_INVALID_ARG, "null argument");
+// trb_render_samples_adaptive's body; aov: the host AOV records of trb_render_samples_adaptive_aov (nullptr: none)
+trb_status render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, trb_aov_sample* aov,
+                                   uint32_t* pixel_spp, trb_stats* stats) {
     trbh::AdSchedule sch;
     trb_status r = adaptive_check(s, cfg, ad, sch);
     if (r != TRB_OK) return r;
@@ -3716,16 +3749,28 @@ trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, 
     CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
     cudaError_t e = cudaMemsetAsync(d_out, 0, n * sizeof(trb_sample), 0); // unused slots stay zero
     if (e != cudaSuccess) { cudaFree(d_out); CU(e); }
+    DeviceBuffer d_aov;
+    if (aov) {
+        e = cudaMalloc(&d_aov.p, n * sizeof(trb_aov_sample));
+        if (e == cudaSuccess) e = cudaMemsetAsync(d_aov.p, 0, n * sizeof(trb_aov_sample), 0); // as the samples: unused slots stay zero
+        if (e != cudaSuccess) {
+            cudaFree(d_out);
+            cudaGetLastError();
+            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(e));
+        }
+    }
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     CU(cudaEventRecord(s->ev0, 0));
     trb::RenderParams rp{};
     rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr);
+    const AovRequest req{static_cast<trb_aov_sample*>(d_aov.p), nullptr, nullptr, nullptr};
+    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr, aov ? &req : nullptr);
     if (r != TRB_OK) { cudaDeviceSynchronize(); cudaFree(d_out); return r; }
     CU(cudaEventRecord(s->ev1, 0));
     e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
     cudaFree(d_out);
     CU(e);
+    if (aov) CU(cudaMemcpy(aov, d_aov.p, n * sizeof(trb_aov_sample), cudaMemcpyDeviceToHost));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
     r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
@@ -3740,9 +3785,9 @@ trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, 
     return TRB_OK;
 }
 
-trb_status trb_render_adaptive_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, uint32_t* d_pixel_spp,
-                                      trb_stats* d_stats, void* stream) {
-    if (!s || !cfg || !ad || !d_film) return fail(TRB_INVALID_ARG, "null argument");
+// trb_render_adaptive_device's body; aov: the device AOV outputs of trb_render_adaptive_aov_device (nullptr: none)
+trb_status render_adaptive_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, const AovRequest* aov, uint32_t* d_pixel_spp,
+                                  trb_stats* d_stats, cudaStream_t st) {
     trbh::AdSchedule sch;
     trb_status r = adaptive_check(s, cfg, ad, sch);
     if (r != TRB_OK) return r;
@@ -3756,7 +3801,50 @@ trb_status trb_render_adaptive_device(trb_scene* s, const trb_render_cfg* cfg, c
     trb::RenderParams rp{};
     rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = reinterpret_cast<float4*>(d_film); rp.stats = reinterpret_cast<trb::DStats*>(d_stats);
     rp.error_flag = s->d_error;
-    return render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, static_cast<cudaStream_t>(stream), d_pixel_spp);
+    return render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, st, d_pixel_spp, aov);
+}
+} // namespace
+
+trb_status trb_render_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
+    if (!s || !cfg || !ad || !film) return fail(TRB_INVALID_ARG, "null argument");
+    return render_adaptive_host(s, cfg, ad, film, nullptr, pixel_spp, stats);
+}
+
+trb_status trb_render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, uint32_t* pixel_spp,
+                                       trb_stats* stats) {
+    if (!s || !cfg || !ad || !samples) return fail(TRB_INVALID_ARG, "null argument");
+    return render_samples_adaptive(s, cfg, ad, n, samples, nullptr, pixel_spp, stats);
+}
+
+trb_status trb_render_adaptive_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, uint32_t* d_pixel_spp,
+                                      trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !ad || !d_film) return fail(TRB_INVALID_ARG, "null argument");
+    return render_adaptive_device(s, cfg, ad, d_film, nullptr, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
+}
+
+// The AOV forms: adaptive_check's statuses cover aov_supported's (the path integrator on the wavefront only)
+trb_status trb_render_adaptive_aov(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, uint32_t* pixel_spp,
+                                   trb_stats* stats) {
+    if (!s || !cfg || !ad || !film || !aov) return fail(TRB_INVALID_ARG, "null argument");
+    return render_adaptive_host(s, cfg, ad, film, aov, pixel_spp, stats);
+}
+
+trb_status trb_render_adaptive_aov_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, const trb_aov_film* d_aov,
+                                          uint32_t* d_pixel_spp, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !ad || !d_film || !d_aov) return fail(TRB_INVALID_ARG, "null argument");
+    if (((reinterpret_cast<uintptr_t>(d_film) | reinterpret_cast<uintptr_t>(d_aov->albedo_w) | reinterpret_cast<uintptr_t>(d_aov->normal_w)) & 15u) ||
+        (reinterpret_cast<uintptr_t>(d_aov->nearest) & 7u))
+        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest)};
+    const bool with_aov = d_aov->albedo_w || d_aov->normal_w || d_aov->nearest;
+    return render_adaptive_device(s, cfg, ad, d_film, with_aov ? &req : nullptr, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_render_samples_adaptive_aov(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, trb_aov_sample* aov,
+                                           uint32_t* pixel_spp, trb_stats* stats) {
+    if (!s || !cfg || !ad || !samples || !aov) return fail(TRB_INVALID_ARG, "null argument");
+    return render_samples_adaptive(s, cfg, ad, n, samples, aov, pixel_spp, stats);
 }
 
 trb_status trb_camera_rays(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_ray* rays, float* xy) {

@@ -2767,9 +2767,9 @@ __device__ __noinline__ f3 aov_albedo(const DScene& sc, const Mat& m, const Fram
 // (n, inst bits) to hi[p * step]: step 2 with hi = lo + 1 is a trb_aov_sample array, step 1 two float4 arrays the film kernels read
 // as they read wf.rad. Reads nothing the shade kernels write and writes nothing they read.
 template <bool ANIM>
-__global__ void __launch_bounds__(128) k_wf_aov(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, float4* __restrict__ lo_out,
-                                                float4* __restrict__ hi_out, uint32_t step) {
-    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < wf.n_paths; p += gridDim.x * blockDim.x) {
+__device__ __forceinline__ void wf_aov_paths(const DScene& sc, const WfState& wf, uint32_t n, float4* __restrict__ lo_out, float4* __restrict__ hi_out,
+                                             uint32_t step) {
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
         const uint4 h4 = wf.hit[p];
         float4 lo = make_float4(0.0f, 0.0f, 0.0f, finf()), hi = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(TRB_MISS));
         if (h4.x != TRB_MISS) {
@@ -2791,12 +2791,36 @@ __global__ void __launch_bounds__(128) k_wf_aov(const __grid_constant__ DScene s
         hi_out[(size_t)p * step] = hi;
     }
 }
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_wf_aov(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, float4* __restrict__ lo_out,
+                                                float4* __restrict__ hi_out, uint32_t step) {
+    wf_aov_paths<ANIM>(sc, wf, wf.n_paths, lo_out, hi_out, step);
+}
+// k_wf_aov for an Adaptive pass (DESIGN.md §4 "Adaptive AOVs"), which is launched for the worst-case path count: only the paths it
+// really holds (WF_N_PATHS, written by k_wf_generate_ad), since the paths past them keep stale state of earlier passes. The paths of
+// pixels that are not sampling this round enter as primary misses and give miss records, which no film or slot reads.
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_wf_aov_ad(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, float4* __restrict__ lo_out,
+                                                   float4* __restrict__ hi_out) {
+    wf_aov_paths<ANIM>(sc, wf, wf.counters[WF_N_PATHS], lo_out, hi_out, 1u);
+}
 
 // nearest: per camera sample of the pass, atomicMin(float_bits(depth) << 32 | inst) on the pixel the sample was taken for
 __global__ void __launch_bounds__(256) k_wf_nearest(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const float4* __restrict__ lo,
                                                     const float4* __restrict__ hi, uint32_t n, unsigned long long* __restrict__ nearest) {
     for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
         const SampleId id = sample_id(sc, rp, p);
+        atomicMin(&nearest[id.pixel], ((unsigned long long)__float_as_uint(lo[p].w) << 32) | __float_as_uint(hi[p].w));
+    }
+}
+// k_wf_nearest for an Adaptive pass: the blocks it really covers (ad_pass_blocks) and the pixels that sampled this round. Runs
+// before k_ad_decide, which clears the flag of a pixel that stops.
+__global__ void __launch_bounds__(256) k_wf_nearest_ad(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const float4* __restrict__ lo,
+                                                       const float4* __restrict__ hi, unsigned long long* __restrict__ nearest) {
+    const uint32_t n = ad_pass_blocks(rp) * 64 * rp.sample_count;
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const SampleId id = sample_id(sc, rp, p);
+        if (!(rp.ad_state[id.pixel].x & trbh::AD_ACTIVE)) continue;
         atomicMin(&nearest[id.pixel], ((unsigned long long)__float_as_uint(lo[p].w) << 32) | __float_as_uint(hi[p].w));
     }
 }
@@ -3311,6 +3335,26 @@ __global__ void __launch_bounds__(128) k_ad_decide(const __grid_constant__ DScen
         const bool more = trbh::ad_finish(st, sch, rp.ad_round);
         rp.ad_state[id.pixel] = make_uint4(st.taken, __float_as_uint(st.avg), __float_as_uint(st.lmin), __float_as_uint(st.lmax));
         if (more) block_flags[id.item] = 1u;
+    }
+}
+
+// The AOV records of a pass (k_wf_aov_ad: lo, hi indexed by path) into the parity layout of k_ad_decide's samples_out
+// (trb_render_samples_adaptive_aov): path t * sample_count + s of a pixel sampling this round goes to slot sample_first + s.
+// Runs before k_ad_decide, which clears the flag of a pixel that stops.
+__global__ void __launch_bounds__(128) k_ad_aov_slots(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const float4* __restrict__ lo,
+                                                      const float4* __restrict__ hi, trb_aov_sample* __restrict__ out) {
+    const uint32_t n = ad_pass_blocks(rp) * 64;
+    for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+        const uint32_t item = t >> 6, pix = t & 63;
+        const uint2 blk = rp.blocks[item];
+        const uint32_t pixel = (blk.y * 8 + (pix >> 3)) * sc.width + blk.x * 8 + (pix & 7);
+        if (!(rp.ad_state[pixel].x & trbh::AD_ACTIVE)) continue;
+        float4* dst = reinterpret_cast<float4*>(out + ((size_t)rp.ad_block_index[item] * 64 + pix) * rp.ad_max_per_pixel + rp.sample_first);
+        for (uint32_t s = 0; s < rp.sample_count; ++s) {
+            const size_t p = (size_t)t * rp.sample_count + s;
+            dst[2 * s] = lo[p];
+            dst[2 * s + 1] = hi[p];
+        }
     }
 }
 

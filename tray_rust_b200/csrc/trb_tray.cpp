@@ -1,7 +1,7 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
-//            [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]]
+//            [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--adaptive MIN MAX]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
 //
@@ -21,7 +21,10 @@
 // --temporal-gradients, only with --denoise-temporal, denoises with trb_denoise_temporal_gradient at the frame's seed; --denoise-moments
 // renders each frame once with AOVs (1 spp allowed), in order, with one history and seed (S + frame) mod 2^32, denoising it with
 // trb_denoise_moments (single node, path integrator, refused with the other denoise flags); --moment-gradients, only with
-// --denoise-moments, denoises with trb_denoise_moments_gradient at the frame's seed; a worker address is host[:port],
+// --denoise-moments, denoises with trb_denoise_moments_gradient at the frame's seed; --adaptive MIN MAX renders each frame with the
+// Adaptive sampler (trb_render_adaptive), or with --denoise-moments by trb_render_adaptive_aov and the moment call (single node, path
+// integrator; refused with --spp, since the sampler owns the schedule, and with --denoise, --denoise-temporal and --temporal-gradients,
+// which need two half sample ranges); a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -45,7 +48,7 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]]\n"
+    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]] [--adaptive MIN MAX]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
     "    trb_tray (-h | --help)\n"
@@ -71,6 +74,10 @@ const char* USAGE =
     "                          Single node only, path integrator.\n"
     "  --moment-gradients      With --denoise-moments only: re-shade a sample of each 3x3 pixel block of the previous frame in\n"
     "                          this one and shorten the moment history where the lighting changed. Single node only.\n"
+    "  --adaptive MIN MAX      Render with the Adaptive sampler: MIN samples per pixel, then more in rounds while a pixel's samples\n"
+    "                          disagree, up to MAX (both rounded up to powers of two). With --denoise-moments each frame is also\n"
+    "                          rendered with albedo, normal and depth and denoised by the moment denoiser.\n"
+    "                          Single node only, path integrator; not with --spp, --denoise or --denoise-temporal.\n"
     "  -h, --help              Show this message.\n";
 
 int die(const char* fmt, ...) {
@@ -161,8 +168,8 @@ struct Args {
     std::vector<std::string> workers;
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
-         denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false;
-    uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0;
+         denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false, adaptive = false;
+    uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0, ad_min = 0, ad_max = 0;
 };
 
 // scene description (host only): the film section, frame range overrides applied
@@ -219,14 +226,16 @@ struct MomentsFrame {
     std::vector<float> colour, albedo, normal, out;
     std::vector<uint64_t> nearest;
     explicit MomentsFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history, bool gradients) {
+    // ad: the Adaptive sampler in place of LowDiscrepancy at spp (trb_render_adaptive_aov; DESIGN.md §4 "Adaptive AOVs"), or nullptr
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history, bool gradients, const trb_adaptive* ad) {
         std::fill(colour.begin(), colour.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
         trb_render_cfg cfg{};
         cfg.spp = spp; cfg.seed = seed; cfg.current_frame = frame;
         const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
-        tray::check(trb_render_aov(s, &cfg, colour.data(), &aov, nullptr)); // includes Scene::update_frame
+        if (ad) { cfg.spp = 0; tray::check(trb_render_adaptive_aov(s, &cfg, ad, colour.data(), &aov, nullptr, nullptr)); } // includes Scene::update_frame
+        else tray::check(trb_render_aov(s, &cfg, colour.data(), &aov, nullptr)); // includes Scene::update_frame
         const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
         if (gradients) {
             const trb_denoise_moments_gradient_output o{out.data(), nullptr, nullptr, nullptr, nullptr};
@@ -251,6 +260,9 @@ int single_node(const Args& a, const OutPath& out) {
     if (denoise && spp < 2) return die("%s needs at least 2 samples per pixel (two half renders); the scene has %u", flag, spp);
     if (a.denoise_moments && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
         return die("--denoise-moments needs the path integrator: the scene's integrator renders no albedo, normal or depth");
+    if (a.adaptive && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("--adaptive needs the path integrator: the Adaptive sampler is built for it only");
+    const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
     try {
         tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
         trb_desc_free(desc.d); desc.d = nullptr;
@@ -259,6 +271,8 @@ int single_node(const Args& a, const OutPath& out) {
         tray::B200 exec;
         tray::Config config;
         config.seed = (uint32_t)a.seed;
+        config.adaptive = a.adaptive;
+        config.sampler = tray::Adaptive{ad.min_spp, ad.max_spp};
         const auto scene_start = std::chrono::steady_clock::now();
         std::unique_ptr<DenoisedFrame> dn;
         if (denoise) dn.reset(new DenoisedFrame((size_t)dim.first * dim.second));
@@ -271,7 +285,7 @@ int single_node(const Args& a, const OutPath& out) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (mf) {
-                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients);
+                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients, a.adaptive ? &ad : nullptr);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(scene.handle(), mf->out.data(), img.data()));
             } else if (dn) {
@@ -483,7 +497,7 @@ int master_node(const Args& a, const OutPath& out) {
 
 int main(int argc, char** argv) {
     bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false,
-         moment_gradients = false;
+         moment_gradients = false, adaptive = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
@@ -491,7 +505,9 @@ int main(int argc, char** argv) {
         denoise_temporal = denoise_temporal || std::strcmp(argv[i], "--denoise-temporal") == 0;
         denoise_moments = denoise_moments || std::strcmp(argv[i], "--denoise-moments") == 0;
         moment_gradients = moment_gradients || std::strcmp(argv[i], "--moment-gradients") == 0;
+        adaptive = adaptive || std::strcmp(argv[i], "--adaptive") == 0;
     }
+    if (worker && adaptive) return die("--adaptive is not available with --worker: the wire format carries no sampler");
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_temporal)
         return die("--denoise-temporal is not available with --worker: the wire format carries no albedo, normal or depth");
@@ -526,6 +542,12 @@ int main(int argc, char** argv) {
         else if (s == "--temporal-gradients") a.temporal_gradients = true;
         else if (s == "--denoise-moments") a.denoise_moments = true;
         else if (s == "--moment-gradients") a.moment_gradients = true;
+        else if (s == "--adaptive") { // two numbers: MIN MAX
+            const char* v2 = i + 2 < argc ? argv[i + 2] : nullptr;
+            ok = parse_u64(v, a.ad_min) && parse_u64(v2, a.ad_max) && a.ad_min <= UINT32_MAX && a.ad_max <= UINT32_MAX;
+            if (!ok) die("--adaptive needs two non-negative integers: MIN MAX");
+            a.adaptive = true; i += 2;
+        }
         else if (!s.empty() && s[0] == '-') { std::fputs(USAGE, stderr); return 2; }
         else if (!have_scene) { a.scene = s; have_scene = true; }
         else a.workers.push_back(s);
@@ -551,6 +573,15 @@ int main(int argc, char** argv) {
         return die("--temporal-gradients is not available with --master: the wire format carries no albedo, normal or depth");
     if (a.temporal_gradients && !a.denoise_temporal) return die("--temporal-gradients needs --denoise-temporal");
     if (a.denoise_temporal && a.has_spp && a.spp < 2) return die("--denoise-temporal needs at least 2 samples per pixel (two half renders)");
+    if (a.master && a.adaptive) return die("--adaptive is not available with --master: the wire format carries no sampler");
+    if (a.adaptive && a.has_spp) return die("--adaptive excludes --spp: the Adaptive sampler owns the sample schedule");
+    if (a.adaptive && (a.denoise || a.denoise_temporal || a.temporal_gradients))
+        return die("--adaptive excludes --denoise, --denoise-temporal and --temporal-gradients: they need two half sample ranges; use --denoise-moments");
+    if (a.adaptive) {
+        const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
+        if (trb_adaptive_schedule(&ad, nullptr, nullptr, nullptr, nullptr) != TRB_OK) return die("--adaptive %llu %llu: %s", (unsigned long long)a.ad_min,
+                                                                                                (unsigned long long)a.ad_max, trb_last_error());
+    }
     if (a.has_start && a.has_end && a.end < a.start)
         return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
     OutPath out;
