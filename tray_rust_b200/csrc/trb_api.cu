@@ -7,7 +7,6 @@
 #include <cstdlib>
 #include <memory>
 #include <thread>
-#include <tuple>
 #include <cub/device/device_radix_sort.cuh>
 #include "trb_host.h"
 #include "trb_kernels.cuh"
@@ -56,6 +55,79 @@ struct DeviceArena { // owns every cudaMalloc of a scene
             if (ptrs[i] == p) { cudaFree(ptrs[i]); ptrs[i] = ptrs.back(); ptrs.pop_back(); return; }
     }
 };
+
+// A failed CUDA call as TRB_OOM (out of memory) or TRB_CUDA, with `what` leading the message; the call's error is cleared
+trb_status cuda_fail(cudaError_t e, const char* what) {
+    cudaGetLastError();
+    return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+}
+
+// A device allocation of `bytes`; a failure is cuda_fail's and leaves *p null
+trb_status device_alloc(void** p, size_t bytes, const char* what) {
+    const cudaError_t e = cudaMalloc(p, bytes);
+    if (e == cudaSuccess) return TRB_OK;
+    *p = nullptr;
+    return cuda_fail(e, what);
+}
+
+// A per-call device temporary, freed with the scope
+struct DeviceBuffer {
+    void* p = nullptr;
+    DeviceBuffer() = default;
+    DeviceBuffer(const DeviceBuffer&) = delete;
+    DeviceBuffer& operator=(const DeviceBuffer&) = delete;
+    ~DeviceBuffer() { reset(); }
+    trb_status alloc(size_t bytes, const char* what) { return device_alloc(&p, bytes, what); }
+    cudaError_t reset() { const cudaError_t e = p ? cudaFree(p) : cudaSuccess; p = nullptr; return e; }
+    template <class T> T* as() const { return static_cast<T*>(p); }
+};
+
+using Span = std::pair<const void*, size_t>;
+using OutSpan = std::pair<void*, size_t>;
+
+// The blocking host form of a call. Each input span is copied into a device buffer of its own, and each output span whose host pointer
+// is not null gets one; enqueue(d) runs on the default stream with d the buffers of the inputs, then of the outputs (a null output's
+// holds null), and the outputs are copied back. Passes a failed enqueue left in flight still read the buffers, so the device is
+// drained before they are freed.
+template <class Enqueue>
+trb_status run_staged(std::initializer_list<Span> ins, std::initializer_list<OutSpan> outs, Enqueue enqueue) {
+    std::vector<DeviceBuffer> d(ins.size() + outs.size());
+    DeviceBuffer* b = d.data();
+    trb_status r;
+    for (const Span& in : ins) {
+        if ((r = b->alloc(in.second, "host-form staging")) != TRB_OK) return r;
+        CU(cudaMemcpy(b->p, in.first, in.second, cudaMemcpyHostToDevice));
+        ++b;
+    }
+    for (const OutSpan& out : outs) {
+        if (out.first && (r = b->alloc(out.second, "host-form staging")) != TRB_OK) return r;
+        ++b;
+    }
+    if ((r = enqueue(d.data())) != TRB_OK) { cudaDeviceSynchronize(); return r; }
+    b = d.data() + ins.size();
+    for (const OutSpan& out : outs) {
+        if (out.first) CU(cudaMemcpy(out.first, b->p, out.second, cudaMemcpyDeviceToHost));
+        ++b;
+    }
+    return TRB_OK;
+}
+
+// The device forms' alignment check: TRB_INVALID_ARG with `msg` unless every pointer is a multiple of its alignment (a power of two)
+trb_status check_aligned(std::initializer_list<std::pair<const void*, uintptr_t>> ptrs, const char* msg) {
+    for (const auto& [p, align] : ptrs)
+        if (reinterpret_cast<uintptr_t>(p) & (align - 1)) return fail(TRB_INVALID_ARG, msg);
+    return TRB_OK;
+}
+
+// Whether two buffers overlap (a null one overlaps nothing)
+bool spans_overlap(Span a, Span b) {
+    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a.first), b0 = reinterpret_cast<uintptr_t>(b.first);
+    return a.first && b.first && a0 < b0 + b.second && b0 < a0 + a.second;
+}
+bool overlaps_any(Span a, std::initializer_list<Span> others) {
+    for (const Span& b : others) if (spans_overlap(a, b)) return true;
+    return false;
+}
 
 struct HostMesh {
     std::vector<trb_bvh_node> nodes;
@@ -556,12 +628,8 @@ trb_status ensure_aov(trb_scene* s) {
     CU(cudaDeviceSynchronize()); // a pass still in flight owns the old buffer
     if (s->d_aov) cudaFree(s->d_aov);
     s->d_aov = nullptr; s->aov_capacity = 0;
-    const cudaError_t err = cudaMalloc(reinterpret_cast<void**>(&s->d_aov), s->wf_capacity * 2 * sizeof(float4));
-    if (err != cudaSuccess) {
-        s->d_aov = nullptr;
-        cudaGetLastError();
-        return fail(err == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(err));
-    }
+    const trb_status r = device_alloc(reinterpret_cast<void**>(&s->d_aov), s->wf_capacity * 2 * sizeof(float4), "AOV records");
+    if (r != TRB_OK) return r;
     s->aov_capacity = s->wf_capacity;
     return TRB_OK;
 }
@@ -599,8 +667,7 @@ trb_status ensure_wavefront(trb_scene* s, size_t n_paths) {
     if (err != cudaSuccess) {
         for (void* p : s->wf_allocs) cudaFree(p);
         s->wf_allocs.clear();
-        cudaGetLastError();
-        return fail(err == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("wavefront state: ") + cudaGetErrorString(err));
+        return cuda_fail(err, "wavefront state");
     }
     s->wf_capacity = cap;
     return TRB_OK;
@@ -1012,11 +1079,37 @@ void stats_out(const trb::DStats& d, trb_stats* o) {
     o->rays_continuation = d.rays_continuation; o->node_tests = d.node_tests; o->tri_tests = d.tri_tests; o->inst_tests = d.inst_tests;
 }
 
+// A host form's trb_stats (none when stats is null): the scene's counters, the kernel time between its events and update_ms
+trb_status stats_readback(trb_scene* s, trb_stats* stats, float update_ms) {
+    if (!stats) return TRB_OK;
+    trb::DStats h;
+    CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
+    std::memset(stats, 0, sizeof *stats);
+    stats_out(h, stats);
+    CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
+    stats->update_ms = update_ms;
+    return TRB_OK;
+}
+
 trb_status check_error_flag(trb_scene* s) {
     int e = 0;
     CU(cudaMemcpy(&e, s->d_error, sizeof e, cudaMemcpyDeviceToHost));
     if (e) { CU(cudaMemset(s->d_error, 0, sizeof(int))); return fail(TRB_CUDA, "BVH traversal stack overflow (depth > 64; the reference would panic)"); }
     return TRB_OK;
+}
+
+// run_staged for the host forms that report counters (trb_intersect, the ray and illumination queries, the sample renders): the
+// scene's counters cleared and its events recorded around enqueue, then the traversal error flag checked
+template <class Enqueue>
+trb_status run_counted(trb_scene* s, std::initializer_list<Span> ins, std::initializer_list<OutSpan> outs, Enqueue enqueue) {
+    const trb_status r = run_staged(ins, outs, [&](const DeviceBuffer* d) {
+        CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
+        CU(cudaEventRecord(s->ev0, 0));
+        const trb_status q = enqueue(d);
+        if (q == TRB_OK) CU(cudaEventRecord(s->ev1, 0));
+        return q;
+    });
+    return r != TRB_OK ? r : check_error_flag(s);
 }
 
 // ---- ray queries (trb_intersect_records / trb_occluded; DESIGN.md §5 "Ray queries") ---------------------------------------
@@ -1025,8 +1118,7 @@ trb_status check_error_flag(trb_scene* s) {
 trb_status query_check(const trb_scene* s, size_t n, const void* rays, const void* out, uint32_t flags, uint32_t allowed, bool device, bool out16) {
     if (!s || (n && (!rays || !out))) return fail(TRB_INVALID_ARG, "null argument");
     if (flags & ~allowed) return fail(TRB_INVALID_ARG, "unsupported flag bits for a ray query");
-    if (device && n && ((reinterpret_cast<uintptr_t>(rays) | (out16 ? reinterpret_cast<uintptr_t>(out) : 0u)) & 15u))
-        return fail(TRB_INVALID_ARG, "device query buffers must be 16-byte aligned");
+    if (device && n) { const trb_status r = check_aligned({{rays, 16}, {out, out16 ? 16 : 1}}, "device query buffers must be 16-byte aligned"); if (r != TRB_OK) return r; }
     if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
     return TRB_OK;
 }
@@ -1117,42 +1209,18 @@ trb_status illum_passes(trb_scene* s, size_t n, const trb_illum_ray* d_rays, uin
 
 trb_status illum_check(const trb_scene* s, size_t n, const void* rays, uint32_t spp, const void* rgb, uint32_t flags, bool device) {
     if (spp == 0 || spp > 65536) return fail(TRB_INVALID_ARG, "spp must be in [1, 65536]");
-    if (device && n && (reinterpret_cast<uintptr_t>(rgb) & 3u)) return fail(TRB_INVALID_ARG, "the device rgb buffer must be 4-byte aligned");
+    if (device && n) { const trb_status r = check_aligned({{rgb, 4}}, "the device rgb buffer must be 4-byte aligned"); if (r != TRB_OK) return r; }
     return query_check(s, n, rays, rgb, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW | TRB_QUERY_CLAMP, device, false);
 }
 
-// The blocking host-buffer form of a query: stage the rays, run enqueue(d_rays, d_out) on the default stream, copy the results back.
+// The host form of a ray or illumination query: the rays staged, enqueue(d_rays, d_out) counted (run_counted), the results and the
+// counters read back; no rays leave zero counters
 template <class Enqueue>
-trb_status query_host(trb_scene* s, size_t n, const void* rays, size_t ray_bytes, void* out, size_t out_bytes, trb_stats* stats, Enqueue enqueue) {
+trb_status run_query(trb_scene* s, size_t n, Span rays, OutSpan out, trb_stats* stats, Enqueue enqueue) {
     if (n == 0) { if (stats) std::memset(stats, 0, sizeof *stats); return TRB_OK; }
     CU(cudaSetDevice(s->device));
-    void* d_rays = nullptr; void* d_res = nullptr;
-    CU(cudaMalloc(&d_rays, ray_bytes));
-    cudaError_t e = cudaMalloc(&d_res, out_bytes);
-    if (e != cudaSuccess) { cudaFree(d_rays); CU(e); }
-    e = cudaMemcpy(d_rays, rays, ray_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0);
-    trb_status r = TRB_OK;
-    if (e == cudaSuccess) {
-        cudaEventRecord(s->ev0, 0);
-        r = enqueue(d_rays, d_res);
-        cudaEventRecord(s->ev1, 0);
-    }
-    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out, d_res, out_bytes, cudaMemcpyDeviceToHost);
-    if (r != TRB_OK) cudaDeviceSynchronize(); // passes already enqueued still read the buffers
-    cudaFree(d_rays); cudaFree(d_res);
-    if (r != TRB_OK) return r;
-    CU(e);
-    r = check_error_flag(s);
-    if (r != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-    }
-    return TRB_OK;
+    const trb_status r = run_counted(s, {rays}, {out}, [&](const DeviceBuffer* d) { return enqueue(d[0].p, d[1].p); });
+    return r != TRB_OK ? r : stats_readback(s, stats, 0.f);
 }
 
 // The static part of the device instance records (everything but the matrices, which update_frame writes); keyframed / animated flags
@@ -1235,37 +1303,17 @@ void spline_dedup(const trb_scene* s, std::vector<uint32_t>& uniq_of, std::vecto
 // loads on the device; `out_align` is the device output's required alignment. `frame`: the query reads the instance matrices.
 trb_status shade_check(const trb_scene* s, size_t n, const void* a, const void* b, const void* out, uintptr_t out_align, bool device, bool frame) {
     if (!s || (n && (!a || !b || !out))) return fail(TRB_INVALID_ARG, "null argument");
-    if (device && n && (((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15u) || (reinterpret_cast<uintptr_t>(out) & (out_align - 1))))
-        return fail(TRB_INVALID_ARG, out_align == 16 ? "device query buffers must be 16-byte aligned"
-                                                     : "device query buffers must be 16-byte aligned, the float output 4-byte aligned");
+    if (device && n) {
+        const trb_status r = check_aligned({{a, 16}, {b, 16}, {out, out_align}}, out_align == 16 ? "device query buffers must be 16-byte aligned"
+                                                                                                 : "device query buffers must be 16-byte aligned, the float output 4-byte aligned");
+        if (r != TRB_OK) return r;
+    }
     if (frame && !s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering"); // scene.rs:179
     return TRB_OK;
 }
 
 // One thread per query, grid-stride: at most 16 CTAs of 128 threads per SM
 inline unsigned shade_grid(const trb_scene* s, size_t n) { return (unsigned)std::min<size_t>((n + 127) / 128, (size_t)s->sm_count * 16); }
-
-// The blocking host-buffer form of a shading query: stage the inputs (b may be null) in one device allocation, run enqueue(d_a, d_b,
-// d_out) on the default stream, copy the results back.
-template <class Enqueue>
-trb_status shade_host(trb_scene* s, size_t n, const void* a, size_t a_bytes, const void* b, size_t b_bytes, void* out, size_t out_bytes,
-                      Enqueue enqueue) {
-    if (n == 0) return TRB_OK;
-    CU(cudaSetDevice(s->device));
-    const size_t b_off = (a_bytes + 255) / 256 * 256, o_off = b_off + (b_bytes + 255) / 256 * 256;
-    char* d = nullptr;
-    CU(cudaMalloc(&d, o_off + out_bytes));
-    cudaError_t e = cudaMemcpy(d, a, a_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && b) e = cudaMemcpy(d + b_off, b, b_bytes, cudaMemcpyHostToDevice);
-    trb_status r = TRB_OK;
-    if (e == cudaSuccess) r = enqueue(d, d + b_off, d + o_off);
-    if (e == cudaSuccess && r == TRB_OK) e = cudaMemcpy(out, d + o_off, out_bytes, cudaMemcpyDeviceToHost);
-    if (r != TRB_OK) cudaDeviceSynchronize();
-    cudaFree(d);
-    if (r != TRB_OK) return r;
-    CU(e);
-    return TRB_OK;
-}
 
 trb_status launch_bsdf_eval(trb_scene* s, size_t n, const trb_intersection* d_rec, const trb_bsdf_eval_query* d_q, float* d_out, cudaStream_t st) {
     trb::k_bsdf_eval<<<shade_grid(s, n), 128, 0, st>>>(s->ds, (uint32_t)s->materials.size(), n, d_rec, d_q, reinterpret_cast<float4*>(d_out));
@@ -1309,8 +1357,7 @@ trb_status film_check(const trb_scene* s, size_t n, const void* samples, const v
     if (!s) return fail(TRB_INVALID_ARG, "null argument");
     if ((uint64_t)n >= (1ull << 32)) return fail(TRB_INVALID_ARG, "film writes take fewer than 2^32 samples");
     if (n && (!samples || !regions || !film)) return fail(TRB_INVALID_ARG, "null argument");
-    if (device && n && ((reinterpret_cast<uintptr_t>(samples) | reinterpret_cast<uintptr_t>(regions) | reinterpret_cast<uintptr_t>(film)) & 3u))
-        return fail(TRB_INVALID_ARG, "device film-write buffers must be 4-byte aligned");
+    if (device && n) return check_aligned({{samples, 4}, {regions, 4}, {film, 4}}, "device film-write buffers must be 4-byte aligned");
     return TRB_OK;
 }
 
@@ -1329,8 +1376,8 @@ trb_status film_write_enqueue(trb_scene* s, uint32_t n, const trb_sample* d_samp
         CU(cudaDeviceSynchronize()); // a write still in flight owns the old scratch
         cudaFree(s->d_film_scratch);
         s->d_film_scratch = nullptr; s->film_scratch_bytes = 0;
-        const cudaError_t e = cudaMalloc(&s->d_film_scratch, need);
-        if (e != cudaSuccess) { cudaGetLastError(); s->d_film_scratch = nullptr; CU(e); }
+        const trb_status r = device_alloc(&s->d_film_scratch, need, "film write scratch");
+        if (r != TRB_OK) return r;
         s->film_scratch_bytes = need;
     }
     char* base = static_cast<char*>(s->d_film_scratch);
@@ -1423,74 +1470,68 @@ trb_status upload_mesh_nodes(trb_scene* s, bool wide) {
 // their leaf-end marks into dtris. The triangle boxes are computed on the device. The SAH build runs on the device, or on the host
 // (BvhBuilder over the boxes read back) when `on_device` is off or its scratch does not fit in free device memory, which keeps the
 // largest meshes loadable. Every scratch buffer is freed before returning, except that with `keep` the device-built node array is
-// handed to the caller (*keep stays null after a host build). `ev_built` / `ev_read` (optional) are recorded on the default stream
+// handed to the caller (keep stays empty after a host build). `ev_built` / `ev_read` (optional) are recorded on the default stream
 // once the tree is built and once it has been read back to the host (a host build records both after building).
 trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, uint32_t n, HostMesh& hm, trb::DTri* dtris,
-                          trb_bvh_node** keep = nullptr, cudaEvent_t ev_built = nullptr, cudaEvent_t ev_read = nullptr) {
-    float* d_boxes = nullptr;
-    uint32_t* d_order = nullptr; // + one word: the node count
-    trb_bvh_node* d_nodes = nullptr;
-    bool built = false;          // d_nodes holds the device-built tree
+                          DeviceBuffer* keep = nullptr, cudaEvent_t ev_built = nullptr, cudaEvent_t ev_read = nullptr) {
+    DeviceBuffer boxes, order, nodes; // order: + one word, the node count
+    bool built = false;               // nodes holds the device-built tree
     const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
-    auto run = [&]() -> trb_status {
-        CU(cudaMalloc(&d_boxes, 24 * (size_t)n));
-        CU(cudaMalloc(&d_order, 4 * ((size_t)n + 1)));
-        trb::bvhb::k_tri_boxes<<<grid(n), 256>>>(dp, di, n, d_boxes);
-        ++g_launches;
-        size_t free_b = 0, total_b = 0;
-        CU(cudaMemGetInfo(&free_b, &total_b));
-        const size_t need = trb::bvhb::build_scratch_bytes(n) + (2 * (size_t)n - 1) * sizeof(trb_bvh_node) + ((size_t)64 << 20);
-        if (on_device && need <= free_b) {
-            CU(cudaMalloc(&d_nodes, (2 * (size_t)n - 1) * sizeof(trb_bvh_node)));
-            bool empty = false;
-            CU(trb::bvhb::build_device(d_boxes, n, 16, d_order + n, d_nodes, d_order, 0, &g_launches, &empty));
-            if (empty) return fail(TRB_INVALID_ARG, "mesh triangles with infinite coordinates: the SAH build would split a node into an empty child");
-            built = true;
-            if (ev_built) CU(cudaEventRecord(ev_built, 0));
-            uint32_t nn = 0;
-            CU(cudaMemcpy(&nn, d_order + n, 4, cudaMemcpyDeviceToHost));
-            hm.nodes.resize(nn);
-            hm.order.resize(n);
-            CU(cudaMemcpy(hm.nodes.data(), d_nodes, (size_t)nn * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
-            CU(cudaMemcpy(hm.order.data(), d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
-            if (ev_read) CU(cudaEventRecord(ev_read, 0));
-        } else {
-            {
-                std::vector<Box3> tb(n);
-                CU(cudaMemcpy(tb.data(), d_boxes, 24 * (size_t)n, cudaMemcpyDeviceToHost));
-                BvhBuilder bb;
-                bb.build(tb, 16);
-                hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
-            }
-            if (ev_built) CU(cudaEventRecord(ev_built, 0));
-            if (ev_read) CU(cudaEventRecord(ev_read, 0));
-            CU(cudaMemcpy(d_order, hm.order.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
+    trb_status r;
+    if ((r = boxes.alloc(24 * (size_t)n, "mesh BVH scratch")) != TRB_OK || (r = order.alloc(4 * ((size_t)n + 1), "mesh BVH scratch")) != TRB_OK) return r;
+    float* d_boxes = boxes.as<float>();
+    uint32_t* d_order = order.as<uint32_t>();
+    trb::bvhb::k_tri_boxes<<<grid(n), 256>>>(dp, di, n, d_boxes);
+    ++g_launches;
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    const size_t need = trb::bvhb::build_scratch_bytes(n) + (2 * (size_t)n - 1) * sizeof(trb_bvh_node) + ((size_t)64 << 20);
+    if (on_device && need <= free_b) {
+        if ((r = nodes.alloc((2 * (size_t)n - 1) * sizeof(trb_bvh_node), "mesh BVH scratch")) != TRB_OK) return r;
+        bool empty = false;
+        CU(trb::bvhb::build_device(d_boxes, n, 16, d_order + n, nodes.as<trb_bvh_node>(), d_order, 0, &g_launches, &empty));
+        if (empty) return fail(TRB_INVALID_ARG, "mesh triangles with infinite coordinates: the SAH build would split a node into an empty child");
+        built = true;
+        if (ev_built) CU(cudaEventRecord(ev_built, 0));
+        uint32_t nn = 0;
+        CU(cudaMemcpy(&nn, d_order + n, 4, cudaMemcpyDeviceToHost));
+        hm.nodes.resize(nn);
+        hm.order.resize(n);
+        CU(cudaMemcpy(hm.nodes.data(), nodes.p, (size_t)nn * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(hm.order.data(), d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
+        if (ev_read) CU(cudaEventRecord(ev_read, 0));
+    } else {
+        {
+            std::vector<Box3> tb(n);
+            CU(cudaMemcpy(tb.data(), d_boxes, 24 * (size_t)n, cudaMemcpyDeviceToHost));
+            BvhBuilder bb;
+            bb.build(tb, 16);
+            hm.nodes = std::move(bb.nodes); hm.order = std::move(bb.order);
         }
-        CU(cudaFree(d_boxes));
-        d_boxes = nullptr;
-        trb::bvhb::k_tri_pack<<<grid(n), 256>>>(dp, di, d_order, n, dtris);
-        ++g_launches;
-        if (!d_nodes) { // host build: the marks are set from the host tree, a chunk of nodes at a time
-            const size_t chunk = std::min<size_t>(hm.nodes.size(), (size_t)1 << 22);
-            CU(cudaMalloc(&d_nodes, chunk * sizeof(trb_bvh_node)));
-            for (size_t i = 0; i < hm.nodes.size(); i += chunk) {
-                const size_t k = std::min(chunk, hm.nodes.size() - i);
-                CU(cudaMemcpy(d_nodes, hm.nodes.data() + i, k * sizeof(trb_bvh_node), cudaMemcpyHostToDevice));
-                trb::bvhb::k_tri_leaf_marks<<<grid(k), 256>>>(d_nodes, (uint32_t)k, dtris);
-                ++g_launches;
-            }
-        } else {
-            trb::bvhb::k_tri_leaf_marks<<<grid(hm.nodes.size()), 256>>>(d_nodes, (uint32_t)hm.nodes.size(), dtris);
+        if (ev_built) CU(cudaEventRecord(ev_built, 0));
+        if (ev_read) CU(cudaEventRecord(ev_read, 0));
+        CU(cudaMemcpy(d_order, hm.order.data(), 4 * (size_t)n, cudaMemcpyHostToDevice));
+    }
+    CU(boxes.reset());
+    trb::bvhb::k_tri_pack<<<grid(n), 256>>>(dp, di, d_order, n, dtris);
+    ++g_launches;
+    if (!built) { // host build: the marks are set from the host tree, a chunk of nodes at a time
+        const size_t chunk = std::min<size_t>(hm.nodes.size(), (size_t)1 << 22);
+        if ((r = nodes.alloc(chunk * sizeof(trb_bvh_node), "mesh BVH scratch")) != TRB_OK) return r;
+        for (size_t i = 0; i < hm.nodes.size(); i += chunk) {
+            const size_t k = std::min(chunk, hm.nodes.size() - i);
+            CU(cudaMemcpy(nodes.p, hm.nodes.data() + i, k * sizeof(trb_bvh_node), cudaMemcpyHostToDevice));
+            trb::bvhb::k_tri_leaf_marks<<<grid(k), 256>>>(nodes.as<trb_bvh_node>(), (uint32_t)k, dtris);
             ++g_launches;
         }
-        CU(cudaGetLastError());
-        CU(cudaDeviceSynchronize());
-        return TRB_OK;
-    };
-    const trb_status r = run();
-    if (r == TRB_OK && keep && built) { *keep = d_nodes; d_nodes = nullptr; }
-    cudaFree(d_boxes); cudaFree(d_order); cudaFree(d_nodes);
-    return r;
+    } else {
+        trb::bvhb::k_tri_leaf_marks<<<grid(hm.nodes.size()), 256>>>(nodes.as<trb_bvh_node>(), (uint32_t)hm.nodes.size(), dtris);
+        ++g_launches;
+    }
+    CU(cudaGetLastError());
+    CU(cudaDeviceSynchronize());
+    if (keep && built) std::swap(keep->p, nodes.p);
+    return TRB_OK;
 }
 
 // DPair records of a device-built mesh tree (d_nodes, n nodes) in one leaf form, with pack_pairs' layout, on the default stream.
@@ -1498,33 +1539,29 @@ trb_status build_mesh_bvh(bool on_device, const float* dp, const uint32_t* di, u
 // records. *fits_narrow: whether every leaf fits the narrow reference. Scratch is freed before returning.
 template <class Records>
 trb_status pack_pairs_device(const trb_bvh_node* d_nodes, uint32_t n, bool wide, Records records, bool* fits_narrow) {
-    uint32_t* d_rec = nullptr; // n + 1 ranks, then the narrow-misfit word
-    void* d_cub = nullptr;
+    DeviceBuffer rec, scan; // rec: n + 1 ranks, then the narrow-misfit word
     const auto grid = [](size_t k) { return (unsigned)((k + 255) / 256); };
-    auto run = [&]() -> trb_status {
-        size_t cub_bytes = 0;
-        CU(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)n + 1));
-        CU(cudaMalloc(&d_rec, 4 * ((size_t)n + 2)));
-        CU(cudaMalloc(&d_cub, std::max<size_t>(1, cub_bytes)));
-        CU(cudaMemset(d_rec + n + 1, 0, 4));
-        trb::bvhb::k_pair_flags<<<grid((size_t)n + 1), 256>>>(d_nodes, n, d_rec);
-        ++g_launches;
-        CU(cub::DeviceScan::ExclusiveSum(d_cub, cub_bytes, d_rec, d_rec, (int)n + 1));
-        uint32_t n_rec = 0;
-        CU(cudaMemcpy(&n_rec, d_rec + n, 4, cudaMemcpyDeviceToHost));
-        trb::DPair* out = nullptr;
-        { const trb_status r = records(n_rec, &out); if (r != TRB_OK) return r; }
-        trb::bvhb::k_pair_pack<<<grid(n), 256>>>(d_nodes, n, d_rec, wide, out, d_rec + n + 1);
-        ++g_launches;
-        CU(cudaGetLastError());
-        uint32_t bad = 0;
-        CU(cudaMemcpy(&bad, d_rec + n + 1, 4, cudaMemcpyDeviceToHost));
-        *fits_narrow = bad == 0;
-        return TRB_OK;
-    };
-    const trb_status r = run();
-    cudaFree(d_rec); cudaFree(d_cub);
-    return r;
+    size_t cub_bytes = 0;
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)n + 1));
+    trb_status r;
+    if ((r = rec.alloc(4 * ((size_t)n + 2), "node record scratch")) != TRB_OK || (r = scan.alloc(std::max<size_t>(1, cub_bytes), "node record scratch")) != TRB_OK)
+        return r;
+    uint32_t* d_rec = rec.as<uint32_t>();
+    CU(cudaMemset(d_rec + n + 1, 0, 4));
+    trb::bvhb::k_pair_flags<<<grid((size_t)n + 1), 256>>>(d_nodes, n, d_rec);
+    ++g_launches;
+    CU(cub::DeviceScan::ExclusiveSum(scan.p, cub_bytes, d_rec, d_rec, (int)n + 1));
+    uint32_t n_rec = 0;
+    CU(cudaMemcpy(&n_rec, d_rec + n, 4, cudaMemcpyDeviceToHost));
+    trb::DPair* out = nullptr;
+    if ((r = records(n_rec, &out)) != TRB_OK) return r;
+    trb::bvhb::k_pair_pack<<<grid(n), 256>>>(d_nodes, n, d_rec, wide, out, d_rec + n + 1);
+    ++g_launches;
+    CU(cudaGetLastError());
+    uint32_t bad = 0;
+    CU(cudaMemcpy(&bad, d_rec + n + 1, 4, cudaMemcpyDeviceToHost));
+    *fits_narrow = bad == 0;
+    return TRB_OK;
 }
 
 // One mesh of a description into fresh buffers of `arena` (trb_scene_create, trb_scene_replace_meshes), checked by validate_mesh: the
@@ -1639,7 +1676,7 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
     if (pos) {
         float* d_pos = nullptr;
         trb::DTri* d_tris = nullptr;
-        trb_bvh_node* d_nodes = nullptr; // the device-built tree (null after a host build)
+        DeviceBuffer d_nodes; // the device-built tree (empty after a host build)
         HostMesh nm;
         auto build = [&]() -> trb_status {
             CU(s->arena.alloc(3 * nv, &d_pos));
@@ -1664,9 +1701,9 @@ trb_status update_mesh(trb_scene* s, uint32_t mi, const float* pos, const float*
         };
         bool narrow = true;
         trb_status r = TRB_OK;
-        if (d_nodes) {
-            r = pack_pairs_device(d_nodes, (uint32_t)nm.nodes.size(), s->wide_leaf, records, &narrow);
-            cudaFree(d_nodes);
+        if (d_nodes.p) {
+            r = pack_pairs_device(d_nodes.as<trb_bvh_node>(), (uint32_t)nm.nodes.size(), s->wide_leaf, records, &narrow);
+            d_nodes.reset();
         } else { // host build: the records are packed on the host, as at creation. A tree that does not fit the scene's narrow form is
                  // packed wide (the form changes below and every mesh is re-packed): either way the buffer is sized for its interior nodes
             narrow = leaves_fit_narrow(nm.nodes);
@@ -1774,8 +1811,7 @@ trb_status edit_check(const trb_scene* s, uint32_t first, uint32_t count, const 
     if (count == 0) { *done = true; return TRB_OK; }
     if (!a) return fail(TRB_INVALID_ARG, "null array");
     if ((uint64_t)first + count > n) return fail(TRB_INVALID_ARG, "edit range out of bounds");
-    if (device && (reinterpret_cast<uintptr_t>(a) & 3u)) return fail(TRB_INVALID_ARG, "device array must be 4-byte aligned");
-    return TRB_OK;
+    return device ? check_aligned({{a, 4}}, "device array must be 4-byte aligned") : TRB_OK;
 }
 
 // The host mirror, the device keyframe table, the level transforms of the one-control-point splines whose point was edited and, when
@@ -2688,12 +2724,6 @@ trb_status aov_supported(const trb_scene* s, const trb_render_cfg* cfg) {
     return TRB_OK;
 }
 
-// a device buffer freed with the scope
-struct DeviceBuffer {
-    void* p = nullptr;
-    ~DeviceBuffer() { if (p) cudaFree(p); }
-};
-
 // additive, like film::Image::add_pixels (image.rs:21-33); a 33 MB read-modify-write: split over a few host threads
 void add_film(float* film, const float* src, size_t n) {
     const unsigned nt = n >= (1u << 20) ? std::min(8u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
@@ -2713,10 +2743,17 @@ struct HostAov {
     trb_status stage(const trb_aov_film* a, size_t npx) {
         if (!a || !(a->albedo_w || a->normal_w || a->nearest)) return TRB_OK;
         aov = a;
-        if (a->albedo_w) { CU(cudaMalloc(&albedo.p, npx * sizeof(float4))); CU(cudaMemsetAsync(albedo.p, 0, npx * sizeof(float4), 0)); }
-        if (a->normal_w) { CU(cudaMalloc(&normal.p, npx * sizeof(float4))); CU(cudaMemsetAsync(normal.p, 0, npx * sizeof(float4), 0)); }
-        if (a->nearest) { CU(cudaMalloc(&nearest.p, npx * sizeof(uint64_t))); CU(cudaMemcpy(nearest.p, a->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice)); }
-        req = {nullptr, static_cast<float4*>(albedo.p), static_cast<float4*>(normal.p), static_cast<unsigned long long*>(nearest.p)};
+        trb_status r;
+        for (auto [h, d] : {std::pair<const float*, DeviceBuffer*>{a->albedo_w, &albedo}, {a->normal_w, &normal}}) {
+            if (!h) continue;
+            if ((r = d->alloc(npx * sizeof(float4), "AOV films")) != TRB_OK) return r;
+            CU(cudaMemsetAsync(d->p, 0, npx * sizeof(float4), 0));
+        }
+        if (a->nearest) {
+            if ((r = nearest.alloc(npx * sizeof(uint64_t), "AOV films")) != TRB_OK) return r;
+            CU(cudaMemcpy(nearest.p, a->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice));
+        }
+        req = {nullptr, albedo.as<float4>(), normal.as<float4>(), nearest.as<unsigned long long>()};
         return TRB_OK;
     }
     const AovRequest* request() const { return aov ? &req : nullptr; }
@@ -2753,7 +2790,7 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, ha.request());
-    if (r != TRB_OK) return r;
+    if (r != TRB_OK) { if (ha.aov) cudaDeviceSynchronize(); return r; } // passes already enqueued still write the AOV films
     CU(cudaEventRecord(s->ev1, 0));
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, 0));
     CU(cudaStreamSynchronize(0));
@@ -2761,15 +2798,7 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     if (r != TRB_OK) return r;
     add_film(film, s->h_film_staging, npx * 4);
     if ((r = ha.unstage(npx)) != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-        stats->update_ms = update_ms;
-    }
-    return TRB_OK;
+    return stats_readback(s, stats, update_ms);
 }
 
 // trb_render_samples' body; aov: the host AOV records of trb_render_samples_aov (nullptr: none)
@@ -2783,40 +2812,15 @@ trb_status render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb
     if (r != TRB_OK) return r;
     if (n != (size_t)nb * 64 * count) return fail(TRB_INVALID_ARG, "sample buffer size must be blocks*64*sample_count");
     if (n == 0) return TRB_OK;
-    trb_sample* d_out = nullptr;
-    CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
-    DeviceBuffer d_aov;
-    if (aov) {
-        const cudaError_t e = cudaMalloc(&d_aov.p, n * sizeof(trb_aov_sample));
-        if (e != cudaSuccess) {
-            cudaFree(d_out);
-            cudaGetLastError();
-            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(e));
-        }
-    }
-    CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     trb::RenderParams rp{};
     rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
-    rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-    const AovRequest req{static_cast<trb_aov_sample*>(d_aov.p), nullptr, nullptr, nullptr};
-    CU(cudaEventRecord(s->ev0, 0));
-    r = launch_render(s, rp, cfg->flags, 1, 0, aov ? &req : nullptr);
-    if (r != TRB_OK) { cudaFree(d_out); return r; }
-    CU(cudaEventRecord(s->ev1, 0));
-    cudaError_t e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
-    cudaFree(d_out);
-    CU(e);
-    if (aov) CU(cudaMemcpy(aov, d_aov.p, n * sizeof(trb_aov_sample), cudaMemcpyDeviceToHost));
-    r = check_error_flag(s);
-    if (r != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-    }
-    return TRB_OK;
+    rp.work_counter = s->d_counter; rp.film = nullptr; rp.stats = s->d_stats; rp.error_flag = s->d_error;
+    r = run_counted(s, {}, {{samples, n * sizeof(trb_sample)}, {aov, n * sizeof(trb_aov_sample)}}, [&](const DeviceBuffer* d) {
+        rp.samples_out = d[0].as<trb_sample>();
+        const AovRequest req{d[1].as<trb_aov_sample>(), nullptr, nullptr, nullptr};
+        return launch_render(s, rp, cfg->flags, 1, 0, aov ? &req : nullptr);
+    });
+    return r != TRB_OK ? r : stats_readback(s, stats, 0.f);
 }
 } // namespace
 
@@ -2839,11 +2843,11 @@ trb_status trb_render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n,
 trb_status trb_render_aov_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, const trb_aov_film* d_aov, trb_stats* d_stats, void* stream) {
     if (!s || !cfg || !d_film || !d_aov) return fail(TRB_INVALID_ARG, "null argument");
     if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
-    const trb_status r = aov_supported(s, cfg);
+    trb_status r = aov_supported(s, cfg);
+    if (r == TRB_OK)
+        r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_aov->nearest, 8}},
+                          "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_film) | reinterpret_cast<uintptr_t>(d_aov->albedo_w) | reinterpret_cast<uintptr_t>(d_aov->normal_w)) & 15u) ||
-        (reinterpret_cast<uintptr_t>(d_aov->nearest) & 7u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
     const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
                          reinterpret_cast<unsigned long long*>(d_aov->nearest)};
     const bool with_aov = d_aov->albedo_w || d_aov->normal_w || d_aov->nearest;
@@ -2886,15 +2890,9 @@ trb_status denoise_check(const trb_scene* s, const trb_denoise_input* in, const 
     if (r != TRB_OK) return r;
     if (!s || !in || !out || !in->colour_a || !in->colour_b || !in->albedo_w || !in->normal_w || !in->nearest) return fail(TRB_INVALID_ARG, "null argument");
     prm.width = (int)s->film.width; prm.height = (int)s->film.height;
-    const size_t npx = (size_t)s->film.width * s->film.height;
-    const uintptr_t o0 = reinterpret_cast<uintptr_t>(out), o1 = o0 + npx * sizeof(float4);
-    const std::pair<const void*, size_t> ins[5] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
-                                                   {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
-                                                   {in->nearest, npx * sizeof(uint64_t)}};
-    for (const auto& [p, bytes] : ins) {
-        const uintptr_t a = reinterpret_cast<uintptr_t>(p);
-        if (a < o1 && o0 < a + bytes) return fail(TRB_INVALID_ARG, "the denoise output overlaps an input");
-    }
+    const size_t npx = (size_t)s->film.width * s->film.height, fb = npx * sizeof(float4);
+    if (overlaps_any({out, fb}, {{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}}))
+        return fail(TRB_INVALID_ARG, "the denoise output overlaps an input");
     return TRB_OK;
 }
 
@@ -2908,11 +2906,8 @@ trb_status denoise_scratch(trb_scene* s, size_t npx, trb::DnScratch& sc, float4*
             cudaFree(s->d_denoise);
         }
         s->d_denoise = nullptr; s->denoise_pixels = 0; s->denoise_moments = false;
-        const cudaError_t e = cudaMalloc(&s->d_denoise, mom ? mom_off + npx * sizeof(float4) : npx * trb::DN_BYTES_PER_PIXEL);
-        if (e != cudaSuccess) {
-            cudaGetLastError(); s->d_denoise = nullptr;
-            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("denoise scratch: ") + cudaGetErrorString(e));
-        }
+        const trb_status r = device_alloc(&s->d_denoise, mom ? mom_off + npx * sizeof(float4) : npx * trb::DN_BYTES_PER_PIXEL, "denoise scratch");
+        if (r != TRB_OK) return r;
         s->denoise_pixels = npx; s->denoise_moments = mom != nullptr;
     }
     float4* base = static_cast<float4*>(s->d_denoise);
@@ -2954,11 +2949,11 @@ trb_status denoise_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_den
 
 trb_status trb_denoise_device(trb_scene* s, const trb_denoise_input* d_in, const trb_denoise_params* params, float* d_out, void* stream) {
     trb::DnParams prm{};
-    const trb_status r = denoise_check(s, d_in, params, d_out, prm);
+    trb_status r = denoise_check(s, d_in, params, d_out, prm);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour_a, 16}, {d_in->colour_b, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_out, 16}, {d_in->nearest, 8}},
+                          "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
-          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out)) & 15u) || (reinterpret_cast<uintptr_t>(d_in->nearest) & 7u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
     CU(cudaSetDevice(s->device));
     return denoise_enqueue(s, prm, *d_in, d_out, static_cast<cudaStream_t>(stream));
 }
@@ -2969,19 +2964,11 @@ trb_status trb_denoise(trb_scene* s, const trb_denoise_input* in, const trb_deno
     if (r != TRB_OK) return r;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_out;
-    for (auto [d, h, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
-                               {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
-        CU(cudaMalloc(&d->p, bytes));
-        CU(cudaMemcpy(d->p, h, bytes, cudaMemcpyHostToDevice));
-    }
-    CU(cudaMalloc(&d_out.p, fb));
-    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
-                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
-    r = denoise_enqueue(s, prm, d_in, static_cast<float*>(d_out.p), 0);
-    if (r != TRB_OK) return r;
-    CU(cudaMemcpy(out, d_out.p, fb, cudaMemcpyDeviceToHost));
-    return TRB_OK;
+    return run_staged({{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}}, {{out, fb}},
+                      [&](const DeviceBuffer* d) {
+                          const trb_denoise_input d_in{d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<float>(), d[4].as<uint64_t>()};
+                          return denoise_enqueue(s, prm, d_in, d[5].as<float>(), 0);
+                      });
 }
 
 // ---- temporal denoising (include/trb.h "Temporal denoising", DESIGN.md §4) -------------------------------------------------------
@@ -3043,11 +3030,6 @@ trb_status trb_denoise_history_reset(trb_denoise_history* h) {
 }
 
 namespace {
-bool spans_overlap(const void* a, size_t abytes, const void* b, size_t bbytes) {
-    const uintptr_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
-    return a && b && a0 < b0 + bbytes && b0 < a0 + abytes;
-}
-
 // trb_denoise_temporal_params, NULL meaning the defaults; checked before anything else
 trb_status temporal_params(const trb_denoise_temporal_params* p, trb::DnParams& prm, trb::DnTemporal& tp) {
     const trb_status r = denoise_params(p ? &p->spatial : nullptr, prm);
@@ -3061,18 +3043,16 @@ trb_status temporal_params(const trb_denoise_temporal_params* p, trb::DnParams& 
     return TRB_OK;
 }
 
-using Span = std::pair<const void*, size_t>;
-
 // The checks shared by the half-film and moment calls after their parameters and null pointers: outputs outs[first..] overlapping an
 // input or an earlier output, the history's scene and film size, a frame
 trb_status history_call_check(const trb_scene* s, const trb_denoise_history* h, const Span* ins, size_t nin, const Span* outs, size_t nout,
                               size_t first) {
     for (size_t k = first; k < nout; ++k) {
         for (size_t j = 0; j < nin; ++j)
-            if (spans_overlap(outs[k].first, outs[k].second, ins[j].first, ins[j].second))
+            if (spans_overlap(outs[k], ins[j]))
                 return fail(TRB_INVALID_ARG, k == 0 ? "the denoise output overlaps an input" : "a temporal denoise output overlaps an input");
         for (size_t j = 0; j < k; ++j)
-            if (spans_overlap(outs[k].first, outs[k].second, outs[j].first, outs[j].second))
+            if (spans_overlap(outs[k], outs[j]))
                 return fail(TRB_INVALID_ARG, "two temporal denoise outputs overlap");
     }
     if (h->scene != s) return fail(TRB_INVALID_ARG, "the denoise history belongs to another scene");
@@ -3095,34 +3075,6 @@ trb_status temporal_check(const trb_scene* s, const trb_denoise_history* h, cons
                          {in->normal_w, npx * sizeof(float4)}, {in->nearest, npx * sizeof(uint64_t)}};
     const Span outs[3] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
     return history_call_check(s, h, ins, 5, outs, 3, 1); // denoise_check tested rgbw
-}
-
-// The host forms' staging: each span copied into a new device buffer (inputs), or a device buffer for each non-null span (outputs)
-trb_status stage_in(const Span* hs, size_t n, DeviceBuffer* d) {
-    for (size_t k = 0; k < n; ++k) {
-        CU(cudaMalloc(&d[k].p, hs[k].second));
-        CU(cudaMemcpy(d[k].p, hs[k].first, hs[k].second, cudaMemcpyHostToDevice));
-    }
-    return TRB_OK;
-}
-trb_status stage_out(const Span* hs, size_t n, DeviceBuffer* d) {
-    for (size_t k = 0; k < n; ++k)
-        if (hs[k].first) CU(cudaMalloc(&d[k].p, hs[k].second));
-    return TRB_OK;
-}
-// ... and the outputs copied back
-trb_status unstage_out(const Span* hs, size_t n, const DeviceBuffer* d) {
-    for (size_t k = 0; k < n; ++k)
-        if (hs[k].first) CU(cudaMemcpy(const_cast<void*>(hs[k].first), d[k].p, hs[k].second, cudaMemcpyDeviceToHost));
-    return TRB_OK;
-}
-
-// A device buffer of `bytes`; a failure is TRB_OOM (out of memory) or TRB_CUDA and leaves *p unset
-trb_status history_alloc(void** p, size_t bytes, const char* what) {
-    const cudaError_t e = cudaMalloc(p, bytes);
-    if (e == cudaSuccess) return TRB_OK;
-    cudaGetLastError(); *p = nullptr;
-    return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 
 // The gradient buffers of G strata, carved out of one allocation at 256-byte offsets: two record sets (64 B per stratum each), the
@@ -3248,14 +3200,14 @@ trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnPara
     // allocated before the old one is released, so a failure leaves the history as it was.
     if (h->px_capacity < npx) {
         void* p = nullptr;
-        r = history_alloc(&p, 2 * 3 * npx * sizeof(float4), "denoise history");
+        r = device_alloc(&p, 2 * 3 * npx * sizeof(float4), "denoise history");
         if (r != TRB_OK) return r;
         if (h->d_px) { CU(cudaDeviceSynchronize()); cudaFree(h->d_px); } // a call still in flight owns the old sets
         h->d_px = p; h->px_capacity = npx; h->has_prev = false;
     }
     if (h->mat_capacity < n) { // both snapshots, the read one copied to its place in the new buffer
         void* p = nullptr;
-        r = history_alloc(&p, 2 * n * 16 * sizeof(float), "denoise history snapshot");
+        r = device_alloc(&p, 2 * n * 16 * sizeof(float), "denoise history snapshot");
         if (r != TRB_OK) return r;
         if (h->d_mats) {
             CU(cudaDeviceSynchronize());
@@ -3270,7 +3222,7 @@ trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnPara
     const size_t S = (size_t)((prm.width + 2) / 3) * ((prm.height + 2) / 3);
     if (gc && h->gr_capacity < S) { // like the pixel sets: bound to one film size, so the records are not kept
         void* p = nullptr;
-        r = history_alloc(&p, gr_layout(S, nullptr, nullptr), "denoise history gradients");
+        r = device_alloc(&p, gr_layout(S, nullptr, nullptr), "denoise history gradients");
         if (r != TRB_OK) return r;
         if (h->d_gr) { CU(cudaDeviceSynchronize()); cudaFree(h->d_gr); }
         h->d_gr = p; h->gr_capacity = S; h->gr_valid = false;
@@ -3361,13 +3313,12 @@ trb_status trb_denoise_temporal_device(trb_scene* s, trb_denoise_history* h, con
                                        const trb_denoise_temporal_output* d_out, void* stream) {
     trb::DnParams prm{};
     trb::DnTemporal tp{};
-    const trb_status r = temporal_check(s, h, d_in, params, d_out, prm, tp);
+    trb_status r = temporal_check(s, h, d_in, params, d_out, prm, tp);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour_a, 16}, {d_in->colour_b, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8},
+                           {d_out->motion, 8}, {d_out->history_length, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length 4-byte");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
-          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
-        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
-        (reinterpret_cast<uintptr_t>(d_out->history_length) & 3u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length 4-byte");
     CU(cudaSetDevice(s->device));
     return temporal_enqueue(s, h, prm, tp, *d_in, *d_out, static_cast<cudaStream_t>(stream));
 }
@@ -3380,16 +3331,11 @@ trb_status trb_denoise_temporal(trb_scene* s, trb_denoise_history* h, const trb_
     if (r != TRB_OK) return r;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    const Span ins[5] = {{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
-    const Span outs[3] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
-    DeviceBuffer d_ins[5], d_outs[3];
-    if ((r = stage_in(ins, 5, d_ins)) != TRB_OK || (r = stage_out(outs, 3, d_outs)) != TRB_OK) return r;
-    const trb_denoise_input d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
-                                 static_cast<const float*>(d_ins[3].p), static_cast<const uint64_t*>(d_ins[4].p)};
-    const trb_denoise_temporal_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p)};
-    r = temporal_enqueue(s, h, prm, tp, d_in, d_out, 0);
-    if (r != TRB_OK) return r;
-    return unstage_out(outs, 3, d_outs);
+    return run_staged({{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}}, [&](const DeviceBuffer* d) {
+                          const trb_denoise_input d_in{d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<float>(), d[4].as<uint64_t>()};
+                          return temporal_enqueue(s, h, prm, tp, d_in, {d[5].as<float>(), d[6].as<float>(), d[7].as<uint32_t>()}, 0);
+                      });
 }
 
 namespace {
@@ -3404,15 +3350,11 @@ trb_status gradient_check(const trb_scene* s, const trb_denoise_history* h, cons
     const trb_denoise_temporal_output o{out->rgbw, out->motion, out->history_length};
     r = temporal_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp);
     if (r != TRB_OK) return r;
-    if (out->lambda) {
-        const size_t npx = (size_t)s->film.width * s->film.height;
-        const std::pair<const void*, size_t> others[8] = {{in->colour_a, npx * sizeof(float4)}, {in->colour_b, npx * sizeof(float4)},
-                                                          {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
-                                                          {in->nearest, npx * sizeof(uint64_t)}, {out->rgbw, npx * sizeof(float4)},
-                                                          {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}};
-        for (const auto& [p, bytes] : others)
-            if (spans_overlap(out->lambda, npx * sizeof(float), p, bytes)) return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
-    }
+    const size_t npx = (size_t)s->film.width * s->film.height, fb = npx * sizeof(float4);
+    if (overlaps_any({out->lambda, npx * sizeof(float)}, {{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb},
+                                                          {in->nearest, npx * sizeof(uint64_t)}, {out->rgbw, fb}, {out->motion, npx * sizeof(float2)},
+                                                          {out->history_length, npx * sizeof(uint32_t)}}))
+        return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
     gc.iterations = iterations;
     gc.lambda = out->lambda;
     return TRB_OK;
@@ -3425,13 +3367,12 @@ trb_status trb_denoise_temporal_gradient_device(trb_scene* s, trb_denoise_histor
     trb::DnParams prm{};
     trb::DnTemporal tp{};
     GradCall gc{};
-    const trb_status r = gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    trb_status r = gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour_a, 16}, {d_in->colour_b, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8},
+                           {d_out->motion, 8}, {d_out->history_length, 4}, {d_out->lambda, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and lambda 4-byte");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_in->colour_a) | reinterpret_cast<uintptr_t>(d_in->colour_b) | reinterpret_cast<uintptr_t>(d_in->albedo_w) |
-          reinterpret_cast<uintptr_t>(d_in->normal_w) | reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
-        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
-        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->lambda)) & 3u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and lambda 4-byte");
     gc.seed = seed;
     CU(cudaSetDevice(s->device));
     const trb_denoise_temporal_output o{d_out->rgbw, d_out->motion, d_out->history_length};
@@ -3448,27 +3389,13 @@ trb_status trb_denoise_temporal_gradient(trb_scene* s, trb_denoise_history* h, c
     gc.seed = seed;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    DeviceBuffer d_a, d_b, d_alb, d_nrm, d_near, d_rgbw, d_motion, d_len, d_lam;
-    for (auto [d, hp, bytes] : {std::tuple<DeviceBuffer*, const void*, size_t>{&d_a, in->colour_a, fb}, {&d_b, in->colour_b, fb}, {&d_alb, in->albedo_w, fb},
-                                {&d_nrm, in->normal_w, fb}, {&d_near, in->nearest, npx * sizeof(uint64_t)}}) {
-        CU(cudaMalloc(&d->p, bytes));
-        CU(cudaMemcpy(d->p, hp, bytes, cudaMemcpyHostToDevice));
-    }
-    CU(cudaMalloc(&d_rgbw.p, fb));
-    if (out->motion) CU(cudaMalloc(&d_motion.p, npx * sizeof(float2)));
-    if (out->history_length) CU(cudaMalloc(&d_len.p, npx * sizeof(uint32_t)));
-    if (out->lambda) CU(cudaMalloc(&d_lam.p, npx * sizeof(float)));
-    gc.lambda = static_cast<float*>(d_lam.p);
-    const trb_denoise_input d_in{static_cast<const float*>(d_a.p), static_cast<const float*>(d_b.p), static_cast<const float*>(d_alb.p),
-                                 static_cast<const float*>(d_nrm.p), static_cast<const uint64_t*>(d_near.p)};
-    const trb_denoise_temporal_output d_out{static_cast<float*>(d_rgbw.p), static_cast<float*>(d_motion.p), static_cast<uint32_t*>(d_len.p)};
-    r = temporal_enqueue(s, h, prm, tp, d_in, d_out, 0, &gc);
-    if (r != TRB_OK) { cudaDeviceSynchronize(); return r; }
-    CU(cudaMemcpy(out->rgbw, d_rgbw.p, fb, cudaMemcpyDeviceToHost));
-    if (out->motion) CU(cudaMemcpy(out->motion, d_motion.p, npx * sizeof(float2), cudaMemcpyDeviceToHost));
-    if (out->history_length) CU(cudaMemcpy(out->history_length, d_len.p, npx * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    if (out->lambda) CU(cudaMemcpy(out->lambda, d_lam.p, npx * sizeof(float), cudaMemcpyDeviceToHost));
-    return TRB_OK;
+    return run_staged({{in->colour_a, fb}, {in->colour_b, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}, {out->lambda, npx * sizeof(float)}},
+                      [&](const DeviceBuffer* d) {
+                          const trb_denoise_input d_in{d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<float>(), d[4].as<uint64_t>()};
+                          gc.lambda = d[8].as<float>();
+                          return temporal_enqueue(s, h, prm, tp, d_in, {d[5].as<float>(), d[6].as<float>(), d[7].as<uint32_t>()}, 0, &gc);
+                      });
 }
 
 // ---- moment denoising (include/trb.h "Moment denoising", DESIGN.md §4) -----------------------------------------------------------
@@ -3542,13 +3469,12 @@ trb_status trb_denoise_moments_device(trb_scene* s, trb_denoise_history* h, cons
                                       const trb_denoise_moments_output* d_out, void* stream) {
     trb::DnParams prm{};
     trb::DnTemporal tp{};
-    const trb_status r = moments_check(s, h, d_in, params, d_out, prm, tp);
+    trb_status r = moments_check(s, h, d_in, params, d_out, prm, tp);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8}, {d_out->motion, 8},
+                           {d_out->history_length, 4}, {d_out->variance, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and variance 4-byte");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_in->colour) | reinterpret_cast<uintptr_t>(d_in->albedo_w) | reinterpret_cast<uintptr_t>(d_in->normal_w) |
-          reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
-        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
-        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->variance)) & 3u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and variance 4-byte");
     CU(cudaSetDevice(s->device));
     return moments_enqueue(s, h, prm, tp, *d_in, *d_out, static_cast<cudaStream_t>(stream));
 }
@@ -3561,18 +3487,12 @@ trb_status trb_denoise_moments(trb_scene* s, trb_denoise_history* h, const trb_d
     if (r != TRB_OK) return r;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    const Span ins[4] = {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
-    const Span outs[4] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
-                          {out->variance, npx * sizeof(float)}};
-    DeviceBuffer d_ins[4], d_outs[4];
-    if ((r = stage_in(ins, 4, d_ins)) != TRB_OK || (r = stage_out(outs, 4, d_outs)) != TRB_OK) return r;
-    const trb_denoise_frame d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
-                                 static_cast<const uint64_t*>(d_ins[3].p)};
-    const trb_denoise_moments_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p),
-                                          static_cast<float*>(d_outs[3].p)};
-    r = moments_enqueue(s, h, prm, tp, d_in, d_out, 0);
-    if (r != TRB_OK) return r;
-    return unstage_out(outs, 4, d_outs);
+    return run_staged({{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)}},
+                      [&](const DeviceBuffer* d) {
+                          return moments_enqueue(s, h, prm, tp, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()},
+                                                 {d[4].as<float>(), d[5].as<float>(), d[6].as<uint32_t>(), d[7].as<float>()}, 0);
+                      });
 }
 
 // ---- moment gradients (include/trb.h "Moment gradients", DESIGN.md §4) -------------------------------------------------------------
@@ -3588,14 +3508,11 @@ trb_status moments_gradient_check(const trb_scene* s, const trb_denoise_history*
     const trb_denoise_moments_output o{out->rgbw, out->motion, out->history_length, out->variance};
     r = moments_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp);
     if (r != TRB_OK) return r;
-    if (out->lambda) {
-        const size_t npx = (size_t)s->film.width * s->film.height;
-        const Span others[8] = {{in->colour, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
-                                {in->nearest, npx * sizeof(uint64_t)}, {out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)},
-                                {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)}};
-        for (const auto& [p, bytes] : others)
-            if (spans_overlap(out->lambda, npx * sizeof(float), p, bytes)) return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
-    }
+    const size_t npx = (size_t)s->film.width * s->film.height, fb = npx * sizeof(float4);
+    if (overlaps_any({out->lambda, npx * sizeof(float)}, {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)},
+                                                          {out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
+                                                          {out->variance, npx * sizeof(float)}}))
+        return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
     gc.iterations = iterations;
     gc.lambda = out->lambda;
     return TRB_OK;
@@ -3607,14 +3524,12 @@ trb_status trb_denoise_moments_gradient_device(trb_scene* s, trb_denoise_history
     trb::DnParams prm{};
     trb::DnTemporal tp{};
     GradCall gc{};
-    const trb_status r = moments_gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    trb_status r = moments_gradient_check(s, h, d_in, params, d_out, prm, tp, gc);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8}, {d_out->motion, 8},
+                           {d_out->history_length, 4}, {d_out->variance, 4}, {d_out->lambda, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length, variance and lambda 4-byte");
     if (r != TRB_OK) return r;
-    if (((reinterpret_cast<uintptr_t>(d_in->colour) | reinterpret_cast<uintptr_t>(d_in->albedo_w) | reinterpret_cast<uintptr_t>(d_in->normal_w) |
-          reinterpret_cast<uintptr_t>(d_out->rgbw)) & 15u) ||
-        ((reinterpret_cast<uintptr_t>(d_in->nearest) | reinterpret_cast<uintptr_t>(d_out->motion)) & 7u) ||
-        ((reinterpret_cast<uintptr_t>(d_out->history_length) | reinterpret_cast<uintptr_t>(d_out->variance) |
-          reinterpret_cast<uintptr_t>(d_out->lambda)) & 3u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, nearest and motion 8-byte, history_length, variance and lambda 4-byte");
     gc.seed = seed;
     CU(cudaSetDevice(s->device));
     const trb_denoise_moments_output o{d_out->rgbw, d_out->motion, d_out->history_length, d_out->variance};
@@ -3631,19 +3546,14 @@ trb_status trb_denoise_moments_gradient(trb_scene* s, trb_denoise_history* h, co
     gc.seed = seed;
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
-    const Span ins[4] = {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}};
-    const Span outs[5] = {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
-                          {out->variance, npx * sizeof(float)}, {out->lambda, npx * sizeof(float)}};
-    DeviceBuffer d_ins[4], d_outs[5];
-    if ((r = stage_in(ins, 4, d_ins)) != TRB_OK || (r = stage_out(outs, 5, d_outs)) != TRB_OK) return r;
-    const trb_denoise_frame d_in{static_cast<const float*>(d_ins[0].p), static_cast<const float*>(d_ins[1].p), static_cast<const float*>(d_ins[2].p),
-                                 static_cast<const uint64_t*>(d_ins[3].p)};
-    const trb_denoise_moments_output d_out{static_cast<float*>(d_outs[0].p), static_cast<float*>(d_outs[1].p), static_cast<uint32_t*>(d_outs[2].p),
-                                          static_cast<float*>(d_outs[3].p)};
-    gc.lambda = static_cast<float*>(d_outs[4].p);
-    r = moments_enqueue(s, h, prm, tp, d_in, d_out, 0, &gc);
-    if (r != TRB_OK) { cudaDeviceSynchronize(); return r; }
-    return unstage_out(outs, 5, d_outs);
+    return run_staged({{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)},
+                       {out->lambda, npx * sizeof(float)}},
+                      [&](const DeviceBuffer* d) {
+                          gc.lambda = d[8].as<float>();
+                          return moments_enqueue(s, h, prm, tp, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()},
+                                                 {d[4].as<float>(), d[5].as<float>(), d[6].as<uint32_t>(), d[7].as<float>()}, 0, &gc);
+                      });
 }
 
 trb_status trb_adaptive_schedule(const trb_adaptive* ad, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step, uint32_t* max_per_pixel) {
@@ -3707,26 +3617,17 @@ trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const t
         trb::RenderParams rp{};
         rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = s->d_film; rp.stats = s->d_stats; rp.error_flag = s->d_error;
         r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr, ha.request());
-        if (r != TRB_OK) return r;
+        if (r != TRB_OK) { if (ha.aov) cudaDeviceSynchronize(); return r; } // passes already enqueued still write the AOV films
     }
     CU(cudaEventRecord(s->ev1, 0));
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, 0));
     CU(cudaStreamSynchronize(0));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
-    for (size_t i = 0; i < npx * 4; ++i) film[i] += s->h_film_staging[i]; // additive, like trb_render
+    add_film(film, s->h_film_staging, npx * 4);
     if ((r = ha.unstage(npx)) != TRB_OK) return r;
     r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
-    if (r != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-        stats->update_ms = update_ms;
-    }
-    return TRB_OK;
+    return r != TRB_OK ? r : stats_readback(s, stats, update_ms);
 }
 
 // trb_render_samples_adaptive's body; aov: the host AOV records of trb_render_samples_adaptive_aov (nullptr: none)
@@ -3745,44 +3646,17 @@ trb_status render_samples_adaptive(trb_scene* s, const trb_render_cfg* cfg, cons
     if (n == 0) return TRB_OK;
     r = ensure_adaptive(s);
     if (r != TRB_OK) return r;
-    trb_sample* d_out = nullptr;
-    CU(cudaMalloc(&d_out, n * sizeof(trb_sample)));
-    cudaError_t e = cudaMemsetAsync(d_out, 0, n * sizeof(trb_sample), 0); // unused slots stay zero
-    if (e != cudaSuccess) { cudaFree(d_out); CU(e); }
-    DeviceBuffer d_aov;
-    if (aov) {
-        e = cudaMalloc(&d_aov.p, n * sizeof(trb_aov_sample));
-        if (e == cudaSuccess) e = cudaMemsetAsync(d_aov.p, 0, n * sizeof(trb_aov_sample), 0); // as the samples: unused slots stay zero
-        if (e != cudaSuccess) {
-            cudaFree(d_out);
-            cudaGetLastError();
-            return fail(e == cudaErrorMemoryAllocation ? TRB_OOM : TRB_CUDA, std::string("AOV records: ") + cudaGetErrorString(e));
-        }
-    }
-    CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
-    CU(cudaEventRecord(s->ev0, 0));
     trb::RenderParams rp{};
-    rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = nullptr; rp.samples_out = d_out; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-    const AovRequest req{static_cast<trb_aov_sample*>(d_aov.p), nullptr, nullptr, nullptr};
-    r = render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr, aov ? &req : nullptr);
-    if (r != TRB_OK) { cudaDeviceSynchronize(); cudaFree(d_out); return r; }
-    CU(cudaEventRecord(s->ev1, 0));
-    e = cudaMemcpy(samples, d_out, n * sizeof(trb_sample), cudaMemcpyDeviceToHost);
-    cudaFree(d_out);
-    CU(e);
-    if (aov) CU(cudaMemcpy(aov, d_aov.p, n * sizeof(trb_aov_sample), cudaMemcpyDeviceToHost));
-    r = check_error_flag(s);
-    if (r != TRB_OK) return r;
-    r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
-    if (r != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-    }
-    return TRB_OK;
+    rp.seed = cfg->seed; rp.work_counter = s->d_counter; rp.film = nullptr; rp.stats = s->d_stats; rp.error_flag = s->d_error;
+    r = run_counted(s, {}, {{samples, n * sizeof(trb_sample)}, {aov, n * sizeof(trb_aov_sample)}}, [&](const DeviceBuffer* d) {
+        CU(cudaMemsetAsync(d[0].p, 0, n * sizeof(trb_sample), 0)); // unused slots stay zero
+        if (aov) CU(cudaMemsetAsync(d[1].p, 0, n * sizeof(trb_aov_sample), 0));
+        rp.samples_out = d[0].as<trb_sample>();
+        const AovRequest req{d[1].as<trb_aov_sample>(), nullptr, nullptr, nullptr};
+        return render_adaptive_rounds(s, sch, rp, d_blocks, nb, cfg->flags, 0, pixel_spp ? s->d_ad_spp : nullptr, aov ? &req : nullptr);
+    });
+    if (r == TRB_OK) r = adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
+    return r != TRB_OK ? r : stats_readback(s, stats, 0.f);
 }
 
 // trb_render_adaptive_device's body; aov: the device AOV outputs of trb_render_adaptive_aov_device (nullptr: none)
@@ -3832,9 +3706,9 @@ trb_status trb_render_adaptive_aov(trb_scene* s, const trb_render_cfg* cfg, cons
 trb_status trb_render_adaptive_aov_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, const trb_aov_film* d_aov,
                                           uint32_t* d_pixel_spp, trb_stats* d_stats, void* stream) {
     if (!s || !cfg || !ad || !d_film || !d_aov) return fail(TRB_INVALID_ARG, "null argument");
-    if (((reinterpret_cast<uintptr_t>(d_film) | reinterpret_cast<uintptr_t>(d_aov->albedo_w) | reinterpret_cast<uintptr_t>(d_aov->normal_w)) & 15u) ||
-        (reinterpret_cast<uintptr_t>(d_aov->nearest) & 7u))
-        return fail(TRB_INVALID_ARG, "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    const trb_status r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_aov->nearest, 8}},
+                                       "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    if (r != TRB_OK) return r;
     const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
                          reinterpret_cast<unsigned long long*>(d_aov->nearest)};
     const bool with_aov = d_aov->albedo_w || d_aov->normal_w || d_aov->nearest;
@@ -3859,20 +3733,15 @@ trb_status trb_camera_rays(trb_scene* s, const trb_render_cfg* cfg, size_t n, tr
     if (r != TRB_OK) return r;
     if (n != (size_t)nb * 64 * count) return fail(TRB_INVALID_ARG, "ray buffer size must be blocks*64*sample_count");
     if (n == 0) return TRB_OK;
-    trb_ray* d_rays = nullptr; float* d_xy = nullptr;
-    CU(cudaMalloc(&d_rays, n * sizeof(trb_ray)));
-    cudaError_t e = cudaMalloc(&d_xy, n * 2 * sizeof(float));
-    if (e != cudaSuccess) { cudaFree(d_rays); CU(e); }
     trb::RenderParams rp{};
     rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
-    if (s->ds.has_anim) trb::k_camera_rays<true><<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)s->sm_count * 8), 256>>>(s->ds, rp, d_rays, d_xy);
-    else trb::k_camera_rays<false><<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)s->sm_count * 8), 256>>>(s->ds, rp, d_rays, d_xy);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpy(rays, d_rays, n * sizeof(trb_ray), cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) e = cudaMemcpy(xy, d_xy, n * 2 * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(d_rays); cudaFree(d_xy);
-    CU(e);
-    return TRB_OK;
+    return run_staged({}, {{rays, n * sizeof(trb_ray)}, {xy, n * 2 * sizeof(float)}}, [&](const DeviceBuffer* d) {
+        const unsigned grid = (unsigned)std::min<size_t>((n + 255) / 256, (size_t)s->sm_count * 8);
+        if (s->ds.has_anim) trb::k_camera_rays<true><<<grid, 256>>>(s->ds, rp, d[0].as<trb_ray>(), d[1].as<float>());
+        else trb::k_camera_rays<false><<<grid, 256>>>(s->ds, rp, d[0].as<trb_ray>(), d[1].as<float>());
+        CU(cudaGetLastError());
+        return TRB_OK;
+    });
 }
 
 trb_status trb_intersect_device(trb_scene* s, size_t n, const trb_ray* d_rays, trb_hit* d_hits, trb_stats* d_stats, void* stream) {
@@ -3891,38 +3760,18 @@ trb_status trb_intersect(trb_scene* s, size_t n, const trb_ray* rays, trb_hit* h
     if (!s || (n && (!rays || !hits))) return fail(TRB_INVALID_ARG, "null argument");
     if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before intersecting");
     if (n == 0) return TRB_OK;
-    CU(cudaSetDevice(s->device));
-    trb_ray* d_rays = nullptr; trb_hit* d_hits = nullptr;
-    CU(cudaMalloc(&d_rays, n * sizeof(trb_ray)));
-    cudaError_t e = cudaMalloc(&d_hits, n * sizeof(trb_hit));
-    if (e != cudaSuccess) { cudaFree(d_rays); CU(e); }
-    e = cudaMemcpy(d_rays, rays, n * sizeof(trb_ray), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0);
-    if (e == cudaSuccess) {
-        cudaEventRecord(s->ev0, 0);
+    return run_query(s, n, {rays, n * sizeof(trb_ray)}, {hits, n * sizeof(trb_hit)}, stats, [&](void* d_rays, void* d_hits) {
         const unsigned grid = (unsigned)std::min<size_t>((n + 127) / 128, (size_t)s->sm_count * 16);
-        intersect_kernel<true>(s)<<<grid, 128>>>(s->ds, n, d_rays, d_hits, s->d_stats, s->d_error); // host variant always counts tests
-        cudaEventRecord(s->ev1, 0);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(hits, d_hits, n * sizeof(trb_hit), cudaMemcpyDeviceToHost);
-    cudaFree(d_rays); cudaFree(d_hits);
-    CU(e);
-    trb_status r = check_error_flag(s);
-    if (r != TRB_OK) return r;
-    if (stats) {
-        trb::DStats h;
-        CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-        std::memset(stats, 0, sizeof *stats);
-        stats_out(h, stats);
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-    }
-    return TRB_OK;
+        intersect_kernel<true>(s)<<<grid, 128>>>(s->ds, n, static_cast<const trb_ray*>(d_rays), static_cast<trb_hit*>(d_hits), s->d_stats,
+                                                 s->d_error); // host variant always counts tests
+        CU(cudaGetLastError());
+        return TRB_OK;
+    });
 }
 
 trb_status trb_intersect_records(trb_scene* s, size_t n, const trb_query_ray* rays, trb_intersection* out, uint32_t flags, trb_stats* stats) {
     const trb_status r = query_check(s, n, rays, out, flags, TRB_RENDER_STATS, false, false);
-    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_query_ray), out, n * sizeof(trb_intersection), stats, [&](const void* d_rays, void* d_out) {
+    return r != TRB_OK ? r : run_query(s, n, {rays, n * sizeof(trb_query_ray)}, {out, n * sizeof(trb_intersection)}, stats, [&](const void* d_rays, void* d_out) {
         return query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), static_cast<trb_intersection*>(d_out), nullptr, flags, s->d_stats, 0);
     });
 }
@@ -3937,7 +3786,7 @@ trb_status trb_intersect_records_device(trb_scene* s, size_t n, const trb_query_
 
 trb_status trb_occluded(trb_scene* s, size_t n, const trb_query_ray* rays, uint8_t* occluded, uint32_t flags, trb_stats* stats) {
     const trb_status r = query_check(s, n, rays, occluded, flags, TRB_RENDER_STATS | TRB_RENDER_REFERENCE_SHADOW, false, false);
-    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_query_ray), occluded, n, stats, [&](const void* d_rays, void* d_out) {
+    return r != TRB_OK ? r : run_query(s, n, {rays, n * sizeof(trb_query_ray)}, {occluded, n}, stats, [&](const void* d_rays, void* d_out) {
         return query_passes(s, n, static_cast<const trb_query_ray*>(d_rays), nullptr, static_cast<uint8_t*>(d_out), flags, s->d_stats, 0);
     });
 }
@@ -3952,7 +3801,7 @@ trb_status trb_occluded_device(trb_scene* s, size_t n, const trb_query_ray* d_ra
 
 trb_status trb_illumination(trb_scene* s, size_t n, const trb_illum_ray* rays, uint32_t spp, uint32_t seed, float* rgb, uint32_t flags, trb_stats* stats) {
     const trb_status r = illum_check(s, n, rays, spp, rgb, flags, false);
-    return r != TRB_OK ? r : query_host(s, n, rays, n * sizeof(trb_illum_ray), rgb, n * 3 * sizeof(float), stats, [&](const void* d_rays, void* d_rgb) {
+    return r != TRB_OK ? r : run_query(s, n, {rays, n * sizeof(trb_illum_ray)}, {rgb, n * 3 * sizeof(float)}, stats, [&](const void* d_rays, void* d_rgb) {
         return illum_passes(s, n, static_cast<const trb_illum_ray*>(d_rays), spp, seed, static_cast<float*>(d_rgb), flags, s->d_stats, 0);
     });
 }
@@ -3967,8 +3816,10 @@ trb_status trb_illumination_device(trb_scene* s, size_t n, const trb_illum_ray* 
 
 trb_status trb_bsdf_eval(trb_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_eval_query* q, float* out4) {
     const trb_status r = shade_check(s, n, rec, q, out4, 16, false, false);
-    return r != TRB_OK ? r : shade_host(s, n, rec, n * sizeof *rec, q, n * sizeof *q, out4, n * 4 * sizeof(float), [&](void* a, void* b, void* o) {
-        return launch_bsdf_eval(s, n, static_cast<const trb_intersection*>(a), static_cast<const trb_bsdf_eval_query*>(b), static_cast<float*>(o), 0);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return run_staged({{rec, n * sizeof *rec}, {q, n * sizeof *q}}, {{out4, n * 4 * sizeof(float)}}, [&](const DeviceBuffer* d) {
+        return launch_bsdf_eval(s, n, d[0].as<trb_intersection>(), d[1].as<trb_bsdf_eval_query>(), d[2].as<float>(), 0);
     });
 }
 
@@ -3981,8 +3832,10 @@ trb_status trb_bsdf_eval_device(trb_scene* s, size_t n, const trb_intersection* 
 
 trb_status trb_bsdf_sample(trb_scene* s, size_t n, const trb_intersection* rec, const trb_bsdf_sample_query* q, trb_bsdf_sample_result* out) {
     const trb_status r = shade_check(s, n, rec, q, out, 16, false, false);
-    return r != TRB_OK ? r : shade_host(s, n, rec, n * sizeof *rec, q, n * sizeof *q, out, n * sizeof *out, [&](void* a, void* b, void* o) {
-        return launch_bsdf_sample(s, n, static_cast<const trb_intersection*>(a), static_cast<const trb_bsdf_sample_query*>(b), static_cast<trb_bsdf_sample_result*>(o), 0);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return run_staged({{rec, n * sizeof *rec}, {q, n * sizeof *q}}, {{out, n * sizeof *out}}, [&](const DeviceBuffer* d) {
+        return launch_bsdf_sample(s, n, d[0].as<trb_intersection>(), d[1].as<trb_bsdf_sample_query>(), d[2].as<trb_bsdf_sample_result>(), 0);
     });
 }
 
@@ -3996,8 +3849,10 @@ trb_status trb_bsdf_sample_device(trb_scene* s, size_t n, const trb_intersection
 
 trb_status trb_light_sample(trb_scene* s, size_t n, const trb_light_query* q, trb_light_sample_result* out) {
     const trb_status r = shade_check(s, n, q, q, out, 16, false, true);
-    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, out, n * sizeof *out, [&](void* a, void*, void* o) {
-        return launch_light_sample(s, n, static_cast<const trb_light_query*>(a), static_cast<trb_light_sample_result*>(o), 0);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return run_staged({{q, n * sizeof *q}}, {{out, n * sizeof *out}}, [&](const DeviceBuffer* d) {
+        return launch_light_sample(s, n, d[0].as<trb_light_query>(), d[1].as<trb_light_sample_result>(), 0);
     });
 }
 
@@ -4010,8 +3865,10 @@ trb_status trb_light_sample_device(trb_scene* s, size_t n, const trb_light_query
 
 trb_status trb_light_pdf(trb_scene* s, size_t n, const trb_light_pdf_query* q, float* pdf) {
     const trb_status r = shade_check(s, n, q, q, pdf, 4, false, true);
-    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, pdf, n * sizeof(float), [&](void* a, void*, void* o) {
-        return launch_light_pdf(s, n, static_cast<const trb_light_pdf_query*>(a), static_cast<float*>(o), 0);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return run_staged({{q, n * sizeof *q}}, {{pdf, n * sizeof(float)}}, [&](const DeviceBuffer* d) {
+        return launch_light_pdf(s, n, d[0].as<trb_light_pdf_query>(), d[1].as<float>(), 0);
     });
 }
 
@@ -4024,8 +3881,10 @@ trb_status trb_light_pdf_device(trb_scene* s, size_t n, const trb_light_pdf_quer
 
 trb_status trb_emitted(trb_scene* s, size_t n, const trb_emit_query* q, float* rgb) {
     const trb_status r = shade_check(s, n, q, q, rgb, 4, false, false);
-    return r != TRB_OK ? r : shade_host(s, n, q, n * sizeof *q, nullptr, 0, rgb, n * 3 * sizeof(float), [&](void* a, void*, void* o) {
-        return launch_emitted(s, n, static_cast<const trb_emit_query*>(a), static_cast<float*>(o), 0);
+    if (r != TRB_OK || n == 0) return r;
+    CU(cudaSetDevice(s->device));
+    return run_staged({{q, n * sizeof *q}}, {{rgb, n * 3 * sizeof(float)}}, [&](const DeviceBuffer* d) {
+        return launch_emitted(s, n, d[0].as<trb_emit_query>(), d[1].as<float>(), 0);
     });
 }
 
@@ -4048,22 +3907,10 @@ trb_status trb_film_write(trb_scene* s, size_t n, const trb_sample* samples, con
     if (r != TRB_OK || n == 0) return r;
     CU(cudaSetDevice(s->device));
     const size_t film_bytes = (size_t)s->film.width * s->film.height * 4 * sizeof(float);
-    const size_t r_off = (n * sizeof(trb_sample) + 255) / 256 * 256, f_off = r_off + (n * sizeof(uint32_t) + 255) / 256 * 256;
-    char* d = nullptr;
-    CU(cudaMalloc(&d, f_off + film_bytes));
-    cudaError_t e = cudaMemcpy(d, samples, n * sizeof(trb_sample), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d + r_off, regions, n * sizeof(uint32_t), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d + f_off, film_rgbw, film_bytes, cudaMemcpyHostToDevice);
-    trb_status st = TRB_OK;
-    if (e == cudaSuccess)
-        st = film_write_enqueue(s, (uint32_t)n, reinterpret_cast<const trb_sample*>(d), reinterpret_cast<const uint32_t*>(d + r_off),
-                                reinterpret_cast<float*>(d + f_off), 0);
-    if (e == cudaSuccess && st == TRB_OK) e = cudaMemcpy(film_rgbw, d + f_off, film_bytes, cudaMemcpyDeviceToHost);
-    if (st != TRB_OK) cudaDeviceSynchronize();
-    cudaFree(d);
-    if (st != TRB_OK) return st;
-    CU(e);
-    return TRB_OK;
+    return run_staged({{samples, n * sizeof(trb_sample)}, {regions, n * sizeof(uint32_t)}}, {{film_rgbw, film_bytes}}, [&](const DeviceBuffer* d) {
+        CU(cudaMemcpy(d[2].p, film_rgbw, film_bytes, cudaMemcpyHostToDevice)); // the samples are added to the caller's film
+        return film_write_enqueue(s, (uint32_t)n, d[0].as<trb_sample>(), d[1].as<uint32_t>(), d[2].as<float>(), 0);
+    });
 }
 
 trb_status trb_film_write_device(trb_scene* s, size_t n, const trb_sample* d_samples, const uint32_t* d_regions, float* d_film_rgbw, void* stream) {
@@ -4075,7 +3922,7 @@ trb_status trb_film_write_device(trb_scene* s, size_t n, const trb_sample* d_sam
 
 trb_status trb_camera_rays_device(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_ray* d_rays, float* d_xy, void* stream) {
     if (!s || !cfg || (n && (!d_rays || !d_xy))) return fail(TRB_INVALID_ARG, "null argument");
-    if (((reinterpret_cast<uintptr_t>(d_rays) | reinterpret_cast<uintptr_t>(d_xy)) & 3u)) return fail(TRB_INVALID_ARG, "device ray buffers must be 4-byte aligned");
+    { const trb_status r = check_aligned({{d_rays, 4}, {d_xy, 4}}, "device ray buffers must be 4-byte aligned"); if (r != TRB_OK) return r; }
     if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
     CU(cudaSetDevice(s->device));
     return camera_rays_enqueue(s, cfg, n, d_rays, d_xy, static_cast<cudaStream_t>(stream));
@@ -4085,17 +3932,12 @@ trb_status trb_film_to_srgb8(trb_scene* s, const float* film, uint8_t* rgb8) {
     if (!s || !film || !rgb8) return fail(TRB_INVALID_ARG, "null argument");
     CU(cudaSetDevice(s->device));
     const size_t npx = (size_t)s->film.width * s->film.height;
-    uint8_t* d_out = nullptr;
-    CU(cudaMalloc(&d_out, npx * 3));
-    cudaError_t e = cudaMemcpy(s->d_film, film, npx * sizeof(float4), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        trb::k_srgb8<<<(unsigned)std::min<size_t>((npx + 255) / 256, (size_t)s->sm_count * 16), 256>>>(npx, s->d_film, d_out);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpy(rgb8, d_out, npx * 3, cudaMemcpyDeviceToHost);
-    cudaFree(d_out);
-    CU(e);
-    return TRB_OK;
+    return run_staged({}, {{rgb8, npx * 3}}, [&](const DeviceBuffer* d) {
+        CU(cudaMemcpy(s->d_film, film, npx * sizeof(float4), cudaMemcpyHostToDevice)); // the input goes through the scene's device film
+        trb::k_srgb8<<<(unsigned)std::min<size_t>((npx + 255) / 256, (size_t)s->sm_count * 16), 256>>>(npx, s->d_film, d[0].as<uint8_t>());
+        CU(cudaGetLastError());
+        return TRB_OK;
+    });
 }
 
 trb_status trb_host_film_to_srgb8(uint32_t width, uint32_t height, const float* film, uint8_t* rgb8) {
@@ -4198,25 +4040,20 @@ trb_status trb_build_bvh(int device, const float* boxes6, uint32_t n, uint32_t m
     if (!boxes6 || n == 0 || !n_nodes) return fail(TRB_INVALID_ARG, "empty geometry"); // bvh.rs:35 assert!(!geometry.is_empty())
     const trb_status c = bvh_device_check(device, n);
     if (c != TRB_OK) return c;
-    float* d_boxes = nullptr;
-    uint32_t* d_order = nullptr; // + one word: the node count
-    trb_bvh_node* d_nodes = nullptr;
-    auto run = [&]() -> trb_status {
-        CU(cudaMalloc(&d_boxes, 24 * (size_t)n));
-        CU(cudaMalloc(&d_order, 4 * ((size_t)n + 1)));
-        CU(cudaMalloc(&d_nodes, (2 * (size_t)n - 1) * sizeof(trb_bvh_node)));
-        CU(cudaMemcpy(d_boxes, boxes6, 24 * (size_t)n, cudaMemcpyHostToDevice));
+    DeviceBuffer order, tree; // order: + one word, the node count; both outlive run_staged's drain
+    return run_staged({{boxes6, 24 * (size_t)n}}, {}, [&](const DeviceBuffer* d) {
+        trb_status r;
+        if ((r = order.alloc(4 * ((size_t)n + 1), "BVH build scratch")) != TRB_OK || (r = tree.alloc((2 * (size_t)n - 1) * sizeof(trb_bvh_node), "BVH build scratch")) != TRB_OK)
+            return r;
+        uint32_t* d_order = order.as<uint32_t>();
         bool empty = false;
-        CU(trb::bvhb::build_device(d_boxes, n, max_geom, d_order + n, d_nodes, d_order, 0, &g_launches, &empty));
+        CU(trb::bvhb::build_device(d[0].as<float>(), n, max_geom, d_order + n, tree.as<trb_bvh_node>(), d_order, 0, &g_launches, &empty));
         if (empty) return fail(TRB_INVALID_ARG, "the SAH build would split a node into an empty child (infinite coordinates)");
         CU(cudaMemcpy(n_nodes, d_order + n, 4, cudaMemcpyDeviceToHost));
-        if (nodes) CU(cudaMemcpy(nodes, d_nodes, (size_t)*n_nodes * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
+        if (nodes) CU(cudaMemcpy(nodes, tree.p, (size_t)*n_nodes * sizeof(trb_bvh_node), cudaMemcpyDeviceToHost));
         if (ordered) CU(cudaMemcpy(ordered, d_order, 4 * (size_t)n, cudaMemcpyDeviceToHost));
         return TRB_OK;
-    };
-    const trb_status r = run();
-    cudaFree(d_boxes); cudaFree(d_order); cudaFree(d_nodes);
-    return r;
+    });
 }
 
 trb_status trb_host_keyframe_transform(const trb_keyframe* kf, float* mat16, float* inv16) {
@@ -4234,17 +4071,12 @@ trb_status trb_selftest_box(uint32_t n_cases, uint32_t seed, uint64_t out[4]) {
     if (!out || n_cases == 0) return fail(TRB_INVALID_ARG, "null argument");
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) { cudaGetLastError(); return fail(TRB_NO_DEVICE, "no CUDA device"); }
-    unsigned long long* d = nullptr;
-    CU(cudaMalloc(&d, 4 * sizeof(unsigned long long)));
-    cudaMemset(d, 0, 4 * sizeof(unsigned long long));
-    trb::k_selftest_box<<<(n_cases + 255) / 256, 256>>>(n_cases, seed, d);
-    g_launches++;
-    unsigned long long h[4] = {0, 0, 0, 0};
-    const cudaError_t e = cudaMemcpy(h, d, sizeof h, cudaMemcpyDeviceToHost);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(TRB_CUDA, cudaGetErrorString(e));
-    for (int k = 0; k < 4; ++k) out[k] = h[k];
-    return TRB_OK;
+    return run_staged({}, {{out, 4 * sizeof(uint64_t)}}, [&](const DeviceBuffer* d) {
+        CU(cudaMemset(d[0].p, 0, 4 * sizeof(unsigned long long)));
+        trb::k_selftest_box<<<(n_cases + 255) / 256, 256>>>(n_cases, seed, d[0].as<unsigned long long>());
+        g_launches++;
+        return TRB_OK;
+    });
 }
 
 trb_status trb_host_quad_check(const trb_bvh_node* nodes, uint32_t n_nodes, const trb_ray* rays, uint32_t n_rays, uint32_t* mismatches,
@@ -4441,29 +4273,11 @@ trb_status shard_pixel_spp_out(trb_scene* s, const trb_render_cfg* mine, bool em
     if (r != TRB_OK) return r;
     return adaptive_pixel_spp_out(s, d_blocks, nb, pixel_spp);
 }
-trb_status film_to_host_add(trb_scene* s, float* film, cudaStream_t st) { // additive, like film::Image::add_pixels (image.rs:21-33)
+trb_status film_to_host_add(trb_scene* s, float* film, cudaStream_t st) {
     const size_t npx = (size_t)s->film.width * s->film.height;
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const float* src = s->h_film_staging;
-    const size_t n = npx * 4;
-    const unsigned nt = n >= (1u << 20) ? std::min(8u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
-    auto add = [film, src](size_t a, size_t b) { for (size_t i = a; i < b; ++i) film[i] += src[i]; };
-    std::vector<std::thread> th;
-    for (unsigned k = 1; k < nt; ++k) th.emplace_back(add, n * k / nt, n * (k + 1) / nt);
-    add(0, n / nt);
-    for (auto& t : th) t.join();
-    return TRB_OK;
-}
-trb_status stats_to_host(trb_scene* s, trb_stats* stats, bool accumulate) {
-    trb::DStats h;
-    CU(cudaSetDevice(s->device));
-    CU(cudaMemcpy(&h, s->d_stats, sizeof h, cudaMemcpyDeviceToHost));
-    trb_stats one; std::memset(&one, 0, sizeof one);
-    stats_out(h, &one);
-    if (!accumulate) { *stats = one; return TRB_OK; }
-    stats->camera_samples += one.camera_samples; stats->rays_primary += one.rays_primary; stats->rays_shadow += one.rays_shadow; stats->rays_mis += one.rays_mis;
-    stats->rays_continuation += one.rays_continuation; stats->node_tests += one.node_tests; stats->tri_tests += one.tri_tests; stats->inst_tests += one.inst_tests;
+    add_film(film, s->h_film_staging, npx * 4);
     return TRB_OK;
 }
 } // namespace
@@ -4550,12 +4364,8 @@ trb_status render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, 
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
     if (ad) { r = shard_pixel_spp_out(s, &mine, empty, pixel_spp); if (r != TRB_OK) return r; }
-    if (stats) {
-        r = stats_to_host(s, stats, false);
-        if (r != TRB_OK) return r;
-        CU(cudaEventElapsedTime(&stats->kernel_ms, s->ev0, s->ev1));
-        stats->update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count() - stats->kernel_ms;
-    }
+    if ((r = stats_readback(s, stats, 0.f)) != TRB_OK) return r;
+    if (stats) stats->update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count() - stats->kernel_ms;
     return TRB_OK;
 }
 } // namespace
@@ -4670,11 +4480,11 @@ trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adapt
         if (r != TRB_OK) return r;
         if (ad) { r = shard_pixel_spp_out(g->scenes[i], &mine[i], empty[i] != 0, pixel_spp); if (r != TRB_OK) return r; } // the replicas' pixels are disjoint
         if (stats) {
-            r = stats_to_host(g->scenes[i], stats, true);
-            if (r != TRB_OK) return r;
-            float ms = 0.f;
-            CU(cudaEventElapsedTime(&ms, g->scenes[i]->ev0, g->scenes[i]->ev1));
-            kernel_ms = std::max(kernel_ms, ms);
+            trb_stats one;
+            if ((r = stats_readback(g->scenes[i], &one, 0.f)) != TRB_OK) return r;
+            stats->camera_samples += one.camera_samples; stats->rays_primary += one.rays_primary; stats->rays_shadow += one.rays_shadow; stats->rays_mis += one.rays_mis;
+            stats->rays_continuation += one.rays_continuation; stats->node_tests += one.node_tests; stats->tri_tests += one.tri_tests; stats->inst_tests += one.inst_tests;
+            kernel_ms = std::max(kernel_ms, one.kernel_ms);
         }
     }
     if (stats) { stats->kernel_ms = kernel_ms; stats->update_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count() - kernel_ms; }
