@@ -1233,6 +1233,25 @@ trb_status trb_render_sharded_adaptive(trb_scene* scene, trb_comm* comm, const t
 trb_status trb_group_render_adaptive(trb_group* group, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
                                      uint32_t* pixel_spp, trb_stats* stats);
 
+/* -- AOVs of multi-GPU renders (DESIGN.md §4 "Multi-GPU AOVs") ----------------------------------------------------------
+ * trb_render_sharded, trb_render_sharded_adaptive, trb_group_render and trb_group_render_adaptive that also render the AOVs
+ * (trb_aov_film). Every rank or replica renders albedo_w, normal_w and nearest of its own shard into device films the scene owns
+ * (allocated by the first such render, 40 B per pixel, released with the film), and ONE NCCL group per frame reduces the colour film
+ * and the three AOVs to the root: the films summed, nearest min-reduced (exact: the shards own disjoint pixels). The root (the
+ * group: the caller) then holds what trb_render_aov / trb_render_adaptive_aov give on one GPU: film_rgbw, albedo_w and normal_w
+ * added into, nearest read and min-merged, a NULL member of `aov` skipped; the sums equal one-GPU output up to float addition order,
+ * nearest and pixel_spp exactly. On a sharded call the non-root ranks may pass film_rgbw and aov as NULL. A one-rank communicator
+ * performs no reduce, and a group of one device calls trb_render_aov / trb_render_adaptive_aov on its replica.
+ * Every check that depends only on arguments all ranks share (null arguments, trb_render_aov's and trb_render_adaptive's statuses,
+ * the group's film sizes) fails on every rank before any rank renders, so no rank is left waiting in the reduce. Blocking. */
+trb_status trb_render_sharded_aov(trb_scene* scene, trb_comm* comm, const trb_render_cfg* cfg, int root, float* film_rgbw,
+                                  const trb_aov_film* aov, trb_stats* stats);
+trb_status trb_render_sharded_adaptive_aov(trb_scene* scene, trb_comm* comm, const trb_render_cfg* cfg, const trb_adaptive* adaptive, int root,
+                                           float* film_rgbw, const trb_aov_film* aov, uint32_t* pixel_spp, trb_stats* stats);
+trb_status trb_group_render_aov(trb_group* group, const trb_render_cfg* cfg, float* film_rgbw, const trb_aov_film* aov, trb_stats* stats);
+trb_status trb_group_render_adaptive_aov(trb_group* group, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                                         const trb_aov_film* aov, uint32_t* pixel_spp, trb_stats* stats);
+
 /* The rounded schedule of Adaptive::new (adaptive.rs:34-49); any output may be NULL. Host only. */
 trb_status trb_adaptive_schedule(const trb_adaptive* adaptive, uint32_t* min_spp, uint32_t* max_spp, uint32_t* step,
                                  uint32_t* max_per_pixel);

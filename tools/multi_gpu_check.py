@@ -4,7 +4,10 @@
 Checks trb_render_sharded (interleaved and reference-style contiguous sharding, ONE ncclReduce per frame issued by libtrb) and
 trb_group_render against the single-GPU render of the same frame: same ray counts, film equal up to float addition order. The
 Adaptive cases (trb_render_sharded_adaptive, trb_group_render_adaptive) check the same against trb_render_adaptive on one GPU,
-and that every pixel's sample count is equal."""
+and that every pixel's sample count is equal. The AOV cases (trb_render_sharded_aov, trb_render_sharded_adaptive_aov,
+trb_group_render_aov, trb_group_render_adaptive_aov) check the albedo and normal films the same way and nearest exactly, and the
+denoise cases check a group's render_denoised and render_denoised_moments (denoised on replica 0) against one GPU's, within the
+tolerance tests/test_multi_gpu_aov_gpu.py states."""
 import json
 import os
 import sys
@@ -27,6 +30,37 @@ def img(f):
     return f[..., :3] / np.maximum(f[..., 3:], 1e-6)
 
 
+def aovs_close(a, b):
+    """the AOV films up to float addition order, nearest exactly"""
+    return (np.allclose(a["albedo_w"], b["albedo_w"], rtol=2e-4, atol=2e-5) and np.allclose(a["normal_w"], b["normal_w"], rtol=2e-4, atol=2e-5)
+            and a["nearest"].tobytes() == b["nearest"].tobytes())
+
+
+def group_aov_cases(g1, grp, n):
+    ok = True
+    ref, aref, st1 = g1.render_aov(spp=SPP, seed=3)
+    film, aovs, st = grp.render_aov(spp=SPP, seed=3)
+    good = st.rays_total() == st1.rays_total() and np.allclose(film, ref, rtol=2e-4, atol=2e-5) and aovs_close(aovs, aref)
+    print(json.dumps({"mode": "trb_group_render_aov", "devices": n, "rays": st.rays_total(), "rays_single": st1.rays_total(),
+                      "nearest_differs": int((aovs["nearest"] != aref["nearest"]).sum()), "ok": bool(good)}))
+    ok = ok and good
+    ref, aref, spp1, st1 = g1.render_adaptive_aov(*AD, seed=3)
+    film, aovs, spp, st = grp.render_adaptive_aov(*AD, seed=3)
+    good = (st.rays_total() == st1.rays_total() and bool((spp == spp1).all()) and np.allclose(film, ref, rtol=2e-4, atol=2e-5)
+            and aovs_close(aovs, aref))
+    print(json.dumps({"mode": "trb_group_render_adaptive_aov", "devices": n, "adaptive": AD, "pixels_with_other_count": int((spp != spp1).sum()),
+                      "nearest_differs": int((aovs["nearest"] != aref["nearest"]).sum()), "ok": bool(good)}))
+    ok = ok and good
+    for name, call in (("render_denoised", lambda r, h: r.render_denoised(SPP, seed=3)),
+                       ("render_denoised_moments", lambda r, h: r.render_denoised_moments(h, 1, seed=3))):
+        want = call(g1, api.DenoiseHistory(g1))[0]
+        got = call(grp, api.DenoiseHistory(grp.scene(0)))[0]
+        good = bool(np.allclose(got, want, rtol=1e-4, atol=1e-5))
+        print(json.dumps({"mode": "Group." + name, "devices": n, "max_abs_diff": float(np.abs(got - want).max()), "ok": good}))
+        ok = ok and good
+    return ok
+
+
 def group_mode(n):
     g1 = api.Scene(desc(), 0)
     ref, st1 = g1.render(spp=SPP, seed=3)
@@ -42,7 +76,7 @@ def group_mode(n):
     print(json.dumps({"mode": "trb_group_render_adaptive", "devices": n, "adaptive": AD, "rays": ast.rays_total(), "rays_single": ast1.rays_total(),
                       "pixels_with_other_count": int((aspp != aspp1).sum()), "rmse": float(np.sqrt(np.mean((img(afilm) - img(aref)) ** 2))),
                       "kernel_ms": ast.kernel_ms, "kernel_ms_single": ast1.kernel_ms, "ok": bool(aok)}))
-    return ok and aok
+    return ok and aok and group_aov_cases(g1, grp, n)
 
 
 def rank_mode():
@@ -78,6 +112,25 @@ def rank_mode():
             print(json.dumps({"mode": "trb_render_sharded_adaptive " + name, "ranks": world, "adaptive": AD, "rays": int(t[1:].sum()),
                               "rays_single": st1.rays_total(), "pixels_with_other_count": int((counts.numpy() != spp1).sum()),
                               "rmse": float(np.sqrt(np.mean((img(film) - img(ref)) ** 2))), "ok": bool(good)}))
+            ok = ok and good
+    for name, kw in (("interleaved", {}), ("contiguous (master.rs:91-93)", dict(shard_count=0xffffffff))):
+        film, aovs, st = comm.render_sharded_aov(g, None, root=0, spp=SPP, seed=3, **kw)  # non-root ranks pass no buffers
+        t = torch.tensor([st.rays_total()], dtype=torch.int64)
+        dist.all_reduce(t)
+        if rank == 0:
+            ref, aref, st1 = g.render_aov(spp=SPP, seed=3)
+            good = int(t[0]) == st1.rays_total() and np.allclose(film, ref, rtol=2e-4, atol=2e-5) and aovs_close(aovs, aref)
+            print(json.dumps({"mode": "trb_render_sharded_aov " + name, "ranks": world, "nearest_differs": int((aovs["nearest"] != aref["nearest"]).sum()),
+                              "ok": bool(good)}))
+            ok = ok and good
+        film, aovs, spp, st = comm.render_sharded_adaptive_aov(g, *AD, None, root=0, seed=3, **kw)
+        counts = torch.from_numpy(spp.astype(np.int64))
+        dist.all_reduce(counts)
+        if rank == 0:
+            ref, aref, spp1, st1 = g.render_adaptive_aov(*AD, seed=3)
+            good = bool((counts.numpy() == spp1).all()) and np.allclose(film, ref, rtol=2e-4, atol=2e-5) and aovs_close(aovs, aref)
+            print(json.dumps({"mode": "trb_render_sharded_adaptive_aov " + name, "ranks": world, "adaptive": AD,
+                              "pixels_with_other_count": int((counts.numpy() != spp1).sum()), "ok": bool(good)}))
             ok = ok and good
     dist.barrier()
     comm.close()

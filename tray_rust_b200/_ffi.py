@@ -323,6 +323,7 @@ TRB_SYMBOLS = [
     "trb_denoise_temporal_device", "trb_denoise_temporal_gradient", "trb_denoise_temporal_gradient_device",
     "trb_denoise_moments", "trb_denoise_moments_device", "trb_denoise_moments_gradient", "trb_denoise_moments_gradient_device",
     "trb_render_adaptive_aov", "trb_render_adaptive_aov_device", "trb_render_samples_adaptive_aov",
+    "trb_render_sharded_aov", "trb_render_sharded_adaptive_aov", "trb_group_render_aov", "trb_group_render_adaptive_aov",
 ]
 
 _trb = None
@@ -455,6 +456,11 @@ def load_trb():
     lib.trb_group_render.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(Stats)]
     lib.trb_render_sharded_adaptive.argtypes = [vp, vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), C.c_int, vp, vp, C.POINTER(Stats)]
     lib.trb_group_render_adaptive.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, vp, C.POINTER(Stats)]
+    lib.trb_render_sharded_aov.argtypes = [vp, vp, C.POINTER(RenderCfg), C.c_int, vp, C.POINTER(AovFilm), C.POINTER(Stats)]
+    lib.trb_render_sharded_adaptive_aov.argtypes = [vp, vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), C.c_int, vp, C.POINTER(AovFilm), vp,
+                                                    C.POINTER(Stats)]
+    lib.trb_group_render_aov.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), C.POINTER(Stats)]
+    lib.trb_group_render_adaptive_aov.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, C.POINTER(Stats)]
     lib.trb_group_scene.argtypes = [vp, C.c_int]
     lib.trb_group_scene.restype = vp
     lib.trb_group_destroy.argtypes = [vp]

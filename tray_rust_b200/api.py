@@ -199,6 +199,87 @@ class _Base:
         self._check(getattr(self._lib, self._pfx + "scene_update_frame")(self._h, frame, start, end))
 
 
+def _render_halves(render_aov, scene_spp, spp, name, kw):
+    """The two half renders of a denoised frame: samples [0, n/2) and [n/2, n) of n = spp (0: scene_spp) rounded up to a power of
+    two, into two films, with the AOVs accumulated over both. Returns (a, b, aovs, (stats_a, stats_b))."""
+    n = 1
+    while n < (spp or scene_spp):
+        n *= 2
+    if n < 2:
+        raise ValueError("a denoised render needs at least 2 samples per pixel (two half renders); got %d" % (spp or scene_spp))
+    for k in ("spp", "sample_first", "sample_count"):
+        if k in kw:
+            raise ValueError("%s chooses %s itself" % (name, k))
+    half = n // 2
+    a, aovs, st_a = render_aov(spp=n, sample_first=0, sample_count=half, **kw)
+    kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
+    b, _, st_b = render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
+                            sample_count=half, **kw)
+    return a, b, aovs, (st_a, st_b)
+
+
+# The bodies of the denoised renders, shared by Scene (its own render_aov) and Group (the group's AOV render, denoised on replica 0):
+# render_aov / render_adaptive_aov renders the frame, `denoiser` (a Scene) denoises it.
+def _render_denoised(render_aov, denoiser, scene_spp, spp, denoise, kw):
+    a, b, aovs, st = _render_halves(render_aov, scene_spp, spp, "render_denoised", kw)
+    out = denoiser.denoise(a, b, aovs, **(denoise or {}))
+    return out, a + b, aovs, st
+
+
+def _render_denoised_temporal(render_aov, denoiser, scene_spp, history, spp, seed, current_frame, denoise, gradients, kw):
+    frame_seed = (seed + current_frame) % (1 << 32)
+    a, b, aovs, st = _render_halves(render_aov, scene_spp, spp, "render_denoised_temporal",
+                                    dict(kw, seed=frame_seed, current_frame=current_frame))
+    if gradients:
+        out = denoiser.denoise_temporal_gradient(history, a, b, aovs, frame_seed, **(denoise or {}))
+    else:
+        out = denoiser.denoise_temporal(history, a, b, aovs, **(denoise or {}))
+    return out, a + b, aovs, st
+
+
+def _render_denoised_moments(render_aov, denoiser, history, spp, seed, current_frame, denoise, gradients, kw):
+    for k in ("sample_first", "sample_count"):
+        if k in kw:
+            raise ValueError("render_denoised_moments renders the whole sample range; %s is not taken" % k)
+    frame_seed = (seed + current_frame) % (1 << 32)
+    film, aovs, st = render_aov(spp=spp, seed=frame_seed, current_frame=current_frame, **kw)
+    if gradients:
+        out = denoiser.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
+    else:
+        out = denoiser.denoise_moments(history, film, aovs, **(denoise or {}))
+    return out, film, aovs, st
+
+
+def _render_denoised_adaptive(render_adaptive_aov, denoiser, history, min_spp, max_spp, seed, current_frame, denoise, gradients, kw):
+    frame_seed = (seed + current_frame) % (1 << 32)
+    film, aovs, pixel_spp, st = render_adaptive_aov(min_spp, max_spp, seed=frame_seed, current_frame=current_frame, **kw)
+    if gradients:
+        out = denoiser.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
+    else:
+        out = denoiser.denoise_moments(history, film, aovs, **(denoise or {}))
+    return out, film, aovs, pixel_spp, st
+
+
+def _aov_outputs(height, width, film, albedo, normal, nearest):
+    """The host film and AOV arrays of the AOV renders (Scene and Group), checked or allocated: (film, aovs, AovFilm)."""
+    if film is None:
+        film = np.zeros((height, width, 4), np.float32)
+    aovs = {}
+    for name, a, shape, dtype, fill in (("albedo_w", albedo, (height, width, 4), np.float32, 0),
+                                        ("normal_w", normal, (height, width, 4), np.float32, 0),
+                                        ("nearest", nearest, (height, width), np.uint64, np.iinfo(np.uint64).max)):
+        if a is True:
+            a = np.full(shape, fill, dtype)
+        if a is None or a is False:
+            continue
+        if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+            raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        aovs[name] = a
+    if not isinstance(film, np.ndarray) or film.dtype != np.float32 or film.shape != (height, width, 4) or not film.flags.c_contiguous:
+        raise ValueError("film must be a C-contiguous float32 array of shape %s" % ((height, width, 4),))
+    return film, aovs, F.AovFilm(*(aovs[k].ctypes.data if k in aovs else None for k in ("albedo_w", "normal_w", "nearest")))
+
+
 class Scene(_Base):
     """A scene resident on one GPU (product path)."""
     _pfx = "trb_"
@@ -212,8 +293,11 @@ class Scene(_Base):
         self._check(self._lib.trb_scene_create(C.byref(desc), device, C.byref(h)))
         self._h = h
         self.device = device
+        self._read_info()
+
+    def _read_info(self):
         w, hh, spp, nb, ni, nl = (F.u32() for _ in range(6))
-        self._check(self._lib.trb_scene_info(h, *(C.byref(x) for x in (w, hh, spp, nb, ni, nl))))
+        self._check(self._lib.trb_scene_info(self._h, *(C.byref(x) for x in (w, hh, spp, nb, ni, nl))))
         self.width, self.height, self.spp, self.total_blocks, self.n_instances, self.n_lights = (x.value for x in (w, hh, spp, nb, ni, nl))
 
     def _check(self, rc):
@@ -252,29 +336,10 @@ class Scene(_Base):
         (allocate, all ones), False / None or a uint64 (height, width) array. Returns (film, aovs, Stats) where aovs maps "albedo_w",
         "normal_w" and "nearest" to the arrays rendered."""
         cfg = _cfg(**kw)
-        film, aovs, out = self._aov_outputs(film, albedo, normal, nearest)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
         st = F.Stats()
         self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
         return film, aovs, st
-
-    def _aov_outputs(self, film, albedo, normal, nearest):
-        """The host film and AOV arrays of render_aov / render_adaptive_aov, checked or allocated: (film, aovs, AovFilm)."""
-        if film is None:
-            film = np.zeros((self.height, self.width, 4), np.float32)
-        aovs = {}
-        for name, a, shape, dtype, fill in (("albedo_w", albedo, (self.height, self.width, 4), np.float32, 0),
-                                            ("normal_w", normal, (self.height, self.width, 4), np.float32, 0),
-                                            ("nearest", nearest, (self.height, self.width), np.uint64, np.iinfo(np.uint64).max)):
-            if a is True:
-                a = np.full(shape, fill, dtype)
-            if a is None or a is False:
-                continue
-            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
-                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
-            aovs[name] = a
-        if not isinstance(film, np.ndarray) or film.dtype != np.float32 or film.shape != (self.height, self.width, 4) or not film.flags.c_contiguous:
-            raise ValueError("film must be a C-contiguous float32 array of shape %s" % ((self.height, self.width, 4),))
-        return film, aovs, F.AovFilm(*(aovs[k].ctypes.data if k in aovs else None for k in ("albedo_w", "normal_w", "nearest")))
 
     def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, **kw):
         """trb_render_aov_device: device films of height*width*4 float32 (16-byte aligned) and a device nearest buffer of height*width
@@ -409,25 +474,7 @@ class Scene(_Base):
         holds its parameters). The two halves are rendered with seed (seed + current_frame) mod 2^32, so that consecutive frames draw
         independent samples (a frame's radiance is a pure function of scene, seed, pixel and sample). With `gradients`, the frame is
         denoised by denoise_temporal_gradient with that frame seed. Returns render_denoised's tuple."""
-        frame_seed = (seed + current_frame) % (1 << 32)
-        n = 1
-        while n < (spp or self.spp):
-            n *= 2
-        if n < 2:
-            raise ValueError("a denoised render needs at least 2 samples per pixel (two half renders); got %d" % (spp or self.spp))
-        for k in ("spp", "sample_first", "sample_count"):
-            if k in kw:
-                raise ValueError("render_denoised_temporal chooses %s itself" % k)
-        half = n // 2
-        a, aovs, st_a = self.render_aov(spp=n, sample_first=0, sample_count=half, seed=frame_seed, current_frame=current_frame, **kw)
-        kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
-        b, _, st_b = self.render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
-                                     sample_count=half, seed=frame_seed, current_frame=current_frame, **kw)
-        if gradients:
-            out = self.denoise_temporal_gradient(history, a, b, aovs, frame_seed, **(denoise or {}))
-        else:
-            out = self.denoise_temporal(history, a, b, aovs, **(denoise or {}))
-        return out, a + b, aovs, (st_a, st_b)
+        return _render_denoised_temporal(self.render_aov, self, self.spp, history, spp, seed, current_frame, denoise, gradients, kw)
 
     def denoise_moments(self, history, colour, aovs, out=None, motion=False, history_length=False, variance=False, **params):
         """trb_denoise_moments (DESIGN.md §4 "Moment denoising"): one colour film of the frame at any spp, (height, width, 4)
@@ -504,29 +551,14 @@ class Scene(_Base):
         (seed + current_frame) mod 2^32, and denoised with `history` by denoise_moments (the dict `denoise` holds its parameters).
         With `gradients`, the frame is denoised by denoise_moments_gradient with that frame seed. Returns (denoised, film, aovs,
         stats)."""
-        for k in ("sample_first", "sample_count"):
-            if k in kw:
-                raise ValueError("render_denoised_moments renders the whole sample range; %s is not taken" % k)
-        frame_seed = (seed + current_frame) % (1 << 32)
-        film, aovs, st = self.render_aov(spp=spp, seed=frame_seed, current_frame=current_frame, **kw)
-        if gradients:
-            out = self.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
-        else:
-            out = self.denoise_moments(history, film, aovs, **(denoise or {}))
-        return out, film, aovs, st
+        return _render_denoised_moments(self.render_aov, self, history, spp, seed, current_frame, denoise, gradients, kw)
 
     def render_denoised_adaptive(self, history, min_spp, max_spp, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
         """render_denoised_moments with the Adaptive sampler (DESIGN.md §4 "Adaptive AOVs"): frame `current_frame` rendered once by
         render_adaptive_aov(min_spp, max_spp) with seed (seed + current_frame) mod 2^32, and denoised with `history` by
         denoise_moments, or with `gradients` by denoise_moments_gradient with that frame seed. For a single image pass
         denoise={"max_history": 1}. Returns (denoised, film, aovs, pixel_spp, stats)."""
-        frame_seed = (seed + current_frame) % (1 << 32)
-        film, aovs, pixel_spp, st = self.render_adaptive_aov(min_spp, max_spp, seed=frame_seed, current_frame=current_frame, **kw)
-        if gradients:
-            out = self.denoise_moments_gradient(history, film, aovs, frame_seed, **(denoise or {}))
-        else:
-            out = self.denoise_moments(history, film, aovs, **(denoise or {}))
-        return out, film, aovs, pixel_spp, st
+        return _render_denoised_adaptive(self.render_adaptive_aov, self, history, min_spp, max_spp, seed, current_frame, denoise, gradients, kw)
 
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:
@@ -534,21 +566,7 @@ class Scene(_Base):
         accumulated over both, and denoised with the parameters in the dict `denoise` (None: the defaults). kw: render_aov's
         (seed, current_frame, flags, block_start, block_count). Returns (denoised, film, aovs, (stats_a, stats_b)), where film is
         the sum of the two halves, the noisy spp-sample film. Raises ValueError below 2 spp."""
-        n = 1
-        while n < (spp or self.spp):
-            n *= 2
-        if n < 2:
-            raise ValueError("a denoised render needs at least 2 samples per pixel (two half renders); got %d" % (spp or self.spp))
-        for k in ("spp", "sample_first", "sample_count"):
-            if k in kw:
-                raise ValueError("render_denoised chooses %s itself" % k)
-        half = n // 2
-        a, aovs, st_a = self.render_aov(spp=n, sample_first=0, sample_count=half, **kw)
-        kw["flags"] = kw.get("flags", 0) | F.RENDER_NO_UPDATE  # the first half set the frame
-        b, _, st_b = self.render_aov(albedo=aovs["albedo_w"], normal=aovs["normal_w"], nearest=aovs["nearest"], spp=n, sample_first=half,
-                                     sample_count=half, **kw)
-        out = self.denoise(a, b, aovs, **(denoise or {}))
-        return out, a + b, aovs, (st_a, st_b)
+        return _render_denoised(self.render_aov, self, self.spp, spp, denoise, kw)
 
     def _mesh_verts(self, mesh):
         if not 0 <= mesh < self._desc.n_meshes:
@@ -754,7 +772,7 @@ class Scene(_Base):
         """trb_render_adaptive_aov: render_adaptive with the AOVs of the samples it takes (DESIGN.md §4 "Adaptive AOVs"), all
         accumulated into; albedo / normal / nearest as for render_aov. Returns (film, aovs, pixel_spp, Stats)."""
         cfg = _cfg(**kw)
-        film, aovs, out = self._aov_outputs(film, albedo, normal, nearest)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
         spp = np.zeros((self.height, self.width), np.uint32)
         st = F.Stats()
         self._check(self._lib.trb_render_adaptive_aov(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), C.byref(out),
@@ -1004,6 +1022,37 @@ class Comm:
                                                           F.ptr(film) if film is not None else None, F.ptr(pixel_spp), C.byref(st)))
         return film, pixel_spp, st
 
+    def _sharded_aov_outputs(self, scene, root, film, albedo, normal, nearest):
+        """render_aov's host arrays on the root; on the other ranks only the arrays passed (they render and reduce every AOV anyway)"""
+        if self.rank == root:
+            return _aov_outputs(scene.height, scene.width, film, albedo, normal, nearest)
+        return film, {}, None
+
+    def render_sharded_aov(self, scene, film=None, albedo=True, normal=True, nearest=True, root=0, **kw):
+        """trb_render_sharded_aov: render_sharded with the AOVs (DESIGN.md §4 "Multi-GPU AOVs"); every rank renders its shard of the
+        colour film and the three AOVs, ONE NCCL group reduces them to the root. On the root albedo / normal / nearest are as for
+        Scene.render_aov and the result equals it; elsewhere they are ignored. Returns (film, aovs, Stats): film None and aovs
+        empty off the root, Stats this rank's."""
+        cfg = _cfg(**kw)
+        film, aovs, out = self._sharded_aov_outputs(scene, root, film, albedo, normal, nearest)
+        st = F.Stats()
+        self._check(self._lib.trb_render_sharded_aov(scene._h, self._h, C.byref(cfg), root, F.ptr(film) if film is not None else None,
+                                                     C.byref(out) if out is not None else None, C.byref(st)))
+        return film, aovs, st
+
+    def render_sharded_adaptive_aov(self, scene, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, pixel_spp=None, root=0, **kw):
+        """trb_render_sharded_adaptive_aov: render_sharded_adaptive with the AOVs, as render_sharded_aov. Returns (film, aovs,
+        pixel_spp (this rank's pixels filled in), Stats)."""
+        cfg = _cfg(**kw)
+        film, aovs, out = self._sharded_aov_outputs(scene, root, film, albedo, normal, nearest)
+        if pixel_spp is None:
+            pixel_spp = np.zeros((scene.height, scene.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_render_sharded_adaptive_aov(scene._h, self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), root,
+                                                              F.ptr(film) if film is not None else None,
+                                                              C.byref(out) if out is not None else None, F.ptr(pixel_spp), C.byref(st)))
+        return film, aovs, pixel_spp, st
+
     def close(self):
         if self._h is not None:
             self._lib.trb_comm_destroy(self._h)
@@ -1016,8 +1065,29 @@ class Comm:
             pass
 
 
+class _Replica(Scene):
+    """A Group's replica as a Scene (trb_group_scene): every Scene call on it, without ownership; the group destroys it. Its
+    DenoiseHistory objects are released when the group closes."""
+
+    def __init__(self, group, index):
+        self._lib, self._desc, self._histories = group._lib, group._desc, []
+        h = self._lib.trb_group_scene(group._h, index)
+        if not h:
+            raise ValueError("replica %d out of range (%d devices)" % (index, len(group.devices)))
+        self._h, self.device = C.c_void_p(h), group.devices[index]
+        self._group = group  # keeps the replica alive while the view is
+        self._read_info()
+
+    def close(self):
+        for hist in self._histories:
+            hist.close()
+        self._h = None
+
+
 class Group:
-    """One process driving several GPUs (trb_group_*): a scene replica per device, tile-sharded render, one film reduce."""
+    """One process driving several GPUs (trb_group_*): a scene replica per device, tile-sharded render, one film reduce.
+    The AOV renders reduce the AOVs with the film; the denoised renders render on every device and denoise on replica 0
+    (scene(0)), so their DenoiseHistory is DenoiseHistory(group.scene(0))."""
 
     def __init__(self, desc, devices):
         self._lib = F.load_trb()
@@ -1030,6 +1100,21 @@ class Group:
             raise TrbError(rc, (self._lib.trb_last_error() or b"").decode())
         self._h, self.devices = h, list(devices)
         self.width, self.height = desc.film.width, desc.film.height
+        self._replicas = {}
+
+    def _check(self, rc):
+        if rc != F.TRB_OK:
+            raise TrbError(rc, (self._lib.trb_last_error() or b"").decode())
+
+    def scene(self, index=0):
+        """Replica `index` as a Scene (trb_group_scene), borrowed: valid until the group closes."""
+        if index not in self._replicas:
+            self._replicas[index] = _Replica(self, index)
+        return self._replicas[index]
+
+    @property
+    def spp(self):
+        return self.scene(0).spp
 
     def render(self, film=None, **kw):
         cfg = _cfg(**kw)
@@ -1053,8 +1138,49 @@ class Group:
             raise TrbError(rc, (self._lib.trb_last_error() or b"").decode())
         return film, spp, st
 
+    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, **kw):
+        """trb_group_render_aov: Scene.render_aov on all the group's devices (DESIGN.md §4 "Multi-GPU AOVs"): every replica renders
+        its shard of the colour film and the three AOVs, ONE NCCL group reduces them to devices[0]. Arguments and result as for
+        Scene.render_aov; equal to it up to float addition order (nearest exactly)."""
+        cfg = _cfg(**kw)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
+        st = F.Stats()
+        self._check(self._lib.trb_group_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
+        return film, aovs, st
+
+    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, **kw):
+        """trb_group_render_adaptive_aov: Scene.render_adaptive_aov on all the group's devices, as render_aov. Returns (film, aovs,
+        pixel_spp, Stats); pixel_spp equals the one-GPU counts exactly."""
+        cfg = _cfg(**kw)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
+        spp = np.zeros((self.height, self.width), np.uint32)
+        st = F.Stats()
+        self._check(self._lib.trb_group_render_adaptive_aov(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), C.byref(out),
+                                                            F.ptr(spp), C.byref(st)))
+        return film, aovs, spp, st
+
+    def render_denoised(self, spp=0, denoise=None, **kw):
+        """Scene.render_denoised with both halves rendered by render_aov on all devices, denoised on replica 0."""
+        return _render_denoised(self.render_aov, self.scene(0), self.spp, spp, denoise, kw)
+
+    def render_denoised_temporal(self, history, spp=0, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
+        """Scene.render_denoised_temporal rendered by render_aov on all devices; `history` is a DenoiseHistory of scene(0)."""
+        return _render_denoised_temporal(self.render_aov, self.scene(0), self.spp, history, spp, seed, current_frame, denoise, gradients, kw)
+
+    def render_denoised_moments(self, history, spp=0, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
+        """Scene.render_denoised_moments rendered by render_aov on all devices; `history` is a DenoiseHistory of scene(0)."""
+        return _render_denoised_moments(self.render_aov, self.scene(0), history, spp, seed, current_frame, denoise, gradients, kw)
+
+    def render_denoised_adaptive(self, history, min_spp, max_spp, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
+        """Scene.render_denoised_adaptive rendered by render_adaptive_aov on all devices; `history` is a DenoiseHistory of scene(0)."""
+        return _render_denoised_adaptive(self.render_adaptive_aov, self.scene(0), history, min_spp, max_spp, seed, current_frame, denoise,
+                                         gradients, kw)
+
     def close(self):
         if self._h is not None:
+            for r in self._replicas.values():
+                r.close()
+            self._replicas = {}
             self._lib.trb_group_destroy(self._h)
             self._h = None
 

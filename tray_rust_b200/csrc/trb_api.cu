@@ -405,13 +405,17 @@ struct trb_scene {
     void* d_denoise = nullptr;
     size_t denoise_pixels = 0;
     bool denoise_moments = false;
+    // the AOV films of a sharded or group AOV render (trb_render_sharded_aov, trb_group_render_aov and their Adaptive forms), allocated
+    // by the first such render for the film's pixel count and released with the film: per pixel albedo_w, then normal_w (float4 each),
+    // then nearest (uint64), each a whole-film run, so that the NCCL reduce can sum both films in one call
+    void* d_shard_aov = nullptr;
     // temporal denoising (trb_denoise_temporal*): the inverse of the camera's cam_world at the current frame's shutter-open, and the
     // object generation, counted up by the calls that renumber instances (replace_objects, replace_meshes with an object section)
     float cam_inv[16] = {};
     uint64_t object_generation = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
-                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, d_denoise}) if (p) cudaFree(p);
+                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, d_denoise, d_shard_aov}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -2126,7 +2130,8 @@ trb_status stage_film(const trb_film& f, StagedFilm& g) {
 }
 
 // Also retires what was made for the old film: the Morton block lists (keyed by the selection, not by the film size) and the Adaptive
-// sampler's per-pixel and per-block state (sized by the pixel count; ensure_adaptive allocates it anew). The caller has drained the device.
+// sampler's per-pixel and per-block state (sized by the pixel count; ensure_adaptive allocates it anew), the denoiser's scratch and the
+// sharded renders' AOV films (both sized by the pixel count and allocated anew by their next use). The caller has drained the device.
 void commit_film(trb_scene* s, StagedFilm& g) {
     trb::DScene& ds = s->ds;
     s->arena.release(ds.filter_table); s->arena.release(s->d_film);
@@ -2149,7 +2154,7 @@ void commit_film(trb_scene* s, StagedFilm& g) {
     for (BlockList& b : s->block_lists) cudaFree(b.dev);
     s->block_lists.clear();
     for (void** p : {(void**)&s->d_ad_state, (void**)&s->d_ad_list[0], (void**)&s->d_ad_list[1], (void**)&s->d_ad_index[0],
-                     (void**)&s->d_ad_index[1], (void**)&s->d_ad_flags, (void**)&s->d_ad_count, (void**)&s->d_ad_spp, &s->d_denoise}) {
+                     (void**)&s->d_ad_index[1], (void**)&s->d_ad_flags, (void**)&s->d_ad_count, (void**)&s->d_ad_spp, &s->d_denoise, &s->d_shard_aov}) {
         if (*p) cudaFree(*p);
         *p = nullptr;
     }
@@ -4243,9 +4248,21 @@ trb_status shard_cfg(const trb_scene* s, const trb_render_cfg* in, int rank, int
     out->shard_index = (uint32_t)rank; out->shard_count = (uint32_t)n_ranks; out->shard_chunk = in->shard_chunk ? in->shard_chunk : 32u;
     return TRB_OK;
 }
+// The scene's AOV films of a sharded or group AOV render (trb_scene::d_shard_aov), allocated on first use
+trb_status shard_aov_films(trb_scene* s, AovRequest& req) {
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    if (!s->d_shard_aov) {
+        const trb_status r = device_alloc(&s->d_shard_aov, npx * (2 * sizeof(float4) + sizeof(uint64_t)), "AOV films");
+        if (r != TRB_OK) return r;
+    }
+    float4* f = static_cast<float4*>(s->d_shard_aov);
+    req = {nullptr, f, f + npx, reinterpret_cast<unsigned long long*>(f + 2 * npx)};
+    return TRB_OK;
+}
 // Exec::render on one replica with the film left on the device: update_frame, clear, all passes of this shard (LowDiscrepancy,
-// or the Adaptive sampler's rounds when `ad` is set).
-trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, bool empty, cudaStream_t st) {
+// or the Adaptive sampler's rounds when `ad` is set). With `aov` it also renders the three AOVs into the scene's AOV films,
+// cleared first (albedo_w and normal_w to zero, nearest to all ones), so that an empty shard contributes nothing to the reduce.
+trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, bool empty, cudaStream_t st, bool aov = false) {
     CU(cudaSetDevice(s->device));
     if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) {
         const float step = s->film.scene_time / (float)s->film.frames;
@@ -4255,12 +4272,22 @@ trb_status render_to_device_film(trb_scene* s, const trb_render_cfg* cfg, const 
     const size_t npx = (size_t)s->film.width * s->film.height;
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), st));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), st));
+    AovRequest req{nullptr, nullptr, nullptr, nullptr};
+    if (aov) {
+        trb_status r = shard_aov_films(s, req);
+        if (r != TRB_OK) return r;
+        CU(cudaMemsetAsync(req.albedo_w, 0, 2 * npx * sizeof(float4), st)); // albedo_w and normal_w
+        CU(cudaMemsetAsync(req.nearest, 0xff, npx * sizeof(uint64_t), st));
+    }
     if (empty) return TRB_OK;
     if (ad) { // per-pixel counts to d_ad_spp, for shard_pixel_spp_out
         trb_status r = ensure_adaptive(s);
         if (r != TRB_OK) return r;
+        if (aov)
+            return render_adaptive_device(s, cfg, ad, reinterpret_cast<float*>(s->d_film), &req, s->d_ad_spp, reinterpret_cast<trb_stats*>(s->d_stats), st);
         return trb_render_adaptive_device(s, cfg, ad, reinterpret_cast<float*>(s->d_film), s->d_ad_spp, reinterpret_cast<trb_stats*>(s->d_stats), st);
     }
+    if (aov) return render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), st, &req);
     return trb_render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), st);
 }
 // the Adaptive sampler's per-pixel counts of this replica's shard -> pixel_spp (host, width*height; other entries untouched)
@@ -4278,6 +4305,38 @@ trb_status film_to_host_add(trb_scene* s, float* film, cudaStream_t st) {
     CU(cudaMemcpyAsync(s->h_film_staging, s->d_film, npx * sizeof(float4), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     add_film(film, s->h_film_staging, npx * 4);
+    return TRB_OK;
+}
+// The AOV films of a sharded or group AOV render, reduced into `root`'s: albedo_w and normal_w (one run of 8 floats per pixel) summed
+// like the colour film, nearest min-reduced. Exact for nearest: a sample writes only its own pixel and the shards own disjoint pixels,
+// so each pixel's key comes from one replica and the others hold all ones (DESIGN.md §4 "Multi-GPU AOVs"). Inside the caller's
+// ncclGroupStart/End, next to the colour film's reduce.
+trb_status reduce_aov_films(trb_scene* s, ncclComm_t comm, int root, cudaStream_t st) {
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    float4* f = static_cast<float4*>(s->d_shard_aov);
+    NC(g_nccl.Reduce(f, f, npx * 8, ncclFloat, ncclSum, root, comm, st));
+    NC(g_nccl.Reduce(f + 2 * npx, f + 2 * npx, npx, ncclUint64, ncclMin, root, comm, st));
+    return TRB_OK;
+}
+// The root's AOV films into the caller's host buffers, as trb_render_aov leaves them: albedo_w and normal_w added into, nearest
+// min-merged with what the caller's buffer holds; a NULL member (or a NULL aov) is skipped
+trb_status aov_films_to_host(trb_scene* s, const trb_aov_film* aov) {
+    if (!aov) return TRB_OK;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)s->film.width * s->film.height;
+    const float4* f = static_cast<const float4*>(s->d_shard_aov);
+    std::vector<float> h;
+    for (auto [dst, src] : {std::pair<float*, const float4*>{aov->albedo_w, f}, {aov->normal_w, f + npx}}) {
+        if (!dst) continue;
+        h.resize(npx * 4);
+        CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
+        add_film(dst, h.data(), npx * 4);
+    }
+    if (aov->nearest) {
+        std::vector<uint64_t> v(npx);
+        CU(cudaMemcpy(v.data(), f + 2 * npx, npx * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < npx; ++i) aov->nearest[i] = std::min(aov->nearest[i], v[i]);
+    }
     return TRB_OK;
 }
 } // namespace
@@ -4337,15 +4396,20 @@ trb_status trb_comm_reduce_film(trb_comm* c, float* d_film, size_t n, int root, 
 } // extern "C"
 
 namespace {
-// trb_render_sharded (ad == nullptr) and trb_render_sharded_adaptive
+// trb_render_sharded (ad == nullptr) and trb_render_sharded_adaptive; with `with_aov` their AOV forms, whose host AOV films `aov`
+// are the root's only (every rank renders and reduces all three AOVs)
 trb_status render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, const trb_adaptive* ad, int root, float* film, uint32_t* pixel_spp,
-                          trb_stats* stats) {
+                          trb_stats* stats, bool with_aov = false, const trb_aov_film* aov = nullptr) {
     if (!s || !c || !cfg || root < 0 || root >= c->n_ranks) return fail(TRB_INVALID_ARG, "null or bad argument");
     if (c->rank == root && !film) return fail(TRB_INVALID_ARG, "the root rank needs a film buffer");
+    if (with_aov && c->rank == root && !aov) return fail(TRB_INVALID_ARG, "null argument");
     if (c->device != s->device) return fail(TRB_INVALID_ARG, "scene and communicator live on different devices");
     if (ad) { // before sharding: a rank whose shard is empty answers like the others
         trbh::AdSchedule sch;
         trb_status r = adaptive_check(s, cfg, ad, sch);
+        if (r != TRB_OK) return r;
+    } else if (with_aov) { // adaptive_check's statuses cover aov_supported's
+        trb_status r = aov_supported(s, cfg);
         if (r != TRB_OK) return r;
     }
     trb_render_cfg mine; bool empty;
@@ -4354,12 +4418,24 @@ trb_status render_sharded(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, 
     auto t0 = std::chrono::steady_clock::now();
     CU(cudaSetDevice(s->device));
     CU(cudaEventRecord(s->ev0, 0));
-    r = render_to_device_film(s, &mine, ad, empty, nullptr);
+    r = render_to_device_film(s, &mine, ad, empty, nullptr, with_aov);
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev1, 0));
-    r = trb_comm_reduce_film(c, reinterpret_cast<float*>(s->d_film), (size_t)s->film.width * s->film.height * 4, root, nullptr); // ONE reduce per frame
+    const size_t nfl = (size_t)s->film.width * s->film.height * 4;
+    if (with_aov && c->n_ranks > 1) { // ONE NCCL group per frame: the colour film and the three AOVs
+        NC(g_nccl.GroupStart());
+        NC(g_nccl.Reduce(s->d_film, s->d_film, nfl, ncclFloat, ncclSum, root, c->comm, nullptr));
+        r = reduce_aov_films(s, c->comm, root, nullptr);
+        NC(g_nccl.GroupEnd());
+    } else {
+        r = trb_comm_reduce_film(c, reinterpret_cast<float*>(s->d_film), nfl, root, nullptr); // ONE reduce per frame
+    }
     if (r != TRB_OK) return r;
-    if (c->rank == root) { r = film_to_host_add(s, film, nullptr); if (r != TRB_OK) return r; }
+    if (c->rank == root) {
+        r = film_to_host_add(s, film, nullptr);
+        if (r == TRB_OK && with_aov) r = aov_films_to_host(s, aov);
+        if (r != TRB_OK) return r;
+    }
     else CU(cudaStreamSynchronize(nullptr));
     r = check_error_flag(s);
     if (r != TRB_OK) return r;
@@ -4380,6 +4456,16 @@ trb_status trb_render_sharded_adaptive(trb_scene* s, trb_comm* c, const trb_rend
                                        uint32_t* pixel_spp, trb_stats* stats) {
     if (!ad) return fail(TRB_INVALID_ARG, "null argument");
     return render_sharded(s, c, cfg, ad, root, film, pixel_spp, stats);
+}
+
+trb_status trb_render_sharded_aov(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, int root, float* film, const trb_aov_film* aov, trb_stats* stats) {
+    return render_sharded(s, c, cfg, nullptr, root, film, nullptr, stats, true, aov);
+}
+
+trb_status trb_render_sharded_adaptive_aov(trb_scene* s, trb_comm* c, const trb_render_cfg* cfg, const trb_adaptive* ad, int root, float* film,
+                                           const trb_aov_film* aov, uint32_t* pixel_spp, trb_stats* stats) {
+    if (!ad) return fail(TRB_INVALID_ARG, "null argument");
+    return render_sharded(s, c, cfg, ad, root, film, pixel_spp, stats, true, aov);
 }
 
 trb_status trb_group_create(const trb_scene_desc* desc, const int* devices, int n, trb_group** out) {
@@ -4432,19 +4518,24 @@ void trb_group_destroy(trb_group* g) {
 } // extern "C"
 
 namespace {
-// trb_group_render (ad == nullptr) and trb_group_render_adaptive
-trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
+// trb_group_render (ad == nullptr) and trb_group_render_adaptive; with `aov` their AOV forms
+trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats,
+                        const trb_aov_film* aov = nullptr) {
     if (!g || !cfg || !film) return fail(TRB_INVALID_ARG, "null argument");
     const int n = (int)g->scenes.size();
     for (const trb_scene* s : g->scenes) // the film reduce is sized by replica 0 (trb_scene_replace_settings edits one replica at a time)
         if (s->film.width != g->scenes[0]->film.width || s->film.height != g->scenes[0]->film.height)
             return fail(TRB_INVALID_ARG, "the group's replicas have different film sizes");
+    if (n == 1 && aov)
+        return ad ? trb_render_adaptive_aov(g->scenes[0], cfg, ad, film, aov, pixel_spp, stats) : trb_render_aov(g->scenes[0], cfg, film, aov, stats);
     if (n == 1) return ad ? trb_render_adaptive(g->scenes[0], cfg, ad, film, pixel_spp, stats) : trb_render(g->scenes[0], cfg, film, stats);
     if (ad) {
         trbh::AdSchedule sch;
         trb_status r = adaptive_check(g->scenes[0], cfg, ad, sch);
         if (r != TRB_OK) return r;
     }
+    if (aov) // every replica, before any renders (adaptive_check's statuses cover aov_supported's on replica 0)
+        for (const trb_scene* s : g->scenes) { const trb_status r = aov_supported(s, cfg); if (r != TRB_OK) return r; }
     auto t0 = std::chrono::steady_clock::now();
     // enqueue every replica's shard (update_frame is host work per replica; the kernels of all devices then run concurrently)
     std::vector<trb_status> rc(n, TRB_OK);
@@ -4456,20 +4547,22 @@ trb_status group_render(trb_group* g, const trb_render_cfg* cfg, const trb_adapt
         bool e = false;
         rc[i] = shard_cfg(g->scenes[i], cfg, i, n, &mine[i], &e);
         empty[i] = e;
-        if (rc[i] == TRB_OK) { cudaSetDevice(g->scenes[i]->device); cudaEventRecord(g->scenes[i]->ev0, 0); rc[i] = render_to_device_film(g->scenes[i], &mine[i], ad, e, nullptr); cudaEventRecord(g->scenes[i]->ev1, 0); }
+        if (rc[i] == TRB_OK) { cudaSetDevice(g->scenes[i]->device); cudaEventRecord(g->scenes[i]->ev0, 0); rc[i] = render_to_device_film(g->scenes[i], &mine[i], ad, e, nullptr, aov != nullptr); cudaEventRecord(g->scenes[i]->ev1, 0); }
         if (rc[i] != TRB_OK) msg[i] = trb_last_error();
     });
     for (auto& t : th) t.join();
     for (int i = 0; i < n; ++i) if (rc[i] != TRB_OK) return fail(rc[i], msg[i]);
     const size_t nfl = (size_t)g->scenes[0]->film.width * g->scenes[0]->film.height * 4;
-    NC(g_nccl.GroupStart()); // ONE reduce per frame, root = devices[0]
+    NC(g_nccl.GroupStart()); // ONE reduce per frame, root = devices[0] (with the AOVs: one NCCL group of the colour film and the three AOVs)
     for (int i = 0; i < n; ++i) {
         CU(cudaSetDevice(g->scenes[i]->device));
         NC(g_nccl.Reduce(g->scenes[i]->d_film, g->scenes[i]->d_film, nfl, ncclFloat, ncclSum, 0, g->comms[i], nullptr));
+        if (aov) { const trb_status r = reduce_aov_films(g->scenes[i], g->comms[i], 0, nullptr); if (r != TRB_OK) return r; }
     }
     NC(g_nccl.GroupEnd());
     CU(cudaSetDevice(g->scenes[0]->device));
     trb_status r = film_to_host_add(g->scenes[0], film, nullptr);
+    if (r == TRB_OK && aov) r = aov_films_to_host(g->scenes[0], aov);
     if (r != TRB_OK) return r;
     float kernel_ms = 0.f;
     if (stats) std::memset(stats, 0, sizeof *stats);
@@ -4501,6 +4594,17 @@ trb_status trb_group_render(trb_group* g, const trb_render_cfg* cfg, float* film
 trb_status trb_group_render_adaptive(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, uint32_t* pixel_spp, trb_stats* stats) {
     if (!ad) return fail(TRB_INVALID_ARG, "null argument");
     return group_render(g, cfg, ad, film, pixel_spp, stats);
+}
+
+trb_status trb_group_render_aov(trb_group* g, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats) {
+    if (!aov) return fail(TRB_INVALID_ARG, "null argument");
+    return group_render(g, cfg, nullptr, film, nullptr, stats, aov);
+}
+
+trb_status trb_group_render_adaptive_aov(trb_group* g, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov,
+                                         uint32_t* pixel_spp, trb_stats* stats) {
+    if (!ad || !aov) return fail(TRB_INVALID_ARG, "null argument");
+    return group_render(g, cfg, ad, film, pixel_spp, stats, aov);
 }
 
 } // extern "C"

@@ -12,6 +12,8 @@
 #include <netinet/in.h>
 #include <sys/socket.h>
 #include <unistd.h>
+#include <cctype>
+#include <cerrno>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -38,6 +40,24 @@ inline bool write_all(int fd, const void* src, size_t n) {
 }
 inline uint64_t get_u64(const std::vector<uint8_t>& b, size_t& o) { uint64_t v = 0; if (o + 8 <= b.size()) std::memcpy(&v, &b[o], 8); o += 8; return v; } // x86-64: little-endian
 inline void put_u64(std::vector<uint8_t>& b, uint64_t v) { const size_t o = b.size(); b.resize(o + 8); std::memcpy(&b[o], &v, 8); }
+
+// --devices: a comma-separated list of distinct CUDA device ordinals ("0,1,2,3"). Returns an empty string, or what is wrong with it.
+inline std::string parse_devices(const char* s, std::vector<int>& out) {
+    out.clear();
+    if (!s || !*s) return "--devices needs a comma-separated list of device ordinals, e.g. 0,1,2,3";
+    const std::string bad = std::string("malformed --devices list '") + s + "': use device ordinals separated by commas, e.g. 0,1,2,3";
+    for (const char* p = s;; ++p) {
+        if (!std::isdigit((unsigned char)*p)) return bad;
+        char* e = nullptr; errno = 0;
+        const unsigned long v = std::strtoul(p, &e, 10);
+        if (errno || v > 0x7fffffffu) return bad;
+        for (int d : out) if (d == (int)v) return std::string("--devices lists device ") + std::to_string(v) + " twice";
+        out.push_back((int)v);
+        if (!*e) return "";
+        if (*e != ',') return bad;
+        p = e;
+    }
+}
 
 struct Instructions { uint64_t encoded_size = 0; std::string scene; uint64_t frame_start = 0, frame_end = 0, block_start = 0, block_count = 0; };
 
@@ -116,21 +136,30 @@ inline std::string decode_frame(const std::vector<uint8_t>& buf, Frame& f) {
 // `tray_rust --worker` (main.rs:148-166, worker.rs:37-89): listens on `port`, accepts ONE connection, reads the Instructions,
 // Scene::load_file(instructions.scene), then for every frame of the inclusive range renders blocks
 // [block_start, block_start + block_count) of the Morton list (trb_render: Exec::render with select_blocks, including
-// update_frame), sends the Frame and clears the film. Exits after the last frame.
-//   [--worker] [-n N] [--port P] [--device D] [--seed S] [--spp N]
+// update_frame), sends the Frame and clears the film. Exits after the last frame. With --devices the blocks are rendered by a
+// trb_group of those GPUs (trb_group_render: the range sharded over them, one film reduce); the Frames are the same message.
+//   [--worker] [-n N] [--port P] [--device D | --devices D0,D1,...] [--seed S] [--spp N]
 // No CPU fallback: without a CUDA device the scene load fails with TRB_NO_DEVICE and the worker exits with status 3.
 inline int worker_main(int argc, char** argv) {
     int port = PORT, device = 0;
     uint32_t seed = 1, spp = 0;
+    bool has_device = false;
+    std::vector<int> devices;
     for (int i = 1; i < argc; ++i) {
         const std::string a = argv[i];
         if (a == "--port" && i + 1 < argc) port = std::atoi(argv[++i]);
-        else if (a == "--device" && i + 1 < argc) device = std::atoi(argv[++i]);
+        else if (a == "--device" && i + 1 < argc) { device = std::atoi(argv[++i]); has_device = true; }
+        else if (a == "--devices") {
+            const std::string bad = parse_devices(i + 1 < argc ? argv[i + 1] : nullptr, devices);
+            if (!bad.empty()) { std::fprintf(stderr, "%s\n", bad.c_str()); return 2; }
+            ++i;
+        }
         else if (a == "--seed" && i + 1 < argc) seed = (uint32_t)std::strtoul(argv[++i], nullptr, 0);
         else if (a == "--spp" && i + 1 < argc) spp = (uint32_t)std::strtoul(argv[++i], nullptr, 0);
         else if (a == "--worker" || a == "-n") { if (a == "-n") ++i; } // accepted for command-line compatibility with `tray_rust --worker [-n threads]`
-        else { std::fprintf(stderr, "usage: %s [--worker] [--port P] [--device D] [--seed S] [--spp N]\n", argv[0]); return 2; }
+        else { std::fprintf(stderr, "usage: %s [--worker] [--port P] [--device D | --devices D0,D1,...] [--seed S] [--spp N]\n", argv[0]); return 2; }
     }
+    if (has_device && !devices.empty()) { std::fprintf(stderr, "--devices and --device exclude each other: list every GPU in --devices\n"); return 2; }
     const int lfd = ::socket(AF_INET, SOCK_STREAM, 0);
     int one = 1;
     ::setsockopt(lfd, SOL_SOCKET, SO_REUSEADDR, &one, sizeof one);
@@ -152,8 +181,14 @@ inline int worker_main(int argc, char** argv) {
                 (unsigned long long)in.encoded_size, in.scene.c_str(), (unsigned long long)in.frame_start, (unsigned long long)in.frame_end,
                 (unsigned long long)in.block_start, (unsigned long long)in.block_count);
     trb_scene* scene = nullptr;
-    trb_status rc = trb_scene_load_json(in.scene.c_str(), 0, 0, spp, device, &scene); // Scene::load_file(&instructions.scene) (worker.rs:39)
-    if (rc != TRB_OK) { std::fprintf(stderr, "trb_scene_load_json status %d: %s\n", (int)rc, trb_last_error()); return rc == TRB_NO_DEVICE ? 3 : 1; }
+    trb_group* group = nullptr;
+    trb_status rc = devices.empty() ? trb_scene_load_json(in.scene.c_str(), 0, 0, spp, device, &scene) // Scene::load_file(&instructions.scene) (worker.rs:39)
+                                    : trb_group_load_json(in.scene.c_str(), 0, 0, spp, devices.data(), (int)devices.size(), &group);
+    if (rc != TRB_OK) {
+        std::fprintf(stderr, "%s status %d: %s\n", devices.empty() ? "trb_scene_load_json" : "trb_group_load_json", (int)rc, trb_last_error());
+        return rc == TRB_NO_DEVICE ? 3 : 1;
+    }
+    if (group) scene = trb_group_scene(group, 0);
     uint32_t w = 0, h = 0;
     trb_scene_info(scene, &w, &h, nullptr, nullptr, nullptr, nullptr);
     std::vector<float> film((size_t)w * h * 4);
@@ -162,14 +197,15 @@ inline int worker_main(int argc, char** argv) {
         trb_render_cfg cfg{};
         cfg.block_start = (uint32_t)in.block_start; cfg.block_count = (uint32_t)in.block_count; cfg.current_frame = (uint32_t)frame; cfg.seed = seed;
         trb_stats st{};
-        rc = trb_render(scene, &cfg, film.data(), &st);
-        if (rc != TRB_OK) { std::fprintf(stderr, "trb_render status %d: %s\n", (int)rc, trb_last_error()); return 1; }
+        rc = group ? trb_group_render(group, &cfg, film.data(), &st) : trb_render(scene, &cfg, film.data(), &st);
+        if (rc != TRB_OK) { std::fprintf(stderr, "%s status %d: %s\n", group ? "trb_group_render" : "trb_render", (int)rc, trb_last_error()); return 1; }
         const std::vector<uint8_t> bytes = encode_frame(frame, film.data(), w, h);
         if (!write_all(fd, bytes.data(), bytes.size())) { std::fprintf(stderr, "Failed to send frame to the master\n"); return 1; }
         std::printf("Frame %llu: rendering took %.4fs\n--------------------\n", (unsigned long long)frame, st.kernel_ms * 1e-3);
         std::fflush(stdout);
     }
-    trb_scene_destroy(scene);
+    if (group) trb_group_destroy(group);
+    else trb_scene_destroy(scene);
     ::close(fd); ::close(lfd);
     return 0;
 }

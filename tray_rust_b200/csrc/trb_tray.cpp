@@ -1,9 +1,9 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
-//   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D] [--denoise]
-//            [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--adaptive MIN MAX]
+//   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D | --devices LIST]
+//            [--denoise] [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--adaptive MIN MAX]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
-//   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]
+//   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]
 //
 // Single node (main.rs:56-109): Scene::load_file, then for every frame of the inclusive range Exec::render (trb_render, which
 // includes update_frame), RenderTarget::get_render (trb_film_to_srgb8), write the image, clear the film.
@@ -24,7 +24,11 @@
 // --denoise-moments, denoises with trb_denoise_moments_gradient at the frame's seed; --adaptive MIN MAX renders each frame with the
 // Adaptive sampler (trb_render_adaptive), or with --denoise-moments by trb_render_adaptive_aov and the moment call (single node, path
 // integrator; refused with --spp, since the sampler owns the schedule, and with --denoise, --denoise-temporal and --temporal-gradients,
-// which need two half sample ranges); a worker address is host[:port],
+// which need two half sample ranges); --devices 0,1,2,3 renders each frame on a trb_group of those GPUs in place of one --device:
+// plain and --adaptive frames by trb_group_render(_adaptive), every denoise mode by the group's AOV renders (trb_group_render_aov,
+// trb_group_render_adaptive_aov) and the denoise call on replica 0, which holds the history; with --worker the master's block range
+// is rendered by trb_group_render, in the same Frames (refused with --device, with --master, and for an empty, malformed or
+// duplicate list, before anything renders); a worker address is host[:port],
 // a bare host meaning port 63234; -n is accepted and ignored. Output: -o without an extension is a directory (created, one level;
 // frames go to frame%05d.png inside), with an extension one file rewritten by every frame, none means ./. PNG (stored deflate
 // blocks) and binary PPM are written; JPEG is not built.
@@ -47,10 +51,11 @@ namespace {
 
 const char* USAGE =
     "Usage:\n"
-    "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N] [--device D]\n"
-    "             [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]] [--adaptive MIN MAX]\n"
+    "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N]\n"
+    "             [--device D | --devices LIST] [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]]\n"
+    "             [--adaptive MIN MAX]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
-    "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D]\n"
+    "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]\n"
     "    trb_tray (-h | --help)\n"
     "\n"
     "Options:\n"
@@ -63,6 +68,9 @@ const char* USAGE =
     "  --seed S                Random seed of the render (default 1).\n"
     "  --spp N                 Samples per pixel, overriding the scene's film.samples.\n"
     "  --device D              CUDA device to render on (default 0).\n"
+    "  --devices LIST          Render each frame on all the CUDA devices of the comma-separated LIST (e.g. 0,1,2,3): the image is\n"
+    "                          split between them and their films summed; every --denoise mode denoises on the first. Not with\n"
+    "                          --device or --master (with --master pass it to each worker).\n"
     "  --denoise               Render each frame's samples as two halves with albedo, normal and depth, and write the denoised\n"
     "                          image. Single node only, path integrator, at least 2 samples per pixel.\n"
     "  --denoise-temporal      As --denoise, accumulating each pixel's history over the frame range through the scene's motion;\n"
@@ -170,6 +178,7 @@ struct Args {
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
          denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false, adaptive = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0, ad_min = 0, ad_max = 0;
+    std::vector<int> devices; // --devices; empty: one --device
 };
 
 // scene description (host only): the film section, frame range overrides applied
@@ -190,22 +199,37 @@ bool load_desc(const Args& a, uint32_t spp, Desc& desc, uint64_t& start, uint64_
 
 uint32_t pow2_at_least(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 
+// Where a frame renders: one scene (--device), or a group of GPUs (--devices) whose renders reduce to replica 0. `scene` is the
+// scene that converts and denoises: the one scene, or the group's replica 0, which also holds the denoise history.
+struct Renderer {
+    trb_scene* scene = nullptr;
+    trb_group* group = nullptr;
+    trb_status aov(const trb_render_cfg* cfg, float* film, const trb_aov_film* aov) const {
+        return group ? trb_group_render_aov(group, cfg, film, aov, nullptr) : trb_render_aov(scene, cfg, film, aov, nullptr);
+    }
+    trb_status adaptive_aov(const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov) const {
+        return group ? trb_group_render_adaptive_aov(group, cfg, ad, film, aov, nullptr, nullptr)
+                     : trb_render_adaptive_aov(scene, cfg, ad, film, aov, nullptr, nullptr);
+    }
+};
+
 // --denoise: samples [0, n/2) and [n/2, n) of the frame into two films, the AOVs over both, then trb_denoise (DESIGN.md §4 "Denoising");
 // --denoise-temporal: the same with trb_denoise_temporal and the history of the frames before (DESIGN.md §4 "Temporal denoising")
 struct DenoisedFrame {
     std::vector<float> a, b, albedo, normal, out;
     std::vector<uint64_t> nearest;
     explicit DenoisedFrame(size_t npx) : a(npx * 4), b(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history = nullptr, bool gradients = false) {
+    void render(const Renderer& r, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history = nullptr, bool gradients = false) {
+        trb_scene* s = r.scene;
         std::fill(a.begin(), a.end(), 0.0f); std::fill(b.begin(), b.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
         trb_render_cfg cfg{};
         cfg.spp = spp; cfg.seed = seed; cfg.current_frame = frame; cfg.sample_count = spp / 2;
         const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
-        tray::check(trb_render_aov(s, &cfg, a.data(), &aov, nullptr)); // includes Scene::update_frame
+        tray::check(r.aov(&cfg, a.data(), &aov)); // includes Scene::update_frame
         cfg.sample_first = spp / 2; cfg.flags = TRB_RENDER_NO_UPDATE;
-        tray::check(trb_render_aov(s, &cfg, b.data(), &aov, nullptr));
+        tray::check(r.aov(&cfg, b.data(), &aov));
         const trb_denoise_input in{a.data(), b.data(), albedo.data(), normal.data(), nearest.data()};
         if (history && gradients) {
             const trb_denoise_gradient_output o{out.data(), nullptr, nullptr, nullptr};
@@ -227,15 +251,16 @@ struct MomentsFrame {
     std::vector<uint64_t> nearest;
     explicit MomentsFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), out(npx * 4), nearest(npx) {}
     // ad: the Adaptive sampler in place of LowDiscrepancy at spp (trb_render_adaptive_aov; DESIGN.md §4 "Adaptive AOVs"), or nullptr
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history, bool gradients, const trb_adaptive* ad) {
+    void render(const Renderer& r, uint32_t spp, uint32_t seed, uint32_t frame, trb_denoise_history* history, bool gradients, const trb_adaptive* ad) {
+        trb_scene* s = r.scene;
         std::fill(colour.begin(), colour.end(), 0.0f);
         std::fill(albedo.begin(), albedo.end(), 0.0f); std::fill(normal.begin(), normal.end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
         trb_render_cfg cfg{};
         cfg.spp = spp; cfg.seed = seed; cfg.current_frame = frame;
         const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
-        if (ad) { cfg.spp = 0; tray::check(trb_render_adaptive_aov(s, &cfg, ad, colour.data(), &aov, nullptr, nullptr)); } // includes Scene::update_frame
-        else tray::check(trb_render_aov(s, &cfg, colour.data(), &aov, nullptr)); // includes Scene::update_frame
+        if (ad) { cfg.spp = 0; tray::check(r.adaptive_aov(&cfg, ad, colour.data(), &aov)); } // includes Scene::update_frame
+        else tray::check(r.aov(&cfg, colour.data(), &aov)); // includes Scene::update_frame
         const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
         if (gradients) {
             const trb_denoise_moments_gradient_output o{out.data(), nullptr, nullptr, nullptr, nullptr};
@@ -264,9 +289,20 @@ int single_node(const Args& a, const OutPath& out) {
         return die("--adaptive needs the path integrator: the Adaptive sampler is built for it only");
     const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
     try {
-        tray::Scene scene = tray::Scene::from_desc(*desc.d, (int)a.device);
+        std::unique_ptr<tray::Scene> one;
+        std::unique_ptr<trb_group, void (*)(trb_group*)> group(nullptr, trb_group_destroy);
+        if (a.devices.empty()) {
+            one.reset(new tray::Scene(tray::Scene::from_desc(*desc.d, (int)a.device)));
+        } else {
+            trb_group* g = nullptr;
+            tray::check(trb_group_create(desc.d, a.devices.data(), (int)a.devices.size(), &g));
+            group.reset(g);
+        }
         trb_desc_free(desc.d); desc.d = nullptr;
-        tray::RenderTarget rt = scene.make_render_target();
+        const Renderer rd{one ? one->handle() : trb_group_scene(group.get(), 0), group.get()};
+        uint32_t width = 0, height = 0;
+        tray::check(trb_scene_info(rd.scene, &width, &height, nullptr, nullptr, nullptr, nullptr));
+        tray::RenderTarget rt(width, height);
         const auto dim = rt.dimensions();
         tray::B200 exec;
         tray::Config config;
@@ -279,23 +315,31 @@ int single_node(const Args& a, const OutPath& out) {
         trb_denoise_history* history = nullptr;
         std::unique_ptr<MomentsFrame> mf;
         if (a.denoise_moments) mf.reset(new MomentsFrame((size_t)dim.first * dim.second));
-        if (a.denoise_temporal || a.denoise_moments) tray::check(trb_denoise_history_create(scene.handle(), &history));
+        if (a.denoise_temporal || a.denoise_moments) tray::check(trb_denoise_history_create(rd.scene, &history));
         const std::unique_ptr<trb_denoise_history, trb_status (*)(trb_denoise_history*)> history_owner(history, trb_denoise_history_destroy);
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (mf) {
-                mf->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients, a.adaptive ? &ad : nullptr);
+                mf->render(rd, spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients, a.adaptive ? &ad : nullptr);
                 img.resize((size_t)dim.first * dim.second * 3);
-                tray::check(trb_film_to_srgb8(scene.handle(), mf->out.data(), img.data()));
+                tray::check(trb_film_to_srgb8(rd.scene, mf->out.data(), img.data()));
             } else if (dn) {
-                if (history) dn->render(scene.handle(), spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.temporal_gradients);
-                else dn->render(scene.handle(), spp, config.seed, (uint32_t)i);
+                if (history) dn->render(rd, spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.temporal_gradients);
+                else dn->render(rd, spp, config.seed, (uint32_t)i);
                 img.resize((size_t)dim.first * dim.second * 3);
-                tray::check(trb_film_to_srgb8(scene.handle(), dn->out.data(), img.data()));
-            } else {
-                exec.render(scene, rt, config);
-                img = tray::get_render(scene, rt);
+                tray::check(trb_film_to_srgb8(rd.scene, dn->out.data(), img.data()));
+            } else if (one) {
+                exec.render(*one, rt, config);
+                img = tray::get_render(*one, rt);
+            } else { // B200::render's calls on the group
+                trb_render_cfg cfg{};
+                cfg.current_frame = (uint32_t)i; cfg.seed = config.seed;
+                std::vector<uint32_t> pixel_spp(a.adaptive ? (size_t)dim.first * dim.second : 0);
+                if (a.adaptive) tray::check(trb_group_render_adaptive(group.get(), &cfg, &ad, rt.data(), pixel_spp.data(), nullptr));
+                else tray::check(trb_group_render(group.get(), &cfg, rt.data(), nullptr));
+                img.resize((size_t)dim.first * dim.second * 3);
+                tray::check(trb_film_to_srgb8(rd.scene, rt.data(), img.data()));
             }
             const std::string file = out.file_for(i);
             if (!save_image(out, file, img.data(), (uint32_t)dim.first, (uint32_t)dim.second)) return 1;
@@ -536,6 +580,11 @@ int main(int argc, char** argv) {
         else if (s == "--seed") ok = number(a.seed, a.has_seed) && a.seed <= UINT32_MAX;
         else if (s == "--spp") ok = number(a.spp, a.has_spp) && a.spp <= UINT32_MAX;
         else if (s == "--device") ok = number(a.device, a.has_device) && a.device <= INT32_MAX;
+        else if (s == "--devices") {
+            const std::string bad = trb_distrib::parse_devices(v, a.devices);
+            if (!bad.empty()) return die("%s", bad.c_str());
+            ++i;
+        }
         else if (s == "--master") a.master = true;
         else if (s == "--denoise") a.denoise = true;
         else if (s == "--denoise-temporal") a.denoise_temporal = true;
@@ -556,6 +605,8 @@ int main(int argc, char** argv) {
     if (!have_scene) { std::fputs(USAGE, stderr); return 2; }
     if (a.master && a.workers.empty()) return die("--master needs at least one worker address");
     if (!a.master && !a.workers.empty()) return die("unexpected argument '%s' (worker addresses follow --master)", a.workers[0].c_str());
+    if (a.master && !a.devices.empty()) return die("--devices is a worker's option with --master: pass it to each worker");
+    if (a.has_device && !a.devices.empty()) return die("--devices and --device exclude each other: list every GPU in --devices");
     if (a.master && (a.has_seed || a.has_spp || a.has_device)) return die("--seed, --spp and --device are the workers' options: pass them to each worker");
     if (a.master && a.denoise_moments)
         return die("--denoise-moments is not available with --master: the wire format carries no albedo, normal or depth");
