@@ -1078,6 +1078,54 @@ trb_status trb_denoise_moments_device(trb_scene* scene, trb_denoise_history* his
                                       const trb_denoise_temporal_params* params, const trb_denoise_moments_output* d_out,
                                       void* cuda_stream);
 
+/* -- Sample variance: denoise one render with the variance of its own samples (DESIGN.md §4 "Sample variance") ------------------
+ * The lum_w film. trb_render_aov_lum and trb_render_adaptive_aov_lum (and their _device forms) add one more AOV film, in the colour
+ * film's layout (width*height RGBW floats, added into). Per camera sample, float32, left to right, never contracted, with c the
+ * radiance the colour film adds for the sample and a the albedo of its AOV record (0 on a miss):
+ *   d = max(a, TRB_DENOISE_EPS_ALBEDO) per channel,  l = L(c / d) = 0.2126 (c.r / d.r) + 0.7152 (c.g / d.g) + 0.0722 (c.b / d.b)
+ *   the sample adds (w * l, w * (l * l), w * w, w) with the colour film's weights w (RenderTarget::write: filter table,
+ *   filter_pixel_width window, 2x2 lock blocks); Mitchell's w can be negative, w * w is not. lum_w.w is the colour film's W up to
+ *   float addition order. An Adaptive render adds every sample of every round under the colour film's Adaptive rules.
+ * Each sample is demodulated by its own albedo, not by the pixel's filtered one: albedo changes inside a pixel's footprint are
+ * antialiasing, not noise, and do not raise the variance.
+ *
+ * trb_denoise_variance: trb_denoise's filter over one film with v from lum_w. Per pixel p, float32, left to right, never contracted:
+ *   1. W = colour.w. W <= 0: the output is (0, 0, 0, 0) and p is never a neighbour. c = colour.rgb / W; d, m, len2, n, z, dz and
+ *      e = c / d are trb_denoise's.
+ *   2. V1 = lum_w.w, V2 = lum_w.z, m1 = lum_w.x / V1, m2 = lum_w.y / V1. If V1 > 0 and V1 * V1 > V2:
+ *        v = max(0, m2 - m1 * m1) * V2 / (V1 * V1 - V2),   max(0, x) = x > 0 ? x : 0
+ *      otherwise (at most one effective sample) v = NaN. For independent samples this is the unbiased estimate of the variance of
+ *      the pixel's weighted mean of l (reliability weights); with equal weights it is s^2 / n. LowDiscrepancy's stratified samples
+ *      have a smaller true variance than independent ones, so v overestimates it and errs toward blurring.
+ *   3. Unless c, albedo, m, len2, e and v are all finite and z is neither NaN nor -inf, p is copied through as (c, 1) and is never
+ *      a neighbour.
+ *   4. (e, v) goes into trb_denoise's a-trous iterations unchanged; the output is (e_N * d, 1) (iterations 0: e * d). Every NaN
+ *      written to rgbw or variance is 0x7fffffff. variance (may be NULL; width*height floats) receives v, or NaN where p is not
+ *      filtered.
+ * No history: a still image, or any frame on its own. The scene's denoise scratch is trb_denoise's 72 bytes per pixel.
+ * The Adaptive forms, trb_render_adaptive_aov_lum*, are declared with the Adaptive AOVs below. */
+
+/* trb_render_aov with the lum_w film (HOST, width*height*4 floats, added into; required). The colour film, the AOVs and every
+ * trb_stats counter equal trb_render_aov's with the same cfg, and so do the statuses. The AOV records are computed even when
+ * aov's three members are NULL. Blocking. */
+trb_status trb_render_aov_lum(trb_scene* scene, const trb_render_cfg* cfg, float* film_rgbw, const trb_aov_film* aov, float* lum_w,
+                              trb_stats* stats);
+/* trb_render_aov_device with the DEVICE lum_w film (16-byte aligned, else TRB_INVALID_ARG). */
+trb_status trb_render_aov_lum_device(trb_scene* scene, const trb_render_cfg* cfg, float* d_film_rgbw, const trb_aov_film* d_aov, float* d_lum_w,
+                                     trb_stats* d_stats, void* cuda_stream);
+
+/* Denoise one film with its lum_w film: HOST inputs and outputs (rgbw required, width*height*4 floats, overwritten; variance may be
+ * NULL), staged per call; blocking. The parameters are trb_denoise's, checked first (no scene is needed to refuse them); then
+ * TRB_INVALID_ARG for a null scene, input member, lum_w or rgbw, or an output overlapping an input or the other output; TRB_OOM when
+ * the scratch does not fit. */
+trb_status trb_denoise_variance(trb_scene* scene, const trb_denoise_frame* in, const float* lum_w, const trb_denoise_params* params,
+                                float* out_rgbw, float* out_variance);
+/* The same with DEVICE buffers (films, lum_w and rgbw 16-byte, nearest 8-byte, variance 4-byte aligned; TRB_INVALID_ARG otherwise),
+ * enqueued on cuda_stream under trb_render_device's one-stream rule: 1 + iterations kernel launches. No host synchronisation, except
+ * once when the scratch grows. */
+trb_status trb_denoise_variance_device(trb_scene* scene, const trb_denoise_frame* d_in, const float* d_lum_w, const trb_denoise_params* params,
+                                       float* d_out_rgbw, float* d_out_variance, void* cuda_stream);
+
 /* -- Moment gradients: temporal gradients on the moment denoiser, so a 1-spp history drops where the lighting changed -------------
  * (DESIGN.md §4 "Moment gradients"). A-SVGF (Schied, Peters, Dachsbacher 2018) is SVGF at one sample per pixel with temporal
  * gradients: "Moment denoising" with the lambda of "Temporal gradients". Per call:
@@ -1220,6 +1268,15 @@ trb_status trb_render_adaptive_aov_device(trb_scene* scene, const trb_render_cfg
  * trb_render_samples_adaptive's. Does not update the frame. */
 trb_status trb_render_samples_adaptive_aov(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, size_t n,
                                            trb_sample* samples, trb_aov_sample* aov, uint32_t* pixel_spp, trb_stats* stats);
+
+/* trb_render_adaptive_aov with the HOST lum_w film of "Sample variance" (width*height*4 floats, added into; required): the film,
+ * AOVs, pixel_spp, counters and statuses are trb_render_adaptive_aov's. */
+trb_status trb_render_adaptive_aov_lum(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                                       const trb_aov_film* aov, float* lum_w, uint32_t* pixel_spp, trb_stats* stats);
+/* trb_render_adaptive_aov_device with the DEVICE lum_w film (16-byte aligned, else TRB_INVALID_ARG). */
+trb_status trb_render_adaptive_aov_lum_device(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* d_film_rgbw,
+                                              const trb_aov_film* d_aov, float* d_lum_w, uint32_t* d_pixel_spp, trb_stats* d_stats,
+                                              void* cuda_stream);
 
 /* trb_render_sharded with the Adaptive sampler: this rank's shard (interleaved chunks, or the reference's contiguous
  * ranges with cfg->shard_count == 0xffffffff) runs the Adaptive rounds into the device film, then ONE reduce to `root`,

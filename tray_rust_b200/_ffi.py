@@ -324,6 +324,8 @@ TRB_SYMBOLS = [
     "trb_denoise_moments", "trb_denoise_moments_device", "trb_denoise_moments_gradient", "trb_denoise_moments_gradient_device",
     "trb_render_adaptive_aov", "trb_render_adaptive_aov_device", "trb_render_samples_adaptive_aov",
     "trb_render_sharded_aov", "trb_render_sharded_adaptive_aov", "trb_group_render_aov", "trb_group_render_adaptive_aov",
+    "trb_render_aov_lum", "trb_render_aov_lum_device", "trb_render_adaptive_aov_lum", "trb_render_adaptive_aov_lum_device",
+    "trb_denoise_variance", "trb_denoise_variance_device",
 ]
 
 _trb = None
@@ -420,6 +422,12 @@ def load_trb():
     lib.trb_render_adaptive_aov.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_aov_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, vp]
     lib.trb_render_samples_adaptive_aov.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), sz, vp, vp, vp, C.POINTER(Stats)]
+    lib.trb_render_aov_lum.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, C.POINTER(Stats)]
+    lib.trb_render_aov_lum_device.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp, vp]
+    lib.trb_render_adaptive_aov_lum.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, C.POINTER(Stats)]
+    lib.trb_render_adaptive_aov_lum_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, vp, vp]
+    lib.trb_denoise_variance.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp]
+    lib.trb_denoise_variance_device.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp, vp]
     lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
     lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]

@@ -260,14 +260,16 @@ def _render_denoised_adaptive(render_adaptive_aov, denoiser, history, min_spp, m
     return out, film, aovs, pixel_spp, st
 
 
-def _aov_outputs(height, width, film, albedo, normal, nearest):
-    """The host film and AOV arrays of the AOV renders (Scene and Group), checked or allocated: (film, aovs, AovFilm)."""
+def _aov_outputs(height, width, film, albedo, normal, nearest, lum=False):
+    """The host film and AOV arrays of the AOV renders (Scene and Group), checked or allocated: (film, aovs, AovFilm). aovs holds
+    "lum_w" too when `lum` asks for it."""
     if film is None:
         film = np.zeros((height, width, 4), np.float32)
     aovs = {}
     for name, a, shape, dtype, fill in (("albedo_w", albedo, (height, width, 4), np.float32, 0),
                                         ("normal_w", normal, (height, width, 4), np.float32, 0),
-                                        ("nearest", nearest, (height, width), np.uint64, np.iinfo(np.uint64).max)):
+                                        ("nearest", nearest, (height, width), np.uint64, np.iinfo(np.uint64).max),
+                                        ("lum_w", lum, (height, width, 4), np.float32, 0)):
         if a is True:
             a = np.full(shape, fill, dtype)
         if a is None or a is False:
@@ -330,24 +332,32 @@ class Scene(_Base):
         cfg = _cfg(**kw)
         self._check(self._lib.trb_render_device(self._h, C.byref(cfg), d_film_ptr, d_stats_ptr, stream))
 
-    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, **kw):
+    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, lum=False, **kw):
         """trb_render_aov: the colour film and the AOVs of the same render (DESIGN.md §4 "AOVs"), all accumulated into.
         albedo / normal: True (allocate, zero), False / None (not rendered) or a float32 (height, width, 4) film; nearest: True
-        (allocate, all ones), False / None or a uint64 (height, width) array. Returns (film, aovs, Stats) where aovs maps "albedo_w",
-        "normal_w" and "nearest" to the arrays rendered."""
+        (allocate, all ones), False / None or a uint64 (height, width) array. lum: True or a float32 (height, width, 4) film adds
+        the lum_w film of the samples' luminance moments (trb_render_aov_lum, DESIGN.md §4 "Sample variance") as aovs["lum_w"].
+        Returns (film, aovs, Stats) where aovs maps "albedo_w", "normal_w" and "nearest" to the arrays rendered."""
         cfg = _cfg(**kw)
-        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest, lum)
         st = F.Stats()
-        self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
+        if "lum_w" in aovs:
+            self._check(self._lib.trb_render_aov_lum(self._h, C.byref(cfg), F.ptr(film), C.byref(out), F.ptr(aovs["lum_w"]), C.byref(st)))
+        else:
+            self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
         return film, aovs, st
 
-    def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, **kw):
+    def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, d_lum=None, **kw):
         """trb_render_aov_device: device films of height*width*4 float32 (16-byte aligned) and a device nearest buffer of height*width
         uint64 (8-byte aligned; initialise it to all ones), pointers as ints, any AOV None. Enqueued on `stream` (a cudaStream_t as an
-        int; None = default stream) without host synchronisation. Never updates the frame."""
+        int; None = default stream) without host synchronisation. Never updates the frame. d_lum: a device lum_w film
+        (trb_render_aov_lum_device), or None."""
         cfg = _cfg(**kw)
         out = F.AovFilm(d_albedo, d_normal, d_nearest)
-        self._check(self._lib.trb_render_aov_device(self._h, C.byref(cfg), d_film, C.byref(out), d_stats, stream))
+        if d_lum is not None:
+            self._check(self._lib.trb_render_aov_lum_device(self._h, C.byref(cfg), d_film, C.byref(out), d_lum, d_stats, stream))
+        else:
+            self._check(self._lib.trb_render_aov_device(self._h, C.byref(cfg), d_film, C.byref(out), d_stats, stream))
 
     def render_samples_aov(self, **kw):
         """trb_render_samples_aov: (samples as render_samples, AOV records as AOV_SAMPLE_DTYPE in the same order, Stats)."""
@@ -560,6 +570,51 @@ class Scene(_Base):
         denoise={"max_history": 1}. Returns (denoised, film, aovs, pixel_spp, stats)."""
         return _render_denoised_adaptive(self.render_adaptive_aov, self, history, min_spp, max_spp, seed, current_frame, denoise, gradients, kw)
 
+    def denoise_variance(self, colour, aovs, out=None, variance=False, **params):
+        """trb_denoise_variance (DESIGN.md §4 "Sample variance"): one colour film, (height, width, 4) float32, denoised with the
+        variance of each pixel's own samples. aovs: render_aov(lum=True)'s dict ("albedo_w", "normal_w", "nearest" and "lum_w").
+        params: denoise's. Returns the denoised RGBW film (into `out` when given), or a tuple of it and the (height, width) float32
+        variance where asked for (True, or an array)."""
+        h, w = self.height, self.width
+        film_shape = (h, w, 4)
+        ins = [("colour", colour, film_shape, np.float32), ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32),
+               ("normal_w", aovs.get("normal_w"), film_shape, np.float32), ("nearest", aovs.get("nearest"), (h, w), np.uint64),
+               ("lum_w", aovs.get("lum_w"), film_shape, np.float32)]
+        outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
+        if variance is True:
+            variance = np.zeros((h, w), np.float32)
+        if variance is not False and variance is not None:
+            outs.append(("variance", variance, (h, w), np.float32))
+        for name, a, shape, dtype in ins + outs:
+            if not isinstance(a, np.ndarray) or a.dtype != dtype or a.shape != shape or not a.flags.c_contiguous:
+                raise ValueError("%s must be a C-contiguous %s array of shape %s" % (name, np.dtype(dtype).name, shape))
+        d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins[:4])), _denoise_params(params)
+        self._check(self._lib.trb_denoise_variance(self._h, C.byref(d_in), ins[4][1].ctypes.data, C.byref(prm), outs[0][1].ctypes.data,
+                                                   outs[1][1].ctypes.data if len(outs) > 1 else None))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_variance_device(self, d_colour, d_albedo, d_normal, d_nearest, d_lum, d_out, d_variance=None, stream=None, **params):
+        """trb_denoise_variance_device: device pointers as ints (d_colour, d_albedo, d_normal, d_lum and d_out height*width*4
+        float32, 16-byte aligned; d_nearest height*width uint64, 8-byte aligned; d_variance height*width float32, 4-byte aligned, or
+        None), enqueued on `stream`. params as for denoise."""
+        d_in, prm = F.DenoiseFrame(d_colour, d_albedo, d_normal, d_nearest), _denoise_params(params)
+        self._check(self._lib.trb_denoise_variance_device(self._h, C.byref(d_in), d_lum, C.byref(prm), d_out, d_variance, stream))
+
+    def render_denoised_variance(self, spp=0, adaptive=None, denoise=None, **kw):
+        """A still frame rendered once with the AOVs and the lum_w film, and denoised by denoise_variance with the parameters in the
+        dict `denoise` (None: the defaults): by render_aov at `spp` samples per pixel (0: the scene's), or with adaptive=(min_spp,
+        max_spp) by render_adaptive_aov. kw: the render's (seed, current_frame, flags, block_start, block_count). Returns (denoised,
+        film, aovs, stats), with pixel_spp before stats for an Adaptive render."""
+        if adaptive is not None:
+            if spp:
+                raise ValueError("render_denoised_variance: the Adaptive sampler chooses the sample counts; spp is not taken")
+            film, aovs, pixel_spp, st = self.render_adaptive_aov(adaptive[0], adaptive[1], lum=True, **kw)
+            return self.denoise_variance(film, aovs, **(denoise or {})), film, aovs, pixel_spp, st
+        film, aovs, st = self.render_aov(lum=True, spp=spp, **kw)
+        return self.denoise_variance(film, aovs, **(denoise or {})), film, aovs, st
+
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:
         samples [0, spp/2) and [spp/2, spp) are rendered into two films by render_aov, with the albedo, normal and nearest AOVs
@@ -768,25 +823,36 @@ class Scene(_Base):
                                                           C.byref(st)))
         return out, spp, st
 
-    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, **kw):
+    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, lum=False, **kw):
         """trb_render_adaptive_aov: render_adaptive with the AOVs of the samples it takes (DESIGN.md §4 "Adaptive AOVs"), all
-        accumulated into; albedo / normal / nearest as for render_aov. Returns (film, aovs, pixel_spp, Stats)."""
+        accumulated into; albedo / normal / nearest / lum as for render_aov (lum: trb_render_adaptive_aov_lum). Returns (film, aovs,
+        pixel_spp, Stats)."""
         cfg = _cfg(**kw)
-        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest)
+        film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest, lum)
         spp = np.zeros((self.height, self.width), np.uint32)
         st = F.Stats()
-        self._check(self._lib.trb_render_adaptive_aov(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), F.ptr(film), C.byref(out),
-                                                      F.ptr(spp), C.byref(st)))
+        ad = F.Adaptive(min_spp, max_spp)
+        if "lum_w" in aovs:
+            self._check(self._lib.trb_render_adaptive_aov_lum(self._h, C.byref(cfg), C.byref(ad), F.ptr(film), C.byref(out), F.ptr(aovs["lum_w"]),
+                                                              F.ptr(spp), C.byref(st)))
+        else:
+            self._check(self._lib.trb_render_adaptive_aov(self._h, C.byref(cfg), C.byref(ad), F.ptr(film), C.byref(out), F.ptr(spp), C.byref(st)))
         return film, aovs, spp, st
 
     def render_adaptive_aov_device(self, min_spp, max_spp, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_pixel_spp=None, d_stats=None,
-                                   stream=None, **kw):
+                                   stream=None, d_lum=None, **kw):
         """trb_render_adaptive_aov_device: render_adaptive_device's pointers plus the AOV buffers of render_aov_device (any None).
-        Enqueued on `stream` without host synchronisation. Never updates the frame."""
+        Enqueued on `stream` without host synchronisation. Never updates the frame. d_lum: a device lum_w film
+        (trb_render_adaptive_aov_lum_device), or None."""
         cfg = _cfg(**kw)
         out = F.AovFilm(d_albedo, d_normal, d_nearest)
-        self._check(self._lib.trb_render_adaptive_aov_device(self._h, C.byref(cfg), C.byref(F.Adaptive(min_spp, max_spp)), d_film, C.byref(out),
-                                                             d_pixel_spp, d_stats, stream))
+        ad = F.Adaptive(min_spp, max_spp)
+        if d_lum is not None:
+            self._check(self._lib.trb_render_adaptive_aov_lum_device(self._h, C.byref(cfg), C.byref(ad), d_film, C.byref(out), d_lum, d_pixel_spp,
+                                                                     d_stats, stream))
+        else:
+            self._check(self._lib.trb_render_adaptive_aov_device(self._h, C.byref(cfg), C.byref(ad), d_film, C.byref(out), d_pixel_spp, d_stats,
+                                                                 stream))
 
     def render_samples_adaptive_aov(self, min_spp, max_spp, **kw):
         """trb_render_samples_adaptive_aov: (samples as render_samples_adaptive, AOV records as AOV_SAMPLE_DTYPE in the same layout,

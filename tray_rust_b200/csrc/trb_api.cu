@@ -623,8 +623,8 @@ trb_status launch_render_t(trb_scene* s, const trb::RenderParams& rp, uint32_t f
     return TRB_OK;
 }
 // The AOVs a render asks for (DESIGN.md §4 "AOVs"): samples = the caller's device records (per-sample mode), else the film outputs
-// (any may be nullptr)
-struct AovRequest { trb_aov_sample* samples; float4* albedo_w; float4* normal_w; unsigned long long* nearest; };
+// (any may be nullptr); lum_w: the sample-variance film of the *_lum renders (include/trb.h "Sample variance")
+struct AovRequest { trb_aov_sample* samples; float4* albedo_w; float4* normal_w; unsigned long long* nearest; float4* lum_w = nullptr; };
 
 // the path-indexed AOV records of film passes, at the path-state capacity
 trb_status ensure_aov(trb_scene* s) {
@@ -907,6 +907,15 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
                     else trb::k_wf_film<true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
                 } else if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
                 else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                g_launches++;
+            }
+            if (aov->lum_w) { // the colour film's kernel once more, over the radiance and the records' albedo half together
+                ra.film = aov->lum_w;
+                if (rp.ad_state) {
+                    if (tu.film_v2) trb::k_wf_film_v2<true, true><<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wf, s->d_aov);
+                    else trb::k_wf_film<true, true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wf, s->d_aov);
+                } else if (tu.film_v2) trb::k_wf_film_v2<false, true><<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wf, s->d_aov);
+                else trb::k_wf_film<false, true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wf, s->d_aov);
                 g_launches++;
             }
             if (aov->nearest) {
@@ -2740,16 +2749,18 @@ void add_film(float* film, const float* src, size_t n) {
 }
 
 // The device side of a host AOV render (trb_render_aov, trb_render_adaptive_aov): films from zero, added into the caller's
-// afterwards; nearest from the caller's
+// afterwards; nearest from the caller's. lum_w (the *_lum renders): the lum_w film, staged as albedo_w and normal_w.
 struct HostAov {
-    DeviceBuffer albedo, normal, nearest;
+    DeviceBuffer albedo, normal, nearest, lum;
     AovRequest req{nullptr, nullptr, nullptr, nullptr};
     const trb_aov_film* aov = nullptr; // nullptr: no AOV output asked for
-    trb_status stage(const trb_aov_film* a, size_t npx) {
-        if (!a || !(a->albedo_w || a->normal_w || a->nearest)) return TRB_OK;
+    float* lum_w = nullptr;
+    trb_status stage(const trb_aov_film* a, size_t npx, float* lum_host = nullptr) {
+        if (!a || !(a->albedo_w || a->normal_w || a->nearest || lum_host)) return TRB_OK;
         aov = a;
+        lum_w = lum_host;
         trb_status r;
-        for (auto [h, d] : {std::pair<const float*, DeviceBuffer*>{a->albedo_w, &albedo}, {a->normal_w, &normal}}) {
+        for (auto [h, d] : {std::pair<const float*, DeviceBuffer*>{a->albedo_w, &albedo}, {a->normal_w, &normal}, {lum_host, &lum}}) {
             if (!h) continue;
             if ((r = d->alloc(npx * sizeof(float4), "AOV films")) != TRB_OK) return r;
             CU(cudaMemsetAsync(d->p, 0, npx * sizeof(float4), 0));
@@ -2758,14 +2769,15 @@ struct HostAov {
             if ((r = nearest.alloc(npx * sizeof(uint64_t), "AOV films")) != TRB_OK) return r;
             CU(cudaMemcpy(nearest.p, a->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice));
         }
-        req = {nullptr, albedo.as<float4>(), normal.as<float4>(), nearest.as<unsigned long long>()};
+        req = {nullptr, albedo.as<float4>(), normal.as<float4>(), nearest.as<unsigned long long>(), lum.as<float4>()};
         return TRB_OK;
     }
     const AovRequest* request() const { return aov ? &req : nullptr; }
     trb_status unstage(size_t npx) {
         if (!aov) return TRB_OK;
         std::vector<float> h;
-        for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, albedo.p}, std::pair<float*, void*>{aov->normal_w, normal.p}}) {
+        for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, albedo.p}, std::pair<float*, void*>{aov->normal_w, normal.p},
+                                std::pair<float*, void*>{lum_w, lum.p}}) {
             if (!dst) continue;
             h.resize(npx * 4);
             CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -2777,7 +2789,7 @@ struct HostAov {
 };
 
 // trb_render's body; aov: the host AOV outputs of trb_render_aov (nullptr: none)
-trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats) {
+trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats, float* lum_w = nullptr) {
     CU(cudaSetDevice(s->device));
     float update_ms = 0.f;
     if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) { // Exec::render: scene.update_frame first (multithreaded.rs:57-60)
@@ -2791,7 +2803,7 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     HostAov ha;
-    trb_status r = ha.stage(aov, npx);
+    trb_status r = ha.stage(aov, npx, lum_w);
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, ha.request());
@@ -2872,6 +2884,27 @@ trb_status trb_render_samples_aov(trb_scene* s, const trb_render_cfg* cfg, size_
     const trb_status r = aov_supported(s, cfg);
     if (r != TRB_OK) return r;
     return render_samples(s, cfg, n, samples, aov, stats);
+}
+
+trb_status trb_render_aov_lum_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, const trb_aov_film* d_aov, float* d_lum_w, trb_stats* d_stats,
+                                     void* stream) {
+    if (!s || !cfg || !d_film || !d_aov || !d_lum_w) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    trb_status r = aov_supported(s, cfg);
+    if (r == TRB_OK)
+        r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_lum_w, 16}, {d_aov->nearest, 8}},
+                          "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    if (r != TRB_OK) return r;
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest), reinterpret_cast<float4*>(d_lum_w)};
+    return render_device(s, cfg, d_film, d_stats, static_cast<cudaStream_t>(stream), &req);
+}
+
+trb_status trb_render_aov_lum(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, float* lum_w, trb_stats* stats) {
+    if (!s || !cfg || !film || !aov || !lum_w) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_status r = aov_supported(s, cfg);
+    if (r != TRB_OK) return r;
+    return render_host(s, cfg, film, aov, stats, lum_w);
 }
 
 namespace {
@@ -2973,6 +3006,67 @@ trb_status trb_denoise(trb_scene* s, const trb_denoise_input* in, const trb_deno
                       [&](const DeviceBuffer* d) {
                           const trb_denoise_input d_in{d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<float>(), d[4].as<uint64_t>()};
                           return denoise_enqueue(s, prm, d_in, d[5].as<float>(), 0);
+                      });
+}
+
+// ---- sample-variance denoising (include/trb.h "Sample variance", DESIGN.md §4) -----------------------------------------------------
+namespace {
+// The checks of both forms: parameters, null pointers, an output overlapping an input or the other output
+trb_status variance_check(const trb_scene* s, const trb_denoise_frame* in, const float* lum_w, const trb_denoise_params* params, const float* rgbw,
+                          const float* variance, trb::DnParams& prm) {
+    const trb_status r = denoise_params(params, prm);
+    if (r != TRB_OK) return r;
+    if (!s || !in || !lum_w || !rgbw || !in->colour || !in->albedo_w || !in->normal_w || !in->nearest) return fail(TRB_INVALID_ARG, "null argument");
+    prm.width = (int)s->film.width; prm.height = (int)s->film.height;
+    const size_t npx = (size_t)s->film.width * s->film.height, fb = npx * sizeof(float4);
+    for (const Span o : {Span{rgbw, fb}, Span{variance, npx * sizeof(float)}})
+        if (overlaps_any(o, {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}, {lum_w, fb}}))
+            return fail(TRB_INVALID_ARG, "the denoise output overlaps an input");
+    if (spans_overlap({rgbw, fb}, {variance, npx * sizeof(float)})) return fail(TRB_INVALID_ARG, "the denoise outputs overlap");
+    return TRB_OK;
+}
+
+// k_dn_variance_prepare and the N a-trous launches on `st`
+trb_status variance_enqueue(trb_scene* s, const trb::DnParams& prm, const trb_denoise_frame& in, const float* lum_w, float* d_rgbw, float* d_var,
+                            cudaStream_t st) {
+    const size_t npx = (size_t)prm.width * prm.height;
+    if (npx == 0) return TRB_OK;
+    trb::DnScratch sc;
+    const trb_status r = denoise_scratch(s, npx, sc);
+    if (r != TRB_OK) return r;
+    float4* out = reinterpret_cast<float4*>(d_rgbw);
+    const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    trb::k_dn_variance_prepare<<<grid, block, 0, st>>>(prm, reinterpret_cast<const float4*>(in.colour), reinterpret_cast<const float4*>(lum_w),
+                                                       reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
+                                                       reinterpret_cast<const unsigned long long*>(in.nearest), sc, out, d_var);
+    g_launches++;
+    CU(cudaGetLastError());
+    return denoise_atrous(prm, sc, out, st);
+}
+} // namespace
+
+trb_status trb_denoise_variance_device(trb_scene* s, const trb_denoise_frame* d_in, const float* d_lum_w, const trb_denoise_params* params, float* d_rgbw,
+                                       float* d_variance, void* stream) {
+    trb::DnParams prm{};
+    trb_status r = variance_check(s, d_in, d_lum_w, params, d_rgbw, d_variance, prm);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_lum_w, 16}, {d_rgbw, 16}, {d_in->nearest, 8}, {d_variance, 4}},
+                          "device films must be 16-byte aligned, the nearest buffer 8-byte aligned, variance 4-byte aligned");
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    return variance_enqueue(s, prm, *d_in, d_lum_w, d_rgbw, d_variance, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_denoise_variance(trb_scene* s, const trb_denoise_frame* in, const float* lum_w, const trb_denoise_params* params, float* rgbw, float* variance) {
+    trb::DnParams prm{};
+    trb_status r = variance_check(s, in, lum_w, params, rgbw, variance, prm);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    return run_staged({{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}, {lum_w, fb}},
+                      {{rgbw, fb}, {variance, npx * sizeof(float)}}, [&](const DeviceBuffer* d) {
+                          return variance_enqueue(s, prm, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()}, d[4].as<float>(),
+                                                  d[5].as<float>(), d[6].as<float>(), 0);
                       });
 }
 
@@ -3592,7 +3686,7 @@ trb_status trb_host_adaptive_decide(const trb_adaptive* ad, const float* lum, si
 namespace {
 // trb_render_adaptive's body; aov: the host AOV outputs of trb_render_adaptive_aov (nullptr: none)
 trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, uint32_t* pixel_spp,
-                                trb_stats* stats) {
+                                trb_stats* stats, float* lum_w = nullptr) {
     trbh::AdSchedule sch;
     trb_status r = adaptive_check(s, cfg, ad, sch);
     if (r != TRB_OK) return r;
@@ -3614,7 +3708,7 @@ trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const t
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     HostAov ha;
-    if ((r = ha.stage(aov, npx)) != TRB_OK) return r;
+    if ((r = ha.stage(aov, npx, lum_w)) != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     if (nb) { // an empty selection renders nothing (block_queue.rs:42-44)
         r = ensure_adaptive(s);
@@ -3718,6 +3812,23 @@ trb_status trb_render_adaptive_aov_device(trb_scene* s, const trb_render_cfg* cf
                          reinterpret_cast<unsigned long long*>(d_aov->nearest)};
     const bool with_aov = d_aov->albedo_w || d_aov->normal_w || d_aov->nearest;
     return render_adaptive_device(s, cfg, ad, d_film, with_aov ? &req : nullptr, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_render_adaptive_aov_lum(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, float* lum_w,
+                                       uint32_t* pixel_spp, trb_stats* stats) {
+    if (!s || !cfg || !ad || !film || !aov || !lum_w) return fail(TRB_INVALID_ARG, "null argument");
+    return render_adaptive_host(s, cfg, ad, film, aov, pixel_spp, stats, lum_w);
+}
+
+trb_status trb_render_adaptive_aov_lum_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, const trb_aov_film* d_aov,
+                                              float* d_lum_w, uint32_t* d_pixel_spp, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !ad || !d_film || !d_aov || !d_lum_w) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_status r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_lum_w, 16}, {d_aov->nearest, 8}},
+                                       "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    if (r != TRB_OK) return r;
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest), reinterpret_cast<float4*>(d_lum_w)};
+    return render_adaptive_device(s, cfg, ad, d_film, &req, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
 }
 
 trb_status trb_render_samples_adaptive_aov(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, size_t n, trb_sample* samples, trb_aov_sample* aov,

@@ -4,7 +4,8 @@
 // iteration, ping-ponging two (e, v) buffers, and the last one remodulates into the output film; k_dn_temporal takes k_dn_prepare's place
 // for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer; k_dn_temporal_moments and
 // k_dn_moments_variance take it for trb_denoise_moments* (k_dn_temporal_moments_grad for trb_denoise_moments_gradient*), one film with
-// the variance from luminance moments. Float32 in the header's order, no
+// the variance from luminance moments; k_dn_variance_prepare takes it for trb_denoise_variance*, one film with the variance of
+// its own samples (the lum_w film). Float32 in the header's order, no
 // atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
 #pragma once
 #include "trb_detmath.cuh"
@@ -49,6 +50,42 @@ __device__ __forceinline__ float dn_grad(float z, bool has_lo, float zlo, bool h
     return 0.0f;
 }
 
+// trb_denoise's pixel from m on, once c, the albedo a, d, e and v are known (shared by k_dn_prepare and k_dn_variance_prepare): m, len2
+// and z, the copy-through test, then the guide, gradient, divisor and first (e, v) records. Returns whether p is filtered. prm and sc
+// are taken by value, as the kernels hold them.
+__device__ __forceinline__ bool dn_prepare_px(const DnParams prm, int x, int y, int i, float c0, float c1, float c2, float a0, float a1, float a2,
+                                              float d0, float d1, float d2, float e0, float e1, float e2, float v, float4 nw,
+                                              const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out) {
+    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
+    const float z = dn_depth(nearest, i);
+    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
+                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && dn_finite(v) &&
+                    z == z && z != __int_as_float(0xff800000);
+    if (!ok) {
+        out[i] = dn_out(c0, c1, c2, 1.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        return false;
+    }
+    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    if (len2 != 0.0f) {
+        const float l = sqrtf(len2);
+        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    }
+    float gx = 0.0f, gy = 0.0f;
+    if (dn_finite(z)) {
+        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
+        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
+        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
+    }
+    sc.guide[i] = make_float4(n0, n1, n2, z);
+    sc.grad[i] = make_float2(gx, gy);
+    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
+    sc.ev[0][i] = make_float4(e0, e1, e2, v);
+    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+    return true;
+}
+
 __global__ void __launch_bounds__(256) k_dn_prepare(const DnParams prm, const float4* __restrict__ ca, const float4* __restrict__ cb,
                                                     const float4* __restrict__ alb, const float4* __restrict__ nrm,
                                                     const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out) {
@@ -71,33 +108,42 @@ __global__ void __launch_bounds__(256) k_dn_prepare(const DnParams prm, const fl
     const float la = dn_lum(A.x / A.w / d0, A.y / A.w / d1, A.z / A.w / d2), lb = dn_lum(B.x / B.w / d0, B.y / B.w / d1, B.z / B.w / d2);
     const float dl = la - lb;
     const float v = dl * dl * 0.25f;
-    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
-    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
-    const float z = dn_depth(nearest, i);
-    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
-                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && dn_finite(v) &&
-                    z == z && z != __int_as_float(0xff800000);
-    if (!ok) {
-        out[i] = dn_out(c0, c1, c2, 1.0f);
+    dn_prepare_px(prm, x, y, i, c0, c1, c2, a0, a1, a2, d0, d1, d2, e0, e1, e2, v, nw, nearest, sc, out);
+}
+
+// trb_denoise_variance's k_dn_prepare (include/trb.h "Sample variance"): one film, and v from the pixel's own samples in lum_w.
+// Writes the same scratch, and var (may be null) receives v, NaN where the pixel is not filtered.
+__global__ void __launch_bounds__(256) k_dn_variance_prepare(const DnParams prm, const float4* __restrict__ col, const float4* __restrict__ lum,
+                                                             const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                             const unsigned long long* __restrict__ nearest, DnScratch sc, float4* __restrict__ out,
+                                                             float* __restrict__ var) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int i = y * prm.width + x;
+    const float qnan = __int_as_float(0x7fffffff);
+    const float4 A = col[i];
+    const float W = A.w;
+    if (W <= 0.0f) {
+        out[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        if (var) var[i] = qnan;
         return;
     }
-    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
-    if (len2 != 0.0f) {
-        const float l = sqrtf(len2);
-        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    const float c0 = A.x / W, c1 = A.y / W, c2 = A.z / W;
+    const float4 al = alb[i], nw = nrm[i], lw = lum[i];
+    const float a0 = al.x / al.w, a1 = al.y / al.w, a2 = al.z / al.w;
+    const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
+    const float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
+    const float V1 = lw.w, V2 = lw.z;
+    float v = qnan; // at most one effective sample
+    if (V1 > 0.0f && V1 * V1 > V2) {
+        const float m1 = lw.x / V1, m2 = lw.y / V1;
+        const float s = m2 - m1 * m1;
+        v = (s > 0.0f ? s : 0.0f) * V2 / (V1 * V1 - V2);
     }
-    float gx = 0.0f, gy = 0.0f;
-    if (dn_finite(z)) {
-        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
-        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
-        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
-    }
-    sc.guide[i] = make_float4(n0, n1, n2, z);
-    sc.grad[i] = make_float2(gx, gy);
-    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
-    sc.ev[0][i] = make_float4(e0, e1, e2, v);
-    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+    const bool filtered = dn_prepare_px(prm, x, y, i, c0, c1, c2, a0, a1, a2, d0, d1, d2, e0, e1, e2, v, nw, nearest, sc, out);
+    if (var) var[i] = filtered ? v : qnan;
 }
 
 // One a-trous iteration at step s from ev_in to ev_out, or, the last one, remodulated into out (ev_out unused)

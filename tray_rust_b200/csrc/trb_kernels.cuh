@@ -1661,6 +1661,8 @@ __device__ __forceinline__ bool lock_block_takes(float s, int i, int lo, int hi,
     return s >= (float)(w0 - fpw) && s < (float)(w1 + fpw);
 }
 
+// LUM: the lum_w film's sums (include/trb.h "Sample variance"): c = (l, l * l, unused) and the third channel takes w * w
+template <bool LUM = false>
 __device__ __forceinline__ void splat_sample(const DScene& sc, float4* tile, const float* s_table, int T, int tx0, int ty0, int x_lo, int x_hi, int y_lo,
                                              int y_hi, uint32_t px, uint32_t py, float sx, float sy, f3 c) {
     const float img_x = sx - 0.5f, img_y = sy - 0.5f;
@@ -1682,7 +1684,7 @@ __device__ __forceinline__ void splat_sample(const DScene& sc, float4* tile, con
             float* t = reinterpret_cast<float*>(&tile[(iy - ty0) * T + (ix - tx0)]);
             atomicAdd(t + 0, wgt * c.x);
             atomicAdd(t + 1, wgt * c.y);
-            atomicAdd(t + 2, wgt * c.z);
+            atomicAdd(t + 2, LUM ? wgt * wgt : wgt * c.z);
             atomicAdd(t + 3, wgt);
         }
     }
@@ -2696,9 +2698,21 @@ __global__ void __launch_bounds__(128, MINB) k_wf_shade_c(const __grid_constant_
     }
 }
 
+// The per-sample value of the lum_w film (include/trb.h "Sample variance"): l = L(c / max(a, TRB_DENOISE_EPS_ALBEDO)) of the sample's
+// radiance c and the albedo a of its AOV record, as (l, l * l, 0)
+__device__ __forceinline__ f3 lum_sample(float4 c, float4 a) {
+    const float d0 = a.x > TRB_DENOISE_EPS_ALBEDO ? a.x : TRB_DENOISE_EPS_ALBEDO, d1 = a.y > TRB_DENOISE_EPS_ALBEDO ? a.y : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a.z > TRB_DENOISE_EPS_ALBEDO ? a.z : TRB_DENOISE_EPS_ALBEDO;
+    const float l = 0.2126f * (c.x / d0) + 0.7152f * (c.y / d1) + 0.0722f * (c.z / d2);
+    return mk(l, l * l, 0.0f);
+}
+
 // RenderTarget::write for a whole pass: one CTA per 8x8 block, footprint accumulated in shared memory.
-template <bool ADAPT = false>
-__global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
+// LUM: the lum_w film instead of the colour film, from the radiance (wf.rad) and the albedo half of each sample's AOV record (alb,
+// indexed like wf.rad); the same weights, window and lock-block rule, with (w l, w l^2, w^2, w) in place of (w c, w).
+template <bool ADAPT = false, bool LUM = false>
+__global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
+                                                            const float4* __restrict__ alb = nullptr) {
     extern __shared__ float4 tile[];
     __shared__ float s_table[256];
     const int T = 9 + 2 * max(sc.fpw_x, sc.fpw_y);
@@ -2723,8 +2737,10 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film(const __grid_constan
             float sx, sy, tm;
             if (ADAPT) sample_position_ad(rp, ps, id, sx, sy, tm);
             else sample_position(rp, ps, id, sx, sy, tm);
-            const float4 c4 = wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s];
-            splat_sample(sc, tile, s_table, T, tx0, ty0, x_lo, x_hi, y_lo, y_hi, id.px, id.py, sx, sy, mk(c4.x, c4.y, c4.z));
+            const size_t p = ((size_t)item * 64 + pix) * rp.sample_count + s;
+            const float4 c4 = wf.rad[p];
+            if (LUM) splat_sample<true>(sc, tile, s_table, T, tx0, ty0, x_lo, x_hi, y_lo, y_hi, id.px, id.py, sx, sy, lum_sample(c4, alb[p]));
+            else splat_sample(sc, tile, s_table, T, tx0, ty0, x_lo, x_hi, y_lo, y_hi, id.px, id.py, sx, sy, mk(c4.x, c4.y, c4.z));
         }
         __syncthreads();
         for (int i = threadIdx.x; i < T * T; i += RENDER_THREADS) {
@@ -2831,8 +2847,10 @@ __global__ void __launch_bounds__(256) k_wf_nearest_ad(const __grid_constant__ D
 // in lockstep (same (dy, dx) offset at the same time, __syncwarp per offset), so their targets are always 32 different tile
 // pixels and a plain 16-byte read-modify-write is race-free; the four copies are summed at the flush. Same weights and
 // products as RenderTarget::write; only the order of the float additions differs (the film bar is an RMSE tolerance).
-template <bool ADAPT = false>
-__global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf) {
+// LUM: the lum_w film, as for k_wf_film.
+template <bool ADAPT = false, bool LUM = false>
+__global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_constant__ DScene sc, const __grid_constant__ RenderParams rp, const __grid_constant__ WfState wf,
+                                                               const float4* __restrict__ alb = nullptr) {
     extern __shared__ float4 tiles[]; // 4 x T*T
     __shared__ float s_table[256];
     const int T = 9 + 2 * max(sc.fpw_x, sc.fpw_y);
@@ -2861,7 +2879,11 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_cons
             float sx, sy, tm;
             if (ADAPT) sample_position_ad(rp, ps, id, sx, sy, tm);
             else sample_position(rp, ps, id, sx, sy, tm);
-            const float4 c4 = on ? wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s] : make_float4(0.f, 0.f, 0.f, 0.f);
+            float4 c4 = on ? wf.rad[((size_t)item * 64 + pix) * rp.sample_count + s] : make_float4(0.f, 0.f, 0.f, 0.f);
+            if (LUM && on) {
+                const f3 l = lum_sample(c4, alb[((size_t)item * 64 + pix) * rp.sample_count + s]);
+                c4 = make_float4(l.x, l.y, l.z, 0.f);
+            }
             const float img_x = sx - 0.5f, img_y = sy - 0.5f;
             for (int dy = -ry; dy <= ry + 1; ++dy) {
                 const int iy = (int)id.py + dy;
@@ -2877,7 +2899,7 @@ __global__ void __launch_bounds__(RENDER_THREADS) k_wf_film_v2(const __grid_cons
                         const float wgt = s_table[fyi * 16 + fxi];
                         float4* t = &mine[(iy - ty0) * T + (ix - tx0)];
                         float4 a = *t;
-                        a.x += wgt * c4.x; a.y += wgt * c4.y; a.z += wgt * c4.z; a.w += wgt;
+                        a.x += wgt * c4.x; a.y += wgt * c4.y; a.z += LUM ? wgt * wgt : wgt * c4.z; a.w += wgt;
                         *t = a;
                     }
                     __syncwarp(); // lockstep per offset: no lane starts (dy, dx + 1) before all finished (dy, dx)

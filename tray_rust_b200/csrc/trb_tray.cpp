@@ -1,7 +1,8 @@
 // trb_tray — the `tray_rust` program (src/main.rs) over the C ABI, with the reference's three modes:
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D | --devices LIST]
-//            [--denoise] [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--adaptive MIN MAX]
+//            [--denoise] [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--denoise-variance]
+//            [--adaptive MIN MAX]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]
 //
@@ -24,7 +25,9 @@
 // --denoise-moments, denoises with trb_denoise_moments_gradient at the frame's seed; --adaptive MIN MAX renders each frame with the
 // Adaptive sampler (trb_render_adaptive), or with --denoise-moments by trb_render_adaptive_aov and the moment call (single node, path
 // integrator; refused with --spp, since the sampler owns the schedule, and with --denoise, --denoise-temporal and --temporal-gradients,
-// which need two half sample ranges); --devices 0,1,2,3 renders each frame on a trb_group of those GPUs in place of one --device:
+// which need two half sample ranges); --denoise-variance renders each frame once with AOVs and the lum_w film (trb_render_aov_lum, or
+// with --adaptive trb_render_adaptive_aov_lum) and denoises it with trb_denoise_variance (single node on one GPU, path integrator, 2
+// samples per pixel or more, refused with the other denoise flags, --devices, --master and --worker); --devices 0,1,2,3 renders each frame on a trb_group of those GPUs in place of one --device:
 // plain and --adaptive frames by trb_group_render(_adaptive), every denoise mode by the group's AOV renders (trb_group_render_aov,
 // trb_group_render_adaptive_aov) and the denoise call on replica 0, which holds the history; with --worker the master's block range
 // is rendered by trb_group_render, in the same Frames (refused with --device, with --master, and for an empty, malformed or
@@ -52,7 +55,8 @@ namespace {
 const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N]\n"
-    "             [--device D | --devices LIST] [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]]\n"
+    "             [--device D | --devices LIST] [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]\n"
+    "             | --denoise-variance]\n"
     "             [--adaptive MIN MAX]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]\n"
@@ -82,6 +86,9 @@ const char* USAGE =
     "                          Single node only, path integrator.\n"
     "  --moment-gradients      With --denoise-moments only: re-shade a sample of each 3x3 pixel block of the previous frame in\n"
     "                          this one and shorten the moment history where the lighting changed. Single node only.\n"
+    "  --denoise-variance      Render each frame once with albedo, normal, depth and the luminance moments of its samples, and\n"
+    "                          denoise it with the variance of each pixel's own samples. Single node on one --device, path\n"
+    "                          integrator, at least 2 samples per pixel (with --adaptive: MIN at least 2).\n"
     "  --adaptive MIN MAX      Render with the Adaptive sampler: MIN samples per pixel, then more in rounds while a pixel's samples\n"
     "                          disagree, up to MAX (both rounded up to powers of two). With --denoise-moments each frame is also\n"
     "                          rendered with albedo, normal and depth and denoised by the moment denoiser.\n"
@@ -176,7 +183,8 @@ struct Args {
     std::vector<std::string> workers;
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
-         denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false, adaptive = false;
+         denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false, adaptive = false,
+         denoise_variance = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0, ad_min = 0, ad_max = 0;
     std::vector<int> devices; // --devices; empty: one --device
 };
@@ -272,6 +280,25 @@ struct MomentsFrame {
     }
 };
 
+// --denoise-variance: the frame's whole sample range into one film with its AOVs and the lum_w film, then trb_denoise_variance
+// (DESIGN.md §4 "Sample variance"); with ad, the Adaptive sampler's render (trb_render_adaptive_aov_lum) in place of LowDiscrepancy
+struct VarianceFrame {
+    std::vector<float> colour, albedo, normal, lum, out;
+    std::vector<uint64_t> nearest;
+    explicit VarianceFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), lum(npx * 4), out(npx * 4), nearest(npx) {}
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, const trb_adaptive* ad) {
+        for (std::vector<float>* v : {&colour, &albedo, &normal, &lum}) std::fill(v->begin(), v->end(), 0.0f);
+        std::fill(nearest.begin(), nearest.end(), ~0ull);
+        trb_render_cfg cfg{};
+        cfg.spp = ad ? 0 : spp; cfg.seed = seed; cfg.current_frame = frame;
+        const trb_aov_film aov{albedo.data(), normal.data(), nearest.data()};
+        if (ad) tray::check(trb_render_adaptive_aov_lum(s, &cfg, ad, colour.data(), &aov, lum.data(), nullptr, nullptr)); // includes Scene::update_frame
+        else tray::check(trb_render_aov_lum(s, &cfg, colour.data(), &aov, lum.data(), nullptr));
+        const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
+        tray::check(trb_denoise_variance(s, &in, lum.data(), nullptr, out.data(), nullptr));
+    }
+};
+
 // ---- single node (main.rs:56-109) -------------------------------------------------------------------------------------------
 int single_node(const Args& a, const OutPath& out) {
     Desc desc;
@@ -287,6 +314,10 @@ int single_node(const Args& a, const OutPath& out) {
         return die("--denoise-moments needs the path integrator: the scene's integrator renders no albedo, normal or depth");
     if (a.adaptive && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
         return die("--adaptive needs the path integrator: the Adaptive sampler is built for it only");
+    if (a.denoise_variance && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("--denoise-variance needs the path integrator: the scene's integrator renders no albedo, normal or depth");
+    if (a.denoise_variance && !a.adaptive && spp < 2)
+        return die("--denoise-variance needs at least 2 samples per pixel (a variance of one sample is undefined); the scene has %u", spp);
     const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
     try {
         std::unique_ptr<tray::Scene> one;
@@ -315,12 +346,18 @@ int single_node(const Args& a, const OutPath& out) {
         trb_denoise_history* history = nullptr;
         std::unique_ptr<MomentsFrame> mf;
         if (a.denoise_moments) mf.reset(new MomentsFrame((size_t)dim.first * dim.second));
+        std::unique_ptr<VarianceFrame> vf;
+        if (a.denoise_variance) vf.reset(new VarianceFrame((size_t)dim.first * dim.second));
         if (a.denoise_temporal || a.denoise_moments) tray::check(trb_denoise_history_create(rd.scene, &history));
         const std::unique_ptr<trb_denoise_history, trb_status (*)(trb_denoise_history*)> history_owner(history, trb_denoise_history_destroy);
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
             std::vector<uint8_t> img;
-            if (mf) {
+            if (vf) {
+                vf->render(rd.scene, spp, config.seed, (uint32_t)i, a.adaptive ? &ad : nullptr);
+                img.resize((size_t)dim.first * dim.second * 3);
+                tray::check(trb_film_to_srgb8(rd.scene, vf->out.data(), img.data()));
+            } else if (mf) {
                 mf->render(rd, spp, (uint32_t)(config.seed + i), (uint32_t)i, history, a.moment_gradients, a.adaptive ? &ad : nullptr);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(rd.scene, mf->out.data(), img.data()));
@@ -541,7 +578,7 @@ int master_node(const Args& a, const OutPath& out) {
 
 int main(int argc, char** argv) {
     bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false,
-         moment_gradients = false, adaptive = false;
+         moment_gradients = false, adaptive = false, denoise_variance = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
@@ -550,6 +587,7 @@ int main(int argc, char** argv) {
         denoise_moments = denoise_moments || std::strcmp(argv[i], "--denoise-moments") == 0;
         moment_gradients = moment_gradients || std::strcmp(argv[i], "--moment-gradients") == 0;
         adaptive = adaptive || std::strcmp(argv[i], "--adaptive") == 0;
+        denoise_variance = denoise_variance || std::strcmp(argv[i], "--denoise-variance") == 0;
     }
     if (worker && adaptive) return die("--adaptive is not available with --worker: the wire format carries no sampler");
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
@@ -561,6 +599,8 @@ int main(int argc, char** argv) {
         return die("--denoise-moments is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && moment_gradients)
         return die("--moment-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && denoise_variance)
+        return die("--denoise-variance is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -591,6 +631,7 @@ int main(int argc, char** argv) {
         else if (s == "--temporal-gradients") a.temporal_gradients = true;
         else if (s == "--denoise-moments") a.denoise_moments = true;
         else if (s == "--moment-gradients") a.moment_gradients = true;
+        else if (s == "--denoise-variance") a.denoise_variance = true;
         else if (s == "--adaptive") { // two numbers: MIN MAX
             const char* v2 = i + 2 < argc ? argv[i + 2] : nullptr;
             ok = parse_u64(v, a.ad_min) && parse_u64(v2, a.ad_max) && a.ad_min <= UINT32_MAX && a.ad_max <= UINT32_MAX;
@@ -632,6 +673,20 @@ int main(int argc, char** argv) {
         const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
         if (trb_adaptive_schedule(&ad, nullptr, nullptr, nullptr, nullptr) != TRB_OK) return die("--adaptive %llu %llu: %s", (unsigned long long)a.ad_min,
                                                                                                 (unsigned long long)a.ad_max, trb_last_error());
+    }
+    if (a.denoise_variance) {
+        if (a.master) return die("--denoise-variance is not available with --master: the wire format carries no albedo, normal or depth");
+        if (!a.devices.empty()) return die("--denoise-variance renders on one GPU: use --device, not --devices");
+        if (a.denoise || a.denoise_temporal || a.temporal_gradients || a.denoise_moments || a.moment_gradients)
+            return die("--denoise-variance excludes --denoise, --denoise-temporal, --temporal-gradients, --denoise-moments and --moment-gradients: choose one denoiser");
+        // --spp 0 keeps the scene's film.samples, as in every mode; single_node checks that value once the scene is read
+        if (a.has_spp && a.spp == 1) return die("--denoise-variance needs at least 2 samples per pixel (a variance of one sample is undefined)");
+        if (a.adaptive) {
+            const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
+            uint32_t mn = 0;
+            if (trb_adaptive_schedule(&ad, &mn, nullptr, nullptr, nullptr) == TRB_OK && mn < 2)
+                return die("--denoise-variance needs --adaptive MIN of at least 2 samples per pixel; MIN rounds to %u", mn);
+        }
     }
     if (a.has_start && a.has_end && a.end < a.start)
         return die("end frame %llu is before start frame %llu", (unsigned long long)a.end, (unsigned long long)a.start);
