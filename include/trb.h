@@ -1165,6 +1165,62 @@ trb_status trb_denoise_moments_gradient_device(trb_scene* scene, trb_denoise_his
                                                const trb_denoise_gradient_params* params, uint32_t seed,
                                                const trb_denoise_moments_gradient_output* d_out, void* cuda_stream);
 
+/* -- Variance temporal denoising: animations denoised with the variance of their own samples, carried through the history ---------
+ * (DESIGN.md §4 "Variance temporal denoising"). "Sample variance" over a history: each frame's lum_w film gives the variance v_f of
+ * the frame's pixel mean, and for the blend ē = alpha e + (1 - alpha) H' of independent frames the history carries V' = Var(H'), so
+ * Var(ē) = alpha^2 v_f + (1 - alpha)^2 V' exactly, for any sequence of alpha. One render per frame at 2 spp or more (LowDiscrepancy
+ * or Adaptive), a variance that shrinks as the history grows, and no spatial estimate. The inputs are a trb_denoise_frame and the
+ * lum_w film of the same render (trb_render_aov_lum* or trb_render_adaptive_aov_lum*) at the scene's current frame; the history is a
+ * trb_denoise_history with the scene, film size, snapshot and generation rules of "Temporal denoising". Per pixel p, float32, left to
+ * right, never contracted:
+ *   1. W, c, d, e, n, z, dz and v_f are trb_denoise_variance's steps 1-3 (v_f from lum_w). A pixel that call does not filter (W <= 0,
+ *      anything non-finite, or v_f NaN: at most one effective sample) is written exactly as it writes it, stores "none", and has
+ *      motion (NaN, NaN), history_length 0 and variance NaN.
+ *   2. Reprojection: steps 1-3 of "Temporal denoising", unchanged, over this family's sets: H' = (sum of w * ē_t in tap order) / S per
+ *      channel, V' = (sum of w * V_t in tap order) / S, and len_prev.
+ *   3. n' = min(len_prev + 1, max_history), or 1 without history; in the gradient form, where there is history, n' =
+ *      min((uint32)floorf((1 - lambda) * (float)len_prev) + 1, max_history) with lambda from the pixel's stratum ("Temporal
+ *      gradients" steps 1, 2 and 4 run unchanged around it). n' > 1: alpha = 1 / (float)n', beta = 1 - alpha,
+ *        ē = alpha * e + beta * H' per channel,  V = (alpha * alpha) * v_f + (beta * beta) * V'
+ *      n' == 1: ē = e, V = v_f.
+ *   4. (ē, V) goes into trb_denoise's a-trous iterations unchanged; the output is remodulated by d (iterations 0: ē * d).
+ *   5. A filtered pixel with finite z stores (ē, z), (V, 0, 0, i), (n, n'): 96 bytes per pixel, as the other families. variance
+ *      receives V. Every NaN written to rgbw, motion or variance is 0x7fffffff.
+ * An empty history or max_history 1 gives trb_denoise_variance's rgbw and variance bit for bit; in the gradient form lambda 0
+ * everywhere gives the plain call's pixel, lambda 1 trb_denoise_variance's.
+ * History families: the half-film calls (trb_denoise_temporal*), the moment calls (trb_denoise_moments*) and these calls each treat
+ * a history last written by another family as empty. Gradient records are valid only after a variance gradient call of the same
+ * object generation and film size; a plain variance call invalidates them. The scene's denoise scratch is 72 bytes per pixel. */
+
+/* Denoise a frame of one film with its lum_w film and its history: HOST inputs and outputs (lum_w width*height*4 floats), staged per
+ * call; blocking. The parameters are trb_denoise_temporal's, checked first (no scene is needed to refuse them); then TRB_INVALID_ARG
+ * for a null scene, history, input member, lum_w or out->rgbw, a history of another scene or film size, a scene without a frame, or
+ * an output overlapping an input or another output; TRB_OOM when scratch or history does not fit. A call that fails leaves the
+ * history as it was. */
+trb_status trb_denoise_variance_temporal(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* in, const float* lum_w,
+                                         const trb_denoise_temporal_params* params, const trb_denoise_moments_output* out);
+
+/* The same with DEVICE buffers (the alignment of trb_denoise_moments_device, lum_w 16-byte aligned; TRB_INVALID_ARG otherwise),
+ * enqueued on cuda_stream under trb_render_device's one-stream rule: 1 + iterations kernel launches and one copy of the instance
+ * transforms. No host synchronisation, except once when the scratch or the history grows. */
+trb_status trb_denoise_variance_temporal_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* d_in,
+                                                const float* d_lum_w, const trb_denoise_temporal_params* params,
+                                                const trb_denoise_moments_output* d_out, void* cuda_stream);
+
+/* trb_denoise_variance_temporal with temporal gradients: the same inputs, history, checks and statuses (the parameters first, and a
+ * failed call leaves the history as it was), plus TRB_INVALID_ARG for iterations above 6 or a lambda output that overlaps another
+ * buffer. `seed` seeds this frame's gradient samples. HOST buffers; blocking. */
+trb_status trb_denoise_variance_temporal_gradient(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* in,
+                                                  const float* lum_w, const trb_denoise_gradient_params* params, uint32_t seed,
+                                                  const trb_denoise_moments_gradient_output* out);
+
+/* The same with DEVICE buffers (the alignment of trb_denoise_variance_temporal_device, lambda 4-byte aligned), enqueued on
+ * cuda_stream under trb_render_device's one-stream rule: trb_denoise_moments_gradient_device's launches without its variance kernel.
+ * No host synchronisation, except when scratch, history or the wavefront state grows. */
+trb_status trb_denoise_variance_temporal_gradient_device(trb_scene* scene, trb_denoise_history* history, const trb_denoise_frame* d_in,
+                                                         const float* d_lum_w, const trb_denoise_gradient_params* params, uint32_t seed,
+                                                         const trb_denoise_moments_gradient_output* d_out, void* cuda_stream);
+
 /* trb_camera_rays with DEVICE buffers on the scene's GPU (4-byte aligned), enqueued on cuda_stream (a cudaStream_t; NULL = default
  * stream) without host synchronisation: the same kernel, so the same bits. The checks and statuses of trb_camera_rays, plus
  * TRB_INVALID_ARG for unaligned buffers; before the first update_frame it is TRB_INVALID_ARG. */

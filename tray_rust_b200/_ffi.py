@@ -326,6 +326,8 @@ TRB_SYMBOLS = [
     "trb_render_sharded_aov", "trb_render_sharded_adaptive_aov", "trb_group_render_aov", "trb_group_render_adaptive_aov",
     "trb_render_aov_lum", "trb_render_aov_lum_device", "trb_render_adaptive_aov_lum", "trb_render_adaptive_aov_lum_device",
     "trb_denoise_variance", "trb_denoise_variance_device",
+    "trb_denoise_variance_temporal", "trb_denoise_variance_temporal_device", "trb_denoise_variance_temporal_gradient",
+    "trb_denoise_variance_temporal_gradient_device",
 ]
 
 _trb = None
@@ -428,6 +430,14 @@ def load_trb():
     lib.trb_render_adaptive_aov_lum_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, vp, vp]
     lib.trb_denoise_variance.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp]
     lib.trb_denoise_variance_device.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp, vp]
+    lib.trb_denoise_variance_temporal.argtypes = [vp, vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseTemporalParams),
+                                                  C.POINTER(DenoiseMomentsOutput)]
+    lib.trb_denoise_variance_temporal_device.argtypes = [vp, vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseTemporalParams),
+                                                         C.POINTER(DenoiseMomentsOutput), vp]
+    lib.trb_denoise_variance_temporal_gradient.argtypes = [vp, vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseGradientParams), u32,
+                                                           C.POINTER(DenoiseMomentsGradientOutput)]
+    lib.trb_denoise_variance_temporal_gradient_device.argtypes = [vp, vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseGradientParams), u32,
+                                                                  C.POINTER(DenoiseMomentsGradientOutput), vp]
     lib.trb_adaptive_schedule.argtypes = [C.POINTER(Adaptive)] + [C.POINTER(u32)] * 4
     lib.trb_host_adaptive_decide.argtypes = [C.POINTER(Adaptive), vp, sz, C.POINTER(u32), C.POINTER(f32)]
     lib.trb_film_to_srgb8.argtypes = [vp, vp, vp]

@@ -501,13 +501,16 @@ class Scene(_Base):
             return outs[0][1]
         return tuple(a for _, a, _, _ in outs)
 
-    def _moments_arrays(self, colour, aovs, out, motion, history_length, variance, lam=False):
+    def _moments_arrays(self, colour, aovs, out, motion, history_length, variance, lam=False, lum=False):
         """The four input arrays and the output arrays of a moment denoise, checked (motion, history_length, variance and lam:
-        True, False/None or an array). Returns (ins, outs) as (name, array, shape, dtype) lists."""
+        True, False/None or an array); with `lum`, aovs["lum_w"] is a fifth input. Returns (ins, outs) as (name, array, shape,
+        dtype) lists."""
         h, w = self.height, self.width
         film_shape = (h, w, 4)
         ins = [("colour", colour, film_shape, np.float32), ("albedo_w", aovs.get("albedo_w"), film_shape, np.float32),
                ("normal_w", aovs.get("normal_w"), film_shape, np.float32), ("nearest", aovs.get("nearest"), (h, w), np.uint64)]
+        if lum:
+            ins.append(("lum_w", aovs.get("lum_w"), film_shape, np.float32))
         outs = [("out", np.zeros(film_shape, np.float32) if out is None else out, film_shape, np.float32)]
         for name, a, shape, dtype in (("motion", motion, (h, w, 2), np.float32), ("history_length", history_length, (h, w), np.uint32),
                                       ("variance", variance, (h, w), np.float32), ("lambda", lam, (h, w), np.float32)):
@@ -614,6 +617,71 @@ class Scene(_Base):
             return self.denoise_variance(film, aovs, **(denoise or {})), film, aovs, pixel_spp, st
         film, aovs, st = self.render_aov(lum=True, spp=spp, **kw)
         return self.denoise_variance(film, aovs, **(denoise or {})), film, aovs, st
+
+    def denoise_variance_temporal(self, history, colour, aovs, out=None, motion=False, history_length=False, variance=False, **params):
+        """trb_denoise_variance_temporal (DESIGN.md §4 "Variance temporal denoising"): one colour film of the frame and the AOVs of
+        the same render with its lum_w film (render_aov(lum=True)'s dict), rendered at the scene's current frame, with the
+        DenoiseHistory `history`. The variance of each pixel's own samples is carried through the history. params:
+        denoise_temporal's. Returns denoise_moments's film or tuple."""
+        ins, outs = self._moments_arrays(colour, aovs, out, motion, history_length, variance, lum=True)
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins[:4])), _temporal_params(params)
+        o = F.DenoiseMomentsOutput(*(got[k].ctypes.data if k in got else None for k in ("out", "motion", "history_length", "variance")))
+        self._check(self._lib.trb_denoise_variance_temporal(self._h, history._h, C.byref(d_in), ins[4][1].ctypes.data, C.byref(prm), C.byref(o)))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_variance_temporal_gradient(self, history, colour, aovs, seed, out=None, motion=False, history_length=False, variance=False,
+                                           lam=False, **params):
+        """trb_denoise_variance_temporal_gradient: denoise_variance_temporal with temporal gradients. `seed` seeds this frame's
+        gradient samples. params: denoise_moments_gradient's. Returns denoise_moments_gradient's film or tuple."""
+        ins, outs = self._moments_arrays(colour, aovs, out, motion, history_length, variance, lam, lum=True)
+        got = {name: a for name, a, _, _ in outs}
+        d_in, prm = F.DenoiseFrame(*(a.ctypes.data for _, a, _, _ in ins[:4])), _gradient_params(params)
+        o = F.DenoiseMomentsGradientOutput(*(got[k].ctypes.data if k in got else None
+                                             for k in ("out", "motion", "history_length", "variance", "lambda")))
+        self._check(self._lib.trb_denoise_variance_temporal_gradient(self._h, history._h, C.byref(d_in), ins[4][1].ctypes.data, C.byref(prm),
+                                                                     seed % (1 << 32), C.byref(o)))
+        if len(outs) == 1:
+            return outs[0][1]
+        return tuple(a for _, a, _, _ in outs)
+
+    def denoise_variance_temporal_device(self, history, d_colour, d_albedo, d_normal, d_nearest, d_lum, d_out, d_motion=None,
+                                         d_history_length=None, d_variance=None, stream=None, **params):
+        """trb_denoise_variance_temporal_device: denoise_moments_device's pointers plus d_lum (height*width*4 float32, 16-byte
+        aligned); enqueued on `stream`. params as for denoise_variance_temporal."""
+        d_in, prm = F.DenoiseFrame(d_colour, d_albedo, d_normal, d_nearest), _temporal_params(params)
+        o = F.DenoiseMomentsOutput(d_out, d_motion, d_history_length, d_variance)
+        self._check(self._lib.trb_denoise_variance_temporal_device(self._h, history._h, C.byref(d_in), d_lum, C.byref(prm), C.byref(o), stream))
+
+    def denoise_variance_temporal_gradient_device(self, history, d_colour, d_albedo, d_normal, d_nearest, d_lum, seed, d_out, d_motion=None,
+                                                  d_history_length=None, d_variance=None, d_lambda=None, stream=None, **params):
+        """trb_denoise_variance_temporal_gradient_device: denoise_variance_temporal_device's pointers plus d_lambda (height*width
+        float32, 4-byte aligned, or None); enqueued on `stream`. params as for denoise_variance_temporal_gradient."""
+        d_in, prm = F.DenoiseFrame(d_colour, d_albedo, d_normal, d_nearest), _gradient_params(params)
+        o = F.DenoiseMomentsGradientOutput(d_out, d_motion, d_history_length, d_variance, d_lambda)
+        self._check(self._lib.trb_denoise_variance_temporal_gradient_device(self._h, history._h, C.byref(d_in), d_lum, C.byref(prm),
+                                                                            seed % (1 << 32), C.byref(o), stream))
+
+    def render_denoised_variance_temporal(self, history, spp=0, adaptive=None, seed=1, current_frame=0, denoise=None, gradients=False, **kw):
+        """Frame `current_frame` of an animation rendered once with the AOVs and the lum_w film, with seed (seed + current_frame)
+        mod 2^32: by render_aov at `spp` (0: the scene's), or with adaptive=(min_spp, max_spp) by render_adaptive_aov. Denoised with
+        `history` by denoise_variance_temporal, or with `gradients` by denoise_variance_temporal_gradient with that frame seed (the
+        dict `denoise` holds the parameters). Returns render_denoised_variance's tuple."""
+        frame_seed = (seed + current_frame) % (1 << 32)
+        kw = dict(kw, seed=frame_seed, current_frame=current_frame)
+        if adaptive is not None:
+            if spp:
+                raise ValueError("render_denoised_variance_temporal: the Adaptive sampler chooses the sample counts; spp is not taken")
+            film, aovs, pixel_spp, st = self.render_adaptive_aov(adaptive[0], adaptive[1], lum=True, **kw)
+        else:
+            film, aovs, st = self.render_aov(lum=True, spp=spp, **kw)
+        if gradients:
+            out = self.denoise_variance_temporal_gradient(history, film, aovs, frame_seed, **(denoise or {}))
+        else:
+            out = self.denoise_variance_temporal(history, film, aovs, **(denoise or {}))
+        return (out, film, aovs, pixel_spp, st) if adaptive is not None else (out, film, aovs, st)
 
     def render_denoised(self, spp=0, denoise=None, **kw):
         """A denoised frame at `spp` samples per pixel (0: the scene's), rounded up to a power of two as every render rounds it:

@@ -3071,6 +3071,13 @@ trb_status trb_denoise_variance(trb_scene* s, const trb_denoise_frame* in, const
 }
 
 // ---- temporal denoising (include/trb.h "Temporal denoising", DESIGN.md §4) -------------------------------------------------------
+// The history families: what a set's records hold. A call finds no history in a set written by another family.
+enum DnFamily : uint8_t {
+    DN_HALVES,   // trb_denoise_temporal*: (ē_a, z), (ē_b, inst)
+    DN_MOMENTS,  // trb_denoise_moments*: (ē, z), (mu1, mu2, 0, inst)
+    DN_VARIANCE, // trb_denoise_variance_temporal*: (ē, z), (V, 0, 0, inst)
+};
+
 // Two per-pixel history sets (trb::DnHistory, 48 B per pixel each) and two instance snapshots (64 B per instance each); `cur` is the
 // set the next call reads. The host fields describe the frame the read set was written at.
 struct trb_denoise_history {
@@ -3087,7 +3094,7 @@ struct trb_denoise_history {
     float cam_inv[16] = {}, tan_fov = 0;
     uint32_t n_instances = 0;
     uint64_t generation = 0;
-    bool moments = false;          // the read set was written by trb_denoise_moments* (moments), not trb_denoise_temporal* (halves)
+    DnFamily family = DN_HALVES;   // the family of the calls that wrote the read set
     // temporal gradients: two record sets and the per-call stratum buffers (trb::GrBuffers) for gr_capacity strata; the records of
     // the read set are valid only after a gradient call, and were written at gr_seed, gr_shutter_open and gr_cam_mat
     void* d_gr = nullptr;
@@ -3289,9 +3296,9 @@ struct HistorySets {
 };
 
 // What a history call does before its kernels, for npx > 0 pixels: grow the history (and, with gc, its gradient buffers) where
-// needed, fill tp's current frame and the read set's snapshot (has_prev only for a history of the call's family, `moments`), and copy
-// this frame's instance transforms into the write snapshot on `st`
-trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnParams& prm, trb::DnTemporal& tp, bool moments, const GradCall* gc,
+// needed, fill tp's current frame and the read set's snapshot (has_prev only for a history of the call's family), and copy this
+// frame's instance transforms into the write snapshot on `st`
+trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnParams& prm, trb::DnTemporal& tp, DnFamily family, const GradCall* gc,
                          HistorySets& hs, cudaStream_t st) {
     const size_t npx = (size_t)prm.width * prm.height, n = s->instances.size();
     trb_status r;
@@ -3338,7 +3345,7 @@ trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnPara
     if (aspect > 1.0f) { tp.x0 = -aspect; tp.x1 = aspect; tp.y0 = -1.0f; tp.y1 = 1.0f; }
     else { tp.x0 = -1.0f; tp.x1 = 1.0f; tp.y0 = -1.0f / aspect; tp.y1 = 1.0f / aspect; }
     tp.n_prev = h->n_instances;
-    tp.has_prev = h->has_prev && h->generation == s->object_generation && h->moments == moments ? 1u : 0u;
+    tp.has_prev = h->has_prev && h->generation == s->object_generation && h->family == family ? 1u : 0u;
     hs.rd = h->cur; hs.wr = h->cur ^ 1u;
     hs.mats_rd = h->d_mats + (size_t)hs.rd * h->mat_capacity * 16;
     float* mats_wr = h->d_mats + (size_t)hs.wr * h->mat_capacity * 16;
@@ -3349,13 +3356,13 @@ trb_status history_begin(trb_scene* s, trb_denoise_history* h, const trb::DnPara
 }
 
 // After a history call's kernels: the history switches to the set just written, and the snapshot becomes the current frame's
-void history_commit(trb_scene* s, trb_denoise_history* h, const HistorySets& hs, bool moments) {
+void history_commit(trb_scene* s, trb_denoise_history* h, const HistorySets& hs, DnFamily family) {
     h->cur = hs.wr; h->has_prev = true; h->bound = true; h->width = s->film.width; h->height = s->film.height;
     std::memcpy(h->cam_inv, s->cam_inv, 64);
     h->tan_fov = s->ds.cam.scaling[0];
     h->n_instances = (uint32_t)s->instances.size();
     h->generation = s->object_generation;
-    h->moments = moments;
+    h->family = family;
 }
 
 // k_dn_temporal (or, with gc, the gradient steps around k_dn_temporal_grad) and the a-trous launches on `st`, then the history's
@@ -3368,7 +3375,7 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
     trb_status r = denoise_scratch(s, npx, sc);
     if (r != TRB_OK) return r;
     HistorySets hs;
-    r = history_begin(s, h, prm, tp, false, gc, hs, st);
+    r = history_begin(s, h, prm, tp, DN_HALVES, gc, hs, st);
     if (r != TRB_OK) return r;
     const uint32_t rd = hs.rd, wr = hs.wr;
     const float* mats_rd = hs.mats_rd;
@@ -3403,7 +3410,7 @@ trb_status temporal_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams&
         if (r != TRB_OK) return r;
         gradient_commit(s, h, *gc);
     }
-    history_commit(s, h, hs, false);
+    history_commit(s, h, hs, DN_HALVES);
     return TRB_OK;
 }
 } // namespace
@@ -3499,56 +3506,74 @@ trb_status trb_denoise_temporal_gradient(trb_scene* s, trb_denoise_history* h, c
 
 // ---- moment denoising (include/trb.h "Moment denoising", DESIGN.md §4) -----------------------------------------------------------
 namespace {
-// The checks of both forms after the parameters: null pointers, overlapping outputs, the history's scene and film size, a frame
+// The checks of both forms after the parameters: null pointers, overlapping outputs, the history's scene and film size, a frame.
+// variance: a trb_denoise_variance_temporal* call, whose lum_w is one more required input.
 trb_status moments_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_temporal_params* params,
-                         const trb_denoise_moments_output* out, trb::DnParams& prm, trb::DnTemporal& tp) {
+                         const trb_denoise_moments_output* out, trb::DnParams& prm, trb::DnTemporal& tp, bool variance = false,
+                         const float* lum_w = nullptr) {
     trb_status r = temporal_params(params, prm, tp);
     if (r != TRB_OK) return r;
-    if (!s || !h || !in || !out || !out->rgbw || !in->colour || !in->albedo_w || !in->normal_w || !in->nearest)
+    if (!s || !h || !in || !out || !out->rgbw || !in->colour || !in->albedo_w || !in->normal_w || !in->nearest || (variance && !lum_w))
         return fail(TRB_INVALID_ARG, "null argument");
     prm.width = (int)s->film.width; prm.height = (int)s->film.height;
     const size_t npx = (size_t)s->film.width * s->film.height;
-    const Span ins[4] = {{in->colour, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
-                         {in->nearest, npx * sizeof(uint64_t)}};
+    const Span ins[5] = {{in->colour, npx * sizeof(float4)}, {in->albedo_w, npx * sizeof(float4)}, {in->normal_w, npx * sizeof(float4)},
+                         {in->nearest, npx * sizeof(uint64_t)}, {lum_w, npx * sizeof(float4)}};
     const Span outs[4] = {{out->rgbw, npx * sizeof(float4)}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
                           {out->variance, npx * sizeof(float)}};
-    return history_call_check(s, h, ins, 4, outs, 4, 0);
+    return history_call_check(s, h, ins, variance ? 5 : 4, outs, 4, 0);
 }
 
 // k_dn_temporal_moments (or, with gc, the gradient steps around k_dn_temporal_moments_grad), k_dn_moments_variance and the a-trous
-// launches on `st`, then the history's switch to the set just written
+// launches on `st`, then the history's switch to the set just written. With lum_w (trb_denoise_variance_temporal*),
+// k_dn_temporal_variance or k_dn_temporal_variance_grad takes the place of the moment kernels, and the history is of the variance
+// family.
 trb_status moments_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& prm, trb::DnTemporal& tp, const trb_denoise_frame& in,
-                           const trb_denoise_moments_output& out, cudaStream_t st, const GradCall* gc = nullptr) {
+                           const trb_denoise_moments_output& out, cudaStream_t st, const GradCall* gc = nullptr, const float* lum_w = nullptr) {
     const size_t npx = (size_t)prm.width * prm.height;
     if (npx == 0) return TRB_OK;
+    const DnFamily family = lum_w ? DN_VARIANCE : DN_MOMENTS;
     trb::DnScratch sc;
     float4* mom = nullptr;
-    trb_status r = denoise_scratch(s, npx, sc, &mom);
+    trb_status r = denoise_scratch(s, npx, sc, lum_w ? nullptr : &mom);
     if (r != TRB_OK) return r;
     HistorySets hs;
-    r = history_begin(s, h, prm, tp, true, gc, hs, st);
+    r = history_begin(s, h, prm, tp, family, gc, hs, st);
     if (r != TRB_OK) return r;
     float4* rgbw = reinterpret_cast<float4*>(out.rgbw);
     const dim3 block(32, 8), grid((prm.width + 31) / 32, (prm.height + 7) / 8);
+    const float4* col = reinterpret_cast<const float4*>(in.colour);
+    const float4* lum = reinterpret_cast<const float4*>(lum_w);
+    const float4* alb = reinterpret_cast<const float4*>(in.albedo_w);
+    const float4* nrm = reinterpret_cast<const float4*>(in.normal_w);
+    const unsigned long long* nearest = reinterpret_cast<const unsigned long long*>(in.nearest);
+    float2* motion = reinterpret_cast<float2*>(out.motion);
     GrBuffers b{};
     if (!gc) {
-        trb::k_dn_temporal_moments<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour), reinterpret_cast<const float4*>(in.albedo_w),
-                                                           reinterpret_cast<const float4*>(in.normal_w), reinterpret_cast<const unsigned long long*>(in.nearest),
-                                                           sc, mom, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd), h->set(hs.wr),
-                                                           reinterpret_cast<float2*>(out.motion), out.history_length);
+        if (lum_w)
+            trb::k_dn_temporal_variance<<<grid, block, 0, st>>>(prm, tp, col, lum, alb, nrm, nearest, sc, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd),
+                                                                h->set(hs.wr), motion, out.history_length, out.variance);
+        else
+            trb::k_dn_temporal_moments<<<grid, block, 0, st>>>(prm, tp, col, alb, nrm, nearest, sc, mom, rgbw, s->d_instances, hs.mats_rd, h->set(hs.rd),
+                                                               h->set(hs.wr), motion, out.history_length);
     } else {
         gr_layout(h->gr_capacity, static_cast<char*>(h->d_gr), &b);
         r = gradient_lambda(s, h, *gc, tp, b, hs.mats_rd, in.nearest, in.normal_w, tp.has_prev && h->gr_valid, st);
         if (r != TRB_OK) return r;
-        trb::k_dn_temporal_moments_grad<<<grid, block, 0, st>>>(prm, tp, reinterpret_cast<const float4*>(in.colour),
-                                                                reinterpret_cast<const float4*>(in.albedo_w), reinterpret_cast<const float4*>(in.normal_w),
-                                                                reinterpret_cast<const unsigned long long*>(in.nearest), sc, mom, rgbw, s->d_instances,
-                                                                hs.mats_rd, h->set(hs.rd), h->set(hs.wr), reinterpret_cast<float2*>(out.motion),
-                                                                out.history_length, b.lam, (uint32_t)((prm.width + 2) / 3), gc->lambda);
+        const uint32_t gw = (uint32_t)((prm.width + 2) / 3);
+        if (lum_w)
+            trb::k_dn_temporal_variance_grad<<<grid, block, 0, st>>>(prm, tp, col, lum, alb, nrm, nearest, sc, rgbw, s->d_instances, hs.mats_rd,
+                                                                     h->set(hs.rd), h->set(hs.wr), motion, out.history_length, out.variance, b.lam, gw,
+                                                                     gc->lambda);
+        else
+            trb::k_dn_temporal_moments_grad<<<grid, block, 0, st>>>(prm, tp, col, alb, nrm, nearest, sc, mom, rgbw, s->d_instances, hs.mats_rd,
+                                                                    h->set(hs.rd), h->set(hs.wr), motion, out.history_length, b.lam, gw, gc->lambda);
     }
     g_launches++;
-    trb::k_dn_moments_variance<<<grid, block, 0, st>>>(prm, sc.guide, sc.grad, mom, sc.ev[0], out.variance);
-    g_launches++;
+    if (!lum_w) {
+        trb::k_dn_moments_variance<<<grid, block, 0, st>>>(prm, sc.guide, sc.grad, mom, sc.ev[0], out.variance);
+        g_launches++;
+    }
     CU(cudaGetLastError());
     r = denoise_atrous(prm, sc, rgbw, st);
     if (r != TRB_OK) return r;
@@ -3559,7 +3584,7 @@ trb_status moments_enqueue(trb_scene* s, trb_denoise_history* h, trb::DnParams& 
     } else {
         h->gr_valid = false;
     }
-    history_commit(s, h, hs, true);
+    history_commit(s, h, hs, family);
     return TRB_OK;
 }
 } // namespace
@@ -3596,21 +3621,23 @@ trb_status trb_denoise_moments(trb_scene* s, trb_denoise_history* h, const trb_d
 
 // ---- moment gradients (include/trb.h "Moment gradients", DESIGN.md §4) -------------------------------------------------------------
 namespace {
-// trb_denoise_gradient_params (NULL meaning the defaults) first, then moments_check and the lambda output's overlaps
+// trb_denoise_gradient_params (NULL meaning the defaults) first, then moments_check and the lambda output's overlaps (variance, lum_w:
+// as for moments_check)
 trb_status moments_gradient_check(const trb_scene* s, const trb_denoise_history* h, const trb_denoise_frame* in, const trb_denoise_gradient_params* params,
-                                  const trb_denoise_moments_gradient_output* out, trb::DnParams& prm, trb::DnTemporal& tp, GradCall& gc) {
+                                  const trb_denoise_moments_gradient_output* out, trb::DnParams& prm, trb::DnTemporal& tp, GradCall& gc,
+                                  bool variance = false, const float* lum_w = nullptr) {
     const uint32_t iterations = params ? params->iterations : 3u;
     trb_status r = temporal_params(params ? &params->temporal : nullptr, prm, tp);
     if (r != TRB_OK) return r;
     if (iterations > 6) return fail(TRB_INVALID_ARG, "temporal gradient iterations must be 0 to 6");
     if (!out) return fail(TRB_INVALID_ARG, "null argument");
     const trb_denoise_moments_output o{out->rgbw, out->motion, out->history_length, out->variance};
-    r = moments_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp);
+    r = moments_check(s, h, in, params ? &params->temporal : nullptr, &o, prm, tp, variance, lum_w);
     if (r != TRB_OK) return r;
     const size_t npx = (size_t)s->film.width * s->film.height, fb = npx * sizeof(float4);
     if (overlaps_any({out->lambda, npx * sizeof(float)}, {{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)},
                                                           {out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)},
-                                                          {out->variance, npx * sizeof(float)}}))
+                                                          {out->variance, npx * sizeof(float)}, {lum_w, fb}}))
         return fail(TRB_INVALID_ARG, "the lambda output overlaps another buffer");
     gc.iterations = iterations;
     gc.lambda = out->lambda;
@@ -3652,6 +3679,77 @@ trb_status trb_denoise_moments_gradient(trb_scene* s, trb_denoise_history* h, co
                           gc.lambda = d[8].as<float>();
                           return moments_enqueue(s, h, prm, tp, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()},
                                                  {d[4].as<float>(), d[5].as<float>(), d[6].as<uint32_t>(), d[7].as<float>()}, 0, &gc);
+                      });
+}
+
+// ---- variance temporal denoising (include/trb.h "Variance temporal denoising", DESIGN.md §4) ---------------------------------------
+// The moment calls' checks and enqueue with lum_w: one more input, and the variance kernels in place of the moment ones
+trb_status trb_denoise_variance_temporal_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* d_in, const float* d_lum_w,
+                                                const trb_denoise_temporal_params* params, const trb_denoise_moments_output* d_out, void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    trb_status r = moments_check(s, h, d_in, params, d_out, prm, tp, true, d_lum_w);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_lum_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8},
+                           {d_out->motion, 8}, {d_out->history_length, 4}, {d_out->variance, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length and variance 4-byte");
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    return moments_enqueue(s, h, prm, tp, *d_in, *d_out, static_cast<cudaStream_t>(stream), nullptr, d_lum_w);
+}
+
+trb_status trb_denoise_variance_temporal(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* in, const float* lum_w,
+                                         const trb_denoise_temporal_params* params, const trb_denoise_moments_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    trb_status r = moments_check(s, h, in, params, out, prm, tp, true, lum_w);
+    if (r != TRB_OK) return r;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    return run_staged({{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}, {lum_w, fb}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)}},
+                      [&](const DeviceBuffer* d) {
+                          return moments_enqueue(s, h, prm, tp, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()},
+                                                 {d[5].as<float>(), d[6].as<float>(), d[7].as<uint32_t>(), d[8].as<float>()}, 0, nullptr, d[4].as<float>());
+                      });
+}
+
+trb_status trb_denoise_variance_temporal_gradient_device(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* d_in, const float* d_lum_w,
+                                                         const trb_denoise_gradient_params* params, uint32_t seed,
+                                                         const trb_denoise_moments_gradient_output* d_out, void* stream) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    trb_status r = moments_gradient_check(s, h, d_in, params, d_out, prm, tp, gc, true, d_lum_w);
+    if (r == TRB_OK)
+        r = check_aligned({{d_in->colour, 16}, {d_in->albedo_w, 16}, {d_in->normal_w, 16}, {d_lum_w, 16}, {d_out->rgbw, 16}, {d_in->nearest, 8},
+                           {d_out->motion, 8}, {d_out->history_length, 4}, {d_out->variance, 4}, {d_out->lambda, 4}},
+                          "device films must be 16-byte aligned, nearest and motion 8-byte, history_length, variance and lambda 4-byte");
+    if (r != TRB_OK) return r;
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const trb_denoise_moments_output o{d_out->rgbw, d_out->motion, d_out->history_length, d_out->variance};
+    return moments_enqueue(s, h, prm, tp, *d_in, o, static_cast<cudaStream_t>(stream), &gc, d_lum_w);
+}
+
+trb_status trb_denoise_variance_temporal_gradient(trb_scene* s, trb_denoise_history* h, const trb_denoise_frame* in, const float* lum_w,
+                                                  const trb_denoise_gradient_params* params, uint32_t seed,
+                                                  const trb_denoise_moments_gradient_output* out) {
+    trb::DnParams prm{};
+    trb::DnTemporal tp{};
+    GradCall gc{};
+    trb_status r = moments_gradient_check(s, h, in, params, out, prm, tp, gc, true, lum_w);
+    if (r != TRB_OK) return r;
+    gc.seed = seed;
+    CU(cudaSetDevice(s->device));
+    const size_t npx = (size_t)prm.width * prm.height, fb = npx * sizeof(float4);
+    return run_staged({{in->colour, fb}, {in->albedo_w, fb}, {in->normal_w, fb}, {in->nearest, npx * sizeof(uint64_t)}, {lum_w, fb}},
+                      {{out->rgbw, fb}, {out->motion, npx * sizeof(float2)}, {out->history_length, npx * sizeof(uint32_t)}, {out->variance, npx * sizeof(float)},
+                       {out->lambda, npx * sizeof(float)}},
+                      [&](const DeviceBuffer* d) {
+                          gc.lambda = d[9].as<float>();
+                          return moments_enqueue(s, h, prm, tp, {d[0].as<float>(), d[1].as<float>(), d[2].as<float>(), d[3].as<uint64_t>()},
+                                                 {d[5].as<float>(), d[6].as<float>(), d[7].as<uint32_t>(), d[8].as<float>()}, 0, &gc, d[4].as<float>());
                       });
 }
 

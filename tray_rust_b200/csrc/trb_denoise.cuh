@@ -5,8 +5,8 @@
 // for trb_denoise_temporal*, blending each pixel's reprojected history into the first (e, v) buffer; k_dn_temporal_moments and
 // k_dn_moments_variance take it for trb_denoise_moments* (k_dn_temporal_moments_grad for trb_denoise_moments_gradient*), one film with
 // the variance from luminance moments; k_dn_variance_prepare takes it for trb_denoise_variance*, one film with the variance of
-// its own samples (the lum_w film). Float32 in the header's order, no
-// atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
+// its own samples (the lum_w film); k_dn_temporal_variance (k_dn_temporal_variance_grad) takes it for trb_denoise_variance_temporal*
+// (the _gradient forms), that variance carried through the history. Float32 in the header's order, no atomics: every pixel's sums run in tap order, so the output is reproducible bit for bit (the oracle restates it in oracle_denoise/).
 #pragma once
 #include "trb_detmath.cuh"
 #include "trb_kernels.cuh"
@@ -111,6 +111,15 @@ __global__ void __launch_bounds__(256) k_dn_prepare(const DnParams prm, const fl
     dn_prepare_px(prm, x, y, i, c0, c1, c2, a0, a1, a2, d0, d1, d2, e0, e1, e2, v, nw, nearest, sc, out);
 }
 
+// Step 2 of "Sample variance": the variance of the pixel's weighted mean of l from its lum_w record, NaN for at most one effective sample
+__device__ __forceinline__ float dn_sample_variance(float4 lw) {
+    const float V1 = lw.w, V2 = lw.z;
+    if (!(V1 > 0.0f && V1 * V1 > V2)) return __int_as_float(0x7fffffff);
+    const float m1 = lw.x / V1, m2 = lw.y / V1;
+    const float s = m2 - m1 * m1;
+    return (s > 0.0f ? s : 0.0f) * V2 / (V1 * V1 - V2);
+}
+
 // trb_denoise_variance's k_dn_prepare (include/trb.h "Sample variance"): one film, and v from the pixel's own samples in lum_w.
 // Writes the same scratch, and var (may be null) receives v, NaN where the pixel is not filtered.
 __global__ void __launch_bounds__(256) k_dn_variance_prepare(const DnParams prm, const float4* __restrict__ col, const float4* __restrict__ lum,
@@ -135,13 +144,7 @@ __global__ void __launch_bounds__(256) k_dn_variance_prepare(const DnParams prm,
     const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
                 d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
     const float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
-    const float V1 = lw.w, V2 = lw.z;
-    float v = qnan; // at most one effective sample
-    if (V1 > 0.0f && V1 * V1 > V2) {
-        const float m1 = lw.x / V1, m2 = lw.y / V1;
-        const float s = m2 - m1 * m1;
-        v = (s > 0.0f ? s : 0.0f) * V2 / (V1 * V1 - V2);
-    }
+    const float v = dn_sample_variance(lw);
     const bool filtered = dn_prepare_px(prm, x, y, i, c0, c1, c2, a0, a1, a2, d0, d1, d2, e0, e1, e2, v, nw, nearest, sc, out);
     if (var) var[i] = filtered ? v : qnan;
 }
@@ -546,6 +549,135 @@ __global__ void __launch_bounds__(256) k_dn_temporal_moments_grad(const DnParams
                                                                   uint32_t* __restrict__ hlen, const float* __restrict__ lam_s, uint32_t gw,
                                                                   float* __restrict__ lam_out) {
     dn_temporal_moments_px<true>(prm, tp, col, alb, nrm, nearest, sc, mom, out, inst, mat_prev, hin, hout, motion, hlen, lam_s, gw, lam_out);
+}
+
+// ---- variance temporal denoising (trb_denoise_variance_temporal*, include/trb.h "Variance temporal denoising") --------------------
+// Steps 1-3 and 5: k_dn_variance_prepare's pixel, the history reprojected and gathered as in "Temporal denoising" (dn_reproject; a
+// set's records are (ē, z), (V, 0, 0, inst bits), (n, n' bits)) and the blend ē = alpha e + beta H', V = alpha^2 v_f + beta^2 V'.
+// Writes the scratch k_dn_prepare writes with ev[0] = (ē, V), the history, motion, history length and variance.
+// The body of k_dn_temporal_variance (GRAD false) and k_dn_temporal_variance_grad (GRAD true: n' shortened by the pixel's stratum's
+// lambda, and lam_out receives it). tp is taken by value, as in dn_temporal_moments_px.
+template <bool GRAD>
+__device__ __forceinline__ void dn_temporal_variance_px(const DnParams prm, const DnTemporal tp, const float4* __restrict__ col,
+                                                        const float4* __restrict__ lum, const float4* __restrict__ alb,
+                                                        const float4* __restrict__ nrm, const unsigned long long* __restrict__ nearest,
+                                                        DnScratch sc, float4* __restrict__ out, const DInstance* __restrict__ inst,
+                                                        const float* __restrict__ mat_prev, const DnHistory hin, const DnHistory hout,
+                                                        float2* __restrict__ motion, uint32_t* __restrict__ hlen, float* __restrict__ var,
+                                                        const float* __restrict__ lam_s, uint32_t gw, float* __restrict__ lam_out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= prm.width || y >= prm.height) return;
+    const int i = y * prm.width + x;
+    const float qnan = __int_as_float(0x7fffffff);
+    float lam = 0.0f;
+    if (GRAD) {
+        lam = lam_s[(uint32_t)(y / 3) * gw + (uint32_t)(x / 3)];
+        if (lam_out) lam_out[i] = lam;
+    }
+    const float4 A = col[i];
+    const float W = A.w;
+    if (W <= 0.0f) {
+        out[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        if (var) var[i] = qnan;
+        return;
+    }
+    const float c0 = A.x / W, c1 = A.y / W, c2 = A.z / W;
+    const float4 al = alb[i], nw = nrm[i], lw = lum[i];
+    const float a0 = al.x / al.w, a1 = al.y / al.w, a2 = al.z / al.w;
+    const float d0 = a0 > TRB_DENOISE_EPS_ALBEDO ? a0 : TRB_DENOISE_EPS_ALBEDO, d1 = a1 > TRB_DENOISE_EPS_ALBEDO ? a1 : TRB_DENOISE_EPS_ALBEDO,
+                d2 = a2 > TRB_DENOISE_EPS_ALBEDO ? a2 : TRB_DENOISE_EPS_ALBEDO;
+    float e0 = c0 / d0, e1 = c1 / d1, e2 = c2 / d2;
+    const float v = dn_sample_variance(lw);
+    const float m0 = nw.x / nw.w, m1 = nw.y / nw.w, m2 = nw.z / nw.w;
+    const float len2 = m0 * m0 + m1 * m1 + m2 * m2;
+    const unsigned long long key = nearest[i];
+    const float z = __uint_as_float((uint32_t)(key >> 32));
+    const bool ok = dn_finite(c0) && dn_finite(c1) && dn_finite(c2) && dn_finite(a0) && dn_finite(a1) && dn_finite(a2) && dn_finite(m0) &&
+                    dn_finite(m1) && dn_finite(m2) && dn_finite(len2) && dn_finite(e0) && dn_finite(e1) && dn_finite(e2) && dn_finite(v) &&
+                    z == z && z != __int_as_float(0xff800000);
+    if (!ok) {
+        out[i] = dn_out(c0, c1, c2, 1.0f);
+        sc.guide[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(0x7fc00000));
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (motion) motion[i] = make_float2(qnan, qnan);
+        if (hlen) hlen[i] = 0u;
+        if (var) var[i] = qnan;
+        return;
+    }
+    float n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+    if (len2 != 0.0f) {
+        const float l = sqrtf(len2);
+        n0 = m0 / l; n1 = m1 / l; n2 = m2 / l;
+    }
+    float gx = 0.0f, gy = 0.0f;
+    if (dn_finite(z)) {
+        const bool l = x > 0, r = x + 1 < prm.width, u = y > 0, dn = y + 1 < prm.height;
+        gx = dn_grad(z, l, l ? dn_depth(nearest, i - 1) : 0.0f, r, r ? dn_depth(nearest, i + 1) : 0.0f);
+        gy = dn_grad(z, u, u ? dn_depth(nearest, i - prm.width) : 0.0f, dn, dn ? dn_depth(nearest, i + prm.width) : 0.0f);
+    }
+    // 2: reconstruct, reproject, gather H' and V' (hv0)
+    const uint32_t id = (uint32_t)key;
+    float mx, my, S, h0, h1, h2, hv0, hv1, hv2;
+    uint32_t len_prev;
+    dn_reproject(prm, tp, x, y, z, id, n0, n1, n2, inst, mat_prev, hin, mx, my, S, h0, h1, h2, hv0, hv1, hv2, len_prev);
+    // 3: blend the colour with 1 / n' and the variance with its square
+    uint32_t np = 1;
+    if (GRAD) {
+        if (S > 0.0f) {
+            const uint32_t len_adj = (uint32_t)floorf((1.0f - lam) * (float)len_prev);
+            np = len_adj + 1 < tp.max_history ? len_adj + 1 : tp.max_history;
+        }
+    } else {
+        if (S > 0.0f) np = len_prev + 1 < tp.max_history ? len_prev + 1 : tp.max_history;
+    }
+    float V = v;
+    if (np > 1) {
+        h0 = h0 / S; h1 = h1 / S; h2 = h2 / S;
+        hv0 = hv0 / S;
+        const float alpha = 1.0f / (float)np, beta = 1.0f - alpha;
+        e0 = alpha * e0 + beta * h0; e1 = alpha * e1 + beta * h1; e2 = alpha * e2 + beta * h2;
+        V = (alpha * alpha) * v + (beta * beta) * hv0;
+    }
+    sc.guide[i] = make_float4(n0, n1, n2, z);
+    sc.grad[i] = make_float2(gx, gy);
+    sc.divisor[i] = make_float4(d0, d1, d2, 0.0f);
+    sc.ev[0][i] = make_float4(e0, e1, e2, V);
+    if (prm.iterations == 0) out[i] = dn_out(e0 * d0, e1 * d1, e2 * d2, 1.0f);
+    // 5: the new history
+    if (dn_finite(z)) {
+        hout.a[i] = make_float4(e0, e1, e2, z);
+        hout.b[i] = make_float4(V, 0.0f, 0.0f, __uint_as_float(id));
+        hout.n[i] = make_float4(n0, n1, n2, __uint_as_float(np));
+    } else {
+        hout.n[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    if (motion) motion[i] = make_float2(mx == mx ? mx : qnan, my == my ? my : qnan);
+    if (hlen) hlen[i] = np;
+    if (var) var[i] = V;
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal_variance(const DnParams prm, const __grid_constant__ DnTemporal tp, const float4* __restrict__ col,
+                                                              const float4* __restrict__ lum, const float4* __restrict__ alb,
+                                                              const float4* __restrict__ nrm, const unsigned long long* __restrict__ nearest,
+                                                              DnScratch sc, float4* __restrict__ out, const DInstance* __restrict__ inst,
+                                                              const float* __restrict__ mat_prev, const DnHistory hin, const DnHistory hout,
+                                                              float2* __restrict__ motion, uint32_t* __restrict__ hlen, float* __restrict__ var) {
+    dn_temporal_variance_px<false>(prm, tp, col, lum, alb, nrm, nearest, sc, out, inst, mat_prev, hin, hout, motion, hlen, var, nullptr, 0u, nullptr);
+}
+
+__global__ void __launch_bounds__(256) k_dn_temporal_variance_grad(const DnParams prm, const __grid_constant__ DnTemporal tp,
+                                                                   const float4* __restrict__ col, const float4* __restrict__ lum,
+                                                                   const float4* __restrict__ alb, const float4* __restrict__ nrm,
+                                                                   const unsigned long long* __restrict__ nearest, DnScratch sc,
+                                                                   float4* __restrict__ out, const DInstance* __restrict__ inst,
+                                                                   const float* __restrict__ mat_prev, const DnHistory hin, const DnHistory hout,
+                                                                   float2* __restrict__ motion, uint32_t* __restrict__ hlen, float* __restrict__ var,
+                                                                   const float* __restrict__ lam_s, uint32_t gw, float* __restrict__ lam_out) {
+    dn_temporal_variance_px<true>(prm, tp, col, lum, alb, nrm, nearest, sc, out, inst, mat_prev, hin, hout, motion, hlen, var, lam_s, gw, lam_out);
 }
 
 // Step 4 of "Moment denoising": each filtered pixel's variance, mu2 - mu1^2 from its own moments once n' >= MIN_HISTORY, else the

@@ -2,7 +2,7 @@
 //
 //   trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <n>] [--end-frame <n>] [--seed S] [--spp N] [--device D | --devices LIST]
 //            [--denoise] [--denoise-temporal [--temporal-gradients]] [--denoise-moments [--moment-gradients]] [--denoise-variance]
-//            [--adaptive MIN MAX]
+//            [--denoise-variance-temporal [--variance-gradients]] [--adaptive MIN MAX]
 //   trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <n>] [--end-frame <n>]
 //   trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]
 //
@@ -27,7 +27,10 @@
 // integrator; refused with --spp, since the sampler owns the schedule, and with --denoise, --denoise-temporal and --temporal-gradients,
 // which need two half sample ranges); --denoise-variance renders each frame once with AOVs and the lum_w film (trb_render_aov_lum, or
 // with --adaptive trb_render_adaptive_aov_lum) and denoises it with trb_denoise_variance (single node on one GPU, path integrator, 2
-// samples per pixel or more, refused with the other denoise flags, --devices, --master and --worker); --devices 0,1,2,3 renders each frame on a trb_group of those GPUs in place of one --device:
+// samples per pixel or more, refused with the other denoise flags, --devices, --master and --worker); --denoise-variance-temporal
+// renders the frames in order the same way, frame k with seed (S + k) mod 2^32, and denoises each with trb_denoise_variance_temporal
+// and one history (refused where --denoise-variance is, and with --denoise-variance); --variance-gradients, only with
+// --denoise-variance-temporal, denoises with trb_denoise_variance_temporal_gradient at the frame's seed; --devices 0,1,2,3 renders each frame on a trb_group of those GPUs in place of one --device:
 // plain and --adaptive frames by trb_group_render(_adaptive), every denoise mode by the group's AOV renders (trb_group_render_aov,
 // trb_group_render_adaptive_aov) and the denoise call on replica 0, which holds the history; with --worker the master's block range
 // is rendered by trb_group_render, in the same Frames (refused with --device, with --master, and for an empty, malformed or
@@ -56,7 +59,7 @@ const char* USAGE =
     "Usage:\n"
     "    trb_tray <scenefile> [-o <path>] [-n <number>] [--start-frame <number>] [--end-frame <number>] [--seed S] [--spp N]\n"
     "             [--device D | --devices LIST] [--denoise | --denoise-temporal [--temporal-gradients] | --denoise-moments [--moment-gradients]\n"
-    "             | --denoise-variance]\n"
+    "             | --denoise-variance | --denoise-variance-temporal [--variance-gradients]]\n"
     "             [--adaptive MIN MAX]\n"
     "    trb_tray <scenefile> --master <workers>... [-o <path>] [--start-frame <number>] [--end-frame <number>]\n"
     "    trb_tray --worker [-n <number>] [--port P] [--seed S] [--spp N] [--device D | --devices LIST]\n"
@@ -89,6 +92,10 @@ const char* USAGE =
     "  --denoise-variance      Render each frame once with albedo, normal, depth and the luminance moments of its samples, and\n"
     "                          denoise it with the variance of each pixel's own samples. Single node on one --device, path\n"
     "                          integrator, at least 2 samples per pixel (with --adaptive: MIN at least 2).\n"
+    "  --denoise-variance-temporal  As --denoise-variance, carrying each pixel's variance through a history over the frame range;\n"
+    "                          frame k is rendered with seed S + k.\n"
+    "  --variance-gradients    With --denoise-variance-temporal only: re-shade a sample of each 3x3 pixel block of the previous frame\n"
+    "                          in this one and shorten the history where the lighting changed.\n"
     "  --adaptive MIN MAX      Render with the Adaptive sampler: MIN samples per pixel, then more in rounds while a pixel's samples\n"
     "                          disagree, up to MAX (both rounded up to powers of two). With --denoise-moments each frame is also\n"
     "                          rendered with albedo, normal and depth and denoised by the moment denoiser.\n"
@@ -184,7 +191,7 @@ struct Args {
     const char* out = nullptr;
     bool master = false, has_start = false, has_end = false, has_seed = false, has_spp = false, has_device = false, denoise = false,
          denoise_temporal = false, temporal_gradients = false, denoise_moments = false, moment_gradients = false, adaptive = false,
-         denoise_variance = false;
+         denoise_variance = false, denoise_variance_temporal = false, variance_gradients = false;
     uint64_t start = 0, end = 0, seed = 1, spp = 0, device = 0, ad_min = 0, ad_max = 0;
     std::vector<int> devices; // --devices; empty: one --device
 };
@@ -281,12 +288,15 @@ struct MomentsFrame {
 };
 
 // --denoise-variance: the frame's whole sample range into one film with its AOVs and the lum_w film, then trb_denoise_variance
-// (DESIGN.md §4 "Sample variance"); with ad, the Adaptive sampler's render (trb_render_adaptive_aov_lum) in place of LowDiscrepancy
+// (DESIGN.md §4 "Sample variance"); with ad, the Adaptive sampler's render (trb_render_adaptive_aov_lum) in place of LowDiscrepancy.
+// --denoise-variance-temporal: the same with trb_denoise_variance_temporal and the history of the frames before, or with
+// --variance-gradients trb_denoise_variance_temporal_gradient at the frame's seed (DESIGN.md §4 "Variance temporal denoising")
 struct VarianceFrame {
     std::vector<float> colour, albedo, normal, lum, out;
     std::vector<uint64_t> nearest;
     explicit VarianceFrame(size_t npx) : colour(npx * 4), albedo(npx * 4), normal(npx * 4), lum(npx * 4), out(npx * 4), nearest(npx) {}
-    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, const trb_adaptive* ad) {
+    void render(trb_scene* s, uint32_t spp, uint32_t seed, uint32_t frame, const trb_adaptive* ad, trb_denoise_history* history = nullptr,
+                bool gradients = false) {
         for (std::vector<float>* v : {&colour, &albedo, &normal, &lum}) std::fill(v->begin(), v->end(), 0.0f);
         std::fill(nearest.begin(), nearest.end(), ~0ull);
         trb_render_cfg cfg{};
@@ -295,7 +305,15 @@ struct VarianceFrame {
         if (ad) tray::check(trb_render_adaptive_aov_lum(s, &cfg, ad, colour.data(), &aov, lum.data(), nullptr, nullptr)); // includes Scene::update_frame
         else tray::check(trb_render_aov_lum(s, &cfg, colour.data(), &aov, lum.data(), nullptr));
         const trb_denoise_frame in{colour.data(), albedo.data(), normal.data(), nearest.data()};
-        tray::check(trb_denoise_variance(s, &in, lum.data(), nullptr, out.data(), nullptr));
+        if (history && gradients) {
+            const trb_denoise_moments_gradient_output o{out.data(), nullptr, nullptr, nullptr, nullptr};
+            tray::check(trb_denoise_variance_temporal_gradient(s, history, &in, lum.data(), nullptr, seed, &o));
+        } else if (history) {
+            const trb_denoise_moments_output o{out.data(), nullptr, nullptr, nullptr};
+            tray::check(trb_denoise_variance_temporal(s, history, &in, lum.data(), nullptr, &o));
+        } else {
+            tray::check(trb_denoise_variance(s, &in, lum.data(), nullptr, out.data(), nullptr));
+        }
     }
 };
 
@@ -314,10 +332,12 @@ int single_node(const Args& a, const OutPath& out) {
         return die("--denoise-moments needs the path integrator: the scene's integrator renders no albedo, normal or depth");
     if (a.adaptive && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
         return die("--adaptive needs the path integrator: the Adaptive sampler is built for it only");
-    if (a.denoise_variance && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
-        return die("--denoise-variance needs the path integrator: the scene's integrator renders no albedo, normal or depth");
-    if (a.denoise_variance && !a.adaptive && spp < 2)
-        return die("--denoise-variance needs at least 2 samples per pixel (a variance of one sample is undefined); the scene has %u", spp);
+    const bool variance = a.denoise_variance || a.denoise_variance_temporal;
+    const char* vflag = a.denoise_variance_temporal ? "--denoise-variance-temporal" : "--denoise-variance";
+    if (variance && desc.d->integrator.type != TRB_INTEGRATOR_PATH)
+        return die("%s needs the path integrator: the scene's integrator renders no albedo, normal or depth", vflag);
+    if (variance && !a.adaptive && spp < 2)
+        return die("%s needs at least 2 samples per pixel (a variance of one sample is undefined); the scene has %u", vflag, spp);
     const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
     try {
         std::unique_ptr<tray::Scene> one;
@@ -347,14 +367,15 @@ int single_node(const Args& a, const OutPath& out) {
         std::unique_ptr<MomentsFrame> mf;
         if (a.denoise_moments) mf.reset(new MomentsFrame((size_t)dim.first * dim.second));
         std::unique_ptr<VarianceFrame> vf;
-        if (a.denoise_variance) vf.reset(new VarianceFrame((size_t)dim.first * dim.second));
-        if (a.denoise_temporal || a.denoise_moments) tray::check(trb_denoise_history_create(rd.scene, &history));
+        if (variance) vf.reset(new VarianceFrame((size_t)dim.first * dim.second));
+        if (a.denoise_temporal || a.denoise_moments || a.denoise_variance_temporal) tray::check(trb_denoise_history_create(rd.scene, &history));
         const std::unique_ptr<trb_denoise_history, trb_status (*)(trb_denoise_history*)> history_owner(history, trb_denoise_history_destroy);
         for (uint64_t i = start; i <= end; ++i) {
             config.current_frame = i;
             std::vector<uint8_t> img;
             if (vf) {
-                vf->render(rd.scene, spp, config.seed, (uint32_t)i, a.adaptive ? &ad : nullptr);
+                if (history) vf->render(rd.scene, spp, (uint32_t)(config.seed + i), (uint32_t)i, a.adaptive ? &ad : nullptr, history, a.variance_gradients);
+                else vf->render(rd.scene, spp, config.seed, (uint32_t)i, a.adaptive ? &ad : nullptr);
                 img.resize((size_t)dim.first * dim.second * 3);
                 tray::check(trb_film_to_srgb8(rd.scene, vf->out.data(), img.data()));
             } else if (mf) {
@@ -578,7 +599,7 @@ int master_node(const Args& a, const OutPath& out) {
 
 int main(int argc, char** argv) {
     bool worker = false, denoise = false, denoise_temporal = false, temporal_gradients = false, denoise_moments = false,
-         moment_gradients = false, adaptive = false, denoise_variance = false;
+         moment_gradients = false, adaptive = false, denoise_variance = false, denoise_variance_temporal = false, variance_gradients = false;
     for (int i = 1; i < argc; ++i) {
         worker = worker || std::strcmp(argv[i], "--worker") == 0;
         temporal_gradients = temporal_gradients || std::strcmp(argv[i], "--temporal-gradients") == 0;
@@ -588,6 +609,8 @@ int main(int argc, char** argv) {
         moment_gradients = moment_gradients || std::strcmp(argv[i], "--moment-gradients") == 0;
         adaptive = adaptive || std::strcmp(argv[i], "--adaptive") == 0;
         denoise_variance = denoise_variance || std::strcmp(argv[i], "--denoise-variance") == 0;
+        denoise_variance_temporal = denoise_variance_temporal || std::strcmp(argv[i], "--denoise-variance-temporal") == 0;
+        variance_gradients = variance_gradients || std::strcmp(argv[i], "--variance-gradients") == 0;
     }
     if (worker && adaptive) return die("--adaptive is not available with --worker: the wire format carries no sampler");
     if (worker && denoise) return die("--denoise is not available with --worker: the wire format carries no albedo, normal or depth");
@@ -601,6 +624,10 @@ int main(int argc, char** argv) {
         return die("--moment-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker && denoise_variance)
         return die("--denoise-variance is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && denoise_variance_temporal)
+        return die("--denoise-variance-temporal is not available with --worker: the wire format carries no albedo, normal or depth");
+    if (worker && variance_gradients)
+        return die("--variance-gradients is not available with --worker: the wire format carries no albedo, normal or depth");
     if (worker) return trb_distrib::worker_main(argc, argv);
     Args a;
     bool have_scene = false;
@@ -632,6 +659,8 @@ int main(int argc, char** argv) {
         else if (s == "--denoise-moments") a.denoise_moments = true;
         else if (s == "--moment-gradients") a.moment_gradients = true;
         else if (s == "--denoise-variance") a.denoise_variance = true;
+        else if (s == "--denoise-variance-temporal") a.denoise_variance_temporal = true;
+        else if (s == "--variance-gradients") a.variance_gradients = true;
         else if (s == "--adaptive") { // two numbers: MIN MAX
             const char* v2 = i + 2 < argc ? argv[i + 2] : nullptr;
             ok = parse_u64(v, a.ad_min) && parse_u64(v2, a.ad_max) && a.ad_min <= UINT32_MAX && a.ad_max <= UINT32_MAX;
@@ -673,6 +702,26 @@ int main(int argc, char** argv) {
         const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
         if (trb_adaptive_schedule(&ad, nullptr, nullptr, nullptr, nullptr) != TRB_OK) return die("--adaptive %llu %llu: %s", (unsigned long long)a.ad_min,
                                                                                                 (unsigned long long)a.ad_max, trb_last_error());
+    }
+    if (a.master && a.variance_gradients)
+        return die("--variance-gradients is not available with --master: the wire format carries no albedo, normal or depth");
+    if (a.variance_gradients && !a.denoise_variance_temporal) return die("--variance-gradients needs --denoise-variance-temporal");
+    if (a.denoise_variance_temporal) {
+        if (a.master)
+            return die("--denoise-variance-temporal is not available with --master: the wire format carries no albedo, normal or depth");
+        if (!a.devices.empty()) return die("--denoise-variance-temporal renders on one GPU: use --device, not --devices");
+        if (a.denoise || a.denoise_temporal || a.temporal_gradients || a.denoise_moments || a.moment_gradients || a.denoise_variance)
+            return die("--denoise-variance-temporal excludes --denoise, --denoise-temporal, --temporal-gradients, --denoise-moments, "
+                       "--moment-gradients and --denoise-variance: choose one denoiser");
+        // --spp 0 keeps the scene's film.samples, as in every mode; single_node checks that value once the scene is read
+        if (a.has_spp && a.spp == 1)
+            return die("--denoise-variance-temporal needs at least 2 samples per pixel (a variance of one sample is undefined)");
+        if (a.adaptive) {
+            const trb_adaptive ad{(uint32_t)a.ad_min, (uint32_t)a.ad_max};
+            uint32_t mn = 0;
+            if (trb_adaptive_schedule(&ad, &mn, nullptr, nullptr, nullptr) == TRB_OK && mn < 2)
+                return die("--denoise-variance-temporal needs --adaptive MIN of at least 2 samples per pixel; MIN rounds to %u", mn);
+        }
     }
     if (a.denoise_variance) {
         if (a.master) return die("--denoise-variance is not available with --master: the wire format carries no albedo, normal or depth");
