@@ -1334,6 +1334,65 @@ trb_status trb_render_adaptive_aov_lum_device(trb_scene* scene, const trb_render
                                               const trb_aov_film* d_aov, float* d_lum_w, uint32_t* d_pixel_spp, trb_stats* d_stats,
                                               void* cuda_stream);
 
+/* -- Motion vectors: each camera sample's screen-space motion to another time, from the scene's own animation (DESIGN.md §4
+ * "Motion vectors") -------------------------------------------------------------------------------------------------------------
+ * For one camera sample: its trb_camera_rays ray, that ray's time t, and its hit as trb_intersect_records returns it (instance i,
+ * world point p). dt is the caller's time offset, a finite float. Per sample, float32, left to right, never contracted:
+ *   1. p_o = M_i(t)^-1 . p, the hit in instance i's object space through the transform the trace uses (the per-path transform table of
+ *      a keyframed instance, the frame's fixed matrices of a static one).
+ *   2. p_now = M_i(t) . p_o and p_then = M_i(t + dt) . p_o, where M_i(tau) is a keyframed instance's AnimatedTransform at tau (as
+ *      eval_anim_xf evaluates it) and a static instance's fixed transform. p_now is p sent through the same transforms as p_then, so
+ *      that both terms of step 4 go through the same arithmetic.
+ *   3. r(tau, x) projects the world point x to raster coordinates with the camera active for the current frame at time tau, inverting
+ *      camera_ray's raster -> camera mapping: q = cam_world(tau)^-1 . x, X = q.x / (q.z * tan_tau), Y = q.y / (q.z * tan_tau),
+ *      r = ((X - x0) / (x1 - x0) * width, (Y - y1) / (y0 - y1) * height) with camera_setup's screen window (x0, x1, y0, y1).
+ *      tan_tau = tan(fov / 2); an animated fov is sampled once per frame at the clamped mid-frame time m (camera.rs:134-141), so
+ *      tan_t is the frame's own and tan_{t+dt} is the spline's at clamp(m + dt): one frame back gives the previous frame's fov.
+ *   4. m = r(t + dt, p_then) - r(t, p_now), in pixels. A scene with nothing keyframed, and any scene at dt = 0, gives (0, 0) exactly.
+ *   5. valid = 1 where the hit is in front of the camera (q.z > 0) at both times; else valid = 0 and m = (0, 0). A miss is invalid.
+ * dt = -(scene_time / frames) gives the backward vectors a temporal filter wants (previous position minus current, the sign of the
+ * temporal denoisers' motion output); +scene_time / frames gives forward flow.
+ * Not seen: edits made between calls (trb_scene_update_keyframes, trb_scene_replace_objects, mesh updates and refits) and a camera cut
+ * between t and t + dt: the motion is that of the current scene and the current frame's camera. Deforming meshes do not move.
+ * Path integrator on the wavefront only: Whitted, NormalsDebug and TRB_RENDER_MEGAKERNEL give TRB_UNSUPPORTED; a non-finite dt is
+ * TRB_INVALID_ARG, checked before anything is enqueued. The first motion render allocates 16 B of record per path in flight. */
+
+/* One sample's motion: valid is 1.0f or 0.0f, so a record is (v dx, v dy, v, 0), the value the motion_w film adds per unit weight.
+ * 16 bytes. */
+typedef struct trb_motion_sample {
+    float dx, dy;
+    float valid;
+    uint32_t reserved; /* 0 */
+} trb_motion_sample;
+
+/* trb_render_samples_aov that also writes each camera sample's motion record into the HOST buffer motion[n], in the same order.
+ * samples[], aov[] and the stats equal trb_render_samples_aov's; its statuses, plus dt's. */
+trb_status trb_render_samples_aov_motion(trb_scene* scene, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov,
+                                         trb_motion_sample* motion, float dt, trb_stats* stats);
+
+/* The motion_w film: RGBW in the colour film's layout (width*height*4 floats, added into). Each sample adds (w v dx, w v dy, w v, w)
+ * with the colour film's weights (RenderTarget::write: filter table, filter_pixel_width window, 2x2 lock blocks); it is the colour
+ * film's kernel over the records in place of the radiance. A pixel's motion is (x / z, y / z) where z > 0; w is the colour film's W
+ * up to float addition order.
+ * trb_render_aov_lum with the HOST motion_w film (required) and lum_w (may be NULL: not rendered). The colour film, the AOVs, lum_w and
+ * every trb_stats counter equal trb_render_aov_lum's (trb_render_aov's without lum_w); so do the statuses, plus dt's. Blocking. */
+trb_status trb_render_aov_motion(trb_scene* scene, const trb_render_cfg* cfg, float* film_rgbw, const trb_aov_film* aov, float* lum_w,
+                                 float* motion_w, float dt, trb_stats* stats);
+/* The same with DEVICE buffers under trb_render_aov_lum_device's contract; d_motion_w (required) and d_lum_w 16-byte aligned, else
+ * TRB_INVALID_ARG. */
+trb_status trb_render_aov_motion_device(trb_scene* scene, const trb_render_cfg* cfg, float* d_film_rgbw, const trb_aov_film* d_aov,
+                                        float* d_lum_w, float* d_motion_w, float dt, trb_stats* d_stats, void* cuda_stream);
+/* trb_render_adaptive_aov_lum with the HOST motion_w film (required; lum_w may be NULL): every sample of every round adds to it under
+ * the colour film's Adaptive rules. The film, AOVs, lum_w, pixel_spp, counters and statuses are trb_render_adaptive_aov_lum's (or
+ * trb_render_adaptive_aov's), plus dt's. */
+trb_status trb_render_adaptive_aov_motion(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* film_rgbw,
+                                          const trb_aov_film* aov, float* lum_w, float* motion_w, float dt, uint32_t* pixel_spp,
+                                          trb_stats* stats);
+/* The same with DEVICE buffers (d_motion_w and d_lum_w 16-byte aligned, else TRB_INVALID_ARG). */
+trb_status trb_render_adaptive_aov_motion_device(trb_scene* scene, const trb_render_cfg* cfg, const trb_adaptive* adaptive, float* d_film_rgbw,
+                                                 const trb_aov_film* d_aov, float* d_lum_w, float* d_motion_w, float dt,
+                                                 uint32_t* d_pixel_spp, trb_stats* d_stats, void* cuda_stream);
+
 /* trb_render_sharded with the Adaptive sampler: this rank's shard (interleaved chunks, or the reference's contiguous
  * ranges with cfg->shard_count == 0xffffffff) runs the Adaptive rounds into the device film, then ONE reduce to `root`,
  * whose host film_rgbw the summed film is ADDED to. pixel_spp (width*height, or NULL) receives the counts of this rank's

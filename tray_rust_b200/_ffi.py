@@ -294,6 +294,7 @@ EMIT_QUERY_DTYPE = np.dtype([("w", "<f4", 3), ("time", "<f4"), ("n", "<f4", 3), 
 KEYFRAME_DTYPE = np.dtype([("translation", "<f4", 3), ("rotation", "<f4", 4), ("scaling", "<f4", 3)])
 COLOR_KEY_DTYPE = np.dtype([("rgba", "<f4", 4), ("time", "<f4")])
 AOV_SAMPLE_DTYPE = np.dtype([("albedo", "<f4", 3), ("depth", "<f4"), ("n", "<f4", 3), ("inst", "<u4")])  # trb_aov_sample, 32 B
+MOTION_SAMPLE_DTYPE = np.dtype([("dx", "<f4"), ("dy", "<f4"), ("valid", "<f4"), ("reserved", "<u4")])  # trb_motion_sample, 16 B
 MATERIAL_DTYPE = np.dtype([("type", "<u4"), ("c0", "<f4", 3), ("c1", "<f4", 3), ("roughness", "<f4"), ("eta", "<f4"), ("merl", "<u4"),
                            ("tex", "<u4", 4)])
 
@@ -326,6 +327,8 @@ TRB_SYMBOLS = [
     "trb_render_sharded_aov", "trb_render_sharded_adaptive_aov", "trb_group_render_aov", "trb_group_render_adaptive_aov",
     "trb_render_aov_lum", "trb_render_aov_lum_device", "trb_render_adaptive_aov_lum", "trb_render_adaptive_aov_lum_device",
     "trb_denoise_variance", "trb_denoise_variance_device",
+    "trb_render_aov_motion", "trb_render_aov_motion_device", "trb_render_adaptive_aov_motion", "trb_render_adaptive_aov_motion_device",
+    "trb_render_samples_aov_motion",
     "trb_denoise_variance_temporal", "trb_denoise_variance_temporal_device", "trb_denoise_variance_temporal_gradient",
     "trb_denoise_variance_temporal_gradient_device",
 ]
@@ -428,6 +431,13 @@ def load_trb():
     lib.trb_render_aov_lum_device.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp, vp]
     lib.trb_render_adaptive_aov_lum.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, C.POINTER(Stats)]
     lib.trb_render_adaptive_aov_lum_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, vp, vp]
+    lib.trb_render_aov_motion.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp, f32, C.POINTER(Stats)]
+    lib.trb_render_aov_motion_device.argtypes = [vp, C.POINTER(RenderCfg), vp, C.POINTER(AovFilm), vp, vp, f32, vp, vp]
+    lib.trb_render_adaptive_aov_motion.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, f32, vp,
+                                                   C.POINTER(Stats)]
+    lib.trb_render_adaptive_aov_motion_device.argtypes = [vp, C.POINTER(RenderCfg), C.POINTER(Adaptive), vp, C.POINTER(AovFilm), vp, vp, f32, vp,
+                                                          vp, vp]
+    lib.trb_render_samples_aov_motion.argtypes = [vp, C.POINTER(RenderCfg), sz, vp, vp, vp, f32, C.POINTER(Stats)]
     lib.trb_denoise_variance.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp]
     lib.trb_denoise_variance_device.argtypes = [vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseParams), vp, vp, vp]
     lib.trb_denoise_variance_temporal.argtypes = [vp, vp, C.POINTER(DenoiseFrame), vp, C.POINTER(DenoiseTemporalParams),

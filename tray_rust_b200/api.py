@@ -81,6 +81,15 @@ def decode_nearest(nearest):
     return (nearest >> np.uint64(32)).astype(np.uint32).view(np.float32), (nearest & np.uint64(0xffffffff)).astype(np.uint32)
 
 
+def decode_motion(motion_w):
+    """The (height, width, 2) float32 motion in pixels of a ``motion_w`` film (include/trb.h "Motion vectors"): its first two
+    channels over its third where that is positive, NaN elsewhere."""
+    motion_w = np.asarray(motion_w, dtype=np.float32)
+    z = motion_w[..., 2:3]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(z > 0, motion_w[..., :2] / z, np.float32(np.nan)).astype(np.float32)
+
+
 def _denoise_params(params):
     unknown = set(params) - set(F.DENOISE_DEFAULTS)
     if unknown:
@@ -332,39 +341,68 @@ class Scene(_Base):
         cfg = _cfg(**kw)
         self._check(self._lib.trb_render_device(self._h, C.byref(cfg), d_film_ptr, d_stats_ptr, stream))
 
-    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, lum=False, **kw):
+    def frame_step(self):
+        """scene_time / frames in float32: one frame's time, as the renders step the frames."""
+        return float(np.float32(self._desc.film.scene_time) / np.float32(self._desc.film.frames))
+
+    def _motion_dt(self, motion):
+        """render_*(motion=...): False / None: no motion film; True: one frame back, -scene_time / frames; a number: that dt"""
+        if motion is None or motion is False:
+            return None
+        return -self.frame_step() if motion is True else float(motion)
+
+    def render_aov(self, film=None, albedo=True, normal=True, nearest=True, lum=False, motion=False, **kw):
         """trb_render_aov: the colour film and the AOVs of the same render (DESIGN.md §4 "AOVs"), all accumulated into.
         albedo / normal: True (allocate, zero), False / None (not rendered) or a float32 (height, width, 4) film; nearest: True
         (allocate, all ones), False / None or a uint64 (height, width) array. lum: True or a float32 (height, width, 4) film adds
         the lum_w film of the samples' luminance moments (trb_render_aov_lum, DESIGN.md §4 "Sample variance") as aovs["lum_w"].
+        motion: True (dt = -scene_time / frames) or a dt adds the motion_w film (trb_render_aov_motion, include/trb.h "Motion
+        vectors") as aovs["motion_w"]; decode_motion turns it into pixels.
         Returns (film, aovs, Stats) where aovs maps "albedo_w", "normal_w" and "nearest" to the arrays rendered."""
         cfg = _cfg(**kw)
         film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest, lum)
         st = F.Stats()
-        if "lum_w" in aovs:
+        dt = self._motion_dt(motion)
+        if dt is not None:
+            aovs["motion_w"] = np.zeros((self.height, self.width, 4), np.float32)
+            self._check(self._lib.trb_render_aov_motion(self._h, C.byref(cfg), F.ptr(film), C.byref(out), F.ptr(aovs["lum_w"]) if "lum_w" in aovs else None,
+                                                        F.ptr(aovs["motion_w"]), dt, C.byref(st)))
+        elif "lum_w" in aovs:
             self._check(self._lib.trb_render_aov_lum(self._h, C.byref(cfg), F.ptr(film), C.byref(out), F.ptr(aovs["lum_w"]), C.byref(st)))
         else:
             self._check(self._lib.trb_render_aov(self._h, C.byref(cfg), F.ptr(film), C.byref(out), C.byref(st)))
         return film, aovs, st
 
-    def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, d_lum=None, **kw):
+    def render_aov_device(self, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_stats=None, stream=None, d_lum=None, d_motion=None,
+                          motion_dt=None, **kw):
         """trb_render_aov_device: device films of height*width*4 float32 (16-byte aligned) and a device nearest buffer of height*width
         uint64 (8-byte aligned; initialise it to all ones), pointers as ints, any AOV None. Enqueued on `stream` (a cudaStream_t as an
         int; None = default stream) without host synchronisation. Never updates the frame. d_lum: a device lum_w film
-        (trb_render_aov_lum_device), or None."""
+        (trb_render_aov_lum_device), or None. d_motion: a device motion_w film (trb_render_aov_motion_device) with motion_dt (None:
+        -scene_time / frames), or None."""
         cfg = _cfg(**kw)
         out = F.AovFilm(d_albedo, d_normal, d_nearest)
-        if d_lum is not None:
+        if d_motion is not None:
+            dt = -self.frame_step() if motion_dt is None else float(motion_dt)
+            self._check(self._lib.trb_render_aov_motion_device(self._h, C.byref(cfg), d_film, C.byref(out), d_lum, d_motion, dt, d_stats, stream))
+        elif d_lum is not None:
             self._check(self._lib.trb_render_aov_lum_device(self._h, C.byref(cfg), d_film, C.byref(out), d_lum, d_stats, stream))
         else:
             self._check(self._lib.trb_render_aov_device(self._h, C.byref(cfg), d_film, C.byref(out), d_stats, stream))
 
-    def render_samples_aov(self, **kw):
-        """trb_render_samples_aov: (samples as render_samples, AOV records as AOV_SAMPLE_DTYPE in the same order, Stats)."""
+    def render_samples_aov(self, motion=False, **kw):
+        """trb_render_samples_aov: (samples as render_samples, AOV records as AOV_SAMPLE_DTYPE in the same order, Stats). motion: True
+        (dt = -scene_time / frames) or a dt: trb_render_samples_aov_motion, returning (samples, aov, motion records as
+        MOTION_SAMPLE_DTYPE, Stats)."""
         cfg = _cfg(**kw)
         n = self._n_samples(cfg)
         out, aov = np.zeros(n, F.SAMPLE_DTYPE), np.zeros(n, F.AOV_SAMPLE_DTYPE)
         st = F.Stats()
+        dt = self._motion_dt(motion)
+        if dt is not None:
+            mo = np.zeros(n, F.MOTION_SAMPLE_DTYPE)
+            self._check(self._lib.trb_render_samples_aov_motion(self._h, C.byref(cfg), n, F.ptr(out), F.ptr(aov), F.ptr(mo), dt, C.byref(st)))
+            return out, aov, mo, st
         self._check(self._lib.trb_render_samples_aov(self._h, C.byref(cfg), n, F.ptr(out), F.ptr(aov), C.byref(st)))
         return out, aov, st
 
@@ -891,16 +929,22 @@ class Scene(_Base):
                                                           C.byref(st)))
         return out, spp, st
 
-    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, lum=False, **kw):
+    def render_adaptive_aov(self, min_spp, max_spp, film=None, albedo=True, normal=True, nearest=True, lum=False, motion=False, **kw):
         """trb_render_adaptive_aov: render_adaptive with the AOVs of the samples it takes (DESIGN.md §4 "Adaptive AOVs"), all
-        accumulated into; albedo / normal / nearest / lum as for render_aov (lum: trb_render_adaptive_aov_lum). Returns (film, aovs,
-        pixel_spp, Stats)."""
+        accumulated into; albedo / normal / nearest / lum / motion as for render_aov (lum: trb_render_adaptive_aov_lum, motion:
+        trb_render_adaptive_aov_motion). Returns (film, aovs, pixel_spp, Stats)."""
         cfg = _cfg(**kw)
         film, aovs, out = _aov_outputs(self.height, self.width, film, albedo, normal, nearest, lum)
         spp = np.zeros((self.height, self.width), np.uint32)
         st = F.Stats()
         ad = F.Adaptive(min_spp, max_spp)
-        if "lum_w" in aovs:
+        dt = self._motion_dt(motion)
+        if dt is not None:
+            aovs["motion_w"] = np.zeros((self.height, self.width, 4), np.float32)
+            self._check(self._lib.trb_render_adaptive_aov_motion(self._h, C.byref(cfg), C.byref(ad), F.ptr(film), C.byref(out),
+                                                                 F.ptr(aovs["lum_w"]) if "lum_w" in aovs else None, F.ptr(aovs["motion_w"]), dt,
+                                                                 F.ptr(spp), C.byref(st)))
+        elif "lum_w" in aovs:
             self._check(self._lib.trb_render_adaptive_aov_lum(self._h, C.byref(cfg), C.byref(ad), F.ptr(film), C.byref(out), F.ptr(aovs["lum_w"]),
                                                               F.ptr(spp), C.byref(st)))
         else:
@@ -908,14 +952,19 @@ class Scene(_Base):
         return film, aovs, spp, st
 
     def render_adaptive_aov_device(self, min_spp, max_spp, d_film, d_albedo=None, d_normal=None, d_nearest=None, d_pixel_spp=None, d_stats=None,
-                                   stream=None, d_lum=None, **kw):
+                                   stream=None, d_lum=None, d_motion=None, motion_dt=None, **kw):
         """trb_render_adaptive_aov_device: render_adaptive_device's pointers plus the AOV buffers of render_aov_device (any None).
         Enqueued on `stream` without host synchronisation. Never updates the frame. d_lum: a device lum_w film
-        (trb_render_adaptive_aov_lum_device), or None."""
+        (trb_render_adaptive_aov_lum_device), or None; d_motion / motion_dt as for render_aov_device
+        (trb_render_adaptive_aov_motion_device)."""
         cfg = _cfg(**kw)
         out = F.AovFilm(d_albedo, d_normal, d_nearest)
         ad = F.Adaptive(min_spp, max_spp)
-        if d_lum is not None:
+        if d_motion is not None:
+            dt = -self.frame_step() if motion_dt is None else float(motion_dt)
+            self._check(self._lib.trb_render_adaptive_aov_motion_device(self._h, C.byref(cfg), C.byref(ad), d_film, C.byref(out), d_lum, d_motion, dt,
+                                                                        d_pixel_spp, d_stats, stream))
+        elif d_lum is not None:
             self._check(self._lib.trb_render_adaptive_aov_lum_device(self._h, C.byref(cfg), C.byref(ad), d_film, C.byref(out), d_lum, d_pixel_spp,
                                                                      d_stats, stream))
         else:

@@ -400,6 +400,10 @@ struct trb_scene {
     // (albedo, depth) in d_aov[p] and (n, inst bits) in d_aov[aov_capacity + p], 32 bytes
     float4* d_aov = nullptr;
     size_t aov_capacity = 0;
+    // motion records of a film render's pass (trb_render_*aov_motion*), allocated by the first motion render at the path-state capacity:
+    // per path (v dx, v dy, v, 0), 16 bytes
+    float4* d_motion = nullptr;
+    size_t motion_capacity = 0;
     // denoiser scratch (trb_denoise*; trb::DnScratch), allocated by the first denoise for the film's pixel count and released with the film;
     // denoise_moments: it also holds the moment records of trb_denoise_moments* (trb::DN_MOMENTS_BYTES_PER_PIXEL)
     void* d_denoise = nullptr;
@@ -415,7 +419,7 @@ struct trb_scene {
     uint64_t object_generation = 0;
     ~trb_scene() {
         for (void* p : {(void*)d_ad_state, (void*)d_ad_list[0], (void*)d_ad_list[1], (void*)d_ad_index[0], (void*)d_ad_index[1], (void*)d_ad_flags,
-                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, d_denoise, d_shard_aov}) if (p) cudaFree(p);
+                        (void*)d_ad_count, (void*)d_ad_spp, d_film_scratch, (void*)d_aov, (void*)d_motion, d_denoise, d_shard_aov}) if (p) cudaFree(p);
         for (auto& b : block_lists) cudaFree(b.dev);
         for (void* p : wf_allocs) cudaFree(p);
         for (auto& e : trace_events) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
@@ -623,8 +627,13 @@ trb_status launch_render_t(trb_scene* s, const trb::RenderParams& rp, uint32_t f
     return TRB_OK;
 }
 // The AOVs a render asks for (DESIGN.md §4 "AOVs"): samples = the caller's device records (per-sample mode), else the film outputs
-// (any may be nullptr); lum_w: the sample-variance film of the *_lum renders (include/trb.h "Sample variance")
-struct AovRequest { trb_aov_sample* samples; float4* albedo_w; float4* normal_w; unsigned long long* nearest; float4* lum_w = nullptr; };
+// (any may be nullptr); lum_w: the sample-variance film of the *_lum renders (include/trb.h "Sample variance"); motion_samples (the
+// caller's device records, per-sample mode) or motion_w (the film) with dt: the motion vectors of the *_motion renders (include/trb.h
+// "Motion vectors")
+struct AovRequest {
+    trb_aov_sample* samples; float4* albedo_w; float4* normal_w; unsigned long long* nearest; float4* lum_w = nullptr;
+    trb_motion_sample* motion_samples = nullptr; float4* motion_w = nullptr; float dt = 0.0f;
+};
 
 // the path-indexed AOV records of film passes, at the path-state capacity
 trb_status ensure_aov(trb_scene* s) {
@@ -636,6 +645,47 @@ trb_status ensure_aov(trb_scene* s) {
     if (r != TRB_OK) return r;
     s->aov_capacity = s->wf_capacity;
     return TRB_OK;
+}
+// the path-indexed motion records of film passes, likewise; only the renders with a motion_w film allocate them
+trb_status ensure_motion(trb_scene* s) {
+    if (s->motion_capacity >= s->wf_capacity) return TRB_OK;
+    CU(cudaDeviceSynchronize());
+    if (s->d_motion) cudaFree(s->d_motion);
+    s->d_motion = nullptr; s->motion_capacity = 0;
+    const trb_status r = device_alloc(reinterpret_cast<void**>(&s->d_motion), s->wf_capacity * sizeof(float4), "motion records");
+    if (r != TRB_OK) return r;
+    s->motion_capacity = s->wf_capacity;
+    return TRB_OK;
+}
+
+// The projection of the motion records at this frame (include/trb.h "Motion vectors"). An animated fov is sampled once per frame at
+// the clamped mid-frame time, as trb_scene_update_frame samples it (camera.rs:134-141); at t + dt it is sampled at mid-frame + dt, so
+// dt = 0 gives the frame's own fov and dt = -(one frame) the previous frame's.
+float motion_tan(const trb_scene* s, float dt) {
+    const trb_camera& c = s->cameras[s->active_camera];
+    float fov = c.fov;
+    if (c.n_fov_ctrl) {
+        const float* kn = s->fov_floats.data() + c.fov_knot_first;
+        const float lo = kn[c.fov_degree], hi = kn[c.n_fov_knots - 1 - c.fov_degree];
+        float t = (s->last_start + s->last_end) / 2.0f + dt;
+        t = t < lo ? lo : (t > hi ? hi : t);
+        fov = trbh::spline_point_f32(c.fov_degree, s->fov_floats.data() + c.fov_ctrl_first, kn, c.n_fov_knots, t);
+    }
+    Mat4 px_to_cam; float scaling[3];
+    trbh::camera_setup(fov, s->film.width, s->film.height, px_to_cam, scaling);
+    return scaling[0];
+}
+trb::MotionCam motion_camera(const trb_scene* s, float dt) {
+    trb::MotionCam mc{};
+    std::memcpy(mc.cam_inv, s->cam_inv, 64);
+    mc.tan_now = motion_tan(s, 0.0f);
+    mc.tan_then = motion_tan(s, dt);
+    mc.dt = dt;
+    const float aspect = (float)s->film.width / (float)s->film.height; // camera_setup's screen window
+    if (aspect > 1.0f) { mc.x0 = -aspect; mc.x1 = aspect; mc.y0 = -1.0f; mc.y1 = 1.0f; }
+    else { mc.x0 = -1.0f; mc.x1 = 1.0f; mc.y0 = -1.0f / aspect; mc.y1 = 1.0f / aspect; }
+    mc.w = (float)s->film.width; mc.h = (float)s->film.height;
+    return mc;
 }
 
 trb_status ensure_wavefront(trb_scene* s, size_t n_paths) {
@@ -840,6 +890,16 @@ trb_status wavefront_rounds(trb_scene* s, const trb::RenderParams& rp, const trb
             } else if (anim) trb::k_wf_aov<true><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
             else trb::k_wf_aov<false><<<agrid, 128, 0, st>>>(s->ds, wf, lo, hi, step);
             g_launches++;
+            if (aov->motion_samples || aov->motion_w) { // the motion records from the same primary hits
+                const trb::MotionCam mc = motion_camera(s, aov->dt);
+                float4* mo = mode == 1 ? reinterpret_cast<float4*>(aov->motion_samples) : s->d_motion;
+                if (rp.ad_state) {
+                    if (anim) trb::k_wf_motion_ad<true><<<agrid, 128, 0, st>>>(s->ds, wf, mc, mo);
+                    else trb::k_wf_motion_ad<false><<<agrid, 128, 0, st>>>(s->ds, wf, mc, mo);
+                } else if (anim) trb::k_wf_motion<true><<<agrid, 128, 0, st>>>(s->ds, wf, mc, mo);
+                else trb::k_wf_motion<false><<<agrid, 128, 0, st>>>(s->ds, wf, mc, mo);
+                g_launches++;
+            }
         }
         if (mode == 0) launch_shade<0>(s, rp, wf, round, st);
         else if (mode == 1) launch_shade<1>(s, rp, wf, round, st);
@@ -918,6 +978,15 @@ trb_status launch_wavefront(trb_scene* s, const trb::RenderParams& rp, uint32_t 
                 else trb::k_wf_film<false, true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wf, s->d_aov);
                 g_launches++;
             }
+            if (aov->motion_w) { // the colour film's kernel over the motion records, which are (v dx, v dy, v, 0) already
+                ra.film = aov->motion_w; wa.rad = s->d_motion;
+                if (rp.ad_state) {
+                    if (tu.film_v2) trb::k_wf_film_v2<true><<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                    else trb::k_wf_film<true><<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                } else if (tu.film_v2) trb::k_wf_film_v2<<<film_grid, trb::RENDER_THREADS, (size_t)4 * T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                else trb::k_wf_film<<<film_grid, trb::RENDER_THREADS, (size_t)T * T * sizeof(float4), st>>>(s->ds, ra, wa);
+                g_launches++;
+            }
             if (aov->nearest) {
                 const unsigned ngrid = (unsigned)std::min<size_t>((n_paths + 255) / 256, (size_t)s->sm_count * 8);
                 if (rp.ad_state) trb::k_wf_nearest_ad<<<ngrid, 256, 0, st>>>(s->ds, rp, s->d_aov, s->d_aov + s->aov_capacity, aov->nearest);
@@ -951,7 +1020,8 @@ trb_status render_passes(trb_scene* s, trb::RenderParams rp, uint32_t flags, int
         if (r != TRB_OK) return r;
     }
     if (aov && mode == 0) {
-        const trb_status r = ensure_aov(s);
+        trb_status r = ensure_aov(s);
+        if (r == TRB_OK && aov->motion_w) r = ensure_motion(s);
         if (r != TRB_OK) return r;
     }
     const uint64_t cap = std::max<uint64_t>(want, 64);  // paths per pass actually used (a larger state left by an earlier call is not required)
@@ -1015,6 +1085,7 @@ trb_status render_adaptive_rounds(trb_scene* s, const trbh::AdSchedule& sch, trb
         if (r != TRB_OK) return r;
     }
     if (aov && (r = ensure_aov(s)) != TRB_OK) return r;
+    if (aov && aov->motion_w && (r = ensure_motion(s)) != TRB_OK) return r;
     const uint64_t cap = want;
     rp.ad_state = s->d_ad_state;
     rp.ad_min = sch.min; rp.ad_max = sch.max; rp.ad_step = sch.step; rp.ad_max_per_pixel = sch.max_per_pixel;
@@ -2749,18 +2820,22 @@ void add_film(float* film, const float* src, size_t n) {
 }
 
 // The device side of a host AOV render (trb_render_aov, trb_render_adaptive_aov): films from zero, added into the caller's
-// afterwards; nearest from the caller's. lum_w (the *_lum renders): the lum_w film, staged as albedo_w and normal_w.
+// afterwards; nearest from the caller's. lum_w (the *_lum renders) and motion_w (the *_motion renders, with dt): staged as albedo_w
+// and normal_w.
 struct HostAov {
-    DeviceBuffer albedo, normal, nearest, lum;
+    DeviceBuffer albedo, normal, nearest, lum, motion;
     AovRequest req{nullptr, nullptr, nullptr, nullptr};
     const trb_aov_film* aov = nullptr; // nullptr: no AOV output asked for
     float* lum_w = nullptr;
-    trb_status stage(const trb_aov_film* a, size_t npx, float* lum_host = nullptr) {
-        if (!a || !(a->albedo_w || a->normal_w || a->nearest || lum_host)) return TRB_OK;
+    float* motion_w = nullptr;
+    trb_status stage(const trb_aov_film* a, size_t npx, float* lum_host = nullptr, float* motion_host = nullptr, float dt = 0.0f) {
+        if (!a || !(a->albedo_w || a->normal_w || a->nearest || lum_host || motion_host)) return TRB_OK;
         aov = a;
         lum_w = lum_host;
+        motion_w = motion_host;
         trb_status r;
-        for (auto [h, d] : {std::pair<const float*, DeviceBuffer*>{a->albedo_w, &albedo}, {a->normal_w, &normal}, {lum_host, &lum}}) {
+        for (auto [h, d] : {std::pair<const float*, DeviceBuffer*>{a->albedo_w, &albedo}, {a->normal_w, &normal}, {lum_host, &lum},
+                            {motion_host, &motion}}) {
             if (!h) continue;
             if ((r = d->alloc(npx * sizeof(float4), "AOV films")) != TRB_OK) return r;
             CU(cudaMemsetAsync(d->p, 0, npx * sizeof(float4), 0));
@@ -2769,7 +2844,7 @@ struct HostAov {
             if ((r = nearest.alloc(npx * sizeof(uint64_t), "AOV films")) != TRB_OK) return r;
             CU(cudaMemcpy(nearest.p, a->nearest, npx * sizeof(uint64_t), cudaMemcpyHostToDevice));
         }
-        req = {nullptr, albedo.as<float4>(), normal.as<float4>(), nearest.as<unsigned long long>(), lum.as<float4>()};
+        req = {nullptr, albedo.as<float4>(), normal.as<float4>(), nearest.as<unsigned long long>(), lum.as<float4>(), nullptr, motion.as<float4>(), dt};
         return TRB_OK;
     }
     const AovRequest* request() const { return aov ? &req : nullptr; }
@@ -2777,7 +2852,7 @@ struct HostAov {
         if (!aov) return TRB_OK;
         std::vector<float> h;
         for (auto [dst, src] : {std::pair<float*, void*>{aov->albedo_w, albedo.p}, std::pair<float*, void*>{aov->normal_w, normal.p},
-                                std::pair<float*, void*>{lum_w, lum.p}}) {
+                                std::pair<float*, void*>{lum_w, lum.p}, std::pair<float*, void*>{motion_w, motion.p}}) {
             if (!dst) continue;
             h.resize(npx * 4);
             CU(cudaMemcpy(h.data(), src, npx * sizeof(float4), cudaMemcpyDeviceToHost));
@@ -2789,7 +2864,8 @@ struct HostAov {
 };
 
 // trb_render's body; aov: the host AOV outputs of trb_render_aov (nullptr: none)
-trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats, float* lum_w = nullptr) {
+trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, trb_stats* stats, float* lum_w = nullptr,
+                       float* motion_w = nullptr, float dt = 0.0f) {
     CU(cudaSetDevice(s->device));
     float update_ms = 0.f;
     if (!(cfg->flags & TRB_RENDER_NO_UPDATE)) { // Exec::render: scene.update_frame first (multithreaded.rs:57-60)
@@ -2803,7 +2879,7 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     HostAov ha;
-    trb_status r = ha.stage(aov, npx, lum_w);
+    trb_status r = ha.stage(aov, npx, lum_w, motion_w, dt);
     if (r != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     r = render_device(s, cfg, reinterpret_cast<float*>(s->d_film), reinterpret_cast<trb_stats*>(s->d_stats), 0, ha.request());
@@ -2819,7 +2895,8 @@ trb_status render_host(trb_scene* s, const trb_render_cfg* cfg, float* film, con
 }
 
 // trb_render_samples' body; aov: the host AOV records of trb_render_samples_aov (nullptr: none)
-trb_status render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov, trb_stats* stats) {
+trb_status render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov, trb_stats* stats,
+                          trb_motion_sample* motion = nullptr, float dt = 0.0f) {
     CU(cudaSetDevice(s->device));
     uint32_t spp, first, count, nb;
     const uint2* d_blocks = nullptr;
@@ -2832,9 +2909,10 @@ trb_status render_samples(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb
     trb::RenderParams rp{};
     rp.blocks = d_blocks; rp.n_blocks = nb; rp.spp = spp; rp.sample_first = first; rp.sample_count = count; rp.seed = cfg->seed;
     rp.work_counter = s->d_counter; rp.film = nullptr; rp.stats = s->d_stats; rp.error_flag = s->d_error;
-    r = run_counted(s, {}, {{samples, n * sizeof(trb_sample)}, {aov, n * sizeof(trb_aov_sample)}}, [&](const DeviceBuffer* d) {
+    r = run_counted(s, {}, {{samples, n * sizeof(trb_sample)}, {aov, n * sizeof(trb_aov_sample)}, {motion, n * sizeof(trb_motion_sample)}},
+                    [&](const DeviceBuffer* d) {
         rp.samples_out = d[0].as<trb_sample>();
-        const AovRequest req{d[1].as<trb_aov_sample>(), nullptr, nullptr, nullptr};
+        const AovRequest req{d[1].as<trb_aov_sample>(), nullptr, nullptr, nullptr, nullptr, d[2].as<trb_motion_sample>(), nullptr, dt};
         return launch_render(s, rp, cfg->flags, 1, 0, aov ? &req : nullptr);
     });
     return r != TRB_OK ? r : stats_readback(s, stats, 0.f);
@@ -2905,6 +2983,46 @@ trb_status trb_render_aov_lum(trb_scene* s, const trb_render_cfg* cfg, float* fi
     const trb_status r = aov_supported(s, cfg);
     if (r != TRB_OK) return r;
     return render_host(s, cfg, film, aov, stats, lum_w);
+}
+
+// ---- motion vectors (include/trb.h "Motion vectors") ----------------------------------------------------------------------------
+namespace {
+trb_status motion_dt(float dt) { return std::isfinite(dt) ? TRB_OK : fail(TRB_INVALID_ARG, "motion dt must be finite"); }
+} // namespace
+
+trb_status trb_render_aov_motion_device(trb_scene* s, const trb_render_cfg* cfg, float* d_film, const trb_aov_film* d_aov, float* d_lum_w, float* d_motion_w,
+                                        float dt, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !d_film || !d_aov || !d_motion_w) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    trb_status r = aov_supported(s, cfg);
+    if (r == TRB_OK)
+        r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_lum_w, 16}, {d_motion_w, 16}, {d_aov->nearest, 8}},
+                          "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    if (r == TRB_OK) r = motion_dt(dt);
+    if (r != TRB_OK) return r;
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest), reinterpret_cast<float4*>(d_lum_w), nullptr,
+                         reinterpret_cast<float4*>(d_motion_w), dt};
+    return render_device(s, cfg, d_film, d_stats, static_cast<cudaStream_t>(stream), &req);
+}
+
+trb_status trb_render_aov_motion(trb_scene* s, const trb_render_cfg* cfg, float* film, const trb_aov_film* aov, float* lum_w, float* motion_w, float dt,
+                                 trb_stats* stats) {
+    if (!s || !cfg || !film || !aov || !motion_w) return fail(TRB_INVALID_ARG, "null argument");
+    trb_status r = aov_supported(s, cfg);
+    if (r == TRB_OK) r = motion_dt(dt);
+    if (r != TRB_OK) return r;
+    return render_host(s, cfg, film, aov, stats, lum_w, motion_w, dt);
+}
+
+trb_status trb_render_samples_aov_motion(trb_scene* s, const trb_render_cfg* cfg, size_t n, trb_sample* samples, trb_aov_sample* aov,
+                                         trb_motion_sample* motion, float dt, trb_stats* stats) {
+    if (!s || !cfg || !samples || !aov || !motion) return fail(TRB_INVALID_ARG, "null argument");
+    if (!s->frame_ready) return fail(TRB_INVALID_ARG, "Update frame must be called before rendering");
+    trb_status r = aov_supported(s, cfg);
+    if (r == TRB_OK) r = motion_dt(dt);
+    if (r != TRB_OK) return r;
+    return render_samples(s, cfg, n, samples, aov, stats, motion, dt);
 }
 
 namespace {
@@ -3784,7 +3902,7 @@ trb_status trb_host_adaptive_decide(const trb_adaptive* ad, const float* lum, si
 namespace {
 // trb_render_adaptive's body; aov: the host AOV outputs of trb_render_adaptive_aov (nullptr: none)
 trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, uint32_t* pixel_spp,
-                                trb_stats* stats, float* lum_w = nullptr) {
+                                trb_stats* stats, float* lum_w = nullptr, float* motion_w = nullptr, float dt = 0.0f) {
     trbh::AdSchedule sch;
     trb_status r = adaptive_check(s, cfg, ad, sch);
     if (r != TRB_OK) return r;
@@ -3806,7 +3924,7 @@ trb_status render_adaptive_host(trb_scene* s, const trb_render_cfg* cfg, const t
     CU(cudaMemsetAsync(s->d_film, 0, npx * sizeof(float4), 0));
     CU(cudaMemsetAsync(s->d_stats, 0, sizeof(trb::DStats), 0));
     HostAov ha;
-    if ((r = ha.stage(aov, npx, lum_w)) != TRB_OK) return r;
+    if ((r = ha.stage(aov, npx, lum_w, motion_w, dt)) != TRB_OK) return r;
     CU(cudaEventRecord(s->ev0, 0));
     if (nb) { // an empty selection renders nothing (block_queue.rs:42-44)
         r = ensure_adaptive(s);
@@ -3926,6 +4044,27 @@ trb_status trb_render_adaptive_aov_lum_device(trb_scene* s, const trb_render_cfg
     if (r != TRB_OK) return r;
     const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
                          reinterpret_cast<unsigned long long*>(d_aov->nearest), reinterpret_cast<float4*>(d_lum_w)};
+    return render_adaptive_device(s, cfg, ad, d_film, &req, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
+}
+
+trb_status trb_render_adaptive_aov_motion(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* film, const trb_aov_film* aov, float* lum_w,
+                                          float* motion_w, float dt, uint32_t* pixel_spp, trb_stats* stats) {
+    if (!s || !cfg || !ad || !film || !aov || !motion_w) return fail(TRB_INVALID_ARG, "null argument");
+    const trb_status r = motion_dt(dt);
+    if (r != TRB_OK) return r;
+    return render_adaptive_host(s, cfg, ad, film, aov, pixel_spp, stats, lum_w, motion_w, dt);
+}
+
+trb_status trb_render_adaptive_aov_motion_device(trb_scene* s, const trb_render_cfg* cfg, const trb_adaptive* ad, float* d_film, const trb_aov_film* d_aov,
+                                                 float* d_lum_w, float* d_motion_w, float dt, uint32_t* d_pixel_spp, trb_stats* d_stats, void* stream) {
+    if (!s || !cfg || !ad || !d_film || !d_aov || !d_motion_w) return fail(TRB_INVALID_ARG, "null argument");
+    trb_status r = check_aligned({{d_film, 16}, {d_aov->albedo_w, 16}, {d_aov->normal_w, 16}, {d_lum_w, 16}, {d_motion_w, 16}, {d_aov->nearest, 8}},
+                                 "device films must be 16-byte aligned, the nearest buffer 8-byte aligned");
+    if (r == TRB_OK) r = motion_dt(dt);
+    if (r != TRB_OK) return r;
+    const AovRequest req{nullptr, reinterpret_cast<float4*>(d_aov->albedo_w), reinterpret_cast<float4*>(d_aov->normal_w),
+                         reinterpret_cast<unsigned long long*>(d_aov->nearest), reinterpret_cast<float4*>(d_lum_w), nullptr,
+                         reinterpret_cast<float4*>(d_motion_w), dt};
     return render_adaptive_device(s, cfg, ad, d_film, &req, d_pixel_spp, d_stats, static_cast<cudaStream_t>(stream));
 }
 

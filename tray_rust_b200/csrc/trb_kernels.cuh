@@ -2841,6 +2841,79 @@ __global__ void __launch_bounds__(256) k_wf_nearest_ad(const __grid_constant__ D
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Motion vectors (include/trb.h "Motion vectors"): one (v dx, v dy, v, 0) record per camera sample from its primary hit, between the
+// round-0 trace and shade like k_wf_aov. Since dx = dy = 0 where v = 0, the record is also the value the motion_w film adds per unit
+// weight: the colour film's kernel reads it in place of the radiance.
+// ------------------------------------------------------------------------------------------
+// The raster projection at the two times: the world -> camera matrix of a static camera (the frame's cam_world inverse; a keyframed
+// camera evaluates its own at each time), tan(fov / 2) at t and at t + dt, camera_setup's screen window and the film size.
+struct MotionCam {
+    float cam_inv[16];
+    float tan_now, tan_then, dt;
+    float x0, x1, y0, y1, w, h;
+};
+// r(tau, x): camera_ray's raster -> camera mapping inverted, as dn_reproject inverts it; false unless x is in front of the camera
+template <bool ANIM>
+__device__ __forceinline__ bool motion_raster(const DScene& sc, const MotionCam& mc, float tau, float tan_fov, f3 x, float& rx, float& ry) {
+    float inv[16];
+    if (ANIM && sc.cam.animated) {
+        float mat[16];
+        eval_anim_xf(sc, sc.cam.spline_first, sc.cam.n_splines, tau, inv, mat);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) inv[i] = mc.cam_inv[i];
+    }
+    const f3 q = xf_point(inv, x);
+    const float X = q.x / (q.z * tan_fov), Y = q.y / (q.z * tan_fov);
+    rx = (X - mc.x0) / (mc.x1 - mc.x0) * mc.w;
+    ry = (Y - mc.y1) / (mc.y0 - mc.y1) * mc.h;
+    return q.z > 0.0f;
+}
+// Per path of the pass (round 0): the hit's world point as surface_at computes it, p_o = M_i(t)^-1 p through the transform the trace
+// and the transform table use, then r(t + dt, M_i(t + dt) p_o) - r(t, M_i(t) p_o). ANIM false: no keyframed transform at all, so the
+// two points are one (a static scene's records are (0, 0, v) unless the fov is animated).
+template <bool ANIM>
+__device__ __forceinline__ void wf_motion_paths(const DScene& sc, const WfState& wf, const MotionCam& mc, uint32_t n, float4* __restrict__ out) {
+    for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n; p += gridDim.x * blockDim.x) {
+        const uint4 h4 = wf.hit[p];
+        float4 rec = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (h4.x != TRB_MISS) {
+            const float4 o4 = wf.org[p], c4 = wf.cont[p];
+            const float time = wf.thr[p].w;
+            const DInstance& in = sc.instances[h4.x];
+            float m[16], w[16];
+            instance_inv_mat<ANIM>(sc, in, time, m, w, wf_xf_row<ANIM>(wf, p));
+            const f3 o = xf_point(m, mk(o4.x, o4.y, o4.z)), d = xf_vector(m, mk(c4.x, c4.y, c4.z));
+            const f3 pw = xf_point(w, o + d * c4.w); // surface_at's s.p
+            const f3 po = xf_point(m, pw);
+            const f3 p_now = xf_point(w, po);
+            f3 p_then = p_now;
+            if (ANIM && (__ldg(&in.flags) & DI_ANIM_XF)) {
+                float inv2[16], mat2[16];
+                eval_anim_xf(sc, __ldg(&in.spline_first), __ldg(&in.n_splines), time + mc.dt, inv2, mat2);
+                p_then = xf_point(mat2, po);
+            }
+            float x0, y0, x1, y1;
+            const bool v0 = motion_raster<ANIM>(sc, mc, time, mc.tan_now, p_now, x0, y0);
+            const bool v1 = motion_raster<ANIM>(sc, mc, time + mc.dt, mc.tan_then, p_then, x1, y1);
+            if (v0 && v1) rec = make_float4(x1 - x0, y1 - y0, 1.0f, 0.0f);
+        }
+        out[p] = rec;
+    }
+}
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_wf_motion(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, const __grid_constant__ MotionCam mc,
+                                                   float4* __restrict__ out) {
+    wf_motion_paths<ANIM>(sc, wf, mc, wf.n_paths, out);
+}
+// k_wf_motion for an Adaptive pass: the paths it really holds (WF_N_PATHS), as k_wf_aov_ad
+template <bool ANIM>
+__global__ void __launch_bounds__(128) k_wf_motion_ad(const __grid_constant__ DScene sc, const __grid_constant__ WfState wf, const __grid_constant__ MotionCam mc,
+                                                      float4* __restrict__ out) {
+    wf_motion_paths<ANIM>(sc, wf, mc, wf.counters[WF_N_PATHS], out);
+}
+
 // LowDiscrepancy::get_samples + get_samples_1d + Camera::generate_ray only (parity of S2 / C)
 // k_wf_film without shared-memory atomics (opt-in: TRB_FILM_V2=1; validated by tools/film_check.py). Each of the CTA's
 // four warps splats into its OWN copy of the tile. Inside a warp the 32 lanes are 32 different pixels walking the footprint
